@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the scan-to-map registration hot path (BASELINE.json config[1]: 100k-pt scan vs 5M-pt map, 1xB200).
+"""Benchmark of the scan-to-map registration hot path (BASELINE.json config[1]: 100k-pt scan vs 5M-pt map, 1xH100).
 
 A step = one synthetic Livox scan through the whole per-scan path (ll_scan_to_pose): feature extraction (K1-K3),
 VoxelGrid x2 per feature class (K4), then the ICP loop against the HBM-resident map: transform + exact 5-NN + residual
@@ -9,6 +9,8 @@ blocks (K6-K7), robust LM solve x2 with inlier selection (K8-K10).  The map inde
   e2e   : scans/s through the same C-ABI call with the raw scan in pinned HOST memory (H2D inside the timed region,
           pose read back to the host), host wall clock around the call.
 L2 is flushed (256 MiB write) between timed steps, outside the timed regions.
+`--dump-outputs DIR` writes what the last timed step returned as DIR/<name>.npy: the RegResult pose and counters and the feature counts (float64), and
+the corner / surface features of that registration (float32).
 
 `--impl reference` times the CPU restatement of the reference (oracle/) on the host cores instead (no GPU used).
 """
@@ -45,28 +47,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return json.load(f)["hbm_gbs"], "measured"
-    return 6650.0, "fallback"
-
-
-def source_sha(name):
-    """sha1 of a kernel source file: ncu summaries under profiles/ are stamped with it, so a stale capture is never quoted."""
-    import hashlib
-    with open(os.path.join(ROOT, "loam_livox_b200", "csrc", name), "rb") as f:
-        return hashlib.sha1(f.read()).hexdigest()
-
-
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel` from the committed `ncu --set full` capture of this same command
-    (profiles/ncu_<kernel>_r2.json, written by profiles/summarize.py together with the sha1 of the kernel's source file).  None when the capture is
-    absent or was taken from a different version of the source."""
-    src = {"knn_blocks_kernel": "knn.cu", "lm_solve_kernel": "solve.cu"}[kernel]
-    p = os.path.join(ROOT, "profiles", f"ncu_{kernel}_r2.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        if d.get("source_sha1") == source_sha(src):
-            return d.get("traffic_bytes_per_launch")
-    return None
+    return 3350.0, "H100 SXM data sheet"
 
 
 def depth_levels(n):
@@ -160,7 +141,7 @@ def host_threads():
 
 def cpu_baseline(threads, n_scans, inputs, trees=None, warmup=1, in_flight=1):
     """`in_flight` > 1 = the reference's throughput mode (maximum_parallel_thread scans registered concurrently, each by a `threads`-thread team;
-    /root/reference/source/laser_mapping.hpp:1737-1742): scans/s of the whole pool."""
+    loam_livox/source/laser_mapping.hpp:1737-1742): scans/s of the whole pool."""
     from oracle import oracle as O
     mc, ms, scans, guesses, _ = inputs
     t0 = time.perf_counter()
@@ -210,16 +191,18 @@ def run_reference(args):
     trees = (O.KdTree(mc), O.KdTree(ms))
     cpu_baseline.t_build = time.perf_counter() - t0
     in_flight = max(1, args.contexts)
-    # "all the host threads it can use": more threads than the path can use make it slower (128 threads: 0.24 scans/s, 16 threads: 11 scans/s on the
-    # same box), so the arm takes the best of a few team sizes, each tried on two scans
+    # "all the host threads it can use": more threads than the path can use make it slower, so the arm takes the best of a few team sizes, each
+    # tried on two scans
     cands = sorted({c for c in (hw, 64, 32, 16, 8, 4, 2, 1) if c * in_flight <= hw} or {1}, reverse=True)
     trial = {c: cpu_baseline(c, 2 * in_flight, inputs, trees=trees, in_flight=in_flight)["value"] for c in cands}
     best = max(trial, key=trial.get)
-    # the requested steps and warm-up, unless that would take longer than the time budget (then as many as fit, and the line says so)
-    budget_s = 150.0
-    per = 1.0 / trial[best]
-    n = int(max(min(args.steps, budget_s / per), min(args.steps, 4)))
-    w = int(max(1, min(args.warmup, 0.1 * budget_s / per)))
+    # the requested steps and warm-up; with --time-budget, only as many as fit the budget (and the line says so)
+    budget_s = args.time_budget
+    n, w = args.steps, args.warmup
+    if budget_s:
+        per = 1.0 / trial[best]
+        n = int(max(min(args.steps, budget_s / per), min(args.steps, 4)))
+        w = int(max(1, min(args.warmup, 0.1 * budget_s / per)))
     cb = cpu_baseline(best, n, inputs, trees=trees, warmup=w, in_flight=in_flight)
     cb["sample"] += (f"; team size chosen among {cands} of {hw} host threads (scans/s on two scans each: " + ", ".join(f"{c}: {trial[c]:.2f}" for c in cands) + ")"
                      + ("" if n == args.steps else f"; {n} of the requested {args.steps} steps fit the {budget_s:.0f} s budget"))
@@ -233,7 +216,7 @@ def run_reference(args):
 
 
 def config_block(wl, args, feats, world, t_index_ms):
-    """Same keys in both arms (the driver compares the two config dicts)."""
+    """Same keys in both arms, so that their config dicts can be compared."""
     if args.mode == "sharded":
         par = f"ONE scan registered by {world} GPU(s): map sharded by spatial cell (owner cells + 1.42 m / 7.07 m halo), features processed by the owner of their cell, " \
               "29 normal-equation sums all-reduced inside the solver kernel over NVLink peer memory"
@@ -243,6 +226,21 @@ def config_block(wl, args, feats, world, t_index_ms):
         par = f"scan-parallel x{world} (one map replica per GPU, no data-path collective)" if world > 1 else "1 GPU"
     return {"workload": WORKLOADS[wl], "pipeline": PIPE, "features_per_scan": feats, "l2": "flushed (256 MiB write) between timed steps, outside the timed regions",
             "parallelism": par, "map_index_build_ms": t_index_ms}
+
+
+def dump_outputs(d, ctx, res, nc, ns, extra=None):
+    """What one call of the timed path hands its caller: every RegResult field except the gpu_ms_* timings, the feature counts and `extra` as
+    float64 .npy files, and the corner / surface features that registration used (scan frame, x y z intensity) as float32 (n, 4) arrays, read
+    back from `ctx` (ll_features_to_pointcloud2 in the default 16-byte layout; about 0.5 MB for C2)."""
+    from loam_livox_b200.registration import features_to_pointcloud2
+    os.makedirs(d, exist_ok=True)
+    out = {name: getattr(res, name) for name, _ in res._fields_ if not name.startswith("gpu_ms")}
+    out["features"] = (nc, ns)
+    out.update(extra or {})
+    for name, v in out.items():
+        np.save(os.path.join(d, f"{name}.npy"), np.array(v, dtype=np.float64).reshape(-1))
+    for which, name in ((0, "features_corner"), (1, "features_surf")):
+        np.save(os.path.join(d, f"{name}.npy"), np.frombuffer(features_to_pointcloud2(ctx, which), np.float32).reshape(-1, 4))
 
 
 # ------------------------------------------------------------------------------------------------ GPU arm
@@ -378,10 +376,11 @@ def run_gpu(args):
             note(res, nc, ns)
         torch.cuda.synchronize()
         total_ms = float(np.sum([a.elapsed_time(b) for a, b in ev]))
+        last = (ctx, res, nc, ns)
     else:
         # throughput mode: K host threads, one context each, all on the shared map; the device time is the span from the first start event to the
         # last end event (events of different streams of one device share a clock); the L2 cannot be flushed between steps of concurrent streams,
-        # so each thread cycles through inputs + map (> 126 MB) instead
+        # so each thread cycles through inputs + map (> 50 MB, the L2 of an H100) instead
         starts = [torch.cuda.Event(enable_timing=True) for _ in range(K)]
         ends = [torch.cuda.Event(enable_timing=True) for _ in range(K)]
         results = [[] for _ in range(K)]
@@ -407,6 +406,9 @@ def run_gpu(args):
         for r in results:
             for (res, nc, ns) in r:
                 note(res, nc, ns)
+        last = (ctxs[(args.steps - 1) % K],) + tuple(results[(args.steps - 1) % K][-1])
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last)
     launches = sum(c.launches() for c in ctxs) - l0
     # ---- e2e: pinned host inputs through the same public call, host wall clock, H2D + result D2H inside
     if K == 1:
@@ -461,7 +463,7 @@ def run_gpu(args):
         for name, alg, ms_l, what in (("knn_blocks_kernel", alg_knn, knn_ms_launch, "transform + exact 5-NN + residual blocks; one launch per ICP iteration"),
                                       ("lm_solve_kernel", alg_solve, solve_ms_launch, "solve #1 + inlier selection + solve #2 + pose; one launch per ICP iteration")):
             ach = alg / (ms_l * 1e-3) / 1e9 if ms_l > 0 else 0.0
-            roofs[name] = {"bound": "hbm", "kernel": f"{name} ({what})", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": ncu_traffic(name),
+            roofs[name] = {"bound": "hbm", "kernel": f"{name} ({what})", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
                            "peak_source": peak_src, "algorithmic_bytes_per_launch": alg, "kernel_ms": ms_l, "launches_per_step": n_iter / len(icp_iters),
                            "share_of_step": ms_l * n_iter / (total_ms * (K if K > 1 else 1))}
         dominant = max(roofs, key=lambda k: roofs[k]["kernel_ms"])
@@ -485,7 +487,7 @@ def run_gpu(args):
         if shard is not None:
             line["shard"] = shard
             ev_n = max(1, int(cyc[5]))
-            mhz = (clocks or {}).get("sm_mhz") or 1965.0
+            mhz = (clocks or {}).get("sm_mhz") or 1980.0
             line["exchange"] = {"in_kernel_allreduce_plus_grid_reduce_us_per_evaluation": float(cyc[2]) / ev_n / mhz, "evaluations_last_registration": ev_n,
                                 "l1_exchange_plus_select_us_per_icp_iteration": 1e3 * float(np.sum(sel_all_ms)) / n_iter,
                                 "note": "cycle counters of the solver's master CTA over the last registration (ll_debug_solver_cycles); the all-reduce is 29 doubles per rank pushed into every peer's staging slot + one flag"}
@@ -548,6 +550,8 @@ def run_stream(args):
             checkpoints[k + 1] = float(np.linalg.norm(t - R0.T @ (poses[k].t - t0w)))
             final_pose = {"scan": k + 1, "q_wxyz": [float(x) for x in q], "t": [float(x) for x in t]}
     clocks = sampler.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, ctx, res, st.n_corner, st.n_surf, {"pose_q_wxyz": q, "pose_t": t, "map_points": (st.map_corner, st.map_surf)})
     if args.dump_poses:
         np.save(args.dump_poses, np.array(track))
     line = {"metric": "scans_per_sec", "value": len(times) / float(np.sum(times)), "unit": "scans/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
@@ -653,6 +657,8 @@ def run_c5(args):
     torch.cuda.synchronize()
     total_ms = float(np.sum([a.elapsed_time(b) for a, b in ev]))
     launches = ctx.launches() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ctx, res, nc, ns)
     e2e_s = 0.0
     for i in range(args.steps):
         with torch.cuda.stream(stream):
@@ -689,8 +695,10 @@ def main():
     ap.add_argument("--contexts", type=int, default=1, help="scans in flight per GPU (throughput mode: K contexts on K host threads sharing one map; the reference runs maximum_parallel_thread of them)")
     ap.add_argument("--matching-mode", type=int, default=0, choices=[0, 1], help="c3 only: mapping/matching_mode (0 = history window, the shipped YAMLs' mode; 1 = cell map)")
     ap.add_argument("--dump-poses", default=None, help="c3 only: write the pose after every scan (q_wxyz, t) to this .npy (diagnostics: first scan at which GPU and oracle part)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write what the last timed step returned as DIR/<name>.npy, to compare two builds output for output")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--cpu-scans", type=int, default=5)
+    ap.add_argument("--time-budget", type=float, default=None, metavar="SECONDS", help="--impl reference only: time fewer than --steps steps when they would take longer than this")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

@@ -1,10 +1,10 @@
 // loamlivox_b200.hpp — header-only C++ mirror of the reference's classes for the hot path, over the C-ABI (loamlivox_b200.h).
 // Same names, argument meaning and return conventions as
-//   Livox_laser                      /root/reference/source/livox_feature_extractor.hpp:77   (extract_laser_features :722, get_features :219)
-//   Point_cloud_registration         /root/reference/source/point_cloud_registration.hpp:38  (find_out_incremental_transfrom :163/:585,
+//   Livox_laser                      loam_livox/source/livox_feature_extractor.hpp:77   (extract_laser_features :722, get_features :219)
+//   Point_cloud_registration         loam_livox/source/point_cloud_registration.hpp:38  (find_out_incremental_transfrom :163/:585,
 //                                                                                               pointcloudAssociateToMap :673)
-//   Points_cloud_map                 /root/reference/source/cell_map_keyframe.hpp:264        (append_cloud :619, cells in radius + FOV :761, laser_mapping.hpp:475-516)
-//   Laser_mapping::process_new_scan  /root/reference/source/laser_mapping.hpp:1316
+//   Points_cloud_map                 loam_livox/source/cell_map_keyframe.hpp:264        (append_cloud :619, cells in radius + FOV :761, laser_mapping.hpp:475-516)
+//   Laser_mapping::process_new_scan  loam_livox/source/laser_mapping.hpp:1316
 // so that laser_feature_extractor.hpp / laser_mapping.hpp can switch with the small adapter shown in INTEGRATION.md.
 // No PCL / Eigen / Ceres needed: clouds are std::vector<ll200::PointXYZI> (layout-identical to pcl::PointXYZI, 32 bytes).
 #pragma once
@@ -27,7 +27,7 @@ class Context {
  public:
   explicit Context(int device = 0, const ll_config* cfg = nullptr) {
     int st = ll_ctx_create(cfg, device, &ctx_);
-    if (st != LL_OK) throw Error(st, "ll_ctx_create failed: a CUDA device (sm_100a) is required, there is no CPU fallback");
+    if (st != LL_OK) throw Error(st, "ll_ctx_create failed: a CUDA device (sm_90a) is required, there is no CPU fallback");
   }
   ~Context() { ll_ctx_destroy(ctx_); }
   Context(const Context&) = delete; Context& operator=(const Context&) = delete;

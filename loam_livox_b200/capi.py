@@ -1,7 +1,7 @@
 """ctypes binding of libloamlivox_b200.so (include/loamlivox_b200.h).
 
 The CUDA library is the product: importing this module without the shared object, or creating a context without a
-B200-class GPU, fails loudly — there is no CPU or PyTorch fallback anywhere in this package.
+Hopper (sm_90a) GPU, fails loudly — there is no CPU or PyTorch fallback anywhere in this package.
 """
 from __future__ import annotations
 
@@ -97,7 +97,7 @@ def lib():
     if _LIB is not None:
         return _LIB
     if not os.path.exists(LIB_PATH):
-        raise LoamLivoxError(f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a). "
+        raise LoamLivoxError(f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). "
                              "There is no CPU fallback.")
     L = C.CDLL(LIB_PATH)
     vp, sz, ci, cf, cd = C.c_void_p, C.c_size_t, C.c_int, C.c_float, C.c_double

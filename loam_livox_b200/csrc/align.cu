@@ -1,5 +1,5 @@
 // Loop-closure reuse of the registration hot path (SURVEY.md 8(f) N4): Scene_alignment::find_tranfrom_of_two_mappings
-// (/root/reference/source/scene_alignment.hpp:269-353, object set-up :233-243): the same find_out_incremental_transfrom, called three times,
+// (loam_livox/source/scene_alignment.hpp:269-353, object set-up :233-243): the same find_out_incremental_transfrom, called three times,
 // coarse to fine (leaf x8, x4, x1), with ICP_LINE = 0, on ONE persistent Point_cloud_registration object -- so m_para_buffer_incremental
 // (q_incre, t_incre), m_q_w_curr and m_t_w_curr carry over from one scale to the next while m_q_w_last / m_t_w_last stay (identity, 0).
 // The four feature clouds (line / plane points of the two keyframes) are the caller's; extracting them (cell eigen-analysis, Maps_keyframe)

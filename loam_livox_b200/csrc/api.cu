@@ -1,7 +1,7 @@
 // C-ABI of libloamlivox_b200.so (see include/loamlivox_b200.h) and the host-side ICP driver.
 //
 // Host logic restated from Point_cloud_registration::find_out_incremental_transfrom
-// (/root/reference/source/point_cloud_registration.hpp:163-583): the gate at :199, the ICP loop :211-532 (the per-iteration work is
+// (loam_livox/source/point_cloud_registration.hpp:163-583): the gate at :199, the ICP loop :211-532 (the per-iteration work is
 // four kernels: kNN+blocks, solve #1, inlier select, solve #2 + pose/termination), the threshold rescale :559 and the reject gate :561-573.
 #include <cmath>
 #include <cstring>
@@ -491,7 +491,7 @@ int ll_register(ll_ctx* ctx, const ll_map* map, const void* scan_corner, size_t 
 
 // One tiny registration (three planes and two edges: 1240 map points, 310 features) through the whole device path, result discarded.  It pays -- once, at a
 // time of the caller's choosing -- what CUDA defers to first use: the module loads of the kNN / solver / sort kernels and the first cooperative launch
-// (1 - 70 ms on the GPU boxes, measured as the first registered scan of a stream: profiles/r2/c3_first_registration.txt).  ll_mapper_create calls it.
+// (otherwise paid by the first registered scan of a stream).  ll_mapper_create calls it.
 int ll_ctx_warmup(ll_ctx* ctx) {
   if (!ctx) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);

@@ -2,10 +2,10 @@
 //
 // Replaces, on the reference side:
 //   Points_cloud_map<float>::append_cloud / set_point_cloud / find_cell / add_cell / find_cell_center
-//                                              /root/reference/source/cell_map_keyframe.hpp:556-571,578-672,681-758
+//                                              loam_livox/source/cell_map_keyframe.hpp:556-571,578-672,681-758
 //   Points_cloud_cell::append_pt / get_pointcloud / set_pointcloud        :331-351,378-419   (cells keep xyz only)
 //   find_cells_in_radius + if_pt_in_fov + per-cell VoxelGrid + down-sample-and-replace (update_buff_for_matching, mode 1)
-//                                              /root/reference/source/laser_mapping.hpp:310-324,471-516, cell_map_keyframe.hpp:761-788
+//                                              loam_livox/source/laser_mapping.hpp:310-324,471-516, cell_map_keyframe.hpp:761-788
 //
 // Layout: an open-addressing hash table of cells keyed by the packed integer cell index (k, j, i) (21 bits each, so that ascending key ==
 // ascending (k, j, i), the order in which the cells are visited), with per-cell frame stamps and an epoch; and ONE flat point store

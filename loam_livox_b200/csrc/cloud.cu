@@ -1,10 +1,10 @@
 // Cloud plumbing kernels: format repack, pointAssociateToMap over a cloud, VoxelGrid down-sampling, inlier selection.
 //
 // Replaces, on the reference side:
-//   pcl::VoxelGrid<PointXYZI>::filter (third-party PCL, restated)  call sites /root/reference/source/laser_feature_extractor.hpp:372-380,
-//                                   /root/reference/source/laser_mapping.hpp:491,509,533-537,1367-1373,1434-1437                 (K4)
-//   pointcloudAssociateToMap        /root/reference/source/point_cloud_registration.hpp:622-661,673-685                           (K6, cloud form)
-//   compute_inlier_residual_threshold (std::set de-dup + order statistic) /root/reference/source/point_cloud_registration.hpp:153-161,484-485 (K10)
+//   pcl::VoxelGrid<PointXYZI>::filter (third-party PCL, restated)  call sites loam_livox/source/laser_feature_extractor.hpp:372-380,
+//                                   loam_livox/source/laser_mapping.hpp:491,509,533-537,1367-1373,1434-1437                 (K4)
+//   pointcloudAssociateToMap        loam_livox/source/point_cloud_registration.hpp:622-661,673-685                           (K6, cloud form)
+//   compute_inlier_residual_threshold (std::set de-dup + order statistic) loam_livox/source/point_cloud_registration.hpp:153-161,484-485 (K10)
 //
 // Compiled with -fmad=false (voxel indices, centroids and the transform must round like the scalar CPU code).
 #include <cub/cub.cuh>

@@ -1,4 +1,4 @@
-// Internal declarations shared by the CUDA translation units of libloamlivox_b200.so (sm_100a only).
+// Internal declarations shared by the CUDA translation units of libloamlivox_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -24,13 +24,13 @@
 struct DevBuf {  // grow-only device allocation
   void* p = nullptr; size_t cap = 0;
   size_t floor = 0;   // smallest size ever allocated: a caller that knows how far the buffer will grow (the streaming mapper) sets it once, then nothing is
-                      // reallocated in steady state (a cudaMalloc + cudaFree pair was measured at 100-800 ms on the GPU boxes: profiles/r2/bench_c3_*)
+                      // reallocated in steady state (a cudaMalloc + cudaFree pair in a process with live streams and graphs stalls the call that triggers it)
   cudaError_t reserve(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
     // first allocation: a little slack; regrowth: at least double, so that a buffer following a growing map is reallocated O(log n) times
-    // (cudaFree synchronises the device and showed up as 10-250 ms spikes in the streaming mapper)
+    // (cudaFree synchronises the device)
     size_t want = bytes + bytes / 8 + 256;
-    if (want < ((size_t)8 << 20)) want = (size_t)8 << 20;   // floor: a (re)allocation costs 60-90 ms on this platform, 8 MB of a 180 GB HBM costs nothing
+    if (want < ((size_t)8 << 20)) want = (size_t)8 << 20;   // floor: every (re)allocation stalls the device, 8 MB of an 80 GB HBM costs nothing
     if (p && want < 2 * cap) want = 2 * cap;
     if (want < floor) want = floor;
     if (p) cudaFree(p);

@@ -1,11 +1,11 @@
 // Livox feature extraction kernels (K1 - K3).
 //
 // Replaces, on the reference side:
-//   Livox_laser::projection_scan_3d_2d (+ eval_point, add_mask_of_point)   /root/reference/source/livox_feature_extractor.hpp:458-607,343-358,322-341   (K1)
-//   Livox_laser::compute_features                                          /root/reference/source/livox_feature_extractor.hpp:361-455                    (K2)
-//   Livox_laser::split_laser_scan (petal bookkeeping), piece bounds        /root/reference/source/livox_feature_extractor.hpp:657-719,
-//                                                                          /root/reference/source/laser_feature_extractor.hpp:313-323
-//   Livox_laser::get_features                                              /root/reference/source/livox_feature_extractor.hpp:219-272                    (K3)
+//   Livox_laser::projection_scan_3d_2d (+ eval_point, add_mask_of_point)   loam_livox/source/livox_feature_extractor.hpp:458-607,343-358,322-341   (K1)
+//   Livox_laser::compute_features                                          loam_livox/source/livox_feature_extractor.hpp:361-455                    (K2)
+//   Livox_laser::split_laser_scan (petal bookkeeping), piece bounds        loam_livox/source/livox_feature_extractor.hpp:657-719,
+//                                                                          loam_livox/source/laser_feature_extractor.hpp:313-323
+//   Livox_laser::get_features                                              loam_livox/source/livox_feature_extractor.hpp:219-272                    (K3)
 //
 // The reference walks the scan sequentially; here every per-point quantity is computed independently (the only true
 // sequential dependences - "copy the previous point's projection for a zero return" and the 50-point split hysteresis -

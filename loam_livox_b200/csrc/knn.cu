@@ -1,11 +1,11 @@
 // Map index ("bucket tree") build and the exact 5-NN search + residual-block construction kernels.
 //
 // Replaces, on the reference side:
-//   pcl::KdTreeFLANN::setInputCloud            /root/reference/source/laser_mapping.hpp:544-545,
-//                                              /root/reference/source/point_cloud_registration.hpp:596-597   (K5)
-//   pointAssociateToMap + nearestKSearch(k=5)  /root/reference/source/point_cloud_registration.hpp:247-249,349-351,622-661 (K6)
-//   gates + functor constructors               /root/reference/source/point_cloud_registration.hpp:254-331,353-431,
-//                                              /root/reference/source/ceres_icp.hpp:246-260,314-336          (K7)
+//   pcl::KdTreeFLANN::setInputCloud            loam_livox/source/laser_mapping.hpp:544-545,
+//                                              loam_livox/source/point_cloud_registration.hpp:596-597   (K5)
+//   pointAssociateToMap + nearestKSearch(k=5)  loam_livox/source/point_cloud_registration.hpp:247-249,349-351,622-661 (K6)
+//   gates + functor constructors               loam_livox/source/point_cloud_registration.hpp:254-331,353-431,
+//                                              loam_livox/source/ceres_icp.hpp:246-260,314-336          (K7)
 //
 // Compiled with -fmad=false: the float distance (FLANN L2_Simple<float>: ((dx*dx)+dy*dy)+dz*dz), the fp64
 // transform and the fp64 line/plane geometry must round exactly like the scalar CPU code.
@@ -276,7 +276,7 @@ struct WarpWalk { float lb[KNN_LEVELS][32]; };   // per warp: the child bounds o
 // ---- optional TMA staging of leaf buckets (LL_KNN_TMA=1; north_star's "TMA/shared-memory staging of KD-tree leaf buckets") --------------------
 // When a level-0 node is opened, the two nearest qualifying buckets are fetched with cp.async.bulk (512 B each) into a warp-private double buffer
 // in shared memory, completion on an mbarrier; the pick that reaches such a bucket waits on the barrier and reads its point from shared memory
-// instead of issuing the load itself.  Same visiting order, same results.  Measured against the plain variant in profiles/r2 (DESIGN.md 3.1).
+// instead of issuing the load itself.  Same visiting order, same results.  Not measured on the H100 (DESIGN.md §7).
 struct __align__(16) WarpStage { float4 pts[2][32]; unsigned long long bar[2]; };
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory"); }

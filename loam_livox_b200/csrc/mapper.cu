@@ -3,11 +3,11 @@
 // resident on the device (the history window, the cell maps, the match-map snapshot and its index, the features).
 //
 // Restates, on the reference side (ROS I/O, threads, mutexes and loop closure left out):
-//   Laser_mapping::process_new_scan                /root/reference/source/laser_mapping.hpp:1316-1521
-//   history window push / pop                      /root/reference/source/laser_mapping.hpp:1439-1487 (mode 0 concatenation :518-531)
-//   Laser_mapping::update_buff_for_matching        /root/reference/source/laser_mapping.hpp:460-566 (mode 1 branch :471-516, whole-map VoxelGrid :533-537,
+//   Laser_mapping::process_new_scan                loam_livox/source/laser_mapping.hpp:1316-1521
+//   history window push / pop                      loam_livox/source/laser_mapping.hpp:1439-1487 (mode 0 concatenation :518-531)
+//   Laser_mapping::update_buff_for_matching        loam_livox/source/laser_mapping.hpp:460-566 (mode 1 branch :471-516, whole-map VoxelGrid :533-537,
 //                                                                                                  KdTreeFLANN build :544-545)
-//   Laser_mapping::init_pointcloud_registration    /root/reference/source/laser_mapping.hpp:1266-1297
+//   Laser_mapping::init_pointcloud_registration    loam_livox/source/laser_mapping.hpp:1266-1297
 // The reference refreshes the match map on a background thread after every registered scan, with the pose of that scan; here the refresh
 // runs at the start of the next scan (same pose, same map content), so the result is the reference's with maximum_parallel_thread = 1.
 #include <chrono>
@@ -77,9 +77,9 @@ struct ll_mapper {
   bool trace = false;       // LL_MAPPER_TRACE=1
 };
 
-// Every buffer whose size follows the map is allocated here, once, for the configured reservation (HBM is 180 GB; a reallocation costs
-// 100-800 ms on the GPU boxes and one such spike per doubling of the map dominated the mean scan time of the 1000-scan stream in round 2's first
-// measurement).  Past the reservation everything still grows by doubling.
+// Every buffer whose size follows the map is allocated here, once, for the configured reservation (a reallocation inside a scan call
+// synchronises the device and stalls that call for far longer than the scan takes; one such stall per doubling of the map dominates the mean
+// scan time of a long stream).  Past the reservation everything still grows by doubling.
 static int mapper_reserve(ll_ctx* ctx, ll_mapper* m) {
   const size_t R = (size_t)(m->cfg.reserve_map_points > 0 ? m->cfg.reserve_map_points : 0), S = (size_t)(m->cfg.reserve_store_points > 0 ? m->cfg.reserve_store_points : 0);
   const size_t F = (size_t)ctx->cfg.max_features + 16;

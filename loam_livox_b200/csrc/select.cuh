@@ -53,7 +53,7 @@ __device__ double block_select(const double* __restrict__ uniq, int n, double ra
   constexpr int BPT = 2048 / NT;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // Pre-pass: the bits all keys share.  The norms of one scan span a few binades, so the top ~10 bits are common; starting the digits below
-  // them spreads the keys over the 2048 bins (digits on the common exponent put 28k shared-memory atomics on 3 addresses: 40 us).
+  // them spreads the keys over the 2048 bins (digits on the common exponent put 28k shared-memory atomics on 3 addresses).
   unsigned long long kand = ~0ull, kor = 0ull;
   for (int base0 = 0; base0 < n; base0 += NT * 8) {
     unsigned long long key[8];

@@ -3,7 +3,7 @@
 // The reference has no multi-GPU path; what it fixes is the pair of match gates that make owner + halo search exact:
 //   surface: the 5th squared distance must be < m_maximum_dis_plane_for_match = 50.0  -> halo sqrt(50) = 7.07 m
 //   corner : ... < m_maximum_dis_line_for_match = 2.0                                 -> halo sqrt(2)  = 1.42 m
-//   (/root/reference/source/point_cloud_registration.hpp:64-65, :254, :353)
+//   (loam_livox/source/point_cloud_registration.hpp:64-65, :254, :353)
 // A correspondence whose 5th neighbour lies beyond the gate is rejected anyway, and a shard is a subset of the map (distances can only grow), so
 // searching [points of the cells a rank owns] + [every point within the halo of one of those cells] gives, for every ACCEPTED correspondence,
 // exactly the neighbours a search of the whole map gives.  Compaction keeps the input order, so index ties break the same way.

@@ -1,14 +1,14 @@
 // Robust 6-DoF Levenberg-Marquardt solve of one ICP iteration as ONE persistent kernel (K8 + K9 + K10 front end).
 //
 // Replaces, on the reference side (Ceres is third-party, restated from its published behaviour, see oracle/orc_solver.hpp):
-//   ceres::Problem / AddResidualBlock / Solve x2   /root/reference/source/point_cloud_registration.hpp:220-228,323,422,460-474,501-508
-//   residual models (autodiff)                     /root/reference/source/ceres_icp.hpp:262-288 (point2line), :338-366 (point2plane)
+//   ceres::Problem / AddResidualBlock / Solve x2   loam_livox/source/point_cloud_registration.hpp:220-228,323,422,460-474,501-508
+//   residual models (autodiff)                     loam_livox/source/ceres_icp.hpp:262-288 (point2line), :338-366 (point2plane)
 //   HuberLoss(0.1), EigenQuaternionParameterization, bounds on t   :220-221, :143-151
 //   problem.Evaluate + inlier threshold front end  :476-499 (the L1 norms are produced here; select.cu finishes K10)
 //   pose composition + ICP termination test        :514-531
 //
-// Design: every residual block is staged once into SHARED MEMORY (52 B per block, SoA) of one of 148 persistent CTAs and
-// stays on-chip for the whole solve (up to ~580k blocks).  One evaluation = every thread evaluates r, J (analytic, fp64), the Huber
+// Design: every residual block is staged once into SHARED MEMORY (52 B per block, SoA) of one of the persistent CTAs (one per SM,
+// 132 on an H100) and stays on-chip for the whole solve (up to ~400k blocks).  One evaluation = every thread evaluates r, J (analytic, fp64), the Huber
 // weight and its 28 normal-equation terms, warp-shuffle + shared-memory reduce per CTA, one 29-double partial per CTA,
 // a ticket barrier, and the LAST CTA to arrive reduces the partials in fixed order (run-to-run deterministic), runs the
 // trust-region logic on one thread and publishes the next trial point.  No host round trip inside a solve.
@@ -615,7 +615,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   if (master && tid == 0) *((volatile unsigned*)&Y->gen) = gen;
 }
 
-#define SOLVE_MAX_SMEM (200 * 1024)   // up to ~470k slots; a typical scan (<= 113 KB of slots per CTA) leaves room for a second CTA per SM (another context's solver)
+#define SOLVE_MAX_SMEM (200 * 1024)   // up to ~405k slots on 132 SMs; a typical scan (<= 113 KB of slots per CTA) leaves room for a second CTA per SM (another context's solver)
 int solve_max_slots(ll_ctx* ctx) { return ctx->num_sms * ((SOLVE_MAX_SMEM / SLOT_BYTES) / SOLVE_THREADS) * SOLVE_THREADS; }
 
 int solve_prepare(ll_ctx* ctx) {
@@ -628,7 +628,7 @@ int solve_prepare(ll_ctx* ctx) {
 }
 int launch_solve(ll_ctx* ctx, const SolveArgs& a) {
   // The evaluation is fp64-throughput bound (64 DFMA/clk/SM): spread the slots over ALL SMs, even when that leaves CTAs partly empty.
-  // tile = slots per CTA and pass (a multiple of 32, <= SOLVE_THREADS); measured: 61 full CTAs 8.3 us/evaluation, 148 CTAs x 224 slots 3.5 us.
+  // tile = slots per CTA and pass (a multiple of 32, <= SOLVE_THREADS); partly empty CTAs on every SM evaluate faster than fewer full ones.
   const int M1 = a.M > 0 ? a.M : 1;
   int tile = ((ll_div_up(M1, ctx->num_sms) + 31) / 32) * 32; if (tile > SOLVE_THREADS) tile = SOLVE_THREADS;
   const int tiles = ll_div_up(M1, tile);

@@ -2,11 +2,11 @@
 
 Names, argument meaning and return conventions follow the reference so the parity tests read like its call sites:
 
-  Livox_laser.extract_laser_features / get_features      /root/reference/source/livox_feature_extractor.hpp:722,219
-  voxel_grid_filter (pcl::VoxelGrid::filter)             /root/reference/source/laser_mapping.hpp:1367-1373
-  Map (update_buff_for_matching's KdTreeFLANN pair)      /root/reference/source/laser_mapping.hpp:533-559
+  Livox_laser.extract_laser_features / get_features      loam_livox/source/livox_feature_extractor.hpp:722,219
+  voxel_grid_filter (pcl::VoxelGrid::filter)             loam_livox/source/laser_mapping.hpp:1367-1373
+  Map (update_buff_for_matching's KdTreeFLANN pair)      loam_livox/source/laser_mapping.hpp:533-559
   Point_cloud_registration.find_out_incremental_transfrom / pointcloudAssociateToMap
-                                                         /root/reference/source/point_cloud_registration.hpp:163,673
+                                                         loam_livox/source/point_cloud_registration.hpp:163,673
 Everything here is plumbing: the arithmetic runs in the CUDA kernels of libloamlivox_b200.so.
 """
 from __future__ import annotations
@@ -28,7 +28,7 @@ class Context:
         h = C.c_void_p()
         st = self._lib.ll_ctx_create(C.byref(self.cfg), device, C.byref(h))
         if st != capi.LL_OK:
-            raise LoamLivoxError(f"ll_ctx_create failed ({st}): a CUDA device (sm_100a) is required, there is no CPU fallback")
+            raise LoamLivoxError(f"ll_ctx_create failed ({st}): a CUDA device (sm_90a) is required, there is no CPU fallback")
         self.h = h
         self.device = device
 
@@ -300,7 +300,7 @@ def features_to_pointcloud2(ctx: Context, which: int) -> bytes:
 
 class Scene_alignment:
     """Mirror of Scene_alignment::find_tranfrom_of_two_mappings from the point where the four feature clouds exist
-    (/root/reference/source/scene_alignment.hpp:269-353): coarse-to-fine registration of keyframe b's features onto keyframe a's."""
+    (loam_livox/source/scene_alignment.hpp:269-353): coarse-to-fine registration of keyframe b's features onto keyframe a's."""
 
     def __init__(self, ctx: Context, line_res: float = 0.4, plane_res: float = 0.4, **kw):
         self.ctx = ctx
@@ -325,8 +325,8 @@ class Scene_alignment:
 
 
 class Points_cloud_map:
-    """Device-resident voxel-cell map as the matching path uses it (Points_cloud_map<float>, /root/reference/source/cell_map_keyframe.hpp:264;
-    append_cloud :619, find_cells_in_radius :761; the consumer is update_buff_for_matching, /root/reference/source/laser_mapping.hpp:471-516)."""
+    """Device-resident voxel-cell map as the matching path uses it (Points_cloud_map<float>, loam_livox/source/cell_map_keyframe.hpp:264;
+    append_cloud :619, find_cells_in_radius :761; the consumer is update_buff_for_matching, loam_livox/source/laser_mapping.hpp:471-516)."""
 
     def __init__(self, ctx: Context, resolution: float = 1.0, revisit_threshold: int = 2000, max_cells: int = 0):
         self.ctx = ctx
@@ -374,7 +374,7 @@ class Points_cloud_map:
 
 
 class Laser_mapping:
-    """Streaming odometry: one call per raw scan (Laser_mapping::process_new_scan, /root/reference/source/laser_mapping.hpp:1316-1521, with the
+    """Streaming odometry: one call per raw scan (Laser_mapping::process_new_scan, loam_livox/source/laser_mapping.hpp:1316-1521, with the
     match-map refresh of update_buff_for_matching :460-566 in matching_mode 1).  All state stays on the device."""
 
     def __init__(self, ctx: Context, **kw):

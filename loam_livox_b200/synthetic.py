@@ -3,7 +3,7 @@
 The reference ships no data, fixtures or tests (SURVEY.md §4), so every input used by tests/ and bench.py is
 generated here: an analytic room (floor, ceiling, four walls) with 24 square pillars, a rosette-scanning
 sensor model whose x axis looks forward (the extractor assumes that:
-/root/reference/source/livox_feature_extractor.hpp:518), closed-form ray casting, and world-frame feature
+loam_livox/source/livox_feature_extractor.hpp:518), closed-form ray casting, and world-frame feature
 maps sampled directly from the scene geometry.  NumPy only; everything is a pure function of its seed.
 """
 from __future__ import annotations
@@ -130,7 +130,7 @@ def make_scan(n, pose=None, seed=SEED, range_sigma=0.004, zero_frac=0.005, nan_f
 
 def make_triple_scan(n_total, pose=None, seed=SEED):
     """Mid-100 style frame: three Mid-40 heads yawed -25/0/+25 degrees, concatenated
-    (/root/reference/source/laser_feature_extractor.hpp:353-358 sums the per-lidar feature clouds)."""
+    (loam_livox/source/laser_feature_extractor.hpp:353-358 sums the per-lidar feature clouds)."""
     n = n_total // 3
     return [make_scan(n, pose, seed + k, yaw_offset_deg=y) for k, y in enumerate((-25.0, 0.0, 25.0))]
 

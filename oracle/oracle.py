@@ -43,7 +43,7 @@ class Trace(C.Structure):
 
 
 def default_params(**kw) -> RegParams:
-    """Precision-YAML values (/root/reference/config/performance_precision.yaml, launch/rosbag.launch:9-11) with the
+    """Precision-YAML values (loam_livox/config/performance_precision.yaml, launch/rosbag.launch:9-11) with the
     residual-block cap raised so the reference's random drop never triggers (SURVEY.md §8d)."""
     p = RegParams()
     p.if_motion_deblur = 0
@@ -186,7 +186,7 @@ def knn_brute(map_pts, q, k=5):
 
 class Extractor:
     """Livox_laser restatement.  Defaults = the values the ROS node writes into the object
-    (/root/reference/config/performance_precision.yaml:14-18, laser_feature_extractor.hpp:152-154,854,859)."""
+    (loam_livox/config/performance_precision.yaml:14-18, laser_feature_extractor.hpp:152-154,854,859)."""
 
     def __init__(self, corner_curvature=0.1, surface_curvature=0.005, minimum_view_angle=5.0, min_dis=0.1, min_sigma=7e-4):
         self.h = lib().orc_extractor_create(corner_curvature, surface_curvature, minimum_view_angle, min_dis, min_sigma)
@@ -304,7 +304,7 @@ def plus(x, delta, bound=0.3):
 
 def scene_align(source_line, source_plane, target_line, target_plane, t_init=(0.0, 0.0, 0.0), line_res=0.4, plane_res=0.4, maximum_icp_iteration=10,
                 maximum_residual_block=5000, accepted_threshold=0.2, rng_seed=0, threads=1):
-    """Scene_alignment::find_tranfrom_of_two_mappings (/root/reference/source/scene_alignment.hpp:269-353; object set-up :233-243) from the point where
+    """Scene_alignment::find_tranfrom_of_two_mappings (loam_livox/source/scene_alignment.hpp:269-353; object set-up :233-243) from the point where
     the four feature clouds exist.  One persistent Point_cloud_registration: increment and pose carry over between the three scales."""
     p = default_params(icp_line=0, icp_plane=1, max_final_cost=20000.0, para_max_speed=1000.0, para_max_angular_rate=360 * 57.3, inliner_dis=0.2,
                        current_frame_index=10000000, mapping_init_accumulate_frames=100, icp_max_iterations=maximum_icp_iteration, cere_max_iterations=50,
@@ -366,7 +366,7 @@ class CellMap:
 
 class Mapper:
     """Laser_mapping::process_new_scan + update_buff_for_matching (matching_mode 0: history window; 1: cell map) glued from the oracle pieces above, single-threaded
-    (/root/reference/source/laser_mapping.hpp:1316-1521, :460-566, :1266-1297).  The background refresh of the match map is run at the start
+    (loam_livox/source/laser_mapping.hpp:1316-1521, :460-566, :1266-1297).  The background refresh of the match map is run at the start
     of the next scan with the pose the previous scan ended with, which is what the reference does with maximum_parallel_thread = 1."""
 
     def __init__(self, params=None, line_resolution=0.1, plane_resolution=0.4, cell_resolution=1.0, revisit_threshold=2000, search_range=100.0,

@@ -1,12 +1,12 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see orc_math.hpp header). PARITY UNPINNED.
 // CPU restatement of the voxel-cell map as the matching path uses it (matching_mode 1):
-//   /root/reference/source/cell_map_keyframe.hpp
+//   loam_livox/source/cell_map_keyframe.hpp
 //     :556-571 find_cell_center     (cell centre = round((p - r/4) / (r/2)) * (r/2) + r/4 with r/2 stored by set_resolution :674-679)
 //     :619-672 append_cloud, :578-617 set_point_cloud (first call; bumps the frame index twice)
 //     :716-758 find_cell (revisit: a cell not touched for >= m_minimum_revisit_threshold frames is replaced by a fresh one)
 //     :681-714 add_cell, :378-419 append_pt, :331-351 get_pointcloud / set_pointcloud (cells keep xyz only: intensity becomes 0)
 //     :761-788 find_cells_in_radius (PCL octree radius search over the cell centres, squared float distance <= r^2)
-//   /root/reference/source/laser_mapping.hpp
+//   loam_livox/source/laser_mapping.hpp
 //     :310-324 if_pt_in_fov, :471-516 update_buff_for_matching, matching_mode 1 (per-cell VoxelGrid, down-sample-and-replace)
 // Deviation (documented): the octree returns cells in an unspecified order; the oracle visits them in ascending (k, j, i) cell-index order.
 #pragma once

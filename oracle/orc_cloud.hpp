@@ -4,12 +4,12 @@
 // and is not installed here; the published algorithms are restated.
 //
 //  * pcl::VoxelGrid<PointXYZI>::applyFilter (PCL 1.8+/1.9, downsample_all_data = true):
-//      call sites  /root/reference/source/laser_feature_extractor.hpp:372-380,
-//                  /root/reference/source/laser_mapping.hpp:491,509,533-537,1367-1373,1434-1437
+//      call sites  loam_livox/source/laser_feature_extractor.hpp:372-380,
+//                  loam_livox/source/laser_mapping.hpp:491,509,533-537,1367-1373,1434-1437
 //  * pcl::KdTreeFLANN<PointXYZI>::setInputCloud / nearestKSearch (FLANN KDTreeSingleIndex, L2_Simple<float>,
 //    leaf_max_size 15, eps 0, sorted):
-//      call sites  /root/reference/source/point_cloud_registration.hpp:249,351,596-597,
-//                  /root/reference/source/laser_mapping.hpp:544-545
+//      call sites  loam_livox/source/point_cloud_registration.hpp:249,351,596-597,
+//                  loam_livox/source/laser_mapping.hpp:544-545
 #pragma once
 #include <algorithm>
 #include <cmath>

@@ -1,14 +1,14 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see orc_math.hpp header). PARITY UNPINNED.
 // CPU restatement of the Livox feature extractor:
-//   /root/reference/source/livox_feature_extractor.hpp
+//   loam_livox/source/livox_feature_extractor.hpp
 //     :722-766 extract_laser_features (driver, timestamp bookkeeping)
 //     :458-607 projection_scan_3d_2d  (masks, projection, petal split)
 //     :343-358 eval_point, :322-341 add_mask_of_point
 //     :361-455 compute_features      (5-pt stencil curvature, view angle, labels)
 //     :657-719 split_laser_scan      (petal grouping -> only count + first/last idx used)
 //     :219-272 get_features          (ordered compaction)
-//   /root/reference/include/tools/tools_eigen_math.hpp:25-46 vector_angle
-//   /root/reference/source/laser_feature_extractor.hpp:285-335 piece-wise glue
+//   loam_livox/include/tools/tools_eigen_math.hpp:25-46 vector_angle
+//   loam_livox/source/laser_feature_extractor.hpp:285-335 piece-wise glue
 #pragma once
 #include <cmath>
 #include <cstdint>

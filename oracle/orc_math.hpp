@@ -7,7 +7,7 @@
 //
 // Follows: Eigen::Quaternion product / _transformVector / angularDistance / slerp,
 //          ceres::Jet forward-mode autodiff (used by AutoDiffCostFunction at
-//          /root/reference/source/ceres_icp.hpp:297-299,376-378).
+//          loam_livox/source/ceres_icp.hpp:297-299,376-378).
 #pragma once
 #include <cmath>
 #include <cstdint>

@@ -1,11 +1,11 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see orc_math.hpp header). PARITY UNPINNED.
 // CPU restatement of Point_cloud_registration:
-//   /root/reference/source/point_cloud_registration.hpp
+//   loam_livox/source/point_cloud_registration.hpp
 //     :163-583 find_out_incremental_transfrom (ICP outer loop, gates, cap drop, 2 solves, inlier select, reject)
 //     :585-605 4-argument overload (builds the trees itself)
 //     :622-661 pointAssociateToMap (+ :607-620 compute_interpolatation_rodrigue, :128-141 refine_blur)
 //     :153-161 compute_inlier_residual_threshold
-//   state hand-off  /root/reference/source/laser_mapping.hpp:1266-1297 init_pointcloud_registration
+//   state hand-off  loam_livox/source/laser_mapping.hpp:1266-1297 init_pointcloud_registration
 // Residual-block cap (:232-238,:339-345,:434-458): the reference draws from a std::random_device-seeded mt19937
 // (include/tools/tools_random.hpp:18-25), which no second implementation can reproduce.  The RULE is restated exactly
 // (pre-skip of a feature when rand*N > 2*cap with N the feature count of its class; after the block list is built, when its size M exceeds

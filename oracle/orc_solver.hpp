@@ -1,11 +1,11 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see orc_math.hpp header). PARITY UNPINNED.
 // CPU restatement of what the reference delegates to Ceres Solver (third-party, not vendored, not
-// version-pinned: /root/reference/CMakeLists.txt:23; API use implies 1.10 <= version < 2.2; the 1.14 behaviour
+// version-pinned: loam_livox/CMakeLists.txt:23; API use implies 1.10 <= version < 2.2; the 1.14 behaviour
 // is restated) for the 7-parameter (q_incre[4] on the Eigen-quaternion manifold + t_incre[3], box-bounded)
-// robust least-squares problem built at /root/reference/source/point_cloud_registration.hpp:220-228,323,422
+// robust least-squares problem built at loam_livox/source/point_cloud_registration.hpp:220-228,323,422
 // and solved at :460-474,:501-508.
 //
-//   residual functors  /root/reference/source/ceres_icp.hpp:238-301 (point2line), :306-380 (point2plane),
+//   residual functors  loam_livox/source/ceres_icp.hpp:238-301 (point2line), :306-380 (point2plane),
 //                      :81-148 / :152-233 (motion-deblur variants), evaluated with forward-mode Jets exactly
 //                      like ceres::AutoDiffCostFunction<F,3,4,3>
 //   loss               ceres::HuberLoss(0.1) shared by every block (:220), Corrector with rho'' <= 0

@@ -40,8 +40,8 @@ def test_host_threads_ignores_omp_env(monkeypatch):
 
 
 def test_reference_arm_contract(tmp_path):
-    """`bench.py --impl reference` as the driver launches it: rank 0 prints ONE JSON line with impl / metric / config / cpu_baseline / e2e, honours the
-    requested steps (they fit the time budget here) and uses the host's cores although torchrun-style OMP_NUM_THREADS=1 is exported; other ranks exit 0 silently."""
+    """`bench.py --impl reference` as torchrun launches it: rank 0 prints ONE JSON line with impl / metric / config / cpu_baseline / e2e, honours the
+    requested steps and uses the host's cores although torchrun-style OMP_NUM_THREADS=1 is exported; other ranks exit 0 silently."""
     import json
     import subprocess
     env = dict(os.environ, OMP_NUM_THREADS="1", RANK="0", WORLD_SIZE="2", LOCAL_RANK="0")

@@ -57,7 +57,7 @@ def test_no_cpu_fallback():
 
 
 def test_pose_log_format_matches_reference_printf():
-    """ll_format_pose_log is host-only code: the poses.log block of /root/reference/source/laser_mapping.hpp:1506-1511."""
+    """ll_format_pose_log is host-only code: the poses.log block of loam_livox/source/laser_mapping.hpp:1506-1511."""
     from loam_livox_b200 import capi
     from loam_livox_b200.registration import format_pose_log
     r = capi.RegResult()

@@ -464,7 +464,7 @@ def test_streaming_mapper_long_sequence(ctx, oracle, mode, window):
 # ---------------------------------------------------------------------------------------------- 8(e): sharded registration on >= 2 GPUs
 @pytest.mark.gpu
 def test_sharded_registration_two_gpus():   # halo-trimmed shards (csrc/shard.cu) + in-kernel all-reduce + L1 / count exchanges vs one GPU with the whole map
-    """Spawns tests/multi_gpu/sharded_check.py under torchrun when the box has >= 2 GPUs (skipped on the 1-GPU round-end box)."""
+    """Spawns tests/multi_gpu/sharded_check.py under torchrun when the box has >= 2 GPUs (skipped on a one-GPU machine)."""
     import os
     import subprocess
     import sys
@@ -604,7 +604,7 @@ def test_full_size_c2_pose_parity_with_the_oracle(oracle):
 @pytest.mark.gpu
 def test_two_contexts_on_two_host_threads_share_one_map(oracle):
     """S3 is called from up to maximum_parallel_thread std::async workers, each with its own Point_cloud_registration, sharing the read-only map
-    snapshot (/root/reference/source/laser_mapping.hpp:1348,1737-1742).  Two ll_ctx on two threads against ONE ll_map: every result equals the
+    snapshot (loam_livox/source/laser_mapping.hpp:1348,1737-1742).  Two ll_ctx on two threads against ONE ll_map: every result equals the
     result of the same registration run alone, bit for bit."""
     import threading
     from loam_livox_b200.registration import Context, Map, Point_cloud_registration

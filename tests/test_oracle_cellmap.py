@@ -1,7 +1,7 @@
 """CPU tests of the oracle's cell map and streaming driver (a14 / config C3) -- oracle only, no GPU.
 
-Reference behaviour being pinned: /root/reference/source/cell_map_keyframe.hpp:556-571 (cell index), :716-758 (revisit), :619-672 (append),
-/root/reference/source/laser_mapping.hpp:310-324 (FOV test), :471-516 (mode-1 assembly), :1316-1521 (process_new_scan)."""
+Reference behaviour being pinned: loam_livox/source/cell_map_keyframe.hpp:556-571 (cell index), :716-758 (revisit), :619-672 (append),
+loam_livox/source/laser_mapping.hpp:310-324 (FOV test), :471-516 (mode-1 assembly), :1316-1521 (process_new_scan)."""
 import numpy as np
 
 from loam_livox_b200 import synthetic as S
