@@ -9,8 +9,6 @@
 #include "common.cuh"
 #include "kernels.cuh"
 
-static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 extern "C" {
 
 void ll_align_cfg_default(ll_align_cfg* c) {

@@ -12,12 +12,10 @@
 
 int launch_inlier_select(ll_ctx* ctx, const double* d_l1, int M, double ratio, double* d_sorted, double* d_unique, int* d_n_unique);
 
-static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 int reg_arrays(ll_ctx* ctx, int M, RegArrays* A) {
   int cap = M > ctx->cfg.max_features ? M : ctx->cfg.max_features;
   int scap = ctx->cfg.max_scan_points > cap ? ctx->cfg.max_scan_points : cap;
-  size_t bytes = align256((size_t)cap * 16) * 2 + align256((size_t)cap * 24) + align256((size_t)cap * 8 + 64) * 3 + align256((size_t)ctx->num_sms * 32 * 8) + 4096 +
+  size_t bytes = align256((size_t)cap * 16) * 2 + align256((size_t)cap * 24) + align256((size_t)cap * 8 + 64) * 3 + 4096 +
                  align256((size_t)cap * 20) * 2 + align256((size_t)cap * 4) * 2 + align256((size_t)scap * 16) * 4;
   LL_CUDA(ctx, ctx->reg_buf.reserve(bytes));
   char* p = ctx->reg_buf.as<char>();
@@ -25,8 +23,7 @@ int reg_arrays(ll_ctx* ctx, int M, RegArrays* A) {
   A->cap = cap;
   A->feat = (float4*)take((size_t)cap * 16); A->blk_a = (float4*)take((size_t)cap * 16); A->blk_v = (double*)take((size_t)cap * 24);
   A->l1 = (double*)take((size_t)cap * 8); A->l1_sorted = (double*)take((size_t)cap * 8 + 64); A->l1_unique = (double*)take((size_t)cap * 8);
-  A->partials = (double*)take((size_t)ctx->num_sms * 32 * 8);
-  A->n_unique = (int*)take(256); A->counts = (int*)take(256); A->bounds = (float*)take(256); A->pose_tmp = (double*)take(256);
+  A->n_unique = (int*)take(256); A->counts = (int*)take(256); A->bounds = (float*)take(256);
   A->knn_idx = (int*)take((size_t)cap * 20); A->knn_d = (float*)take((size_t)cap * 20); A->perm = (int*)take((size_t)cap * 4);
   A->tmp_a = (float4*)take((size_t)scap * 16); A->tmp_b = (float4*)take((size_t)scap * 16); A->tmp_c = (float4*)take((size_t)scap * 16); A->tmp_d = (float4*)take((size_t)scap * 16);
   return LL_OK;
@@ -65,7 +62,6 @@ int ll_ctx_create(const ll_config* cfg, int device, ll_ctx** out) {
   ll_ctx* ctx = new ll_ctx();
   ctx->device = device;
   if (cfg) ctx->cfg = *cfg; else ll_config_default(&ctx->cfg);
-  { const char* e = getenv("LL_KNN_TMA"); ctx->knn_tma = (e && e[0] == '1') ? 1 : 0; }
   // every call is checked: the first failure wins and the half-built context is torn down by ll_ctx_destroy (which tolerates null members)
   cudaError_t e = cudaSetDevice(device);
   auto ok = [&](cudaError_t r) { if (e == cudaSuccess && r != cudaSuccess) e = r; };
@@ -360,11 +356,11 @@ static KnnBlocksArgs knn_args(ll_ctx* ctx, const ll_map* map, const RegArrays& A
   a.rank = map->rank; a.world = map->world; a.grid = map->grid; a.shard_owner = (const int*)map->shard_owner.p;
   return a;
 }
-static SolveArgs solve_args(ll_ctx* ctx, const RegArrays& A, int M, int mode, int max_iter) {
+static SolveArgs solve_args(ll_ctx* ctx, const RegArrays& A, int M, SolveMode mode, int max_iter) {
   SolveArgs s; s.st = ctx->d_reg; s.sync = ctx->d_sync; s.feat = A.feat; s.blk_a = A.blk_a; s.blk_v = A.blk_v; s.l1 = A.l1; s.l1_sorted_unique = A.l1_unique; s.d_n_unique = A.n_unique;
-  s.partials = A.partials; s.M = M; s.max_iterations = max_iter; s.mode = mode; s.rank = ctx->rank; s.world = ctx->solve_world; s.comm_local = (double*)ctx->comm_local;
+  s.M = M; s.max_iterations = max_iter; s.mode = mode; s.rank = ctx->rank; s.world = ctx->solve_world; s.comm_local = (double*)ctx->comm_local;
   for (int i = 0; i < 8; i++) s.comm_peer[i] = (double*)ctx->comm_peers[i];
-  s.cap_check = 0; s.deblur = ctx->reg_deblur; s.prerun_iterations = 0; s.table = nullptr; s.table_mask = 0; s.uniq = nullptr; s.n_uniq = nullptr;
+  s.cap_check = 0; s.deblur = ctx->reg_deblur; s.prerun_iterations = 0; s.table = nullptr; s.table_mask = 0;
   return s;
 }
 
@@ -417,20 +413,20 @@ int register_device(ll_ctx* ctx, const ll_map* map, const RegArrays& A, int nc, 
     if (e) LL_CUDA(ctx, cudaEventRecord(e[1], s));
     if (it == 0) LL_CUDA(ctx, cudaEventRecord(ctx->ev2, s));
     if (!sharded) {
-      // one launch: solve #1 -> L1 norms -> de-duplication + order statistic -> outlier drop -> solve #2 -> pose (lm_solve_kernel, mode 4)
-      SolveArgs sa = solve_args(ctx, A, M, 4, in->cere_max_iterations);
+      // one launch: solve #1 -> L1 norms -> de-duplication + order statistic -> outlier drop -> solve #2 -> pose
+      SolveArgs sa = solve_args(ctx, A, M, SOLVE_FUSED, in->cere_max_iterations);
       sa.prerun_iterations = in->cere_prerun_times; sa.table = (unsigned long long*)ctx->scratch.p; sa.table_mask = set_cap - 1;
-      sa.n_uniq = (int*)A.l1_sorted; sa.uniq = A.l1_sorted + 2; sa.cap_check = cap_check;
+      sa.cap_check = cap_check;
       if (e) { LL_CUDA(ctx, cudaEventRecord(e[2], s)); LL_CUDA(ctx, cudaEventRecord(e[3], s)); }
       LL_TRY(launch_solve(ctx, sa));
     } else {
       if (cap_check) LL_TRY(launch_count_exchange(ctx));
-      { SolveArgs sa = solve_args(ctx, A, M, 0, in->cere_prerun_times); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
+      { SolveArgs sa = solve_args(ctx, A, M, SOLVE_FIRST, in->cere_prerun_times); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
       if (e) LL_CUDA(ctx, cudaEventRecord(e[2], s));
       LL_TRY(launch_l1_exchange(ctx, A.l1, M));
       LL_TRY(launch_inlier_select(ctx, x_l1, M, in->inlier_ratio, A.l1_sorted, A.l1_unique, A.n_unique));
       if (e) LL_CUDA(ctx, cudaEventRecord(e[3], s));
-      { SolveArgs sa = solve_args(ctx, A, M, 1, in->cere_max_iterations); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
+      { SolveArgs sa = solve_args(ctx, A, M, SOLVE_SECOND, in->cere_max_iterations); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
     }
     if (e) LL_CUDA(ctx, cudaEventRecord(e[4], s));
     LL_CUDA(ctx, cudaMemcpyAsync(slots[it & 1], ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
@@ -553,7 +549,7 @@ int ll_normal_equations(ll_ctx* ctx, const double x[7], double out28[28]) {
   RegArrays A; LL_TRY(reg_arrays(ctx, M, &A));
   cudaStream_t s = ctx->stream;
   LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg->x, x, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
-  LL_TRY(launch_solve(ctx, solve_args(ctx, A, M, 3, 0)));
+  LL_TRY(launch_solve(ctx, solve_args(ctx, A, M, SOLVE_EVALUATE, 0)));
   RegDevState* hs = (RegDevState*)((char*)ctx->pinned + align256(sizeof(RegDevState)));
   LL_CUDA(ctx, cudaMemcpyAsync(hs, ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
@@ -569,7 +565,7 @@ int ll_solve(ll_ctx* ctx, int max_iterations, double x_io[7], double* initial_co
   RegArrays A; LL_TRY(reg_arrays(ctx, M, &A));
   cudaStream_t s = ctx->stream;
   LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg->x, x_io, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
-  LL_TRY(launch_solve(ctx, solve_args(ctx, A, M, 2, max_iterations)));
+  LL_TRY(launch_solve(ctx, solve_args(ctx, A, M, SOLVE_PLAIN, max_iterations)));
   RegDevState* hs = (RegDevState*)((char*)ctx->pinned + align256(sizeof(RegDevState)));
   LL_CUDA(ctx, cudaMemcpyAsync(hs, ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
@@ -703,7 +699,7 @@ int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, d
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   int* h = (int*)ctx->pinned + 8192;
   const int nc = h[5], ns = h[7], meta_scans = h[13];
-  { int lo = h[10], hi = h[11]; lo = lo >= 0 ? lo : lo ^ 0x7fffffff; hi = hi >= 0 ? hi : hi ^ 0x7fffffff; memcpy(&ctx->last_full_min_t, &lo, 4); memcpy(&ctx->last_full_max_t, &hi, 4); }
+  ctx->last_full_min_t = ll_ord2f(h[10]); ctx->last_full_max_t = ll_ord2f(h[11]);
   *nc_out = nc; *ns_out = ns;
   *dropped = (meta_scans <= 5 && !pc->whole_frame) ? 1 : 0;
   if (*dropped) return LL_OK;

@@ -19,7 +19,6 @@
 #include "kernels.cuh"
 #include "exact_math.cuh"
 
-static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 #define CM_EMPTY 0xffffffffffffffffull
 #define CM_BIAS (1 << 20)
 

@@ -14,7 +14,6 @@
 #include "select.cuh"
 
 #define FULL 0xffffffffu
-static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 // ------------------------------------------------------------------------------------------------ upload / repack
 __global__ void repack_pcl32_kernel(const float* __restrict__ src, int n, float4* __restrict__ dst) {
@@ -115,14 +114,12 @@ struct VgMeta {
   float inv;
   int ticket;           // blocks of vg_minmax_setup_kernel that have finished (the last one does the set-up and resets it)
 };
-__device__ __forceinline__ int f2ord(float f) { int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }
-__device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
 
 // Min / max over the finite points, then -- by the last block to finish -- the grid set-up of VoxelGrid::applyFilter (one launch instead of
 // init + minmax + setup; `m` is cleared by a memset node: mins are kept as the bitwise complement of their order-preserving key, so that
 // "all zero" is the neutral element of the atomicMax that reduces both the mins and the maxs).
-__device__ __forceinline__ unsigned f2key(float f) { return (unsigned)f2ord(f) ^ 0x80000000u; }     // unsigned order == float order
-__device__ __forceinline__ float key2f(unsigned k) { return ord2f((int)(k ^ 0x80000000u)); }
+__device__ __forceinline__ unsigned f2key(float f) { return (unsigned)ll_f2ord(f) ^ 0x80000000u; }     // unsigned order == float order
+__device__ __forceinline__ float key2f(unsigned k) { return ll_ord2f((int)(k ^ 0x80000000u)); }
 __global__ void vg_minmax_setup_kernel(const float4* __restrict__ in, VgMeta* m, int n_host, const int* __restrict__ d_n, float leaf) {
   const int n = d_n ? min(*d_n, n_host) : n_host;
   float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY}; int cnt = 0;

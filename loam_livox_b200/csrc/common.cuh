@@ -3,11 +3,11 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <string.h>
 #include <string>
 #include <vector>
 #include "../../include/loamlivox_b200.h"
 
-#define LL_WARP 32
 #define LL_KNN 5
 
 #define LL_CUDA(ctx, expr)                                                                        \
@@ -19,6 +19,27 @@
     }                                                                                             \
   } while (0)
 #define LL_TRY(expr) do { int _s = (expr); if (_s != LL_OK) return _s; } while (0)
+
+// sub-allocations inside one device arena start on 256-byte boundaries
+static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// Order-preserving float <-> int encoding: for non-NaN floats, int order == float order, so box bounds reduce with integer atomicMin / atomicMax.
+__host__ __device__ inline int ll_f2ord(float f) {
+#ifdef __CUDA_ARCH__
+  const int i = __float_as_int(f);
+#else
+  int i; memcpy(&i, &f, 4);
+#endif
+  return i >= 0 ? i : i ^ 0x7fffffff;
+}
+__host__ __device__ inline float ll_ord2f(int i) {
+  i = i >= 0 ? i : i ^ 0x7fffffff;
+#ifdef __CUDA_ARCH__
+  return __int_as_float(i);
+#else
+  float f; memcpy(&f, &i, 4); return f;
+#endif
+}
 
 // ------------------------------------------------------------------------------------------------ device arrays
 struct DevBuf {  // grow-only device allocation
@@ -45,10 +66,10 @@ struct DevBuf {  // grow-only device allocation
 };
 
 // ------------------------------------------------------------------------------------------------ map index
-// "Bucket tree": map points sorted along a 63-bit Hilbert curve (isotropic cells), cut into leaf buckets of 32 points
-// (512 B = one coalesced warp load), with a 32-ary tree of axis-aligned boxes above them (a node record = its 32 children's
-// boxes, 1 KB).  Search is exact: a box gives a true lower bound of the fp32 distance.  lo[l] holds level l's node records;
-// hi[0] the base of the node array (top level first).
+// "Bucket tree": map points sorted along a Hilbert curve (isotropic cells, 3 x 5..21 key bits: the width follows the map size), cut into
+// leaf buckets of 32 points (512 B = one coalesced warp load), with a 32-ary tree of axis-aligned boxes above them (a node record = its 32
+// children's boxes, 1 KB).  Search is exact: a box gives a true lower bound of the fp32 distance.  lo[l] holds level l's node records
+// (the node array is laid out top level first).
 #define LL_MAX_LEVELS 8
 struct BucketTree {
   int n = 0;             // points given (the count of finite ones stays on the device)
@@ -56,8 +77,7 @@ struct BucketTree {
   int n_levels = 0;      // number of box levels (>= 1 when n > 0)
   int level_count[LL_MAX_LEVELS] = {0};   // boxes per level (unpadded)
   float4* pts = nullptr;                  // [n_pad] x,y,z, w = __int_as_float(original index); pad = +inf
-  float4* lo[LL_MAX_LEVELS] = {nullptr};  // [level_count padded to 32] box minima (w unused)
-  float4* hi[LL_MAX_LEVELS] = {nullptr};
+  float4* lo[LL_MAX_LEVELS] = {nullptr};  // [level_count x 64] node records: child c of node j = rec[2c] (min xyz), rec[2c + 1] (max xyz), rec = lo[l] + 64 j
   float4* src = nullptr;                  // [n_src] the cloud as given to ll_map_build (x,y,z,intensity)
   int n_src = 0;
   float* d_bbox = nullptr;                // device: min xyz, max xyz of the finite points (6 floats inside `storage`)
@@ -98,7 +118,7 @@ struct ExtractState {
 };
 
 // Solver / registration device state shared between kernels (lives in global memory)
-struct RegDevState;  // defined in solve.cuh
+struct RegDevState;  // defined in kernels.cuh
 
 struct ll_ctx {
   int device = 0;
@@ -112,7 +132,6 @@ struct ll_ctx {
   int last_nc = 0, last_ns = 0;   // features of the last registration (ll_last_features_dev)
   float last_full_min_t = 10000.f, last_full_max_t = -10000.f;   // find_min_max_intensity over the last front end's full cloud (laser_mapping.hpp:1336)
   int num_sms = 0;
-  int knn_tma = 0;         // LL_KNN_TMA=1 in the environment at ll_ctx_create: the variant of knn_blocks_kernel that stages leaf buckets with cp.async.bulk (measurement only)
   // arenas
   DevBuf scratch;      // CUB temp storage
   DevBuf stage_in;     // raw uploads (PCL32 or XYZI16)

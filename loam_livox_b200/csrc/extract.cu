@@ -15,8 +15,6 @@
 #include "common.cuh"
 #include "kernels.cuh"
 
-static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 #define SELF_EDGE_SRC 0x80   // private: this point raised e_pt_circle_edge (marks idx-2, idx-1, idx+1 too)
 #define SELF_PROCESSED 0x40  // private: the point went through the normal projection path (e_pt_small_view_angle is never set by the reference)
 #define PUBLIC_MASK 0x3f
@@ -200,12 +198,11 @@ __global__ void ex_piece_kernel(const int* __restrict__ scan_first, const int* _
   out[2 * i + 1] = ((float)scan_last[end_scans < 0 ? 0 : end_scans]) / (float)n;
 }
 
-__device__ __forceinline__ int ts_ord(float f) { int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }   // order-preserving float -> int
 // K3: membership flags packed for one 64-bit prefix sum: bits 0-20 corner, 21-41 surface, 42-62 full
 __global__ void ex_flags_kernel(int n, const int* __restrict__ pt_type, const int* __restrict__ pt_label, const float* __restrict__ depth, const float* __restrict__ d_bounds,
                                 float min_blur, float max_blur, unsigned long long* __restrict__ packed, int* __restrict__ counts) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i == 0) { counts[10] = ts_ord(10000.0f); counts[11] = ts_ord(-10000.0f); }   // find_min_max_intensity's start values (laser_mapping.hpp:1246-1247)
+  if (i == 0) { counts[10] = ll_f2ord(10000.0f); counts[11] = ll_f2ord(-10000.0f); }   // find_min_max_intensity's start values (laser_mapping.hpp:1246-1247)
   if (i >= n) return;
   if (d_bounds) { min_blur = d_bounds[0]; max_blur = d_bounds[1]; }
   const float maximum_idx = max_blur * (float)n, minimum_idx = min_blur * (float)n;
@@ -231,7 +228,7 @@ __global__ void ex_scatter_kernel(int n, const float4* __restrict__ raw, const f
   const unsigned long long f = in ? packed[i] : 0ull, o = in ? offs[i] : 0ull;
   float4 p = make_float4(0.f, 0.f, 0.f, 0.f); if (in) { p = raw[i]; p.w = time_stamp[i]; }
   // find_min_max_intensity over the full cloud (laser_mapping.hpp:1243-1253, :1336): min / max time stamp of the points that go to `full`
-  { const bool fl = (f >> 42) & 1ull; const int k = ts_ord(p.w);
+  { const bool fl = (f >> 42) & 1ull; const int k = ll_f2ord(p.w);
     const int mn = __reduce_min_sync(0xffffffffu, fl ? k : 0x7fffffff), mx = __reduce_max_sync(0xffffffffu, fl ? k : (int)0x80000000);
     if ((threadIdx.x & 31) == 0 && mn != 0x7fffffff) { atomicMin(&counts[10], mn); atomicMax(&counts[11], mx); } }
   if (!in) return;

@@ -5,13 +5,17 @@
 struct TreeView {
   const float4* pts;                    // [n_pad] Hilbert-ordered points, w = original index
   const float4* src;                    // [n_src] the cloud in its original order
-  const float4* nodes[LL_MAX_LEVELS];   // node records per level (6 float4 each); level 0's children are the 8-point buckets
+  const float4* nodes[LL_MAX_LEVELS];   // node records per level (64 float4 each: 32 child boxes); level 0's children are the 32-point buckets
   int n, n_levels;
   const float* bbox;                    // device: map bounding box (min xyz, max xyz)
 };
 TreeView make_view(const BucketTree& t);
 int build_bucket_tree(ll_ctx* ctx, const float4* d_src, int n_src, BucketTree* t);
 int build_bucket_tree_on(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_src, int n_src, BucketTree* t);
+// Bounding box of the finite points (knn.cu): bbox[0..2] = min, bbox[3..5] = max (ll_f2ord encoding), bbox[6] = their count.
+// bbox_init_kernel (one warp) resets it; every bbox_kernel launch after that widens it by one more cloud.
+__global__ void bbox_init_kernel(int* bbox);
+__global__ void bbox_kernel(const float4* __restrict__ src, int n, int* __restrict__ bbox);
 
 struct RegDevState;
 struct KnnBlocksArgs {
@@ -53,7 +57,6 @@ struct RegDevState {
   int cap, rng_seed, n_blocks_all;
   // motion deblur (N1): time-stamp range of refine_blur, and compute_interpolatation_rodrigue's outputs (:607-620) after every solve #2
   double min_ts, max_ts, interp_theta, interp_hat[9], interp_hat_sq[9];
-  unsigned int bar_count, bar_gen;
   long long prof[16];  // [8..12]: fused K10 section: L1 + insert, barrier, select, barrier, drop   // master-CTA cycle counters of the solver: eval, wait, grid reduce, lm_step, publish, #evaluations, staging, epilogue
   LmState lm;
 };
@@ -69,6 +72,14 @@ struct SolveSync {
   unsigned gen;                       // generation base of the next launch; grows monotonically over the life of the context
 };
 
+// What one lm_solve_kernel launch does.
+enum SolveMode : int {
+  SOLVE_FIRST = 0,      // solve #1, then the L1 norm of every block at the solution (sharded mode)
+  SOLVE_SECOND = 1,     // drop the blocks above the inlier threshold, solve #2, compose the pose + ICP termination test (sharded mode)
+  SOLVE_PLAIN = 2,      // one plain solve (parity hook)
+  SOLVE_EVALUATE = 3,   // evaluate once at st->x, sums to st->lm.H / g / x_cost (parity hook)
+  SOLVE_FUSED = 4,      // one whole ICP iteration in one launch: solve #1 -> K10 inlier threshold -> solve #2 -> pose
+};
 struct SolveArgs {
   RegDevState* st;
   SolveSync* sync;
@@ -78,15 +89,13 @@ struct SolveArgs {
   double* l1;                // [M] loss-corrected L1 norm per slot (+inf for invalid slots)
   const double* l1_sorted_unique;  // [>= n_unique] for the threshold of solve #2
   const int* d_n_unique;
-  double* partials;          // [grid x 32]
   int M;
   int max_iterations;
-  int mode;                  // 4: fused (see below) ; 0: solve #1 (write l1 at the end) ; 1: solve #2 (apply threshold first, compose pose at the end) ;
-                             // 2: plain solve (parity hook) ; 3: evaluate once at st->x (parity hook, writes sums to st->lm.H/g/x_cost)
+  SolveMode mode;
   // multi-GPU
   int rank, world; double* comm_local; double* comm_peer[8];
-  // mode 4 (one launch per ICP iteration: solve #1 -> K10 -> solve #2)
-  int prerun_iterations; unsigned long long* table; unsigned table_mask; double* uniq; int* n_uniq;
+  // SOLVE_FUSED: solve #1's iteration count and the hash set of the L1 norms (K10)
+  int prerun_iterations; unsigned long long* table; unsigned table_mask;
   int cap_check;             // 1: the block count can exceed the cap (host: slots > cap): apply the drop rule (:434-458) while staging
   int deblur;                // 1: *_mb functors (ceres_icp.hpp:81-233), s per block from the feature's time stamp
 };
@@ -105,7 +114,6 @@ int solve_prepare(ll_ctx* ctx);   // once per context: opt the solver kernels in
 int launch_l1_exchange(ll_ctx* ctx, const double* d_l1, int M);
 // Sharded mode, residual-block cap: all ranks' block counts of this ICP iteration summed into RegDevState::n_blocks_all (peer stores + flags).
 int launch_count_exchange(ll_ctx* ctx);
-int solve_max_slots(ll_ctx* ctx);
 
 // ---------------------------------------------------------------------------------------------- clouds (cloud.cu)
 int upload_cloud(ll_ctx* ctx, const void* src, size_t n, int fmt, int where, float4* d_dst);   // async on ctx->stream
@@ -129,8 +137,8 @@ int launch_piece_bounds(ll_ctx* ctx, int pieces, float* d_start_end /* 2*pieces 
 
 // ---------------------------------------------------------------------------------------------- host driver pieces (api.cu)
 struct RegArrays {
-  float4* feat; float4* blk_a; double* blk_v; double* l1; double* l1_sorted; double* l1_unique; double* partials;
-  int* n_unique; int* knn_idx; float* knn_d; int* perm; float4* tmp_a; float4* tmp_b; float4* tmp_c; float4* tmp_d; int* counts; float* bounds; double* pose_tmp;
+  float4* feat; float4* blk_a; double* blk_v; double* l1; double* l1_sorted; double* l1_unique;
+  int* n_unique; int* knn_idx; float* knn_d; int* perm; float4* tmp_a; float4* tmp_b; float4* tmp_c; float4* tmp_d; int* counts; float* bounds;
   int cap;
 };
 int reg_arrays(ll_ctx* ctx, int M, RegArrays* A);

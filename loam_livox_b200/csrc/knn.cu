@@ -17,18 +17,13 @@
 #include "exact_math.cuh"
 
 #define FULL 0xffffffffu
-#ifndef LL_GROUP
-#define LL_GROUP 32
-#endif
-#define BUCKET LL_GROUP  // points per leaf bucket (one per lane of a query group)
-#define FANOUT LL_GROUP  // children per node; a node record holds its 8 children's boxes, child c = rec[2c] (lo.xyz) + rec[2c+1] (hi.xyz): 256 B
-#define NODE_F4 (2 * LL_GROUP)
+#define BUCKET 32     // points per leaf bucket: one per lane of the query's warp
+#define FANOUT 32     // children per node; a node record holds its 32 children's boxes, child c = rec[2c] (lo.xyz) + rec[2c+1] (hi.xyz): 1 KB
+#define NODE_F4 64    // float4s per node record
+static_assert(BUCKET == 32 && FANOUT == 32 && NODE_F4 == 2 * FANOUT, "the search maps one bucket point / one child box to each lane of a warp");
 
 // ------------------------------------------------------------------------------------------------ build
-__device__ __forceinline__ int f2ord(float f) { int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }
-__device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
-
-// bbox[0..2] = min (ordered-int encoding), bbox[3..5] = max, bbox[6] = number of finite points
+// bbox[0..2] = min (ll_f2ord encoding), bbox[3..5] = max, bbox[6] = number of finite points
 __global__ void bbox_kernel(const float4* __restrict__ src, int n, int* __restrict__ bbox) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
@@ -49,13 +44,13 @@ __global__ void bbox_kernel(const float4* __restrict__ src, int n, int* __restri
   }
   if ((threadIdx.x & 31) == 0) {
 #pragma unroll
-    for (int k = 0; k < 3; k++) { atomicMin(&bbox[k], f2ord(lo[k])); atomicMax(&bbox[3 + k], f2ord(hi[k])); }
+    for (int k = 0; k < 3; k++) { atomicMin(&bbox[k], ll_f2ord(lo[k])); atomicMax(&bbox[3 + k], ll_f2ord(hi[k])); }
     atomicAdd(&bbox[6], cnt);
   }
 }
 __global__ void bbox_init_kernel(int* bbox) {
-  if (threadIdx.x < 3) bbox[threadIdx.x] = f2ord(INFINITY);
-  else if (threadIdx.x < 6) bbox[threadIdx.x] = f2ord(-INFINITY);
+  if (threadIdx.x < 3) bbox[threadIdx.x] = ll_f2ord(INFINITY);
+  else if (threadIdx.x < 6) bbox[threadIdx.x] = ll_f2ord(-INFINITY);
   else if (threadIdx.x == 6) bbox[6] = 0;
 }
 
@@ -68,8 +63,33 @@ __device__ __forceinline__ unsigned long long spread21(unsigned v) {
   x = (x | x << 2) & 0x1249249249249249ull;
   return x;
 }
-// Hilbert index (Skilling's transpose form, `bits` per axis, <= 21) on an ISOTROPIC grid (one scale for all axes): consecutive runs along a
-// Hilbert curve are connected blobs, so fixed-size buckets get tight, nearly cubic boxes.  The key only decides WHICH points share a bucket (the
+// Hilbert index (Skilling's transpose form, `bits` per axis, <= 21) of the finite point c on an ISOTROPIC grid over the box lo..hi (one scale
+// for all axes, the box's longest side), axes interleaved x first: < 2^(3 bits).  Consecutive runs along a Hilbert curve are connected blobs.
+__device__ __forceinline__ unsigned long long hilbert_key(const float c[3], const float lo[3], const float hi[3], int bits) {
+  const float ext = fmaxf(fmaxf(hi[0] - lo[0], hi[1] - lo[1]), hi[2] - lo[2]);
+  const float scale = (float)(1u << bits), top = scale - 1.0f;
+  unsigned X[3];
+#pragma unroll
+  for (int k = 0; k < 3; k++) {
+    float u = ext > 0.f ? (c[k] - lo[k]) / ext : 0.f;
+    u = fminf(fmaxf(u, 0.f), 1.f);
+    X[k] = (unsigned)fminf(u * scale, top);
+  }
+  for (unsigned Q = 1u << (bits - 1); Q > 1; Q >>= 1) {
+    const unsigned P = Q - 1;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+      if (X[k] & Q) X[0] ^= P;
+      else { unsigned t = (X[0] ^ X[k]) & P; X[0] ^= t; X[k] ^= t; }
+    }
+  }
+  X[1] ^= X[0]; X[2] ^= X[1];
+  unsigned t = 0;
+  for (unsigned Q = 1u << (bits - 1); Q > 1; Q >>= 1) if (X[2] & Q) t ^= Q - 1;
+  X[0] ^= t; X[1] ^= t; X[2] ^= t;
+  return (spread21(X[0]) << 2) | (spread21(X[1]) << 1) | spread21(X[2]);
+}
+// Map keys: fixed-size buckets of consecutive points get tight, nearly cubic boxes.  The key only decides WHICH points share a bucket (the
 // boxes are computed from the points themselves, so the search is exact for any key): its width follows the map size (about 8 cells per bucket
 // side at the finest level), which is what bounds the number of radix passes of the sort below.
 template <typename KeyT>
@@ -79,29 +99,9 @@ __global__ void hilbert_kernel(const float4* __restrict__ src, int n, const int*
   float4 p = src[i];
   unsigned long long key = 1ull << (3 * bits);   // non-finite points: one bit above every real key -> they sort to the end
   if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) {
-    const float lo[3] = {ord2f(bbox[0]), ord2f(bbox[1]), ord2f(bbox[2])}, hi[3] = {ord2f(bbox[3]), ord2f(bbox[4]), ord2f(bbox[5])};
-    const float ext = fmaxf(fmaxf(hi[0] - lo[0], hi[1] - lo[1]), hi[2] - lo[2]);
-    const float c[3] = {p.x, p.y, p.z}; unsigned X[3];
-    const float scale = (float)(1u << bits), top = scale - 1.0f;
-#pragma unroll
-    for (int k = 0; k < 3; k++) {
-      float u = ext > 0.f ? (c[k] - lo[k]) / ext : 0.f;
-      u = fminf(fmaxf(u, 0.f), 1.f);
-      X[k] = (unsigned)fminf(u * scale, top);
-    }
-    for (unsigned Q = 1u << (bits - 1); Q > 1; Q >>= 1) {
-      const unsigned P = Q - 1;
-#pragma unroll
-      for (int k = 0; k < 3; k++) {
-        if (X[k] & Q) X[0] ^= P;
-        else { unsigned t = (X[0] ^ X[k]) & P; X[0] ^= t; X[k] ^= t; }
-      }
-    }
-    X[1] ^= X[0]; X[2] ^= X[1];
-    unsigned t = 0;
-    for (unsigned Q = 1u << (bits - 1); Q > 1; Q >>= 1) if (X[2] & Q) t ^= Q - 1;
-    X[0] ^= t; X[1] ^= t; X[2] ^= t;
-    key = (spread21(X[0]) << 2) | (spread21(X[1]) << 1) | spread21(X[2]);   // < 2^(3 bits)
+    const float lo[3] = {ll_ord2f(bbox[0]), ll_ord2f(bbox[1]), ll_ord2f(bbox[2])}, hi[3] = {ll_ord2f(bbox[3]), ll_ord2f(bbox[4]), ll_ord2f(bbox[5])};
+    const float c[3] = {p.x, p.y, p.z};
+    key = hilbert_key(c, lo, hi, bits);
   }
   keys[i] = (KeyT)key;
   vals[i] = i;
@@ -140,10 +140,8 @@ __global__ void node_kernel(const float4* __restrict__ pts, const float4* __rest
   o[2 * c] = make_float4(l0, l1, l2, 0.f); o[2 * c + 1] = make_float4(h0, h1, h2, 0.f);
 }
 __global__ void bbox_publish_kernel(const int* __restrict__ bbox, float* __restrict__ out6) {   // decoded box for the query-sort kernel
-  if (threadIdx.x < 6) out6[threadIdx.x] = ord2f(bbox[threadIdx.x]);
+  if (threadIdx.x < 6) out6[threadIdx.x] = ll_ord2f(bbox[threadIdx.x]);
 }
-
-static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 // Everything is enqueued on the context's stream and nothing is read back: the layout is sized from n_src (the non-finite points -- there are
 // usually none -- only leave a few all-pad buckets with neutral boxes at the end), the count of finite points and the box stay on the device.
@@ -182,7 +180,6 @@ int build_bucket_tree_on(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const flo
   t->pts = (float4*)p; p += align256((size_t)t->n_pad * 16);
   float4* nodes = (float4*)p; p += align256(node_total * NODE_F4 * 16);
   { size_t off = 0; for (int l = t->n_levels - 1; l >= 0; l--) { t->lo[l] = nodes + off * NODE_F4; off += (size_t)t->level_count[l]; } }
-  t->hi[0] = nodes;   // base of the node array (top level first)
   t->src = (float4*)p; p += align256((size_t)n_src * 16);
   t->d_bbox = (float*)p;
   bbox_init_kernel<<<1, 32, 0, s>>>(bbox); ctx->launches++;
@@ -273,32 +270,13 @@ __device__ __forceinline__ void top_merge(LaneTop& t, float d, int id, bool c, i
 
 struct WarpWalk { float lb[KNN_LEVELS][32]; };   // per warp: the child bounds of the node open at every level
 
-// ---- optional TMA staging of leaf buckets (LL_KNN_TMA=1; north_star's "TMA/shared-memory staging of KD-tree leaf buckets") --------------------
-// When a level-0 node is opened, the two nearest qualifying buckets are fetched with cp.async.bulk (512 B each) into a warp-private double buffer
-// in shared memory, completion on an mbarrier; the pick that reaches such a bucket waits on the barrier and reads its point from shared memory
-// instead of issuing the load itself.  Same visiting order, same results.  Not measured on the H100 (DESIGN.md §7).
-struct __align__(16) WarpStage { float4 pts[2][32]; unsigned long long bar[2]; };
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity) {
-  asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gmem, unsigned bytes, unsigned long long* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
 // All 32 lanes of the warp call this together; `active` is warp-uniform.
 // seed_ids: the query's 5 neighbours of the previous ICP iteration (or null / -1): their distances to the moved query seed the list, so the
 // bound is tight before the first box is opened.
-template <bool TMA>
-__device__ __forceinline__ void warp_knn5(const TreeView& tv, WarpWalk& ws, WarpStage* stg, bool active, float qx, float qy, float qz, LaneTop& t, const int* seed_ids) {
+__device__ __forceinline__ void warp_knn5(const TreeView& tv, WarpWalk& ws, bool active, float qx, float qy, float qz, LaneTop& t, const int* seed_ids) {
   const int lane = threadIdx.x & 31;
   top_init(t);
   if (!(active && tv.n > 0)) return;
-  int pre_child[2] = {-1, -1}; unsigned pre_phase[2] = {0u, 0u};   // TMA: which bucket sits (or is landing) in each stage, and the barrier's next parity
-  if (TMA) { if (lane == 0) { mbar_init(&stg->bar[0], 1); mbar_init(&stg->bar[1], 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); } __syncwarp(); }
   if (seed_ids) {
     int sid = -1;
     if (lane < LL_KNN) sid = seed_ids[lane];
@@ -321,24 +299,6 @@ __device__ __forceinline__ void warp_knn5(const TreeView& tv, WarpWalk& ws, Warp
       const unsigned m = __ballot_sync(FULL, lb <= t.d5 && lb < INFINITY);
       if (lane == l) remv = m;
       open_node = false;   // (every lane only ever reads back its own slot of the row: no synchronisation needed)
-      if (TMA && l == 0 && m) {   // stage the two nearest qualifying buckets
-        const unsigned k1 = ((m >> lane) & 1u) ? __float_as_uint(lb) : 0xffffffffu;
-        const unsigned m1 = __reduce_min_sync(FULL, k1);
-        const int c1 = __ffs(__ballot_sync(FULL, k1 == m1)) - 1;
-        const unsigned k2 = lane == c1 ? 0xffffffffu : k1;
-        const unsigned m2 = __reduce_min_sync(FULL, k2);
-        const int c2 = m2 == 0xffffffffu ? -1 : __ffs(__ballot_sync(FULL, k2 == m2)) - 1;
-        const int want[2] = {idx * FANOUT + c1, c2 >= 0 ? idx * FANOUT + c2 : -1};
-#pragma unroll
-        for (int b = 0; b < 2; b++) {
-          if (pre_child[b] >= 0) { mbar_wait(&stg->bar[b], pre_phase[b]); pre_phase[b] ^= 1u; pre_child[b] = -1; }   // a staged bucket that was pruned: let its copy land first
-          if (want[b] >= 0) {
-            __syncwarp(); fence_proxy_async();   // every lane is done reading the stage (generic proxy) before the async proxy overwrites it
-            if (lane == 0) { mbar_expect_tx(&stg->bar[b], 512u); tma_bulk_g2s(stg->pts[b], tv.pts + (size_t)want[b] * BUCKET, 512u, &stg->bar[b]); }
-            pre_child[b] = want[b];
-          }
-        }
-      }
     }
     // pick the nearest remaining child of the node open at level l that can still hold a neighbour
     const float lb = ws.lb[l][lane];
@@ -356,24 +316,11 @@ __device__ __forceinline__ void warp_knn5(const TreeView& tv, WarpWalk& ws, Warp
     if (lane == l) remv = okm & ~(1u << c);   // (okm is a subset of rem) the children that failed the test now can never pass it later
     const int child = idx * FANOUT + c;
     if (l == 0) {                // a bucket: one point per lane
-      float4 P;
-      if (TMA && (child == pre_child[0] || child == pre_child[1])) {
-        const int b = child == pre_child[0] ? 0 : 1;
-        mbar_wait(&stg->bar[b], pre_phase[b]); pre_phase[b] ^= 1u; pre_child[b] = -1;
-        P = stg->pts[b][lane];
-      } else P = __ldg(tv.pts + (size_t)child * BUCKET + lane);
+      const float4 P = __ldg(tv.pts + (size_t)child * BUCKET + lane);
       top_merge(t, dist2_exact(qx, qy, qz, P.x, P.y, P.z), __float_as_int(P.w), true, lane);   // pad points are +inf: never candidates
     } else { l--; idx = child; open_node = true; }
   }
-  if (TMA) {   // no copy may still be in flight when the CTA's shared memory goes away
-#pragma unroll
-    for (int b = 0; b < 2; b++) if (pre_child[b] >= 0) mbar_wait(&stg->bar[b], pre_phase[b]);
-  }
 }
-
-#ifdef LL_KNN_R1
-#include "knn_r1.cuh"
-#endif
 
 // Parity hook (ll_knn): world-frame queries in caller order.
 __global__ void __launch_bounds__(KNN_THREADS) knn_query_kernel(TreeView tv, const float4* __restrict__ q, int nq, int* __restrict__ idx5, float* __restrict__ d5) {
@@ -383,12 +330,7 @@ __global__ void __launch_bounds__(KNN_THREADS) knn_query_kernel(TreeView tv, con
   float4 p = make_float4(0.f, 0.f, 0.f, 0.f); if (have) p = __ldg(&q[g]);
   const bool active = have && isfinite(p.x) && isfinite(p.y) && isfinite(p.z);
   LaneTop t;
-#ifdef LL_KNN_R1
-  __shared__ r1::GroupStack stacks[WARPS_PER_CTA];
-  r1::warp_knn5_r1(tv, stacks[threadIdx.x >> 5], active, p.x, p.y, p.z, t, nullptr);
-#else
-  warp_knn5<false>(tv, walks[threadIdx.x >> 5], nullptr, active, p.x, p.y, p.z, t, nullptr);
-#endif
+  warp_knn5(tv, walks[threadIdx.x >> 5], active, p.x, p.y, p.z, t, nullptr);
   if (have && lane < LL_KNN) { idx5[g * LL_KNN + lane] = (t.id == 0x7fffffff) ? -1 : t.id; d5[g * LL_KNN + lane] = t.d; }
 }
 
@@ -403,23 +345,8 @@ __global__ void query_key_kernel(KnnBlocksArgs a, unsigned* __restrict__ keys, i
   double wx, wy, wz; qrot_d(a.pose, (double)f.x, (double)f.y, (double)f.z, wx, wy, wz);
   const float c[3] = {(float)(wx + a.pose[4]), (float)(wy + a.pose[5]), (float)(wz + a.pose[6])};
   const float* bb = is_corner ? a.corner.bbox : a.surf.bbox;   // device memory: the box never visits the host
-  const float ext = fmaxf(fmaxf(bb[3] - bb[0], bb[4] - bb[1]), bb[5] - bb[2]);
-  unsigned X[3]; bool ok = true;
-#pragma unroll
-  for (int k = 0; k < 3; k++) { if (!isfinite(c[k])) ok = false; float u = ext > 0.f ? (c[k] - bb[k]) / ext : 0.f; u = fminf(fmaxf(u, 0.f), 1.f); X[k] = (unsigned)fminf(u * 128.0f, 127.0f); }   // 7 bits per axis: 21-bit curve + class bit = 3 radix passes, and tiles of ~0.3 m are fine enough
-  for (unsigned Q = 1u << 6; Q > 1; Q >>= 1) {
-    const unsigned P = Q - 1;
-#pragma unroll
-    for (int k = 0; k < 3; k++) { if (X[k] & Q) X[0] ^= P; else { unsigned tt = (X[0] ^ X[k]) & P; X[0] ^= tt; X[k] ^= tt; } }
-  }
-  X[1] ^= X[0]; X[2] ^= X[1];
-  unsigned tt = 0;
-  for (unsigned Q = 1u << 6; Q > 1; Q >>= 1) if (X[2] & Q) tt ^= Q - 1;
-  X[0] ^= tt; X[1] ^= tt; X[2] ^= tt;
-  unsigned h = 0;
-#pragma unroll
-  for (int b = 6; b >= 0; b--) h = (h << 3) | (((X[0] >> b) & 1u) << 2) | (((X[1] >> b) & 1u) << 1) | ((X[2] >> b) & 1u);
-  if (!ok) h = 0x1fffffu;
+  // 7 bits per axis: 21-bit curve + class bit = 3 radix passes, and tiles of ~0.3 m are fine enough; non-finite features sort last in their class
+  const unsigned h = (isfinite(c[0]) && isfinite(c[1]) && isfinite(c[2])) ? (unsigned)hilbert_key(c, bb, bb + 3, 7) : 0x1fffffu;
   keys[i] = (is_corner ? 0u : 0x200000u) | h; vals[i] = i;
 }
 
@@ -463,14 +390,12 @@ __device__ __forceinline__ void emit_block(const KnnBlocksArgs& a, const TreeVie
   a.blk_v[(size_t)w * 3 + 0] = vx; a.blk_v[(size_t)w * 3 + 1] = vy; a.blk_v[(size_t)w * 3 + 2] = vz;
 }
 
-// K6 + K7 fused, one query group (LL_GROUP lanes) per scan feature, features taken in spatially sorted order (perm).
+// K6 + K7 fused, one warp per scan feature, features taken in spatially sorted order (perm).
 // Writes one residual-block slot per feature (indexed by the ORIGINAL feature order): blk_a[slot] = (a.x, a.y, a.z, type) with
 // type 0 invalid / 1 line / 2 plane, blk_v[slot*3..] = unit line direction or (un-normalised) plane normal, in fp64.
-template <bool TMA>
 __global__ void __launch_bounds__(KNN_THREADS) knn_blocks_kernel(KnnBlocksArgs a) {
   if (a.st->icp_done) return;   // launched ahead of the termination test by the host: the ICP loop has already ended
   __shared__ WarpWalk walks[WARPS_PER_CTA];
-  __shared__ WarpStage stages[TMA ? WARPS_PER_CTA : 1];
   const int j = blockIdx.x * WARPS_PER_CTA + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   const int M = a.n_corner + a.n_surf;
@@ -511,12 +436,7 @@ __global__ void __launch_bounds__(KNN_THREADS) knn_blocks_kernel(KnnBlocksArgs a
     if (have && ncls > 2 * a.cap) skipped = ll_cap_uniform_f(a.rng_seed, a.st->icp_iter, is_corner ? 0 : 1, is_corner ? w : w - a.n_corner) * (float)ncls > (float)(2 * a.cap); }
   const bool active = have && owned && finite_in && !skipped;
   LaneTop t;
-#ifdef LL_KNN_R1
-  __shared__ r1::GroupStack stacks[WARPS_PER_CTA];
-  r1::warp_knn5_r1(tv, stacks[threadIdx.x >> 5], active, qx, qy, qz, t, (a.seed_ids && have) ? a.seed_ids + (size_t)w * LL_KNN : nullptr);
-#else
-  warp_knn5<TMA>(tv, walks[threadIdx.x >> 5], TMA ? &stages[threadIdx.x >> 5] : nullptr, active, qx, qy, qz, t, (a.seed_ids && have) ? a.seed_ids + (size_t)w * LL_KNN : nullptr);
-#endif
+  warp_knn5(tv, walks[threadIdx.x >> 5], active, qx, qy, qz, t, (a.seed_ids && have) ? a.seed_ids + (size_t)w * LL_KNN : nullptr);
   if (!have) return;
   if (active && lane < LL_KNN) {   // the neighbours seed the next ICP iteration's search (5 lanes, one 20-byte row)
     if (a.seed_ids) a.seed_ids[(size_t)w * LL_KNN + lane] = (t.id == 0x7fffffff) ? -1 : t.id;
@@ -550,8 +470,7 @@ int launch_query_sort(ll_ctx* ctx, const KnnBlocksArgs& a, int* d_perm) {
 int launch_knn_blocks(ll_ctx* ctx, const KnnBlocksArgs& a) {
   int M = a.n_corner + a.n_surf;
   if (M == 0) return LL_OK;
-  if (ctx->knn_tma) knn_blocks_kernel<true><<<ll_div_up(M, WARPS_PER_CTA), KNN_THREADS, 0, ctx->stream>>>(a);
-  else knn_blocks_kernel<false><<<ll_div_up(M, WARPS_PER_CTA), KNN_THREADS, 0, ctx->stream>>>(a);
+  knn_blocks_kernel<<<ll_div_up(M, WARPS_PER_CTA), KNN_THREADS, 0, ctx->stream>>>(a);
   ctx->launches++;
   LL_CUDA(ctx, cudaGetLastError());
   return LL_OK;

@@ -24,7 +24,6 @@ int ll_cellmap_append(ll_ctx*, ll_cellmap*, const void*, size_t, int, int);
 int ll_cellmap_assemble(ll_ctx*, ll_cellmap*, const double*, const double*, float, float, float, int, ll_point*, size_t, size_t*, int*, const ll_point**);
 int ll_cellmap_reserve(ll_ctx*, ll_cellmap*, size_t, size_t);
 }
-static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 static inline double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
 // m_laser_cloud_{corner,surface}_history (std::list<PointCloud>, :1446-1478) as ONE flat device array: the clouds of the window lie one after the

@@ -19,32 +19,6 @@
 #include "common.cuh"
 #include "kernels.cuh"
 
-static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
-__device__ __forceinline__ int sh_f2ord(float f) { int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }
-__device__ __forceinline__ float sh_ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
-
-__global__ void sh_bbox_init_kernel(int* bbox) {
-  if (threadIdx.x < 3) bbox[threadIdx.x] = sh_f2ord(INFINITY);
-  else if (threadIdx.x < 6) bbox[threadIdx.x] = sh_f2ord(-INFINITY);
-}
-__global__ void sh_bbox_kernel(const float4* __restrict__ p, int n, int* __restrict__ bbox) {
-  float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const float4 q = p[i];
-    if (isfinite(q.x) && isfinite(q.y) && isfinite(q.z)) {
-      lo[0] = fminf(lo[0], q.x); lo[1] = fminf(lo[1], q.y); lo[2] = fminf(lo[2], q.z);
-      hi[0] = fmaxf(hi[0], q.x); hi[1] = fmaxf(hi[1], q.y); hi[2] = fmaxf(hi[2], q.z);
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-    for (int k = 0; k < 3; k++) { lo[k] = fminf(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o)); hi[k] = fmaxf(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o)); }
-  if ((threadIdx.x & 31) == 0)
-#pragma unroll
-    for (int k = 0; k < 3; k++) { atomicMin(&bbox[k], sh_f2ord(lo[k])); atomicMax(&bbox[3 + k], sh_f2ord(hi[k])); }
-}
 __global__ void sh_hist_kernel(const float4* __restrict__ p, int n, ShardGrid g, int* __restrict__ hist) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -133,16 +107,16 @@ int ll_map_build_sharded(ll_ctx* ctx, const void* corner, size_t nc, const void*
   // ---- grid over the bounding box of the whole map (identical on every rank: every rank sees the same two clouds)
   LL_CUDA(ctx, ctx->scratch2.reserve(4096));
   int* d_bbox = ctx->scratch2.as<int>();
-  sh_bbox_init_kernel<<<1, 32, 0, s>>>(d_bbox); ctx->launches++;
-  if (nc) { sh_bbox_kernel<<<std::min(ll_div_up((int)nc, 256), ctx->num_sms * 8), 256, 0, s>>>(d_c, (int)nc, d_bbox); ctx->launches++; }
-  if (ns) { sh_bbox_kernel<<<std::min(ll_div_up((int)ns, 256), ctx->num_sms * 8), 256, 0, s>>>(d_s, (int)ns, d_bbox); ctx->launches++; }
+  bbox_init_kernel<<<1, 32, 0, s>>>(d_bbox); ctx->launches++;   // (knn.cu; the count of finite points in d_bbox[6] is not used here)
+  if (nc) { bbox_kernel<<<std::min(ll_div_up((int)nc, 256), ctx->num_sms * 8), 256, 0, s>>>(d_c, (int)nc, d_bbox); ctx->launches++; }
+  if (ns) { bbox_kernel<<<std::min(ll_div_up((int)ns, 256), ctx->num_sms * 8), 256, 0, s>>>(d_s, (int)ns, d_bbox); ctx->launches++; }
   int hb[6];
   LL_CUDA(ctx, cudaMemcpyAsync(hb, d_bbox, sizeof(hb), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   ll_map* m = new ll_map(); m->device = ctx->device; m->rank = rank; m->world = world; m->cell_size = cell_size; m->halo[0] = halo_corner; m->halo[1] = halo_surf;
   ShardGrid& g = m->grid; g.cell = cell_size; g.inv_cell = 1.0f / cell_size;
   float lo[3], hi[3];
-  for (int k = 0; k < 3; k++) { int v = hb[k]; v = v >= 0 ? v : v ^ 0x7fffffff; memcpy(&lo[k], &v, 4); v = hb[3 + k]; v = v >= 0 ? v : v ^ 0x7fffffff; memcpy(&hi[k], &v, 4); }
+  for (int k = 0; k < 3; k++) { lo[k] = ll_ord2f(hb[k]); hi[k] = ll_ord2f(hb[3 + k]); }
   size_t ncell = 1;
   for (int k = 0; k < 3; k++) {
     if (!(lo[k] <= hi[k])) { lo[k] = 0.f; hi[k] = 0.f; }   // no finite point at all

@@ -4,14 +4,15 @@
 //   ceres::Problem / AddResidualBlock / Solve x2   loam_livox/source/point_cloud_registration.hpp:220-228,323,422,460-474,501-508
 //   residual models (autodiff)                     loam_livox/source/ceres_icp.hpp:262-288 (point2line), :338-366 (point2plane)
 //   HuberLoss(0.1), EigenQuaternionParameterization, bounds on t   :220-221, :143-151
-//   problem.Evaluate + inlier threshold front end  :476-499 (the L1 norms are produced here; select.cu finishes K10)
+//   problem.Evaluate + compute_inlier_residual_threshold   :476-499, :153-161 (K10)
 //   pose composition + ICP termination test        :514-531
 //
-// Design: every residual block is staged once into SHARED MEMORY (52 B per block, SoA) of one of the persistent CTAs (one per SM,
-// 132 on an H100) and stays on-chip for the whole solve (up to ~400k blocks).  One evaluation = every thread evaluates r, J (analytic, fp64), the Huber
-// weight and its 28 normal-equation terms, warp-shuffle + shared-memory reduce per CTA, one 29-double partial per CTA,
-// a ticket barrier, and the LAST CTA to arrive reduces the partials in fixed order (run-to-run deterministic), runs the
-// trust-region logic on one thread and publishes the next trial point.  No host round trip inside a solve.
+// Design (DESIGN.md §3.2): every residual block is staged once into SHARED MEMORY (SoA) of one of the persistent CTAs (one per SM, 132 on an
+// H100) and stays on-chip for the whole solve.  One evaluation = every thread evaluates its blocks' r, J, Huber weight and normal-equation
+// terms, a CTA reduce, then a master-less exchange: every CTA publishes its 29 sums in a tagged row, reads all rows and reduces them in fixed
+// order, so every CTA holds bit-identical sums and advances its own copy of the trust-region state.  SOLVE_FUSED runs a whole ICP iteration
+// in one launch: solve #1, the L1 norms, K10's inlier threshold over the grid (hash-set de-duplication + radix select), the outlier drop,
+// solve #2 and the pose.  No host round trip inside a launch.
 #include <cfloat>
 #include <cstdlib>
 #include "common.cuh"
@@ -232,10 +233,10 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   __shared__ LmState s_lm;     // EVERY CTA keeps its own copy of the solver state and advances it identically
   __shared__ double s_gmax;
   __shared__ StepOut s_pre[2]; // the next iteration's ComputeStep under both outcomes of the accept test, evaluated by warp 1 while warp 0 decides
-  __shared__ K10Smem s_k10;    // mode 4 (fused) only
+  __shared__ K10Smem s_k10;    // SOLVE_FUSED only
   RegDevState* st = a.st;
   SolveSync* Y = a.sync;
-  if ((a.mode == 4 || a.mode <= 1) && *((volatile int*)&st->icp_done)) return;   // speculative launch after the ICP loop ended (uniform over the grid)
+  if ((a.mode == SOLVE_FUSED || a.mode <= SOLVE_SECOND) && *((volatile int*)&st->icp_done)) return;   // ICP work (fused, solve #1 or #2) launched after the ICP loop ended (uniform over the grid)
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int cap = tiles_per_cta * SOLVE_THREADS;
   const SmemSlots S = carve(s_dyn, cap, MB);
@@ -243,18 +244,18 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   unsigned gen = *((volatile unsigned*)&Y->gen);   // uniform over the grid: written by the previous launch's CTA 0 at its very end
 
   const long long t_k0 = clock64();
-  // mode 4 = one whole ICP iteration's solver work in ONE launch: solve #1 (prerun iterations) -> L1 norms -> std::set de-duplication + order
+  // SOLVE_FUSED = one whole ICP iteration's solver work in ONE launch: solve #1 (prerun iterations) -> L1 norms -> std::set de-duplication + order
   // statistic (K10) -> drop outliers from the staged blocks -> solve #2 -> pose.  The hash set and the histograms are cleared here; the first
   // exchange orders the clear before any insert.
-  const bool fused = a.mode == 4;
-  int cur_mode = fused ? 0 : a.mode;
+  const bool fused = a.mode == SOLVE_FUSED;
+  SolveMode cur_mode = fused ? SOLVE_FIRST : a.mode;
   if (fused) {
     for (unsigned idx = blockIdx.x * SOLVE_THREADS + threadIdx.x; idx <= a.table_mask; idx += gridDim.x * SOLVE_THREADS) a.table[idx] = L1_EMPTY;
     for (unsigned idx = blockIdx.x * SOLVE_THREADS + threadIdx.x; idx < K10_PASSES * 2048u + 64u; idx += gridDim.x * SOLVE_THREADS) ((unsigned*)Y->hist)[idx] = 0u;   // hist + list_cnt + pad
   }
   // ---- stage this CTA's residual blocks
   double thr = 0;
-  if (a.mode == 1) {   // K10 tail: threshold = max(inliner_dis, element floor(ratio * n_unique) of the sorted unique L1 norms)
+  if (a.mode == SOLVE_SECOND) {   // K10 tail: threshold = max(inliner_dis, element floor(ratio * n_unique) of the sorted unique L1 norms)
     int nu = *a.d_n_unique;
     if (nu > 0 && !isfinite(a.l1_sorted_unique[nu - 1])) nu--;   // the +inf of invalid slots is not a residual
     int k = (int)(st->inlier_ratio * (double)nu);
@@ -275,7 +276,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
     if (i < a.M && tid < tile) {
       const float4 ba = a.blk_a[i]; type = __float_as_int(ba.w);
       if (type != 0 && cap_keep <= 1.0f && ll_cap_uniform_f(cap_seed, cap_iter, 2, i) > cap_keep) type = 0;
-      if (type != 0 && a.mode == 1 && (a.l1[i] > thr)) type = 0;
+      if (type != 0 && a.mode == SOLVE_SECOND && (a.l1[i] > thr)) type = 0;
       if (type != 0) {
         const float4 f = a.feat[i];
         S.p[0][li] = f.x; S.p[1][li] = f.y; S.p[2][li] = f.z;
@@ -422,7 +423,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
     }
     const long long t_e3 = clock64();
     // ---- advance the solver: warp 1 evaluates the next iteration's ComputeStep under both outcomes while warp 0 digests the evaluation
-    if (cur_mode == 3) {
+    if (cur_mode == SOLVE_EVALUATE) {
       if (tid == 0) { LmState& L = s_lm; for (int i = 0; i < 21; i++) L.H[i] = s_sum[i]; for (int i = 0; i < 6; i++) L.g[i] = s_sum[21 + i]; L.x_cost = s_sum[27]; L.n_valid = (int)(s_sum[28] + 0.5); L.done = 1; }
     } else {
       StepIn in; double gx[7], gg[6];
@@ -453,11 +454,11 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
     setup_trial<MB>(E, L.x_best);   // the epilogue (L1 norms) evaluates at the solution
     if (master) {
       st->lm = L;   // whole solver state (parity hooks / host diagnostics read it)
-      if (cur_mode != 3) {
+      if (cur_mode != SOLVE_EVALUATE) {
         for (int k = 0; k < 7; k++) st->x[k] = L.x_best[k];
         st->total_lm_iterations += L.iteration; st->total_evaluations += L.total_evaluations;
       }
-      if (cur_mode == 1) {   // :514-531 pose composition + ICP termination test
+      if (cur_mode == SOLVE_SECOND) {   // :514-531 pose composition + ICP termination test
         double qi[4] = {L.x_best[3], L.x_best[0], L.x_best[1], L.x_best[2]}, ti[3] = {L.x_best[4], L.x_best[5], L.x_best[6]};
         const double* ql = st->pose_last; double tcur[3], qcur[4];
         d_qrot(ql, ti, tcur); for (int k = 0; k < 3; k++) tcur[k] += st->pose_last[4 + k];
@@ -487,7 +488,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   __syncthreads();
   // ---- epilogue of solve #1: loss-corrected L1 norm of every block at the solution (problem.Evaluate, :476-481)
   const long long t_p0 = clock64();
-  if (cur_mode == 0) {
+  if (cur_mode == SOLVE_FIRST) {
     for (int k = 0; k < tiles_per_cta; k++) {
       const int i = (blockIdx.x + gridDim.x * k) * tile + tid, li = k * SOLVE_THREADS + tid;
       double my_l1 = INFINITY;
@@ -605,7 +606,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
       const int i = (blockIdx.x + gridDim.x * k) * tile + tid, li = k * SOLVE_THREADS + tid;
       if (i < a.M && tid < tile) { const int t = S.type[li] & 0xff; S.type[li] = (t != 0 && a.l1[i] > thr2) ? 0 : t; }
     }
-    cur_mode = 1;
+    cur_mode = SOLVE_SECOND;
     __syncthreads();
     if (master && tid == 0) { const long long q4 = clock64(); st->prof[8] += q0 - t_p0; st->prof[10] += q3 - q0; st->prof[12] += q4 - q3; }
   }
@@ -616,7 +617,6 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
 }
 
 #define SOLVE_MAX_SMEM (200 * 1024)   // up to ~405k slots on 132 SMs; a typical scan (<= 113 KB of slots per CTA) leaves room for a second CTA per SM (another context's solver)
-int solve_max_slots(ll_ctx* ctx) { return ctx->num_sms * ((SOLVE_MAX_SMEM / SLOT_BYTES) / SOLVE_THREADS) * SOLVE_THREADS; }
 
 int solve_prepare(ll_ctx* ctx) {
   LL_CUDA(ctx, cudaFuncSetAttribute((void*)lm_solve_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SOLVE_MAX_SMEM));
