@@ -189,6 +189,11 @@ int ll_build_blocks(ll_ctx* ctx, const ll_map* map, const void* scan_corner, siz
 int ll_normal_equations(ll_ctx* ctx, const double x[7], double out28[28]);
 /* ... and one ceres::Solve-equivalent on the blocks currently resident (max_iterations as in Solver::Options). */
 int ll_solve(ll_ctx* ctx, int max_iterations, double x_io[7], double* initial_cost, double* final_cost, int* iterations);
+/* ... and compute_inlier_residual_threshold (point_cloud_registration.hpp:153-161) over n caller-given L1 norms (non-negative; n <= max_features).
+ * path 0: the grid-wide select of the fused solver kernel; path 1: the sharded mode's l1_unique / l1_select kernels.
+ * +inf and NaN entries are not residuals.  *n_distinct = number of distinct values; *value = element min(floor(ratio n), n-1) of them
+ * (0 when there is none). */
+int ll_inlier_select(ll_ctx* ctx, const double* l1, size_t n, double ratio, int path, double* value, int* n_distinct);
 
 /* ---- N4: loop-closure reuse of S3 ----------------------------------------------------------------------- */
 /* Replaces Scene_alignment::find_tranfrom_of_two_mappings (scene_alignment.hpp:269-353) from the point where the four feature clouds exist:

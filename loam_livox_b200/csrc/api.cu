@@ -399,7 +399,7 @@ int register_device(ll_ctx* ctx, const ll_map* map, const RegArrays& A, int nc, 
   if (map->world > 1 && ctx->world != map->world) { ctx->set_error("a sharded map needs a context connected to the same number of ranks (ll_comm_connect)"); return LL_ERR_INVALID; }
   if (sharded && M > ctx->cfg.max_features) { ctx->set_error("more features than max_features (exchange buffer)"); return LL_ERR_CAPACITY; }
   double* x_l1 = sharded ? (double*)((char*)ctx->comm_local + LL_COMM_X_OFF) : nullptr;
-  unsigned set_cap = 1024; while (set_cap < (unsigned)(2 * M)) set_cap <<= 1;   // hash set of the L1 norms (K10)
+  const unsigned set_cap = l1_set_capacity(M);   // hash set of the L1 norms (K10)
   LL_CUDA(ctx, ctx->scratch.reserve((size_t)set_cap * 8 + 256));
   // One ICP iteration's device work + a snapshot of the 1.7 KB state into pinned slot `it & 1`.
   RegDevState* slots[2] = {hs, (RegDevState*)((char*)hs + align256(sizeof(RegDevState)))};
@@ -571,6 +571,34 @@ int ll_solve(ll_ctx* ctx, int max_iterations, double x_io[7], double* initial_co
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   for (int k = 0; k < 7; k++) x_io[k] = hs->x[k];
   if (initial_cost) *initial_cost = hs->lm.initial_cost; if (final_cost) *final_cost = hs->lm.final_cost; if (iterations) *iterations = hs->lm.iteration;
+  return LL_OK;
+}
+int ll_inlier_select(ll_ctx* ctx, const double* l1, size_t n, double ratio, int path, double* value, int* n_distinct) {
+  if (!ctx || (n > 0 && !l1) || !value || !n_distinct || (path != 0 && path != 1) || !(ratio >= 0.0)) return LL_ERR_INVALID;
+  for (size_t i = 0; i < n; i++) if (l1[i] < 0.0) { ctx->set_error("L1 norms are never negative"); return LL_ERR_INVALID; }
+  if (n > (size_t)ctx->cfg.max_features) { ctx->set_error("more values than max_features"); return LL_ERR_CAPACITY; }
+  cudaSetDevice(ctx->device);
+  const int M = (int)n;
+  RegArrays A; LL_TRY(reg_arrays(ctx, M, &A));
+  cudaStream_t s = ctx->stream;
+  if (M > 0) LL_CUDA(ctx, cudaMemcpyAsync(A.l1, l1, n * sizeof(double), cudaMemcpyHostToDevice, s));
+  LL_CUDA(ctx, cudaMemsetAsync(A.l1_sorted, 0, 64, s));   // [0]: distinct count (path 1)
+  LL_CUDA(ctx, cudaMemsetAsync(A.l1_unique, 0, sizeof(double), s));
+  LL_CUDA(ctx, cudaMemsetAsync(A.n_unique, 0, sizeof(int), s));
+  if (path == 0) {
+    double* d_ratio = &ctx->d_reg->inlier_ratio;   // read on the device as the fused solver reads it (ll_register rewrites the whole state)
+    LL_CUDA(ctx, cudaMemcpyAsync(d_ratio, &ratio, sizeof(double), cudaMemcpyHostToDevice, s));
+    const unsigned set_cap = l1_set_capacity(M);
+    LL_CUDA(ctx, ctx->scratch.reserve((size_t)set_cap * 8 + 256));
+    LL_TRY(launch_k10_select(ctx, A.l1, M, d_ratio, (unsigned long long*)ctx->scratch.p, set_cap - 1, A.l1_unique, A.n_unique));
+  } else if (M > 0) {   // the sharded mode's kernels: distinct values compacted behind a count in l1_sorted, the order statistic into l1_unique[0]
+    LL_TRY(launch_inlier_select(ctx, A.l1, M, ratio, A.l1_sorted, A.l1_unique, A.n_unique));
+  }
+  double v = 0.0; int nd = 0;
+  LL_CUDA(ctx, cudaMemcpyAsync(&v, A.l1_unique, sizeof(double), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(&nd, path == 0 ? A.n_unique : (int*)A.l1_sorted, sizeof(int), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  *value = nd > 0 ? v : 0.0; *n_distinct = nd;
   return LL_OK;
 }
 

@@ -251,7 +251,7 @@ __global__ void __launch_bounds__(1024) l1_select_kernel(const double* __restric
 
 int launch_inlier_select(ll_ctx* ctx, const double* d_l1, int M, double ratio, double* d_sorted, double* d_unique, int* d_n_unique) {
   cudaStream_t s = ctx->stream;
-  unsigned cap = 1024; while (cap < (unsigned)(2 * M)) cap <<= 1;
+  const unsigned cap = l1_set_capacity(M);
   LL_CUDA(ctx, ctx->scratch.reserve((size_t)cap * 8 + 256));
   unsigned long long* table = (unsigned long long*)ctx->scratch.p;
   int* n_tmp = (int*)d_sorted;   // d_sorted doubles as [count | compacted distinct values]

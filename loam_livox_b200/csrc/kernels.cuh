@@ -109,6 +109,10 @@ struct SolveArgs {
 #define LL_COMM_X_OFF 16384
 int launch_solve(ll_ctx* ctx, const SolveArgs& a);
 int solve_prepare(ll_ctx* ctx);   // once per context: opt the solver kernels in to their dynamic shared memory
+// Parity hook: the fused solver's K10 (grid-wide de-duplication + radix select) over n values; *d_value, *d_n_distinct on the device.
+int launch_k10_select(ll_ctx* ctx, const double* d_l1, int n, const double* d_ratio, unsigned long long* table, unsigned table_mask, double* d_value, int* d_n_distinct);
+// Slots of the hash set of M L1 norms (K10): a power of two >= 2 M.
+inline unsigned l1_set_capacity(int M) { unsigned cap = 1024; while (cap < (unsigned)(2 * M)) cap <<= 1; return cap; }
 // Sharded mode, K10: every rank pushes the loss-corrected L1 norms of the slots it owns into every peer's X buffer (NVLink stores), then a
 // flag barrier; afterwards X is identical on all ranks (NaN where nobody produced a block).
 int launch_l1_exchange(ll_ctx* ctx, const double* d_l1, int M);

@@ -25,7 +25,7 @@ __device__ __forceinline__ void l1_set_insert(unsigned long long* __restrict__ t
   __syncthreads();
   if (threadIdx.x == 0) { int tot = 0; for (int w = 0; w < nwarp; w++) { const int c = s_scratch[w]; s_scratch[w] = tot; tot += c; } s_scratch[32] = tot ? atomicAdd(n_unique, tot) : 0; }
   __syncthreads();
-  if (is_new) uniq[s_scratch[32] + s_scratch[warp] + __popc(m & ((1u << lane) - 1u))] = v;
+  if (is_new) uniq[s_scratch[32] + s_scratch[warp] + __popc(m & ((1u << lane) - 1u))] = v == 0.0 ? 0.0 : v;   // +0.0 for a -0.0: block_select ranks bit patterns
   __syncthreads();
 }
 

@@ -220,9 +220,97 @@ __device__ __forceinline__ void grid_sync(SolveSync* Y, unsigned& gen) {
   sync_wait_all(Y, gen);
 }
 
-// K10 (compute_inlier_residual_threshold, :153-161) spread over the grid: see the fused section of the kernel.
+// K10 (compute_inlier_residual_threshold, :153-161) spread over the grid.  Used by the fused section of lm_solve_kernel and by k10_select_kernel
+// (the parity hook ll_inlier_select), so that both run the same code.
 #define K10_PASSES 6
 struct K10Smem { unsigned hist[2048]; unsigned warp_sum[SOLVE_THREADS / 32 + 1]; unsigned long long prefix, mask; int k, cnt_bin, n_distinct, done; int scratch[40]; double result; };
+
+// Clear the hash set of the L1 norms and the K10 histograms / candidate counter; a grid exchange must follow before any insert.
+__device__ __forceinline__ void k10_clear(unsigned long long* table, unsigned table_mask, SolveSync* Y) {
+  for (unsigned idx = blockIdx.x * SOLVE_THREADS + threadIdx.x; idx <= table_mask; idx += gridDim.x * SOLVE_THREADS) table[idx] = L1_EMPTY;
+  for (unsigned idx = blockIdx.x * SOLVE_THREADS + threadIdx.x; idx < K10_PASSES * 2048u + 64u; idx += gridDim.x * SOLVE_THREADS) ((unsigned*)Y->hist)[idx] = 0u;   // hist + list_cnt + pad
+}
+
+// The element of rank min(floor(ratio * n), n - 1) among the n DISTINCT values l1[i] of the slots whose flag (bit 8 of type[li], shared memory)
+// says this thread represents the value.  Radix select on the bit patterns (non-negative doubles order like their bits), 11-bit digits from the
+// exponent down: per pass every CTA histograms the distinct values it represents (shared memory), adds its non-empty bins to the global
+// histogram, one exchange, and every CTA finds the bin of the wanted rank in the same histogram.  When that bin holds <= 64 values they are
+// collected and ranked directly.  Grid-collective; ends with s_k10.n_distinct and s_k10.result (valid when n_distinct > 0) on every CTA.
+__device__ __forceinline__ void k10_select(K10Smem& s_k10, SolveSync* Y, unsigned& gen, const int* type, const double* l1, int M, int tiles_per_cta, int tile, const double* ratio) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid == 0) { s_k10.prefix = 0ull; s_k10.mask = 0ull; s_k10.k = -1; s_k10.done = 0; s_k10.result = 0.0; }
+  __syncthreads();
+  for (int pass = 0; pass < K10_PASSES && !s_k10.done; pass++) {
+    const int shift = pass < 5 ? 52 - 11 * pass : 0; const unsigned dmask = pass < 5 ? 2047u : 255u;   // bits 62..52, 51..41, 40..30, 29..19, 18..8, 7..0
+    for (int b = tid; b < 2048; b += SOLVE_THREADS) s_k10.hist[b] = 0u;
+    __syncthreads();
+    const unsigned long long prefix = s_k10.prefix, himask = s_k10.mask;
+    for (int k = 0; k < tiles_per_cta; k++) {
+      const int i = (blockIdx.x + gridDim.x * k) * tile + tid, li = k * SOLVE_THREADS + tid;
+      if (i < M && tid < tile && (type[li] & 0x100)) {
+        const unsigned long long key = l1_key(l1[i]);
+        if ((key & himask) == prefix) atomicAdd(&s_k10.hist[(unsigned)(key >> shift) & dmask], 1u);
+      }
+    }
+    __syncthreads();
+    unsigned* gh = Y->hist[pass];
+    for (int b = tid; b < 2048; b += SOLVE_THREADS) { const unsigned c = s_k10.hist[b]; if (c) atomicAdd(&gh[b], c); }
+    grid_sync(Y, gen);
+    // every CTA: exclusive scan of the global histogram, find the bin that holds rank k
+    constexpr int BPT = 2048 / SOLVE_THREADS;
+    unsigned h[BPT], run = 0;
+#pragma unroll
+    for (int b = 0; b < BPT; b++) { h[b] = __ldcg(&gh[tid * BPT + b]); run += h[b]; }
+    unsigned incl = run;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const unsigned v = __shfl_up_sync(FULL, incl, o); if (lane >= o) incl += v; }
+    if (lane == 31) s_k10.warp_sum[warp] = incl;
+    __syncthreads();
+    if (tid == 0) { unsigned t = 0; for (int w = 0; w < SOLVE_THREADS / 32; w++) { const unsigned c = s_k10.warp_sum[w]; s_k10.warp_sum[w] = t; t += c; } s_k10.warp_sum[SOLVE_THREADS / 32] = t; }
+    __syncthreads();
+    if (pass == 0 && tid == 0) {
+      const int n = (int)s_k10.warp_sum[SOLVE_THREADS / 32]; s_k10.n_distinct = n;
+      int k = (int)(*ratio * (double)n); if (k > n - 1) k = n - 1; s_k10.k = k;
+      if (n == 0) s_k10.done = 1;   // no block at all: the solve reported termination -1 already
+    }
+    __syncthreads();
+    if (!s_k10.done) {
+      const unsigned excl = s_k10.warp_sum[warp] + incl - run; const unsigned k = (unsigned)s_k10.k;
+      __syncthreads();
+      if (k >= excl && k < excl + run) {   // exactly one thread
+        unsigned below = excl; int j = 0;
+#pragma unroll
+        for (int b = 0; b < BPT; b++) { if (k >= below + h[b] && j == b) { below += h[b]; j = b + 1; } }
+        const int jj = j < BPT ? j : BPT - 1;
+        s_k10.k = (int)(k - below); s_k10.cnt_bin = (int)h[jj];
+        s_k10.prefix = prefix | ((unsigned long long)(tid * BPT + jj) << shift);
+        s_k10.mask = himask | ((unsigned long long)dmask << shift);
+      }
+      __syncthreads();
+      if (s_k10.cnt_bin <= 64 || pass == K10_PASSES - 1) {
+        // collect the members of the bin (<= 64 distinct values, or all equal in their 63 bits: then any of them is the answer) and rank them
+        const unsigned long long pf = s_k10.prefix, hm = s_k10.mask;
+        for (int kk = 0; kk < tiles_per_cta; kk++) {
+          const int i = (blockIdx.x + gridDim.x * kk) * tile + tid, li = kk * SOLVE_THREADS + tid;
+          if (i < M && tid < tile && (type[li] & 0x100)) {
+            const double v = l1[i];
+            if ((l1_key(v) & hm) == pf) { const unsigned slot = atomicAdd(&Y->list_cnt, 1u); if (slot < 64u) Y->list[slot] = v; }
+          }
+        }
+        grid_sync(Y, gen);
+        {   // rank the <= 64 collected values: one value per thread out of shared memory (distinct values: exactly one has the wanted rank)
+          double* cand = (double*)s_k10.hist;
+          const int m = min((int)*((volatile unsigned*)&Y->list_cnt), 64);
+          if (tid < m) cand[tid] = __ldcg(&Y->list[tid]);
+          __syncthreads();
+          if (tid < m) { const double mine = cand[tid]; int rank = 0; for (int q = 0; q < m; q++) rank += (cand[q] < mine) ? 1 : 0; if (rank == s_k10.k) s_k10.result = mine; }
+          if (tid == 0) s_k10.done = 1;
+        }
+        __syncthreads();
+      }
+    }
+  }
+}
 
 template <bool MB>
 __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a, int tiles_per_cta, int tile) {
@@ -249,10 +337,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   // exchange orders the clear before any insert.
   const bool fused = a.mode == SOLVE_FUSED;
   SolveMode cur_mode = fused ? SOLVE_FIRST : a.mode;
-  if (fused) {
-    for (unsigned idx = blockIdx.x * SOLVE_THREADS + threadIdx.x; idx <= a.table_mask; idx += gridDim.x * SOLVE_THREADS) a.table[idx] = L1_EMPTY;
-    for (unsigned idx = blockIdx.x * SOLVE_THREADS + threadIdx.x; idx < K10_PASSES * 2048u + 64u; idx += gridDim.x * SOLVE_THREADS) ((unsigned*)Y->hist)[idx] = 0u;   // hist + list_cnt + pad
-  }
+  if (fused) k10_clear(a.table, a.table_mask, Y);
   // ---- stage this CTA's residual blocks
   double thr = 0;
   if (a.mode == SOLVE_SECOND) {   // K10 tail: threshold = max(inliner_dis, element floor(ratio * n_unique) of the sorted unique L1 norms)
@@ -522,83 +607,9 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
     }
   }
   if (fused && ph == 0) {
-    // ---- K10 over the whole grid (:153-161): the element of rank floor(ratio * n) among the DISTINCT L1 norms.  Radix select on the bit patterns
-    // (non-negative doubles order like their bits), 11-bit digits from the exponent down: per pass every CTA histograms the distinct values it
-    // represents (shared memory), adds its non-empty bins to the global histogram, one exchange, and every CTA finds the bin of the wanted rank in
-    // the same histogram.  When that bin holds <= 64 values they are collected and ranked directly.
+    // ---- K10 over the whole grid (:153-161): the element of rank floor(ratio * n) among the DISTINCT L1 norms (k10_select)
     const long long q0 = clock64();
-    if (tid == 0) { s_k10.prefix = 0ull; s_k10.mask = 0ull; s_k10.k = -1; s_k10.done = 0; s_k10.result = 0.0; }
-    __syncthreads();
-    for (int pass = 0; pass < K10_PASSES && !s_k10.done; pass++) {
-      const int shift = pass < 5 ? 52 - 11 * pass : 0; const unsigned dmask = pass < 5 ? 2047u : 255u;   // bits 62..52, 51..41, 40..30, 29..19, 18..8, 7..0
-      for (int b = tid; b < 2048; b += SOLVE_THREADS) s_k10.hist[b] = 0u;
-      __syncthreads();
-      const unsigned long long prefix = s_k10.prefix, himask = s_k10.mask;
-      for (int k = 0; k < tiles_per_cta; k++) {
-        const int i = (blockIdx.x + gridDim.x * k) * tile + tid, li = k * SOLVE_THREADS + tid;
-        if (i < a.M && tid < tile && (S.type[li] & 0x100)) {
-          const unsigned long long key = l1_key(a.l1[i]);
-          if ((key & himask) == prefix) atomicAdd(&s_k10.hist[(unsigned)(key >> shift) & dmask], 1u);
-        }
-      }
-      __syncthreads();
-      unsigned* gh = Y->hist[pass];
-      for (int b = tid; b < 2048; b += SOLVE_THREADS) { const unsigned c = s_k10.hist[b]; if (c) atomicAdd(&gh[b], c); }
-      grid_sync(Y, gen);
-      // every CTA: exclusive scan of the global histogram, find the bin that holds rank k
-      constexpr int BPT = 2048 / SOLVE_THREADS;
-      unsigned h[BPT], run = 0;
-#pragma unroll
-      for (int b = 0; b < BPT; b++) { h[b] = __ldcg(&gh[tid * BPT + b]); run += h[b]; }
-      unsigned incl = run;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const unsigned v = __shfl_up_sync(FULL, incl, o); if (lane >= o) incl += v; }
-      if (lane == 31) s_k10.warp_sum[warp] = incl;
-      __syncthreads();
-      if (tid == 0) { unsigned t = 0; for (int w = 0; w < SOLVE_THREADS / 32; w++) { const unsigned c = s_k10.warp_sum[w]; s_k10.warp_sum[w] = t; t += c; } s_k10.warp_sum[SOLVE_THREADS / 32] = t; }
-      __syncthreads();
-      if (pass == 0 && tid == 0) {
-        const int n = (int)s_k10.warp_sum[SOLVE_THREADS / 32]; s_k10.n_distinct = n;
-        int k = (int)(st->inlier_ratio * (double)n); if (k > n - 1) k = n - 1; s_k10.k = k;
-        if (n == 0) s_k10.done = 1;   // no block at all: the solve reported termination -1 already
-      }
-      __syncthreads();
-      if (!s_k10.done) {
-        const unsigned excl = s_k10.warp_sum[warp] + incl - run; const unsigned k = (unsigned)s_k10.k;
-        __syncthreads();
-        if (k >= excl && k < excl + run) {   // exactly one thread
-          unsigned below = excl; int j = 0;
-#pragma unroll
-          for (int b = 0; b < BPT; b++) { if (k >= below + h[b] && j == b) { below += h[b]; j = b + 1; } }
-          const int jj = j < BPT ? j : BPT - 1;
-          s_k10.k = (int)(k - below); s_k10.cnt_bin = (int)h[jj];
-          s_k10.prefix = prefix | ((unsigned long long)(tid * BPT + jj) << shift);
-          s_k10.mask = himask | ((unsigned long long)dmask << shift);
-        }
-        __syncthreads();
-        if (s_k10.cnt_bin <= 64 || pass == K10_PASSES - 1) {
-          // collect the members of the bin (<= 64 distinct values, or all equal in their 63 bits: then any of them is the answer) and rank them
-          const unsigned long long pf = s_k10.prefix, hm = s_k10.mask;
-          for (int kk = 0; kk < tiles_per_cta; kk++) {
-            const int i = (blockIdx.x + gridDim.x * kk) * tile + tid, li = kk * SOLVE_THREADS + tid;
-            if (i < a.M && tid < tile && (S.type[li] & 0x100)) {
-              const double v = a.l1[i];
-              if ((l1_key(v) & hm) == pf) { const unsigned slot = atomicAdd(&Y->list_cnt, 1u); if (slot < 64u) Y->list[slot] = v; }
-            }
-          }
-          grid_sync(Y, gen);
-          {   // rank the <= 64 collected values: one value per thread out of shared memory (distinct values: exactly one has the wanted rank)
-            double* cand = (double*)s_k10.hist;
-            const int m = min((int)*((volatile unsigned*)&Y->list_cnt), 64);
-            if (tid < m) cand[tid] = __ldcg(&Y->list[tid]);
-            __syncthreads();
-            if (tid < m) { const double mine = cand[tid]; int rank = 0; for (int q = 0; q < m; q++) rank += (cand[q] < mine) ? 1 : 0; if (rank == s_k10.k) s_k10.result = mine; }
-            if (tid == 0) s_k10.done = 1;
-          }
-          __syncthreads();
-        }
-      }
-    }
+    k10_select(s_k10, Y, gen, S.type, a.l1, a.M, tiles_per_cta, tile, &st->inlier_ratio);
     const double thr2 = fmax(st->inliner_dis, s_k10.n_distinct > 0 ? s_k10.result : 0.0);   // :484-485
     if (master && tid == 0) { st->inlier_threshold = thr2; st->n_unique = s_k10.n_distinct; }
     const long long q3 = clock64();
@@ -626,20 +637,61 @@ int solve_prepare(ll_ctx* ctx) {
   }
   return LL_OK;
 }
-int launch_solve(ll_ctx* ctx, const SolveArgs& a) {
+// How M slots are spread over the persistent CTAs: CTA b owns the tiles b, b + grid, b + 2 grid, ... of `tile` slots each.
+struct SolveGrid { int tile, tiles_per_cta, grid; };
+static SolveGrid solve_grid(const ll_ctx* ctx, int M) {
   // The evaluation is fp64-throughput bound (64 DFMA/clk/SM): spread the slots over ALL SMs, even when that leaves CTAs partly empty.
   // tile = slots per CTA and pass (a multiple of 32, <= SOLVE_THREADS); partly empty CTAs on every SM evaluate faster than fewer full ones.
-  const int M1 = a.M > 0 ? a.M : 1;
-  int tile = ((ll_div_up(M1, ctx->num_sms) + 31) / 32) * 32; if (tile > SOLVE_THREADS) tile = SOLVE_THREADS;
-  const int tiles = ll_div_up(M1, tile);
-  int grid = tiles < ctx->num_sms ? tiles : ctx->num_sms; if (grid > LL_SYNC_ROWS) grid = LL_SYNC_ROWS;
-  int tiles_per_cta = ll_div_up(tiles, grid);
+  const int M1 = M > 0 ? M : 1;
+  SolveGrid g;
+  g.tile = ((ll_div_up(M1, ctx->num_sms) + 31) / 32) * 32; if (g.tile > SOLVE_THREADS) g.tile = SOLVE_THREADS;
+  const int tiles = ll_div_up(M1, g.tile);
+  g.grid = tiles < ctx->num_sms ? tiles : ctx->num_sms; if (g.grid > LL_SYNC_ROWS) g.grid = LL_SYNC_ROWS;
+  g.tiles_per_cta = ll_div_up(tiles, g.grid);
+  return g;
+}
+int launch_solve(ll_ctx* ctx, const SolveArgs& a) {
+  const SolveGrid sg = solve_grid(ctx, a.M);
+  int tile = sg.tile, tiles_per_cta = sg.tiles_per_cta; const int grid = sg.grid;
   const int mb = a.deblur ? 1 : 0;
   const size_t smem = (size_t)tiles_per_cta * SOLVE_THREADS * (mb ? SLOT_BYTES_MB : SLOT_BYTES);
   if (smem > SOLVE_MAX_SMEM) { ctx->set_error("too many residual-block slots for the shared-memory-resident solver"); return LL_ERR_CAPACITY; }
   void* fn = mb ? (void*)lm_solve_kernel<true> : (void*)lm_solve_kernel<false>;
   SolveArgs args = a; args.sync = ctx->d_sync; void* kargs[] = {&args, &tiles_per_cta, &tile};
   LL_CUDA(ctx, cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(SOLVE_THREADS), kargs, smem, ctx->stream));   // co-residency of the whole grid is what the exchanges rely on
+  ctx->launches++;
+  return LL_OK;
+}
+
+// Parity hook (ll_inlier_select, path 0): the fused kernel's K10 over n caller-given values, spread over the CTAs as lm_solve_kernel spreads M = n
+// slots.  Same generation protocol as the solver: `gen` is read at entry and handed to the next launch at the end.
+__global__ void __launch_bounds__(SOLVE_THREADS) k10_select_kernel(SolveSync* Y, const double* l1, int n, const double* ratio, unsigned long long* table, unsigned table_mask,
+                                                                   int tiles_per_cta, int tile, double* value, int* n_distinct) {
+  extern __shared__ int s_flag[];   // [tiles_per_cta * SOLVE_THREADS]: bit 8 = this thread represents its slot's value (lm_solve_kernel: S.type)
+  __shared__ K10Smem s_k10;
+  const int tid = threadIdx.x;
+  unsigned gen = *((volatile unsigned*)&Y->gen);
+  k10_clear(table, table_mask, Y);
+  grid_sync(Y, gen);   // the clear before any insert
+  for (int k = 0; k < tiles_per_cta; k++) {   // as the epilogue of solve #1: +inf / NaN (and slots past n) are not residuals
+    const int i = (blockIdx.x + gridDim.x * k) * tile + tid, li = k * SOLVE_THREADS + tid;
+    const double v = (i < n && tid < tile) ? l1[i] : INFINITY;
+    s_flag[li] = l1_set_insert_flag(table, table_mask, v, v < INFINITY) ? 0x100 : 0;
+  }
+  k10_select(s_k10, Y, gen, s_flag, l1, n, tiles_per_cta, tile, ratio);
+  if (blockIdx.x == 0 && tid == 0) {
+    *value = s_k10.n_distinct > 0 ? s_k10.result : 0.0; *n_distinct = s_k10.n_distinct;
+    *((volatile unsigned*)&Y->gen) = gen;
+  }
+}
+int launch_k10_select(ll_ctx* ctx, const double* d_l1, int n, const double* d_ratio, unsigned long long* table, unsigned table_mask, double* d_value, int* d_n_distinct) {
+  const SolveGrid sg = solve_grid(ctx, n);
+  int tile = sg.tile, tiles_per_cta = sg.tiles_per_cta;
+  SolveSync* Y = ctx->d_sync;
+  const size_t smem = (size_t)tiles_per_cta * SOLVE_THREADS * sizeof(int);   // 4 B per slot: 48 KB up to ~1.6M values on 132 SMs
+  if (smem > 48 * 1024) LL_CUDA(ctx, cudaFuncSetAttribute((void*)k10_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  void* kargs[] = {&Y, &d_l1, &n, &d_ratio, &table, &table_mask, &tiles_per_cta, &tile, &d_value, &d_n_distinct};
+  LL_CUDA(ctx, cudaLaunchCooperativeKernel((void*)k10_select_kernel, dim3(sg.grid), dim3(SOLVE_THREADS), kargs, smem, ctx->stream));
   ctx->launches++;
   return LL_OK;
 }

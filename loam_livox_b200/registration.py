@@ -255,6 +255,15 @@ class Point_cloud_registration:
         return x, ic.value, fc.value, it.value
 
 
+def inlier_select(ctx: Context, l1, ratio: float, path: int):
+    """compute_inlier_residual_threshold (point_cloud_registration.hpp:153-161) over caller-given L1 norms (ll_inlier_select): path 0 = the fused
+    solver kernel's grid-wide select, path 1 = the sharded mode's kernels.  Returns (value, number of distinct values); +inf / NaN are skipped."""
+    v = np.ascontiguousarray(l1, np.float64)
+    out, nd = C.c_double(), C.c_int()
+    ctx.check(ctx._lib.ll_inlier_select(ctx.h, v.ctypes.data, v.shape[0], float(ratio), int(path), C.byref(out), C.byref(nd)))
+    return out.value, nd.value
+
+
 def scan_to_pose(ctx: Context, match_map: Map, raw, stamp, pipeline: capi.PipelineCfg, state: capi.RegState, where=capi.LL_HOST, n=None, fmt=None):
     """Whole per-scan step: raw scan -> features -> VoxelGrid x2 -> registration (ll_scan_to_pose)."""
     if where == capi.LL_HOST:

@@ -147,11 +147,97 @@ def test_solver_respects_bounds_and_iteration_cap(oracle):
     assert abs(np.linalg.norm(x[:4]) - 1.0) < 1e-12
 
 
+K10_SIZES = (1, 2, 63, 64, 65, 1024, 1025, 2049, 30000, 400000)
+K10_RATIOS = (0.0, 0.5, 0.8, 0.999999)
+
+
+def _chain(start, count, stride_ulp=1):
+    """count non-negative doubles start, start + stride ulp, start + 2 stride ulp, ... (their bit patterns are consecutive integers)."""
+    return (np.float64(start).view(np.int64) + np.int64(stride_ulp) * np.arange(count, dtype=np.int64)).view(np.float64)
+
+
+def _ratio_for_rank(k, n):
+    """A ratio r with int(r * n) == k (the rank compute_inlier_residual_threshold takes among n distinct values)."""
+    r = (k + 0.5) / n
+    assert int(r * n) == k
+    return r
+
+
+def k10_vectors(n, seed=0):
+    """(name, L1 norms, ratios) for compute_inlier_residual_threshold at the edges of its radix select (11-bit digits of the bit pattern from the
+    exponent down: bits 62..52, 51..41, 40..30, 29..19, 18..8, then 7..0; a bin of <= 64 distinct values is ranked directly).  `focus` values
+    are the ones a ratio is aimed at: the first and the last member of the run / cluster that forces the deep passes."""
+    rng = np.random.default_rng(seed + 7 * n)
+    out = []
+
+    def add(name, v, focus=()):
+        v = np.asarray(v, np.float64)[:n]
+        u = np.unique(v[np.isfinite(v)])
+        ratios = list(K10_RATIOS)
+        for f in focus:
+            k = np.searchsorted(u, f)
+            if len(u) and k < len(u) and u[k] == f:
+                ratios.append(_ratio_for_rank(int(k), len(u)))
+        out.append((name, v, ratios))
+
+    def pad(core, lo=1e-3, hi=(8.0, 1e3)):
+        """core values plus filler below (< lo) and above (in hi) them, shuffled: the core's ranks sit inside the vector."""
+        m = max(n - len(core), 0)
+        fill = np.concatenate([rng.uniform(lo * 0.1, lo, m // 2), rng.uniform(*hi, m - m // 2)])
+        v = np.concatenate([core[:n], fill])
+        return v[rng.permutation(len(v))]
+
+    out_cont = np.exp(rng.uniform(np.log(1e-4), np.log(3.0), n))            # a scan's L1 norms: ~30k distinct values over a few binades
+    add("continuous", out_cont)
+    add("all_equal", np.full(n, 0.0371))
+    add("ten_values", rng.choice(rng.uniform(0.0, 2.0, 10), n))
+    z = rng.uniform(0.0, 1.0, n)
+    z[rng.random(n) < 0.5] = 0.0
+    z[(z == 0.0) & (rng.random(n) < 0.5)] = -0.0                             # zeros as -0.0 and +0.0 (one std::set entry), positives
+    add("zeros_signed", z)
+    add("zeros_negative_only", np.where(rng.random(n) < 0.3, -0.0, rng.uniform(0.0, 1.0, n)))
+    # runs of doubles that share all digits above one pass: 65+ members force that pass; stride 1 (a 256-aligned run) reaches the last pass
+    for stride, name in ((1 << 41, "pass1"), (1 << 30, "pass2"), (1 << 19, "pass3"), (1 << 8, "pass4"), (1, "pass5")):
+        for cnt in (64, 65, 200):
+            run = _chain(1.0, cnt, stride)                                   # 1.0: mantissa 0, aligned to every digit boundary
+            add(f"run_{name}_{cnt}", pad(run), (run[0], run[min(cnt, n) - 1]))
+    # a run in one bin of the last pass with duplicates, and runs that straddle a digit boundary at each pass (around a power of two, ...)
+    dup = np.repeat(_chain(1.5, 100, 1), 3)
+    add("run_pass5_dup", pad(dup), (dup[0], dup[-1]))
+    for bit in (52, 41, 30, 19, 8):
+        edge = np.float64(1.0).view(np.int64) + (np.int64(1) << bit)         # first double whose digit above `bit` is one more than 1.0's
+        run = _chain(np.int64(edge - 100).view(np.float64), 200, 1)
+        below = run[99]
+        add(f"straddle_bit{bit}", pad(run), (run[0], below, run[100], run[-1]))
+    wide = np.concatenate([_chain(5e-324, 40, 1), np.logspace(-300, 300, 200), [np.finfo(np.float64).tiny, 2.2e-308, 1e300]])
+    add("subnormal_to_1e300", rng.choice(wide, n) if n > len(wide) else wide[rng.permutation(len(wide))][:n], (5e-324, 1e300))
+    s = out_cont.copy()
+    s[rng.random(n) < 0.1] = np.inf                                          # invalid slots
+    s[rng.random(n) < 0.05] = np.nan                                         # slots nobody owns (sharded mode)
+    add("inf_nan_sprinkled", s)
+    return out
+
+
+def _k10_reference(v, ratio):
+    u = np.unique(v[np.isfinite(v)])
+    return (u[min(int(ratio * len(u)), len(u) - 1)] if len(u) else 0.0), len(u)
+
+
 def test_inlier_threshold_is_order_statistic_of_unique_values(oracle):
     r = np.zeros(30)
     r[0::3] = [5, 1, 1, 3, 2, 2, 4, 1, 9, 7]      # L1 norms, with duplicates
     uniq = np.unique(np.abs(r.reshape(-1, 3)).sum(1))
     assert oracle.inlier_threshold(r, 0.8) == uniq[int(0.8 * len(uniq))]
+    # the edge vectors of the library's K10 tests: the oracle (std::set) and NumPy agree on every one (finite values, ratio < 1: no clamp)
+    for n in K10_SIZES:
+        for name, v, ratios in k10_vectors(n):
+            if not np.isfinite(v).all() or (n > 30000 and name not in ("continuous", "ten_values", "zeros_signed", "run_pass5_65")):
+                continue                                                     # (std::set of 400k values: ~0.3 s per call)
+            r = np.zeros(3 * n)
+            r[0::3] = v                                                      # L1 norm of (v, 0, 0) = |v|
+            for ratio in (ratios if n <= 30000 else ratios[2:3] + ratios[4:]):
+                want, _ = _k10_reference(v, ratio)
+                assert oracle.inlier_threshold(r, ratio) == want, (name, n, ratio)
 
 
 def test_registration_recovers_injected_motion(oracle):
