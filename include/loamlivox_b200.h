@@ -194,6 +194,18 @@ int ll_solve(ll_ctx* ctx, int max_iterations, double x_io[7], double* initial_co
  * +inf and NaN entries are not residuals.  *n_distinct = number of distinct values; *value = element min(floor(ratio n), n-1) of them
  * (0 when there is none). */
 int ll_inlier_select(ll_ctx* ctx, const double* l1, size_t n, double ratio, int path, double* value, int* n_distinct);
+/* ... and caller-given residual blocks in place of ll_build_blocks': n slots (n <= max_features and within the solver's shared memory, else
+ * LL_ERR_CAPACITY before anything is enqueued), type 0 invalid / 1 line / 2 plane, the feature p (scan frame; intensity = time stamp, the blur
+ * factor of the *_mb functors comes from it as in a registration), the anchor a3 (fp32, as the kNN kernel stores it) and the direction / normal
+ * v3.  The state `in` is loaded as ll_register loads it (last pose, loss, bounds, inlier rule, if_motion_deblur).  ll_normal_equations, ll_solve
+ * and ll_solve_fused then run the unchanged staging and evaluation of the solver kernel over exactly these blocks. */
+int ll_set_blocks(ll_ctx* ctx, const ll_reg_state* in, size_t n, const int32_t* type, const ll_point* p, const float* a3, const double* v3);
+/* ... and one fused ICP iteration of the solver over the resident blocks (one launch, as ll_register runs it): solve #1 (prerun iterations) from
+ * x_io, the loss-corrected L1 norm of every slot, the inlier threshold max(inliner_dis, K10 order statistic), the drop of the blocks above it,
+ * solve #2 (max_iterations).  x_io <- solve #2's result; *n_distinct = distinct finite L1 norms, *n_kept = blocks solve #2 evaluated,
+ * l1_out[n] (or NULL) = the L1 norms (+inf for invalid slots), iterations[2] = LM iterations of solve #1 and #2. */
+int ll_solve_fused(ll_ctx* ctx, int prerun, int max_iterations, double x_io[7], double* threshold, int* n_distinct, int* n_kept, double* l1_out,
+                   int iterations[2]);
 
 /* ---- N4: loop-closure reuse of S3 ----------------------------------------------------------------------- */
 /* Replaces Scene_alignment::find_tranfrom_of_two_mappings (scene_alignment.hpp:269-353) from the point where the four feature clouds exist:

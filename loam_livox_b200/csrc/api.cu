@@ -379,6 +379,7 @@ int register_device(ll_ctx* ctx, const ll_map* map, const RegArrays& A, int nc, 
   ctx->last_nc = nc; ctx->last_ns = ns;
   const int cap_check = M > in->maximum_allow_residual_block ? 1 : 0;   // fewer slots than the cap: neither the pre-skip nor the drop rule can fire
   if (M == 0) { ctx->set_error("no features"); return LL_ERR_NO_BLOCKS; }
+  LL_TRY(solve_capacity(ctx, M, in->if_motion_deblur ? 1 : 0));   // before anything of this registration is enqueued
   RegDevState* h = (RegDevState*)ctx->pinned;
   fill_state(h, in);
   LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, sizeof(RegDevState), cudaMemcpyHostToDevice, s));
@@ -571,6 +572,57 @@ int ll_solve(ll_ctx* ctx, int max_iterations, double x_io[7], double* initial_co
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   for (int k = 0; k < 7; k++) x_io[k] = hs->x[k];
   if (initial_cost) *initial_cost = hs->lm.initial_cost; if (final_cost) *final_cost = hs->lm.final_cost; if (iterations) *iterations = hs->lm.iteration;
+  return LL_OK;
+}
+int ll_set_blocks(ll_ctx* ctx, const ll_reg_state* in, size_t n, const int32_t* type, const ll_point* p, const float* a3, const double* v3) {
+  if (!ctx || !in || (n > 0 && (!type || !p || !a3 || !v3))) return LL_ERR_INVALID;
+  if (n > (size_t)ctx->cfg.max_features) { ctx->set_error("more blocks than max_features"); return LL_ERR_CAPACITY; }
+  const int M = (int)n;
+  LL_TRY(solve_capacity(ctx, M, in->if_motion_deblur ? 1 : 0));
+  for (int i = 0; i < M; i++) if (type[i] < 0 || type[i] > 2) { ctx->set_error("block type must be 0, 1 (line) or 2 (plane)"); return LL_ERR_INVALID; }
+  cudaSetDevice(ctx->device);
+  RegArrays A; LL_TRY(reg_arrays(ctx, M, &A));
+  cudaStream_t s = ctx->stream;
+  std::vector<float4> ba(M);
+  for (int i = 0; i < M; i++) { ba[i].x = a3[3 * i]; ba[i].y = a3[3 * i + 1]; ba[i].z = a3[3 * i + 2]; memcpy(&ba[i].w, &type[i], 4); }
+  if (M > 0) {
+    LL_CUDA(ctx, cudaMemcpyAsync(A.feat, p, (size_t)M * 16, cudaMemcpyHostToDevice, s));
+    LL_CUDA(ctx, cudaMemcpyAsync(A.blk_a, ba.data(), (size_t)M * 16, cudaMemcpyHostToDevice, s));
+    LL_CUDA(ctx, cudaMemcpyAsync(A.blk_v, v3, (size_t)M * 24, cudaMemcpyHostToDevice, s));
+  }
+  RegDevState* h = (RegDevState*)ctx->pinned; fill_state(h, in);
+  for (int i = 0; i < M; i++) h->n_blocks += type[i] != 0 ? 1 : 0;   // what the kNN kernel counts: the drop rule of the residual-block cap reads it
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, sizeof(RegDevState), cudaMemcpyHostToDevice, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));   // the pageable staging above goes out of scope
+  ctx->hook_slots = M; ctx->hook_cap_check = M > in->maximum_allow_residual_block ? 1 : 0;
+  ctx->reg_deblur = in->if_motion_deblur ? 1 : 0; ctx->solve_world = 1;
+  return LL_OK;
+}
+int ll_solve_fused(ll_ctx* ctx, int prerun, int max_iterations, double x_io[7], double* threshold, int* n_distinct, int* n_kept, double* l1_out, int iterations[2]) {
+  if (!ctx || !x_io) return LL_ERR_INVALID;
+  cudaSetDevice(ctx->device);
+  const int M = ctx->hook_slots;
+  RegArrays A; LL_TRY(reg_arrays(ctx, M, &A));
+  cudaStream_t s = ctx->stream;
+  const unsigned set_cap = l1_set_capacity(M);
+  LL_CUDA(ctx, ctx->scratch.reserve((size_t)set_cap * 8 + 256));
+  double* hx = (double*)((char*)ctx->pinned + 2 * align256(sizeof(RegDevState)));
+  for (int k = 0; k < 7; k++) hx[k] = x_io[k];
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg->x, hx, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
+  // a fused launch ends with the ICP termination test: the flag and the iteration totals start afresh for every call
+  LL_CUDA(ctx, cudaMemsetAsync(&ctx->d_reg->icp_done, 0, sizeof(int), s));
+  LL_CUDA(ctx, cudaMemsetAsync(&ctx->d_reg->total_lm_iterations, 0, 2 * sizeof(int), s));   // total_lm_iterations, total_evaluations
+  SolveArgs sa = solve_args(ctx, A, M, SOLVE_FUSED, max_iterations);
+  sa.prerun_iterations = prerun; sa.table = (unsigned long long*)ctx->scratch.p; sa.table_mask = set_cap - 1;
+  sa.cap_check = ctx->hook_cap_check;
+  LL_TRY(launch_solve(ctx, sa));
+  RegDevState* hs = (RegDevState*)((char*)ctx->pinned + align256(sizeof(RegDevState)));
+  LL_CUDA(ctx, cudaMemcpyAsync(hs, ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
+  if (l1_out && M > 0) LL_CUDA(ctx, cudaMemcpyAsync(l1_out, A.l1, (size_t)M * sizeof(double), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  for (int k = 0; k < 7; k++) x_io[k] = hs->x[k];
+  if (threshold) *threshold = hs->inlier_threshold; if (n_distinct) *n_distinct = hs->n_unique; if (n_kept) *n_kept = hs->num_residual_blocks;
+  if (iterations) { iterations[1] = hs->lm.iteration; iterations[0] = hs->total_lm_iterations - hs->lm.iteration; }
   return LL_OK;
 }
 int ll_inlier_select(ll_ctx* ctx, const double* l1, size_t n, double ratio, int path, double* value, int* n_distinct) {

@@ -128,7 +128,8 @@ struct ll_ctx {
   cudaEvent_t evp[5 * 16 + 2] = {nullptr};   // per-ICP-iteration phase events
   std::string err;
   uint64_t launches = 0;
-  int hook_slots = 0;      // slot count left behind by ll_build_blocks for the parity hooks
+  int hook_slots = 0;      // slot count left behind by ll_build_blocks / ll_set_blocks for the parity hooks
+  int hook_cap_check = 0;  // ll_set_blocks: the slots exceed the state's residual-block cap (ll_solve_fused applies the drop rule, as a registration does)
   int last_nc = 0, last_ns = 0;   // features of the last registration (ll_last_features_dev)
   float last_full_min_t = 10000.f, last_full_max_t = -10000.f;   // find_min_max_intensity over the last front end's full cloud (laser_mapping.hpp:1336)
   int num_sms = 0;

@@ -108,6 +108,9 @@ struct SolveArgs {
 #define LL_COMM_CTRL_OFF 8192
 #define LL_COMM_X_OFF 16384
 int launch_solve(ll_ctx* ctx, const SolveArgs& a);
+// LL_OK when M residual-block slots fit the shared memory of the solver's CTAs (deblur: the *_mb slot layout), else LL_ERR_CAPACITY with the
+// context's error set.  The one copy of the rule launch_solve applies: callers check with it before they enqueue anything.
+int solve_capacity(ll_ctx* ctx, int M, int deblur);
 int solve_prepare(ll_ctx* ctx);   // once per context: opt the solver kernels in to their dynamic shared memory
 // Parity hook: the fused solver's K10 (grid-wide de-duplication + radix select) over n values; *d_value, *d_n_distinct on the device.
 int launch_k10_select(ll_ctx* ctx, const double* d_l1, int n, const double* d_ratio, unsigned long long* table, unsigned table_mask, double* d_value, int* d_n_distinct);

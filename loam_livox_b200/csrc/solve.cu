@@ -650,12 +650,18 @@ static SolveGrid solve_grid(const ll_ctx* ctx, int M) {
   g.tiles_per_cta = ll_div_up(tiles, g.grid);
   return g;
 }
+// Dynamic shared memory of one solver CTA: whole tiles of SOLVE_THREADS slots, SLOT_BYTES (fast path) or SLOT_BYTES_MB (*_mb functors) each.
+static size_t solve_smem_bytes(const SolveGrid& sg, int deblur) { return (size_t)sg.tiles_per_cta * SOLVE_THREADS * (deblur ? SLOT_BYTES_MB : SLOT_BYTES); }
+int solve_capacity(ll_ctx* ctx, int M, int deblur) {
+  if (solve_smem_bytes(solve_grid(ctx, M), deblur) > SOLVE_MAX_SMEM) { ctx->set_error("too many residual-block slots for the shared-memory-resident solver"); return LL_ERR_CAPACITY; }
+  return LL_OK;
+}
 int launch_solve(ll_ctx* ctx, const SolveArgs& a) {
   const SolveGrid sg = solve_grid(ctx, a.M);
   int tile = sg.tile, tiles_per_cta = sg.tiles_per_cta; const int grid = sg.grid;
   const int mb = a.deblur ? 1 : 0;
-  const size_t smem = (size_t)tiles_per_cta * SOLVE_THREADS * (mb ? SLOT_BYTES_MB : SLOT_BYTES);
-  if (smem > SOLVE_MAX_SMEM) { ctx->set_error("too many residual-block slots for the shared-memory-resident solver"); return LL_ERR_CAPACITY; }
+  LL_TRY(solve_capacity(ctx, a.M, mb));
+  const size_t smem = solve_smem_bytes(sg, mb);
   void* fn = mb ? (void*)lm_solve_kernel<true> : (void*)lm_solve_kernel<false>;
   SolveArgs args = a; args.sync = ctx->d_sync; void* kargs[] = {&args, &tiles_per_cta, &tile};
   LL_CUDA(ctx, cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(SOLVE_THREADS), kargs, smem, ctx->stream));   // co-residency of the whole grid is what the exchanges rely on

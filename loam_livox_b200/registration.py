@@ -234,6 +234,7 @@ class Point_cloud_registration:
         ca, sa = C.c_int(), C.c_int()
         self.ctx.check(self.ctx._lib.ll_build_blocks(self.ctx.h, match_map.h, c.ctypes.data, c.shape[0], s.ctypes.data, s.shape[0], fmt, capi.LL_HOST, C.byref(self.state),
                                                      typ.ctypes.data, a3.ctypes.data, v3.ctypes.data, C.byref(ca), C.byref(sa)))
+        self._hook_slots = M
         return typ, a3, v3, ca.value, sa.value
 
     def normal_equations(self, x7):
@@ -253,6 +254,28 @@ class Point_cloud_registration:
         ic, fc, it = C.c_double(), C.c_double(), C.c_int()
         self.ctx.check(self.ctx._lib.ll_solve(self.ctx.h, max_iterations, x.ctypes.data, C.byref(ic), C.byref(fc), C.byref(it)))
         return x, ic.value, fc.value, it.value
+
+    def set_blocks(self, typ, p, a3, v3):
+        """Caller-given residual blocks in place of build_blocks' (ll_set_blocks): typ [M] (0 invalid / 1 line / 2 plane), p [M,4] features (scan
+        frame, intensity = time stamp), a3 [M,3] anchors (fp32), v3 [M,3] directions / normals; the state is self.state."""
+        t = np.ascontiguousarray(typ, np.int32)
+        p = np.ascontiguousarray(p, np.float32)
+        a = np.ascontiguousarray(a3, np.float32)
+        v = np.ascontiguousarray(v3, np.float64)
+        M = t.shape[0]
+        assert p.shape == (M, 4) and a.shape == (M, 3) and v.shape == (M, 3)
+        self.ctx.check(self.ctx._lib.ll_set_blocks(self.ctx.h, C.byref(self.state), M, t.ctypes.data, p.ctypes.data, a.ctypes.data, v.ctypes.data))
+        self._hook_slots = M
+
+    def solve_fused(self, x7, prerun, max_iterations, want_l1=True):
+        """One fused ICP iteration of the solver over the resident blocks (ll_solve_fused).  Returns (x, threshold, n_distinct, n_kept, l1 or
+        None, (solve #1 iterations, solve #2 iterations))."""
+        x = np.array(x7, np.float64)
+        thr, nd, nk, it = C.c_double(), C.c_int(), C.c_int(), np.zeros(2, np.int32)
+        l1 = np.empty(getattr(self, "_hook_slots", 0)) if want_l1 else None
+        self.ctx.check(self.ctx._lib.ll_solve_fused(self.ctx.h, int(prerun), int(max_iterations), x.ctypes.data, C.byref(thr), C.byref(nd), C.byref(nk),
+                                                    l1.ctypes.data if want_l1 else None, it.ctypes.data))
+        return x, thr.value, nd.value, nk.value, l1, (int(it[0]), int(it[1]))
 
 
 def inlier_select(ctx: Context, l1, ratio: float, path: int):

@@ -142,13 +142,14 @@ def test_blocks_normal_equations_and_solve(ctx, oracle):
         assert np.allclose(xg, xo, rtol=0, atol=1e-9)
 
 
-@pytest.mark.parametrize("cfg", [(5000, 45000, 1000, 9000), (20000, 180000, 3000, 27000)])
+@pytest.mark.parametrize("cfg", [(5000, 45000, 1000, 9000), (20000, 180000, 3000, 27000),
+                                 (20000, 180000, 4000, 36000), (50000, 450000, 15000, 135000)])   # 40k / 150k features: 2 and 5 tiles per solver CTA
 def test_register_pose_parity(ctx, oracle, cfg):
     from loam_livox_b200.registration import Map, Point_cloud_registration
     mc, ms, fc, fs, pose = _mk(*cfg)
     m = Map(ctx, mc, ms)
     tc, ts = oracle.KdTree(mc), oracle.KdTree(ms)
-    for seed in range(3):
+    for seed in range(3 if cfg[2] + cfg[3] <= 30000 else 1):   # one start point at the multi-tile sizes (the oracle's CPU time)
         guess = S.perturb_pose(pose, np.random.default_rng(seed))
         reg = Point_cloud_registration(ctx)
         reg.set_pose(guess.q, guess.t)
@@ -511,15 +512,22 @@ def test_deblur_blocks_normal_equations_and_solve(ctx, oracle):
 
 @pytest.mark.gpu
 def test_deblur_register_parity_on_distorted_scan(ctx, oracle):
-    """if_motion_deblur = 1 end to end: Rodrigues-interpolated matching transform + *_mb residuals, on a scan distorted by sensor motion."""
+    """if_motion_deblur = 1 end to end: Rodrigues-interpolated matching transform + *_mb residuals, on a scan distorted by sensor motion; at
+    10 000, 40 000 and 150 000 features (1, 2 and 5 tiles per solver CTA)."""
+    for nf in (10000, 40000, 150000):
+        _deblur_register_parity(ctx, oracle, nf)
+
+
+def _deblur_register_parity(ctx, oracle, nf):
     from loam_livox_b200.registration import Map, Point_cloud_registration
-    mc, ms = S.make_map(5000, 45000)
+    mc, ms = S.make_map(nf // 2, 9 * nf // 2)
     m = Map(ctx, mc, ms)
     tc, ts = oracle.KdTree(mc), oracle.KdTree(ms)
     last = S.default_pose()
-    for k, (eul, dt) in enumerate((((0.01, -0.02, 0.06), (0.20, -0.05, 0.02)), ((-0.03, 0.01, -0.10), (-0.10, 0.15, 0.0)))):
+    motions = (((0.01, -0.02, 0.06), (0.20, -0.05, 0.02)), ((-0.03, 0.01, -0.10), (-0.10, 0.15, 0.0)))
+    for k, (eul, dt) in enumerate(motions if nf == 10000 else motions[:1]):   # one motion at the multi-tile sizes (the oracle's CPU time)
         curr = S.Pose(S.quat_mul(last.q, S.quat_from_euler(*eul)), last.t + np.array(dt))
-        fc, fs = S.make_distorted_features(last, curr, 1000, 9000, seed=k)
+        fc, fs = S.make_distorted_features(last, curr, nf // 10, 9 * nf // 10, seed=k)
         reg = Point_cloud_registration(ctx, if_motion_deblur=1)
         reg.set_pose(last.q, last.t)
         st = reg.find_out_incremental_transfrom(m, fc, fs)
