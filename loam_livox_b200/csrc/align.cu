@@ -28,14 +28,15 @@ int ll_scene_align(ll_ctx* ctx, const void* src_line, size_t n_sl, const void* s
   const size_t ns[4] = {n_sl, n_sp, n_tl, n_tp}; const void* srcs[4] = {src_line, src_plane, tgt_line, tgt_plane};
   if ((int)(n_tl + n_tp) > ctx->cfg.max_features) { ctx->set_error("more target features than max_features"); return LL_ERR_CAPACITY; }
   // the four input clouds and their down-sampled versions, on the device (one arena)
-  size_t off_in[4], off_ds[4], total = 0;
-  for (int k = 0; k < 4; k++) { off_in[k] = total; total += align256((ns[k] + 1) * 16); }
-  for (int k = 0; k < 4; k++) { off_ds[k] = total; total += align256((ns[k] + 1) * 16); }
+  float4* d_in[4]; float4* d_ds[4]; int* d_cnt;
   DevBuf arena;   // released on every exit path below
-  LL_CUDA(ctx, arena.reserve(total + 256));
-  char* base = arena.as<char>(); int* d_cnt = (int*)(base + total);
+  LL_CUDA(ctx, arena.carve([&](Carve& c) {
+    for (int k = 0; k < 4; k++) d_in[k] = c.take<float4>(ns[k] + 1);
+    for (int k = 0; k < 4; k++) d_ds[k] = c.take<float4>(ns[k] + 1);
+    d_cnt = c.take<int>(4);
+  }));
   auto fail = [&](int st) { arena.release(); return st; };
-  for (int k = 0; k < 4; k++) { const int st = upload_cloud(ctx, srcs[k], ns[k], fmt, where, (float4*)(base + off_in[k])); if (st != LL_OK) return fail(st); }
+  for (int k = 0; k < 4; k++) { const int st = upload_cloud(ctx, srcs[k], ns[k], fmt, where, d_in[k]); if (st != LL_OK) return fail(st); }
   // m_pc_reg as set_up_log_dir / find_tranfrom_of_two_mappings leave it (:233-243, :292-306)
   ll_reg_state st; ll_reg_state_default(&st);
   st.icp_line = 0; st.icp_plane = 1;
@@ -59,17 +60,17 @@ int ll_scene_align(ll_ctx* ctx, const void* src_line, size_t n_sl, const void* s
     int h_cnt[4] = {0, 0, 0, 0};
     for (int k = 0; k < 4; k++) {
       if (ns[k] == 0) { cudaMemsetAsync(d_cnt + k, 0, 4, s); continue; }
-      const int stv = launch_voxel_grid(ctx, (const float4*)(base + off_in[k]), (int)ns[k], nullptr, leaf[k], (float4*)(base + off_ds[k]), d_cnt + k);
+      const int stv = launch_voxel_grid(ctx, s, ctx->scratch, d_in[k], (int)ns[k], nullptr, leaf[k], d_ds[k], d_cnt + k);
       if (stv != LL_OK) { if (map) ll_map_release(map); return fail(stv); }
     }
     if (cudaMemcpyAsync(h_cnt, d_cnt, sizeof(h_cnt), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) { if (map) ll_map_release(map); return fail(LL_ERR_CUDA); }
     runs++;
     if (h_cnt[0] == 0 || h_cnt[1] == 0) continue;   // the 4-argument overload returns 1 without touching anything (:595-603)
-    int stm = map ? ll_map_rebuild(ctx, map, base + off_ds[0], (size_t)h_cnt[0], base + off_ds[1], (size_t)h_cnt[1], LL_FMT_XYZI16, LL_DEVICE)
-                  : ll_map_build(ctx, base + off_ds[0], (size_t)h_cnt[0], base + off_ds[1], (size_t)h_cnt[1], LL_FMT_XYZI16, LL_DEVICE, &map);
+    int stm = map ? ll_map_rebuild(ctx, map, d_ds[0], (size_t)h_cnt[0], d_ds[1], (size_t)h_cnt[1], LL_FMT_XYZI16, LL_DEVICE)
+                  : ll_map_build(ctx, d_ds[0], (size_t)h_cnt[0], d_ds[1], (size_t)h_cnt[1], LL_FMT_XYZI16, LL_DEVICE, &map);
     if (stm != LL_OK) { if (map) ll_map_release(map); return fail(stm); }
     ll_reg_result r;
-    const int str = ll_register(ctx, map, base + off_ds[2], (size_t)h_cnt[2], base + off_ds[3], (size_t)h_cnt[3], LL_FMT_XYZI16, LL_DEVICE, &st, &r);
+    const int str = ll_register(ctx, map, d_ds[2], (size_t)h_cnt[2], d_ds[3], (size_t)h_cnt[3], LL_FMT_XYZI16, LL_DEVICE, &st, &r);
     if (str != LL_OK) { ll_map_release(map); return fail(str); }
     *out = r;
     // the object persists: pose and increment carry over to the next scale; q_w_last / t_w_last stay (identity, 0)

@@ -3,6 +3,7 @@
 // Host logic restated from Point_cloud_registration::find_out_incremental_transfrom
 // (loam_livox/source/point_cloud_registration.hpp:163-583): the gate at :199, the ICP loop :211-532 (the per-iteration work is
 // four kernels: kNN+blocks, solve #1, inlier select, solve #2 + pose/termination), the threshold rescale :559 and the reject gate :561-573.
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <cstdlib>
@@ -10,22 +11,26 @@
 #include "common.cuh"
 #include "kernels.cuh"
 
-int launch_inlier_select(ll_ctx* ctx, const double* d_l1, int M, double ratio, double* d_sorted, double* d_unique, int* d_n_unique);
-
-int reg_arrays(ll_ctx* ctx, int M, RegArrays* A) {
-  int cap = M > ctx->cfg.max_features ? M : ctx->cfg.max_features;
-  int scap = ctx->cfg.max_scan_points > cap ? ctx->cfg.max_scan_points : cap;
-  size_t bytes = align256((size_t)cap * 16) * 2 + align256((size_t)cap * 24) + align256((size_t)cap * 8 + 64) * 3 + 4096 +
-                 align256((size_t)cap * 20) * 2 + align256((size_t)cap * 4) * 2 + align256((size_t)scap * 16) * 4;
-  LL_CUDA(ctx, ctx->reg_buf.reserve(bytes));
-  char* p = ctx->reg_buf.as<char>();
-  auto take = [&](size_t b) { char* r = p; p += align256(b); return r; };
-  A->cap = cap;
-  A->feat = (float4*)take((size_t)cap * 16); A->blk_a = (float4*)take((size_t)cap * 16); A->blk_v = (double*)take((size_t)cap * 24);
-  A->l1 = (double*)take((size_t)cap * 8); A->l1_sorted = (double*)take((size_t)cap * 8 + 64); A->l1_unique = (double*)take((size_t)cap * 8);
-  A->n_unique = (int*)take(256); A->counts = (int*)take(256); A->bounds = (float*)take(256);
-  A->knn_idx = (int*)take((size_t)cap * 20); A->knn_d = (float*)take((size_t)cap * 20); A->perm = (int*)take((size_t)cap * 4);
-  A->tmp_a = (float4*)take((size_t)scap * 16); A->tmp_b = (float4*)take((size_t)scap * 16); A->tmp_c = (float4*)take((size_t)scap * 16); A->tmp_d = (float4*)take((size_t)scap * 16);
+// Everything whose size the config fixes, laid out once at creation: the registration arrays (max_features slots; the front end's feature
+// clouds: max_scan_points), the extractor's arrays and the front end's scratch arenas.  Callers reject more than max_features slots, so none of
+// this moves afterwards.
+static int ctx_alloc(ll_ctx* ctx) {
+  const size_t cap = (size_t)ctx->cfg.max_features, scap = ctx->cfg.max_scan_points > ctx->cfg.max_features ? (size_t)ctx->cfg.max_scan_points : cap;
+  RegArrays& A = ctx->A;
+  LL_CUDA(ctx, ctx->reg_buf.carve([&](Carve& c) {
+    A.feat = c.take<float4>(cap); A.blk_a = c.take<float4>(cap); A.blk_v = c.take<double>(cap * 3);
+    A.l1 = c.take<double>(cap); A.l1_sorted = c.take<double>(cap + 8); A.l1_unique = c.take<double>(cap);
+    A.n_unique = c.take<int>(1); A.counts = c.take<int>(16); A.bounds = c.take<float>(32);
+    A.knn_idx = c.take<int>(cap * LL_KNN); A.knn_d = c.take<float>(cap * LL_KNN); A.perm = c.take<int>(cap);
+    A.tmp_a = c.take<float4>(scap); A.tmp_b = c.take<float4>(scap); A.tmp_c = c.take<float4>(scap); A.tmp_d = c.take<float4>(scap);
+  }));
+  LL_TRY(extract_alloc(ctx));
+  // the front end: extraction + get_features + the surface VoxelGrids on fe_main, the corner VoxelGrids on fe_corner, the petals on fe_petals
+  const int n = ctx->cfg.max_scan_points;
+  const size_t vg = voxel_grid_bytes(n), pet = petals_bytes(n), gf = get_features_bytes(n);
+  LL_CUDA(ctx, ctx->fe_main.reserve(std::max(vg, std::max(pet, gf))));
+  LL_CUDA(ctx, ctx->fe_corner.reserve(vg));
+  LL_CUDA(ctx, ctx->fe_petals.reserve(pet));
   return LL_OK;
 }
 
@@ -69,35 +74,29 @@ int ll_ctx_create(const ll_config* cfg, int device, ll_ctx** out) {
   ok(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
   ok(cudaStreamCreateWithFlags(&ctx->stream2, cudaStreamNonBlocking));
   ok(cudaStreamCreateWithFlags(&ctx->stream3, cudaStreamNonBlocking));
-  ok(cudaEventCreateWithFlags(&ctx->ev_fork3, cudaEventDisableTiming)); ok(cudaEventCreateWithFlags(&ctx->ev_join3, cudaEventDisableTiming));
-  ok(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming)); ok(cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming));
-  ok(cudaEventCreateWithFlags(&ctx->ev_it[0], cudaEventDisableTiming)); ok(cudaEventCreateWithFlags(&ctx->ev_it[1], cudaEventDisableTiming));
-  ok(cudaEventCreate(&ctx->ev0)); ok(cudaEventCreate(&ctx->ev1)); ok(cudaEventCreate(&ctx->ev2)); ok(cudaEventCreate(&ctx->ev3));
-  for (int i = 0; i < 5 * 16 + 2; i++) ok(cudaEventCreate(&ctx->evp[i]));
-  ctx->pinned_cap = 1 << 16; ok(cudaHostAlloc(&ctx->pinned, ctx->pinned_cap, cudaHostAllocDefault));
+  ctx->sev.each([&](cudaEvent_t& ev) { ok(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); });
+  ctx->ev.each([&](cudaEvent_t& ev) { ok(cudaEventCreate(&ev)); });
+  ok(cudaHostAlloc((void**)&ctx->pin, sizeof(PinnedStage), cudaHostAllocDefault));
   void* dreg = nullptr; ok(cudaMalloc(&dreg, sizeof(RegDevState))); if (dreg) ok(cudaMemset(dreg, 0, sizeof(RegDevState))); ctx->d_reg = (RegDevState*)dreg;
   if (e == cudaSuccess && solve_prepare(ctx) != LL_OK) e = cudaErrorUnknown;   // per-function attributes of the solver kernels (no process-global flag: contexts are created from any thread)
+  if (e == cudaSuccess && ctx_alloc(ctx) != LL_OK) e = cudaErrorMemoryAllocation;
   if (e != cudaSuccess) { cudaGetLastError(); ll_ctx_destroy(ctx); return LL_ERR_CUDA; }
   *out = ctx; return LL_OK;
 }
 void ll_ctx_destroy(ll_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
-  if (ctx->stream) cudaStreamSynchronize(ctx->stream); if (ctx->stream2) cudaStreamSynchronize(ctx->stream2); if (ctx->stream3) cudaStreamSynchronize(ctx->stream3);
-  ctx->scratch3.release(); if (ctx->stream3) cudaStreamDestroy(ctx->stream3); if (ctx->ev_fork3) cudaEventDestroy(ctx->ev_fork3); if (ctx->ev_join3) cudaEventDestroy(ctx->ev_join3);
+  for (cudaStream_t s : {ctx->stream, ctx->stream2, ctx->stream3}) if (s) cudaStreamSynchronize(s);
   if (ctx->fg.exec) cudaGraphExecDestroy(ctx->fg.exec);
-  ctx->scratch2.release(); ctx->scratch_fe.release(); if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
-  if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork); if (ctx->ev_join) cudaEventDestroy(ctx->ev_join);
-  for (int i = 0; i < 2; i++) if (ctx->ev_it[i]) cudaEventDestroy(ctx->ev_it[i]);
-  ctx->scratch.release(); ctx->stage_in.release(); ctx->extract_buf.release(); ctx->feat_buf.release(); ctx->reg_buf.release();
-  if (ctx->pinned) cudaFreeHost(ctx->pinned);
+  for (DevBuf* b : {&ctx->scratch, &ctx->scratch2, &ctx->fe_main, &ctx->fe_corner, &ctx->fe_petals, &ctx->stage_in, &ctx->extract_buf, &ctx->feat_buf, &ctx->reg_buf}) b->release();
+  if (ctx->pin) cudaFreeHost(ctx->pin);
   if (ctx->d_reg) cudaFree(ctx->d_reg);
   if (ctx->d_sync) cudaFree(ctx->d_sync);
   if (ctx->comm_local) cudaFree(ctx->comm_local);
   for (int i = 0; i < 8; i++) if (ctx->comm_peers[i] && i != ctx->rank) cudaIpcCloseMemHandle(ctx->comm_peers[i]);
-  for (int i = 0; i < 5 * 16 + 2; i++) if (ctx->evp[i]) cudaEventDestroy(ctx->evp[i]);
-  if (ctx->ev0) cudaEventDestroy(ctx->ev0); if (ctx->ev1) cudaEventDestroy(ctx->ev1); if (ctx->ev2) cudaEventDestroy(ctx->ev2); if (ctx->ev3) cudaEventDestroy(ctx->ev3);
-  if (ctx->stream) cudaStreamDestroy(ctx->stream);
+  ctx->sev.each([](cudaEvent_t& ev) { if (ev) cudaEventDestroy(ev); });
+  ctx->ev.each([](cudaEvent_t& ev) { if (ev) cudaEventDestroy(ev); });
+  for (cudaStream_t s : {ctx->stream3, ctx->stream2, ctx->stream}) if (s) cudaStreamDestroy(s);
   delete ctx;
 }
 const char* ll_last_error(const ll_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
@@ -110,19 +109,19 @@ uint64_t ll_launch_count(const ll_ctx* ctx) { return ctx->launches; }
 static int extract_prepare(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp) {
   if ((int)n > ctx->cfg.max_scan_points) { ctx->set_error("scan larger than max_scan_points"); return LL_ERR_CAPACITY; }
   ExtractState& e = ctx->ex;
-  LL_TRY(extract_reserve(ctx, ctx->cfg.max_scan_points));
   if (stamp <= 0.0000001 || (stamp < e.last_maximum_time_stamp)) e.current_time = e.last_maximum_time_stamp; else e.current_time = stamp - e.first_receive_time;
   if (e.first_receive_time <= 0) e.first_receive_time = stamp;
   e.n = (int)n;
   if (n > 0) e.last_maximum_time_stamp = (double)(float)(e.current_time + (double)(((float)(n - 1)) * ctx->cfg.time_interval_pts));
   LL_TRY(upload_cloud(ctx, raw, n, fmt, where, e.raw));
-  double* h = (double*)((char*)ctx->pinned + 49152); *h = e.current_time;
-  LL_CUDA(ctx, cudaMemcpyAsync(e.d_time, h, sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  ctx->pin->extract_time = e.current_time;
+  LL_CUDA(ctx, cudaMemcpyAsync(e.d_time, &ctx->pin->extract_time, sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
   return LL_OK;
 }
-static int extract_enqueue(ll_ctx* ctx) {
+// The extraction on the context's stream; the petal bookkeeping's temporaries in `scratch`.
+static int extract_enqueue(ll_ctx* ctx, DevBuf& scratch) {
   ExtractState& e = ctx->ex;
-  if (e.n >= 5) LL_TRY(launch_extract(ctx, e.n));
+  if (e.n >= 5) { LL_TRY(launch_extract_points(ctx, e.n)); LL_TRY(launch_extract_petals(ctx, e.n, ctx->stream, scratch)); }
   else LL_CUDA(ctx, cudaMemsetAsync(e.d_meta, 0, 16, ctx->stream));
   return LL_OK;
 }
@@ -131,9 +130,9 @@ int ll_extract(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, doubl
   cudaSetDevice(ctx->device);
   ExtractState& e = ctx->ex;
   LL_TRY(extract_prepare(ctx, raw, n, fmt, where, stamp));
-  LL_TRY(extract_enqueue(ctx));
+  LL_TRY(extract_enqueue(ctx, ctx->scratch));
   if (n_scans) {
-    int* h = (int*)ctx->pinned;
+    int* h = ctx->pin->counts;
     LL_CUDA(ctx, cudaMemcpyAsync(h, e.d_meta, 3 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     *n_scans = h[1];
@@ -148,9 +147,9 @@ int ll_extract_reset(ll_ctx* ctx) {
 int ll_piece_bounds(ll_ctx* ctx, int pieces, float* start, float* end) {
   if (!ctx || pieces < 1 || pieces > 16) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
-  RegArrays A; LL_TRY(reg_arrays(ctx, 0, &A));
+  const RegArrays& A = ctx->A;
   LL_TRY(launch_piece_bounds(ctx, pieces, A.bounds));
-  float* h = (float*)ctx->pinned;
+  float* h = ctx->pin->bounds;
   LL_CUDA(ctx, cudaMemcpyAsync(h, A.bounds, 2 * pieces * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   for (int i = 0; i < pieces; i++) { start[i] = h[2 * i]; end[i] = h[2 * i + 1]; }
@@ -159,9 +158,9 @@ int ll_piece_bounds(ll_ctx* ctx, int pieces, float* start, float* end) {
 int ll_get_features(ll_ctx* ctx, float minimum_blur, float maximum_blur, ll_point* corners, size_t* n_corners, ll_point* surface, size_t* n_surface, ll_point* full, size_t* n_full) {
   if (!ctx) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
-  RegArrays A; LL_TRY(reg_arrays(ctx, 0, &A));
-  LL_TRY(launch_get_features(ctx, nullptr, minimum_blur, maximum_blur, A.tmp_a, A.tmp_b, A.tmp_c, A.counts));
-  int* h = (int*)ctx->pinned;
+  const RegArrays& A = ctx->A;
+  LL_TRY(launch_get_features(ctx, ctx->stream, ctx->scratch, nullptr, minimum_blur, maximum_blur, A.tmp_a, A.tmp_b, A.tmp_c, A.counts));
+  int* h = ctx->pin->counts;
   LL_CUDA(ctx, cudaMemcpyAsync(h, A.counts, 3 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   int nc = ctx->ex.n ? h[0] : 0, ns = ctx->ex.n ? h[1] : 0, nf = ctx->ex.n ? h[2] : 0;
@@ -208,11 +207,11 @@ int ll_voxel_downsample(ll_ctx* ctx, const void* in, size_t n, int fmt, int wher
   if (!ctx || !n_out || !(leaf > 0.f)) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
   *n_out = 0; if (n == 0) return LL_OK;
-  LL_CUDA(ctx, ctx->feat_buf.reserve(align256(n * 16) * 2 + 512));
-  float4* d_in = ctx->feat_buf.as<float4>(); float4* d_out = (float4*)((char*)d_in + align256(n * 16)); int* d_n = (int*)((char*)d_out + align256(n * 16));
+  float4* d_in; float4* d_out; int* d_n;
+  LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) { d_in = c.take<float4>(n); d_out = c.take<float4>(n); d_n = c.take<int>(1); }));
   LL_TRY(upload_cloud(ctx, in, n, fmt, where, d_in));
-  LL_TRY(launch_voxel_grid(ctx, d_in, (int)n, nullptr, leaf, d_out, d_n));
-  int* h = (int*)ctx->pinned;
+  LL_TRY(launch_voxel_grid(ctx, ctx->stream, ctx->scratch, d_in, (int)n, nullptr, leaf, d_out, d_n));
+  int* h = ctx->pin->counts;
   LL_CUDA(ctx, cudaMemcpyAsync(h, d_n, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   *n_out = (size_t)h[0];
@@ -223,12 +222,12 @@ int ll_transform(ll_ctx* ctx, const double q[4], const double t[3], const void* 
   if (!ctx || !q || !t) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
   if (n == 0) return LL_OK;
-  LL_CUDA(ctx, ctx->feat_buf.reserve(align256(n * 16) * 2 + 512));
-  float4* d_in = ctx->feat_buf.as<float4>(); float4* d_out = (float4*)((char*)d_in + align256(n * 16)); double* d_pose = (double*)((char*)d_out + align256(n * 16));
-  double* h = (double*)ctx->pinned; for (int k = 0; k < 4; k++) h[k] = q[k]; for (int k = 0; k < 3; k++) h[4 + k] = t[k];
+  float4* d_in; float4* d_out; double* d_pose;
+  LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) { d_in = c.take<float4>(n); d_out = c.take<float4>(n); d_pose = c.take<double>(7); }));
+  double* h = ctx->pin->pose; for (int k = 0; k < 4; k++) h[k] = q[k]; for (int k = 0; k < 3; k++) h[4 + k] = t[k];
   LL_CUDA(ctx, cudaMemcpyAsync(d_pose, h, 7 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
   LL_TRY(upload_cloud(ctx, in, n, fmt, where, d_in));
-  LL_TRY(launch_transform(ctx, d_pose, d_in, (int)n, d_out));
+  LL_TRY(launch_transform(ctx, ctx->stream, d_pose, d_in, (int)n, d_out));
   LL_CUDA(ctx, cudaMemcpyAsync(out, d_out, n * 16, cudaMemcpyDeviceToHost, ctx->stream));
   LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return LL_OK;
@@ -238,10 +237,10 @@ int ll_voxel_downsample_dev(ll_ctx* ctx, const ll_point* in_dev, size_t n, float
   if (!ctx || !n_out || !(leaf > 0.f)) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
   *n_out = 0; if (n == 0) return LL_OK;
-  LL_CUDA(ctx, ctx->feat_buf.reserve(512));
-  int* d_n = ctx->feat_buf.as<int>();
-  LL_TRY(launch_voxel_grid(ctx, (const float4*)in_dev, (int)n, nullptr, leaf, (float4*)out_dev, d_n));
-  int* h = (int*)ctx->pinned;
+  int* d_n;
+  LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) { d_n = c.take<int>(1); }));
+  LL_TRY(launch_voxel_grid(ctx, ctx->stream, ctx->scratch, (const float4*)in_dev, (int)n, nullptr, leaf, (float4*)out_dev, d_n));
+  int* h = ctx->pin->counts;
   LL_CUDA(ctx, cudaMemcpyAsync(h, d_n, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   *n_out = (size_t)h[0];
@@ -251,17 +250,17 @@ int ll_transform_dev(ll_ctx* ctx, const double q[4], const double t[3], const ll
   if (!ctx || !q || !t) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
   if (n == 0) return LL_OK;
-  LL_CUDA(ctx, ctx->feat_buf.reserve(512));
-  double* d_pose = (double*)((char*)ctx->feat_buf.p + 256);
-  double* h = (double*)((char*)ctx->pinned + 1024); for (int k = 0; k < 4; k++) h[k] = q[k]; for (int k = 0; k < 3; k++) h[4 + k] = t[k];
+  double* d_pose;
+  LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) { d_pose = c.take<double>(7); }));
+  double* h = ctx->pin->pose; for (int k = 0; k < 4; k++) h[k] = q[k]; for (int k = 0; k < 3; k++) h[4 + k] = t[k];
   LL_CUDA(ctx, cudaMemcpyAsync(d_pose, h, 7 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-  LL_TRY(launch_transform(ctx, d_pose, (const float4*)in_dev, (int)n, (float4*)out_dev));
+  LL_TRY(launch_transform(ctx, ctx->stream, d_pose, (const float4*)in_dev, (int)n, (float4*)out_dev));
   LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return LL_OK;
 }
 int ll_last_features_dev(ll_ctx* ctx, const ll_point** corner_dev, size_t* n_corner, const ll_point** surf_dev, size_t* n_surf) {
   if (!ctx) return LL_ERR_INVALID;
-  RegArrays A; LL_TRY(reg_arrays(ctx, 0, &A));
+  const RegArrays& A = ctx->A;
   if (corner_dev) *corner_dev = (const ll_point*)A.feat; if (n_corner) *n_corner = (size_t)ctx->last_nc;
   if (surf_dev) *surf_dev = (const ll_point*)(A.feat + ctx->last_nc); if (n_surf) *n_surf = (size_t)ctx->last_ns;
   return LL_OK;
@@ -274,20 +273,21 @@ static int map_index(ll_ctx* ctx, ll_map* m, const void* corner, size_t nc, cons
   const float4* d_c = (const float4*)corner; const float4* d_s = (const float4*)surf;
   int st = LL_OK;
   if (!in_place) {
-    LL_CUDA(ctx, ctx->feat_buf.reserve(align256(nc * 16) + align256(ns * 16) + 512));
-    float4* b = ctx->feat_buf.as<float4>(); d_c = b; d_s = (const float4*)((char*)b + align256(nc * 16));
-    st = upload_cloud(ctx, corner, nc, fmt, where, (float4*)d_c);
-    if (st == LL_OK) st = upload_cloud(ctx, surf, ns, fmt, where, (float4*)d_s);
+    float4* b_c; float4* b_s;
+    LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) { b_c = c.take<float4>(nc); b_s = c.take<float4>(ns); }));
+    d_c = b_c; d_s = b_s;
+    st = upload_cloud(ctx, corner, nc, fmt, where, b_c);
+    if (st == LL_OK) st = upload_cloud(ctx, surf, ns, fmt, where, b_s);
     if (st != LL_OK) return st;
   }
   // the two indices side by side: corner on the side stream with its own scratch, surface on the context's stream
   cudaStream_t s = ctx->stream;
-  LL_CUDA(ctx, cudaEventRecord(ctx->ev_fork, s));
-  LL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
-  st = build_bucket_tree_on(ctx, ctx->stream2, ctx->scratch2, d_c, (int)nc, &m->corner);
-  const int st2 = build_bucket_tree_on(ctx, s, ctx->scratch, d_s, (int)ns, &m->surf);
-  LL_CUDA(ctx, cudaEventRecord(ctx->ev_join, ctx->stream2));
-  LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->ev_join, 0));
+  LL_CUDA(ctx, cudaEventRecord(ctx->sev.fork, s));
+  LL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->sev.fork, 0));
+  st = build_bucket_tree(ctx, ctx->stream2, ctx->scratch2, d_c, (int)nc, &m->corner);
+  const int st2 = build_bucket_tree(ctx, s, ctx->scratch, d_s, (int)ns, &m->surf);
+  LL_CUDA(ctx, cudaEventRecord(ctx->sev.join, ctx->stream2));
+  LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->sev.join, 0));
   if (st == LL_OK) st = st2;
   // host inputs may be freed by the caller as soon as this returns; device inputs are consumed in stream order (the per-scan refresh never waits)
   if (st == LL_OK && where == LL_HOST && cudaStreamSynchronize(s) != cudaSuccess) st = LL_ERR_CUDA;
@@ -322,8 +322,8 @@ int ll_knn(ll_ctx* ctx, const ll_map* map, int which, const ll_point* queries, s
   if (!ctx || !map) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
   if (nq == 0) return LL_OK;
-  LL_CUDA(ctx, ctx->feat_buf.reserve(align256(nq * 16) + align256(nq * 20) * 2));
-  float4* d_q = ctx->feat_buf.as<float4>(); int* d_idx = (int*)((char*)d_q + align256(nq * 16)); float* d_d = (float*)((char*)d_idx + align256(nq * 20));
+  float4* d_q; int* d_idx; float* d_d;
+  LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) { d_q = c.take<float4>(nq); d_idx = c.take<int>(nq * LL_KNN); d_d = c.take<float>(nq * LL_KNN); }));
   LL_CUDA(ctx, cudaMemcpyAsync(d_q, queries, nq * 16, cudaMemcpyHostToDevice, ctx->stream));
   LL_TRY(launch_knn_query(ctx, which == 0 ? map->corner : map->surf, d_q, (int)nq, d_idx, d_d));
   LL_CUDA(ctx, cudaMemcpyAsync(idx5, d_idx, nq * 20, cudaMemcpyDeviceToHost, ctx->stream));
@@ -344,7 +344,8 @@ static void fill_state(RegDevState* h, const ll_reg_state* in) {
   h->cap = in->maximum_allow_residual_block; h->rng_seed = in->rng_seed;
   h->if_motion_deblur = in->if_motion_deblur ? 1 : 0; h->min_ts = in->minimum_pt_time_stamp; h->max_ts = in->maximum_pt_time_stamp;   // interp_* = 0: reset_incremtal_parameter (:120-125)
 }
-static KnnBlocksArgs knn_args(ll_ctx* ctx, const ll_map* map, const RegArrays& A, int nc, int ns, const ll_reg_state* in, bool debug) {
+static KnnBlocksArgs knn_args(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg_state* in, bool debug) {
+  const RegArrays& A = ctx->A;
   KnnBlocksArgs a; a.corner = make_view(map->corner); a.surf = make_view(map->surf); a.feat = A.feat; a.n_corner = nc; a.n_surf = ns;
   a.pose = ctx->d_reg->pose_curr; a.max_dis_line = in->maximum_dis_line_for_match; a.max_dis_plane = in->maximum_dis_plane_for_match;
   a.icp_line = in->icp_line; a.icp_plane = in->icp_plane; a.blk_a = A.blk_a; a.blk_v = A.blk_v;
@@ -356,7 +357,8 @@ static KnnBlocksArgs knn_args(ll_ctx* ctx, const ll_map* map, const RegArrays& A
   a.rank = map->rank; a.world = map->world; a.grid = map->grid; a.shard_owner = (const int*)map->shard_owner.p;
   return a;
 }
-static SolveArgs solve_args(ll_ctx* ctx, const RegArrays& A, int M, SolveMode mode, int max_iter) {
+static SolveArgs solve_args(ll_ctx* ctx, int M, SolveMode mode, int max_iter) {
+  const RegArrays& A = ctx->A;
   SolveArgs s; s.st = ctx->d_reg; s.sync = ctx->d_sync; s.feat = A.feat; s.blk_a = A.blk_a; s.blk_v = A.blk_v; s.l1 = A.l1; s.l1_sorted_unique = A.l1_unique; s.d_n_unique = A.n_unique;
   s.M = M; s.max_iterations = max_iter; s.mode = mode; s.rank = ctx->rank; s.world = ctx->solve_world; s.comm_local = (double*)ctx->comm_local;
   for (int i = 0; i < 8; i++) s.comm_peer[i] = (double*)ctx->comm_peers[i];
@@ -367,8 +369,10 @@ static SolveArgs solve_args(ll_ctx* ctx, const RegArrays& A, int M, SolveMode mo
 }  // extern "C"
 
 // Registration on features already resident in A.feat (device). Core of ll_register / ll_scan_to_pose.
-int register_device(ll_ctx* ctx, const ll_map* map, const RegArrays& A, int nc, int ns, const ll_reg_state* in, ll_reg_result* out) {
+int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg_state* in, ll_reg_result* out) {
   cudaStream_t s = ctx->stream;
+  const RegArrays& A = ctx->A;
+  RegEvents& ev = ctx->ev;
   memset(out, 0, sizeof(*out));
   out->status = 1;
   for (int k = 0; k < 4; k++) { out->q_w_curr[k] = in->q_w_curr[k]; out->q_w_incre[k] = k == 0 ? in->para_buffer_incremental[3] : in->para_buffer_incremental[k - 1]; }
@@ -380,17 +384,17 @@ int register_device(ll_ctx* ctx, const ll_map* map, const RegArrays& A, int nc, 
   const int cap_check = M > in->maximum_allow_residual_block ? 1 : 0;   // fewer slots than the cap: neither the pre-skip nor the drop rule can fire
   if (M == 0) { ctx->set_error("no features"); return LL_ERR_NO_BLOCKS; }
   LL_TRY(solve_capacity(ctx, M, in->if_motion_deblur ? 1 : 0));   // before anything of this registration is enqueued
-  RegDevState* h = (RegDevState*)ctx->pinned;
+  RegDevState* h = &ctx->pin->state_in;
   fill_state(h, in);
   LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, sizeof(RegDevState), cudaMemcpyHostToDevice, s));
-  LL_CUDA(ctx, cudaEventRecord(ctx->ev0, s));
+  LL_CUDA(ctx, cudaEventRecord(ev.total[0], s));
   out->registered = 1;
-  KnnBlocksArgs ka = knn_args(ctx, map, A, nc, ns, in, false);
+  KnnBlocksArgs ka = knn_args(ctx, map, nc, ns, in, false);
   LL_CUDA(ctx, cudaMemsetAsync(A.knn_idx, 0xff, (size_t)M * LL_KNN * 4, s));   // no seeds for the first ICP iteration
-  LL_CUDA(ctx, cudaEventRecord(ctx->evp[80], s));
-  LL_TRY(launch_query_sort(ctx, ka, A.perm));   // spatial tiles of features (Hilbert order at the initial pose)
-  LL_CUDA(ctx, cudaEventRecord(ctx->evp[81], s));
-  int iter = 0; RegDevState* hs = (RegDevState*)((char*)ctx->pinned + align256(sizeof(RegDevState)));
+  LL_CUDA(ctx, cudaEventRecord(ev.sort[0], s));
+  LL_TRY(launch_query_sort(ctx, s, ctx->scratch, ka, A.perm));   // spatial tiles of features (Hilbert order at the initial pose)
+  LL_CUDA(ctx, cudaEventRecord(ev.sort[1], s));
+  int iter = 0; RegDevState* hs = &ctx->pin->snap[0];
   const bool sharded = ctx->world > 1 && map->world > 1;
   if (sharded && (map->world != ctx->world || map->rank != ctx->rank)) { ctx->set_error("map shard and context disagree on rank/world"); return LL_ERR_INVALID; }
   // (the shard was built with halo * 1.0001 + 1 mm, shard.cu: a halo handed over as the float nearest to sqrt(gate) must pass)
@@ -400,38 +404,38 @@ int register_device(ll_ctx* ctx, const ll_map* map, const RegArrays& A, int nc, 
   if (map->world > 1 && ctx->world != map->world) { ctx->set_error("a sharded map needs a context connected to the same number of ranks (ll_comm_connect)"); return LL_ERR_INVALID; }
   if (sharded && M > ctx->cfg.max_features) { ctx->set_error("more features than max_features (exchange buffer)"); return LL_ERR_CAPACITY; }
   double* x_l1 = sharded ? (double*)((char*)ctx->comm_local + LL_COMM_X_OFF) : nullptr;
-  const unsigned set_cap = l1_set_capacity(M);   // hash set of the L1 norms (K10)
-  LL_CUDA(ctx, ctx->scratch.reserve((size_t)set_cap * 8 + 256));
+  unsigned long long* set_table = nullptr;   // hash set of the L1 norms (K10)
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { set_table = l1_set_layout(c, M); }));
   // One ICP iteration's device work + a snapshot of the 1.7 KB state into pinned slot `it & 1`.
-  RegDevState* slots[2] = {hs, (RegDevState*)((char*)hs + align256(sizeof(RegDevState)))};
+  RegDevState* slots = ctx->pin->snap;
   auto enqueue_iteration = [&](int it) -> int {
-    cudaEvent_t* e = it < 16 ? &ctx->evp[5 * it] : nullptr;
+    cudaEvent_t* e = it < LL_TIMED_ITERS ? ev.phase[it] : nullptr;
     LL_CUDA(ctx, cudaMemsetAsync(&ctx->d_reg->corner_avail, 0, 3 * sizeof(int), s));   // corner_avail, surf_avail, n_blocks
     if (sharded) LL_CUDA(ctx, cudaMemsetAsync(x_l1, 0xff, (size_t)M * sizeof(double), s));   // NaN = nobody owns a block here (peers fill it after solve #1)
-    if (it == 0) LL_CUDA(ctx, cudaEventRecord(ctx->ev1, s));
+    if (it == 0) LL_CUDA(ctx, cudaEventRecord(ev.knn_first[0], s));
     if (e) LL_CUDA(ctx, cudaEventRecord(e[0], s));
     LL_TRY(launch_knn_blocks(ctx, ka));
     if (e) LL_CUDA(ctx, cudaEventRecord(e[1], s));
-    if (it == 0) LL_CUDA(ctx, cudaEventRecord(ctx->ev2, s));
+    if (it == 0) LL_CUDA(ctx, cudaEventRecord(ev.knn_first[1], s));
     if (!sharded) {
       // one launch: solve #1 -> L1 norms -> de-duplication + order statistic -> outlier drop -> solve #2 -> pose
-      SolveArgs sa = solve_args(ctx, A, M, SOLVE_FUSED, in->cere_max_iterations);
-      sa.prerun_iterations = in->cere_prerun_times; sa.table = (unsigned long long*)ctx->scratch.p; sa.table_mask = set_cap - 1;
+      SolveArgs sa = solve_args(ctx, M, SOLVE_FUSED, in->cere_max_iterations);
+      sa.prerun_iterations = in->cere_prerun_times; sa.table = set_table; sa.table_mask = l1_set_capacity(M) - 1;
       sa.cap_check = cap_check;
       if (e) { LL_CUDA(ctx, cudaEventRecord(e[2], s)); LL_CUDA(ctx, cudaEventRecord(e[3], s)); }
       LL_TRY(launch_solve(ctx, sa));
     } else {
       if (cap_check) LL_TRY(launch_count_exchange(ctx));
-      { SolveArgs sa = solve_args(ctx, A, M, SOLVE_FIRST, in->cere_prerun_times); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
+      { SolveArgs sa = solve_args(ctx, M, SOLVE_FIRST, in->cere_prerun_times); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
       if (e) LL_CUDA(ctx, cudaEventRecord(e[2], s));
       LL_TRY(launch_l1_exchange(ctx, A.l1, M));
-      LL_TRY(launch_inlier_select(ctx, x_l1, M, in->inlier_ratio, A.l1_sorted, A.l1_unique, A.n_unique));
+      LL_TRY(launch_inlier_select(ctx, s, ctx->scratch, x_l1, M, in->inlier_ratio, A.l1_sorted, A.l1_unique, A.n_unique));
       if (e) LL_CUDA(ctx, cudaEventRecord(e[3], s));
-      { SolveArgs sa = solve_args(ctx, A, M, SOLVE_SECOND, in->cere_max_iterations); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
+      { SolveArgs sa = solve_args(ctx, M, SOLVE_SECOND, in->cere_max_iterations); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
     }
     if (e) LL_CUDA(ctx, cudaEventRecord(e[4], s));
-    LL_CUDA(ctx, cudaMemcpyAsync(slots[it & 1], ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
-    LL_CUDA(ctx, cudaEventRecord(ctx->ev_it[it & 1], s));
+    LL_CUDA(ctx, cudaMemcpyAsync(&slots[it & 1], ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
+    LL_CUDA(ctx, cudaEventRecord(ctx->sev.it[it & 1], s));
     return LL_OK;
   };
   // The host stays one iteration ahead: iteration k+1 is enqueued before iteration k's state is read back, so the GPU never waits for the
@@ -440,20 +444,20 @@ int register_device(ll_ctx* ctx, const ll_map* map, const RegArrays& A, int nc, 
   LL_TRY(enqueue_iteration(0));
   for (iter = 0; iter < in->icp_max_iterations; iter++) {
     if (speculate && iter + 1 < in->icp_max_iterations) LL_TRY(enqueue_iteration(iter + 1));
-    LL_CUDA(ctx, cudaEventSynchronize(ctx->ev_it[iter & 1]));
-    hs = slots[iter & 1];
+    LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.it[iter & 1]));
+    hs = &slots[iter & 1];
     if (hs->lm.termination == -1) {   // the iteration enqueued ahead returns at once (icp_done is set on the device); drain it before the arena is reused
       cudaStreamSynchronize(s); ctx->set_error("no residual block survived the gates / cap / inlier selection"); return LL_ERR_NO_BLOCKS;
     }
     if (hs->icp_done) break;
     if (!speculate && iter + 1 < in->icp_max_iterations) LL_TRY(enqueue_iteration(iter + 1));
   }
-  LL_CUDA(ctx, cudaEventRecord(ctx->ev3, s));
-  LL_CUDA(ctx, cudaEventSynchronize(ctx->ev3));
-  cudaEventElapsedTime(&out->gpu_ms_total, ctx->ev0, ctx->ev3); cudaEventElapsedTime(&out->gpu_ms_knn, ctx->ev1, ctx->ev2);
-  cudaEventElapsedTime(&out->gpu_ms_sort, ctx->evp[80], ctx->evp[81]);
+  LL_CUDA(ctx, cudaEventRecord(ev.total[1], s));
+  LL_CUDA(ctx, cudaEventSynchronize(ev.total[1]));
+  cudaEventElapsedTime(&out->gpu_ms_total, ev.total[0], ev.total[1]); cudaEventElapsedTime(&out->gpu_ms_knn, ev.knn_first[0], ev.knn_first[1]);
+  cudaEventElapsedTime(&out->gpu_ms_sort, ev.sort[0], ev.sort[1]);
   { const int done_iters = (iter < in->icp_max_iterations ? iter + 1 : in->icp_max_iterations);
-    for (int i = 0; i < done_iters && i < 16; i++) { float a = 0, b = 0, c = 0, d = 0; cudaEvent_t* e = &ctx->evp[5 * i];
+    for (int i = 0; i < done_iters && i < LL_TIMED_ITERS; i++) { float a = 0, b = 0, c = 0, d = 0; cudaEvent_t* e = ev.phase[i];
       cudaEventElapsedTime(&a, e[0], e[1]); cudaEventElapsedTime(&b, e[1], e[2]); cudaEventElapsedTime(&c, e[2], e[3]); cudaEventElapsedTime(&d, e[3], e[4]);
       out->gpu_ms_knn_all += a; out->gpu_ms_solve_all += b + d; out->gpu_ms_select_all += c; } }
   out->icp_iterations = (iter + 1 < in->icp_max_iterations) ? iter + 1 : in->icp_max_iterations;
@@ -480,10 +484,9 @@ int ll_register(ll_ctx* ctx, const ll_map* map, const void* scan_corner, size_t 
   if (!ctx || !map || !in || !out) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
   if ((int)(nc + ns) > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
-  RegArrays A; LL_TRY(reg_arrays(ctx, (int)(nc + ns), &A));
-  LL_TRY(upload_cloud(ctx, scan_corner, nc, fmt, where, A.feat));
-  LL_TRY(upload_cloud(ctx, scan_surf, ns, fmt, where, A.feat + nc));
-  return register_device(ctx, map, A, (int)nc, (int)ns, in, out);
+  LL_TRY(upload_cloud(ctx, scan_corner, nc, fmt, where, ctx->A.feat));
+  LL_TRY(upload_cloud(ctx, scan_surf, ns, fmt, where, ctx->A.feat + nc));
+  return register_device(ctx, map, (int)nc, (int)ns, in, out);
 }
 
 // One tiny registration (three planes and two edges: 1240 map points, 310 features) through the whole device path, result discarded.  It pays -- once, at a
@@ -520,13 +523,13 @@ int ll_build_blocks(ll_ctx* ctx, const ll_map* map, const void* scan_corner, siz
   cudaSetDevice(ctx->device);
   const int M = (int)(nc + ns);
   if (M > ctx->cfg.max_features) return LL_ERR_CAPACITY;
-  RegArrays A; LL_TRY(reg_arrays(ctx, M, &A));
+  const RegArrays& A = ctx->A;
   cudaStream_t s = ctx->stream;
   LL_TRY(upload_cloud(ctx, scan_corner, nc, fmt, where, A.feat));
   LL_TRY(upload_cloud(ctx, scan_surf, ns, fmt, where, A.feat + nc));
-  RegDevState* h = (RegDevState*)ctx->pinned; fill_state(h, in);
+  RegDevState* h = &ctx->pin->state_in; fill_state(h, in);
   LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, sizeof(RegDevState), cudaMemcpyHostToDevice, s));
-  { KnnBlocksArgs ka = knn_args(ctx, map, A, (int)nc, (int)ns, in, true); LL_CUDA(ctx, cudaMemsetAsync(A.knn_idx, 0xff, (size_t)M * LL_KNN * 4, s)); LL_TRY(launch_query_sort(ctx, ka, A.perm)); LL_TRY(launch_knn_blocks(ctx, ka)); }
+  { KnnBlocksArgs ka = knn_args(ctx, map, (int)nc, (int)ns, in, true); LL_CUDA(ctx, cudaMemsetAsync(A.knn_idx, 0xff, (size_t)M * LL_KNN * 4, s)); LL_TRY(launch_query_sort(ctx, s, ctx->scratch, ka, A.perm)); LL_TRY(launch_knn_blocks(ctx, ka)); }
   std::vector<float4> ba(M); std::vector<double> bv((size_t)M * 3);
   int cnt[2];
   LL_CUDA(ctx, cudaMemcpyAsync(ba.data(), A.blk_a, (size_t)M * 16, cudaMemcpyDeviceToHost, s));
@@ -543,17 +546,29 @@ int ll_build_blocks(ll_ctx* ctx, const ll_map* map, const void* scan_corner, siz
   ctx->hook_slots = M;   // slot count for ll_normal_equations / ll_solve
   return LL_OK;
 }
+}  // extern "C"
+
+// The solver parity hooks: x to the device state, one solver launch over the hook's slots, the state back into snap[0] (and the L1 norms
+// into l1_out when given), then synchronise.
+static int hook_solve(ll_ctx* ctx, const double x[7], const SolveArgs& sa, double* l1_out = nullptr) {
+  cudaStream_t s = ctx->stream;
+  PinnedStage* pin = ctx->pin;
+  for (int k = 0; k < 7; k++) pin->x[k] = x[k];
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg->x, pin->x, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
+  LL_TRY(launch_solve(ctx, sa));
+  LL_CUDA(ctx, cudaMemcpyAsync(&pin->snap[0], ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
+  if (l1_out && sa.M > 0) LL_CUDA(ctx, cudaMemcpyAsync(l1_out, ctx->A.l1, (size_t)sa.M * sizeof(double), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  return LL_OK;
+}
+
+extern "C" {
+
 int ll_normal_equations(ll_ctx* ctx, const double x[7], double out28[28]) {
   if (!ctx || !x || !out28) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
-  const int M = ctx->hook_slots;
-  RegArrays A; LL_TRY(reg_arrays(ctx, M, &A));
-  cudaStream_t s = ctx->stream;
-  LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg->x, x, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
-  LL_TRY(launch_solve(ctx, solve_args(ctx, A, M, SOLVE_EVALUATE, 0)));
-  RegDevState* hs = (RegDevState*)((char*)ctx->pinned + align256(sizeof(RegDevState)));
-  LL_CUDA(ctx, cudaMemcpyAsync(hs, ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  LL_TRY(hook_solve(ctx, x, solve_args(ctx, ctx->hook_slots, SOLVE_EVALUATE, 0)));
+  const RegDevState* hs = &ctx->pin->snap[0];
   for (int i = 0; i < 21; i++) out28[i] = hs->lm.H[i];
   for (int i = 0; i < 6; i++) out28[21 + i] = hs->lm.g[i];
   out28[27] = hs->lm.x_cost;
@@ -562,14 +577,8 @@ int ll_normal_equations(ll_ctx* ctx, const double x[7], double out28[28]) {
 int ll_solve(ll_ctx* ctx, int max_iterations, double x_io[7], double* initial_cost, double* final_cost, int* iterations) {
   if (!ctx || !x_io) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
-  const int M = ctx->hook_slots;
-  RegArrays A; LL_TRY(reg_arrays(ctx, M, &A));
-  cudaStream_t s = ctx->stream;
-  LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg->x, x_io, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
-  LL_TRY(launch_solve(ctx, solve_args(ctx, A, M, SOLVE_PLAIN, max_iterations)));
-  RegDevState* hs = (RegDevState*)((char*)ctx->pinned + align256(sizeof(RegDevState)));
-  LL_CUDA(ctx, cudaMemcpyAsync(hs, ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  LL_TRY(hook_solve(ctx, x_io, solve_args(ctx, ctx->hook_slots, SOLVE_PLAIN, max_iterations)));
+  const RegDevState* hs = &ctx->pin->snap[0];
   for (int k = 0; k < 7; k++) x_io[k] = hs->x[k];
   if (initial_cost) *initial_cost = hs->lm.initial_cost; if (final_cost) *final_cost = hs->lm.final_cost; if (iterations) *iterations = hs->lm.iteration;
   return LL_OK;
@@ -581,7 +590,7 @@ int ll_set_blocks(ll_ctx* ctx, const ll_reg_state* in, size_t n, const int32_t* 
   LL_TRY(solve_capacity(ctx, M, in->if_motion_deblur ? 1 : 0));
   for (int i = 0; i < M; i++) if (type[i] < 0 || type[i] > 2) { ctx->set_error("block type must be 0, 1 (line) or 2 (plane)"); return LL_ERR_INVALID; }
   cudaSetDevice(ctx->device);
-  RegArrays A; LL_TRY(reg_arrays(ctx, M, &A));
+  const RegArrays& A = ctx->A;
   cudaStream_t s = ctx->stream;
   std::vector<float4> ba(M);
   for (int i = 0; i < M; i++) { ba[i].x = a3[3 * i]; ba[i].y = a3[3 * i + 1]; ba[i].z = a3[3 * i + 2]; memcpy(&ba[i].w, &type[i], 4); }
@@ -590,7 +599,7 @@ int ll_set_blocks(ll_ctx* ctx, const ll_reg_state* in, size_t n, const int32_t* 
     LL_CUDA(ctx, cudaMemcpyAsync(A.blk_a, ba.data(), (size_t)M * 16, cudaMemcpyHostToDevice, s));
     LL_CUDA(ctx, cudaMemcpyAsync(A.blk_v, v3, (size_t)M * 24, cudaMemcpyHostToDevice, s));
   }
-  RegDevState* h = (RegDevState*)ctx->pinned; fill_state(h, in);
+  RegDevState* h = &ctx->pin->state_in; fill_state(h, in);
   for (int i = 0; i < M; i++) h->n_blocks += type[i] != 0 ? 1 : 0;   // what the kNN kernel counts: the drop rule of the residual-block cap reads it
   LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, sizeof(RegDevState), cudaMemcpyHostToDevice, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));   // the pageable staging above goes out of scope
@@ -602,24 +611,16 @@ int ll_solve_fused(ll_ctx* ctx, int prerun, int max_iterations, double x_io[7], 
   if (!ctx || !x_io) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
   const int M = ctx->hook_slots;
-  RegArrays A; LL_TRY(reg_arrays(ctx, M, &A));
   cudaStream_t s = ctx->stream;
-  const unsigned set_cap = l1_set_capacity(M);
-  LL_CUDA(ctx, ctx->scratch.reserve((size_t)set_cap * 8 + 256));
-  double* hx = (double*)((char*)ctx->pinned + 2 * align256(sizeof(RegDevState)));
-  for (int k = 0; k < 7; k++) hx[k] = x_io[k];
-  LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg->x, hx, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
+  SolveArgs sa = solve_args(ctx, M, SOLVE_FUSED, max_iterations);
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { sa.table = l1_set_layout(c, M); }));
+  sa.prerun_iterations = prerun; sa.table_mask = l1_set_capacity(M) - 1;
+  sa.cap_check = ctx->hook_cap_check;
   // a fused launch ends with the ICP termination test: the flag and the iteration totals start afresh for every call
   LL_CUDA(ctx, cudaMemsetAsync(&ctx->d_reg->icp_done, 0, sizeof(int), s));
   LL_CUDA(ctx, cudaMemsetAsync(&ctx->d_reg->total_lm_iterations, 0, 2 * sizeof(int), s));   // total_lm_iterations, total_evaluations
-  SolveArgs sa = solve_args(ctx, A, M, SOLVE_FUSED, max_iterations);
-  sa.prerun_iterations = prerun; sa.table = (unsigned long long*)ctx->scratch.p; sa.table_mask = set_cap - 1;
-  sa.cap_check = ctx->hook_cap_check;
-  LL_TRY(launch_solve(ctx, sa));
-  RegDevState* hs = (RegDevState*)((char*)ctx->pinned + align256(sizeof(RegDevState)));
-  LL_CUDA(ctx, cudaMemcpyAsync(hs, ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
-  if (l1_out && M > 0) LL_CUDA(ctx, cudaMemcpyAsync(l1_out, A.l1, (size_t)M * sizeof(double), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  LL_TRY(hook_solve(ctx, x_io, sa, l1_out));
+  const RegDevState* hs = &ctx->pin->snap[0];
   for (int k = 0; k < 7; k++) x_io[k] = hs->x[k];
   if (threshold) *threshold = hs->inlier_threshold; if (n_distinct) *n_distinct = hs->n_unique; if (n_kept) *n_kept = hs->num_residual_blocks;
   if (iterations) { iterations[1] = hs->lm.iteration; iterations[0] = hs->total_lm_iterations - hs->lm.iteration; }
@@ -631,7 +632,7 @@ int ll_inlier_select(ll_ctx* ctx, const double* l1, size_t n, double ratio, int 
   if (n > (size_t)ctx->cfg.max_features) { ctx->set_error("more values than max_features"); return LL_ERR_CAPACITY; }
   cudaSetDevice(ctx->device);
   const int M = (int)n;
-  RegArrays A; LL_TRY(reg_arrays(ctx, M, &A));
+  const RegArrays& A = ctx->A;
   cudaStream_t s = ctx->stream;
   if (M > 0) LL_CUDA(ctx, cudaMemcpyAsync(A.l1, l1, n * sizeof(double), cudaMemcpyHostToDevice, s));
   LL_CUDA(ctx, cudaMemsetAsync(A.l1_sorted, 0, 64, s));   // [0]: distinct count (path 1)
@@ -640,11 +641,11 @@ int ll_inlier_select(ll_ctx* ctx, const double* l1, size_t n, double ratio, int 
   if (path == 0) {
     double* d_ratio = &ctx->d_reg->inlier_ratio;   // read on the device as the fused solver reads it (ll_register rewrites the whole state)
     LL_CUDA(ctx, cudaMemcpyAsync(d_ratio, &ratio, sizeof(double), cudaMemcpyHostToDevice, s));
-    const unsigned set_cap = l1_set_capacity(M);
-    LL_CUDA(ctx, ctx->scratch.reserve((size_t)set_cap * 8 + 256));
-    LL_TRY(launch_k10_select(ctx, A.l1, M, d_ratio, (unsigned long long*)ctx->scratch.p, set_cap - 1, A.l1_unique, A.n_unique));
+    unsigned long long* table = nullptr;
+    LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { table = l1_set_layout(c, M); }));
+    LL_TRY(launch_k10_select(ctx, A.l1, M, d_ratio, table, l1_set_capacity(M) - 1, A.l1_unique, A.n_unique));
   } else if (M > 0) {   // the sharded mode's kernels: distinct values compacted behind a count in l1_sorted, the order statistic into l1_unique[0]
-    LL_TRY(launch_inlier_select(ctx, A.l1, M, ratio, A.l1_sorted, A.l1_unique, A.n_unique));
+    LL_TRY(launch_inlier_select(ctx, s, ctx->scratch, A.l1, M, ratio, A.l1_sorted, A.l1_unique, A.n_unique));
   }
   double v = 0.0; int nd = 0;
   LL_CUDA(ctx, cudaMemcpyAsync(&v, A.l1_unique, sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -669,7 +670,7 @@ int ll_set_point_layout(ll_ctx* ctx, const ll_point_layout* L) {
 int ll_features_to_pointcloud2(ll_ctx* ctx, int which, void* out_host, size_t cap_bytes, size_t* n_points) {
   if (!ctx || !n_points || (which != 0 && which != 1)) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
-  RegArrays A; LL_TRY(reg_arrays(ctx, 0, &A));
+  const RegArrays& A = ctx->A;
   const int n = which == 0 ? ctx->last_nc : ctx->last_ns;
   const float4* src = which == 0 ? A.feat : A.feat + ctx->last_nc;
   *n_points = (size_t)n;
@@ -707,63 +708,68 @@ int ll_debug_solver_cycles(ll_ctx* ctx, long long out8[16]) {
 // Laser_feature::laserCloudHandler for one frame, on the device: extraction, piece bounds, get_features, the extractor's VoxelGrids
 // (laser_feature_extractor.hpp:285-380) and the mapping node's input VoxelGrids (laser_mapping.hpp:1367-1373).  Leaves the features in
 // A.feat (corners then surfaces).  *dropped = 1 when the frame has <= 5 petals (:287).
-// Everything of the front end that is enqueued on the device, in the order the reference runs it; counts land in pinned memory.
-static int front_end_enqueue(ll_ctx* ctx, const ll_pipeline_cfg* pc, const RegArrays& A, int ncap) {
-  cudaStream_t s = ctx->stream;
-  const bool petals_aside = pc->whole_frame && ctx->ex.n >= 5;   // nothing downstream of get_features reads the petal bookkeeping then
-  if (petals_aside) {
-    LL_TRY(launch_extract_points(ctx, ctx->ex.n));
-    LL_CUDA(ctx, cudaEventRecord(ctx->ev_fork3, s));
-    LL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream3, ctx->ev_fork3, 0));
-    LL_TRY(launch_extract_petals(ctx, ctx->ex.n, ctx->stream3, ctx->scratch3));
-    LL_CUDA(ctx, cudaEventRecord(ctx->ev_join3, ctx->stream3));
-  } else LL_TRY(extract_enqueue(ctx));
-  const float* d_bounds = nullptr;
-  if (!pc->whole_frame) { LL_TRY(launch_piece_bounds(ctx, pc->pieces, A.bounds)); d_bounds = A.bounds + 2 * pc->use_piece; }
-  LL_TRY(launch_get_features(ctx, d_bounds, 0.f, 1.f, A.tmp_a, A.tmp_b, nullptr, A.counts));
-  int* cnt = A.counts;   // [0] corners [1] surf [2] full [4..7] VoxelGrid outputs
-  // corner chain on the side stream, surface chain on the main stream (laser_feature_extractor.hpp:372-380 then laser_mapping.hpp:1367-1373)
-  LL_CUDA(ctx, cudaEventRecord(ctx->ev_fork, s));
-  LL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_fork, 0));
-  LL_TRY(launch_voxel_grid_on(ctx, ctx->stream2, ctx->scratch2, A.tmp_a, ncap, cnt + 0, pc->extractor_leaf_corner, A.tmp_d, cnt + 4));
-  LL_TRY(launch_voxel_grid_on(ctx, ctx->stream2, ctx->scratch2, A.tmp_d, ncap, cnt + 4, pc->mapping_leaf_corner, A.tmp_a, cnt + 5));
-  LL_CUDA(ctx, cudaEventRecord(ctx->ev_join, ctx->stream2));
-  LL_TRY(launch_voxel_grid(ctx, A.tmp_b, ncap, cnt + 1, pc->extractor_leaf_surf, A.tmp_c, cnt + 6));
-  LL_TRY(launch_voxel_grid(ctx, A.tmp_c, ncap, cnt + 6, pc->mapping_leaf_surf, A.tmp_b, cnt + 7));
-  LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->ev_join, 0));
-  if (petals_aside) LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->ev_join3, 0));
-  int* h = (int*)ctx->pinned + 8192;
-  LL_CUDA(ctx, cudaMemcpyAsync(h, cnt, 12 * sizeof(int), cudaMemcpyDeviceToHost, s));   // [10], [11]: min / max time stamp of the full cloud
-  LL_CUDA(ctx, cudaMemcpyAsync(h + 12, ctx->ex.d_meta, 12, cudaMemcpyDeviceToHost, s));
+// The four VoxelGrids of a frame's features (laser_feature_extractor.hpp:372-380 then laser_mapping.hpp:1367-1373): the corner chain
+// tmp_a -> tmp_d -> tmp_a on stream2 (fe_corner), the surface chain tmp_b -> tmp_c -> tmp_b on the context's stream (fe_main).  The input
+// counts are nc_cap / ns_cap, or the device counts d_nc / d_ns when given; the outputs land in counts[4..7].
+static int voxel_chains(ll_ctx* ctx, const ll_pipeline_cfg* pc, int nc_cap, const int* d_nc, int ns_cap, const int* d_ns) {
+  cudaStream_t s = ctx->stream, s2 = ctx->stream2;
+  const RegArrays& A = ctx->A; int* cnt = A.counts;
+  LL_CUDA(ctx, cudaEventRecord(ctx->sev.fork, s));
+  LL_CUDA(ctx, cudaStreamWaitEvent(s2, ctx->sev.fork, 0));
+  LL_TRY(launch_voxel_grid(ctx, s2, ctx->fe_corner, A.tmp_a, nc_cap, d_nc, pc->extractor_leaf_corner, A.tmp_d, cnt + 4));
+  LL_TRY(launch_voxel_grid(ctx, s2, ctx->fe_corner, A.tmp_d, nc_cap, cnt + 4, pc->mapping_leaf_corner, A.tmp_a, cnt + 5));
+  LL_CUDA(ctx, cudaEventRecord(ctx->sev.join, s2));
+  LL_TRY(launch_voxel_grid(ctx, s, ctx->fe_main, A.tmp_b, ns_cap, d_ns, pc->extractor_leaf_surf, A.tmp_c, cnt + 6));
+  LL_TRY(launch_voxel_grid(ctx, s, ctx->fe_main, A.tmp_c, ns_cap, cnt + 6, pc->mapping_leaf_surf, A.tmp_b, cnt + 7));
+  LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->sev.join, 0));
   return LL_OK;
 }
 
-int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc, const RegArrays& A, int* nc_out, int* ns_out, int* dropped) {
+// Everything of the front end that is enqueued on the device, in the order the reference runs it; counts land in pinned memory.
+static int front_end_enqueue(ll_ctx* ctx, const ll_pipeline_cfg* pc, int ncap) {
   cudaStream_t s = ctx->stream;
+  const RegArrays& A = ctx->A;
+  const bool petals_aside = pc->whole_frame && ctx->ex.n >= 5;   // nothing downstream of get_features reads the petal bookkeeping then
+  if (petals_aside) {
+    LL_TRY(launch_extract_points(ctx, ctx->ex.n));
+    LL_CUDA(ctx, cudaEventRecord(ctx->sev.fork3, s));
+    LL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream3, ctx->sev.fork3, 0));
+    LL_TRY(launch_extract_petals(ctx, ctx->ex.n, ctx->stream3, ctx->fe_petals));
+    LL_CUDA(ctx, cudaEventRecord(ctx->sev.join3, ctx->stream3));
+  } else LL_TRY(extract_enqueue(ctx, ctx->fe_main));
+  const float* d_bounds = nullptr;
+  if (!pc->whole_frame) { LL_TRY(launch_piece_bounds(ctx, pc->pieces, A.bounds)); d_bounds = A.bounds + 2 * pc->use_piece; }
+  LL_TRY(launch_get_features(ctx, s, ctx->fe_main, d_bounds, 0.f, 1.f, A.tmp_a, A.tmp_b, nullptr, A.counts));
+  LL_TRY(voxel_chains(ctx, pc, ncap, A.counts + 0, ncap, A.counts + 1));   // counts: [0] corners [1] surf [2] full
+  if (petals_aside) LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->sev.join3, 0));
+  // [10], [11]: min / max time stamp of the full cloud
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->pin->fe_counts, A.counts, sizeof(ctx->pin->fe_counts), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->pin->fe_meta, ctx->ex.d_meta, sizeof(ctx->pin->fe_meta), cudaMemcpyDeviceToHost, s));
+  return LL_OK;
+}
+
+int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped) {
+  cudaStream_t s = ctx->stream;
+  const RegArrays& A = ctx->A;
   LL_TRY(extract_prepare(ctx, raw, n, fmt, where, stamp));
   const int ncap = (int)n;
-  // the front end runs on its own scratch arena (swapped in under the usual name for the duration of this function)
-  struct ScratchSwap { ll_ctx* c; ScratchSwap(ll_ctx* c_) : c(c_) { DevBuf t = c->scratch; c->scratch = c->scratch_fe; c->scratch_fe = t; }
-                       ~ScratchSwap() { DevBuf t = c->scratch; c->scratch = c->scratch_fe; c->scratch_fe = t; } } swap_guard(ctx);
   ll_ctx::FrontGraph& g = ctx->fg;
-  void* bufs[6] = {ctx->extract_buf.p, ctx->reg_buf.p, ctx->scratch.p, ctx->scratch2.p, (void*)(size_t)ctx->scratch.cap, ctx->scratch3.p};
-  const bool same = g.n == n && memcmp(&g.pc, pc, sizeof(*pc)) == 0 && memcmp(g.bufs, bufs, sizeof(bufs)) == 0;
+  const bool same = g.n == n && memcmp(&g.pc, pc, sizeof(*pc)) == 0;
   if (same && g.exec) {
     LL_CUDA(ctx, cudaGraphLaunch(g.exec, s));
     ctx->launches += g.launches;
   } else if (same && g.warm && n >= 5) {
-    // second call with this shape: every arena has its final size, so nothing allocates while the stream is being captured
+    // second call with this shape: captured (every buffer the front end touches was laid out at creation)
     if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
     const uint64_t l0 = ctx->launches;
     cudaGraph_t graph = nullptr;
     LL_CUDA(ctx, cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-    const int st = front_end_enqueue(ctx, pc, A, ncap);
+    const int st = front_end_enqueue(ctx, pc, ncap);
     const cudaError_t ce = cudaStreamEndCapture(s, &graph);
-    void* after[6] = {ctx->extract_buf.p, ctx->reg_buf.p, ctx->scratch.p, ctx->scratch2.p, (void*)(size_t)ctx->scratch.cap, ctx->scratch3.p};
-    if (st != LL_OK || ce != cudaSuccess || memcmp(after, bufs, sizeof(bufs)) != 0) {   // should not happen: fall back to eager launches
+    if (st != LL_OK || ce != cudaSuccess) {   // should not happen: fall back to eager launches
       if (graph) cudaGraphDestroy(graph);
       cudaGetLastError(); g.warm = false; g.n = 0;
-      LL_TRY(front_end_enqueue(ctx, pc, A, ncap));
+      LL_TRY(front_end_enqueue(ctx, pc, ncap));
     } else {
       g.launches = ctx->launches - l0;
       LL_CUDA(ctx, cudaGraphInstantiate(&g.exec, graph, 0));
@@ -772,13 +778,12 @@ int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, d
     }
   } else {
     if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
-    LL_TRY(front_end_enqueue(ctx, pc, A, ncap));
-    void* after[6] = {ctx->extract_buf.p, ctx->reg_buf.p, ctx->scratch.p, ctx->scratch2.p, (void*)(size_t)ctx->scratch.cap, ctx->scratch3.p};
-    g.n = n; g.pc = *pc; memcpy(g.bufs, after, sizeof(after)); g.warm = true;
+    LL_TRY(front_end_enqueue(ctx, pc, ncap));
+    g.n = n; g.pc = *pc; g.warm = true;
   }
   LL_CUDA(ctx, cudaStreamSynchronize(s));
-  int* h = (int*)ctx->pinned + 8192;
-  const int nc = h[5], ns = h[7], meta_scans = h[13];
+  const int* h = ctx->pin->fe_counts;
+  const int nc = h[5], ns = h[7], meta_scans = ctx->pin->fe_meta[1];
   ctx->last_full_min_t = ll_ord2f(h[10]); ctx->last_full_max_t = ll_ord2f(h[11]);
   *nc_out = nc; *ns_out = ns;
   *dropped = (meta_scans <= 5 && !pc->whole_frame) ? 1 : 0;
@@ -793,12 +798,11 @@ extern "C" int ll_scan_to_pose(ll_ctx* ctx, const ll_map* map, const void* raw, 
                     ll_reg_result* out, int* n_corner_used, int* n_surf_used) {
   if (!ctx || !map || !pc || !in || !out) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
-  RegArrays A; LL_TRY(reg_arrays(ctx, 0, &A));
   int nc = 0, ns = 0, dropped = 0;
-  LL_TRY(scan_front_end(ctx, raw, n, fmt, where, stamp, pc, A, &nc, &ns, &dropped));
+  LL_TRY(scan_front_end(ctx, raw, n, fmt, where, stamp, pc, &nc, &ns, &dropped));
   if (n_corner_used) *n_corner_used = nc; if (n_surf_used) *n_surf_used = ns;
   if (dropped) { memset(out, 0, sizeof(*out)); out->status = 1; ctx->set_error("frame dropped: <= 5 petals"); return LL_OK; }
-  return register_device(ctx, map, A, nc, ns, in, out);
+  return register_device(ctx, map, nc, ns, in, out);
 }
 
 // Multi-head frame (Mid-100: three Mid-40 heads, launch/rosbag_mid100.launch): Laser_feature::laserCloudHandler runs ONE Livox_laser object over
@@ -811,33 +815,29 @@ extern "C" int ll_frame_to_pose(ll_ctx* ctx, const ll_map* map, int n_heads, con
   cudaStream_t s = ctx->stream;
   size_t total = 0; for (int h = 0; h < n_heads; h++) total += ns[h];
   if ((int)total > ctx->cfg.max_scan_points) { ctx->set_error("frame (all heads) larger than max_scan_points"); return LL_ERR_CAPACITY; }
-  RegArrays A; LL_TRY(reg_arrays(ctx, 0, &A));
+  const RegArrays& A = ctx->A;
   int acc_c = 0, acc_s = 0;
-  int* hc = (int*)ctx->pinned + 8192;
+  int* hc = ctx->pin->fe_counts; const int* hm = ctx->pin->fe_meta;
   for (int h = 0; h < n_heads; h++) {
     LL_TRY(extract_prepare(ctx, raws[h], ns[h], fmt, where, stamps[h]));
-    LL_TRY(extract_enqueue(ctx));
+    LL_TRY(extract_enqueue(ctx, ctx->fe_main));
     const float* d_bounds = nullptr;
     if (!pc->whole_frame) { LL_TRY(launch_piece_bounds(ctx, pc->pieces, A.bounds)); d_bounds = A.bounds + 2 * pc->use_piece; }
-    LL_TRY(launch_get_features(ctx, d_bounds, 0.f, 1.f, A.tmp_a + acc_c, A.tmp_b + acc_s, nullptr, A.counts));
+    LL_TRY(launch_get_features(ctx, s, ctx->fe_main, d_bounds, 0.f, 1.f, A.tmp_a + acc_c, A.tmp_b + acc_s, nullptr, A.counts));
     LL_CUDA(ctx, cudaMemcpyAsync(hc, A.counts, 3 * sizeof(int), cudaMemcpyDeviceToHost, s));
-    LL_CUDA(ctx, cudaMemcpyAsync(hc + 4, ctx->ex.d_meta, 12, cudaMemcpyDeviceToHost, s));
+    LL_CUDA(ctx, cudaMemcpyAsync(ctx->pin->fe_meta, ctx->ex.d_meta, sizeof(ctx->pin->fe_meta), cudaMemcpyDeviceToHost, s));
     LL_CUDA(ctx, cudaStreamSynchronize(s));
-    if (ns[h] >= 5 && (hc[5] > 5 || pc->whole_frame)) { acc_c += hc[0]; acc_s += hc[1]; }   // hc[5] = meta[1] = laserCloudScans.size()
+    if (ns[h] >= 5 && (hm[1] > 5 || pc->whole_frame)) { acc_c += hc[0]; acc_s += hc[1]; }   // meta[1] = laserCloudScans.size()
   }
-  int* cnt = A.counts;   // [4..7] VoxelGrid outputs
-  LL_TRY(launch_voxel_grid(ctx, A.tmp_a, acc_c, nullptr, pc->extractor_leaf_corner, A.tmp_d, cnt + 4));
-  LL_TRY(launch_voxel_grid(ctx, A.tmp_d, acc_c > 0 ? acc_c : 0, cnt + 4, pc->mapping_leaf_corner, A.tmp_a, cnt + 5));
-  LL_TRY(launch_voxel_grid(ctx, A.tmp_b, acc_s, nullptr, pc->extractor_leaf_surf, A.tmp_c, cnt + 6));
-  LL_TRY(launch_voxel_grid(ctx, A.tmp_c, acc_s > 0 ? acc_s : 0, cnt + 6, pc->mapping_leaf_surf, A.tmp_b, cnt + 7));
-  LL_CUDA(ctx, cudaMemcpyAsync(hc, cnt, 8 * sizeof(int), cudaMemcpyDeviceToHost, s));
+  LL_TRY(voxel_chains(ctx, pc, acc_c, nullptr, acc_s, nullptr));   // counts[4..7]
+  LL_CUDA(ctx, cudaMemcpyAsync(hc, A.counts, 8 * sizeof(int), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   const int nc = hc[5], nsf = hc[7];
   if (n_corner_used) *n_corner_used = nc; if (n_surf_used) *n_surf_used = nsf;
   if (nc + nsf > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
   LL_CUDA(ctx, cudaMemcpyAsync(A.feat, A.tmp_a, (size_t)nc * 16, cudaMemcpyDeviceToDevice, s));
   LL_CUDA(ctx, cudaMemcpyAsync(A.feat + nc, A.tmp_b, (size_t)nsf * 16, cudaMemcpyDeviceToDevice, s));
-  return register_device(ctx, map, A, nc, nsf, in, out);
+  return register_device(ctx, map, nc, nsf, in, out);
 }
 
 extern "C" {

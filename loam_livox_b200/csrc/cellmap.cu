@@ -169,16 +169,32 @@ __global__ void cm_rebuild_kernel(const float4* __restrict__ pts, const int* __r
   else if (t < nk + nc && t < cap) { const int c = t - nk; const float4 p = cen[c]; npts[t] = make_float4(p.x, p.y, p.z, 0.f); nslot[t] = cen_slot[c]; nepoch[t] = epoch[cen_slot[c]]; }
 }
 
-static inline size_t cm_store_bytes(size_t cap) { return align256(cap * 16) + 2 * align256(cap * 4); }
+// A point store of `cap` points: points | their cells | the cells' epochs when stored
+struct CmStore {
+  float4* pts; int* slot; int* epoch;
+  void layout(Carve& c, size_t cap) { pts = c.take<float4>(cap); slot = c.take<int>(cap); epoch = c.take<int>(cap); }
+};
+static inline size_t cm_store_bytes(size_t cap) { CmStore st; return layout_bytes([&](Carve& c) { st.layout(c, cap); }); }
+// Store capacity for `need` points, growing from `cur` (0: none yet) by doubling
+static inline size_t cm_store_cap(size_t cur, size_t need) { size_t cap = cur > 0 ? cur : (1 << 16); while (cap < need) cap *= 2; return cap; }
+static const size_t CM_MAX_STORE = (size_t)1 << 30;
+// An append's upload of n points and their cell slots
+struct CmAppend {
+  float4* in; int* slot;
+  void layout(Carve& c, size_t n) { in = c.take<float4>(n); slot = c.take<int>(n); }
+};
+
 static int cm_reserve_store(ll_ctx* ctx, ll_cellmap* m, int need) {
   if (need <= m->cap_pts) return LL_OK;
-  int cap = m->cap_pts > 0 ? m->cap_pts : (1 << 16); while (cap < need) cap *= 2;
+  const int cap = (int)cm_store_cap((size_t)m->cap_pts, (size_t)need);
+  CmStore st;
   if (m->n_pts == 0 && m->store_buf.cap >= cm_store_bytes((size_t)cap)) {   // nothing to carry over and the (pre-reserved) allocation is large enough
-    float4* np = m->store_buf.as<float4>(); m->pts = np; m->pt_slot = (int*)((char*)np + align256((size_t)cap * 16)); m->pt_epoch = (int*)((char*)m->pt_slot + align256((size_t)cap * 4));
+    LL_CUDA(ctx, m->store_buf.carve([&](Carve& c) { st.layout(c, cap); }));
+    m->pts = st.pts; m->pt_slot = st.slot; m->pt_epoch = st.epoch;
     m->cap_pts = cap; return LL_OK;
   }
-  DevBuf nb; LL_CUDA(ctx, nb.reserve(cm_store_bytes((size_t)cap)));
-  float4* np = nb.as<float4>(); int* ns = (int*)((char*)np + align256((size_t)cap * 16)); int* ne = (int*)((char*)ns + align256((size_t)cap * 4));
+  DevBuf nb; LL_CUDA(ctx, nb.carve([&](Carve& c) { st.layout(c, cap); }));
+  float4* np = st.pts; int* ns = st.slot; int* ne = st.epoch;
   if (m->n_pts > 0) {
     LL_CUDA(ctx, cudaMemcpyAsync(np, m->pts, (size_t)m->n_pts * 16, cudaMemcpyDeviceToDevice, ctx->stream));
     LL_CUDA(ctx, cudaMemcpyAsync(ns, m->pt_slot, (size_t)m->n_pts * 4, cudaMemcpyDeviceToDevice, ctx->stream));
@@ -189,14 +205,27 @@ static int cm_reserve_store(ll_ctx* ctx, ll_cellmap* m, int need) {
   return LL_OK;
 }
 
-// CUB temporary storage of the assembly (select over the table / the store, 64-bit pair sort of the selected points)
-static size_t cm_cub_bytes(int T, int N, cudaStream_t s) {
-  const int big = T > N ? T : N;
-  size_t cub_a = 0, cub_b = 0;
-  cub::DeviceSelect::Flagged(nullptr, cub_a, cub::CountingInputIterator<int>(0), (unsigned char*)nullptr, (int*)nullptr, (int*)nullptr, big, s);
-  cub::DeviceRadixSort::SortPairs(nullptr, cub_b, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr, big, 0, 64, s);
-  return cub_a > cub_b ? cub_a : cub_b;
-}
+// The assembly's scratch over a table of T slots and a store of N points
+struct CmAssemble {
+  size_t cub_bytes = 0;   // CUB temporaries: select over the table / the store, 64-bit pair sort of the selected points
+  unsigned char* sel; int* cslots; unsigned long long* ckeys; unsigned long long* ckeys2; int* cslots2; int* rank;
+  unsigned char* fsel; unsigned char* fkeep; int* isel; int* ikeep; unsigned long long* vk; unsigned long long* vk2; int* isel2;
+  unsigned char* heads; int* seg; int* cslot; int* cnt; char* cub_tmp;
+  CmAssemble(int T, int N) {
+    const int big = T > N ? T : N;
+    size_t cub_a = 0, cub_b = 0;
+    cub::DeviceSelect::Flagged(nullptr, cub_a, cub::CountingInputIterator<int>(0), (unsigned char*)nullptr, (int*)nullptr, (int*)nullptr, big);
+    cub::DeviceRadixSort::SortPairs(nullptr, cub_b, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr, big, 0, 64);
+    cub_bytes = cub_a > cub_b ? cub_a : cub_b;
+  }
+  void layout(Carve& c, size_t T, size_t N) {
+    sel = c.take<unsigned char>(T); cslots = c.take<int>(T); ckeys = c.take<unsigned long long>(T); ckeys2 = c.take<unsigned long long>(T); cslots2 = c.take<int>(T); rank = c.take<int>(T);
+    fsel = c.take<unsigned char>(N); fkeep = c.take<unsigned char>(N); isel = c.take<int>(N); ikeep = c.take<int>(N); vk = c.take<unsigned long long>(N); vk2 = c.take<unsigned long long>(N);
+    isel2 = c.take<int>(N); heads = c.take<unsigned char>(N); seg = c.take<int>(N); cslot = c.take<int>(N);
+    cnt = c.take<int>(16); cub_tmp = c.take<char>(cub_bytes);
+  }
+};
+static size_t cm_assemble_bytes(int T, int N) { CmAssemble a(T, N); return layout_bytes([&](Carve& c) { a.layout(c, T, N); }); }
 
 extern "C" {
 
@@ -205,16 +234,15 @@ extern "C" {
 int ll_cellmap_reserve(ll_ctx* ctx, ll_cellmap* m, size_t store_points, size_t scan_points) {
   if (!ctx || !m) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
-  size_t cap = 1 << 16; while (cap < store_points) cap *= 2;
-  if (cap > (size_t)1 << 30) return LL_ERR_INVALID;
-  if (m->n_pts == 0) { LL_CUDA(ctx, m->store_buf.reserve_floor(cm_store_bytes(cap))); LL_TRY(cm_reserve_store(ctx, m, (int)cap)); }
-  else LL_TRY(cm_reserve_store(ctx, m, (int)cap));
+  const size_t cap = cm_store_cap(0, store_points);
+  if (cap > CM_MAX_STORE) return LL_ERR_INVALID;
+  if (m->n_pts == 0) LL_CUDA(ctx, m->store_buf.reserve_floor(cm_store_bytes(cap)));
+  LL_TRY(cm_reserve_store(ctx, m, (int)cap));
   LL_CUDA(ctx, m->store_alt.reserve_floor(cm_store_bytes(cap)));
-  LL_CUDA(ctx, m->out_buf.reserve_floor(cap * 16 + 256));
-  if (scan_points) LL_CUDA(ctx, m->tmp_buf.reserve_floor(align256(scan_points * 16) + align256(scan_points * 4) + 256));
-  // the assembly's scratch (layout in ll_cellmap_assemble): 29 B per table slot + 39 B per stored point + alignment + CUB
-  const size_t T = (size_t)m->table_cap;
-  LL_CUDA(ctx, ctx->scratch.reserve_floor(29 * T + 39 * cap + 20 * 256 + cm_cub_bytes((int)T, (int)cap, ctx->stream) + 1024));
+  LL_CUDA(ctx, m->out_buf.reserve_floor(layout_bytes([&](Carve& c) { c.take<float4>(cap); })));
+  CmAppend ap;
+  if (scan_points) LL_CUDA(ctx, m->tmp_buf.reserve_floor(layout_bytes([&](Carve& c) { ap.layout(c, scan_points); })));
+  LL_CUDA(ctx, ctx->scratch.reserve_floor(cm_assemble_bytes(m->table_cap, (int)cap)));
   return LL_OK;
 }
 
@@ -224,12 +252,12 @@ int ll_cellmap_create(ll_ctx* ctx, float resolution, int revisit_threshold, int 
   ll_cellmap* m = new ll_cellmap(); m->device = ctx->device; m->resolution = resolution * 0.5f; m->revisit_threshold = revisit_threshold;
   int cap = 1 << 12; while (cap < 2 * (max_cells > 0 ? max_cells : (1 << 20))) cap <<= 1;
   m->table_cap = cap;
-  size_t bytes = align256((size_t)cap * 8) + 4 * align256((size_t)cap * 4) + 256;
-  if (m->table_buf.reserve(bytes) != cudaSuccess) { delete m; ctx->set_error("cell table allocation failed"); return LL_ERR_CUDA; }
-  char* p = m->table_buf.as<char>();
-  m->keys = (unsigned long long*)p; p += align256((size_t)cap * 8);
-  m->last_update = (int*)p; p += align256((size_t)cap * 4); m->create_frame = (int*)p; p += align256((size_t)cap * 4);
-  m->epoch = (int*)p; p += align256((size_t)cap * 4); m->bump = (int*)p; p += align256((size_t)cap * 4); m->d_counters = (int*)p;
+  const cudaError_t e = m->table_buf.carve([&](Carve& c) {
+    m->keys = c.take<unsigned long long>(cap);
+    m->last_update = c.take<int>(cap); m->create_frame = c.take<int>(cap); m->epoch = c.take<int>(cap); m->bump = c.take<int>(cap);
+    m->d_counters = c.take<int>(16);
+  });
+  if (e != cudaSuccess) { delete m; ctx->set_error("cell table allocation failed"); return LL_ERR_CUDA; }
   cudaMemsetAsync(m->keys, 0xff, (size_t)cap * 8, ctx->stream); cudaMemsetAsync(m->d_counters, 0, 64, ctx->stream);
   if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) { m->table_buf.release(); delete m; return LL_ERR_CUDA; }
   *out = m; return LL_OK;
@@ -260,8 +288,8 @@ int ll_cellmap_append(ll_ctx* ctx, ll_cellmap* m, const void* pts, size_t n, int
   const bool first = m->current_frame_idx == 0 && m->n_pts == 0;
   if (n > 0) {
     LL_TRY(cm_reserve_store(ctx, m, m->n_pts + (int)n));
-    LL_CUDA(ctx, m->tmp_buf.reserve(align256(n * 16) + align256(n * 4) + 256));
-    float4* d_in = m->tmp_buf.as<float4>(); int* d_slot = (int*)((char*)d_in + align256(n * 16));
+    CmAppend ap; LL_CUDA(ctx, m->tmp_buf.carve([&](Carve& c) { ap.layout(c, n); }));
+    float4* d_in = ap.in; int* d_slot = ap.slot;
     LL_TRY(upload_cloud(ctx, pts, n, fmt, where, d_in));
     const float box = m->resolution * 1.0f, half = m->resolution * 0.5f;
     const int blocks = ll_div_up((int)n, 256), cur = m->current_frame_idx;
@@ -293,21 +321,15 @@ int ll_cellmap_assemble(ll_ctx* ctx, ll_cellmap* m, const double q_wxyz[4], cons
   if (N == 0) return LL_OK;
   CmView v; for (int k = 0; k < 4; k++) v.q[k] = q_wxyz[k]; for (int k = 0; k < 3; k++) { v.t[k] = t[k]; v.sp[k] = (float)t[k]; }
   v.r2 = (double)search_range * (double)search_range; v.fov = fov_deg; v.box = m->resolution * 1.0f; v.half = m->resolution * 0.5f;
-  size_t cub_c = cm_cub_bytes(T, N, s);
-  // scratch layout
-  size_t o = 0; auto take = [&](size_t b) { size_t r = o; o += align256(b); return r; };
-  const size_t o_sel = take(T), o_cslots = take((size_t)T * 4), o_ckeys = take((size_t)T * 8), o_ckeys2 = take((size_t)T * 8), o_cslots2 = take((size_t)T * 4), o_rank = take((size_t)T * 4),
-               o_fsel = take(N), o_fkeep = take(N), o_isel = take((size_t)N * 4), o_ikeep = take((size_t)N * 4), o_vk = take((size_t)N * 8), o_vk2 = take((size_t)N * 8), o_isel2 = take((size_t)N * 4),
-               o_heads = take(N), o_seg = take((size_t)N * 4), o_cslot = take((size_t)N * 4), o_cnt = take(64), o_cub = take(cub_c + 256);
-  LL_CUDA(ctx, ctx->scratch.reserve(o));
-  char* b = ctx->scratch.as<char>();
-  unsigned char* sel = (unsigned char*)(b + o_sel); int* cslots = (int*)(b + o_cslots); unsigned long long* ckeys = (unsigned long long*)(b + o_ckeys); unsigned long long* ckeys2 = (unsigned long long*)(b + o_ckeys2);
-  int* cslots2 = (int*)(b + o_cslots2); int* rank = (int*)(b + o_rank); unsigned char* fsel = (unsigned char*)(b + o_fsel); unsigned char* fkeep = (unsigned char*)(b + o_fkeep);
-  int* isel = (int*)(b + o_isel); int* ikeep = (int*)(b + o_ikeep); unsigned long long* vk = (unsigned long long*)(b + o_vk); unsigned long long* vk2 = (unsigned long long*)(b + o_vk2); int* isel2 = (int*)(b + o_isel2);
-  unsigned char* heads = (unsigned char*)(b + o_heads); int* seg = (int*)(b + o_seg); int* cslot = (int*)(b + o_cslot); int* cnt = (int*)(b + o_cnt); void* cub_tmp = b + o_cub;
+  CmAssemble a(T, N);
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { a.layout(c, T, N); }));
+  unsigned char* sel = a.sel; int* cslots = a.cslots; unsigned long long* ckeys = a.ckeys; unsigned long long* ckeys2 = a.ckeys2;
+  int* cslots2 = a.cslots2; int* rank = a.rank; unsigned char* fsel = a.fsel; unsigned char* fkeep = a.fkeep;
+  int* isel = a.isel; int* ikeep = a.ikeep; unsigned long long* vk = a.vk; unsigned long long* vk2 = a.vk2; int* isel2 = a.isel2;
+  unsigned char* heads = a.heads; int* seg = a.seg; int* cslot = a.cslot; int* cnt = a.cnt; void* cub_tmp = a.cub_tmp; size_t cub_c = a.cub_bytes;
   // cnt: [0] selected cells, [1] selected points, [2] kept points, [3] segments (output points)
-  LL_CUDA(ctx, m->out_buf.reserve((size_t)N * 16 + 256));
-  float4* d_out = m->out_buf.as<float4>();
+  float4* d_out = nullptr;
+  LL_CUDA(ctx, m->out_buf.carve([&](Carve& c) { d_out = c.take<float4>(N); }));
   // 1. cells within range and inside the FOV, ranked by ascending key
   cm_select_cells_kernel<<<ll_div_up(T, 256), 256, 0, s>>>(m->keys, T, v, sel);
   LL_CUDA(ctx, cub::DeviceSelect::Flagged(cub_tmp, cub_c, cub::CountingInputIterator<int>(0), sel, cslots, cnt + 0, T, s));
@@ -340,10 +362,10 @@ int ll_cellmap_assemble(ll_ctx* ctx, ll_cellmap* m, const double q_wxyz[4], cons
   // 3. down-sample-and-replace (m_down_sample_replace = 1, laser_mapping.hpp:277,492-495,510-513): rebuild the store
   if (down_sample_replace) {
     const int n_new = n_keep + n_cen;
-    int cap_new = m->cap_pts; while (cap_new < n_new) cap_new *= 2;
+    const int cap_new = (int)cm_store_cap((size_t)m->cap_pts, (size_t)n_new);
     DevBuf& nb = m->store_alt;   // ping-pong: the two stores persist, so a refresh allocates nothing in steady state
-    LL_CUDA(ctx, nb.reserve(align256((size_t)cap_new * 16) + 2 * align256((size_t)cap_new * 4)));
-    float4* np = nb.as<float4>(); int* ns = (int*)((char*)np + align256((size_t)cap_new * 16)); int* ne = (int*)((char*)ns + align256((size_t)cap_new * 4));
+    CmStore st; LL_CUDA(ctx, nb.carve([&](Carve& c) { st.layout(c, cap_new); }));
+    float4* np = st.pts; int* ns = st.slot; int* ne = st.epoch;
     cm_rebuild_kernel<<<ll_div_up(n_new > 0 ? n_new : 1, 256), 256, 0, s>>>(m->pts, m->pt_slot, m->pt_epoch, ikeep, cnt + 2, d_out, cslot, cnt + 3, m->epoch, np, ns, ne, cap_new);
     { DevBuf t = m->store_buf; m->store_buf = m->store_alt; m->store_alt = t; }   // stream-ordered: later work on this stream sees the new store
     m->pts = np; m->pt_slot = ns; m->pt_epoch = ne; m->cap_pts = cap_new; m->n_pts = n_new;

@@ -96,8 +96,7 @@ __global__ void transform_kernel(const double* __restrict__ pose7, const float4*
   double wx, wy, wz; qrot_d(q, (double)p.x, (double)p.y, (double)p.z, wx, wy, wz);
   out[i] = make_float4((float)(wx + pose7[4]), (float)(wy + pose7[5]), (float)(wz + pose7[6]), p.w);
 }
-int launch_transform(ll_ctx* ctx, const double* d_pose7, const float4* d_in, int n, float4* d_out) { return launch_transform_on(ctx, ctx->stream, d_pose7, d_in, n, d_out); }
-int launch_transform_on(ll_ctx* ctx, cudaStream_t s, const double* d_pose7, const float4* d_in, int n, float4* d_out) {
+int launch_transform(ll_ctx* ctx, cudaStream_t s, const double* d_pose7, const float4* d_in, int n, float4* d_out) {
   if (n == 0) return LL_OK;
   transform_kernel<<<ll_div_up(n, 256), 256, 0, s>>>(d_pose7, d_in, n, nullptr, d_out); ctx->launches++;
   LL_CUDA(ctx, cudaGetLastError());
@@ -200,31 +199,38 @@ __global__ void vg_centroid_kernel(const float4* __restrict__ in, const VgMeta* 
   out[s] = make_float4(sx / cnt, sy / cnt, sz / cnt, si / cnt);
 }
 
-int launch_voxel_grid(ll_ctx* ctx, const float4* d_in, int n_cap, const int* d_n_in, float leaf, float4* d_out, int* d_n_out) {
-  return launch_voxel_grid_on(ctx, ctx->stream, ctx->scratch, d_in, n_cap, d_n_in, leaf, d_out, d_n_out);
-}
-// Same, on an explicit stream with its own scratch arena (two VoxelGrid chains of one scan run side by side: every kernel here is far too
-// small to fill the GPU, so the chains overlap almost perfectly).
-int launch_voxel_grid_on(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_in, int n_cap, const int* d_n_in, float leaf, float4* d_out, int* d_n_out) {
-  if (n_cap <= 0) { LL_CUDA(ctx, cudaMemsetAsync(d_n_out, 0, sizeof(int), s)); return LL_OK; }
+// The scratch of one VoxelGrid over n_cap points (n_cap > 0).
+struct VgScratch {
   size_t sort_bytes = 0, sel_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, n_cap, 0, 32, s);
-  cub::DeviceSelect::If(nullptr, sel_bytes, cub::CountingInputIterator<int>(0), (int*)nullptr, (int*)nullptr, n_cap, VgHead{nullptr}, s);
-  size_t tmp_bytes = sort_bytes > sel_bytes ? sort_bytes : sel_bytes;
-  size_t o_meta = 0, o_k0 = align256(sizeof(VgMeta) + 16), o_k1 = o_k0 + align256((size_t)n_cap * 4), o_v0 = o_k1 + align256((size_t)n_cap * 4), o_v1 = o_v0 + align256((size_t)n_cap * 4),
-         o_seg = o_v1 + align256((size_t)n_cap * 4), o_tmp = o_seg + align256((size_t)n_cap * 4);
-  LL_CUDA(ctx, scratch.reserve(o_tmp + tmp_bytes + 256));
-  char* base = scratch.as<char>();
-  VgMeta* meta = (VgMeta*)(base + o_meta); int* d_num_seg = (int*)(base + o_meta + sizeof(VgMeta));
-  unsigned* k0 = (unsigned*)(base + o_k0); unsigned* k1 = (unsigned*)(base + o_k1); int* v0 = (int*)(base + o_v0); int* v1 = (int*)(base + o_v1);
-  int* seg = (int*)(base + o_seg);
+  VgMeta* meta; int* d_num_seg; unsigned* k0; unsigned* k1; int* v0; int* v1; int* seg; char* tmp;
+  explicit VgScratch(int n_cap) {
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, n_cap, 0, 32);
+    cub::DeviceSelect::If(nullptr, sel_bytes, cub::CountingInputIterator<int>(0), (int*)nullptr, (int*)nullptr, n_cap, VgHead{nullptr});
+  }
+  void layout(Carve& c, int n_cap) {
+    meta = c.take<VgMeta>(1); d_num_seg = c.take<int>(1);
+    k0 = c.take<unsigned>(n_cap); k1 = c.take<unsigned>(n_cap); v0 = c.take<int>(n_cap); v1 = c.take<int>(n_cap); seg = c.take<int>(n_cap);
+    tmp = c.take<char>(sort_bytes > sel_bytes ? sort_bytes : sel_bytes);
+  }
+};
+size_t voxel_grid_bytes(int n_cap) {
+  if (n_cap <= 0) return 0;
+  VgScratch v(n_cap);
+  return layout_bytes([&](Carve& c) { v.layout(c, n_cap); });
+}
+// On an explicit stream with its own scratch arena: VoxelGrid chains run side by side (every kernel here is far too small to fill the GPU,
+// so the chains overlap almost perfectly).
+int launch_voxel_grid(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_in, int n_cap, const int* d_n_in, float leaf, float4* d_out, int* d_n_out) {
+  if (n_cap <= 0) { LL_CUDA(ctx, cudaMemsetAsync(d_n_out, 0, sizeof(int), s)); return LL_OK; }
+  VgScratch v(n_cap);
+  LL_CUDA(ctx, scratch.carve([&](Carve& c) { v.layout(c, n_cap); }));
   const int blocks = ll_div_up(n_cap, 256);
-  LL_CUDA(ctx, cudaMemsetAsync(meta, 0, sizeof(VgMeta), s));
-  vg_minmax_setup_kernel<<<min(blocks, ctx->num_sms * 2), 256, 0, s>>>(d_in, meta, n_cap, d_n_in, leaf);
-  vg_keys_kernel<<<blocks, 256, 0, s>>>(d_in, meta, n_cap, k0, v0);
-  LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(base + o_tmp, sort_bytes, k0, k1, v0, v1, n_cap, 0, 32, s));
-  LL_CUDA(ctx, cub::DeviceSelect::If(base + o_tmp, sel_bytes, cub::CountingInputIterator<int>(0), seg, d_num_seg, n_cap, VgHead{k1}, s));
-  vg_centroid_kernel<<<blocks, 256, 0, s>>>(d_in, meta, v1, seg, d_num_seg, n_cap, d_out, d_n_out);
+  LL_CUDA(ctx, cudaMemsetAsync(v.meta, 0, sizeof(VgMeta), s));
+  vg_minmax_setup_kernel<<<min(blocks, ctx->num_sms * 2), 256, 0, s>>>(d_in, v.meta, n_cap, d_n_in, leaf);
+  vg_keys_kernel<<<blocks, 256, 0, s>>>(d_in, v.meta, n_cap, v.k0, v.v0);
+  LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(v.tmp, v.sort_bytes, v.k0, v.k1, v.v0, v.v1, n_cap, 0, 32, s));
+  LL_CUDA(ctx, cub::DeviceSelect::If(v.tmp, v.sel_bytes, cub::CountingInputIterator<int>(0), v.seg, v.d_num_seg, n_cap, VgHead{v.k1}, s));
+  vg_centroid_kernel<<<blocks, 256, 0, s>>>(d_in, v.meta, v.v1, v.seg, v.d_num_seg, n_cap, d_out, d_n_out);
   ctx->launches += 11;   // minmax+setup, keys, radix sort (histogram, scan, 4 onesweep passes), select (init, sweep), centroid
   LL_CUDA(ctx, cudaGetLastError());
   return LL_OK;
@@ -249,11 +255,10 @@ __global__ void __launch_bounds__(1024) l1_select_kernel(const double* __restric
   if (threadIdx.x == 0) { out[0] = v; *n_out = 1; }
 }
 
-int launch_inlier_select(ll_ctx* ctx, const double* d_l1, int M, double ratio, double* d_sorted, double* d_unique, int* d_n_unique) {
-  cudaStream_t s = ctx->stream;
+int launch_inlier_select(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const double* d_l1, int M, double ratio, double* d_sorted, double* d_unique, int* d_n_unique) {
   const unsigned cap = l1_set_capacity(M);
-  LL_CUDA(ctx, ctx->scratch.reserve((size_t)cap * 8 + 256));
-  unsigned long long* table = (unsigned long long*)ctx->scratch.p;
+  unsigned long long* table = nullptr;
+  LL_CUDA(ctx, scratch.carve([&](Carve& c) { table = l1_set_layout(c, M); }));
   int* n_tmp = (int*)d_sorted;   // d_sorted doubles as [count | compacted distinct values]
   double* uniq = d_sorted + 2;
   LL_CUDA(ctx, cudaMemsetAsync(table, 0xff, (size_t)cap * 8, s));

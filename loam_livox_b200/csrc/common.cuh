@@ -20,8 +20,20 @@
   } while (0)
 #define LL_TRY(expr) do { int _s = (expr); if (_s != LL_OK) return _s; } while (0)
 
-// sub-allocations inside one device arena start on 256-byte boundaries
-static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+// The layout of one device arena, written once: a layout function calls take() once per sub-array, in order.  Run on Carve() (null base) it
+// only counts the bytes; run on Carve(base) it also assigns the pointers.  Sub-arrays start on 256-byte boundaries.
+struct Carve {
+  char* base = nullptr; size_t bytes = 0;
+  Carve() = default;
+  explicit Carve(void* b) : base((char*)b) {}
+  template <typename T> T* take(size_t count) {
+    char* r = base ? base + bytes : nullptr;
+    bytes += (count * sizeof(T) + 255) & ~(size_t)255;
+    return (T*)r;
+  }
+};
+// Bytes of the layout `f` (a callable taking Carve&).
+template <typename F> size_t layout_bytes(F&& f) { Carve c; f(c); return c.bytes; }
 
 // Order-preserving float <-> int encoding: for non-NaN floats, int order == float order, so box bounds reduce with integer atomicMin / atomicMax.
 __host__ __device__ inline int ll_f2ord(float f) {
@@ -63,6 +75,12 @@ struct DevBuf {  // grow-only device allocation
   void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
   cudaError_t reserve_floor(size_t bytes) { if (bytes > floor) floor = bytes; return reserve(floor); }   // allocate the floor now
   template <typename T> T* as() const { return (T*)p; }
+  // Grows the buffer to the layout `f` (a callable taking Carve&), then assigns the layout's pointers inside it.
+  template <typename F> cudaError_t carve(F&& f) {
+    const cudaError_t e = reserve(layout_bytes(f));
+    if (e == cudaSuccess) { Carve c(p); f(c); }
+    return e;
+  }
 };
 
 // ------------------------------------------------------------------------------------------------ map index
@@ -117,15 +135,40 @@ struct ExtractState {
   double first_receive_time = -1, current_time = 0, last_maximum_time_stamp = 0;
 };
 
+// Registration arrays (device, one arena sized for max_features / max_scan_points at context creation)
+struct RegArrays {
+  float4* feat; float4* blk_a; double* blk_v; double* l1; double* l1_sorted; double* l1_unique;
+  int* n_unique; int* knn_idx; float* knn_d; int* perm; float4* tmp_a; float4* tmp_b; float4* tmp_c; float4* tmp_d; int* counts; float* bounds;
+};
+
 // Solver / registration device state shared between kernels (lives in global memory)
 struct RegDevState;  // defined in kernels.cuh
+struct PinnedStage;  // pinned host staging of the small transfers (kernels.cuh)
+
+// Timing events of a registration (ll_reg_result::gpu_ms_*): [0] start, [1] end
+#define LL_TIMED_ITERS 16
+struct RegEvents {
+  cudaEvent_t total[2] = {nullptr, nullptr}, knn_first[2] = {nullptr, nullptr}, sort[2] = {nullptr, nullptr};
+  cudaEvent_t phase[LL_TIMED_ITERS][5] = {};   // per ICP iteration, the bounds of its phases: kNN, solve #1, inlier select, solve #2
+  template <typename F> void each(F&& f) {
+    for (cudaEvent_t* g : {total, knn_first, sort}) { f(g[0]); f(g[1]); }
+    for (auto& it : phase) for (cudaEvent_t& e : it) f(e);
+  }
+};
+// Ordering events of the side streams (no timing)
+struct SyncEvents {
+  cudaEvent_t fork = nullptr, join = nullptr;     // stream <-> stream2
+  cudaEvent_t fork3 = nullptr, join3 = nullptr;   // stream <-> stream3
+  cudaEvent_t it[2] = {nullptr, nullptr};         // ICP iteration `it` has been snapshot into PinnedStage::snap[it & 1]
+  template <typename F> void each(F&& f) { for (cudaEvent_t* e : {&fork, &join, &fork3, &join3, &it[0], &it[1]}) f(*e); }
+};
 
 struct ll_ctx {
   int device = 0;
   ll_config cfg;
   cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;
-  cudaEvent_t evp[5 * 16 + 2] = {nullptr};   // per-ICP-iteration phase events
+  RegEvents ev;
+  SyncEvents sev;
   std::string err;
   uint64_t launches = 0;
   int hook_slots = 0;      // slot count left behind by ll_build_blocks / ll_set_blocks for the parity hooks
@@ -133,25 +176,28 @@ struct ll_ctx {
   int last_nc = 0, last_ns = 0;   // features of the last registration (ll_last_features_dev)
   float last_full_min_t = 10000.f, last_full_max_t = -10000.f;   // find_min_max_intensity over the last front end's full cloud (laser_mapping.hpp:1336)
   int num_sms = 0;
-  // arenas
-  DevBuf scratch;      // CUB temp storage
+  // arenas.  Sized at creation from the config, never moved afterwards: extract_buf, reg_buf and the front end's fe_*.
+  DevBuf scratch;      // stream: CUB temporaries, the K10 hash set, the query sort, the index build and VoxelGrids of the map side
+  DevBuf scratch2;     // stream2: the same for the corner half of the map side (index build, whole-map / append VoxelGrids, shard build)
+  DevBuf fe_main, fe_corner, fe_petals;   // the front end's arenas on stream / stream2 / stream3 (what its captured graph touches)
   DevBuf stage_in;     // raw uploads (PCL32 or XYZI16)
   ll_point_layout layout = {16, 0, 4, 8, 12, LL_I_FLOAT32};   // LL_FMT_STRIDED records
   DevBuf extract_buf;  // ExtractState arrays
-  DevBuf feat_buf;     // feature clouds / voxel-grid temporaries
-  DevBuf reg_buf;      // registration arrays
-  void* pinned = nullptr; size_t pinned_cap = 0;   // pinned host staging for small D2H/H2D control blocks
+  DevBuf feat_buf;     // uploads and results of the cloud entry points (ll_voxel_downsample, ll_transform, ll_knn, host-side map builds)
+  DevBuf reg_buf;      // RegArrays
+  RegArrays A;
+  PinnedStage* pin = nullptr;   // pinned host staging of the small H2D / D2H transfers
   ExtractState ex;
   RegDevState* d_reg = nullptr;   // device
   struct SolveSync* d_sync = nullptr;   // device: exchange rows of the solver kernels (solve.cu)
   // multi-GPU
   int rank = 0, world = 1;
-  cudaStream_t stream3 = nullptr; cudaEvent_t ev_fork3 = nullptr, ev_join3 = nullptr; DevBuf scratch3;   // second side stream: the petal bookkeeping of the extractor (whole_frame front end)
-  cudaStream_t stream2 = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_it[2] = {nullptr, nullptr}; DevBuf scratch2, scratch_fe;   // side stream of the per-scan front end; the front end's own scratch arenas (fixed once the scan size is
-                                 // known: the captured graph must never see them reallocated by the map refresh or the registration)
+  cudaStream_t stream2 = nullptr;   // side stream: the corner halves of the front end and of the map side
+  cudaStream_t stream3 = nullptr;   // second side stream: the petal bookkeeping of the extractor (whole_frame front end)
   // The per-scan front end (extract + get_features + 4 VoxelGrids + count read-back) replayed as ONE CUDA graph: ~60 launches whose
-  // enqueue cost on the host (CUB dispatch included) was longer than their execution.  Re-captured when the shape or any buffer changes.
-  struct FrontGraph { cudaGraphExec_t exec = nullptr; size_t n = 0; ll_pipeline_cfg pc; void* bufs[6] = {nullptr}; bool warm = false; uint64_t launches = 0; } fg;
+  // enqueue cost on the host (CUB dispatch included) was longer than their execution.  Every buffer it touches is fixed at creation, so it is
+  // re-captured only when the scan size or the pipeline config changes.
+  struct FrontGraph { cudaGraphExec_t exec = nullptr; size_t n = 0; ll_pipeline_cfg pc; bool warm = false; uint64_t launches = 0; } fg;
   int reg_deblur = 0;                      // if_motion_deblur of the registration whose blocks are on the device
   int solve_world = 1;                     // world size the solver kernels all-reduce over (1 unless the map in use is sharded)
   void* comm_local = nullptr;              // this rank's staging slot (device memory, IPC-exported)

@@ -239,20 +239,19 @@ __global__ void ex_scatter_kernel(int n, const float4* __restrict__ raw, const f
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-int extract_reserve(ll_ctx* ctx, int n) {
+int extract_alloc(ll_ctx* ctx) {
   ExtractState& e = ctx->ex;
-  size_t per = 16 + 4 * 7 + 3 + 4 * 5 + 8 * 2;   // generous bytes per point
-  LL_CUDA(ctx, ctx->extract_buf.reserve((size_t)n * per + 64 * 256));
-  char* p = ctx->extract_buf.as<char>();
-  auto take = [&](size_t bytes) { char* r = p; p += align256(bytes); return r; };
-  e.raw = (float4*)take((size_t)n * 16);
-  e.pt_type = (int*)take((size_t)n * 4); e.pt_label = (int*)take((size_t)n * 4);
-  e.curvature = (float*)take((size_t)n * 4); e.view_angle = (float*)take((size_t)n * 4); e.depth_sq2 = (float*)take((size_t)n * 4);
-  e.time_stamp = (float*)take((size_t)n * 4); e.polar_dis_sq2 = (float*)take((size_t)n * 4);
-  e.polar_dir = (int8_t*)take((size_t)n); e.self_mask = (uint8_t*)take((size_t)n); e.cand = (uint8_t*)take((size_t)n);
-  e.cand_idx = (int*)take((size_t)n * 4); e.split_idx = (int*)take((size_t)(n + 1) * 4);
-  e.scan_first = (int*)take((size_t)(n + 1) * 4); e.scan_last = (int*)take((size_t)(n + 1) * 4);
-  e.d_num_cand = (int*)take(256); e.d_meta = (int*)take(256); e.d_time = (double*)take(256);
+  const size_t n = (size_t)ctx->cfg.max_scan_points;
+  LL_CUDA(ctx, ctx->extract_buf.carve([&](Carve& c) {
+    e.raw = c.take<float4>(n);
+    e.pt_type = c.take<int>(n); e.pt_label = c.take<int>(n);
+    e.curvature = c.take<float>(n); e.view_angle = c.take<float>(n); e.depth_sq2 = c.take<float>(n);
+    e.time_stamp = c.take<float>(n); e.polar_dis_sq2 = c.take<float>(n);
+    e.polar_dir = c.take<int8_t>(n); e.self_mask = c.take<uint8_t>(n); e.cand = c.take<uint8_t>(n);
+    e.cand_idx = c.take<int>(n); e.split_idx = c.take<int>(n + 1);
+    e.scan_first = c.take<int>(n + 1); e.scan_last = c.take<int>(n + 1);
+    e.d_num_cand = c.take<int>(1); e.d_meta = c.take<int>(4); e.d_time = c.take<double>(1);
+  }));
   return LL_OK;
 }
 
@@ -277,21 +276,22 @@ int launch_extract_points(ll_ctx* ctx, int n) {
 }
 // The petal bookkeeping (split indices with the 50-point hysteresis, petal angles, first / last surviving point per petal: :529-604, split_laser_scan).
 // Only the piece bounds and the "<= 5 petals" test read its results, so with whole_frame = 1 the front end runs it on a side stream.
+// CUB temp | petal angles
+struct PetalsLayout {
+  size_t sel_bytes = 0; char* tmp; float* seg_angle;
+  explicit PetalsLayout(int n) { cub::DeviceSelect::Flagged(nullptr, sel_bytes, cub::CountingInputIterator<int>(0), (unsigned char*)nullptr, (int*)nullptr, (int*)nullptr, n); }
+  void layout(Carve& c, int n) { tmp = c.take<char>(sel_bytes); seg_angle = c.take<float>(n + 1); }
+};
+size_t petals_bytes(int n) { PetalsLayout P(n); return layout_bytes([&](Carve& c) { P.layout(c, n); }); }
 int launch_extract_petals(ll_ctx* ctx, int n, cudaStream_t s, DevBuf& scratch) {
   ExtractState& e = ctx->ex;
-  size_t sel_bytes = 0;
-  cub::DeviceSelect::Flagged(nullptr, sel_bytes, cub::CountingInputIterator<int>(0), (unsigned char*)nullptr, (int*)nullptr, (int*)nullptr, n, s);
-  LL_CUDA(ctx, scratch.reserve(sel_bytes + (size_t)(n + 1) * 4 + 512));
-  float* seg_angle = (float*)((char*)scratch.p + align256(sel_bytes));
-  LL_CUDA(ctx, cub::DeviceSelect::Flagged(scratch.p, sel_bytes, cub::CountingInputIterator<int>(0), e.cand, e.cand_idx, e.d_num_cand, n, s));
-  ex_petal_kernel<<<1, 32, 0, s>>>(e.raw, n, e.polar_dis_sq2, e.pt_type, e.cand, e.cand_idx, e.d_num_cand, e.split_idx, seg_angle, e.scan_first, e.scan_last, e.d_meta);
+  PetalsLayout P(n);
+  LL_CUDA(ctx, scratch.carve([&](Carve& c) { P.layout(c, n); }));
+  LL_CUDA(ctx, cub::DeviceSelect::Flagged(P.tmp, P.sel_bytes, cub::CountingInputIterator<int>(0), e.cand, e.cand_idx, e.d_num_cand, n, s));
+  ex_petal_kernel<<<1, 32, 0, s>>>(e.raw, n, e.polar_dis_sq2, e.pt_type, e.cand, e.cand_idx, e.d_num_cand, e.split_idx, P.seg_angle, e.scan_first, e.scan_last, e.d_meta);
   ctx->launches += 3;
   LL_CUDA(ctx, cudaGetLastError());
   return LL_OK;
-}
-int launch_extract(ll_ctx* ctx, int n) {
-  LL_TRY(launch_extract_points(ctx, n));
-  return launch_extract_petals(ctx, n, ctx->stream, ctx->scratch);
 }
 
 int launch_piece_bounds(ll_ctx* ctx, int pieces, float* d_start_end) {
@@ -301,19 +301,22 @@ int launch_piece_bounds(ll_ctx* ctx, int pieces, float* d_start_end) {
   return LL_OK;
 }
 
-int launch_get_features(ll_ctx* ctx, const float* d_bounds, float min_blur, float max_blur, float4* d_corners, float4* d_surf, float4* d_full, int* d_counts) {
-  ExtractState& e = ctx->ex; cudaStream_t s = ctx->stream; const int n = e.n;
+// flags | their prefix sum | CUB temp
+struct FeaturesLayout {
+  size_t scan_bytes = 0; unsigned long long* packed; unsigned long long* offs; char* tmp;
+  explicit FeaturesLayout(int n) { cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr, n); }
+  void layout(Carve& c, int n) { packed = c.take<unsigned long long>(n); offs = c.take<unsigned long long>(n); tmp = c.take<char>(scan_bytes); }
+};
+size_t get_features_bytes(int n) { FeaturesLayout F(n); return layout_bytes([&](Carve& c) { F.layout(c, n); }); }
+int launch_get_features(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float* d_bounds, float min_blur, float max_blur, float4* d_corners, float4* d_surf, float4* d_full, int* d_counts) {
+  ExtractState& e = ctx->ex; const int n = e.n;
   if (n == 0) { LL_CUDA(ctx, cudaMemsetAsync(d_counts, 0, 3 * sizeof(int), s)); return LL_OK; }
-  size_t scan_bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr, n, s);
-  size_t o_p = 0, o_o = align256((size_t)n * 8), o_t = o_o + align256((size_t)n * 8);
-  LL_CUDA(ctx, ctx->scratch.reserve(o_t + scan_bytes + 256));
-  char* base = ctx->scratch.as<char>();
-  unsigned long long* packed = (unsigned long long*)(base + o_p); unsigned long long* offs = (unsigned long long*)(base + o_o);
+  FeaturesLayout F(n);
+  LL_CUDA(ctx, scratch.carve([&](Carve& c) { F.layout(c, n); }));
   const int blocks = ll_div_up(n, 256);
-  ex_flags_kernel<<<blocks, 256, 0, s>>>(n, e.pt_type, e.pt_label, e.depth_sq2, d_bounds, min_blur, max_blur, packed, d_counts);
-  LL_CUDA(ctx, cub::DeviceScan::ExclusiveSum(base + o_t, scan_bytes, packed, offs, n, s));
-  ex_scatter_kernel<<<blocks, 256, 0, s>>>(n, e.raw, e.time_stamp, packed, offs, d_corners, d_surf, d_full, d_counts);
+  ex_flags_kernel<<<blocks, 256, 0, s>>>(n, e.pt_type, e.pt_label, e.depth_sq2, d_bounds, min_blur, max_blur, F.packed, d_counts);
+  LL_CUDA(ctx, cub::DeviceScan::ExclusiveSum(F.tmp, F.scan_bytes, F.packed, F.offs, n, s));
+  ex_scatter_kernel<<<blocks, 256, 0, s>>>(n, e.raw, e.time_stamp, F.packed, F.offs, d_corners, d_surf, d_full, d_counts);
   ctx->launches += 4;
   LL_CUDA(ctx, cudaGetLastError());
   return LL_OK;

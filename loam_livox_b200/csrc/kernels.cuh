@@ -10,8 +10,9 @@ struct TreeView {
   const float* bbox;                    // device: map bounding box (min xyz, max xyz)
 };
 TreeView make_view(const BucketTree& t);
-int build_bucket_tree(ll_ctx* ctx, const float4* d_src, int n_src, BucketTree* t);
-int build_bucket_tree_on(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_src, int n_src, BucketTree* t);
+int build_bucket_tree(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_src, int n_src, BucketTree* t);
+size_t tree_scratch_bytes(int n_src);   // what build_bucket_tree carves from `scratch` and from BucketTree::storage for n_src points
+size_t tree_storage_bytes(int n_src);
 // Bounding box of the finite points (knn.cu): bbox[0..2] = min, bbox[3..5] = max (ll_f2ord encoding), bbox[6] = their count.
 // bbox_init_kernel (one warp) resets it; every bbox_kernel launch after that widens it by one more cloud.
 __global__ void bbox_init_kernel(int* bbox);
@@ -37,7 +38,8 @@ struct KnnBlocksArgs {
 };
 int launch_knn_query(ll_ctx* ctx, const BucketTree& t, const float4* d_q, int nq, int* d_idx, float* d_d);
 int launch_knn_blocks(ll_ctx* ctx, const KnnBlocksArgs& a);
-int launch_query_sort(ll_ctx* ctx, const KnnBlocksArgs& a, int* d_perm);
+int launch_query_sort(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const KnnBlocksArgs& a, int* d_perm);
+size_t query_sort_bytes(int M);
 
 // ---------------------------------------------------------------------------------------------- solver (solve.cu)
 #include "lm_state.h"   // FnSample, LmState (the state machine itself: lm_core.cuh, included by solve.cu)
@@ -59,6 +61,22 @@ struct RegDevState {
   double min_ts, max_ts, interp_theta, interp_hat[9], interp_hat_sq[9];
   long long prof[16];  // [8..12]: fused K10 section: L1 + insert, barrier, select, barrier, drop   // master-CTA cycle counters of the solver: eval, wait, grid reduce, lm_step, publish, #evaluations, staging, epilogue
   LmState lm;
+};
+
+// Pinned host staging of the small transfers, one field per transfer.  The rule every field relies on: a field the host writes before an
+// async copy is not written again until that copy has completed (every entry point synchronises before it returns; register_device reads
+// snap[it & 1] only after the event recorded behind its copy).
+struct PinnedStage {
+  RegDevState state_in;   // the registration state uploaded by register_device / ll_build_blocks / ll_set_blocks
+  RegDevState snap[2];    // state read-backs: ICP iteration `it` into snap[it & 1]; the solver parity hooks use snap[0]
+  double x[7];            // x of the solver parity hooks
+  double pose[7];         // ll_transform / ll_transform_dev
+  double mapper_pose[7];  // the mapper's world-frame transform of the new features
+  double extract_time;    // ExtractState::d_time
+  int fe_counts[12];      // front end: RegArrays::counts ([0..2] get_features, [4..7] VoxelGrid outputs, [10..11] time-stamp range)
+  int fe_meta[3];         // front end: ExtractState::d_meta
+  int counts[3];          // count read-backs of the single-call entry points
+  float bounds[32];       // ll_piece_bounds
 };
 
 // Grid-wide exchange area of the solver kernels (one per context, device memory, zeroed once at creation; see solve.cu):
@@ -116,6 +134,8 @@ int solve_prepare(ll_ctx* ctx);   // once per context: opt the solver kernels in
 int launch_k10_select(ll_ctx* ctx, const double* d_l1, int n, const double* d_ratio, unsigned long long* table, unsigned table_mask, double* d_value, int* d_n_distinct);
 // Slots of the hash set of M L1 norms (K10): a power of two >= 2 M.
 inline unsigned l1_set_capacity(int M) { unsigned cap = 1024; while (cap < (unsigned)(2 * M)) cap <<= 1; return cap; }
+// The hash set's place at the start of a scratch arena.
+inline unsigned long long* l1_set_layout(Carve& c, int M) { return c.take<unsigned long long>(l1_set_capacity(M)); }
 // Sharded mode, K10: every rank pushes the loss-corrected L1 norms of the slots it owns into every peer's X buffer (NVLink stores), then a
 // flag barrier; afterwards X is identical on all ranks (NaN where nobody produced a block).
 int launch_l1_exchange(ll_ctx* ctx, const double* d_l1, int M);
@@ -124,30 +144,23 @@ int launch_count_exchange(ll_ctx* ctx);
 
 // ---------------------------------------------------------------------------------------------- clouds (cloud.cu)
 int upload_cloud(ll_ctx* ctx, const void* src, size_t n, int fmt, int where, float4* d_dst);   // async on ctx->stream
-int launch_transform(ll_ctx* ctx, const double* d_pose7, const float4* d_in, int n, float4* d_out);
-int launch_transform_on(ll_ctx* ctx, cudaStream_t s, const double* d_pose7, const float4* d_in, int n, float4* d_out);
+int launch_transform(ll_ctx* ctx, cudaStream_t s, const double* d_pose7, const float4* d_in, int n, float4* d_out);
 int launch_pack_strided(ll_ctx* ctx, const float4* d_src, int n, unsigned char* d_dst);   // 16-byte points -> PointCloud2 records (ctx->layout)
+int launch_inlier_select(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const double* d_l1, int M, double ratio, double* d_sorted, double* d_unique, int* d_n_unique);
 // VoxelGrid on device: d_in [n] -> d_out [<= n], *d_n_out on device. n given by host, or by device count d_n_in (may be null).
-struct VoxelTemps { DevBuf* buf; };
-int launch_inlier_select(ll_ctx* ctx, const double* d_l1, int M, double ratio, double* d_sorted, double* d_unique, int* d_n_unique);
-int launch_voxel_grid(ll_ctx* ctx, const float4* d_in, int n_cap, const int* d_n_in, float leaf, float4* d_out, int* d_n_out);
-int launch_voxel_grid_on(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_in, int n_cap, const int* d_n_in, float leaf, float4* d_out, int* d_n_out);
+int launch_voxel_grid(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_in, int n_cap, const int* d_n_in, float leaf, float4* d_out, int* d_n_out);
+size_t voxel_grid_bytes(int n_cap);   // what launch_voxel_grid carves from `scratch`
 
 // ---------------------------------------------------------------------------------------------- extractor (extract.cu)
-int extract_reserve(ll_ctx* ctx, int n);
-int launch_extract(ll_ctx* ctx, int n);   // current_time is read from ctx->ex.d_time
-int launch_extract_points(ll_ctx* ctx, int n);
+int extract_alloc(ll_ctx* ctx);   // ExtractState arrays for max_scan_points (ll_ctx_create)
+int launch_extract_points(ll_ctx* ctx, int n);   // current_time is read from ctx->ex.d_time
 int launch_extract_petals(ll_ctx* ctx, int n, cudaStream_t s, DevBuf& scratch);
-int launch_get_features(ll_ctx* ctx, const float* d_bounds /*min_blur,max_blur on device*/, float min_blur, float max_blur,
+int launch_get_features(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float* d_bounds /*min_blur,max_blur on device*/, float min_blur, float max_blur,
                         float4* d_corners, float4* d_surf, float4* d_full, int* d_counts /*3*/);
 int launch_piece_bounds(ll_ctx* ctx, int pieces, float* d_start_end /* 2*pieces */);
+size_t petals_bytes(int n);         // what launch_extract_petals carves from `scratch`
+size_t get_features_bytes(int n);   // what launch_get_features carves from `scratch`
 
 // ---------------------------------------------------------------------------------------------- host driver pieces (api.cu)
-struct RegArrays {
-  float4* feat; float4* blk_a; double* blk_v; double* l1; double* l1_sorted; double* l1_unique;
-  int* n_unique; int* knn_idx; float* knn_d; int* perm; float4* tmp_a; float4* tmp_b; float4* tmp_c; float4* tmp_d; int* counts; float* bounds;
-  int cap;
-};
-int reg_arrays(ll_ctx* ctx, int M, RegArrays* A);
-int register_device(ll_ctx* ctx, const ll_map* map, const RegArrays& A, int nc, int ns, const ll_reg_state* in, ll_reg_result* out);
-int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc, const RegArrays& A, int* nc_out, int* ns_out, int* dropped);
+int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg_state* in, ll_reg_result* out);
+int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);

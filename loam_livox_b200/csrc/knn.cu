@@ -143,59 +143,68 @@ __global__ void bbox_publish_kernel(const int* __restrict__ bbox, float* __restr
   if (threadIdx.x < 6) out6[threadIdx.x] = ll_ord2f(bbox[threadIdx.x]);
 }
 
-// Everything is enqueued on the context's stream and nothing is read back: the layout is sized from n_src (the non-finite points -- there are
+// The index of n_src points: its shape (key width, level sizes), the scratch of its build and its storage.
+struct TreeLayout {
+  int n_src, bits, sort_bits, n_pad, n_levels = 0, level_count[LL_MAX_LEVELS] = {0};
+  bool k32, too_deep = false;
+  size_t temp_bytes = 0, node_total = 0;
+  int* bbox; void* k0; void* k1; int* v0; int* v1; char* tmp;       // scratch
+  float4* pts; float4* nodes; float4* src; float* d_bbox;           // storage
+  explicit TreeLayout(int n) : n_src(n) {
+    // key width: lidar maps are surfaces, so a grid of 2^b cells per axis has ~4^b occupied cells; b = ceil(log2(n) / 2) - 1 keeps the occupied
+    // cells well below a bucket's 32 points (5M points: b = 11, 34 sorted bits = 5 radix passes instead of 8; 30k points: b = 7, 3 passes)
+    int lg = 0; while ((1ll << lg) < (long long)(n_src > 0 ? n_src : 1)) lg++;
+    bits = (lg + 1) / 2 - 1; if (bits < 5) bits = 5; if (bits > 21) bits = 21;
+    sort_bits = 3 * bits + 1;   // one more bit than the key: non-finite points get the key 2^(3 bits) and sort behind every real one
+    k32 = sort_bits <= 32;
+    if (k32) cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, n_src > 0 ? n_src : 1, 0, sort_bits);
+    else cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr, n_src > 0 ? n_src : 1, 0, sort_bits);
+    n_pad = ll_div_up(n_src > 0 ? n_src : 1, BUCKET) * BUCKET;
+    // level sizes: level 0 nodes have buckets as children; the top level has exactly one node
+    int cnt = ll_div_up(n_pad / BUCKET, FANOUT);
+    for (;;) { level_count[n_levels++] = cnt; if (cnt <= 1) break; if (n_levels == LL_MAX_LEVELS) { too_deep = true; break; } cnt = ll_div_up(cnt, FANOUT); }
+    for (int l = 0; l < n_levels; l++) node_total += (size_t)level_count[l];
+  }
+  void scratch_layout(Carve& c) {   // bbox (8 ints) | keys | keys_out | vals | vals_out | CUB temp
+    const size_t ksz = k32 ? 4 : 8;
+    bbox = c.take<int>(16); k0 = c.take<char>(n_src * ksz); k1 = c.take<char>(n_src * ksz); v0 = c.take<int>(n_src); v1 = c.take<int>(n_src); tmp = c.take<char>(temp_bytes);
+  }
+  void storage_layout(Carve& c) {   // points | nodes (top level first) | source copy | box
+    pts = c.take<float4>(n_pad); nodes = c.take<float4>(node_total * NODE_F4); src = c.take<float4>(n_src); d_bbox = c.take<float>(6);
+  }
+};
+size_t tree_scratch_bytes(int n_src) { TreeLayout L(n_src); return layout_bytes([&](Carve& c) { L.scratch_layout(c); }); }
+size_t tree_storage_bytes(int n_src) { TreeLayout L(n_src); return layout_bytes([&](Carve& c) { L.storage_layout(c); }); }
+
+// Enqueued on stream s with its own scratch arena (the corner and the surface index of one map are built side by side: every kernel of a
+// 100k-point build is far too small to fill the GPU).  Nothing is read back: the layout is sized from n_src (the non-finite points -- there are
 // usually none -- only leave a few all-pad buckets with neutral boxes at the end), the count of finite points and the box stay on the device.
-int build_bucket_tree(ll_ctx* ctx, const float4* d_src, int n_src, BucketTree* t) { return build_bucket_tree_on(ctx, ctx->stream, ctx->scratch, d_src, n_src, t); }
-// Same on an explicit stream with its own scratch arena: the corner and the surface index of one map are built side by side (every kernel of a
-// 100k-point build is far too small to fill the GPU).
-int build_bucket_tree_on(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_src, int n_src, BucketTree* t) {
+int build_bucket_tree(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_src, int n_src, BucketTree* t) {
   { DevBuf keep = t->storage; *t = BucketTree(); t->storage = keep; }   // re-indexing in place (ll_map_rebuild) reuses the allocation
   t->n_src = n_src;
-  // key width: lidar maps are surfaces, so a grid of 2^b cells per axis has ~4^b occupied cells; b = ceil(log2(n) / 2) - 1 keeps the occupied
-  // cells well below a bucket's 32 points (5M points: b = 11, 34 sorted bits = 5 radix passes instead of 8; 30k points: b = 7, 3 passes)
-  int lg = 0; while ((1ll << lg) < (long long)(n_src > 0 ? n_src : 1)) lg++;
-  int bits = (lg + 1) / 2 - 1; if (bits < 5) bits = 5; if (bits > 21) bits = 21;
-  const int key_bits = 3 * bits, sort_bits = key_bits + 1;   // one more bit: non-finite points get the key 2^key_bits and sort behind every real one
-  const bool k32 = sort_bits <= 32;
-  const size_t ksz = k32 ? 4 : 8;
-  // scratch: bbox(8 ints) | keys | keys_out | vals | vals_out | cub temp
-  size_t temp_bytes = 0;
-  if (k32) cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, n_src > 0 ? n_src : 1, 0, sort_bits, s);
-  else cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr, n_src > 0 ? n_src : 1, 0, sort_bits, s);
-  size_t off_bbox = 0, off_k0 = align256(64), off_k1 = off_k0 + align256((size_t)n_src * ksz), off_v0 = off_k1 + align256((size_t)n_src * ksz),
-         off_v1 = off_v0 + align256((size_t)n_src * 4), off_tmp = off_v1 + align256((size_t)n_src * 4);
-  LL_CUDA(ctx, scratch.reserve(off_tmp + temp_bytes + 256));
-  char* base = scratch.as<char>();
-  int* bbox = (int*)(base + off_bbox);
-  int* v0 = (int*)(base + off_v0); int* v1 = (int*)(base + off_v1);
-  t->n = n_src; t->n_pad = ll_div_up(n_src > 0 ? n_src : 1, BUCKET) * BUCKET;
-  // level sizes: level 0 nodes have buckets as children; the top level has exactly one node
-  int cnt = ll_div_up(t->n_pad / BUCKET, FANOUT); t->n_levels = 0;
-  for (;;) { t->level_count[t->n_levels++] = cnt; if (cnt <= 1) break; if (t->n_levels == LL_MAX_LEVELS) { ctx->set_error("map too large for LL_MAX_LEVELS"); return LL_ERR_CAPACITY; } cnt = ll_div_up(cnt, FANOUT); }
-  // node storage is laid out top level first
-  size_t node_total = 0; for (int l = 0; l < t->n_levels; l++) node_total += (size_t)t->level_count[l];
-  size_t bytes = align256((size_t)t->n_pad * 16) + align256((size_t)n_src * 16) + align256(node_total * NODE_F4 * 16) + 256;
-  LL_CUDA(ctx, t->storage.reserve(bytes));
-  char* p = t->storage.as<char>();
-  t->pts = (float4*)p; p += align256((size_t)t->n_pad * 16);
-  float4* nodes = (float4*)p; p += align256(node_total * NODE_F4 * 16);
-  { size_t off = 0; for (int l = t->n_levels - 1; l >= 0; l--) { t->lo[l] = nodes + off * NODE_F4; off += (size_t)t->level_count[l]; } }
-  t->src = (float4*)p; p += align256((size_t)n_src * 16);
-  t->d_bbox = (float*)p;
+  TreeLayout L(n_src);
+  if (L.too_deep) { ctx->set_error("map too large for LL_MAX_LEVELS"); return LL_ERR_CAPACITY; }
+  LL_CUDA(ctx, scratch.carve([&](Carve& c) { L.scratch_layout(c); }));
+  LL_CUDA(ctx, t->storage.carve([&](Carve& c) { L.storage_layout(c); }));
+  t->n = n_src; t->n_pad = L.n_pad; t->n_levels = L.n_levels;
+  for (int l = 0; l < L.n_levels; l++) t->level_count[l] = L.level_count[l];
+  { size_t off = 0; for (int l = t->n_levels - 1; l >= 0; l--) { t->lo[l] = L.nodes + off * NODE_F4; off += (size_t)t->level_count[l]; } }
+  t->pts = L.pts; t->src = L.src; t->d_bbox = L.d_bbox;
+  int* bbox = L.bbox; int* v0 = L.v0; int* v1 = L.v1;
   bbox_init_kernel<<<1, 32, 0, s>>>(bbox); ctx->launches++;
   if (n_src > 0) {
     int grid = min(ll_div_up(n_src, 256), ctx->num_sms * 8);
     bbox_kernel<<<grid, 256, 0, s>>>(d_src, n_src, bbox); ctx->launches++;
-    if (k32) {
-      unsigned* k0 = (unsigned*)(base + off_k0); unsigned* k1 = (unsigned*)(base + off_k1);
-      hilbert_kernel<unsigned><<<ll_div_up(n_src, 256), 256, 0, s>>>(d_src, n_src, bbox, bits, k0, v0); ctx->launches++;
-      LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(base + off_tmp, temp_bytes, k0, k1, v0, v1, n_src, 0, sort_bits, s));
+    if (L.k32) {
+      unsigned* k0 = (unsigned*)L.k0; unsigned* k1 = (unsigned*)L.k1;
+      hilbert_kernel<unsigned><<<ll_div_up(n_src, 256), 256, 0, s>>>(d_src, n_src, bbox, L.bits, k0, v0); ctx->launches++;
+      LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(L.tmp, L.temp_bytes, k0, k1, v0, v1, n_src, 0, L.sort_bits, s));
     } else {
-      unsigned long long* k0 = (unsigned long long*)(base + off_k0); unsigned long long* k1 = (unsigned long long*)(base + off_k1);
-      hilbert_kernel<unsigned long long><<<ll_div_up(n_src, 256), 256, 0, s>>>(d_src, n_src, bbox, bits, k0, v0); ctx->launches++;
-      LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(base + off_tmp, temp_bytes, k0, k1, v0, v1, n_src, 0, sort_bits, s));
+      unsigned long long* k0 = (unsigned long long*)L.k0; unsigned long long* k1 = (unsigned long long*)L.k1;
+      hilbert_kernel<unsigned long long><<<ll_div_up(n_src, 256), 256, 0, s>>>(d_src, n_src, bbox, L.bits, k0, v0); ctx->launches++;
+      LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(L.tmp, L.temp_bytes, k0, k1, v0, v1, n_src, 0, L.sort_bits, s));
     }
-    ctx->launches += 3 + (sort_bits + 7) / 8;
+    ctx->launches += 3 + (L.sort_bits + 7) / 8;
     LL_CUDA(ctx, cudaMemcpyAsync(t->src, d_src, (size_t)n_src * 16, cudaMemcpyDeviceToDevice, s));
   }
   bbox_publish_kernel<<<1, 32, 0, s>>>(bbox, t->d_bbox); ctx->launches++;
@@ -454,16 +463,20 @@ int launch_knn_query(ll_ctx* ctx, const BucketTree& t, const float4* d_q, int nq
   return LL_OK;
 }
 // Sorts the features spatially (once per registration, at the initial pose): perm[] lists corner features then surface features.
-int launch_query_sort(ll_ctx* ctx, const KnnBlocksArgs& a, int* d_perm) {
+// keys | keys_out | vals | CUB temp (the sorted values go to perm)
+struct QuerySortLayout {
+  size_t tmp_bytes = 0; unsigned* k0; unsigned* k1; int* v0; char* tmp;
+  explicit QuerySortLayout(int M) { cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, M, 0, 22); }
+  void layout(Carve& c, int M) { k0 = c.take<unsigned>(M); k1 = c.take<unsigned>(M); v0 = c.take<int>(M); tmp = c.take<char>(tmp_bytes); }
+};
+size_t query_sort_bytes(int M) { QuerySortLayout q(M); return layout_bytes([&](Carve& c) { q.layout(c, M); }); }
+int launch_query_sort(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const KnnBlocksArgs& a, int* d_perm) {
   const int M = a.n_corner + a.n_surf;
   if (M == 0) return LL_OK;
-  size_t tmp = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, M, 0, 22, ctx->stream);
-  size_t o_k0 = 0, o_k1 = align256((size_t)M * 4), o_v0 = o_k1 + align256((size_t)M * 4), o_t = o_v0 + align256((size_t)M * 4);
-  LL_CUDA(ctx, ctx->scratch.reserve(o_t + tmp + 256));
-  char* base = ctx->scratch.as<char>();
-  query_key_kernel<<<ll_div_up(M, 256), 256, 0, ctx->stream>>>(a, (unsigned*)(base + o_k0), (int*)(base + o_v0));
-  LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(base + o_t, tmp, (unsigned*)(base + o_k0), (unsigned*)(base + o_k1), (int*)(base + o_v0), d_perm, M, 0, 22, ctx->stream));
+  QuerySortLayout q(M);
+  LL_CUDA(ctx, scratch.carve([&](Carve& c) { q.layout(c, M); }));
+  query_key_kernel<<<ll_div_up(M, 256), 256, 0, s>>>(a, q.k0, q.v0);
+  LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(q.tmp, q.tmp_bytes, q.k0, q.k1, q.v0, d_perm, M, 0, 22, s));
   ctx->launches += 4;
   return LL_OK;
 }

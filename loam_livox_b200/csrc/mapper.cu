@@ -10,6 +10,7 @@
 //   Laser_mapping::init_pointcloud_registration    loam_livox/source/laser_mapping.hpp:1266-1297
 // The reference refreshes the match map on a background thread after every registered scan, with the pose of that scan; here the refresh
 // runs at the start of the next scan (same pose, same map content), so the result is the reference's with maximum_parallel_thread = 1.
+#include <algorithm>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -17,13 +18,6 @@
 #include "common.cuh"
 #include "kernels.cuh"
 
-extern "C" {
-int ll_cellmap_create(ll_ctx*, float, int, int, ll_cellmap**);
-void ll_cellmap_release(ll_cellmap*);
-int ll_cellmap_append(ll_ctx*, ll_cellmap*, const void*, size_t, int, int);
-int ll_cellmap_assemble(ll_ctx*, ll_cellmap*, const double*, const double*, float, float, float, int, ll_point*, size_t, size_t*, int*, const ll_point**);
-int ll_cellmap_reserve(ll_ctx*, ll_cellmap*, size_t, size_t);
-}
 static inline double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
 // m_laser_cloud_{corner,surface}_history (std::list<PointCloud>, :1446-1478) as ONE flat device array: the clouds of the window lie one after the
@@ -68,12 +62,23 @@ struct ll_mapper {
   int frame_index = 0;
   double last_time_stamp = 0;   // m_last_time_stamp (laser_mapping.hpp:140)
   double q_w_curr[4] = {1, 0, 0, 0}, t_w_curr[3] = {0, 0, 0};
-  DevBuf work;   // transformed / down-sampled feature clouds
-  DevBuf snap;   // match-map snapshot clouds (corner, surf) between refreshes
+  DevBuf work;   // transformed / down-sampled feature clouds (work_layout)
+  DevBuf snap;   // match-map snapshot clouds (corner, surf) between refreshes (snap_layout)
   int snap_n[2] = {0, 0}, fov[2] = {0, 0};
   bool have_map = false;
   bool map_dirty = false;   // m_if_mapping_updated_{corner,surface}
   bool trace = false;       // LL_MAPPER_TRACE=1
+};
+
+// snap: the match-map snapshot (the two whole-map VoxelGrid outputs) and their counts
+struct SnapLayout {
+  float4* c; float4* s; int* cnt;
+  void layout(Carve& k, size_t mc, size_t ms) { c = k.take<float4>(mc + 1); s = k.take<float4>(ms + 1); cnt = k.take<int>(2); }
+};
+// work: a scan's features in the world frame (w2 corner, w3 surface), down-sampled (w0, w1), their counts and the pose
+struct WorkLayout {
+  float4* w0; float4* w1; float4* w2; float4* w3; int* cnt; double* pose;
+  void layout(Carve& k, size_t n) { w0 = k.take<float4>(n); w1 = k.take<float4>(n); w2 = k.take<float4>(n); w3 = k.take<float4>(n); cnt = k.take<int>(2); pose = k.take<double>(7); }
 };
 
 // Every buffer whose size follows the map is allocated here, once, for the configured reservation (a reallocation inside a scan call
@@ -81,18 +86,21 @@ struct ll_mapper {
 // scan time of a long stream).  Past the reservation everything still grows by doubling.
 static int mapper_reserve(ll_ctx* ctx, ll_mapper* m) {
   const size_t R = (size_t)(m->cfg.reserve_map_points > 0 ? m->cfg.reserve_map_points : 0), S = (size_t)(m->cfg.reserve_store_points > 0 ? m->cfg.reserve_store_points : 0);
-  const size_t F = (size_t)ctx->cfg.max_features + 16;
-  LL_CUDA(ctx, m->work.reserve_floor(4 * align256(F * 16) + 1024));
+  const int F = ctx->cfg.max_features;
+  WorkLayout w; LL_CUDA(ctx, m->work.reserve_floor(layout_bytes([&](Carve& c) { w.layout(c, F); })));
   if (S) { LL_TRY(ll_cellmap_reserve(ctx, m->cells_corner, S, F)); LL_TRY(ll_cellmap_reserve(ctx, m->cells_surf, S, F)); }
+  // The two map-side arenas, each at the largest of its consumers.  Both: the append's VoxelGrid of a scan's features (corner half on stream2 /
+  // scratch2, surface half on the context's stream / scratch) and the refresh's whole-map VoxelGrid and index build (the halves side by side
+  // the same way).  scratch alone: the registration's query sort and K10 hash set.
+  size_t side = voxel_grid_bytes(F);
+  if (R) side = std::max(side, std::max(voxel_grid_bytes((int)R), tree_scratch_bytes((int)R)));
+  const size_t reg = std::max(query_sort_bytes(F), layout_bytes([&](Carve& c) { l1_set_layout(c, F); }));
+  LL_CUDA(ctx, ctx->scratch.reserve_floor(std::max(side, reg)));
+  LL_CUDA(ctx, ctx->scratch2.reserve_floor(side));
   if (!R) return LL_OK;
   LL_TRY(m->his_corner.reserve(ctx, R)); LL_TRY(m->his_surf.reserve(ctx, R));
-  LL_CUDA(ctx, m->snap.reserve_floor(2 * align256((R + 1) * 16) + 256));
-  LL_CUDA(ctx, ctx->feat_buf.reserve_floor(2 * align256(R * 16) + 512));
-  // index build (build_bucket_tree): 2 key + 2 value arrays and the radix sort's temporaries; whole-map VoxelGrid (launch_voxel_grid_on): the same order
-  LL_CUDA(ctx, ctx->scratch.reserve_floor(64 * R + ((size_t)16 << 20)));
-  LL_CUDA(ctx, ctx->scratch2.reserve_floor(64 * R + ((size_t)16 << 20)));   // the corner chains run on the side stream with this arena
-  // tree storage: padded points + source copy + boxes (1 KB per 32 buckets per level, < 1.04 B per point-byte)
-  for (BucketTree* t : {&m->match_map->corner, &m->match_map->surf}) LL_CUDA(ctx, t->storage.reserve_floor(34 * R + ((size_t)4 << 20)));
+  SnapLayout sn; LL_CUDA(ctx, m->snap.reserve_floor(layout_bytes([&](Carve& c) { sn.layout(c, R, R); })));
+  for (BucketTree* t : {&m->match_map->corner, &m->match_map->surf}) LL_CUDA(ctx, t->storage.reserve_floor(tree_storage_bytes((int)R)));
   return LL_OK;
 }
 
@@ -151,9 +159,9 @@ int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int
   cudaStream_t s = ctx->stream;
   if (stats) memset(stats, 0, sizeof(*stats));
   double tp = now_ms();
-  RegArrays A; LL_TRY(reg_arrays(ctx, 0, &A));
+  const RegArrays& A = ctx->A;
   int nc = 0, ns = 0, dropped = 0;
-  LL_TRY(scan_front_end(ctx, raw, n, fmt, where, stamp, &m->cfg.pipeline, A, &nc, &ns, &dropped));
+  LL_TRY(scan_front_end(ctx, raw, n, fmt, where, stamp, &m->cfg.pipeline, &nc, &ns, &dropped));
   memset(out, 0, sizeof(*out)); out->status = 1;
   for (int k = 0; k < 4; k++) out->q_w_curr[k] = m->q_w_curr[k]; for (int k = 0; k < 3; k++) out->t_w_curr[k] = m->t_w_curr[k];
   if (stats) { stats->n_corner = nc; stats->n_surf = ns; stats->ms_front_end = (float)(now_ms() - tp); }
@@ -176,15 +184,15 @@ int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int
     LL_TRY(ll_cellmap_assemble(ctx, m->cells_surf, m->q_w_curr, m->t_w_curr, m->cfg.maximum_search_range_surface, m->cfg.maximum_in_fov_angle, m->cfg.plane_resolution,
                                m->cfg.down_sample_replace, nullptr, 0, &ms, &fov_s, &d_ms));
     }
-    LL_CUDA(ctx, m->snap.reserve(align256((mc + 1) * 16) + align256((ms + 1) * 16) + 256));
-    float4* s0 = m->snap.as<float4>(); float4* s1 = (float4*)((char*)s0 + align256((mc + 1) * 16)); int* d_sc = (int*)((char*)s1 + align256((ms + 1) * 16));
+    SnapLayout sn; LL_CUDA(ctx, m->snap.carve([&](Carve& c) { sn.layout(c, mc, ms); }));
+    float4* s0 = sn.c; float4* s1 = sn.s; int* d_sc = sn.cnt;
     int hc[2] = {0, 0};
     // the two whole-map VoxelGrids side by side (corner on the side stream with its own scratch)
     cudaStream_t s2 = ctx->stream2;
-    LL_CUDA(ctx, cudaEventRecord(ctx->ev_fork, s)); LL_CUDA(ctx, cudaStreamWaitEvent(s2, ctx->ev_fork, 0));
-    if (mc > 0) LL_TRY(launch_voxel_grid_on(ctx, s2, ctx->scratch2, (const float4*)d_mc, (int)mc, nullptr, m->cfg.line_resolution, s0, d_sc)); else LL_CUDA(ctx, cudaMemsetAsync(d_sc, 0, 4, s2));      // :533-534
-    if (ms > 0) LL_TRY(launch_voxel_grid(ctx, (const float4*)d_ms, (int)ms, nullptr, m->cfg.plane_resolution, s1, d_sc + 1)); else LL_CUDA(ctx, cudaMemsetAsync(d_sc + 1, 0, 4, s));   // :536-537
-    LL_CUDA(ctx, cudaEventRecord(ctx->ev_join, s2)); LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->ev_join, 0));
+    LL_CUDA(ctx, cudaEventRecord(ctx->sev.fork, s)); LL_CUDA(ctx, cudaStreamWaitEvent(s2, ctx->sev.fork, 0));
+    if (mc > 0) LL_TRY(launch_voxel_grid(ctx, s2, ctx->scratch2, (const float4*)d_mc, (int)mc, nullptr, m->cfg.line_resolution, s0, d_sc)); else LL_CUDA(ctx, cudaMemsetAsync(d_sc, 0, 4, s2));      // :533-534
+    if (ms > 0) LL_TRY(launch_voxel_grid(ctx, s, ctx->scratch, (const float4*)d_ms, (int)ms, nullptr, m->cfg.plane_resolution, s1, d_sc + 1)); else LL_CUDA(ctx, cudaMemsetAsync(d_sc + 1, 0, 4, s));   // :536-537
+    LL_CUDA(ctx, cudaEventRecord(ctx->sev.join, s2)); LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->sev.join, 0));
     LL_CUDA(ctx, cudaMemcpyAsync(hc, d_sc, 8, cudaMemcpyDeviceToHost, s));
     LL_CUDA(ctx, cudaStreamSynchronize(s));
     m->have_map = false;
@@ -196,10 +204,8 @@ int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int
     m->map_dirty = false;
   }
   if (stats) { stats->ms_refresh = (float)(now_ms() - tp); stats->map_corner = m->snap_n[0]; stats->map_surf = m->snap_n[1]; stats->cells_in_fov_corner = m->fov[0]; stats->cells_in_fov_surf = m->fov[1]; }
-  const size_t cap = (size_t)(nc > ns ? nc : ns) + 16;
-  LL_CUDA(ctx, m->work.reserve(4 * align256(cap * 16) + 1024));
-  float4* w0 = m->work.as<float4>(); float4* w1 = (float4*)((char*)w0 + align256(cap * 16)); float4* w2 = (float4*)((char*)w1 + align256(cap * 16)); float4* w3 = (float4*)((char*)w2 + align256(cap * 16));
-  int* d_cnt = (int*)((char*)w3 + align256(cap * 16));
+  WorkLayout wl; LL_CUDA(ctx, m->work.carve([&](Carve& c) { wl.layout(c, (size_t)(nc > ns ? nc : ns)); }));
+  float4* w0 = wl.w0; float4* w1 = wl.w1; float4* w2 = wl.w2; float4* w3 = wl.w3; int* d_cnt = wl.cnt;
   int hc[2] = {0, 0};
   // ---- init_pointcloud_registration + find_out_incremental_transfrom (:1266-1297, :1405)
   ll_reg_state st = m->cfg.reg;
@@ -211,20 +217,20 @@ int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int
   st.para_buffer_incremental[0] = st.para_buffer_incremental[1] = st.para_buffer_incremental[2] = 0; st.para_buffer_incremental[3] = 1;
   st.para_buffer_incremental[4] = st.para_buffer_incremental[5] = st.para_buffer_incremental[6] = 0;
   tp = now_ms();
-  if (m->have_map) LL_TRY(register_device(ctx, m->match_map, A, nc, ns, &st, out));
+  if (m->have_map) LL_TRY(register_device(ctx, m->match_map, nc, ns, &st, out));
   if (stats) stats->ms_register = (float)(now_ms() - tp);
   tp = now_ms();   // no map yet: the gate of :199 returns 1
   if (out->status == 0) return LL_OK;                                           // rejected: frame discarded (:1413-1416)
   // ---- new features to the world frame (:1422-1432), VoxelGrid (:1434-1437), cell maps (:1492-1493)
-  double* h = (double*)((char*)ctx->pinned + 40960); for (int k = 0; k < 4; k++) h[k] = out->q_w_curr[k]; for (int k = 0; k < 3; k++) h[4 + k] = out->t_w_curr[k];
-  double* d_pose = (double*)(d_cnt + 16);
+  double* h = ctx->pin->mapper_pose; for (int k = 0; k < 4; k++) h[k] = out->q_w_curr[k]; for (int k = 0; k < 3; k++) h[4 + k] = out->t_w_curr[k];
+  double* d_pose = wl.pose;
   LL_CUDA(ctx, cudaMemcpyAsync(d_pose, h, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
   {
     cudaStream_t s2 = ctx->stream2;
-    LL_CUDA(ctx, cudaEventRecord(ctx->ev_fork, s)); LL_CUDA(ctx, cudaStreamWaitEvent(s2, ctx->ev_fork, 0));
-    if (nc > 0) { LL_TRY(launch_transform_on(ctx, s2, d_pose, A.feat, nc, w2)); LL_TRY(launch_voxel_grid_on(ctx, s2, ctx->scratch2, w2, nc, nullptr, m->cfg.line_resolution, w0, d_cnt)); } else LL_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, 4, s2));
-    if (ns > 0) { LL_TRY(launch_transform(ctx, d_pose, A.feat + nc, ns, w3)); LL_TRY(launch_voxel_grid(ctx, w3, ns, nullptr, m->cfg.plane_resolution, w1, d_cnt + 1)); } else LL_CUDA(ctx, cudaMemsetAsync(d_cnt + 1, 0, 4, s));
-    LL_CUDA(ctx, cudaEventRecord(ctx->ev_join, s2)); LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->ev_join, 0));
+    LL_CUDA(ctx, cudaEventRecord(ctx->sev.fork, s)); LL_CUDA(ctx, cudaStreamWaitEvent(s2, ctx->sev.fork, 0));
+    if (nc > 0) { LL_TRY(launch_transform(ctx, s2, d_pose, A.feat, nc, w2)); LL_TRY(launch_voxel_grid(ctx, s2, ctx->scratch2, w2, nc, nullptr, m->cfg.line_resolution, w0, d_cnt)); } else LL_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, 4, s2));
+    if (ns > 0) { LL_TRY(launch_transform(ctx, s, d_pose, A.feat + nc, ns, w3)); LL_TRY(launch_voxel_grid(ctx, s, ctx->scratch, w3, ns, nullptr, m->cfg.plane_resolution, w1, d_cnt + 1)); } else LL_CUDA(ctx, cudaMemsetAsync(d_cnt + 1, 0, 4, s));
+    LL_CUDA(ctx, cudaEventRecord(ctx->sev.join, s2)); LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->sev.join, 0));
   }
   LL_CUDA(ctx, cudaMemcpyAsync(hc, d_cnt, 8, cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));

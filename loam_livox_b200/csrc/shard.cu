@@ -99,14 +99,13 @@ int ll_map_build_sharded(ll_ctx* ctx, const void* corner, size_t nc, const void*
   size_t sel_bytes = 0;
   cub::DeviceSelect::Flagged(nullptr, sel_bytes, (const float4*)nullptr, (const unsigned char*)nullptr, (float4*)nullptr, (int*)nullptr, (int)(nmax > 0 ? nmax : 1), s);
   // feat_buf: [corner cloud | surface cloud | compacted cloud]; scratch2: bbox, histogram / owner table, keep flags, CUB temp
-  const size_t o_c = 0, o_s = align256(nc * 16), o_k = o_s + align256(ns * 16);
-  LL_CUDA(ctx, ctx->feat_buf.reserve(o_k + align256(nmax * 16) + 256));
-  float4* d_c = (float4*)(ctx->feat_buf.as<char>() + o_c); float4* d_s = (float4*)(ctx->feat_buf.as<char>() + o_s); float4* d_k = (float4*)(ctx->feat_buf.as<char>() + o_k);
+  float4* d_c; float4* d_s; float4* d_k;
+  LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) { d_c = c.take<float4>(nc); d_s = c.take<float4>(ns); d_k = c.take<float4>(nmax); }));
   LL_TRY(upload_cloud(ctx, corner, nc, fmt, where, d_c));
   LL_TRY(upload_cloud(ctx, surf, ns, fmt, where, d_s));
   // ---- grid over the bounding box of the whole map (identical on every rank: every rank sees the same two clouds)
-  LL_CUDA(ctx, ctx->scratch2.reserve(4096));
-  int* d_bbox = ctx->scratch2.as<int>();
+  int* d_bbox = nullptr;
+  LL_CUDA(ctx, ctx->scratch2.carve([&](Carve& c) { d_bbox = c.take<int>(16); }));
   bbox_init_kernel<<<1, 32, 0, s>>>(d_bbox); ctx->launches++;   // (knn.cu; the count of finite points in d_bbox[6] is not used here)
   if (nc) { bbox_kernel<<<std::min(ll_div_up((int)nc, 256), ctx->num_sms * 8), 256, 0, s>>>(d_c, (int)nc, d_bbox); ctx->launches++; }
   if (ns) { bbox_kernel<<<std::min(ll_div_up((int)ns, 256), ctx->num_sms * 8), 256, 0, s>>>(d_s, (int)ns, d_bbox); ctx->launches++; }
@@ -127,10 +126,9 @@ int ll_map_build_sharded(ll_ctx* ctx, const void* corner, size_t nc, const void*
   auto fail = [&](int st, const char* why) { if (why) ctx->set_error(why); m->corner.storage.release(); m->surf.storage.release(); m->shard_owner.release(); delete m; return st; };
   if (ncell > ((size_t)1 << 24)) return fail(LL_ERR_CAPACITY, "shard grid has more than 2^24 cells: raise cell_size");
   // ---- points per cell -> owner table (host, deterministic) -> device
-  const size_t o_hist = 256, o_keep = o_hist + align256(ncell * 4), o_cnt = o_keep + align256(nmax + 1), o_tmp = o_cnt + 256;
-  if (ctx->scratch2.reserve(o_tmp + sel_bytes + 256) != cudaSuccess) return fail(LL_ERR_CUDA, "shard scratch allocation failed");
-  char* sb = ctx->scratch2.as<char>();
-  int* d_hist = (int*)(sb + o_hist); unsigned char* d_keep = (unsigned char*)(sb + o_keep); int* d_cnt = (int*)(sb + o_cnt);
+  int* d_hist; unsigned char* d_keep; int* d_cnt; char* d_tmp;
+  auto layout = [&](Carve& c) { d_bbox = c.take<int>(16); d_hist = c.take<int>(ncell); d_keep = c.take<unsigned char>(nmax + 1); d_cnt = c.take<int>(1); d_tmp = c.take<char>(sel_bytes); };
+  if (ctx->scratch2.carve(layout) != cudaSuccess) return fail(LL_ERR_CUDA, "shard scratch allocation failed");
   cudaMemsetAsync(d_hist, 0, ncell * 4, s);
   if (nc) { sh_hist_kernel<<<ll_div_up((int)nc, 256), 256, 0, s>>>(d_c, (int)nc, g, d_hist); ctx->launches++; }
   if (ns) { sh_hist_kernel<<<ll_div_up((int)ns, 256), 256, 0, s>>>(d_s, (int)ns, g, d_hist); ctx->launches++; }
@@ -148,12 +146,12 @@ int ll_map_build_sharded(ll_ctx* ctx, const void* corner, size_t nc, const void*
     int kept = 0;
     if (ns2[w] > 0) {
       sh_keep_kernel<<<ll_div_up((int)ns2[w], 256), 256, 0, s>>>(srcs[w], (int)ns2[w], g, (const int*)m->shard_owner.p, rank, halos[w], d_keep); ctx->launches++;
-      if (cub::DeviceSelect::Flagged(sb + o_tmp, sel_bytes, srcs[w], d_keep, d_k, d_cnt, (int)ns2[w], s) != cudaSuccess) return fail(LL_ERR_CUDA, "shard compaction failed");
+      if (cub::DeviceSelect::Flagged(d_tmp, sel_bytes, srcs[w], d_keep, d_k, d_cnt, (int)ns2[w], s) != cudaSuccess) return fail(LL_ERR_CUDA, "shard compaction failed");
       ctx->launches += 2;
       if (cudaMemcpyAsync(&kept, d_cnt, 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) return fail(LL_ERR_CUDA, "shard count read-back failed");
     }
     m->shard_total[w] = (long long)ns2[w];
-    const int st = build_bucket_tree(ctx, d_k, kept, trees[w]);
+    const int st = build_bucket_tree(ctx, s, ctx->scratch, d_k, kept, trees[w]);
     if (st != LL_OK) return fail(st, nullptr);
   }
   if (cudaStreamSynchronize(s) != cudaSuccess) return fail(LL_ERR_CUDA, "shard build failed");
