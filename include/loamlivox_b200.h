@@ -190,10 +190,10 @@ int ll_normal_equations(ll_ctx* ctx, const double x[7], double out28[28]);
 /* ... and one ceres::Solve-equivalent on the blocks currently resident (max_iterations as in Solver::Options). */
 int ll_solve(ll_ctx* ctx, int max_iterations, double x_io[7], double* initial_cost, double* final_cost, int* iterations);
 /* ... and compute_inlier_residual_threshold (point_cloud_registration.hpp:153-161) over n caller-given L1 norms (non-negative; n <= max_features).
- * path 0: the grid-wide select of the fused solver kernel; path 1: the sharded mode's l1_unique / l1_select kernels.
+ * The grid-wide select of the fused solver kernel, the same kernel the sharded mode runs between its two solves.
  * +inf and NaN entries are not residuals.  *n_distinct = number of distinct values; *value = element min(floor(ratio n), n-1) of them
  * (0 when there is none). */
-int ll_inlier_select(ll_ctx* ctx, const double* l1, size_t n, double ratio, int path, double* value, int* n_distinct);
+int ll_inlier_select(ll_ctx* ctx, const double* l1, size_t n, double ratio, double* value, int* n_distinct);
 /* ... and caller-given residual blocks in place of ll_build_blocks': n slots (n <= max_features and within the solver's shared memory, else
  * LL_ERR_CAPACITY before anything is enqueued), type 0 invalid / 1 line / 2 plane, the feature p (scan frame; intensity = time stamp, the blur
  * factor of the *_mb functors comes from it as in a registration), the anchor a3 (fp32, as the kNN kernel stores it) and the direction / normal

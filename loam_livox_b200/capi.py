@@ -134,7 +134,7 @@ def lib():
     L.ll_build_blocks.argtypes = [vp, vp, vp, sz, vp, sz, ci, ci, C.POINTER(RegState), vp, vp, vp, C.POINTER(ci), C.POINTER(ci)]
     L.ll_normal_equations.argtypes = [vp, vp, vp]
     L.ll_solve.argtypes = [vp, ci, vp, C.POINTER(cd), C.POINTER(cd), C.POINTER(ci)]
-    L.ll_inlier_select.argtypes = [vp, vp, sz, cd, ci, C.POINTER(cd), C.POINTER(ci)]
+    L.ll_inlier_select.argtypes = [vp, vp, sz, cd, C.POINTER(cd), C.POINTER(ci)]
     L.ll_set_blocks.argtypes = [vp, C.POINTER(RegState), sz, vp, vp, vp, vp]
     L.ll_solve_fused.argtypes = [vp, ci, ci, vp, C.POINTER(cd), C.POINTER(ci), C.POINTER(ci), vp, vp]
     L.ll_transform.argtypes = [vp, vp, vp, vp, sz, ci, ci, vp]

@@ -19,8 +19,8 @@ static int ctx_alloc(ll_ctx* ctx) {
   RegArrays& A = ctx->A;
   LL_CUDA(ctx, ctx->reg_buf.carve([&](Carve& c) {
     A.feat = c.take<float4>(cap); A.blk_a = c.take<float4>(cap); A.blk_v = c.take<double>(cap * 3);
-    A.l1 = c.take<double>(cap); A.l1_sorted = c.take<double>(cap + 8); A.l1_unique = c.take<double>(cap);
-    A.n_unique = c.take<int>(1); A.counts = c.take<int>(16); A.bounds = c.take<float>(32);
+    A.l1 = c.take<double>(cap); A.k10_value = c.take<double>(1);
+    A.k10_n_distinct = c.take<int>(1); A.counts = c.take<int>(16); A.bounds = c.take<float>(32);
     A.knn_idx = c.take<int>(cap * LL_KNN); A.knn_d = c.take<float>(cap * LL_KNN); A.perm = c.take<int>(cap);
     A.tmp_a = c.take<float4>(scap); A.tmp_b = c.take<float4>(scap); A.tmp_c = c.take<float4>(scap); A.tmp_d = c.take<float4>(scap);
   }));
@@ -359,7 +359,7 @@ static KnnBlocksArgs knn_args(ll_ctx* ctx, const ll_map* map, int nc, int ns, co
 }
 static SolveArgs solve_args(ll_ctx* ctx, int M, SolveMode mode, int max_iter) {
   const RegArrays& A = ctx->A;
-  SolveArgs s; s.st = ctx->d_reg; s.sync = ctx->d_sync; s.feat = A.feat; s.blk_a = A.blk_a; s.blk_v = A.blk_v; s.l1 = A.l1; s.l1_sorted_unique = A.l1_unique; s.d_n_unique = A.n_unique;
+  SolveArgs s; s.st = ctx->d_reg; s.sync = ctx->d_sync; s.feat = A.feat; s.blk_a = A.blk_a; s.blk_v = A.blk_v; s.l1 = A.l1; s.k10_value = A.k10_value; s.k10_n_distinct = A.k10_n_distinct;
   s.M = M; s.max_iterations = max_iter; s.mode = mode; s.rank = ctx->rank; s.world = ctx->solve_world; s.comm_local = (double*)ctx->comm_local;
   for (int i = 0; i < 8; i++) s.comm_peer[i] = (double*)ctx->comm_peers[i];
   s.cap_check = 0; s.deblur = ctx->reg_deblur; s.prerun_iterations = 0; s.table = nullptr; s.table_mask = 0;
@@ -429,7 +429,7 @@ int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg
       { SolveArgs sa = solve_args(ctx, M, SOLVE_FIRST, in->cere_prerun_times); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
       if (e) LL_CUDA(ctx, cudaEventRecord(e[2], s));
       LL_TRY(launch_l1_exchange(ctx, A.l1, M));
-      LL_TRY(launch_inlier_select(ctx, s, ctx->scratch, x_l1, M, in->inlier_ratio, A.l1_sorted, A.l1_unique, A.n_unique));
+      LL_TRY(launch_k10_select(ctx, x_l1, M, &ctx->d_reg->inlier_ratio, set_table, l1_set_capacity(M) - 1, A.k10_value, A.k10_n_distinct));
       if (e) LL_CUDA(ctx, cudaEventRecord(e[3], s));
       { SolveArgs sa = solve_args(ctx, M, SOLVE_SECOND, in->cere_max_iterations); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
     }
@@ -626,8 +626,8 @@ int ll_solve_fused(ll_ctx* ctx, int prerun, int max_iterations, double x_io[7], 
   if (iterations) { iterations[1] = hs->lm.iteration; iterations[0] = hs->total_lm_iterations - hs->lm.iteration; }
   return LL_OK;
 }
-int ll_inlier_select(ll_ctx* ctx, const double* l1, size_t n, double ratio, int path, double* value, int* n_distinct) {
-  if (!ctx || (n > 0 && !l1) || !value || !n_distinct || (path != 0 && path != 1) || !(ratio >= 0.0)) return LL_ERR_INVALID;
+int ll_inlier_select(ll_ctx* ctx, const double* l1, size_t n, double ratio, double* value, int* n_distinct) {
+  if (!ctx || (n > 0 && !l1) || !value || !n_distinct || !(ratio >= 0.0)) return LL_ERR_INVALID;
   for (size_t i = 0; i < n; i++) if (l1[i] < 0.0) { ctx->set_error("L1 norms are never negative"); return LL_ERR_INVALID; }
   if (n > (size_t)ctx->cfg.max_features) { ctx->set_error("more values than max_features"); return LL_ERR_CAPACITY; }
   cudaSetDevice(ctx->device);
@@ -635,23 +635,14 @@ int ll_inlier_select(ll_ctx* ctx, const double* l1, size_t n, double ratio, int 
   const RegArrays& A = ctx->A;
   cudaStream_t s = ctx->stream;
   if (M > 0) LL_CUDA(ctx, cudaMemcpyAsync(A.l1, l1, n * sizeof(double), cudaMemcpyHostToDevice, s));
-  LL_CUDA(ctx, cudaMemsetAsync(A.l1_sorted, 0, 64, s));   // [0]: distinct count (path 1)
-  LL_CUDA(ctx, cudaMemsetAsync(A.l1_unique, 0, sizeof(double), s));
-  LL_CUDA(ctx, cudaMemsetAsync(A.n_unique, 0, sizeof(int), s));
-  if (path == 0) {
-    double* d_ratio = &ctx->d_reg->inlier_ratio;   // read on the device as the fused solver reads it (ll_register rewrites the whole state)
-    LL_CUDA(ctx, cudaMemcpyAsync(d_ratio, &ratio, sizeof(double), cudaMemcpyHostToDevice, s));
-    unsigned long long* table = nullptr;
-    LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { table = l1_set_layout(c, M); }));
-    LL_TRY(launch_k10_select(ctx, A.l1, M, d_ratio, table, l1_set_capacity(M) - 1, A.l1_unique, A.n_unique));
-  } else if (M > 0) {   // the sharded mode's kernels: distinct values compacted behind a count in l1_sorted, the order statistic into l1_unique[0]
-    LL_TRY(launch_inlier_select(ctx, s, ctx->scratch, A.l1, M, ratio, A.l1_sorted, A.l1_unique, A.n_unique));
-  }
-  double v = 0.0; int nd = 0;
-  LL_CUDA(ctx, cudaMemcpyAsync(&v, A.l1_unique, sizeof(double), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaMemcpyAsync(&nd, path == 0 ? A.n_unique : (int*)A.l1_sorted, sizeof(int), cudaMemcpyDeviceToHost, s));
+  double* d_ratio = &ctx->d_reg->inlier_ratio;   // read on the device as a registration reads it (ll_register rewrites the whole state)
+  LL_CUDA(ctx, cudaMemcpyAsync(d_ratio, &ratio, sizeof(double), cudaMemcpyHostToDevice, s));
+  unsigned long long* table = nullptr;
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { table = l1_set_layout(c, M); }));
+  LL_TRY(launch_k10_select(ctx, A.l1, M, d_ratio, table, l1_set_capacity(M) - 1, A.k10_value, A.k10_n_distinct));
+  LL_CUDA(ctx, cudaMemcpyAsync(value, A.k10_value, sizeof(double), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(n_distinct, A.k10_n_distinct, sizeof(int), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
-  *value = nd > 0 ? v : 0.0; *n_distinct = nd;
   return LL_OK;
 }
 

@@ -1,17 +1,15 @@
-// Cloud plumbing kernels: format repack, pointAssociateToMap over a cloud, VoxelGrid down-sampling, inlier selection.
+// Cloud plumbing kernels: format repack, pointAssociateToMap over a cloud, VoxelGrid down-sampling.
 //
 // Replaces, on the reference side:
 //   pcl::VoxelGrid<PointXYZI>::filter (third-party PCL, restated)  call sites loam_livox/source/laser_feature_extractor.hpp:372-380,
 //                                   loam_livox/source/laser_mapping.hpp:491,509,533-537,1367-1373,1434-1437                 (K4)
 //   pointcloudAssociateToMap        loam_livox/source/point_cloud_registration.hpp:622-661,673-685                           (K6, cloud form)
-//   compute_inlier_residual_threshold (std::set de-dup + order statistic) loam_livox/source/point_cloud_registration.hpp:153-161,484-485 (K10)
 //
 // Compiled with -fmad=false (voxel indices, centroids and the transform must round like the scalar CPU code).
 #include <cub/cub.cuh>
 #include "common.cuh"
 #include "kernels.cuh"
 #include "exact_math.cuh"
-#include "select.cuh"
 
 #define FULL 0xffffffffu
 
@@ -232,40 +230,6 @@ int launch_voxel_grid(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4
   LL_CUDA(ctx, cub::DeviceSelect::If(v.tmp, v.sel_bytes, cub::CountingInputIterator<int>(0), v.seg, v.d_num_seg, n_cap, VgHead{v.k1}, s));
   vg_centroid_kernel<<<blocks, 256, 0, s>>>(d_in, v.meta, v.v1, v.seg, v.d_num_seg, n_cap, d_out, d_n_out);
   ctx->launches += 11;   // minmax+setup, keys, radix sort (histogram, scan, 4 onesweep passes), select (init, sweep), centroid
-  LL_CUDA(ctx, cudaGetLastError());
-  return LL_OK;
-}
-
-// ------------------------------------------------------------------------------------------------ inlier selection (K10)
-// compute_inlier_residual_threshold (:153-161): std::set<double> of the per-block L1 norms, element floor(ratio * size).
-// De-duplication = one pass through a global-memory hash set (atomicCAS on the 64-bit patterns; duplicates are rare but must
-// not be counted), which also compacts the distinct values; the order statistic = an 8-pass byte-wise radix select by one CTA.
-// Exact, and ~6x cheaper than sort + unique for the few 10^4 blocks of a scan.
-__global__ void l1_unique_kernel(const double* __restrict__ l1, int M, unsigned long long* __restrict__ table, unsigned table_mask, double* __restrict__ uniq, int* __restrict__ n_unique) {
-  __shared__ int s_scratch[34];
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  l1_set_insert(table, table_mask, uniq, n_unique, i < M ? l1[i] : INFINITY, i < M, s_scratch);
-}
-// One CTA: writes out[0] = the order statistic and *n_out = 1 (the solver kernel then picks element floor(ratio * 1) = 0).
-__global__ void __launch_bounds__(1024) l1_select_kernel(const double* __restrict__ uniq, const int* __restrict__ n_unique, double ratio, double* __restrict__ out, int* __restrict__ n_out) {
-  __shared__ SelectSmem S;
-  const int n = *n_unique;
-  if (n <= 0) { if (threadIdx.x == 0) *n_out = 0; return; }
-  const double v = block_select<1024>(uniq, n, ratio, S);
-  if (threadIdx.x == 0) { out[0] = v; *n_out = 1; }
-}
-
-int launch_inlier_select(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const double* d_l1, int M, double ratio, double* d_sorted, double* d_unique, int* d_n_unique) {
-  const unsigned cap = l1_set_capacity(M);
-  unsigned long long* table = nullptr;
-  LL_CUDA(ctx, scratch.carve([&](Carve& c) { table = l1_set_layout(c, M); }));
-  int* n_tmp = (int*)d_sorted;   // d_sorted doubles as [count | compacted distinct values]
-  double* uniq = d_sorted + 2;
-  LL_CUDA(ctx, cudaMemsetAsync(table, 0xff, (size_t)cap * 8, s));
-  LL_CUDA(ctx, cudaMemsetAsync(n_tmp, 0, sizeof(int), s));
-  l1_unique_kernel<<<ll_div_up(M, 256), 256, 0, s>>>(d_l1, M, table, cap - 1, uniq, n_tmp);
-  l1_select_kernel<<<1, 1024, 0, s>>>(uniq, n_tmp, ratio, d_unique, d_n_unique);
-  ctx->launches += 2;
   LL_CUDA(ctx, cudaGetLastError());
   return LL_OK;
 }

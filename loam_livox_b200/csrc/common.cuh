@@ -137,8 +137,8 @@ struct ExtractState {
 
 // Registration arrays (device, one arena sized for max_features / max_scan_points at context creation)
 struct RegArrays {
-  float4* feat; float4* blk_a; double* blk_v; double* l1; double* l1_sorted; double* l1_unique;
-  int* n_unique; int* knn_idx; float* knn_d; int* perm; float4* tmp_a; float4* tmp_b; float4* tmp_c; float4* tmp_d; int* counts; float* bounds;
+  float4* feat; float4* blk_a; double* blk_v; double* l1; double* k10_value;
+  int* k10_n_distinct; int* knn_idx; float* knn_d; int* perm; float4* tmp_a; float4* tmp_b; float4* tmp_c; float4* tmp_d; int* counts; float* bounds;
 };
 
 // Solver / registration device state shared between kernels (lives in global memory)

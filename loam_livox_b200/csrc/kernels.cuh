@@ -105,8 +105,8 @@ struct SolveArgs {
   const float4* blk_a;       // [M] (a.xyz, type)
   const double* blk_v;       // [M*3]
   double* l1;                // [M] loss-corrected L1 norm per slot (+inf for invalid slots)
-  const double* l1_sorted_unique;  // [>= n_unique] for the threshold of solve #2
-  const int* d_n_unique;
+  const double* k10_value;   // SOLVE_SECOND: the K10 order statistic and distinct count (launch_k10_select) for the threshold of solve #2
+  const int* k10_n_distinct;
   int M;
   int max_iterations;
   SolveMode mode;
@@ -130,7 +130,8 @@ int launch_solve(ll_ctx* ctx, const SolveArgs& a);
 // context's error set.  The one copy of the rule launch_solve applies: callers check with it before they enqueue anything.
 int solve_capacity(ll_ctx* ctx, int M, int deblur);
 int solve_prepare(ll_ctx* ctx);   // once per context: opt the solver kernels in to their dynamic shared memory
-// Parity hook: the fused solver's K10 (grid-wide de-duplication + radix select) over n values; *d_value, *d_n_distinct on the device.
+// The fused solver's K10 (grid-wide de-duplication + radix select) over n values, +inf / NaN skipped; *d_value, *d_n_distinct on the device.
+// The sharded mode's select over the exchanged L1 norms, and the parity hook ll_inlier_select.
 int launch_k10_select(ll_ctx* ctx, const double* d_l1, int n, const double* d_ratio, unsigned long long* table, unsigned table_mask, double* d_value, int* d_n_distinct);
 // Slots of the hash set of M L1 norms (K10): a power of two >= 2 M.
 inline unsigned l1_set_capacity(int M) { unsigned cap = 1024; while (cap < (unsigned)(2 * M)) cap <<= 1; return cap; }
@@ -146,7 +147,6 @@ int launch_count_exchange(ll_ctx* ctx);
 int upload_cloud(ll_ctx* ctx, const void* src, size_t n, int fmt, int where, float4* d_dst);   // async on ctx->stream
 int launch_transform(ll_ctx* ctx, cudaStream_t s, const double* d_pose7, const float4* d_in, int n, float4* d_out);
 int launch_pack_strided(ll_ctx* ctx, const float4* d_src, int n, unsigned char* d_dst);   // 16-byte points -> PointCloud2 records (ctx->layout)
-int launch_inlier_select(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const double* d_l1, int M, double ratio, double* d_sorted, double* d_unique, int* d_n_unique);
 // VoxelGrid on device: d_in [n] -> d_out [<= n], *d_n_out on device. n given by host, or by device count d_n_in (may be null).
 int launch_voxel_grid(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_in, int n_cap, const int* d_n_in, float leaf, float4* d_out, int* d_n_out);
 size_t voxel_grid_bytes(int n_cap);   // what launch_voxel_grid carves from `scratch`

@@ -18,7 +18,6 @@
 #include "common.cuh"
 #include "kernels.cuh"
 #include "exact_math.cuh"
-#include "select.cuh"
 
 #define FULL 0xffffffffu
 #define NSUM 29          // 21 JtJ (upper, row-major) + 6 Jtr + cost + valid-block count
@@ -220,9 +219,28 @@ __device__ __forceinline__ void grid_sync(SolveSync* Y, unsigned& gen) {
   sync_wait_all(Y, gen);
 }
 
-// K10 (compute_inlier_residual_threshold, :153-161) spread over the grid.  Used by the fused section of lm_solve_kernel and by k10_select_kernel
-// (the parity hook ll_inlier_select), so that both run the same code.
+// K10 (compute_inlier_residual_threshold, :153-161) spread over the grid: de-duplicate the per-block L1 norms (std::set<double>), take element
+// floor(ratio * size).  Used by the fused section of lm_solve_kernel and by k10_select_kernel (the sharded mode's select between solve #1 and
+// solve #2, and the parity hook ll_inlier_select), so that all of them run the same code.
 #define K10_PASSES 6
+#define L1_EMPTY 0xffffffffffffffffull
+
+// Bit pattern of a non-negative double as an order-preserving key (-0.0 == 0.0 in a std::set).
+__device__ __forceinline__ unsigned long long l1_key(double v) { return (unsigned long long)__double_as_longlong(v == 0.0 ? 0.0 : v); }
+// Insert into the global hash set: true when this call created the entry, i.e. the caller is the (only) representative of a distinct value.
+__device__ __forceinline__ bool l1_set_insert_flag(unsigned long long* __restrict__ table, unsigned table_mask, double v, bool valid) {
+  if (!(valid && v < INFINITY)) return false;   // +inf = invalid slot, NaN never compares
+  const unsigned long long key = l1_key(v);
+  unsigned h = (unsigned)((key * 0x9E3779B97F4A7C15ull) >> 40) & table_mask;
+  for (;;) {
+    const unsigned long long prev = atomicCAS(&table[h], L1_EMPTY, key);
+    if (prev == L1_EMPTY) return true;
+    if (prev == key) return false;
+    h = (h + 1) & table_mask;
+  }
+}
+// The inlier threshold of solve #2 (:484-485): max(inliner_dis, the K10 order statistic), which counts as 0 when there is no distinct value.
+__device__ __forceinline__ double k10_threshold(double inliner_dis, double value, int n_distinct) { return fmax(inliner_dis, n_distinct > 0 ? value : 0.0); }
 struct K10Smem { unsigned hist[2048]; unsigned warp_sum[SOLVE_THREADS / 32 + 1]; unsigned long long prefix, mask; int k, cnt_bin, n_distinct, done; int scratch[40]; double result; };
 
 // Clear the hash set of the L1 norms and the K10 histograms / candidate counter; a grid exchange must follow before any insert.
@@ -340,12 +358,8 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   if (fused) k10_clear(a.table, a.table_mask, Y);
   // ---- stage this CTA's residual blocks
   double thr = 0;
-  if (a.mode == SOLVE_SECOND) {   // K10 tail: threshold = max(inliner_dis, element floor(ratio * n_unique) of the sorted unique L1 norms)
-    int nu = *a.d_n_unique;
-    if (nu > 0 && !isfinite(a.l1_sorted_unique[nu - 1])) nu--;   // the +inf of invalid slots is not a residual
-    int k = (int)(st->inlier_ratio * (double)nu);
-    double rt = nu > 0 ? a.l1_sorted_unique[k < nu ? k : nu - 1] : 0.0;
-    thr = fmax(st->inliner_dis, rt);
+  if (a.mode == SOLVE_SECOND) {   // K10 tail: the threshold from the order statistic and distinct count launch_k10_select left on the device
+    thr = k10_threshold(st->inliner_dis, *a.k10_value, *a.k10_n_distinct);
     if (master && tid == 0) st->inlier_threshold = thr;
   }
   // Residual-block cap, drop rule (:434-458): with M blocks and M > cap, block i leaves the problem when rand_i > (float)cap / (float)M.
@@ -610,7 +624,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
     // ---- K10 over the whole grid (:153-161): the element of rank floor(ratio * n) among the DISTINCT L1 norms (k10_select)
     const long long q0 = clock64();
     k10_select(s_k10, Y, gen, S.type, a.l1, a.M, tiles_per_cta, tile, &st->inlier_ratio);
-    const double thr2 = fmax(st->inliner_dis, s_k10.n_distinct > 0 ? s_k10.result : 0.0);   // :484-485
+    const double thr2 = k10_threshold(st->inliner_dis, s_k10.result, s_k10.n_distinct);
     if (master && tid == 0) { st->inlier_threshold = thr2; st->n_unique = s_k10.n_distinct; }
     const long long q3 = clock64();
     for (int k = 0; k < tiles_per_cta; k++) {                // :487-499: blocks above the threshold leave the problem
@@ -669,8 +683,8 @@ int launch_solve(ll_ctx* ctx, const SolveArgs& a) {
   return LL_OK;
 }
 
-// Parity hook (ll_inlier_select, path 0): the fused kernel's K10 over n caller-given values, spread over the CTAs as lm_solve_kernel spreads M = n
-// slots.  Same generation protocol as the solver: `gen` is read at entry and handed to the next launch at the end.
+// The fused kernel's K10 over n given values (the sharded mode's exchanged L1 norms, or the values of ll_inlier_select), spread over the CTAs as
+// lm_solve_kernel spreads M = n slots.  Same generation protocol as the solver: `gen` is read at entry and handed to the next launch at the end.
 __global__ void __launch_bounds__(SOLVE_THREADS) k10_select_kernel(SolveSync* Y, const double* l1, int n, const double* ratio, unsigned long long* table, unsigned table_mask,
                                                                    int tiles_per_cta, int tile, double* value, int* n_distinct) {
   extern __shared__ int s_flag[];   // [tiles_per_cta * SOLVE_THREADS]: bit 8 = this thread represents its slot's value (lm_solve_kernel: S.type)

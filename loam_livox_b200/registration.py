@@ -278,12 +278,12 @@ class Point_cloud_registration:
         return x, thr.value, nd.value, nk.value, l1, (int(it[0]), int(it[1]))
 
 
-def inlier_select(ctx: Context, l1, ratio: float, path: int):
-    """compute_inlier_residual_threshold (point_cloud_registration.hpp:153-161) over caller-given L1 norms (ll_inlier_select): path 0 = the fused
-    solver kernel's grid-wide select, path 1 = the sharded mode's kernels.  Returns (value, number of distinct values); +inf / NaN are skipped."""
+def inlier_select(ctx: Context, l1, ratio: float):
+    """compute_inlier_residual_threshold (point_cloud_registration.hpp:153-161) over caller-given L1 norms (ll_inlier_select): the fused solver
+    kernel's grid-wide select, as the sharded mode runs it.  Returns (value, number of distinct values); +inf / NaN are skipped."""
     v = np.ascontiguousarray(l1, np.float64)
     out, nd = C.c_double(), C.c_int()
-    ctx.check(ctx._lib.ll_inlier_select(ctx.h, v.ctypes.data, v.shape[0], float(ratio), int(path), C.byref(out), C.byref(nd)))
+    ctx.check(ctx._lib.ll_inlier_select(ctx.h, v.ctypes.data, v.shape[0], float(ratio), C.byref(out), C.byref(nd)))
     return out.value, nd.value
 
 

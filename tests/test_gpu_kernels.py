@@ -1,7 +1,7 @@
 """GPU tests of three hot-path kernels at the edges the end-to-end scenes never reach, each against an exact reference:
 
-- K10, the inlier threshold (compute_inlier_residual_threshold, point_cloud_registration.hpp:153-161), through ll_inlier_select over BOTH of the
-  library's implementations (the fused solver kernel's grid-wide select, and the sharded mode's l1_unique / l1_select kernels), against NumPy;
+- K10, the inlier threshold (compute_inlier_residual_threshold, point_cloud_registration.hpp:153-161), through ll_inlier_select: the fused solver
+  kernel's grid-wide select, as the sharded mode runs it between its two solves, against NumPy;
 - the kNN bucket tree (ll_knn) at the sizes where the tree changes shape and on degenerate geometry, against the oracle's brute force;
 - VoxelGrid (ll_voxel_downsample) at voxel faces, the int32 overflow gate, large voxel populations and the block-size boundaries of its kernels,
   against the oracle and the independent NumPy restatement of tests/test_oracle.py.
@@ -20,9 +20,9 @@ from test_oracle import K10_SIZES, _voxel_numpy, k10_vectors
 pytestmark = pytest.mark.gpu
 
 
-# ---------------------------------------------------------------------------------------------- K10: inlier threshold, both implementations
+# ---------------------------------------------------------------------------------------------- K10: inlier threshold
 @pytest.mark.parametrize("n", K10_SIZES)
-def test_inlier_select_matches_numpy_on_both_paths(ctx, n):
+def test_inlier_select_matches_numpy(ctx, n):
     """Continuous values, all equal, ten values, signed zeros, runs of consecutive doubles that force every radix pass (bins of 64 / 65 values,
     the last pass), runs straddling a digit boundary, subnormals to 1e300, +inf / NaN slots; every ratio also at 1.0 (clamped to the last value)."""
     from loam_livox_b200.registration import inlier_select
@@ -31,26 +31,23 @@ def test_inlier_select_matches_numpy_on_both_paths(ctx, n):
         u = np.unique(v[np.isfinite(v)])
         for ratio in list(ratios) + [1.0]:
             want = u[min(int(ratio * len(u)), len(u) - 1)]
-            for path in (0, 1):
-                got, nd = inlier_select(ctx, v, ratio, path)
-                if not (nd == len(u) and got == want):
-                    bad.append((name, ratio, path, got, want, nd, len(u)))
+            got, nd = inlier_select(ctx, v, ratio)
+            if not (nd == len(u) and got == want):
+                bad.append((name, ratio, got, want, nd, len(u)))
     assert not bad, bad[:8]
 
 
 def test_inlier_select_without_values_and_bad_arguments(ctx):
     from loam_livox_b200.registration import inlier_select
     for v in (np.zeros(0), np.array([np.inf, np.nan, np.inf]), np.full(5000, np.nan)):
-        for path in (0, 1):
-            assert inlier_select(ctx, v, 0.8, path) == (0.0, 0)
+        assert inlier_select(ctx, v, 0.8) == (0.0, 0)
     L, out, nd = capi.lib(), C.c_double(), C.c_int()
     big = np.ones(ctx.cfg.max_features + 1)
-    assert L.ll_inlier_select(ctx.h, big.ctypes.data, big.shape[0], 0.8, 0, C.byref(out), C.byref(nd)) == capi.LL_ERR_CAPACITY
+    assert L.ll_inlier_select(ctx.h, big.ctypes.data, big.shape[0], 0.8, C.byref(out), C.byref(nd)) == capi.LL_ERR_CAPACITY
     ok = np.ones(10)
-    assert L.ll_inlier_select(ctx.h, ok.ctypes.data, 10, 0.8, 2, C.byref(out), C.byref(nd)) == capi.LL_ERR_INVALID
     neg = np.array([1.0, -1.0])
-    assert L.ll_inlier_select(ctx.h, neg.ctypes.data, 2, 0.8, 0, C.byref(out), C.byref(nd)) == capi.LL_ERR_INVALID
-    assert inlier_select(ctx, ok, 0.8, 0) == (1.0, 1)   # the context is still usable
+    assert L.ll_inlier_select(ctx.h, neg.ctypes.data, 2, 0.8, C.byref(out), C.byref(nd)) == capi.LL_ERR_INVALID
+    assert inlier_select(ctx, ok, 0.8) == (1.0, 1)   # the context is still usable
 
 
 def _mk(nc, ns, qc, qs, seed=0):
@@ -85,7 +82,7 @@ def test_inlier_select_keeps_the_solver_generation_protocol(oracle):
     assert _register(c, m, fc, fs, guess) == want
     v = np.random.default_rng(1).uniform(0, 1, 40000)
     for _ in range(3):   # several hook launches: each advances the generation by one exchange per radix pass + 2
-        assert inlier_select(c, v, 0.8, 0)[1] == 40000
+        assert inlier_select(c, v, 0.8)[1] == 40000
     assert _register(c, m, fc, fs, guess) == want
     m.release()
     c.close()
