@@ -180,6 +180,19 @@ __device__ __forceinline__ void fast_accumulate(const FastSlot& s, const EvalCon
   }
 }
 
+// One level of the CTA reduce's transposing butterfly: lanes that differ in bit OFF swap halves of w[0 .. 2 OFF) and add, so that w[0 .. OFF) holds
+// pairwise sums (after the five levels, lane L holds the warp's total of sum L).
+template <int OFF>
+__device__ __forceinline__ void butterfly_level(double (&w)[32], int lane) {
+  const bool upper = (lane & OFF) != 0;
+#pragma unroll
+  for (int i = 0; i < OFF; i++) {
+    const double send = upper ? w[i] : w[i + OFF];          // the half this lane gives away
+    const double keep = upper ? w[i + OFF] : w[i];
+    w[i] = keep + __shfl_xor_sync(FULL, send, OFF);
+  }
+}
+
 struct SmemSlots { float* p[3]; float* a[3]; double* v[3]; double* ap[3]; int* type; float* s; };
 // MB (general path): v = line direction / plane normal (world), a = anchor (world, fp32-exact), s = blur factor      -> 56 B / slot
 // !MB (fast path):   v = R_last^T v, ap = R_last^T (a - t_last): the evaluation never touches the last pose again   -> 64 B / slot
@@ -203,8 +216,10 @@ __device__ __forceinline__ SmemSlots carve(unsigned char* base, int cap, bool mb
 // no publish step.  Rows are double-buffered by generation parity: a CTA can be at most one exchange ahead of the slowest one.  Generations grow
 // monotonically over the life of the context (SolveSync::gen is never reset), so a stale tag can never match.
 __device__ __forceinline__ double* sync_row(SolveSync* Y, unsigned gen, int cta) { return Y->rows[gen & 1u][cta]; }
-__device__ __forceinline__ void sync_arrive(SolveSync* Y, unsigned gen) {   // called by one thread after the CTA's row (if any) is written and fenced
-  __threadfence();
+// Called by one thread after a warp or CTA barrier that follows the writes it publishes (the CTA's row, K10's histogram atomics).  The release is
+// cumulative: it orders every write the barrier made this thread observe, so no separate fence is needed (a __threadfence here is a sequentially
+// consistent fence on the path of every exchange).
+__device__ __forceinline__ void sync_arrive(SolveSync* Y, unsigned gen) {
   st_release_u32((unsigned*)(sync_row(Y, gen, blockIdx.x) + 31), gen);
 }
 __device__ __forceinline__ void sync_wait_all(SolveSync* Y, unsigned gen) {   // CTA-collective
@@ -340,6 +355,8 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   __shared__ double s_gmax;
   __shared__ StepOut s_pre[2]; // the next iteration's ComputeStep under both outcomes of the accept test, evaluated by warp 1 while warp 0 decides
   __shared__ K10Smem s_k10;    // SOLVE_FUSED only
+  __shared__ long long s_prof[16];   // the master CTA's cycle counters, added to RegDevState::prof once at the end: a global read-modify-write per
+                                     // evaluation would put an L2 round trip on the master's path, and every other CTA waits for the master's row
   RegDevState* st = a.st;
   SolveSync* Y = a.sync;
   if ((a.mode == SOLVE_FUSED || a.mode <= SOLVE_SECOND) && *((volatile int*)&st->icp_done)) return;   // ICP work (fused, solve #1 or #2) launched after the ICP loop ended (uniform over the grid)
@@ -348,6 +365,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   const SmemSlots S = carve(s_dyn, cap, MB);
   const bool master = blockIdx.x == 0;   // the CTA that writes results back to RegDevState and talks to the peers (nothing waits for it otherwise)
   unsigned gen = *((volatile unsigned*)&Y->gen);   // uniform over the grid: written by the previous launch's CTA 0 at its very end
+  if (tid < 16) s_prof[tid] = 0;
 
   const long long t_k0 = clock64();
   // SOLVE_FUSED = one whole ICP iteration's solver work in ONE launch: solve #1 (prerun iterations) -> L1 norms -> std::set de-duplication + order
@@ -410,7 +428,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   }
   __syncthreads();
 
-  if (master && tid == 0 && ph == 0) st->prof[6] += clock64() - t_k0;
+  if (master && tid == 0 && ph == 0) s_prof[6] += clock64() - t_k0;
   for (;;) {
     const long long t_e0 = clock64();
     // ---- evaluate: r, J, Huber, 29 partial sums per thread
@@ -451,16 +469,9 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
       double w[32];
 #pragma unroll
       for (int i = 0; i < 32; i++) w[i] = i < NSUM ? acc[i] : 0.0;
-#pragma unroll
-      for (int off = 16; off >= 1; off >>= 1) {
-        const bool upper = (lane & off) != 0;
-#pragma unroll
-        for (int i = 0; i < off; i++) {
-          const double send = upper ? w[i] : w[i + off];          // the half this lane gives away
-          const double keep = upper ? w[i + off] : w[i];
-          w[i] = keep + __shfl_xor_sync(FULL, send, off);
-        }
-      }
+      // one call per level with a constant width, so that every index is a constant and w stays in registers (a loop over the widths left
+      // w in local memory: a dependent local load and store per shuffle)
+      butterfly_level<16>(w, lane); butterfly_level<8>(w, lane); butterfly_level<4>(w, lane); butterfly_level<2>(w, lane); butterfly_level<1>(w, lane);
       if (lane < NSUM) s_red[warp][lane] = w[0];
     } else if (lane < NSUM) s_red[warp][lane] = 0.0;
     __syncthreads();
@@ -475,21 +486,29 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
     sync_wait_all(Y, gen);
     const long long t_e2 = clock64();
     {
-      const int val = tid & 31, grp = tid >> 5;   // (SOLVE_THREADS / 32) groups x 32 values
-      double v = 0;
-      if (val < NSUM) {   // rows grp, grp + 8, ...: four loads in flight, four partial sums combined in a fixed order
-        constexpr int G = SOLVE_THREADS / 32;
-        double v0 = 0, v1 = 0, v2 = 0, v3 = 0; int b = grp; const int nb = (int)gridDim.x;
-        for (; b + 3 * G < nb; b += 4 * G) {
-          const double a0 = __ldcg(&sync_row(Y, gen, b)[val]), a1 = __ldcg(&sync_row(Y, gen, b + G)[val]), a2 = __ldcg(&sync_row(Y, gen, b + 2 * G)[val]), a3 = __ldcg(&sync_row(Y, gen, b + 3 * G)[val]);
-          v0 += a0; v1 += a1; v2 += a2; v3 += a3;
-        }
-        for (; b < nb; b += G) v0 += __ldcg(&sync_row(Y, gen, b)[val]);
-        v = (v0 + v1) + (v2 + v3);
-        s_red[grp][val] = v;
+      // Thread (grp, val) sums value `val` of rows grp, grp + G, grp + 2G, ...: every row load is issued before the first add (one L2 round trip,
+      // not one per four rows).  The sum is the fixed-order one every CTA computes: four chains over rows j = 0, 1, 2, 3 (mod 4) while a whole
+      // group of four is left, the remaining rows into the first chain, (v0 + v1) + (v2 + v3), then the G group sums in order.
+      // (Each thread acquiring the tags of its own rows instead of the poll + barrier above was measured slower: back-to-back acquires do not
+      // overlap, each waits for the one before.)
+      constexpr int G = SOLVE_THREADS / 32, RMAX = (LL_SYNC_ROWS + G - 1) / G;
+      static_assert(RMAX % 4 == 0, "the row loop below runs whole groups of four");
+      const int val = tid & 31, grp = tid >> 5, nb = (int)gridDim.x;
+      const int n = grp < nb ? (nb - grp + G - 1) / G : 0;   // rows of this group
+      if (val < NSUM) {
+        double r[RMAX];
+#pragma unroll
+        for (int j = 0; j < RMAX; j++) r[j] = j < n ? __ldcg(&sync_row(Y, gen, grp + j * G)[val]) : 0.0;
+        double v0 = 0, v1 = 0, v2 = 0, v3 = 0;
+        const int whole = n & ~3;
+#pragma unroll
+        for (int j = 0; j < RMAX; j += 4) if (j < whole) { v0 += r[j]; v1 += r[j + 1]; v2 += r[j + 2]; v3 += r[j + 3]; }
+#pragma unroll
+        for (int j = 0; j < RMAX; j++) if (j >= whole && j < n) v0 += r[j];
+        s_red[grp][val] = (v0 + v1) + (v2 + v3);
       }
       __syncthreads();
-      if (tid < NSUM) { double t = 0; for (int g = 0; g < SOLVE_THREADS / 32; g++) t += s_red[g][tid]; s_sum[tid] = t; }
+      if (tid < NSUM) { double t = 0; for (int g = 0; g < G; g++) t += s_red[g][tid]; s_sum[tid] = t; }
       __syncthreads();
     }
     if (a.world > 1) {
@@ -530,21 +549,21 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
       if (tid == 64) { for (int k = 0; k < 7; k++) gx[k] = s_lm.trial[k]; for (int c = 0; c < 6; c++) gg[c] = -s_sum[21 + c]; }
       __syncthreads();
       const long long t_h0 = clock64();
-      if (warp == 1 && lane < 2) { compute_step(in, bound, s_pre[lane]); if (master && lane == 0) st->prof[13] += clock64() - t_h0; }   // Cholesky + model cost + Plus: the long pole of an LM step ...
-      else if (tid == 0) { lm_step(s_lm, s_sum, bound, true); if (master) st->prof[14] += clock64() - t_h0; }   // ... next to the accept test and the bookkeeping ...
+      if (warp == 1 && lane < 2) { compute_step(in, bound, s_pre[lane]); if (master && lane == 0) s_prof[13] += clock64() - t_h0; }   // Cholesky + model cost + Plus: the long pole of an LM step ...
+      else if (tid == 0) { lm_step(s_lm, s_sum, bound, true); if (master) s_prof[14] += clock64() - t_h0; }   // ... next to the accept test and the bookkeeping ...
       else if (tid == 64) {   // ... and the gradient test of the accepted point (max |x - Plus(x, -g)|), which only the NEXT iteration's entry check reads
         double pg[7]; d_plus(gx, gg, bound, pg); double mx = 0; for (int k = 0; k < 7; k++) mx = fmax(mx, fabs(gx[k] - pg[k])); s_gmax = mx;
       }
       __syncthreads();
       if (tid == 0 && s_lm.pending == 0) s_lm.last_gmax = s_gmax;   // pending == 0 <=> the point just evaluated became x
-      if (master && tid == 0) st->prof[15] += clock64() - t_h0;
+      if (master && tid == 0) s_prof[15] += clock64() - t_h0;
       if (tid == 0 && s_lm.pending >= 0) lm_next_iteration(s_lm, bound, &s_pre[s_lm.pending]);
     }
     // (volatile: the plain test was if-converted into a load of `done` by EVERY thread, which racecheck reports against thread 0's write in lm_finish --
     // harmless, only thread 0 ever used the value, but there is no reason to keep a flagged access)
     if (tid == 0) { if (!*(volatile int*)&s_lm.done) setup_trial<MB>(E, s_lm.trial); }
     __syncthreads();
-    if (master && tid == 0) { const long long t_e4 = clock64(); st->prof[0] += t_e1 - t_e0; st->prof[1] += t_e2 - t_e1; st->prof[2] += t_e3 - t_e2; st->prof[3] += t_e4 - t_e3; st->prof[5] += 1; }
+    if (master && tid == 0) { const long long t_e4 = clock64(); s_prof[0] += t_e1 - t_e0; s_prof[1] += t_e2 - t_e1; s_prof[2] += t_e3 - t_e2; s_prof[3] += t_e4 - t_e3; s_prof[5] += 1; }
     if (s_lm.done) break;
   }
   // ---- the solve has ended (on every CTA, with the same state)
@@ -633,12 +652,15 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
     }
     cur_mode = SOLVE_SECOND;
     __syncthreads();
-    if (master && tid == 0) { const long long q4 = clock64(); st->prof[8] += q0 - t_p0; st->prof[10] += q3 - q0; st->prof[12] += q4 - q3; }
+    if (master && tid == 0) { const long long q4 = clock64(); s_prof[8] += q0 - t_p0; s_prof[10] += q3 - q0; s_prof[12] += q4 - q3; }
   }
-  if (master && tid == 0) st->prof[7] += clock64() - t_p0;
+  if (master && tid == 0) s_prof[7] += clock64() - t_p0;
   }   // phase
   // hand the generation base to the next launch (stream-ordered): every CTA ended with the same `gen`
-  if (master && tid == 0) *((volatile unsigned*)&Y->gen) = gen;
+  if (master && tid == 0) {
+    *((volatile unsigned*)&Y->gen) = gen;
+    for (int k = 0; k < 16; k++) st->prof[k] += s_prof[k];
+  }
 }
 
 #define SOLVE_MAX_SMEM (200 * 1024)   // up to ~405k slots on 132 SMs; a typical scan (<= 113 KB of slots per CTA) leaves room for a second CTA per SM (another context's solver)
