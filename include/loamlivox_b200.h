@@ -95,6 +95,11 @@ int ll_extract_petal_angles(ll_ctx* ctx, float* out, int cap, int* n_out);
 /* Replaces pcl::VoxelGrid<PointXYZI>::filter at laser_feature_extractor.hpp:372-380 and
  * laser_mapping.hpp:491,509,533-537,1367-1373,1434-1437.  `out` must hold n points. */
 int ll_voxel_downsample(ll_ctx* ctx, const void* in, size_t n, int fmt, int where, float leaf, ll_point* out, size_t* n_out);
+/* The same over n_seg (1 ... 256) disjoint contiguous segments of one host cloud, in one device pass: segment k is [seg_end[k - 1], seg_end[k])
+ * (seg_end ascending, <= n; points past the last end belong to no segment).  Each segment is filtered exactly as ll_voxel_downsample filters it
+ * alone (own bounds, grid and int32-overflow pass-through; equal voxels of two segments never merge).  out receives the segments' outputs one
+ * after another (at most n points), n_out_per_seg[k] their counts.  What the streaming mapper's piecewise front end runs (ll_mapper_process_frame). */
+int ll_voxel_downsample_segments(ll_ctx* ctx, const ll_point* in, size_t n, const size_t* seg_end, int n_seg, float leaf, ll_point* out, size_t* n_out_per_seg);
 
 /* ---- S2: map snapshot + index ---------------------------------------------------------------------- */
 /* Replaces pcl::KdTreeFLANN::setInputCloud x2 in Laser_mapping::update_buff_for_matching
@@ -303,6 +308,20 @@ void ll_mapper_release(ll_mapper* mapper);
 /* One raw scan through process_new_scan (laser_mapping.hpp:1316-1521): features, match-map refresh from the cell maps, registration
  * (out->status 1 accepted/skipped, 0 rejected and discarded), world-frame features appended to the cell maps, pose adopted. */
 int  ll_mapper_process_scan(ll_mapper* mapper, const void* raw, size_t n, int fmt, int where, double stamp, ll_reg_result* out, ll_mapper_stats* stats);
+/* One sensor frame through Laser_feature::laserCloudHandler and, for every piece it publishes, Laser_mapping::process_new_scan
+ * (laser_feature_extractor.hpp:305-389, laser_mapping.hpp:1316-1521): what the shipped configs run (common/odom_mode 1, if_motion_deblur 0).
+ * n_heads (1 ... 8) raw clouds (Mid-100: 3), one extractor over the heads in turn as ll_frame_to_pose; a head with <= 5 petals contributes
+ * nothing, and when no head contributes nothing is published (*n_pieces = 0, the mapper untouched).  The frame is cut into
+ * pieces = reg.if_motion_deblur ? 1 : pipeline.pieces (1 ... 16) pieces of consecutive petals (pipeline.whole_frame and use_piece are not
+ * read); piece i's features are the piece-i clouds of the contributing heads in head order, down-sampled by the extractor's and the mapping
+ * node's VoxelGrids.  odom_mode 1 registers every piece as a scan of its own (frame index, time-stamp range, map refresh, append and pose
+ * adoption per piece), 0 only piece 0.  out / stats (stats may be NULL) receive one entry per published piece; cap is their length.
+ * LL_ERR_INVALID (nothing changed) for odom_mode outside {0, 1}, pieces outside 1 ... 16 or cap below the pieces to publish;
+ * LL_ERR_CAPACITY up front when the heads exceed max_scan_points, and before piece i's registration when its features exceed max_features
+ * (*n_pieces then counts the pieces completed, whose entries are valid). */
+#define LL_MAX_PIECES_PER_FRAME 16
+int  ll_mapper_process_frame(ll_mapper* mapper, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+                             int odom_mode, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces);
 int  ll_mapper_pose(const ll_mapper* mapper, double q_wxyz[4], double t[3], int* frame_index);
 
 /* ---- wire formats (SURVEY 8(f) N3) ---------------------------------------------------------------------------------------------- */

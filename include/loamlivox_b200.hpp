@@ -206,6 +206,20 @@ class Laser_mapping {
     if (result) *result = r; if (stats) *stats = st;
     return r.status;
   }
+  // one sensor frame (one raw cloud per head; Mid-100: 3) cut into pieces, each piece registered as a scan (odom_mode 1, the shipped configs;
+  // 0: piece 0 only).  One entry per published piece in results / stats (empty when no head has more than 5 petals).
+  void process_new_frame(const std::vector<PointCloud>& heads, const std::vector<double>& time_stamps, int odom_mode = 1,
+                         std::vector<ll_reg_result>* results = nullptr, std::vector<ll_mapper_stats>* stats = nullptr) {
+    if (heads.size() != time_stamps.size()) throw Error(LL_ERR_INVALID, "one time stamp per head");
+    std::vector<const void*> raws; std::vector<size_t> ns;
+    for (const PointCloud& h : heads) { raws.push_back(h.data()); ns.push_back(h.size()); }
+    std::vector<ll_reg_result> r(LL_MAX_PIECES_PER_FRAME); std::vector<ll_mapper_stats> st(LL_MAX_PIECES_PER_FRAME); int n = 0;
+    ctx_.check(ll_mapper_process_frame(mapper_, (int)heads.size(), raws.data(), ns.data(), LL_FMT_PCL32, LL_HOST, time_stamps.data(), odom_mode,
+                                       r.data(), st.data(), (int)r.size(), &n));
+    ctx_.check(ll_mapper_pose(mapper_, m_q_w_curr.data(), m_t_w_curr.data(), &m_current_frame_index));
+    r.resize(n); st.resize(n);
+    if (results) *results = r; if (stats) *stats = st;
+  }
   std::array<double, 4> m_q_w_curr{{1, 0, 0, 0}};   // (w, x, y, z)
   std::array<double, 3> m_t_w_curr{{0, 0, 0}};
   int m_current_frame_index = 0;

@@ -18,6 +18,7 @@ LL_I_NONE, LL_I_UINT8, LL_I_UINT16, LL_I_FLOAT32 = 0, 2, 4, 7   # sensor_msgs/Po
 LL_HOST, LL_DEVICE = 0, 1
 LL_OK, LL_ERR_INVALID, LL_ERR_CUDA, LL_ERR_CAPACITY, LL_ERR_NO_BLOCKS, LL_ERR_CAP_BINDS = 0, -1, -2, -3, -4, -5
 LL_IPC_HANDLE_BYTES = 64
+LL_MAX_PIECES_PER_FRAME = 16
 
 EXPORTS = [
     "ll_config_default", "ll_ctx_create", "ll_ctx_destroy", "ll_ctx_warmup", "ll_last_error", "ll_ctx_stream", "ll_ctx_sync", "ll_extract", "ll_extract_reset", "ll_piece_bounds",
@@ -26,6 +27,7 @@ EXPORTS = [
     "ll_scan_to_pose", "ll_comm_local_handle", "ll_comm_connect", "ll_launch_count", "ll_cellmap_create", "ll_cellmap_release", "ll_cellmap_append",
     "ll_cellmap_assemble", "ll_cellmap_reserve", "ll_cellmap_stats", "ll_voxel_downsample_dev", "ll_transform_dev", "ll_last_features_dev", "ll_mapper_config_default", "ll_mapper_create", "ll_mapper_release",
     "ll_mapper_process_scan", "ll_mapper_pose", "ll_map_rebuild", "ll_debug_solver_cycles", "ll_state_snapshot_bytes", "ll_set_point_layout", "ll_format_pose_log", "ll_reg_state_yaml", "ll_cap_uniform", "ll_map_shard_info", "ll_shard_plan", "ll_align_cfg_default", "ll_scene_align", "ll_frame_to_pose", "ll_features_to_pointcloud2",
+    "ll_mapper_process_frame", "ll_voxel_downsample_segments",
 ]
 
 
@@ -117,6 +119,7 @@ def lib():
     L.ll_extract_split_idx.argtypes = [vp, vp, ci, C.POINTER(ci)]
     L.ll_extract_petal_angles.argtypes = [vp, vp, ci, C.POINTER(ci)]
     L.ll_voxel_downsample.argtypes = [vp, vp, sz, ci, ci, cf, vp, C.POINTER(sz)]
+    L.ll_voxel_downsample_segments.argtypes = [vp, vp, sz, vp, ci, cf, vp, vp]
     L.ll_map_build.argtypes = [vp, vp, sz, vp, sz, ci, ci, C.POINTER(vp)]
     L.ll_map_build_sharded.argtypes = [vp, vp, sz, vp, sz, ci, ci, ci, ci, cf, cf, cf, C.POINTER(vp)]
     L.ll_map_shard_info.argtypes = [vp, C.POINTER(ShardInfo), vp, sz]
@@ -163,6 +166,7 @@ def lib():
     L.ll_mapper_create.argtypes = [vp, C.POINTER(MapperConfig), C.POINTER(vp)]
     L.ll_mapper_release.argtypes = [vp]
     L.ll_mapper_process_scan.argtypes = [vp, vp, sz, ci, ci, cd, C.POINTER(RegResult), C.POINTER(MapperStats)]
+    L.ll_mapper_process_frame.argtypes = [vp, ci, vp, vp, ci, ci, vp, ci, C.POINTER(RegResult), C.POINTER(MapperStats), ci, C.POINTER(ci)]
     L.ll_mapper_pose.argtypes = [vp, vp, vp, C.POINTER(ci)]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64

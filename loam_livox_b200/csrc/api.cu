@@ -105,8 +105,9 @@ int ll_ctx_sync(ll_ctx* ctx) { cudaSetDevice(ctx->device); LL_CUDA(ctx, cudaStre
 uint64_t ll_launch_count(const ll_ctx* ctx) { return ctx->launches; }
 
 // ---------------------------------------------------------------------------------------------- S1
-// Host half of extract_laser_features: time-stamp bookkeeping (:724-736), upload, scan time to the device.
-static int extract_prepare(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp) {
+// Host half of extract_laser_features: time-stamp bookkeeping (:724-736), upload, scan time to the device (staged through `pin_time`, by
+// default the single extract_time slot).
+static int extract_prepare(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp, double* pin_time = nullptr) {
   if ((int)n > ctx->cfg.max_scan_points) { ctx->set_error("scan larger than max_scan_points"); return LL_ERR_CAPACITY; }
   ExtractState& e = ctx->ex;
   if (stamp <= 0.0000001 || (stamp < e.last_maximum_time_stamp)) e.current_time = e.last_maximum_time_stamp; else e.current_time = stamp - e.first_receive_time;
@@ -114,8 +115,9 @@ static int extract_prepare(ll_ctx* ctx, const void* raw, size_t n, int fmt, int 
   e.n = (int)n;
   if (n > 0) e.last_maximum_time_stamp = (double)(float)(e.current_time + (double)(((float)(n - 1)) * ctx->cfg.time_interval_pts));
   LL_TRY(upload_cloud(ctx, raw, n, fmt, where, e.raw));
-  ctx->pin->extract_time = e.current_time;
-  LL_CUDA(ctx, cudaMemcpyAsync(e.d_time, &ctx->pin->extract_time, sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  if (!pin_time) pin_time = &ctx->pin->extract_time;
+  *pin_time = e.current_time;
+  LL_CUDA(ctx, cudaMemcpyAsync(e.d_time, pin_time, sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
   return LL_OK;
 }
 // The extraction on the context's stream; the petal bookkeeping's temporaries in `scratch`.
@@ -228,6 +230,23 @@ int ll_voxel_downsample(ll_ctx* ctx, const void* in, size_t n, int fmt, int wher
   LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   *n_out = (size_t)h[0];
   if (out && h[0] > 0) { LL_CUDA(ctx, cudaMemcpyAsync(out, d_out, (size_t)h[0] * 16, cudaMemcpyDeviceToHost, ctx->stream)); LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); }
+  return LL_OK;
+}
+int ll_voxel_downsample_segments(ll_ctx* ctx, const ll_point* in, size_t n, const size_t* seg_end, int n_seg, float leaf, ll_point* out, size_t* n_out_per_seg) {
+  if (!ctx || !seg_end || !n_out_per_seg || (!in && n) || n_seg < 1 || n_seg > 256 || !(leaf > 0.f) || n >= (size_t)1 << 31) return LL_ERR_INVALID;
+  for (int k = 0; k < n_seg; k++) if (seg_end[k] > n || (k && seg_end[k] < seg_end[k - 1])) { ctx->set_error("segment ends must ascend and stay within n"); return LL_ERR_INVALID; }
+  cudaSetDevice(ctx->device);
+  cudaStream_t s = ctx->stream;
+  float4* d_in = nullptr; float4* d_out = nullptr; int* d_end; int* d_oend;
+  LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) { d_in = c.take<float4>(n); d_out = c.take<float4>(n); d_end = c.take<int>(n_seg); d_oend = c.take<int>(n_seg); }));
+  std::vector<int> h(n_seg); for (int k = 0; k < n_seg; k++) h[k] = (int)seg_end[k];
+  LL_CUDA(ctx, cudaMemcpyAsync(d_end, h.data(), n_seg * sizeof(int), cudaMemcpyHostToDevice, s));
+  LL_TRY(upload_cloud(ctx, in, n, LL_FMT_XYZI16, LL_HOST, d_in));
+  LL_TRY(launch_voxel_grid_segments(ctx, s, ctx->scratch, d_in, (int)n, d_end, n_seg, leaf, d_out, d_oend));
+  LL_CUDA(ctx, cudaMemcpyAsync(h.data(), d_oend, n_seg * sizeof(int), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  for (int k = 0; k < n_seg; k++) n_out_per_seg[k] = (size_t)(h[k] - (k ? h[k - 1] : 0));
+  if (out && h[n_seg - 1] > 0) { LL_CUDA(ctx, cudaMemcpyAsync(out, d_out, (size_t)h[n_seg - 1] * 16, cudaMemcpyDeviceToHost, s)); LL_CUDA(ctx, cudaStreamSynchronize(s)); }
   return LL_OK;
 }
 int ll_transform(ll_ctx* ctx, const double q[4], const double t[3], const void* in, size_t n, int fmt, int where, ll_point* out) {
@@ -841,6 +860,39 @@ extern "C" int ll_frame_to_pose(ll_ctx* ctx, const ll_map* map, int n_heads, con
   LL_CUDA(ctx, cudaMemcpyAsync(A.feat, A.tmp_a, (size_t)nc * 16, cudaMemcpyDeviceToDevice, s));
   LL_CUDA(ctx, cudaMemcpyAsync(A.feat + nc, A.tmp_b, (size_t)nsf * 16, cudaMemcpyDeviceToDevice, s));
   return register_device(ctx, map, nc, nsf, in, out);
+}
+
+// Laser_feature::laserCloudHandler for a whole frame, every piece at once (laser_feature_extractor.hpp:303-389): each head extracted once and
+// compacted once with bounds 0 ... 1 (its corner / surface / full clouds at the head's base in tmp_a / tmp_b / tmp_c), the slices of every
+// piece read from that compaction, piece i's slices of all heads gathered into segment i, then the extractor's and the mapping node's
+// VoxelGrids as one segmented pass each: the corner chain on stream2, the surface chain on the context's stream.  The launch count does not
+// depend on the number of pieces.
+int frame_front_end(ll_ctx* ctx, const FrameArena& fa, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+                    int pieces, const ll_pipeline_cfg* pc) {
+  cudaStream_t s = ctx->stream, s2 = ctx->stream2;
+  const RegArrays& A = ctx->A;
+  FrameBases B; int base = 0, max_n = 0;
+  for (int h = 0; h < n_heads; h++) {
+    B.base[h] = base;
+    LL_TRY(extract_prepare(ctx, raws[h], ns[h], fmt, where, stamps[h], &ctx->pin->head_time[h]));
+    LL_TRY(extract_enqueue(ctx, ctx->fe_main));
+    LL_TRY(launch_piece_bounds(ctx, pieces, A.bounds));
+    LL_TRY(launch_get_features(ctx, s, ctx->fe_main, nullptr, 0.f, 1.f, A.tmp_a + base, A.tmp_b + base, A.tmp_c + base, A.counts));
+    LL_TRY(launch_piece_slices(ctx, s, ctx->fe_main, A.bounds, pieces, A.tmp_c + base, &fa.dev->head[h]));
+    base += (int)ns[h]; max_n = std::max(max_n, (int)ns[h]);
+  }
+  LL_TRY(launch_gather_pieces(ctx, s, fa.dev, B, n_heads, pieces, max_n, A.tmp_a, A.tmp_b, fa.cls[0], fa.cls[1]));
+  const int cap = pieces * base;   // a piece holds at most every point of the frame once
+  LL_CUDA(ctx, cudaEventRecord(ctx->sev.fork, s));
+  LL_CUDA(ctx, cudaStreamWaitEvent(s2, ctx->sev.fork, 0));
+  LL_TRY(launch_voxel_grid_segments(ctx, s2, *fa.vg[1], fa.cls[0], cap, fa.dev->seg_end[0], pieces, pc->extractor_leaf_corner, fa.mid[0], fa.dev->mid_end[0]));
+  LL_TRY(launch_voxel_grid_segments(ctx, s2, *fa.vg[1], fa.mid[0], cap, fa.dev->mid_end[0], pieces, pc->mapping_leaf_corner, fa.cls[0], fa.dev->out.out_end[0]));
+  LL_CUDA(ctx, cudaEventRecord(ctx->sev.join, s2));
+  LL_TRY(launch_voxel_grid_segments(ctx, s, *fa.vg[0], fa.cls[1], cap, fa.dev->seg_end[1], pieces, pc->extractor_leaf_surf, fa.mid[1], fa.dev->mid_end[1]));
+  LL_TRY(launch_voxel_grid_segments(ctx, s, *fa.vg[0], fa.mid[1], cap, fa.dev->mid_end[1], pieces, pc->mapping_leaf_surf, fa.cls[1], fa.dev->out.out_end[1]));
+  LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->sev.join, 0));
+  LL_CUDA(ctx, cudaMemcpyAsync(&ctx->pin->frame, &fa.dev->out, sizeof(FrameOut), cudaMemcpyDeviceToHost, s));
+  return LL_OK;
 }
 
 extern "C" {

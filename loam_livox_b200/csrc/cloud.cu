@@ -102,25 +102,44 @@ int launch_transform(ll_ctx* ctx, cudaStream_t s, const double* d_pose7, const f
 }
 
 // ------------------------------------------------------------------------------------------------ VoxelGrid
+// One pass filters nseg disjoint contiguous segments of the input, each exactly as a VoxelGrid of that segment alone: segment s is
+// [end[s - 1], end[s]) (end[-1] = 0; every end clamped to n_cap; end == null: one segment of n_cap points).  Each segment gets its own bounds,
+// grid and int32-overflow decision; the segment id sits above the 32 voxel-key bits of the sort key, so equal voxels of two segments never
+// merge and, the radix sort being stable, every voxel still sums its points in ascending input order.  The outputs follow one another:
+// segment s's voxels are out[out_end[s - 1], out_end[s]).  One segment sorts 32-bit keys, as a single-cloud VoxelGrid always did.
 struct VgMeta {
   int mn[3], mx[3];     // ordered-int encodings of the float min / max
   int n_finite;
   int passthrough;      // dx*dy*dz overflows int32: PCL warns and copies the input through
-  int n_in;
+  int n_in, begin;      // the segment's input range
   int min_b[3]; int mul[3];
   float inv;
-  int ticket;           // blocks of vg_minmax_setup_kernel that have finished (the last one does the set-up and resets it)
+  int ticket;           // blocks of the segment's row of vg_minmax_setup_kernel that have finished (the last one does the set-up and resets it)
 };
+struct VgSegs {
+  const int* end; int nseg, n_cap;
+  __device__ __forceinline__ int end_of(int s) const { return end ? min(end[s], n_cap) : n_cap; }
+  __device__ __forceinline__ int begin_of(int s) const { return s ? min(end_of(s - 1), end_of(s)) : 0; }
+  __device__ __forceinline__ int find(int i) const {   // segment holding input index i (nseg: past the last segment)
+    if (nseg == 1) return i < end_of(0) ? 0 : 1;
+    int lo = 0, hi = nseg;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (i < end_of(mid)) hi = mid; else lo = mid + 1; }
+    return lo;
+  }
+};
+template <typename K> __device__ __forceinline__ unsigned vg_low(K k) { return (unsigned)(k & 0xffffffffu); }
+template <typename K> __device__ __forceinline__ int vg_seg(K k) { return sizeof(K) == 4 ? 0 : (int)((unsigned long long)k >> 32); }
 
-// Min / max over the finite points, then -- by the last block to finish -- the grid set-up of VoxelGrid::applyFilter (one launch instead of
-// init + minmax + setup; `m` is cleared by a memset node: mins are kept as the bitwise complement of their order-preserving key, so that
-// "all zero" is the neutral element of the atomicMax that reduces both the mins and the maxs).
+// Min / max over the finite points of segment blockIdx.y, then -- by the last block of that segment to finish -- the grid set-up of
+// VoxelGrid::applyFilter (one launch instead of init + minmax + setup; `m` is cleared by a memset node: mins are kept as the bitwise complement
+// of their order-preserving key, so that "all zero" is the neutral element of the atomicMax that reduces both the mins and the maxs).
 __device__ __forceinline__ unsigned f2key(float f) { return (unsigned)ll_f2ord(f) ^ 0x80000000u; }     // unsigned order == float order
 __device__ __forceinline__ float key2f(unsigned k) { return ll_ord2f((int)(k ^ 0x80000000u)); }
-__global__ void vg_minmax_setup_kernel(const float4* __restrict__ in, VgMeta* m, int n_host, const int* __restrict__ d_n, float leaf) {
-  const int n = d_n ? min(*d_n, n_host) : n_host;
+__global__ void vg_minmax_setup_kernel(const float4* __restrict__ in, VgMeta* metas, VgSegs g, float leaf) {
+  VgMeta* m = metas + blockIdx.y;
+  const int b = g.begin_of(blockIdx.y), n = g.end_of(blockIdx.y);
   float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY}; int cnt = 0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+  for (int i = b + blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     float4 p = in[i];
     if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) {
       lo[0] = fminf(lo[0], p.x); lo[1] = fminf(lo[1], p.y); lo[2] = fminf(lo[2], p.z);
@@ -147,7 +166,7 @@ __global__ void vg_minmax_setup_kernel(const float4* __restrict__ in, VgMeta* m,
   __threadfence();
   // ---- set-up (the last block sees every block's contribution)
   volatile VgMeta* v = m;
-  m->n_in = n; m->passthrough = 0; m->ticket = 0;
+  m->n_in = n - b; m->begin = b; m->passthrough = 0; m->ticket = 0;
   const float inv = 1.0f / leaf; m->inv = inv;
   if (v->n_finite == 0) { for (int k = 0; k < 3; k++) { m->min_b[k] = 0; m->mul[k] = 0; } return; }
   float mn[3], mx[3]; for (int k = 0; k < 3; k++) { mn[k] = key2f(~(unsigned)v->mn[k]); mx[k] = key2f((unsigned)v->mx[k]); }
@@ -157,13 +176,20 @@ __global__ void vg_minmax_setup_kernel(const float4* __restrict__ in, VgMeta* m,
   for (int k = 0; k < 3; k++) { m->min_b[k] = (int)floorf(mn[k] * inv); int max_b = (int)floorf(mx[k] * inv); div_b[k] = max_b - m->min_b[k] + 1; }
   m->mul[0] = 1; m->mul[1] = div_b[0]; m->mul[2] = div_b[0] * div_b[1];
 }
-__global__ void vg_keys_kernel(const float4* __restrict__ in, const VgMeta* __restrict__ m, int n_cap, unsigned* __restrict__ keys, int* __restrict__ vals) {
+// Sort key of input index i: the segment id above the 32 voxel-key bits (K = 32-bit: one segment).  Non-finite points take the low word
+// 0xffffffff (the end of their segment), points past the last segment the largest key.  A pass-through segment keys every point by its
+// position, so that each one is a voxel of its own and the centroid kernel copies it.
+template <typename K>
+__global__ void vg_keys_kernel(const float4* __restrict__ in, const VgMeta* __restrict__ metas, VgSegs g, K* __restrict__ keys, int* __restrict__ vals) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_cap) return;
+  if (i >= g.n_cap) return;
+  const int s = g.find(i);
   unsigned key = 0xffffffffu;
-  if (i < m->n_in) {
+  if (s < g.nseg) {
+    const VgMeta* m = metas + s;
     float4 p = in[i];
-    if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) {
+    if (m->passthrough) key = (unsigned)(i - m->begin);
+    else if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) {
       const float inv = m->inv;
       int ijk0 = (int)(floorf(p.x * inv) - (float)m->min_b[0]);
       int ijk1 = (int)(floorf(p.y * inv) - (float)m->min_b[1]);
@@ -171,65 +197,87 @@ __global__ void vg_keys_kernel(const float4* __restrict__ in, const VgMeta* __re
       key = (unsigned)(ijk0 * m->mul[0] + ijk1 * m->mul[1] + ijk2 * m->mul[2]);
     }
   }
-  keys[i] = key; vals[i] = i;
+  keys[i] = sizeof(K) == 4 ? (K)key : (K)(((unsigned long long)s << 32) | key);
+  vals[i] = i;
 }
 // First element of every run of equal (valid) keys in the sorted key array: the predicate of the stream compaction that lists the voxels.
-struct VgHead {
-  const unsigned* keys;
-  __device__ __forceinline__ bool operator()(int i) const { const unsigned k = keys[i]; return k != 0xffffffffu && (i == 0 || keys[i - 1] != k); }
+template <typename K> struct VgHead {
+  const K* keys;
+  __device__ __forceinline__ bool operator()(int i) const { const K k = keys[i]; return vg_low(k) != 0xffffffffu && (i == 0 || keys[i - 1] != k); }
 };
-// One thread per voxel: sequential float sum in ascending input index (radix sort is stable), like CentroidPoint<PointXYZI>.
-__global__ void vg_centroid_kernel(const float4* __restrict__ in, const VgMeta* __restrict__ m, const int* __restrict__ vals, const int* __restrict__ seg_start,
-                                   const int* __restrict__ d_num_seg, int n_cap, float4* __restrict__ out, int* __restrict__ d_n_out) {
-  int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m->passthrough) {
-    if (s < m->n_in) out[s] = in[s];
-    if (s == 0) *d_n_out = m->n_in;
-    return;
+// One thread per voxel: sequential float sum in ascending input index (radix sort is stable), like CentroidPoint<PointXYZI>.  Voxel v of the
+// whole pass is output v; out_end[s] = the voxels of segments 0..s (one thread per segment of block 0 finds it by bisection).
+template <typename K>
+__global__ void vg_centroid_kernel(const float4* __restrict__ in, const VgMeta* __restrict__ metas, int nseg, const K* __restrict__ keys, const int* __restrict__ vals,
+                                   const int* __restrict__ heads, const int* __restrict__ d_num_heads, float4* __restrict__ out, int* __restrict__ out_end) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  const int nh = *d_num_heads;
+  if (blockIdx.x == 0 && threadIdx.x < nseg) {
+    int e = nh;
+    if (sizeof(K) == 8) {   // first voxel of a later segment
+      int lo = 0, hi = nh;
+      while (lo < hi) { const int mid = (lo + hi) >> 1; if (vg_seg(keys[heads[mid]]) > (int)threadIdx.x) hi = mid; else lo = mid + 1; }
+      e = lo;
+    }
+    out_end[threadIdx.x] = e;
   }
-  const int nseg = *d_num_seg;
-  if (s == 0) *d_n_out = nseg;
-  if (s >= nseg) return;
-  const int b = seg_start[s], e = (s + 1 < nseg) ? seg_start[s + 1] : m->n_finite;
+  if (v >= nh) return;
+  const int b = heads[v];
+  const VgMeta* m = metas + vg_seg(keys[b]);
+  if (m->passthrough) { out[v] = in[vals[b]]; return; }
+  const int e = min(v + 1 < nh ? heads[v + 1] : 0x7fffffff, m->begin + m->n_finite);
   float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
   for (int li = b; li < e; li++) { const float4 p = in[vals[li]]; sx += p.x; sy += p.y; sz += p.z; si += p.w; }
   const float cnt = (float)(e - b);
-  out[s] = make_float4(sx / cnt, sy / cnt, sz / cnt, si / cnt);
+  out[v] = make_float4(sx / cnt, sy / cnt, sz / cnt, si / cnt);
 }
 
-// The scratch of one VoxelGrid over n_cap points (n_cap > 0).
-struct VgScratch {
+static int vg_sort_bits(int nseg) { int b = 32; if (nseg > 1) for (int v = nseg; v > 0; v >>= 1) b++; return b; }   // segment ids 0..nseg
+// The scratch of one VoxelGrid pass over n_cap points (n_cap > 0) in nseg segments.
+template <typename K> struct VgScratch {
   size_t sort_bytes = 0, sel_bytes = 0;
-  VgMeta* meta; int* d_num_seg; unsigned* k0; unsigned* k1; int* v0; int* v1; int* seg; char* tmp;
-  explicit VgScratch(int n_cap) {
-    cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, n_cap, 0, 32);
-    cub::DeviceSelect::If(nullptr, sel_bytes, cub::CountingInputIterator<int>(0), (int*)nullptr, (int*)nullptr, n_cap, VgHead{nullptr});
+  VgMeta* meta; int* d_num_heads; K* k0; K* k1; int* v0; int* v1; int* heads; char* tmp;
+  VgScratch(int n_cap, int nseg) {
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (K*)nullptr, (K*)nullptr, (int*)nullptr, (int*)nullptr, n_cap, 0, vg_sort_bits(nseg));
+    cub::DeviceSelect::If(nullptr, sel_bytes, cub::CountingInputIterator<int>(0), (int*)nullptr, (int*)nullptr, n_cap, VgHead<K>{nullptr});
   }
-  void layout(Carve& c, int n_cap) {
-    meta = c.take<VgMeta>(1); d_num_seg = c.take<int>(1);
-    k0 = c.take<unsigned>(n_cap); k1 = c.take<unsigned>(n_cap); v0 = c.take<int>(n_cap); v1 = c.take<int>(n_cap); seg = c.take<int>(n_cap);
+  void layout(Carve& c, int n_cap, int nseg) {
+    meta = c.take<VgMeta>(nseg); d_num_heads = c.take<int>(1);
+    k0 = c.take<K>(n_cap); k1 = c.take<K>(n_cap); v0 = c.take<int>(n_cap); v1 = c.take<int>(n_cap); heads = c.take<int>(n_cap);
     tmp = c.take<char>(sort_bytes > sel_bytes ? sort_bytes : sel_bytes);
   }
 };
-size_t voxel_grid_bytes(int n_cap) {
+size_t voxel_grid_bytes(int n_cap, int nseg) {
   if (n_cap <= 0) return 0;
-  VgScratch v(n_cap);
-  return layout_bytes([&](Carve& c) { v.layout(c, n_cap); });
+  if (nseg > 1) { VgScratch<unsigned long long> v(n_cap, nseg); return layout_bytes([&](Carve& c) { v.layout(c, n_cap, nseg); }); }
+  VgScratch<unsigned> v(n_cap, 1);
+  return layout_bytes([&](Carve& c) { v.layout(c, n_cap, 1); });
+}
+template <typename K>
+static int voxel_grid_pass(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_in, int n_cap, const int* d_end, int nseg, float leaf, float4* d_out, int* d_out_end) {
+  VgScratch<K> v(n_cap, nseg);
+  LL_CUDA(ctx, scratch.carve([&](Carve& c) { v.layout(c, n_cap, nseg); }));
+  const int blocks = ll_div_up(n_cap, 256);
+  const VgSegs g{d_end, nseg, n_cap};
+  LL_CUDA(ctx, cudaMemsetAsync(v.meta, 0, nseg * sizeof(VgMeta), s));
+  vg_minmax_setup_kernel<<<dim3(min(blocks, ctx->num_sms * 2), nseg), 256, 0, s>>>(d_in, v.meta, g, leaf);
+  vg_keys_kernel<K><<<blocks, 256, 0, s>>>(d_in, v.meta, g, v.k0, v.v0);
+  LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(v.tmp, v.sort_bytes, v.k0, v.k1, v.v0, v.v1, n_cap, 0, vg_sort_bits(nseg), s));
+  LL_CUDA(ctx, cub::DeviceSelect::If(v.tmp, v.sel_bytes, cub::CountingInputIterator<int>(0), v.heads, v.d_num_heads, n_cap, VgHead<K>{v.k1}, s));
+  vg_centroid_kernel<K><<<blocks, 256, 0, s>>>(d_in, v.meta, nseg, v.k1, v.v1, v.heads, v.d_num_heads, d_out, d_out_end);
+  // minmax+setup, keys, radix sort (histogram, scan, one onesweep pass per 8 key bits), select (init, sweep), centroid
+  ctx->launches += 7 + (uint64_t)(vg_sort_bits(nseg) + 7) / 8;
+  LL_CUDA(ctx, cudaGetLastError());
+  return LL_OK;
 }
 // On an explicit stream with its own scratch arena: VoxelGrid chains run side by side (every kernel here is far too small to fill the GPU,
 // so the chains overlap almost perfectly).
+int launch_voxel_grid_segments(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_in, int n_cap, const int* d_end, int nseg, float leaf, float4* d_out, int* d_out_end) {
+  if (nseg < 1) return LL_OK;
+  if (n_cap <= 0) { LL_CUDA(ctx, cudaMemsetAsync(d_out_end, 0, nseg * sizeof(int), s)); return LL_OK; }
+  if (nseg == 1) return voxel_grid_pass<unsigned>(ctx, s, scratch, d_in, n_cap, d_end, 1, leaf, d_out, d_out_end);
+  return voxel_grid_pass<unsigned long long>(ctx, s, scratch, d_in, n_cap, d_end, nseg, leaf, d_out, d_out_end);
+}
 int launch_voxel_grid(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_in, int n_cap, const int* d_n_in, float leaf, float4* d_out, int* d_n_out) {
-  if (n_cap <= 0) { LL_CUDA(ctx, cudaMemsetAsync(d_n_out, 0, sizeof(int), s)); return LL_OK; }
-  VgScratch v(n_cap);
-  LL_CUDA(ctx, scratch.carve([&](Carve& c) { v.layout(c, n_cap); }));
-  const int blocks = ll_div_up(n_cap, 256);
-  LL_CUDA(ctx, cudaMemsetAsync(v.meta, 0, sizeof(VgMeta), s));
-  vg_minmax_setup_kernel<<<min(blocks, ctx->num_sms * 2), 256, 0, s>>>(d_in, v.meta, n_cap, d_n_in, leaf);
-  vg_keys_kernel<<<blocks, 256, 0, s>>>(d_in, v.meta, n_cap, v.k0, v.v0);
-  LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(v.tmp, v.sort_bytes, v.k0, v.k1, v.v0, v.v1, n_cap, 0, 32, s));
-  LL_CUDA(ctx, cub::DeviceSelect::If(v.tmp, v.sel_bytes, cub::CountingInputIterator<int>(0), v.seg, v.d_num_seg, n_cap, VgHead{v.k1}, s));
-  vg_centroid_kernel<<<blocks, 256, 0, s>>>(d_in, v.meta, v.v1, v.seg, v.d_num_seg, n_cap, d_out, d_n_out);
-  ctx->launches += 11;   // minmax+setup, keys, radix sort (histogram, scan, 4 onesweep passes), select (init, sweep), centroid
-  LL_CUDA(ctx, cudaGetLastError());
-  return LL_OK;
+  return launch_voxel_grid_segments(ctx, s, scratch, d_in, n_cap, d_n_in, 1, leaf, d_out, d_n_out);
 }

@@ -11,6 +11,7 @@
 // sequential dependences - "copy the previous point's projection for a zero return" and the 50-point split hysteresis -
 // are a short walk-back per zero return and a single-thread pass over the few direction-flip candidates).
 // Compiled with -fmad=false: all float arithmetic must round like the scalar CPU code.
+#include <algorithm>
 #include <cub/cub.cuh>
 #include "common.cuh"
 #include "kernels.cuh"
@@ -240,6 +241,69 @@ __global__ void ex_scatter_kernel(int n, const float4* __restrict__ raw, const f
   if (i == n - 1) { const unsigned long long t = o + f; counts[0] = (int)(t & 0x1fffff); counts[1] = (int)((t >> 21) & 0x1fffff); counts[2] = (int)((t >> 42) & 0x1fffff); }
 }
 
+// Piece blockIdx.x of one head: the first / last index that ex_flags_kernel's range test keeps for the piece's bounds (same float expressions,
+// evaluated on both sides of the closed-form guess), the class slices between the prefix sums there, and the largest time stamp of the full
+// slice.  A head with <= 5 petals gets empty slices.
+__device__ __forceinline__ unsigned long long prefix_at(const unsigned long long* offs, const unsigned long long* packed, int i, bool past) {
+  return past ? offs[i] + packed[i] : offs[i];
+}
+__global__ void ex_piece_slices_kernel(int n, const float* __restrict__ d_bounds, const int* __restrict__ meta, const unsigned long long* __restrict__ packed,
+                                       const unsigned long long* __restrict__ offs, const float4* __restrict__ full, FrameSlices* __restrict__ out) {
+  const int i = blockIdx.x;
+  __shared__ int s_off, s_len, s_max;
+  if (threadIdx.x == 0) {
+    const bool live = n > 0 && meta[1] > 5;
+    if (i == 0) out->live = live ? 1 : 0;
+    int lo = 0, hi = -1;
+    if (live) {
+      const float minimum_idx = d_bounds[2 * i] * (float)n, maximum_idx = d_bounds[2 * i + 1] * (float)n;
+      lo = (int)fminf(fmaxf(ceilf(minimum_idx), 0.f), (float)n);
+      while (lo > 0 && !((float)(lo - 1) < minimum_idx)) lo--;
+      while (lo < n && (float)lo < minimum_idx) lo++;
+      hi = (int)fminf(fmaxf(floorf(maximum_idx), -1.f), (float)(n - 1));
+      while (hi < n - 1 && !((float)(hi + 1) > maximum_idx)) hi++;
+      while (hi >= 0 && (float)hi > maximum_idx) hi--;
+    }
+    unsigned long long a = 0, b = 0;
+    if (lo <= hi) { a = prefix_at(offs, packed, lo, false); b = prefix_at(offs, packed, hi, true); }
+    for (int k = 0; k < 3; k++) {
+      const int o = (int)((a >> (21 * k)) & 0x1fffff), e = (int)((b >> (21 * k)) & 0x1fffff);
+      out->off[k][i] = lo <= hi ? o : 0; out->len[k][i] = lo <= hi ? e - o : 0;
+    }
+    s_off = out->off[2][i]; s_len = out->len[2][i]; s_max = ll_f2ord(-10000.0f);
+  }
+  __syncthreads();
+  int mx = (int)0x80000000;
+  for (int k = threadIdx.x; k < s_len; k += blockDim.x) mx = max(mx, ll_f2ord(full[s_off + k].w));
+  mx = __reduce_max_sync(0xffffffffu, mx);
+  if ((threadIdx.x & 31) == 0) atomicMax(&s_max, mx);
+  __syncthreads();
+  if (threadIdx.x == 0) out->tmax[i] = s_max;
+}
+
+// grid (chunks, pieces x heads, 2 classes): the slice of head h for piece i goes to segment i after the slices of heads 0 .. h-1.  Block
+// (0, 0, 0) also writes the segment ends, the per-piece time-stamp maxima and the number of live heads.
+__global__ void ex_gather_pieces_kernel(const FrameSlices* __restrict__ sl, FrameBases B, int n_heads, int pieces, const float4* __restrict__ src_c,
+                                        const float4* __restrict__ src_s, float4* __restrict__ dst_c, float4* __restrict__ dst_s, int* __restrict__ seg_end,
+                                        FrameOut* __restrict__ fo) {
+  const int cls = blockIdx.z, pair = blockIdx.y, i = pair / n_heads, h = pair % n_heads;
+  int dst = 0;
+  for (int p = 0; p < pair; p++) dst += sl[p % n_heads].len[cls][p / n_heads];
+  const int len = sl[h].len[cls][i];
+  const float4* src = (cls ? src_s : src_c) + B.base[h] + sl[h].off[cls][i];
+  float4* d = (cls ? dst_s : dst_c) + dst;
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < len; k += gridDim.x * blockDim.x) d[k] = src[k];
+  if (blockIdx.x != 0 || pair != 0 || cls != 0) return;
+  const int t = threadIdx.x;
+  if (t < pieces) {
+    int ec = 0, es = 0, mx = ll_f2ord(-10000.0f);
+    for (int p = 0; p <= t; p++) for (int hh = 0; hh < n_heads; hh++) { ec += sl[hh].len[0][p]; es += sl[hh].len[1][p]; }
+    for (int hh = 0; hh < n_heads; hh++) mx = max(mx, sl[hh].tmax[t]);
+    seg_end[t] = ec; seg_end[LL_MAX_PIECES + t] = es; fo->tmax[t] = mx;
+  }
+  if (t == 0) { int live = 0; for (int hh = 0; hh < n_heads; hh++) live += sl[hh].live; fo->heads_live = live; }
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 int extract_alloc(ll_ctx* ctx) {
   ExtractState& e = ctx->ex;
@@ -320,6 +384,21 @@ int launch_get_features(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const floa
   LL_CUDA(ctx, cub::DeviceScan::ExclusiveSum(F.tmp, F.scan_bytes, F.packed, F.offs, n, s));
   ex_scatter_kernel<<<blocks, 256, 0, s>>>(n, e.raw, e.time_stamp, F.packed, F.offs, d_corners, d_surf, d_full, d_counts);
   ctx->launches += 4;
+  LL_CUDA(ctx, cudaGetLastError());
+  return LL_OK;
+}
+int launch_piece_slices(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float* d_bounds, int pieces, const float4* full, FrameSlices* out) {
+  ExtractState& e = ctx->ex; const int n = e.n;
+  FeaturesLayout F(n);   // the flags and prefix sums launch_get_features left in `scratch`
+  LL_CUDA(ctx, scratch.carve([&](Carve& c) { F.layout(c, n); }));
+  ex_piece_slices_kernel<<<pieces, 256, 0, s>>>(n, d_bounds, e.d_meta, F.packed, F.offs, full, out); ctx->launches++;
+  LL_CUDA(ctx, cudaGetLastError());
+  return LL_OK;
+}
+int launch_gather_pieces(ll_ctx* ctx, cudaStream_t s, FrameDev* dev, const FrameBases& B, int n_heads, int pieces, int max_head_n,
+                         const float4* src_c, const float4* src_s, float4* dst_c, float4* dst_s) {
+  const dim3 grid(std::max(1, std::min(ll_div_up(max_head_n, 256 * 8), 64)), pieces * n_heads, 2);
+  ex_gather_pieces_kernel<<<grid, 256, 0, s>>>(dev->head, B, n_heads, pieces, src_c, src_s, dst_c, dst_s, &dev->seg_end[0][0], &dev->out); ctx->launches++;
   LL_CUDA(ctx, cudaGetLastError());
   return LL_OK;
 }

@@ -63,6 +63,28 @@ struct RegDevState {
   LmState lm;
 };
 
+// The piecewise frame front end (frame_front_end).  get_features decides range membership per point and the class of a point does not
+// depend on the range, so the corner / surface / full clouds of piece i are contiguous slices of the whole-scan compaction (bounds 0 ... 1):
+// from the prefix count at the first index inside the piece's bounds to the prefix count past the last one.
+#define LL_MAX_HEADS 8
+#define LL_MAX_PIECES 16
+struct FrameSlices {                   // one head: per class (corner, surface, full) and piece, the slice of the head's compaction
+  int off[3][LL_MAX_PIECES], len[3][LL_MAX_PIECES];
+  int tmax[LL_MAX_PIECES];             // ll_f2ord of the largest time stamp of the full slice (-10000: find_min_max_intensity's start value)
+  int live;                            // the head has > 5 petals (laser_feature_extractor.hpp:287); else every slice is empty
+};
+struct FrameBases { int base[LL_MAX_HEADS]; };   // where each head's compaction starts in the class arrays
+struct FrameOut {                      // what the host reads after the front end of a frame
+  int out_end[2][LL_MAX_PIECES];       // corner / surface: end of piece i's down-sampled features
+  int tmax[LL_MAX_PIECES];             // per piece, over the heads
+  int heads_live;
+};
+struct FrameDev {
+  FrameSlices head[LL_MAX_HEADS];
+  int seg_end[2][LL_MAX_PIECES], mid_end[2][LL_MAX_PIECES];   // gathered segments / the extractor's VoxelGrid outputs
+  FrameOut out;
+};
+
 // Pinned host staging of the small transfers, one field per transfer.  The rule every field relies on: a field the host writes before an
 // async copy is not written again until that copy has completed (every entry point synchronises before it returns; register_device reads
 // snap[it & 1] only after the event recorded behind its copy).
@@ -77,6 +99,8 @@ struct PinnedStage {
   int fe_meta[3];         // front end: ExtractState::d_meta
   int counts[3];          // count read-backs of the single-call entry points
   float bounds[32];       // ll_piece_bounds
+  double head_time[LL_MAX_HEADS];   // ExtractState::d_time of each head of a piecewise frame (its heads are enqueued without a synchronisation)
+  FrameOut frame;         // piecewise frame front end: FrameDev::out
 };
 
 // Grid-wide exchange area of the solver kernels (one per context, device memory, zeroed once at creation; see solve.cu):
@@ -149,7 +173,10 @@ int launch_transform(ll_ctx* ctx, cudaStream_t s, const double* d_pose7, const f
 int launch_pack_strided(ll_ctx* ctx, const float4* d_src, int n, unsigned char* d_dst);   // 16-byte points -> PointCloud2 records (ctx->layout)
 // VoxelGrid on device: d_in [n] -> d_out [<= n], *d_n_out on device. n given by host, or by device count d_n_in (may be null).
 int launch_voxel_grid(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_in, int n_cap, const int* d_n_in, float leaf, float4* d_out, int* d_n_out);
-size_t voxel_grid_bytes(int n_cap);   // what launch_voxel_grid carves from `scratch`
+// The same over nseg (1 ... 256) disjoint contiguous segments of d_in, segment s ending at the device index d_end[s] (clamped to n_cap; d_end may be
+// null when nseg == 1): each segment filtered as if alone, the outputs one segment after another, d_out_end[s] = the end of segment s's output.
+int launch_voxel_grid_segments(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_in, int n_cap, const int* d_end, int nseg, float leaf, float4* d_out, int* d_out_end);
+size_t voxel_grid_bytes(int n_cap, int nseg = 1);   // what launch_voxel_grid(_segments) carves from `scratch`
 
 // ---------------------------------------------------------------------------------------------- extractor (extract.cu)
 int extract_alloc(ll_ctx* ctx);   // ExtractState arrays for max_scan_points (ll_ctx_create)
@@ -161,6 +188,22 @@ int launch_piece_bounds(ll_ctx* ctx, int pieces, float* d_start_end /* 2*pieces 
 size_t petals_bytes(int n);         // what launch_extract_petals carves from `scratch`
 size_t get_features_bytes(int n);   // what launch_get_features carves from `scratch`
 
+// ---------------------------------------------------------------------------------------------- piecewise frame front end (extract.cu)
+// After launch_get_features(bounds 0 ... 1, full kept) of one head, on the same stream and scratch: the slices of `pieces` pieces from the
+// bounds at d_bounds (launch_piece_bounds), and the time-stamp maximum of each full slice (`full` = the head's full cloud).
+int launch_piece_slices(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float* d_bounds, int pieces, const float4* full, FrameSlices* out);
+// Piece i's slices of every head, in head order, into segment i of dst_c / dst_s; seg_end, out.tmax and out.heads_live of `dev`.
+int launch_gather_pieces(ll_ctx* ctx, cudaStream_t s, FrameDev* dev, const FrameBases& B, int n_heads, int pieces, int max_head_n,
+                         const float4* src_c, const float4* src_s, float4* dst_c, float4* dst_s);
+
 // ---------------------------------------------------------------------------------------------- host driver pieces (api.cu)
 int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg_state* in, ll_reg_result* out);
 int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);
+// The device arrays of a piecewise frame front end (owned by the streaming mapper): gathered segments of cap points per class, the first
+// VoxelGrids' outputs, and the segmented VoxelGrids' scratch arenas (vg[0] on the context's stream, vg[1] on stream2).
+struct FrameArena { FrameDev* dev; float4* cls[2]; float4* mid[2]; int cap; DevBuf* vg[2]; };
+// Every head through the extractor, the slices of every piece, the gathers and the four segmented VoxelGrids (laser_feature_extractor.hpp:
+// 303-380, laser_mapping.hpp:1367-1373), enqueued without a host synchronisation; dev->out lands in ctx->pin->frame.  Piece i's features
+// are then cls[0] / cls[1] [out_end[.][i - 1], out_end[.][i]).
+int frame_front_end(ll_ctx* ctx, const FrameArena& fa, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+                    int pieces, const ll_pipeline_cfg* pc);

@@ -68,6 +68,14 @@ struct ll_mapper {
   bool have_map = false;
   bool map_dirty = false;   // m_if_mapping_updated_{corner,surface}
   bool trace = false;       // LL_MAPPER_TRACE=1
+  DevBuf frame, frame_vg[2];   // the piecewise front end of ll_mapper_process_frame (FrameLayout; segmented VoxelGrid scratch on stream / stream2)
+  int frame_pieces = 0;        // the pieces `frame` was laid out for
+};
+
+// frame: the front end's device record and, per class, the gathered piece segments and the first VoxelGrid's outputs
+struct FrameLayout {
+  FrameDev* dev; float4* cls[2]; float4* mid[2];
+  void layout(Carve& k, size_t cap) { dev = k.take<FrameDev>(1); for (int c = 0; c < 2; c++) { cls[c] = k.take<float4>(cap); mid[c] = k.take<float4>(cap); } }
 };
 
 // snap: the match-map snapshot (the two whole-map VoxelGrid outputs) and their counts
@@ -88,6 +96,12 @@ static int mapper_reserve(ll_ctx* ctx, ll_mapper* m) {
   const size_t R = (size_t)(m->cfg.reserve_map_points > 0 ? m->cfg.reserve_map_points : 0), S = (size_t)(m->cfg.reserve_store_points > 0 ? m->cfg.reserve_store_points : 0);
   const int F = ctx->cfg.max_features;
   WorkLayout w; LL_CUDA(ctx, m->work.reserve_floor(layout_bytes([&](Carve& c) { w.layout(c, F); })));
+  // the piecewise front end: pieces x max_scan_points per class (overlapping pieces repeat points), nothing allocated per frame
+  { const int P = m->cfg.pipeline.pieces >= 1 && m->cfg.pipeline.pieces <= LL_MAX_PIECES ? m->cfg.pipeline.pieces : 1;
+    const size_t cap = (size_t)P * ctx->cfg.max_scan_points;
+    FrameLayout fl; LL_CUDA(ctx, m->frame.reserve_floor(layout_bytes([&](Carve& c) { fl.layout(c, cap); })));
+    for (DevBuf& b : m->frame_vg) LL_CUDA(ctx, b.reserve_floor(std::max(voxel_grid_bytes((int)cap, P), voxel_grid_bytes(ctx->cfg.max_scan_points, 1))));
+    m->frame_pieces = P; }
   if (S) { LL_TRY(ll_cellmap_reserve(ctx, m->cells_corner, S, F)); LL_TRY(ll_cellmap_reserve(ctx, m->cells_surf, S, F)); }
   // The two map-side arenas, each at the largest of its consumers.  Both: the append's VoxelGrid of a scan's features (corner half on stream2 /
   // scratch2, surface half on the context's stream / scratch) and the refresh's whole-map VoxelGrid and index build (the halves side by side
@@ -143,7 +157,8 @@ void ll_mapper_release(ll_mapper* m) {
   cudaSetDevice(m->ctx->device);
   ll_cellmap_release(m->cells_corner); ll_cellmap_release(m->cells_surf);
   if (m->match_map) ll_map_release(m->match_map);
-  m->work.release(); m->snap.release(); m->his_corner.release(); m->his_surf.release(); delete m;
+  m->work.release(); m->snap.release(); m->his_corner.release(); m->his_surf.release();
+  m->frame.release(); m->frame_vg[0].release(); m->frame_vg[1].release(); delete m;
 }
 int ll_mapper_pose(const ll_mapper* m, double q_wxyz[4], double t[3], int* frame_index) {
   if (!m) return LL_ERR_INVALID;
@@ -152,25 +167,24 @@ int ll_mapper_pose(const ll_mapper* m, double q_wxyz[4], double t[3], int* frame
   return LL_OK;
 }
 
-// One scan: features -> (refresh match map from the cell maps) -> registration -> world-frame features -> VoxelGrid -> cell maps.
-int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int where, double stamp, ll_reg_result* out, ll_mapper_stats* stats) {
-  if (!m || !out) return LL_ERR_INVALID;
-  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
-  cudaStream_t s = ctx->stream;
-  if (stats) memset(stats, 0, sizeof(*stats));
-  double tp = now_ms();
-  const RegArrays& A = ctx->A;
-  int nc = 0, ns = 0, dropped = 0;
-  LL_TRY(scan_front_end(ctx, raw, n, fmt, where, stamp, &m->cfg.pipeline, &nc, &ns, &dropped));
+static void out_init(const ll_mapper* m, ll_reg_result* out) {
   memset(out, 0, sizeof(*out)); out->status = 1;
   for (int k = 0; k < 4; k++) out->q_w_curr[k] = m->q_w_curr[k]; for (int k = 0; k < 3; k++) out->t_w_curr[k] = m->t_w_curr[k];
-  if (stats) { stats->n_corner = nc; stats->n_surf = ns; stats->ms_front_end = (float)(now_ms() - tp); }
-  tp = now_ms();
-  if (dropped) return LL_OK;                                                     // laser_feature_extractor.hpp:287
+}
+
+// One mapper step on features already in A.feat (nc corners, then ns surfaces) whose full cloud's largest time stamp is max_t: (refresh the
+// match map) -> registration -> world-frame features -> VoxelGrid -> history window and cell maps -> pose.  Every registered scan of
+// ll_mapper_process_scan and every published piece of ll_mapper_process_frame goes through it.
+static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result* out, ll_mapper_stats* stats) {
+  ll_ctx* ctx = m->ctx;
+  cudaStream_t s = ctx->stream;
+  const RegArrays& A = ctx->A;
+  out_init(m, out);
+  double tp = now_ms();
   // :1336-1350: the time-stamp range of this scan comes from the full cloud (min of refine_blur = the previous scan's maximum), and
   // init_pointcloud_registration copies m_current_frame_index BEFORE it is incremented
   const int frame_index_for_reg = m->frame_index;
-  const double minimum_pt_time_stamp = m->last_time_stamp, maximum_pt_time_stamp = (double)ctx->last_full_max_t;
+  const double minimum_pt_time_stamp = m->last_time_stamp, maximum_pt_time_stamp = max_t;
   m->last_time_stamp = maximum_pt_time_stamp;
   m->frame_index++;                                                              // m_current_frame_index++ (:1350)
   // ---- update_buff_for_matching (mode 1): snapshot of the cells in range and in the FOV, whole-map VoxelGrid, index
@@ -260,6 +274,58 @@ int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int
   m->map_dirty = true;                                                           // m_if_mapping_updated_* (:1490-1491)
   if (stats) { stats->appended_corner = hc[0]; stats->appended_surf = hc[1]; stats->ms_append = (float)(now_ms() - tp); }
   for (int k = 0; k < 4; k++) m->q_w_curr[k] = out->q_w_curr[k]; for (int k = 0; k < 3; k++) m->t_w_curr[k] = out->t_w_curr[k];   // :1496-1505
+  return LL_OK;
+}
+
+// One scan: features -> mapper_step.
+int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int where, double stamp, ll_reg_result* out, ll_mapper_stats* stats) {
+  if (!m || !out) return LL_ERR_INVALID;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  const double tp = now_ms();
+  int nc = 0, ns = 0, dropped = 0;
+  LL_TRY(scan_front_end(ctx, raw, n, fmt, where, stamp, &m->cfg.pipeline, &nc, &ns, &dropped));
+  out_init(m, out);
+  if (stats) { stats->n_corner = nc; stats->n_surf = ns; stats->ms_front_end = (float)(now_ms() - tp); }
+  if (dropped) return LL_OK;                                                     // laser_feature_extractor.hpp:287
+  return mapper_step(m, nc, ns, (double)ctx->last_full_max_t, out, stats);
+}
+
+// One frame: the piecewise front end (every head, every piece, one host read), then per published piece its features into A.feat and
+// mapper_step.  A rejected piece leaves the pose as it was, and the next piece continues from there.
+int ll_mapper_process_frame(ll_mapper* m, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+                            int odom_mode, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces) {
+  if (!m || !out || !raws || !ns || !stamps || !n_pieces || n_heads < 1 || n_heads > LL_MAX_HEADS) return LL_ERR_INVALID;
+  *n_pieces = 0;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  const int pieces = m->cfg.reg.if_motion_deblur ? 1 : m->cfg.pipeline.pieces;   // laser_feature_extractor.hpp:305-309
+  if (pieces < 1 || pieces > m->frame_pieces) { ctx->set_error("pieces must be 1 ... 16"); return LL_ERR_INVALID; }
+  if (odom_mode != 0 && odom_mode != 1) { ctx->set_error("odom_mode must be 0 or 1"); return LL_ERR_INVALID; }
+  const int publish = odom_mode ? pieces : 1;                                   // :385-388
+  if (cap < publish) { ctx->set_error("cap smaller than the pieces to publish"); return LL_ERR_INVALID; }
+  size_t total = 0;
+  for (int h = 0; h < n_heads; h++) { if (!raws[h] && ns[h]) return LL_ERR_INVALID; total += ns[h]; }
+  if (total > (size_t)ctx->cfg.max_scan_points) { ctx->set_error("frame (all heads) larger than max_scan_points"); return LL_ERR_CAPACITY; }
+  const double tp = now_ms();
+  FrameLayout fl; LL_CUDA(ctx, m->frame.carve([&](Carve& c) { fl.layout(c, (size_t)m->frame_pieces * ctx->cfg.max_scan_points); }));
+  const FrameArena fa{fl.dev, {fl.cls[0], fl.cls[1]}, {fl.mid[0], fl.mid[1]}, m->frame_pieces * ctx->cfg.max_scan_points, {&m->frame_vg[0], &m->frame_vg[1]}};
+  LL_TRY(frame_front_end(ctx, fa, n_heads, raws, ns, fmt, where, stamps, pieces, &m->cfg.pipeline));
+  LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  const FrameOut fo = ctx->pin->frame;
+  const float ms_front_end = (float)(now_ms() - tp);
+  if (fo.heads_live == 0) return LL_OK;                                          // laser_feature_extractor.hpp:287, every head
+  for (int i = 0; i < publish; i++) {
+    const int c0 = i ? fo.out_end[0][i - 1] : 0, s0 = i ? fo.out_end[1][i - 1] : 0;
+    const int nc = fo.out_end[0][i] - c0, nsf = fo.out_end[1][i] - s0;
+    ll_mapper_stats* st = stats ? stats + i : nullptr;
+    if (st) { memset(st, 0, sizeof(*st)); st->n_corner = nc; st->n_surf = nsf; st->ms_front_end = i == 0 ? ms_front_end : 0.f; }
+    out_init(m, out + i);
+    if (nc + nsf > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
+    LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat, fa.cls[0] + c0, (size_t)nc * 16, cudaMemcpyDeviceToDevice, ctx->stream));
+    LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat + nc, fa.cls[1] + s0, (size_t)nsf * 16, cudaMemcpyDeviceToDevice, ctx->stream));
+    LL_TRY(mapper_step(m, nc, nsf, (double)ll_ord2f(fo.tmax[i]), out + i, st));
+    *n_pieces = i + 1;
+  }
   return LL_OK;
 }
 

@@ -148,6 +148,18 @@ def voxel_grid_filter(ctx: Context, cloud, leaf: float):
     return out[:m.value].copy()
 
 
+def voxel_grid_segments(ctx: Context, cloud, seg_end, leaf: float):
+    """VoxelGrid over disjoint contiguous segments of one cloud in one device pass (ll_voxel_downsample_segments): segment k is
+    cloud[seg_end[k - 1]:seg_end[k]], each filtered as if alone.  Returns the list of per-segment outputs."""
+    pts = np.ascontiguousarray(cloud, np.float32).reshape(-1, 4)
+    ends = np.ascontiguousarray(seg_end, np.uint64)
+    out = np.empty((max(pts.shape[0], 1), 4), np.float32)
+    counts = np.zeros(ends.shape[0], np.uint64)
+    ctx.check(ctx._lib.ll_voxel_downsample_segments(ctx.h, pts.ctypes.data, pts.shape[0], ends.ctypes.data, ends.shape[0], float(leaf), out.ctypes.data, counts.ctypes.data))
+    b = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+    return [out[b[k]:b[k + 1]].copy() for k in range(ends.shape[0])]
+
+
 class Map:
     """The match-map snapshot: two world-frame clouds + their exact-kNN indices (m_kdtree_{corner,surf}_from_map_last)."""
 
@@ -455,6 +467,24 @@ class Laser_mapping:
         res, stats = capi.RegResult(), capi.MapperStats()
         self.ctx.check(self.ctx._lib.ll_mapper_process_scan(self.h, ptr, n, fmt, where, float(stamp), C.byref(res), C.byref(stats)))
         return res, stats
+
+    def process_new_frame(self, heads, stamps, odom_mode=1, where=capi.LL_HOST, ns=None, fmt=None):
+        """One sensor frame (a list of raw clouds, one per head; Mid-100: 3) cut into pieces, every piece registered as a scan of its own
+        (odom_mode 1, the shipped configs; 0: piece 0 only).  Returns a list of (RegResult, MapperStats), one per published piece."""
+        k = len(heads)
+        if where == capi.LL_HOST:
+            arrs = [_pts(h) for h in heads]
+            fmt = arrs[0][1] if arrs else capi.LL_FMT_XYZI16
+            ptrs = (C.c_void_p * k)(*[a.ctypes.data for a, _ in arrs])
+            sizes = (C.c_size_t * k)(*[a.shape[0] for a, _ in arrs])
+        else:
+            ptrs = (C.c_void_p * k)(*[int(h) for h in heads])
+            sizes = (C.c_size_t * k)(*[int(n) for n in ns])
+        st = (C.c_double * k)(*[float(t) for t in stamps])
+        cap = capi.LL_MAX_PIECES_PER_FRAME
+        res, stats, n = (capi.RegResult * cap)(), (capi.MapperStats * cap)(), C.c_int()
+        self.ctx.check(self.ctx._lib.ll_mapper_process_frame(self.h, k, ptrs, sizes, fmt, where, st, int(odom_mode), res, stats, cap, C.byref(n)))
+        return [(res[i], stats[i]) for i in range(n.value)]
 
     def pose(self):
         q, t, f = np.empty(4), np.empty(3), C.c_int()
