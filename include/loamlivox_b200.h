@@ -189,6 +189,21 @@ typedef struct {
 int ll_register(ll_ctx* ctx, const ll_map* map, const void* scan_corner, size_t n_corner, const void* scan_surf, size_t n_surf,
                 int fmt, int where, const ll_reg_state* in, ll_reg_result* out);
 
+/* n independent registrations against one map in one call (several robots in one prior map, the keyframes of a recorded sequence, several
+ * initial guesses for one scan): one kNN launch and one solver launch per ICP iteration for all of them, the solver's cooperative grid cut into
+ * one CTA group per item.  Item i is (corners[i], n_corner[i], surfs[i], n_surf[i], in[i]); items may point to the same scan.
+ * out[i] and item_status[i] are what ll_register(ctx, map, corners[i], ..., &in[i], &out[i]) would return for item i alone -- the :199 gate, the
+ * reject gate, the residual-block cap with in[i].rng_seed (drawn by the item-local feature index), in[i].icp_max_iterations -- except that the
+ * gpu_ms_* fields of every out[i] time the whole batch.  The pose agrees with the single call to the last bits (the order of the solver's
+ * grid reduce follows the CTA count of the item's group, which depends on the batch).
+ * item_status[i] = LL_OK, or LL_ERR_NO_BLOCKS when item i would fail alone; such an item drops out and the others carry on.  The call itself
+ * returns LL_OK, or, before anything is enqueued (the error text names the item): LL_ERR_INVALID for n outside 1 ... LL_MAX_BATCH, a null
+ * pointer, a sharded map or items that disagree on if_motion_deblur; LL_ERR_CAPACITY when the features of all items exceed max_features or the
+ * slots of an item do not fit the shared memory of its CTA group. */
+#define LL_MAX_BATCH 16
+int ll_register_batch(ll_ctx* ctx, const ll_map* map, int n, const void* const* corners, const size_t* n_corner, const void* const* surfs,
+                      const size_t* n_surf, int fmt, int where, const ll_reg_state* in, ll_reg_result* out, int* item_status);
+
 /* Step-by-step parity hooks (tests): one ICP iteration's residual blocks at the pose in `in`
  * (type 0 invalid / 1 line / 2 plane, a[3], v[3] per slot; slots = corner features then surface features) ... */
 int ll_build_blocks(ll_ctx* ctx, const ll_map* map, const void* scan_corner, size_t n_corner, const void* scan_surf, size_t n_surf,

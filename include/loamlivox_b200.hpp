@@ -12,6 +12,7 @@
 #include <cstring>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 #include "loamlivox_b200.h"
 
@@ -127,6 +128,18 @@ class Point_cloud_registration {
     for (int k = 0; k < 3; k++) { m_t_w_curr[k] = r.t_w_curr[k]; m_t_w_incre[k] = r.t_w_incre[k]; }
     m_inlier_threshold = r.inlier_threshold; m_final_opt_summary = r;
     return r.status;
+  }
+  // Several independent registrations against one map in one call (ll_register_batch): clouds[i] = (corner, surface) features of item i,
+  // states[i] its parameters and initial pose.  results[i] / item_status[i] are what ll_register would return for item i alone (LL_OK, or
+  // LL_ERR_NO_BLOCKS for an item that dropped out); the gpu_ms_* fields time the whole batch.  An error of the whole call throws.
+  void register_batch(const Match_map& map, const std::vector<std::pair<const PointCloud*, const PointCloud*>>& clouds, const std::vector<ll_reg_state>& states,
+                      std::vector<ll_reg_result>& results, std::vector<int>& item_status) {
+    if (clouds.size() != states.size()) throw Error(LL_ERR_INVALID, "one state per item");
+    const size_t n = clouds.size();
+    std::vector<const void*> c(n), s(n); std::vector<size_t> nc(n), ns(n);
+    for (size_t i = 0; i < n; i++) { c[i] = clouds[i].first->data(); nc[i] = clouds[i].first->size(); s[i] = clouds[i].second->data(); ns[i] = clouds[i].second->size(); }
+    results.assign(n, ll_reg_result{}); item_status.assign(n, LL_OK);
+    ctx_.check(ll_register_batch(ctx_.get(), map.get(), (int)n, c.data(), nc.data(), s.data(), ns.data(), LL_FMT_PCL32, LL_HOST, states.data(), results.data(), item_status.data()));
   }
   // pointcloudAssociateToMap (:673-685), non-deblur branch
   unsigned int pointcloudAssociateToMap(const PointCloud& pc_in, PointCloud& pt_out) {

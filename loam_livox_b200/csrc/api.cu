@@ -77,7 +77,8 @@ int ll_ctx_create(const ll_config* cfg, int device, ll_ctx** out) {
   ctx->sev.each([&](cudaEvent_t& ev) { ok(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); });
   ctx->ev.each([&](cudaEvent_t& ev) { ok(cudaEventCreate(&ev)); });
   ok(cudaHostAlloc((void**)&ctx->pin, sizeof(PinnedStage), cudaHostAllocDefault));
-  void* dreg = nullptr; ok(cudaMalloc(&dreg, sizeof(RegDevState))); if (dreg) ok(cudaMemset(dreg, 0, sizeof(RegDevState))); ctx->d_reg = (RegDevState*)dreg;
+  // one registration state per batch item (d_reg[0]: ll_register and the parity hooks)
+  void* dreg = nullptr; ok(cudaMalloc(&dreg, LL_MAX_BATCH * sizeof(RegDevState))); if (dreg) ok(cudaMemset(dreg, 0, LL_MAX_BATCH * sizeof(RegDevState))); ctx->d_reg = (RegDevState*)dreg;
   if (e == cudaSuccess && solve_prepare(ctx) != LL_OK) e = cudaErrorUnknown;   // per-function attributes of the solver kernels (no process-global flag: contexts are created from any thread)
   if (e == cudaSuccess && ctx_alloc(ctx) != LL_OK) e = cudaErrorMemoryAllocation;
   if (e != cudaSuccess) { cudaGetLastError(); ll_ctx_destroy(ctx); return LL_ERR_CUDA; }
@@ -372,60 +373,81 @@ static void fill_state(RegDevState* h, const ll_reg_state* in) {
   h->q_last_opt[0] = 1.0;
   h->bound = (double)(float)in->para_max_speed; h->huber_a = in->huber_a; h->inliner_dis = in->inliner_dis; h->inlier_ratio = in->inlier_ratio;
   h->min_icp_R = in->minimum_icp_R_diff; h->min_icp_T = in->minimum_icp_T_diff;
-  h->cap = in->maximum_allow_residual_block; h->rng_seed = in->rng_seed;
+  h->cap = in->maximum_allow_residual_block; h->rng_seed = in->rng_seed; h->icp_max_iterations = in->icp_max_iterations;
   h->if_motion_deblur = in->if_motion_deblur ? 1 : 0; h->min_ts = in->minimum_pt_time_stamp; h->max_ts = in->maximum_pt_time_stamp;   // interp_* = 0: reset_incremtal_parameter (:120-125)
 }
-static KnnBlocksArgs knn_args(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg_state* in, bool debug) {
+// The n items of a registration batch: item j's features are slots off[j] ... off[j] + nc[j] + ns[j] of A.feat (corners first), one item after
+// another; its parameters in[j], its state d_reg[j].
+struct RegBatch { int n; int nc[LL_MAX_BATCH], ns[LL_MAX_BATCH], off[LL_MAX_BATCH + 1]; const ll_reg_state* in[LL_MAX_BATCH]; };
+static KnnBlocksArgs knn_args(ll_ctx* ctx, const ll_map* map, const RegBatch& b, bool debug) {
   const RegArrays& A = ctx->A;
-  KnnBlocksArgs a; a.corner = make_view(map->corner); a.surf = make_view(map->surf); a.feat = A.feat; a.n_corner = nc; a.n_surf = ns;
-  a.pose = ctx->d_reg->pose_curr; a.max_dis_line = in->maximum_dis_line_for_match; a.max_dis_plane = in->maximum_dis_plane_for_match;
-  a.icp_line = in->icp_line; a.icp_plane = in->icp_plane; a.blk_a = A.blk_a; a.blk_v = A.blk_v;
-  a.corner_avail = &ctx->d_reg->corner_avail; a.surf_avail = &ctx->d_reg->surf_avail; a.n_blocks = &ctx->d_reg->n_blocks;
-  a.cap = in->maximum_allow_residual_block; a.rng_seed = in->rng_seed;
+  KnnBlocksArgs a; a.corner = make_view(map->corner); a.surf = make_view(map->surf); a.feat = A.feat; a.M = b.off[b.n]; a.n_items = b.n;
+  for (int j = 0; j < b.n; j++) {
+    const ll_reg_state* in = b.in[j]; KnnItem& I = a.item[j];
+    I.off = b.off[j]; I.n_corner = b.nc[j]; I.n_surf = b.ns[j]; I.icp_line = in->icp_line; I.icp_plane = in->icp_plane;
+    I.cap = in->maximum_allow_residual_block; I.rng_seed = in->rng_seed;
+    I.max_dis_line = in->maximum_dis_line_for_match; I.max_dis_plane = in->maximum_dis_plane_for_match;
+  }
+  a.blk_a = A.blk_a; a.blk_v = A.blk_v;
   a.seed_ids = A.knn_idx; a.knn_d = debug ? A.knn_d : nullptr; a.perm = A.perm;
   ctx->solve_world = (map->world > 1 && ctx->world > 1) ? ctx->world : 1;   // replicas of the whole map never exchange anything
-  a.st = ctx->d_reg; a.deblur = in->if_motion_deblur ? 1 : 0; ctx->reg_deblur = a.deblur;
+  a.st = ctx->d_reg; a.deblur = b.in[0]->if_motion_deblur ? 1 : 0; ctx->reg_deblur = a.deblur;   // (the items of a batch agree on it)
   a.rank = map->rank; a.world = map->world; a.grid = map->grid; a.shard_owner = (const int*)map->shard_owner.p;
   return a;
 }
+static RegBatch single_batch(int nc, int ns, const ll_reg_state* in) {
+  RegBatch b; b.n = 1; b.nc[0] = nc; b.ns[0] = ns; b.off[0] = 0; b.off[1] = nc + ns; b.in[0] = in;
+  return b;
+}
+// One solver item over slots 0 ... M - 1 (the parity hooks and the sharded mode's two solves).
 static SolveArgs solve_args(ll_ctx* ctx, int M, SolveMode mode, int max_iter) {
   const RegArrays& A = ctx->A;
   SolveArgs s; s.st = ctx->d_reg; s.sync = ctx->d_sync; s.feat = A.feat; s.blk_a = A.blk_a; s.blk_v = A.blk_v; s.l1 = A.l1; s.k10_value = A.k10_value; s.k10_n_distinct = A.k10_n_distinct;
-  s.M = M; s.max_iterations = max_iter; s.mode = mode; s.rank = ctx->rank; s.world = ctx->solve_world; s.comm_local = (double*)ctx->comm_local;
+  s.mode = mode; s.rank = ctx->rank; s.world = ctx->solve_world; s.comm_local = (double*)ctx->comm_local;
   for (int i = 0; i < 8; i++) s.comm_peer[i] = (double*)ctx->comm_peers[i];
-  s.cap_check = 0; s.deblur = ctx->reg_deblur; s.prerun_iterations = 0; s.table = nullptr; s.table_mask = 0;
+  s.deblur = ctx->reg_deblur; s.n_items = 1;
+  SolveItem& I = s.item[0];
+  I.off = 0; I.M = M; I.max_iterations = max_iter; I.prerun_iterations = 0; I.cap_check = 0; I.table = nullptr; I.table_mask = 0;
   return s;
 }
 
 }  // extern "C"
 
-// Registration on features already resident in A.feat (device). Core of ll_register / ll_scan_to_pose.
-int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg_state* in, ll_reg_result* out) {
-  cudaStream_t s = ctx->stream;
-  const RegArrays& A = ctx->A;
-  RegEvents& ev = ctx->ev;
+// What an item returns before any device work: the result initialised from its state, the gate (:199) and the empty item.  Returns 1 when the
+// item goes on to the device; else *status is its outcome (LL_OK with registered = 0 under the gate, LL_ERR_NO_BLOCKS without features).
+static int item_prologue(ll_ctx* ctx, const ll_map* map, int M, const ll_reg_state* in, ll_reg_result* out, int* status) {
   memset(out, 0, sizeof(*out));
   out->status = 1;
   for (int k = 0; k < 4; k++) { out->q_w_curr[k] = in->q_w_curr[k]; out->q_w_incre[k] = k == 0 ? in->para_buffer_incremental[3] : in->para_buffer_incremental[k - 1]; }
   for (int k = 0; k < 3; k++) { out->t_w_curr[k] = in->t_w_curr[k]; out->t_w_incre[k] = in->para_buffer_incremental[4 + k]; }
+  *status = LL_OK;
   // gate (:199): CORNER_MIN_MAP_NUM 0, SURFACE_MIN_MAP_NUM 50
-  if (!(map->corner.n_src > 0 && map->surf.n_src > 50 && in->current_frame_index > in->mapping_init_accumulate_frames)) return LL_OK;
-  const int M = nc + ns;
-  ctx->last_nc = nc; ctx->last_ns = ns;
-  const int cap_check = M > in->maximum_allow_residual_block ? 1 : 0;   // fewer slots than the cap: neither the pre-skip nor the drop rule can fire
-  if (M == 0) { ctx->set_error("no features"); return LL_ERR_NO_BLOCKS; }
-  LL_TRY(solve_capacity(ctx, M, in->if_motion_deblur ? 1 : 0));   // before anything of this registration is enqueued
-  RegDevState* h = &ctx->pin->state_in;
-  fill_state(h, in);
-  LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, sizeof(RegDevState), cudaMemcpyHostToDevice, s));
+  if (!(map->corner.n_src > 0 && map->surf.n_src > 50 && in->current_frame_index > in->mapping_init_accumulate_frames)) return 0;
+  if (M == 0) { ctx->set_error("no features"); *status = LL_ERR_NO_BLOCKS; return 0; }
+  return 1;
+}
+
+// The ICP loops of the batch's items on the device (every item has passed item_prologue and the capacity check): one kNN launch and one solver
+// launch per ICP iteration for all of them.  outs[j] / status[j] belong to item j.
+static int register_batch(ll_ctx* ctx, const ll_map* map, const RegBatch& b, ll_reg_result* const* outs, int* const* status) {
+  cudaStream_t s = ctx->stream;
+  const RegArrays& A = ctx->A;
+  RegEvents& ev = ctx->ev;
+  const int n = b.n, Mtot = b.off[n];
+  ctx->last_nc = b.nc[0]; ctx->last_ns = b.ns[0];
+  RegDevState* h = ctx->pin->state_in;
+  for (int j = 0; j < n; j++) fill_state(&h[j], b.in[j]);
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, n * sizeof(RegDevState), cudaMemcpyHostToDevice, s));
   LL_CUDA(ctx, cudaEventRecord(ev.total[0], s));
-  out->registered = 1;
-  KnnBlocksArgs ka = knn_args(ctx, map, nc, ns, in, false);
-  LL_CUDA(ctx, cudaMemsetAsync(A.knn_idx, 0xff, (size_t)M * LL_KNN * 4, s));   // no seeds for the first ICP iteration
+  for (int j = 0; j < n; j++) outs[j]->registered = 1;
+  KnnBlocksArgs ka = knn_args(ctx, map, b, false);
+  LL_CUDA(ctx, cudaMemsetAsync(A.knn_idx, 0xff, (size_t)Mtot * LL_KNN * 4, s));   // no seeds for the first ICP iteration
   LL_CUDA(ctx, cudaEventRecord(ev.sort[0], s));
-  LL_TRY(launch_query_sort(ctx, s, ctx->scratch, ka, A.perm));   // spatial tiles of features (Hilbert order at the initial pose)
+  LL_TRY(launch_query_sort(ctx, s, ctx->scratch, ka, A.perm));   // spatial tiles of features (Hilbert order at the initial poses)
   LL_CUDA(ctx, cudaEventRecord(ev.sort[1], s));
-  int iter = 0; RegDevState* hs = &ctx->pin->snap[0];
+  int iter = 0;
+  const ll_reg_state* in = b.in[0];   // the sharded mode (one item)
+  const int M = Mtot;
   const bool sharded = ctx->world > 1 && map->world > 1;
   if (sharded && (map->world != ctx->world || map->rank != ctx->rank)) { ctx->set_error("map shard and context disagree on rank/world"); return LL_ERR_INVALID; }
   // (the shard was built with halo * 1.0001 + 1 mm, shard.cu: a halo handed over as the float nearest to sqrt(gate) must pass)
@@ -434,14 +456,17 @@ int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg
   }
   if (map->world > 1 && ctx->world != map->world) { ctx->set_error("a sharded map needs a context connected to the same number of ranks (ll_comm_connect)"); return LL_ERR_INVALID; }
   if (sharded && M > ctx->cfg.max_features) { ctx->set_error("more features than max_features (exchange buffer)"); return LL_ERR_CAPACITY; }
+  const int cap_check = M > in->maximum_allow_residual_block ? 1 : 0;   // fewer slots than the cap: neither the pre-skip nor the drop rule can fire
   double* x_l1 = sharded ? (double*)((char*)ctx->comm_local + LL_COMM_X_OFF) : nullptr;
-  unsigned long long* set_table = nullptr;   // hash set of the L1 norms (K10)
-  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { set_table = l1_set_layout(c, M); }));
-  // One ICP iteration's device work + a snapshot of the 1.7 KB state into pinned slot `it & 1`.
-  RegDevState* slots = ctx->pin->snap;
+  unsigned long long* set_table[LL_MAX_BATCH];   // hash set of each item's L1 norms (K10)
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { for (int j = 0; j < n; j++) set_table[j] = l1_set_layout(c, b.nc[j] + b.ns[j]); }));
+  // One ICP iteration's device work + a snapshot of the n 1.7 KB states into pinned slot `it & 1`.
+  RegDevState (*slots)[LL_MAX_BATCH] = ctx->pin->snap;
   auto enqueue_iteration = [&](int it) -> int {
     cudaEvent_t* e = it < LL_TIMED_ITERS ? ev.phase[it] : nullptr;
-    LL_CUDA(ctx, cudaMemsetAsync(&ctx->d_reg->corner_avail, 0, 3 * sizeof(int), s));   // corner_avail, surf_avail, n_blocks
+    // corner_avail, surf_avail, n_blocks of every item (one item: the plain memset, cheaper to enqueue than the strided one)
+    if (n == 1) LL_CUDA(ctx, cudaMemsetAsync(&ctx->d_reg->corner_avail, 0, 3 * sizeof(int), s));
+    else LL_CUDA(ctx, cudaMemset2DAsync(&ctx->d_reg->corner_avail, sizeof(RegDevState), 0, 3 * sizeof(int), n, s));
     if (sharded) LL_CUDA(ctx, cudaMemsetAsync(x_l1, 0xff, (size_t)M * sizeof(double), s));   // NaN = nobody owns a block here (peers fill it after solve #1)
     if (it == 0) LL_CUDA(ctx, cudaEventRecord(ev.knn_first[0], s));
     if (e) LL_CUDA(ctx, cudaEventRecord(e[0], s));
@@ -449,64 +474,98 @@ int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg
     if (e) LL_CUDA(ctx, cudaEventRecord(e[1], s));
     if (it == 0) LL_CUDA(ctx, cudaEventRecord(ev.knn_first[1], s));
     if (!sharded) {
-      // one launch: solve #1 -> L1 norms -> de-duplication + order statistic -> outlier drop -> solve #2 -> pose
-      SolveArgs sa = solve_args(ctx, M, SOLVE_FUSED, in->cere_max_iterations);
-      sa.prerun_iterations = in->cere_prerun_times; sa.table = set_table; sa.table_mask = l1_set_capacity(M) - 1;
-      sa.cap_check = cap_check;
+      // one launch: per item, solve #1 -> L1 norms -> de-duplication + order statistic -> outlier drop -> solve #2 -> pose
+      SolveArgs sa = solve_args(ctx, M, SOLVE_FUSED, 0);
+      sa.n_items = n;
+      for (int j = 0; j < n; j++) {
+        SolveItem& I = sa.item[j]; const int Mj = b.nc[j] + b.ns[j];
+        I.off = b.off[j]; I.M = Mj; I.max_iterations = b.in[j]->cere_max_iterations; I.prerun_iterations = b.in[j]->cere_prerun_times;
+        I.cap_check = Mj > b.in[j]->maximum_allow_residual_block ? 1 : 0; I.table = set_table[j]; I.table_mask = l1_set_capacity(Mj) - 1;
+      }
       if (e) { LL_CUDA(ctx, cudaEventRecord(e[2], s)); LL_CUDA(ctx, cudaEventRecord(e[3], s)); }
       LL_TRY(launch_solve(ctx, sa));
     } else {
       if (cap_check) LL_TRY(launch_count_exchange(ctx));
-      { SolveArgs sa = solve_args(ctx, M, SOLVE_FIRST, in->cere_prerun_times); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
+      { SolveArgs sa = solve_args(ctx, M, SOLVE_FIRST, in->cere_prerun_times); sa.item[0].cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
       if (e) LL_CUDA(ctx, cudaEventRecord(e[2], s));
       LL_TRY(launch_l1_exchange(ctx, A.l1, M));
-      LL_TRY(launch_k10_select(ctx, x_l1, M, &ctx->d_reg->inlier_ratio, set_table, l1_set_capacity(M) - 1, A.k10_value, A.k10_n_distinct));
+      LL_TRY(launch_k10_select(ctx, x_l1, M, &ctx->d_reg->inlier_ratio, set_table[0], l1_set_capacity(M) - 1, A.k10_value, A.k10_n_distinct));
       if (e) LL_CUDA(ctx, cudaEventRecord(e[3], s));
-      { SolveArgs sa = solve_args(ctx, M, SOLVE_SECOND, in->cere_max_iterations); sa.cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
+      { SolveArgs sa = solve_args(ctx, M, SOLVE_SECOND, in->cere_max_iterations); sa.item[0].cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
     }
     if (e) LL_CUDA(ctx, cudaEventRecord(e[4], s));
-    LL_CUDA(ctx, cudaMemcpyAsync(&slots[it & 1], ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
+    LL_CUDA(ctx, cudaMemcpyAsync(slots[it & 1], ctx->d_reg, n * sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
     LL_CUDA(ctx, cudaEventRecord(ctx->sev.it[it & 1], s));
     return LL_OK;
   };
-  // The host stays one iteration ahead: iteration k+1 is enqueued before iteration k's state is read back, so the GPU never waits for the
-  // PCIe round trip of the termination test.  The kernels of an iteration enqueued after the loop has ended return at once (st->icp_done).
+  // The host stays one iteration ahead: iteration k+1 is enqueued before iteration k's states are read back, so the GPU never waits for the
+  // PCIe round trip of the termination test.  The kernels of an iteration enqueued after an item's loop has ended return at once for that item
+  // (st->icp_done: set on the device by convergence, by the item's own icp_max_iterations, or when no residual block is left).
   const bool speculate = !sharded;
+  int max_iters = 0; for (int j = 0; j < n; j++) max_iters = std::max(max_iters, b.in[j]->icp_max_iterations);
+  RegDevState fin[LL_MAX_BATCH];   // each item's state at the iteration its loop ended
+  int done[LL_MAX_BATCH] = {0}, iters[LL_MAX_BATCH] = {0}, n_done = 0;
   LL_TRY(enqueue_iteration(0));
-  for (iter = 0; iter < in->icp_max_iterations; iter++) {
-    if (speculate && iter + 1 < in->icp_max_iterations) LL_TRY(enqueue_iteration(iter + 1));
+  for (iter = 0; iter < max_iters; iter++) {
+    if (speculate && iter + 1 < max_iters) LL_TRY(enqueue_iteration(iter + 1));
     LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.it[iter & 1]));
-    hs = &slots[iter & 1];
-    if (hs->lm.termination == -1) {   // the iteration enqueued ahead returns at once (icp_done is set on the device); drain it before the arena is reused
-      cudaStreamSynchronize(s); ctx->set_error("no residual block survived the gates / cap / inlier selection"); return LL_ERR_NO_BLOCKS;
+    for (int j = 0; j < n; j++) {
+      if (done[j]) continue;
+      const RegDevState* hs = &slots[iter & 1][j];
+      if (hs->lm.termination == -1) {
+        done[j] = -1; n_done++; *status[j] = LL_ERR_NO_BLOCKS;
+        ctx->set_error(n == 1 ? std::string("no residual block survived the gates / cap / inlier selection")
+                              : "item " + std::to_string(j) + ": no residual block survived the gates / cap / inlier selection");
+      } else if (hs->icp_done || iter + 1 >= b.in[j]->icp_max_iterations) { done[j] = 1; n_done++; fin[j] = *hs; iters[j] = iter + 1; }
     }
-    if (hs->icp_done) break;
-    if (!speculate && iter + 1 < in->icp_max_iterations) LL_TRY(enqueue_iteration(iter + 1));
+    if (n_done == n) break;
+    if (!speculate && iter + 1 < max_iters) LL_TRY(enqueue_iteration(iter + 1));
   }
+  // (an iteration enqueued ahead returns at once; it is drained here, before the arena is reused)
   LL_CUDA(ctx, cudaEventRecord(ev.total[1], s));
   LL_CUDA(ctx, cudaEventSynchronize(ev.total[1]));
-  cudaEventElapsedTime(&out->gpu_ms_total, ev.total[0], ev.total[1]); cudaEventElapsedTime(&out->gpu_ms_knn, ev.knn_first[0], ev.knn_first[1]);
-  cudaEventElapsedTime(&out->gpu_ms_sort, ev.sort[0], ev.sort[1]);
-  { const int done_iters = (iter < in->icp_max_iterations ? iter + 1 : in->icp_max_iterations);
+  ll_reg_result t; memset(&t, 0, sizeof(t));   // the batch's timings, given to every item
+  cudaEventElapsedTime(&t.gpu_ms_total, ev.total[0], ev.total[1]); cudaEventElapsedTime(&t.gpu_ms_knn, ev.knn_first[0], ev.knn_first[1]);
+  cudaEventElapsedTime(&t.gpu_ms_sort, ev.sort[0], ev.sort[1]);
+  { const int done_iters = (iter < max_iters ? iter + 1 : max_iters);
     for (int i = 0; i < done_iters && i < LL_TIMED_ITERS; i++) { float a = 0, b = 0, c = 0, d = 0; cudaEvent_t* e = ev.phase[i];
       cudaEventElapsedTime(&a, e[0], e[1]); cudaEventElapsedTime(&b, e[1], e[2]); cudaEventElapsedTime(&c, e[2], e[3]); cudaEventElapsedTime(&d, e[3], e[4]);
-      out->gpu_ms_knn_all += a; out->gpu_ms_solve_all += b + d; out->gpu_ms_select_all += c; } }
-  out->icp_iterations = (iter + 1 < in->icp_max_iterations) ? iter + 1 : in->icp_max_iterations;
-  out->corner_used = hs->corner_avail; out->surf_used = hs->surf_avail; out->num_residual_blocks = hs->num_residual_blocks;
-  out->total_lm_iterations = hs->total_lm_iterations; out->total_evaluations = hs->total_evaluations;
-  for (int k = 0; k < 4; k++) out->q_w_curr[k] = hs->pose_curr[k];
-  for (int k = 0; k < 3; k++) out->t_w_curr[k] = hs->pose_curr[4 + k];
-  out->q_w_incre[0] = hs->x[3]; out->q_w_incre[1] = hs->x[0]; out->q_w_incre[2] = hs->x[1]; out->q_w_incre[3] = hs->x[2];
-  for (int k = 0; k < 3; k++) out->t_w_incre[k] = hs->x[4 + k];
-  out->final_cost = hs->final_cost; out->initial_cost = hs->initial_cost; out->angular_diff = hs->angular_diff; out->t_diff = hs->t_diff;
-  out->inlier_threshold = hs->inlier_threshold * hs->final_cost / hs->initial_cost;   // :559
-  const float minimize_cost = (float)hs->final_cost;
-  if (hs->angular_diff > (double)(float)in->para_max_angular_rate || minimize_cost > (float)in->max_final_cost) {   // :561-573
-    out->status = 0;
-    for (int k = 0; k < 4; k++) out->q_w_curr[k] = in->q_w_last[k];
-    for (int k = 0; k < 3; k++) out->t_w_curr[k] = in->t_w_last[k];
+      t.gpu_ms_knn_all += a; t.gpu_ms_solve_all += b + d; t.gpu_ms_select_all += c; } }
+  for (int j = 0; j < n; j++) {
+    if (done[j] != 1) continue;
+    const RegDevState* hs = &fin[j]; const ll_reg_state* in = b.in[j]; ll_reg_result* out = outs[j];
+    out->gpu_ms_total = t.gpu_ms_total; out->gpu_ms_knn = t.gpu_ms_knn; out->gpu_ms_sort = t.gpu_ms_sort;
+    out->gpu_ms_knn_all = t.gpu_ms_knn_all; out->gpu_ms_solve_all = t.gpu_ms_solve_all; out->gpu_ms_select_all = t.gpu_ms_select_all;
+    out->icp_iterations = iters[j];
+    out->corner_used = hs->corner_avail; out->surf_used = hs->surf_avail; out->num_residual_blocks = hs->num_residual_blocks;
+    out->total_lm_iterations = hs->total_lm_iterations; out->total_evaluations = hs->total_evaluations;
+    for (int k = 0; k < 4; k++) out->q_w_curr[k] = hs->pose_curr[k];
+    for (int k = 0; k < 3; k++) out->t_w_curr[k] = hs->pose_curr[4 + k];
+    out->q_w_incre[0] = hs->x[3]; out->q_w_incre[1] = hs->x[0]; out->q_w_incre[2] = hs->x[1]; out->q_w_incre[3] = hs->x[2];
+    for (int k = 0; k < 3; k++) out->t_w_incre[k] = hs->x[4 + k];
+    out->final_cost = hs->final_cost; out->initial_cost = hs->initial_cost; out->angular_diff = hs->angular_diff; out->t_diff = hs->t_diff;
+    out->inlier_threshold = hs->inlier_threshold * hs->final_cost / hs->initial_cost;   // :559
+    const float minimize_cost = (float)hs->final_cost;
+    if (hs->angular_diff > (double)(float)in->para_max_angular_rate || minimize_cost > (float)in->max_final_cost) {   // :561-573
+      out->status = 0;
+      for (int k = 0; k < 4; k++) out->q_w_curr[k] = in->q_w_last[k];
+      for (int k = 0; k < 3; k++) out->t_w_curr[k] = in->t_w_last[k];
+    }
   }
   return LL_OK;
+}
+
+int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg_state* in, ll_reg_result* out) {
+  int st = LL_OK;
+  if (!item_prologue(ctx, map, nc + ns, in, out, &st)) {
+    if (st != LL_OK) { ctx->last_nc = 0; ctx->last_ns = 0; }   // an empty registration has no features
+    return st;
+  }
+  const int M = nc + ns;
+  LL_TRY(solve_capacity(ctx, 1, &M, in->if_motion_deblur ? 1 : 0));   // before anything of this registration is enqueued
+  int* stp = &st;
+  LL_TRY(register_batch(ctx, map, single_batch(nc, ns, in), &out, &stp));
+  return st;
 }
 
 extern "C" {
@@ -518,6 +577,39 @@ int ll_register(ll_ctx* ctx, const ll_map* map, const void* scan_corner, size_t 
   LL_TRY(upload_cloud(ctx, scan_corner, nc, fmt, where, ctx->A.feat));
   LL_TRY(upload_cloud(ctx, scan_surf, ns, fmt, where, ctx->A.feat + nc));
   return register_device(ctx, map, (int)nc, (int)ns, in, out);
+}
+
+int ll_register_batch(ll_ctx* ctx, const ll_map* map, int n, const void* const* corners, const size_t* n_corner, const void* const* surfs, const size_t* n_surf,
+                      int fmt, int where, const ll_reg_state* in, ll_reg_result* out, int* item_status) {
+  if (!ctx || !map || !corners || !n_corner || !surfs || !n_surf || !in || !out || !item_status) return LL_ERR_INVALID;
+  if (n < 1 || n > LL_MAX_BATCH) { ctx->set_error("n = " + std::to_string(n) + ": a batch holds 1 ... " + std::to_string(LL_MAX_BATCH) + " items"); return LL_ERR_INVALID; }
+  if (map->world > 1) { ctx->set_error("a sharded map registers one scan at a time (ll_register)"); return LL_ERR_INVALID; }
+  cudaSetDevice(ctx->device);
+  size_t total = 0;
+  for (int i = 0; i < n; i++) {
+    if ((!corners[i] && n_corner[i]) || (!surfs[i] && n_surf[i])) { ctx->set_error("item " + std::to_string(i) + ": null feature cloud"); return LL_ERR_INVALID; }
+    if ((in[i].if_motion_deblur != 0) != (in[0].if_motion_deblur != 0)) { ctx->set_error("item " + std::to_string(i) + ": if_motion_deblur differs from item 0's"); return LL_ERR_INVALID; }
+    total += n_corner[i] + n_surf[i];
+  }
+  if (total > (size_t)ctx->cfg.max_features) { ctx->set_error("the items' features (" + std::to_string(total) + ") exceed max_features"); return LL_ERR_CAPACITY; }
+  // the items that go on to the device, their features one after another
+  RegBatch b; b.n = 0; b.off[0] = 0;
+  int idx[LL_MAX_BATCH], M[LL_MAX_BATCH];
+  for (int i = 0; i < n; i++) {
+    if (!item_prologue(ctx, map, (int)(n_corner[i] + n_surf[i]), &in[i], &out[i], &item_status[i])) continue;
+    const int j = b.n++;
+    idx[j] = i; b.nc[j] = (int)n_corner[i]; b.ns[j] = (int)n_surf[i]; b.in[j] = &in[i]; M[j] = b.nc[j] + b.ns[j]; b.off[j + 1] = b.off[j] + M[j];
+  }
+  if (b.n == 0) return LL_OK;
+  int bad = 0;
+  if (solve_capacity(ctx, b.n, M, in[0].if_motion_deblur ? 1 : 0, &bad) != LL_OK) { ctx->set_error("item " + std::to_string(idx[bad]) + ": " + ctx->err); return LL_ERR_CAPACITY; }
+  for (int j = 0; j < b.n; j++) {
+    LL_TRY(upload_cloud(ctx, corners[idx[j]], b.nc[j], fmt, where, ctx->A.feat + b.off[j]));
+    LL_TRY(upload_cloud(ctx, surfs[idx[j]], b.ns[j], fmt, where, ctx->A.feat + b.off[j] + b.nc[j]));
+  }
+  ll_reg_result* outs[LL_MAX_BATCH]; int* sts[LL_MAX_BATCH];
+  for (int j = 0; j < b.n; j++) { outs[j] = &out[idx[j]]; sts[j] = &item_status[idx[j]]; }
+  return register_batch(ctx, map, b, outs, sts);
 }
 
 // One tiny registration (three planes and two edges: 1240 map points, 310 features) through the whole device path, result discarded.  It pays -- once, at a
@@ -558,9 +650,9 @@ int ll_build_blocks(ll_ctx* ctx, const ll_map* map, const void* scan_corner, siz
   cudaStream_t s = ctx->stream;
   LL_TRY(upload_cloud(ctx, scan_corner, nc, fmt, where, A.feat));
   LL_TRY(upload_cloud(ctx, scan_surf, ns, fmt, where, A.feat + nc));
-  RegDevState* h = &ctx->pin->state_in; fill_state(h, in);
+  RegDevState* h = ctx->pin->state_in; fill_state(h, in);
   LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, sizeof(RegDevState), cudaMemcpyHostToDevice, s));
-  { KnnBlocksArgs ka = knn_args(ctx, map, (int)nc, (int)ns, in, true); LL_CUDA(ctx, cudaMemsetAsync(A.knn_idx, 0xff, (size_t)M * LL_KNN * 4, s)); LL_TRY(launch_query_sort(ctx, s, ctx->scratch, ka, A.perm)); LL_TRY(launch_knn_blocks(ctx, ka)); }
+  { KnnBlocksArgs ka = knn_args(ctx, map, single_batch((int)nc, (int)ns, in), true); LL_CUDA(ctx, cudaMemsetAsync(A.knn_idx, 0xff, (size_t)M * LL_KNN * 4, s)); LL_TRY(launch_query_sort(ctx, s, ctx->scratch, ka, A.perm)); LL_TRY(launch_knn_blocks(ctx, ka)); }
   std::vector<float4> ba(M); std::vector<double> bv((size_t)M * 3);
   int cnt[2];
   LL_CUDA(ctx, cudaMemcpyAsync(ba.data(), A.blk_a, (size_t)M * 16, cudaMemcpyDeviceToHost, s));
@@ -587,8 +679,8 @@ static int hook_solve(ll_ctx* ctx, const double x[7], const SolveArgs& sa, doubl
   for (int k = 0; k < 7; k++) pin->x[k] = x[k];
   LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg->x, pin->x, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
   LL_TRY(launch_solve(ctx, sa));
-  LL_CUDA(ctx, cudaMemcpyAsync(&pin->snap[0], ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
-  if (l1_out && sa.M > 0) LL_CUDA(ctx, cudaMemcpyAsync(l1_out, ctx->A.l1, (size_t)sa.M * sizeof(double), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(&pin->snap[0][0], ctx->d_reg, sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
+  if (l1_out && sa.item[0].M > 0) LL_CUDA(ctx, cudaMemcpyAsync(l1_out, ctx->A.l1, (size_t)sa.item[0].M * sizeof(double), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   return LL_OK;
 }
@@ -599,7 +691,7 @@ int ll_normal_equations(ll_ctx* ctx, const double x[7], double out28[28]) {
   if (!ctx || !x || !out28) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
   LL_TRY(hook_solve(ctx, x, solve_args(ctx, ctx->hook_slots, SOLVE_EVALUATE, 0)));
-  const RegDevState* hs = &ctx->pin->snap[0];
+  const RegDevState* hs = &ctx->pin->snap[0][0];
   for (int i = 0; i < 21; i++) out28[i] = hs->lm.H[i];
   for (int i = 0; i < 6; i++) out28[21 + i] = hs->lm.g[i];
   out28[27] = hs->lm.x_cost;
@@ -609,7 +701,7 @@ int ll_solve(ll_ctx* ctx, int max_iterations, double x_io[7], double* initial_co
   if (!ctx || !x_io) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
   LL_TRY(hook_solve(ctx, x_io, solve_args(ctx, ctx->hook_slots, SOLVE_PLAIN, max_iterations)));
-  const RegDevState* hs = &ctx->pin->snap[0];
+  const RegDevState* hs = &ctx->pin->snap[0][0];
   for (int k = 0; k < 7; k++) x_io[k] = hs->x[k];
   if (initial_cost) *initial_cost = hs->lm.initial_cost; if (final_cost) *final_cost = hs->lm.final_cost; if (iterations) *iterations = hs->lm.iteration;
   return LL_OK;
@@ -618,7 +710,7 @@ int ll_set_blocks(ll_ctx* ctx, const ll_reg_state* in, size_t n, const int32_t* 
   if (!ctx || !in || (n > 0 && (!type || !p || !a3 || !v3))) return LL_ERR_INVALID;
   if (n > (size_t)ctx->cfg.max_features) { ctx->set_error("more blocks than max_features"); return LL_ERR_CAPACITY; }
   const int M = (int)n;
-  LL_TRY(solve_capacity(ctx, M, in->if_motion_deblur ? 1 : 0));
+  LL_TRY(solve_capacity(ctx, 1, &M, in->if_motion_deblur ? 1 : 0));
   for (int i = 0; i < M; i++) if (type[i] < 0 || type[i] > 2) { ctx->set_error("block type must be 0, 1 (line) or 2 (plane)"); return LL_ERR_INVALID; }
   cudaSetDevice(ctx->device);
   const RegArrays& A = ctx->A;
@@ -630,7 +722,7 @@ int ll_set_blocks(ll_ctx* ctx, const ll_reg_state* in, size_t n, const int32_t* 
     LL_CUDA(ctx, cudaMemcpyAsync(A.blk_a, ba.data(), (size_t)M * 16, cudaMemcpyHostToDevice, s));
     LL_CUDA(ctx, cudaMemcpyAsync(A.blk_v, v3, (size_t)M * 24, cudaMemcpyHostToDevice, s));
   }
-  RegDevState* h = &ctx->pin->state_in; fill_state(h, in);
+  RegDevState* h = ctx->pin->state_in; fill_state(h, in);
   for (int i = 0; i < M; i++) h->n_blocks += type[i] != 0 ? 1 : 0;   // what the kNN kernel counts: the drop rule of the residual-block cap reads it
   LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, sizeof(RegDevState), cudaMemcpyHostToDevice, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));   // the pageable staging above goes out of scope
@@ -644,14 +736,15 @@ int ll_solve_fused(ll_ctx* ctx, int prerun, int max_iterations, double x_io[7], 
   const int M = ctx->hook_slots;
   cudaStream_t s = ctx->stream;
   SolveArgs sa = solve_args(ctx, M, SOLVE_FUSED, max_iterations);
-  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { sa.table = l1_set_layout(c, M); }));
-  sa.prerun_iterations = prerun; sa.table_mask = l1_set_capacity(M) - 1;
-  sa.cap_check = ctx->hook_cap_check;
+  SolveItem& I = sa.item[0];
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { I.table = l1_set_layout(c, M); }));
+  I.prerun_iterations = prerun; I.table_mask = l1_set_capacity(M) - 1;
+  I.cap_check = ctx->hook_cap_check;
   // a fused launch ends with the ICP termination test: the flag and the iteration totals start afresh for every call
   LL_CUDA(ctx, cudaMemsetAsync(&ctx->d_reg->icp_done, 0, sizeof(int), s));
   LL_CUDA(ctx, cudaMemsetAsync(&ctx->d_reg->total_lm_iterations, 0, 2 * sizeof(int), s));   // total_lm_iterations, total_evaluations
   LL_TRY(hook_solve(ctx, x_io, sa, l1_out));
-  const RegDevState* hs = &ctx->pin->snap[0];
+  const RegDevState* hs = &ctx->pin->snap[0][0];
   for (int k = 0; k < 7; k++) x_io[k] = hs->x[k];
   if (threshold) *threshold = hs->inlier_threshold; if (n_distinct) *n_distinct = hs->n_unique; if (n_kept) *n_kept = hs->num_residual_blocks;
   if (iterations) { iterations[1] = hs->lm.iteration; iterations[0] = hs->total_lm_iterations - hs->lm.iteration; }

@@ -19,27 +19,32 @@ __global__ void bbox_init_kernel(int* bbox);
 __global__ void bbox_kernel(const float4* __restrict__ src, int n, int* __restrict__ bbox);
 
 struct RegDevState;
+// One registration of a batch (ll_register_batch; ll_register is the batch of one): its features are slots off ... off + n_corner + n_surf of
+// the feature arena, corners first.
+struct KnnItem {
+  int off, n_corner, n_surf;
+  int icp_line, icp_plane;
+  int cap, rng_seed;            // residual-block cap (pre-skip of features at 2 x cap, :232-238, :339-345), drawn by the item-local feature index
+  double max_dis_line, max_dis_plane;
+};
 struct KnnBlocksArgs {
   TreeView corner, surf;
-  const float4* feat;     // [n_corner + n_surf] scan-frame features (x,y,z,timestamp)
-  int n_corner, n_surf;
-  const double* pose;     // device: q_curr (w,x,y,z), t_curr
-  double max_dis_line, max_dis_plane;
-  int icp_line, icp_plane;
+  const float4* feat;     // [M] scan-frame features (x,y,z,timestamp), the items one after another
+  int M, n_items;
+  KnnItem item[LL_MAX_BATCH];   // ascending off
   float4* blk_a; double* blk_v;
-  int* corner_avail; int* surf_avail; int* n_blocks;   // three consecutive counters in RegDevState, cleared before every launch
-  int cap, rng_seed;            // residual-block cap (pre-skip of features at 2 x cap, :232-238, :339-345)
   int* seed_ids;                // [M x 5] neighbour ids of the previous ICP iteration (-1 = none): seeds of the next search
   float* knn_d;                 // optional debug output [M x 5]
-  const int* perm;              // spatially sorted feature order (corners then surfaces), or null = caller order
-  int rank, world; ShardGrid grid; const int* shard_owner;   // sharded map: a query is processed by the rank that owns its cell
-  const RegDevState* st;        // motion deblur reads q_last/t_last, t_incre and the Rodrigues terms from here
+  const int* perm;              // spatially sorted feature order (per item: corners then surfaces), or null = caller order
+  int rank, world; ShardGrid grid; const int* shard_owner;   // sharded map (one item): a query is processed by the rank that owns its cell
+  RegDevState* st;              // [n_items]: the pose, the deblur terms, icp_done, and the counters corner_avail / surf_avail / n_blocks
+                                // (cleared before every launch)
   int deblur;
 };
 int launch_knn_query(ll_ctx* ctx, const BucketTree& t, const float4* d_q, int nq, int* d_idx, float* d_d);
 int launch_knn_blocks(ll_ctx* ctx, const KnnBlocksArgs& a);
 int launch_query_sort(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const KnnBlocksArgs& a, int* d_perm);
-size_t query_sort_bytes(int M);
+size_t query_sort_bytes(int M, int n_items);
 
 // ---------------------------------------------------------------------------------------------- solver (solve.cu)
 #include "lm_state.h"   // FnSample, LmState (the state machine itself: lm_core.cuh, included by solve.cu)
@@ -57,6 +62,7 @@ struct RegDevState {
   // residual-block cap: m_maximum_allow_residual_block, the seed of ll_cap_uniform_f, and the number of blocks the kNN kernel of this ICP
   // iteration emitted (n_blocks, next to corner_avail: this rank; n_blocks_all: all ranks, = n_blocks unless the map is sharded)
   int cap, rng_seed, n_blocks_all;
+  int icp_max_iterations;      // solve #2 sets icp_done when icp_iter reaches it: a batch item stops at its own limit while others run on
   // motion deblur (N1): time-stamp range of refine_blur, and compute_interpolatation_rodrigue's outputs (:607-620) after every solve #2
   double min_ts, max_ts, interp_theta, interp_hat[9], interp_hat_sq[9];
   long long prof[16];  // [8..12]: fused K10 section: L1 + insert, barrier, select, barrier, drop   // master-CTA cycle counters of the solver: eval, wait, grid reduce, lm_step, publish, #evaluations, staging, epilogue
@@ -89,8 +95,8 @@ struct FrameDev {
 // async copy is not written again until that copy has completed (every entry point synchronises before it returns; register_device reads
 // snap[it & 1] only after the event recorded behind its copy).
 struct PinnedStage {
-  RegDevState state_in;   // the registration state uploaded by register_device / ll_build_blocks / ll_set_blocks
-  RegDevState snap[2];    // state read-backs: ICP iteration `it` into snap[it & 1]; the solver parity hooks use snap[0]
+  RegDevState state_in[LL_MAX_BATCH];   // the registration states uploaded by register_batch / ll_build_blocks / ll_set_blocks (item order)
+  RegDevState snap[2][LL_MAX_BATCH];    // state read-backs: ICP iteration `it` of every item into snap[it & 1]; the solver parity hooks use snap[0][0]
   double x[7];            // x of the solver parity hooks
   double pose[7];         // ll_transform / ll_transform_dev
   double mapper_pose[7];  // the mapper's world-frame transform of the new features
@@ -104,14 +110,19 @@ struct PinnedStage {
 };
 
 // Grid-wide exchange area of the solver kernels (one per context, device memory, zeroed once at creation; see solve.cu):
-// one tagged 256-byte row per CTA and parity, the broadcast row of the sharded mode, the K10 histograms / candidate list, the generation base.
+// one tagged 256-byte row per CTA and parity, the broadcast row of the sharded mode, per CTA group (batch item) the K10 histograms / candidate
+// list, the generation base.
 #define LL_SYNC_ROWS 160
+struct K10Area {
+  unsigned hist[6][2048]; unsigned list_cnt; unsigned _pad[63];   // K10 radix-select histograms + candidate counter (cleared together by every fused launch)
+  double list[64];
+};
 struct SolveSync {
   double rows[2][LL_SYNC_ROWS][32];   // [parity][cta]: 29 sums, [31] = generation tag (low 32 bits)
   double bcast[2][32];                // world > 1: the all-reduced sums, from CTA 0 to the other CTAs of the rank
-  unsigned hist[6][2048]; unsigned list_cnt; unsigned _pad[63];   // K10 radix-select histograms + candidate counter (cleared together by every fused launch)
-  double list[64];
+  K10Area k10[LL_MAX_BATCH];          // [group]
   unsigned gen;                       // generation base of the next launch; grows monotonically over the life of the context
+  unsigned gen_max, exits;            // launches of several groups: the largest generation any group reached, and the CTAs that have ended
 };
 
 // What one lm_solve_kernel launch does.
@@ -122,24 +133,30 @@ enum SolveMode : int {
   SOLVE_EVALUATE = 3,   // evaluate once at st->x, sums to st->lm.H / g / x_cost (parity hook)
   SOLVE_FUSED = 4,      // one whole ICP iteration in one launch: solve #1 -> K10 inlier threshold -> solve #2 -> pose
 };
+// One item of a solver launch: its slots, its solve, and (filled in by launch_solve) the CTA group that runs it.
+struct SolveItem {
+  int off, M;                // slots off ... off + M of the arrays below
+  int max_iterations;
+  int prerun_iterations;     // SOLVE_FUSED: solve #1's iteration count
+  int cap_check;             // 1: the block count can exceed the cap (host: slots > cap): apply the drop rule (:434-458) while staging
+  unsigned long long* table; unsigned table_mask;   // SOLVE_FUSED: the hash set of the item's L1 norms (K10)
+  int first, n_cta, tile, tiles_per_cta;            // CTAs first ... first + n_cta - 1; `tile` slots per CTA and pass (batch_grid)
+};
 struct SolveArgs {
-  RegDevState* st;
+  RegDevState* st;           // [n_items]
   SolveSync* sync;
-  const float4* feat;        // [M] scan-frame points
-  const float4* blk_a;       // [M] (a.xyz, type)
-  const double* blk_v;       // [M*3]
-  double* l1;                // [M] loss-corrected L1 norm per slot (+inf for invalid slots)
+  const float4* feat;        // [slots] scan-frame points
+  const float4* blk_a;       // [slots] (a.xyz, type)
+  const double* blk_v;       // [slots*3]
+  double* l1;                // [slots] loss-corrected L1 norm per slot (+inf for invalid slots)
   const double* k10_value;   // SOLVE_SECOND: the K10 order statistic and distinct count (launch_k10_select) for the threshold of solve #2
   const int* k10_n_distinct;
-  int M;
-  int max_iterations;
   SolveMode mode;
-  // multi-GPU
+  // multi-GPU (one item)
   int rank, world; double* comm_local; double* comm_peer[8];
-  // SOLVE_FUSED: solve #1's iteration count and the hash set of the L1 norms (K10)
-  int prerun_iterations; unsigned long long* table; unsigned table_mask;
-  int cap_check;             // 1: the block count can exceed the cap (host: slots > cap): apply the drop rule (:434-458) while staging
   int deblur;                // 1: *_mb functors (ceres_icp.hpp:81-233), s per block from the feature's time stamp
+  int n_items;               // 1 ... LL_MAX_BATCH; more than one only in SOLVE_FUSED
+  SolveItem item[LL_MAX_BATCH];
 };
 // Layout of the IPC-exported staging buffer of a rank (ll_comm_local_handle):
 //   [0, 8192)            2 parities x 8 ranks x 64 doubles: the 29 sums of one evaluation + a generation flag at double index 32
@@ -150,9 +167,10 @@ struct SolveArgs {
 #define LL_COMM_CTRL_OFF 8192
 #define LL_COMM_X_OFF 16384
 int launch_solve(ll_ctx* ctx, const SolveArgs& a);
-// LL_OK when M residual-block slots fit the shared memory of the solver's CTAs (deblur: the *_mb slot layout), else LL_ERR_CAPACITY with the
-// context's error set.  The one copy of the rule launch_solve applies: callers check with it before they enqueue anything.
-int solve_capacity(ll_ctx* ctx, int M, int deblur);
+// LL_OK when the residual-block slots M[0 .. n) of a launch's items fit the shared memory of their CTA groups (deblur: the *_mb slot layout),
+// else LL_ERR_CAPACITY with the context's error set and *bad_item (may be null) = the first item that does not fit.  The one copy of the rule
+// launch_solve applies: callers check with it before they enqueue anything.
+int solve_capacity(ll_ctx* ctx, int n, const int* M, int deblur, int* bad_item = nullptr);
 int solve_prepare(ll_ctx* ctx);   // once per context: opt the solver kernels in to their dynamic shared memory
 // The fused solver's K10 (grid-wide de-duplication + radix select) over n values, +inf / NaN skipped; *d_value, *d_n_distinct on the device.
 // The sharded mode's select over the exchanged L1 norms, and the parity hook ll_inlier_select.
@@ -197,6 +215,7 @@ int launch_gather_pieces(ll_ctx* ctx, cudaStream_t s, FrameDev* dev, const Frame
                          const float4* src_c, const float4* src_s, float4* dst_c, float4* dst_s);
 
 // ---------------------------------------------------------------------------------------------- host driver pieces (api.cu)
+// Registration of the features already resident in A.feat (corners then surfaces): the batch of one.  Core of ll_register / ll_scan_to_pose.
 int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg_state* in, ll_reg_result* out);
 int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);
 // The device arrays of a piecewise frame front end (owned by the streaming mapper): gathered segments of cap points per class, the first

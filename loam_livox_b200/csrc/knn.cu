@@ -343,30 +343,42 @@ __global__ void __launch_bounds__(KNN_THREADS) knn_query_kernel(TreeView tv, con
   if (have && lane < LL_KNN) { idx5[g * LL_KNN + lane] = (t.id == 0x7fffffff) ? -1 : t.id; d5[g * LL_KNN + lane] = t.d; }
 }
 
-// Spatial sort key of a feature at the current pose: class bit (corner/surface) | 21-bit Hilbert index (7 bits per axis) inside the tree's box.
-// Neighbouring queries then sit in the same warp / CTA, walk the same tree nodes and buckets, and hit them in L1.
+// The batch item whose slots hold feature w (items are laid out one after another in ascending off).
+__device__ __forceinline__ int knn_item_of(const KnnBlocksArgs& a, int w) {
+  int it = 0;
+  while (it + 1 < a.n_items && w >= a.item[it + 1].off) it++;
+  return it;
+}
+// Bits of the batch item index on top of the query sort key (0 for a single registration: the key, and so the sort, are the single call's).
+static int item_key_bits(int n_items) { int b = 0; while ((1 << b) < n_items) b++; return b; }
+
+// Spatial sort key of a feature at its item's current pose: item index | class bit (corner/surface) | 21-bit Hilbert index (7 bits per axis)
+// inside the tree's box.  Neighbouring queries then sit in the same warp / CTA, walk the same tree nodes and buckets, and hit them in L1.
 __global__ void query_key_kernel(KnnBlocksArgs a, unsigned* __restrict__ keys, int* __restrict__ vals) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int M = a.n_corner + a.n_surf;
-  if (i >= M) return;
-  const bool is_corner = i < a.n_corner;
+  if (i >= a.M) return;
+  const int it = knn_item_of(a, i);
+  const bool is_corner = i - a.item[it].off < a.item[it].n_corner;
+  const double* pose = a.st[it].pose_curr;
   const float4 f = __ldg(&a.feat[i]);
-  double wx, wy, wz; qrot_d(a.pose, (double)f.x, (double)f.y, (double)f.z, wx, wy, wz);
-  const float c[3] = {(float)(wx + a.pose[4]), (float)(wy + a.pose[5]), (float)(wz + a.pose[6])};
+  double wx, wy, wz; qrot_d(pose, (double)f.x, (double)f.y, (double)f.z, wx, wy, wz);
+  const float c[3] = {(float)(wx + pose[4]), (float)(wy + pose[5]), (float)(wz + pose[6])};
   const float* bb = is_corner ? a.corner.bbox : a.surf.bbox;   // device memory: the box never visits the host
   // 7 bits per axis: 21-bit curve + class bit = 3 radix passes, and tiles of ~0.3 m are fine enough; non-finite features sort last in their class
   const unsigned h = (isfinite(c[0]) && isfinite(c[1]) && isfinite(c[2])) ? (unsigned)hilbert_key(c, bb, bb + 3, 7) : 0x1fffffu;
-  keys[i] = (is_corner ? 0u : 0x200000u) | h; vals[i] = i;
+  keys[i] = ((unsigned)it << 22) | (is_corner ? 0u : 0x200000u) | h; vals[i] = i;
 }
 
-// Gates + functor constructors (K7) for one feature whose 5 nearest neighbours are id[0..4] (d4 = the 5th squared distance); lane 0 writes slot `w`.
-__device__ __forceinline__ void emit_block(const KnnBlocksArgs& a, const TreeView& tv, bool is_corner, bool active, int w, int id0, int id1, int id2, int id4, float d4) {
+// Gates + functor constructors (K7) for one feature of item I whose 5 nearest neighbours are id[0..4] (d4 = the 5th squared distance); lane 0
+// writes slot `w` and counts into the item's state st.
+__device__ __forceinline__ void emit_block(const KnnBlocksArgs& a, const KnnItem& I, RegDevState* st, const TreeView& tv, bool is_corner, bool active, int w,
+                                           int id0, int id1, int id2, int id4, float d4) {
   int type = 0; double ax = 0, ay = 0, az = 0, vx = 0, vy = 0, vz = 0;
   if (active) {
     const bool found5 = id4 != 0x7fffffff;
     if (is_corner) {
-      if (found5 && (double)d4 < a.max_dis_line) {
-        if (a.icp_line) {
+      if (found5 && (double)d4 < I.max_dis_line) {
+        if (I.icp_line) {
           const float4 p1 = __ldg(&tv.src[id0]), p2 = __ldg(&tv.src[id1]);
           double d0 = (double)p1.x - (double)p2.x, d1 = (double)p1.y - (double)p2.y, d2 = (double)p1.z - (double)p2.z;
           double dn = sqrt(d0 * d0 + d1 * d1 + d2 * d2);
@@ -375,13 +387,13 @@ __device__ __forceinline__ void emit_block(const KnnBlocksArgs& a, const TreeVie
             double u0 = (double)p2.x - (double)p1.x, u1 = (double)p2.y - (double)p1.y, u2 = (double)p2.z - (double)p1.z;
             double n = sqrt(u0 * u0 + u1 * u1 + u2 * u2);
             vx = u0 / n; vy = u1 / n; vz = u2 / n; ax = p1.x; ay = p1.y; az = p1.z; type = 1;
-            atomicAdd(a.corner_avail, 1);
+            atomicAdd(&st->corner_avail, 1);
           }
         }
       }
     } else {
-      if (found5 && (double)d4 < a.max_dis_plane) {
-        if (a.icp_plane) {
+      if (found5 && (double)d4 < I.max_dis_plane) {
+        if (I.icp_plane) {
           const float4 pa = __ldg(&tv.src[id0]), pb = __ldg(&tv.src[id2]), pc = __ldg(&tv.src[id4]);
           double b0 = (double)pb.x - (double)pa.x, b1 = (double)pb.y - (double)pa.y, b2 = (double)pb.z - (double)pa.z;
           double nb = sqrt(b0 * b0 + b1 * b1 + b2 * b2); b0 = b0 / nb; b1 = b1 / nb; b2 = b2 / nb;
@@ -390,36 +402,40 @@ __device__ __forceinline__ void emit_block(const KnnBlocksArgs& a, const TreeVie
           vx = b1 * c2 - b2 * c1; vy = b2 * c0 - b0 * c2; vz = b0 * c1 - b1 * c0;   // NOT re-normalised (ceres_icp.hpp:334)
           ax = pa.x; ay = pa.y; az = pa.z; type = 2;
         }
-        atomicAdd(a.surf_avail, 1);
+        atomicAdd(&st->surf_avail, 1);
       }
     }
   }
-  if (type != 0) atomicAdd(a.n_blocks, 1);   // residual_block_ids.size() of this ICP iteration (the cap's drop rule needs it, :436)
+  if (type != 0) atomicAdd(&st->n_blocks, 1);   // residual_block_ids.size() of this ICP iteration (the cap's drop rule needs it, :436)
   a.blk_a[w] = make_float4((float)ax, (float)ay, (float)az, __int_as_float(type));
   a.blk_v[(size_t)w * 3 + 0] = vx; a.blk_v[(size_t)w * 3 + 1] = vy; a.blk_v[(size_t)w * 3 + 2] = vz;
 }
 
-// K6 + K7 fused, one warp per scan feature, features taken in spatially sorted order (perm).
+// K6 + K7 fused, one warp per scan feature, features taken in spatially sorted order (perm), each against the pose of its batch item.
 // Writes one residual-block slot per feature (indexed by the ORIGINAL feature order): blk_a[slot] = (a.x, a.y, a.z, type) with
 // type 0 invalid / 1 line / 2 plane, blk_v[slot*3..] = unit line direction or (un-normalised) plane normal, in fp64.
-__global__ void __launch_bounds__(KNN_THREADS) knn_blocks_kernel(KnnBlocksArgs a) {
-  if (a.st->icp_done) return;   // launched ahead of the termination test by the host: the ICP loop has already ended
+// (5 CTAs of 256 threads per SM: at most 48 registers.  The search is latency-bound; one register more is 56 with the allocation granularity,
+// 4 CTAs per SM, and the kernel ~9 % slower on an H100.)
+__global__ void __launch_bounds__(KNN_THREADS, 5) knn_blocks_kernel(KnnBlocksArgs a) {
   __shared__ WarpWalk walks[WARPS_PER_CTA];
   const int j = blockIdx.x * WARPS_PER_CTA + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  const int M = a.n_corner + a.n_surf;
-  const bool have = j < M;
-  const int w = have ? (a.perm ? a.perm[j] : j) : 0;      // original feature index
-  const bool is_corner = w < a.n_corner;
+  if (j >= a.M) return;
+  const int w = a.perm ? a.perm[j] : j;      // original feature index
+  const int it = knn_item_of(a, w);
+  const KnnItem& I = a.item[it];
+  RegDevState* st = a.st + it;
+  if (st->icp_done) return;   // (warp-uniform) launched ahead of the termination test by the host: this item's ICP loop has already ended
+  const int lw = w - I.off;   // item-local feature index
+  const bool is_corner = lw < I.n_corner;
   const TreeView& tv = is_corner ? a.corner : a.surf;
-  float4 f = make_float4(0.f, 0.f, 0.f, 0.f); if (have) f = __ldg(&a.feat[w]);
+  const float4 f = __ldg(&a.feat[w]);
   // pointAssociateToMap (non-deblur branch): p_w = q_curr * p + t_curr in fp64, stored as fp32
-  const double* qc = a.pose; const double* tc = a.pose + 4;
+  const double* qc = st->pose_curr; const double* tc = st->pose_curr + 4;
   double wx, wy, wz; qrot_d(qc, (double)f.x, (double)f.y, (double)f.z, wx, wy, wz);
   float qx = (float)(wx + tc[0]), qy = (float)(wy + tc[1]), qz = (float)(wz + tc[2]);
   if (a.deblur) {
     // pointAssociateToMap, deblur branch (:627-654, if_undistore_in_matching = 1): Rodrigues-interpolated increment applied before q_last
-    const RegDevState* st = a.st;
     const double is = (double)refine_blur_f(f.w, (float)st->min_ts, (float)st->max_ts);
     if (is != 1.0) {
       const double th = st->interp_theta * is; double sn, cs; sincos(th, &sn, &cs); const double oc = 1.0 - cs;
@@ -441,19 +457,18 @@ __global__ void __launch_bounds__(KNN_THREADS) knn_blocks_kernel(KnnBlocksArgs a
   // Residual-block cap, pre-skip (:232-238 corners, :339-345 surfaces): with N features of this class and N > 2 cap, a feature is skipped when
   // rand * N > 2 cap (float arithmetic, like m_rand_float), before it is transformed or searched.  Drawn per (seed, ICP iteration, class, index).
   bool skipped = false;
-  { const int ncls = is_corner ? a.n_corner : a.n_surf;
-    if (have && ncls > 2 * a.cap) skipped = ll_cap_uniform_f(a.rng_seed, a.st->icp_iter, is_corner ? 0 : 1, is_corner ? w : w - a.n_corner) * (float)ncls > (float)(2 * a.cap); }
-  const bool active = have && owned && finite_in && !skipped;
+  { const int ncls = is_corner ? I.n_corner : I.n_surf;
+    if (ncls > 2 * I.cap) skipped = ll_cap_uniform_f(I.rng_seed, st->icp_iter, is_corner ? 0 : 1, is_corner ? lw : lw - I.n_corner) * (float)ncls > (float)(2 * I.cap); }
+  const bool active = owned && finite_in && !skipped;
   LaneTop t;
-  warp_knn5(tv, walks[threadIdx.x >> 5], active, qx, qy, qz, t, (a.seed_ids && have) ? a.seed_ids + (size_t)w * LL_KNN : nullptr);
-  if (!have) return;
+  warp_knn5(tv, walks[threadIdx.x >> 5], active, qx, qy, qz, t, a.seed_ids ? a.seed_ids + (size_t)w * LL_KNN : nullptr);
   if (active && lane < LL_KNN) {   // the neighbours seed the next ICP iteration's search (5 lanes, one 20-byte row)
     if (a.seed_ids) a.seed_ids[(size_t)w * LL_KNN + lane] = (t.id == 0x7fffffff) ? -1 : t.id;
     if (a.knn_d) a.knn_d[(size_t)w * LL_KNN + lane] = t.d;
   }
   const int id0 = __shfl_sync(FULL, t.id, 0), id1 = __shfl_sync(FULL, t.id, 1), id2 = __shfl_sync(FULL, t.id, 2);
   if (lane != 0) return;
-  emit_block(a, tv, is_corner, active, w, id0, id1, id2, t.id5, t.d5);
+  emit_block(a, I, st, tv, is_corner, active, w, id0, id1, id2, t.id5, t.d5);
 }
 
 int launch_knn_query(ll_ctx* ctx, const BucketTree& t, const float4* d_q, int nq, int* d_idx, float* d_d) {
@@ -462,26 +477,28 @@ int launch_knn_query(ll_ctx* ctx, const BucketTree& t, const float4* d_q, int nq
   LL_CUDA(ctx, cudaGetLastError());
   return LL_OK;
 }
-// Sorts the features spatially (once per registration, at the initial pose): perm[] lists corner features then surface features.
-// keys | keys_out | vals | CUB temp (the sorted values go to perm)
+// Sorts the features spatially (once per registration, at the initial poses): perm[] lists, item after item, corner features then surface
+// features.  keys | keys_out | vals | CUB temp (the sorted values go to perm)
 struct QuerySortLayout {
-  size_t tmp_bytes = 0; unsigned* k0; unsigned* k1; int* v0; char* tmp;
-  explicit QuerySortLayout(int M) { cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, M, 0, 22); }
+  size_t tmp_bytes = 0; unsigned* k0; unsigned* k1; int* v0; char* tmp; int end_bit;
+  QuerySortLayout(int M, int n_items) : end_bit(22 + item_key_bits(n_items)) {
+    cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, M, 0, end_bit);
+  }
   void layout(Carve& c, int M) { k0 = c.take<unsigned>(M); k1 = c.take<unsigned>(M); v0 = c.take<int>(M); tmp = c.take<char>(tmp_bytes); }
 };
-size_t query_sort_bytes(int M) { QuerySortLayout q(M); return layout_bytes([&](Carve& c) { q.layout(c, M); }); }
+size_t query_sort_bytes(int M, int n_items) { QuerySortLayout q(M, n_items); return layout_bytes([&](Carve& c) { q.layout(c, M); }); }
 int launch_query_sort(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const KnnBlocksArgs& a, int* d_perm) {
-  const int M = a.n_corner + a.n_surf;
+  const int M = a.M;
   if (M == 0) return LL_OK;
-  QuerySortLayout q(M);
+  QuerySortLayout q(M, a.n_items);
   LL_CUDA(ctx, scratch.carve([&](Carve& c) { q.layout(c, M); }));
   query_key_kernel<<<ll_div_up(M, 256), 256, 0, s>>>(a, q.k0, q.v0);
-  LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(q.tmp, q.tmp_bytes, q.k0, q.k1, q.v0, d_perm, M, 0, 22, s));
+  LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(q.tmp, q.tmp_bytes, q.k0, q.k1, q.v0, d_perm, M, 0, q.end_bit, s));
   ctx->launches += 4;
   return LL_OK;
 }
 int launch_knn_blocks(ll_ctx* ctx, const KnnBlocksArgs& a) {
-  int M = a.n_corner + a.n_surf;
+  const int M = a.M;
   if (M == 0) return LL_OK;
   knn_blocks_kernel<<<ll_div_up(M, WARPS_PER_CTA), KNN_THREADS, 0, ctx->stream>>>(a);
   ctx->launches++;

@@ -108,7 +108,7 @@ static int mapper_reserve(ll_ctx* ctx, ll_mapper* m) {
   // the same way).  scratch alone: the registration's query sort and K10 hash set.
   size_t side = voxel_grid_bytes(F);
   if (R) side = std::max(side, std::max(voxel_grid_bytes((int)R), tree_scratch_bytes((int)R)));
-  const size_t reg = std::max(query_sort_bytes(F), layout_bytes([&](Carve& c) { l1_set_layout(c, F); }));
+  const size_t reg = std::max(query_sort_bytes(F, 1), layout_bytes([&](Carve& c) { l1_set_layout(c, F); }));
   LL_CUDA(ctx, ctx->scratch.reserve_floor(std::max(side, reg)));
   LL_CUDA(ctx, ctx->scratch2.reserve_floor(side));
   if (!R) return LL_OK;

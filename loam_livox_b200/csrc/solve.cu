@@ -13,6 +13,7 @@
 // order, so every CTA holds bit-identical sums and advances its own copy of the trust-region state.  SOLVE_FUSED runs a whole ICP iteration
 // in one launch: solve #1, the L1 norms, K10's inlier threshold over the grid (hash-set de-duplication + radix select), the outlier drop,
 // solve #2 and the pose.  No host round trip inside a launch.
+#include <algorithm>
 #include <cfloat>
 #include <cstdlib>
 #include "common.cuh"
@@ -215,6 +216,9 @@ __device__ __forceinline__ SmemSlots carve(unsigned char* base, int cap, bool mb
 // and reduces the rows itself in fixed order -- bit-identical sums everywhere, so every CTA advances its own copy of the solver state and there is
 // no publish step.  Rows are double-buffered by generation parity: a CTA can be at most one exchange ahead of the slowest one.  Generations grow
 // monotonically over the life of the context (SolveSync::gen is never reset), so a stale tag can never match.
+// A launch may cut its grid into CTA groups (one per batch item, SolveArgs::item): a group exchanges over its own rows (CTAs first ... first +
+// n - 1) and counts its own generations; rows of different groups never meet.
+struct CtaGroup { int first, n; };
 __device__ __forceinline__ double* sync_row(SolveSync* Y, unsigned gen, int cta) { return Y->rows[gen & 1u][cta]; }
 // Called by one thread after a warp or CTA barrier that follows the writes it publishes (the CTA's row, K10's histogram atomics).  The release is
 // cumulative: it orders every write the barrier made this thread observe, so no separate fence is needed (a __threadfence here is a sequentially
@@ -222,16 +226,28 @@ __device__ __forceinline__ double* sync_row(SolveSync* Y, unsigned gen, int cta)
 __device__ __forceinline__ void sync_arrive(SolveSync* Y, unsigned gen) {
   st_release_u32((unsigned*)(sync_row(Y, gen, blockIdx.x) + 31), gen);
 }
-__device__ __forceinline__ void sync_wait_all(SolveSync* Y, unsigned gen) {   // CTA-collective
-  if (threadIdx.x < gridDim.x) { const unsigned* f = (const unsigned*)(sync_row(Y, gen, threadIdx.x) + 31); while (ld_acquire_u32(f) != gen) {} }
+__device__ __forceinline__ void sync_wait_all(SolveSync* Y, unsigned gen, CtaGroup g) {   // CTA-collective
+  if (threadIdx.x < g.n) { const unsigned* f = (const unsigned*)(sync_row(Y, gen, g.first + threadIdx.x) + 31); while (ld_acquire_u32(f) != gen) {} }
   __syncthreads();
 }
-// plain barrier (no payload)
-__device__ __forceinline__ void grid_sync(SolveSync* Y, unsigned& gen) {
+// plain barrier of the group (no payload)
+__device__ __forceinline__ void grid_sync(SolveSync* Y, unsigned& gen, CtaGroup g) {
   gen++;
   __syncthreads();
   if (threadIdx.x == 0) sync_arrive(Y, gen);
-  sync_wait_all(Y, gen);
+  sync_wait_all(Y, gen, g);
+}
+// End of a launch, thread 0 of every CTA: hand the generation base to the next launch (stream-ordered).  One group: every CTA ended with the same
+// `gen`, CTA 0 stores it.  Several groups end at different generations, and a CTA of a slow group may not yet have read the base when a fast
+// group ends: the base must only move once every CTA has ended, so the last CTA to end stores the largest generation any group reached.
+__device__ __forceinline__ void hand_over_gen(SolveSync* Y, unsigned gen, int n_groups) {
+  if (n_groups == 1) { if (blockIdx.x == 0) *((volatile unsigned*)&Y->gen) = gen; return; }
+  atomicMax(&Y->gen_max, gen);
+  __threadfence();
+  if (atomicAdd(&Y->exits, 1u) == gridDim.x - 1) {
+    Y->exits = 0u;
+    *((volatile unsigned*)&Y->gen) = atomicMax(&Y->gen_max, 0u);
+  }
 }
 
 // K10 (compute_inlier_residual_threshold, :153-161) spread over the grid: de-duplicate the per-block L1 norms (std::set<double>), take element
@@ -258,18 +274,21 @@ __device__ __forceinline__ bool l1_set_insert_flag(unsigned long long* __restric
 __device__ __forceinline__ double k10_threshold(double inliner_dis, double value, int n_distinct) { return fmax(inliner_dis, n_distinct > 0 ? value : 0.0); }
 struct K10Smem { unsigned hist[2048]; unsigned warp_sum[SOLVE_THREADS / 32 + 1]; unsigned long long prefix, mask; int k, cnt_bin, n_distinct, done; int scratch[40]; double result; };
 
-// Clear the hash set of the L1 norms and the K10 histograms / candidate counter; a grid exchange must follow before any insert.
-__device__ __forceinline__ void k10_clear(unsigned long long* table, unsigned table_mask, SolveSync* Y) {
-  for (unsigned idx = blockIdx.x * SOLVE_THREADS + threadIdx.x; idx <= table_mask; idx += gridDim.x * SOLVE_THREADS) table[idx] = L1_EMPTY;
-  for (unsigned idx = blockIdx.x * SOLVE_THREADS + threadIdx.x; idx < K10_PASSES * 2048u + 64u; idx += gridDim.x * SOLVE_THREADS) ((unsigned*)Y->hist)[idx] = 0u;   // hist + list_cnt + pad
+// Clear the group's hash set of the L1 norms and its K10 histograms / candidate counter; a group exchange must follow before any insert.
+__device__ __forceinline__ void k10_clear(unsigned long long* table, unsigned table_mask, K10Area* K, CtaGroup g) {
+  const unsigned cta = blockIdx.x - g.first, stride = (unsigned)g.n * SOLVE_THREADS;
+  for (unsigned idx = cta * SOLVE_THREADS + threadIdx.x; idx <= table_mask; idx += stride) table[idx] = L1_EMPTY;
+  for (unsigned idx = cta * SOLVE_THREADS + threadIdx.x; idx < K10_PASSES * 2048u + 64u; idx += stride) ((unsigned*)K->hist)[idx] = 0u;   // hist + list_cnt + pad
 }
 
 // The element of rank min(floor(ratio * n), n - 1) among the n DISTINCT values l1[i] of the slots whose flag (bit 8 of type[li], shared memory)
 // says this thread represents the value.  Radix select on the bit patterns (non-negative doubles order like their bits), 11-bit digits from the
-// exponent down: per pass every CTA histograms the distinct values it represents (shared memory), adds its non-empty bins to the global
+// exponent down: per pass every CTA histograms the distinct values it represents (shared memory), adds its non-empty bins to the group's
 // histogram, one exchange, and every CTA finds the bin of the wanted rank in the same histogram.  When that bin holds <= 64 values they are
-// collected and ranked directly.  Grid-collective; ends with s_k10.n_distinct and s_k10.result (valid when n_distinct > 0) on every CTA.
-__device__ __forceinline__ void k10_select(K10Smem& s_k10, SolveSync* Y, unsigned& gen, const int* type, const double* l1, int M, int tiles_per_cta, int tile, const double* ratio) {
+// collected and ranked directly.  Group-collective; ends with s_k10.n_distinct and s_k10.result (valid when n_distinct > 0) on every CTA.
+__device__ __forceinline__ void k10_select(K10Smem& s_k10, SolveSync* Y, K10Area* K, CtaGroup g, unsigned& gen, const int* type, const double* l1, int M, int tiles_per_cta,
+                                           int tile, const double* ratio) {
+  const int cta = blockIdx.x - g.first;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (tid == 0) { s_k10.prefix = 0ull; s_k10.mask = 0ull; s_k10.k = -1; s_k10.done = 0; s_k10.result = 0.0; }
   __syncthreads();
@@ -279,16 +298,16 @@ __device__ __forceinline__ void k10_select(K10Smem& s_k10, SolveSync* Y, unsigne
     __syncthreads();
     const unsigned long long prefix = s_k10.prefix, himask = s_k10.mask;
     for (int k = 0; k < tiles_per_cta; k++) {
-      const int i = (blockIdx.x + gridDim.x * k) * tile + tid, li = k * SOLVE_THREADS + tid;
+      const int i = (cta + g.n * k) * tile + tid, li = k * SOLVE_THREADS + tid;
       if (i < M && tid < tile && (type[li] & 0x100)) {
         const unsigned long long key = l1_key(l1[i]);
         if ((key & himask) == prefix) atomicAdd(&s_k10.hist[(unsigned)(key >> shift) & dmask], 1u);
       }
     }
     __syncthreads();
-    unsigned* gh = Y->hist[pass];
+    unsigned* gh = K->hist[pass];
     for (int b = tid; b < 2048; b += SOLVE_THREADS) { const unsigned c = s_k10.hist[b]; if (c) atomicAdd(&gh[b], c); }
-    grid_sync(Y, gen);
+    grid_sync(Y, gen, g);
     // every CTA: exclusive scan of the global histogram, find the bin that holds rank k
     constexpr int BPT = 2048 / SOLVE_THREADS;
     unsigned h[BPT], run = 0;
@@ -324,17 +343,17 @@ __device__ __forceinline__ void k10_select(K10Smem& s_k10, SolveSync* Y, unsigne
         // collect the members of the bin (<= 64 distinct values, or all equal in their 63 bits: then any of them is the answer) and rank them
         const unsigned long long pf = s_k10.prefix, hm = s_k10.mask;
         for (int kk = 0; kk < tiles_per_cta; kk++) {
-          const int i = (blockIdx.x + gridDim.x * kk) * tile + tid, li = kk * SOLVE_THREADS + tid;
+          const int i = (cta + g.n * kk) * tile + tid, li = kk * SOLVE_THREADS + tid;
           if (i < M && tid < tile && (type[li] & 0x100)) {
             const double v = l1[i];
-            if ((l1_key(v) & hm) == pf) { const unsigned slot = atomicAdd(&Y->list_cnt, 1u); if (slot < 64u) Y->list[slot] = v; }
+            if ((l1_key(v) & hm) == pf) { const unsigned slot = atomicAdd(&K->list_cnt, 1u); if (slot < 64u) K->list[slot] = v; }
           }
         }
-        grid_sync(Y, gen);
+        grid_sync(Y, gen, g);
         {   // rank the <= 64 collected values: one value per thread out of shared memory (distinct values: exactly one has the wanted rank)
           double* cand = (double*)s_k10.hist;
-          const int m = min((int)*((volatile unsigned*)&Y->list_cnt), 64);
-          if (tid < m) cand[tid] = __ldcg(&Y->list[tid]);
+          const int m = min((int)*((volatile unsigned*)&K->list_cnt), 64);
+          if (tid < m) cand[tid] = __ldcg(&K->list[tid]);
           __syncthreads();
           if (tid < m) { const double mine = cand[tid]; int rank = 0; for (int q = 0; q < m; q++) rank += (cand[q] < mine) ? 1 : 0; if (rank == s_k10.k) s_k10.result = mine; }
           if (tid == 0) s_k10.done = 1;
@@ -345,8 +364,10 @@ __device__ __forceinline__ void k10_select(K10Smem& s_k10, SolveSync* Y, unsigne
   }
 }
 
-template <bool MB>
-__global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a, int tiles_per_cta, int tile) {
+// BATCH: the launch has several items (CTA groups).  A launch of one item is the instance without: its group is the whole grid, its slots start
+// at 0 and its fields are plain kernel parameters, as in a launch that knows nothing of batches.
+template <bool MB, bool BATCH>
+__global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a) {
   extern __shared__ __align__(16) unsigned char s_dyn[];
   __shared__ EvalConst E;
   __shared__ double s_red[SOLVE_THREADS / 32][NSUM + 1];
@@ -357,14 +378,28 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   __shared__ K10Smem s_k10;    // SOLVE_FUSED only
   __shared__ long long s_prof[16];   // the master CTA's cycle counters, added to RegDevState::prof once at the end: a global read-modify-write per
                                      // evaluation would put an L2 round trip on the master's path, and every other CTA waits for the master's row
-  RegDevState* st = a.st;
+  // this CTA's item: its group of CTAs, its slots (item-local index i = slot - off), its state
+  int item = 0;
+  if (BATCH) while (item + 1 < a.n_items && (int)blockIdx.x >= a.item[item + 1].first) item++;
+  const SolveItem& I = a.item[item];
+  const CtaGroup grp = {BATCH ? I.first : 0, BATCH ? I.n_cta : (int)gridDim.x};
+  const int cta = BATCH ? (int)blockIdx.x - grp.first : (int)blockIdx.x, tiles_per_cta = I.tiles_per_cta, tile = I.tile, M = I.M;
+  const int off = BATCH ? I.off : 0;
+  const float4* feat = a.feat + off; const float4* blk_a = a.blk_a + off; const double* blk_v = a.blk_v + (size_t)off * 3; double* l1 = a.l1 + off;
+  RegDevState* st = a.st + item;
   SolveSync* Y = a.sync;
-  if ((a.mode == SOLVE_FUSED || a.mode <= SOLVE_SECOND) && *((volatile int*)&st->icp_done)) return;   // ICP work (fused, solve #1 or #2) launched after the ICP loop ended (uniform over the grid)
+  K10Area* K = &Y->k10[item];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int n_groups = BATCH ? a.n_items : 1;
+  // ICP work (fused, solve #1 or #2) launched after the item's ICP loop ended (uniform over the group)
+  if ((a.mode == SOLVE_FUSED || a.mode <= SOLVE_SECOND) && *((volatile int*)&st->icp_done)) {
+    if (BATCH && tid == 0) hand_over_gen(Y, *((volatile unsigned*)&Y->gen), n_groups);   // (one group: the base stays where it is)
+    return;
+  }
   const int cap = tiles_per_cta * SOLVE_THREADS;
   const SmemSlots S = carve(s_dyn, cap, MB);
-  const bool master = blockIdx.x == 0;   // the CTA that writes results back to RegDevState and talks to the peers (nothing waits for it otherwise)
-  unsigned gen = *((volatile unsigned*)&Y->gen);   // uniform over the grid: written by the previous launch's CTA 0 at its very end
+  const bool master = cta == 0;   // the CTA that writes results back to RegDevState and talks to the peers (nothing waits for it otherwise)
+  unsigned gen = *((volatile unsigned*)&Y->gen);   // uniform over the grid: written at the very end of the previous launch (hand_over_gen)
   if (tid < 16) s_prof[tid] = 0;
 
   const long long t_k0 = clock64();
@@ -373,7 +408,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   // exchange orders the clear before any insert.
   const bool fused = a.mode == SOLVE_FUSED;
   SolveMode cur_mode = fused ? SOLVE_FIRST : a.mode;
-  if (fused) k10_clear(a.table, a.table_mask, Y);
+  if (fused) k10_clear(I.table, I.table_mask, K, grp);
   // ---- stage this CTA's residual blocks
   double thr = 0;
   if (a.mode == SOLVE_SECOND) {   // K10 tail: the threshold from the order statistic and distinct count launch_k10_select left on the device
@@ -382,22 +417,22 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   }
   // Residual-block cap, drop rule (:434-458): with M blocks and M > cap, block i leaves the problem when rand_i > (float)cap / (float)M.
   float cap_keep = 2.0f; int cap_iter = 0, cap_seed = 0;
-  if (a.cap_check) {
+  if (I.cap_check) {
     const int nb = a.world > 1 ? st->n_blocks_all : st->n_blocks;
     if (nb > st->cap) cap_keep = (float)st->cap / (float)nb;
     cap_iter = st->icp_iter; cap_seed = st->rng_seed;
   }
   for (int k = 0; k < tiles_per_cta; k++) {
-    const int i = (blockIdx.x + gridDim.x * k) * tile + tid, li = k * SOLVE_THREADS + tid;   // tile <= SOLVE_THREADS slots per CTA and pass: threads >= tile idle
+    const int i = (cta + grp.n * k) * tile + tid, li = k * SOLVE_THREADS + tid;   // tile <= SOLVE_THREADS slots per CTA and pass: threads >= tile idle
     int type = 0;
-    if (i < a.M && tid < tile) {
-      const float4 ba = a.blk_a[i]; type = __float_as_int(ba.w);
+    if (i < M && tid < tile) {
+      const float4 ba = blk_a[i]; type = __float_as_int(ba.w);
       if (type != 0 && cap_keep <= 1.0f && ll_cap_uniform_f(cap_seed, cap_iter, 2, i) > cap_keep) type = 0;
-      if (type != 0 && a.mode == SOLVE_SECOND && (a.l1[i] > thr)) type = 0;
+      if (type != 0 && a.mode == SOLVE_SECOND && (l1[i] > thr)) type = 0;
       if (type != 0) {
-        const float4 f = a.feat[i];
+        const float4 f = feat[i];
         S.p[0][li] = f.x; S.p[1][li] = f.y; S.p[2][li] = f.z;
-        const double v0 = a.blk_v[(size_t)i * 3], v1 = a.blk_v[(size_t)i * 3 + 1], v2 = a.blk_v[(size_t)i * 3 + 2];
+        const double v0 = blk_v[(size_t)i * 3], v1 = blk_v[(size_t)i * 3 + 1], v2 = blk_v[(size_t)i * 3 + 2];
         if (MB) {
           S.a[0][li] = ba.x; S.a[1][li] = ba.y; S.a[2][li] = ba.z; S.v[0][li] = v0; S.v[1][li] = v1; S.v[2][li] = v2;
           S.s[li] = refine_blur_f(f.w, (float)st->min_ts, (float)st->max_ts);   // refine_blur(pointOri.intensity, ...) * 1.0 (:309, :407)
@@ -422,7 +457,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
     if (ph == 0) setup_static(E, st);
     setup_trial<MB>(E, tr);
     LmState& L = s_lm;
-    L.phase = 0; L.iteration = 0; L.max_iterations = (fused && ph == 0) ? a.prerun_iterations : a.max_iterations; L.num_invalid = 0; L.done = 0; L.termination = 0; L.last_successful = 1; L.reuse_diagonal = 0;
+    L.phase = 0; L.iteration = 0; L.max_iterations = (fused && ph == 0) ? I.prerun_iterations : I.max_iterations; L.num_invalid = 0; L.done = 0; L.termination = 0; L.last_successful = 1; L.reuse_diagonal = 0;
     L.ls_iters = 0; L.n_valid = 0; L.total_iterations = 0; L.total_evaluations = 0; L.pending = -1;
     for (int k = 0; k < 7; k++) { L.trial[k] = tr[k]; L.x_best[k] = tr[k]; }
   }
@@ -483,29 +518,29 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
       if (lane == 0) sync_arrive(Y, gen);
     }
     const long long t_e1 = clock64();
-    sync_wait_all(Y, gen);
+    sync_wait_all(Y, gen, grp);
     const long long t_e2 = clock64();
     {
-      // Thread (grp, val) sums value `val` of rows grp, grp + G, grp + 2G, ...: every row load is issued before the first add (one L2 round trip,
+      // Thread (rg, val) sums value `val` of the group's rows rg, rg + G, rg + 2G, ...: every row load is issued before the first add (one L2 round trip,
       // not one per four rows).  The sum is the fixed-order one every CTA computes: four chains over rows j = 0, 1, 2, 3 (mod 4) while a whole
       // group of four is left, the remaining rows into the first chain, (v0 + v1) + (v2 + v3), then the G group sums in order.
       // (Each thread acquiring the tags of its own rows instead of the poll + barrier above was measured slower: back-to-back acquires do not
       // overlap, each waits for the one before.)
       constexpr int G = SOLVE_THREADS / 32, RMAX = (LL_SYNC_ROWS + G - 1) / G;
       static_assert(RMAX % 4 == 0, "the row loop below runs whole groups of four");
-      const int val = tid & 31, grp = tid >> 5, nb = (int)gridDim.x;
-      const int n = grp < nb ? (nb - grp + G - 1) / G : 0;   // rows of this group
+      const int val = tid & 31, rg = tid >> 5, nb = grp.n;
+      const int n = rg < nb ? (nb - rg + G - 1) / G : 0;   // rows of this row group
       if (val < NSUM) {
         double r[RMAX];
 #pragma unroll
-        for (int j = 0; j < RMAX; j++) r[j] = j < n ? __ldcg(&sync_row(Y, gen, grp + j * G)[val]) : 0.0;
+        for (int j = 0; j < RMAX; j++) r[j] = j < n ? __ldcg(&sync_row(Y, gen, grp.first + rg + j * G)[val]) : 0.0;
         double v0 = 0, v1 = 0, v2 = 0, v3 = 0;
         const int whole = n & ~3;
 #pragma unroll
         for (int j = 0; j < RMAX; j += 4) if (j < whole) { v0 += r[j]; v1 += r[j + 1]; v2 += r[j + 2]; v3 += r[j + 3]; }
 #pragma unroll
         for (int j = 0; j < RMAX; j++) if (j >= whole && j < n) v0 += r[j];
-        s_red[grp][val] = (v0 + v1) + (v2 + v3);
+        s_red[rg][val] = (v0 + v1) + (v2 + v3);
       }
       __syncthreads();
       if (tid < NSUM) { double t = 0; for (int g = 0; g < G; g++) t += s_red[g][tid]; s_sum[tid] = t; }
@@ -600,6 +635,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
         if (d_angdist(st->q_last_opt, qi) < 57.3 * st->min_icp_R && sqrt(dt) < st->min_icp_T) st->icp_done = 1;
         else { for (int k = 0; k < 4; k++) st->q_last_opt[k] = qi[k]; for (int k = 0; k < 3; k++) st->t_last_opt[k] = ti[k]; }
         st->icp_iter++;
+        if (st->icp_iter >= st->icp_max_iterations) st->icp_done = 1;
       }
     }
   }
@@ -608,10 +644,10 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   const long long t_p0 = clock64();
   if (cur_mode == SOLVE_FIRST) {
     for (int k = 0; k < tiles_per_cta; k++) {
-      const int i = (blockIdx.x + gridDim.x * k) * tile + tid, li = k * SOLVE_THREADS + tid;
+      const int i = (cta + grp.n * k) * tile + tid, li = k * SOLVE_THREADS + tid;
       double my_l1 = INFINITY;
-      if (i < a.M && tid < tile) {
-        double l1 = INFINITY;
+      if (i < M && tid < tile) {
+        double l1v = INFINITY;
         Slot s; s.type = S.type[li] & 0xff;
         if (s.type != 0) {
           double r[3];
@@ -630,25 +666,25 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
           }
           double rho0; const double wgt = huber_weight(r[0] * r[0] + r[1] * r[1] + r[2] * r[2], E.huber_a, E.huber_b, rho0);
           const double sc = sqrt(wgt);
-          l1 = fabs(sc * r[0]) + fabs(sc * r[1]) + fabs(sc * r[2]);
+          l1v = fabs(sc * r[0]) + fabs(sc * r[1]) + fabs(sc * r[2]);
         }
-        a.l1[i] = l1;
-        my_l1 = l1;
+        l1[i] = l1v;
+        my_l1 = l1v;
       }
       // std::set de-duplication: the thread whose insert created the entry represents the value from here on (bit 8 of its slot's type)
-      if (fused && l1_set_insert_flag(a.table, a.table_mask, my_l1, my_l1 < INFINITY)) S.type[li] |= 0x100;
+      if (fused && l1_set_insert_flag(I.table, I.table_mask, my_l1, my_l1 < INFINITY)) S.type[li] |= 0x100;
     }
   }
   if (fused && ph == 0) {
-    // ---- K10 over the whole grid (:153-161): the element of rank floor(ratio * n) among the DISTINCT L1 norms (k10_select)
+    // ---- K10 over the item's group (:153-161): the element of rank floor(ratio * n) among the DISTINCT L1 norms (k10_select)
     const long long q0 = clock64();
-    k10_select(s_k10, Y, gen, S.type, a.l1, a.M, tiles_per_cta, tile, &st->inlier_ratio);
+    k10_select(s_k10, Y, K, grp, gen, S.type, l1, M, tiles_per_cta, tile, &st->inlier_ratio);
     const double thr2 = k10_threshold(st->inliner_dis, s_k10.result, s_k10.n_distinct);
     if (master && tid == 0) { st->inlier_threshold = thr2; st->n_unique = s_k10.n_distinct; }
     const long long q3 = clock64();
     for (int k = 0; k < tiles_per_cta; k++) {                // :487-499: blocks above the threshold leave the problem
-      const int i = (blockIdx.x + gridDim.x * k) * tile + tid, li = k * SOLVE_THREADS + tid;
-      if (i < a.M && tid < tile) { const int t = S.type[li] & 0xff; S.type[li] = (t != 0 && a.l1[i] > thr2) ? 0 : t; }
+      const int i = (cta + grp.n * k) * tile + tid, li = k * SOLVE_THREADS + tid;
+      if (i < M && tid < tile) { const int t = S.type[li] & 0xff; S.type[li] = (t != 0 && l1[i] > thr2) ? 0 : t; }
     }
     cur_mode = SOLVE_SECOND;
     __syncthreads();
@@ -656,50 +692,73 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a,
   }
   if (master && tid == 0) s_prof[7] += clock64() - t_p0;
   }   // phase
-  // hand the generation base to the next launch (stream-ordered): every CTA ended with the same `gen`
-  if (master && tid == 0) {
-    *((volatile unsigned*)&Y->gen) = gen;
-    for (int k = 0; k < 16; k++) st->prof[k] += s_prof[k];
-  }
+  if (master && tid == 0) for (int k = 0; k < 16; k++) st->prof[k] += s_prof[k];
+  if (tid == 0) hand_over_gen(Y, gen, n_groups);
 }
+template <bool MB>
+static void* solve_fn(bool batch) { return batch ? (void*)lm_solve_kernel<MB, true> : (void*)lm_solve_kernel<MB, false>; }
 
 #define SOLVE_MAX_SMEM (200 * 1024)   // up to ~405k slots on 132 SMs; a typical scan (<= 113 KB of slots per CTA) leaves room for a second CTA per SM (another context's solver)
 
 int solve_prepare(ll_ctx* ctx) {
-  LL_CUDA(ctx, cudaFuncSetAttribute((void*)lm_solve_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SOLVE_MAX_SMEM));
-  LL_CUDA(ctx, cudaFuncSetAttribute((void*)lm_solve_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SOLVE_MAX_SMEM));
+  for (bool batch : {false, true}) {
+    LL_CUDA(ctx, cudaFuncSetAttribute(solve_fn<true>(batch), cudaFuncAttributeMaxDynamicSharedMemorySize, SOLVE_MAX_SMEM));
+    LL_CUDA(ctx, cudaFuncSetAttribute(solve_fn<false>(batch), cudaFuncAttributeMaxDynamicSharedMemorySize, SOLVE_MAX_SMEM));
+  }
   if (!ctx->d_sync) {
     void* p = nullptr; LL_CUDA(ctx, cudaMalloc(&p, sizeof(SolveSync))); LL_CUDA(ctx, cudaMemset(p, 0, sizeof(SolveSync))); ctx->d_sync = (SolveSync*)p;
   }
   return LL_OK;
 }
-// How M slots are spread over the persistent CTAs: CTA b owns the tiles b, b + grid, b + 2 grid, ... of `tile` slots each.
+// How M slots are spread over `ncta` persistent CTAs: CTA b owns the tiles b, b + grid, b + 2 grid, ... of `tile` slots each.
 struct SolveGrid { int tile, tiles_per_cta, grid; };
-static SolveGrid solve_grid(const ll_ctx* ctx, int M) {
-  // The evaluation is fp64-throughput bound (64 DFMA/clk/SM): spread the slots over ALL SMs, even when that leaves CTAs partly empty.
+static SolveGrid solve_grid(int ncta, int M) {
+  // The evaluation is fp64-throughput bound (64 DFMA/clk/SM): spread the slots over ALL the CTAs, even when that leaves CTAs partly empty.
   // tile = slots per CTA and pass (a multiple of 32, <= SOLVE_THREADS); partly empty CTAs on every SM evaluate faster than fewer full ones.
   const int M1 = M > 0 ? M : 1;
   SolveGrid g;
-  g.tile = ((ll_div_up(M1, ctx->num_sms) + 31) / 32) * 32; if (g.tile > SOLVE_THREADS) g.tile = SOLVE_THREADS;
+  g.tile = ((ll_div_up(M1, ncta) + 31) / 32) * 32; if (g.tile > SOLVE_THREADS) g.tile = SOLVE_THREADS;
   const int tiles = ll_div_up(M1, g.tile);
-  g.grid = tiles < ctx->num_sms ? tiles : ctx->num_sms; if (g.grid > LL_SYNC_ROWS) g.grid = LL_SYNC_ROWS;
+  g.grid = tiles < ncta ? tiles : ncta;
   g.tiles_per_cta = ll_div_up(tiles, g.grid);
   return g;
 }
+// The CTA groups of a launch of n items with M[i] slots (a pure function of the slot counts and the SM count): T = min(SMs, LL_SYNC_ROWS) CTAs
+// at most, every group at least one, the rest shared in proportion to the slots; within group i the rule of solve_grid with its CTA count.  One
+// item: the group is solve_grid(T, M), the whole grid.
+static void batch_grid(int num_sms, int n, const int* M, SolveGrid* g) {
+  const int T = num_sms < LL_SYNC_ROWS ? num_sms : LL_SYNC_ROWS;
+  long long tot = 0; for (int i = 0; i < n; i++) tot += M[i] > 0 ? M[i] : 1;
+  for (int i = 0; i < n; i++) g[i] = solve_grid(1 + (int)((long long)(T - n) * (M[i] > 0 ? M[i] : 1) / tot), M[i]);
+}
 // Dynamic shared memory of one solver CTA: whole tiles of SOLVE_THREADS slots, SLOT_BYTES (fast path) or SLOT_BYTES_MB (*_mb functors) each.
 static size_t solve_smem_bytes(const SolveGrid& sg, int deblur) { return (size_t)sg.tiles_per_cta * SOLVE_THREADS * (deblur ? SLOT_BYTES_MB : SLOT_BYTES); }
-int solve_capacity(ll_ctx* ctx, int M, int deblur) {
-  if (solve_smem_bytes(solve_grid(ctx, M), deblur) > SOLVE_MAX_SMEM) { ctx->set_error("too many residual-block slots for the shared-memory-resident solver"); return LL_ERR_CAPACITY; }
+int solve_capacity(ll_ctx* ctx, int n, const int* M, int deblur, int* bad_item) {
+  SolveGrid g[LL_MAX_BATCH];
+  batch_grid(ctx->num_sms, n, M, g);
+  for (int i = 0; i < n; i++) if (solve_smem_bytes(g[i], deblur) > SOLVE_MAX_SMEM) {
+    if (bad_item) *bad_item = i;
+    ctx->set_error(n == 1 ? std::string("too many residual-block slots for the shared-memory-resident solver")
+                          : "too many residual-block slots for the shared memory of a " + std::to_string(g[i].grid) + "-CTA group");
+    return LL_ERR_CAPACITY;
+  }
   return LL_OK;
 }
 int launch_solve(ll_ctx* ctx, const SolveArgs& a) {
-  const SolveGrid sg = solve_grid(ctx, a.M);
-  int tile = sg.tile, tiles_per_cta = sg.tiles_per_cta; const int grid = sg.grid;
   const int mb = a.deblur ? 1 : 0;
-  LL_TRY(solve_capacity(ctx, a.M, mb));
-  const size_t smem = solve_smem_bytes(sg, mb);
-  void* fn = mb ? (void*)lm_solve_kernel<true> : (void*)lm_solve_kernel<false>;
-  SolveArgs args = a; args.sync = ctx->d_sync; void* kargs[] = {&args, &tiles_per_cta, &tile};
+  int M[LL_MAX_BATCH]; SolveGrid g[LL_MAX_BATCH];
+  for (int i = 0; i < a.n_items; i++) M[i] = a.item[i].M;
+  LL_TRY(solve_capacity(ctx, a.n_items, M, mb));
+  batch_grid(ctx->num_sms, a.n_items, M, g);
+  SolveArgs args = a; args.sync = ctx->d_sync;
+  int grid = 0; size_t smem = 0;
+  for (int i = 0; i < a.n_items; i++) {
+    SolveItem& it = args.item[i];
+    it.first = grid; it.n_cta = g[i].grid; it.tile = g[i].tile; it.tiles_per_cta = g[i].tiles_per_cta;
+    grid += g[i].grid; smem = std::max(smem, solve_smem_bytes(g[i], mb));
+  }
+  void* fn = mb ? solve_fn<true>(a.n_items > 1) : solve_fn<false>(a.n_items > 1);
+  void* kargs[] = {&args};
   LL_CUDA(ctx, cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(SOLVE_THREADS), kargs, smem, ctx->stream));   // co-residency of the whole grid is what the exchanges rely on
   ctx->launches++;
   return LL_OK;
@@ -712,22 +771,22 @@ __global__ void __launch_bounds__(SOLVE_THREADS) k10_select_kernel(SolveSync* Y,
   extern __shared__ int s_flag[];   // [tiles_per_cta * SOLVE_THREADS]: bit 8 = this thread represents its slot's value (lm_solve_kernel: S.type)
   __shared__ K10Smem s_k10;
   const int tid = threadIdx.x;
+  const CtaGroup grp = {0, (int)gridDim.x};
+  K10Area* K = &Y->k10[0];
   unsigned gen = *((volatile unsigned*)&Y->gen);
-  k10_clear(table, table_mask, Y);
-  grid_sync(Y, gen);   // the clear before any insert
+  k10_clear(table, table_mask, K, grp);
+  grid_sync(Y, gen, grp);   // the clear before any insert
   for (int k = 0; k < tiles_per_cta; k++) {   // as the epilogue of solve #1: +inf / NaN (and slots past n) are not residuals
     const int i = (blockIdx.x + gridDim.x * k) * tile + tid, li = k * SOLVE_THREADS + tid;
     const double v = (i < n && tid < tile) ? l1[i] : INFINITY;
     s_flag[li] = l1_set_insert_flag(table, table_mask, v, v < INFINITY) ? 0x100 : 0;
   }
-  k10_select(s_k10, Y, gen, s_flag, l1, n, tiles_per_cta, tile, ratio);
-  if (blockIdx.x == 0 && tid == 0) {
-    *value = s_k10.n_distinct > 0 ? s_k10.result : 0.0; *n_distinct = s_k10.n_distinct;
-    *((volatile unsigned*)&Y->gen) = gen;
-  }
+  k10_select(s_k10, Y, K, grp, gen, s_flag, l1, n, tiles_per_cta, tile, ratio);
+  if (blockIdx.x == 0 && tid == 0) { *value = s_k10.n_distinct > 0 ? s_k10.result : 0.0; *n_distinct = s_k10.n_distinct; }
+  if (tid == 0) hand_over_gen(Y, gen, 1);
 }
 int launch_k10_select(ll_ctx* ctx, const double* d_l1, int n, const double* d_ratio, unsigned long long* table, unsigned table_mask, double* d_value, int* d_n_distinct) {
-  const SolveGrid sg = solve_grid(ctx, n);
+  SolveGrid sg; batch_grid(ctx->num_sms, 1, &n, &sg);
   int tile = sg.tile, tiles_per_cta = sg.tiles_per_cta;
   SolveSync* Y = ctx->d_sync;
   const size_t smem = (size_t)tiles_per_cta * SOLVE_THREADS * sizeof(int);   // 4 B per slot: 48 KB up to ~1.6M values on 132 SMs

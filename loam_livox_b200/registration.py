@@ -297,6 +297,30 @@ class Point_cloud_registration:
         return x, thr.value, nd.value, nk.value, l1, (int(it[0]), int(it[1]))
 
 
+def register_batch(ctx: Context, match_map: Map, items, states):
+    """n (1 ... LL_MAX_BATCH) independent registrations against one map in one call (ll_register_batch): items[i] = (corner, surf) feature
+    clouds, states[i] = its capi.RegState.  Items may share a scan.  Returns (results, item_status): item i's RegResult and status are what
+    find_out_incremental_transfrom would give for it alone (status LL_OK, or LL_ERR_NO_BLOCKS for an item that would fail alone and dropped
+    out); the gpu_ms_* fields of every result time the whole batch.  An error of the whole call (count, sharded map, mixed deblur, capacity)
+    raises, with nothing run."""
+    n = len(items)
+    if len(states) != n:
+        raise ValueError("one state per item")
+    arrs = [(_pts(c), _pts(s)) for c, s in items]
+    fmt = arrs[0][0][1] if arrs else capi.LL_FMT_XYZI16
+    if any(c[1] != fmt or s[1] != fmt for c, s in arrs):
+        raise ValueError("every cloud of a batch has the same point format")
+    corners = (C.c_void_p * max(n, 1))(*[c[0].ctypes.data for c, _ in arrs])
+    surfs = (C.c_void_p * max(n, 1))(*[s[0].ctypes.data for _, s in arrs])
+    nc = (C.c_size_t * max(n, 1))(*[c[0].shape[0] for c, _ in arrs])
+    ns = (C.c_size_t * max(n, 1))(*[s[0].shape[0] for _, s in arrs])
+    st = (capi.RegState * max(n, 1))(*states)
+    res = (capi.RegResult * max(n, 1))()
+    status = (C.c_int * max(n, 1))()
+    ctx.check(ctx._lib.ll_register_batch(ctx.h, match_map.h, n, corners, nc, surfs, ns, fmt, capi.LL_HOST, st, res, status))
+    return [res[i] for i in range(n)], [int(status[i]) for i in range(n)]
+
+
 def inlier_select(ctx: Context, l1, ratio: float):
     """compute_inlier_residual_threshold (point_cloud_registration.hpp:153-161) over caller-given L1 norms (ll_inlier_select): the fused solver
     kernel's grid-wide select, as the sharded mode runs it.  Returns (value, number of distinct values); +inf / NaN are skipped."""
