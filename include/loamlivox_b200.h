@@ -66,7 +66,8 @@ void ll_ctx_destroy(ll_ctx* ctx);
  * do not land in the first registered scan.  ll_mapper_create calls it; nothing else depends on it. */
 int  ll_ctx_warmup(ll_ctx* ctx);
 const char* ll_last_error(const ll_ctx* ctx);
-/* CUDA stream of the context as a cudaStream_t cast to void* (all work of a context is enqueued on it). */
+/* CUDA stream of the context as a cudaStream_t cast to void* (all work of a context is enqueued on it, except the front end of the sequence
+ * calls ll_mapper_process_frames / _scans, which runs on streams of its own and has completed when they return). */
 void* ll_ctx_stream(ll_ctx* ctx);
 int  ll_ctx_sync(ll_ctx* ctx);
 
@@ -337,6 +338,28 @@ int  ll_mapper_process_scan(ll_mapper* mapper, const void* raw, size_t n, int fm
 #define LL_MAX_PIECES_PER_FRAME 16
 int  ll_mapper_process_frame(ll_mapper* mapper, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
                              int odom_mode, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces);
+/* Sequences (recorded data replayed or mapped offline faster than real time): the front end of input k + 1 runs on the device, on streams of
+ * the least priority (the context's own streams have the greatest), while input k is registered.  A live node gains nothing (the next frame does not exist yet) and keeps the single calls.
+ *
+ * ll_mapper_process_frames: n_frames frames of n_heads heads each, in order: the results of n_frames calls of ll_mapper_process_frame.
+ * Frame f's heads are raws / ns / stamps [f * n_heads + h].  out / stats (stats may be NULL): cap entries per frame (out[f * cap + i] = piece i
+ * of frame f); n_pieces[f] as the single call's *n_pieces.
+ * ll_mapper_process_scans: n_scans raw scans, the results of n_scans calls of ll_mapper_process_scan (out[k], stats[k]).
+ *
+ * Identity: every entry equals the single call's in every ll_reg_result field except gpu_ms_*, and in every integer field of ll_mapper_stats;
+ * ll_mapper_pose and the mapper and extractor state after the call equal the single calls' too.  ms_* stay host wall clock per phase;
+ * ms_front_end is the time this call spent enqueuing and waiting for that input's front end, so it falls when the front end is hidden.
+ * Validation first: null pointers, n_frames / n_scans < 1, n_heads outside 1 ... 8, an unknown fmt or where, a bad odom_mode, pieces or cap
+ * (LL_ERR_INVALID) and any frame or scan over max_scan_points (LL_ERR_CAPACITY) are found for the whole sequence before anything is
+ * enqueued; nothing changes then.  An error while running (a piece or scan over max_features: LL_ERR_CAPACITY; or an error of the single
+ * call's registration) stops the sequence at input f: *n_frames_done / *n_scans_done = f, n_pieces[f] = the pieces of frame f completed, and
+ * the mapper and the extractor's time bookkeeping are exactly as after the single calls up to and including the failing one, so the caller
+ * can go on with input f + 1 by either API.  Inputs need only stay valid for the duration of the call; nothing is pending between calls. */
+int  ll_mapper_process_frames(ll_mapper* mapper, int n_frames, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where,
+                              const double* stamps, int odom_mode, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces,
+                              int* n_frames_done);
+int  ll_mapper_process_scans(ll_mapper* mapper, int n_scans, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+                             ll_reg_result* out, ll_mapper_stats* stats, int* n_scans_done);
 int  ll_mapper_pose(const ll_mapper* mapper, double q_wxyz[4], double t[3], int* frame_index);
 
 /* ---- wire formats (SURVEY 8(f) N3) ---------------------------------------------------------------------------------------------- */

@@ -8,6 +8,7 @@
 // so that laser_feature_extractor.hpp / laser_mapping.hpp can switch with the small adapter shown in INTEGRATION.md.
 // No PCL / Eigen / Ceres needed: clouds are std::vector<ll200::PointXYZI> (layout-identical to pcl::PointXYZI, 32 bytes).
 #pragma once
+#include <algorithm>
 #include <array>
 #include <cstring>
 #include <stdexcept>
@@ -232,6 +233,46 @@ class Laser_mapping {
     ctx_.check(ll_mapper_pose(mapper_, m_q_w_curr.data(), m_t_w_curr.data(), &m_current_frame_index));
     r.resize(n); st.resize(n);
     if (results) *results = r; if (stats) *stats = st;
+  }
+  // several frames of recorded data in one call: what process_new_frame returns for each in turn, the front end of frame f + 1 running on the
+  // device under the registrations of frame f (heads of every frame in the same number).  results / stats: one entry per frame.  On an error
+  // they hold what completed (the frames before the failing one, then its completed pieces) before Error is thrown; *done = the frames completed.
+  void process_new_frames(const std::vector<std::vector<PointCloud>>& frames, const std::vector<std::vector<double>>& time_stamps, int odom_mode = 1,
+                          std::vector<std::vector<ll_reg_result>>* results = nullptr, std::vector<std::vector<ll_mapper_stats>>* stats = nullptr, int* done_out = nullptr) {
+    if (frames.empty() || frames.size() != time_stamps.size()) throw Error(LL_ERR_INVALID, "one list of time stamps per frame");
+    const size_t nh = frames[0].size(), cap = LL_MAX_PIECES_PER_FRAME;
+    std::vector<const void*> raws; std::vector<size_t> ns; std::vector<double> stamps;
+    for (size_t f = 0; f < frames.size(); f++) {
+      if (frames[f].size() != nh || time_stamps[f].size() != nh) throw Error(LL_ERR_INVALID, "the same heads in every frame, one time stamp per head");
+      for (size_t h = 0; h < nh; h++) { raws.push_back(frames[f][h].data()); ns.push_back(frames[f][h].size()); stamps.push_back(time_stamps[f][h]); }
+    }
+    std::vector<ll_reg_result> r(frames.size() * cap); std::vector<ll_mapper_stats> st(frames.size() * cap); std::vector<int> n(frames.size()); int done = 0;
+    const int status = ll_mapper_process_frames(mapper_, (int)frames.size(), (int)nh, raws.data(), ns.data(), LL_FMT_PCL32, LL_HOST, stamps.data(), odom_mode,
+                                                r.data(), st.data(), (int)cap, n.data(), &done);
+    const size_t kept = status == LL_OK ? frames.size() : std::min(frames.size(), (size_t)done + 1);
+    if (results) { results->clear(); for (size_t f = 0; f < kept; f++) results->emplace_back(r.begin() + f * cap, r.begin() + f * cap + n[f]); }
+    if (stats) { stats->clear(); for (size_t f = 0; f < kept; f++) stats->emplace_back(st.begin() + f * cap, st.begin() + f * cap + n[f]); }
+    if (done_out) *done_out = done;
+    ctx_.check(ll_mapper_pose(mapper_, m_q_w_curr.data(), m_t_w_curr.data(), &m_current_frame_index));
+    ctx_.check(status);
+  }
+  // several raw scans of recorded data in one call: what process_new_scan returns for each in turn, the front end of scan k + 1 under the
+  // mapper step of scan k.  Returns the int of find_out_incremental_transfrom per scan.  On an error results / stats hold the scans completed
+  // before Error is thrown; *done = their number.
+  std::vector<int> process_new_scans(const std::vector<PointCloud>& raws, const std::vector<double>& time_stamps, std::vector<ll_reg_result>* results = nullptr,
+                                     std::vector<ll_mapper_stats>* stats = nullptr, int* done_out = nullptr) {
+    if (raws.empty() || raws.size() != time_stamps.size()) throw Error(LL_ERR_INVALID, "one time stamp per scan");
+    std::vector<const void*> ptrs; std::vector<size_t> ns;
+    for (const PointCloud& c : raws) { ptrs.push_back(c.data()); ns.push_back(c.size()); }
+    std::vector<ll_reg_result> r(raws.size()); std::vector<ll_mapper_stats> st(raws.size()); int done = 0;
+    const int rc = ll_mapper_process_scans(mapper_, (int)raws.size(), ptrs.data(), ns.data(), LL_FMT_PCL32, LL_HOST, time_stamps.data(), r.data(), st.data(), &done);
+    r.resize(rc == LL_OK ? raws.size() : (size_t)done); st.resize(r.size());
+    if (results) *results = r; if (stats) *stats = st;
+    if (done_out) *done_out = done;
+    ctx_.check(ll_mapper_pose(mapper_, m_q_w_curr.data(), m_t_w_curr.data(), &m_current_frame_index));
+    ctx_.check(rc);
+    std::vector<int> status; for (const ll_reg_result& x : r) status.push_back(x.status);
+    return status;
   }
   std::array<double, 4> m_q_w_curr{{1, 0, 0, 0}};   // (w, x, y, z)
   std::array<double, 3> m_t_w_curr{{0, 0, 0}};

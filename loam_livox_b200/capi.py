@@ -28,7 +28,7 @@ EXPORTS = [
     "ll_scan_to_pose", "ll_comm_local_handle", "ll_comm_connect", "ll_launch_count", "ll_cellmap_create", "ll_cellmap_release", "ll_cellmap_append",
     "ll_cellmap_assemble", "ll_cellmap_reserve", "ll_cellmap_stats", "ll_voxel_downsample_dev", "ll_transform_dev", "ll_last_features_dev", "ll_mapper_config_default", "ll_mapper_create", "ll_mapper_release",
     "ll_mapper_process_scan", "ll_mapper_pose", "ll_map_rebuild", "ll_debug_solver_cycles", "ll_state_snapshot_bytes", "ll_set_point_layout", "ll_format_pose_log", "ll_reg_state_yaml", "ll_cap_uniform", "ll_map_shard_info", "ll_shard_plan", "ll_align_cfg_default", "ll_scene_align", "ll_frame_to_pose", "ll_features_to_pointcloud2",
-    "ll_mapper_process_frame", "ll_voxel_downsample_segments", "ll_register_batch",
+    "ll_mapper_process_frame", "ll_voxel_downsample_segments", "ll_register_batch", "ll_mapper_process_frames", "ll_mapper_process_scans",
 ]
 
 
@@ -169,6 +169,8 @@ def lib():
     L.ll_mapper_release.argtypes = [vp]
     L.ll_mapper_process_scan.argtypes = [vp, vp, sz, ci, ci, cd, C.POINTER(RegResult), C.POINTER(MapperStats)]
     L.ll_mapper_process_frame.argtypes = [vp, ci, vp, vp, ci, ci, vp, ci, C.POINTER(RegResult), C.POINTER(MapperStats), ci, C.POINTER(ci)]
+    L.ll_mapper_process_frames.argtypes = [vp, ci, ci, vp, vp, ci, ci, vp, ci, C.POINTER(RegResult), C.POINTER(MapperStats), ci, vp, C.POINTER(ci)]
+    L.ll_mapper_process_scans.argtypes = [vp, ci, vp, vp, ci, ci, vp, C.POINTER(RegResult), C.POINTER(MapperStats), C.POINTER(ci)]
     L.ll_mapper_pose.argtypes = [vp, vp, vp, C.POINTER(ci)]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64

@@ -36,7 +36,7 @@ int ll_scene_align(ll_ctx* ctx, const void* src_line, size_t n_sl, const void* s
     d_cnt = c.take<int>(4);
   }));
   auto fail = [&](int st) { arena.release(); return st; };
-  for (int k = 0; k < 4; k++) { const int st = upload_cloud(ctx, srcs[k], ns[k], fmt, where, d_in[k]); if (st != LL_OK) return fail(st); }
+  for (int k = 0; k < 4; k++) { const int st = upload_cloud(ctx, s, srcs[k], ns[k], fmt, where, d_in[k]); if (st != LL_OK) return fail(st); }
   // m_pc_reg as set_up_log_dir / find_tranfrom_of_two_mappings leave it (:233-243, :292-306)
   ll_reg_state st; ll_reg_state_default(&st);
   st.icp_line = 0; st.icp_plane = 1;

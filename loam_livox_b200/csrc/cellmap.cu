@@ -299,7 +299,7 @@ int ll_cellmap_append(ll_ctx* ctx, ll_cellmap* m, const void* pts, size_t n, int
     LL_TRY(cm_reserve_store(ctx, m, m->n_pts + (int)n));
     CmAppend ap; LL_CUDA(ctx, m->tmp_buf.carve([&](Carve& c) { ap.layout(c, n); }));
     float4* d_in = ap.in; int* d_slot = ap.slot;
-    LL_TRY(upload_cloud(ctx, pts, n, fmt, where, d_in));
+    LL_TRY(upload_cloud(ctx, s, pts, n, fmt, where, d_in));
     const float box = m->resolution * 1.0f, half = m->resolution * 0.5f;
     const int blocks = ll_div_up((int)n, 256), cur = m->current_frame_idx;
     cm_locate_kernel<<<blocks, 256, 0, s>>>(d_in, (int)n, box, half, cur, m->keys, (unsigned)(m->table_cap - 1), m->create_frame, m->last_update, m->epoch, m->bump, m->d_counters, d_slot);

@@ -56,9 +56,8 @@ int launch_pack_strided(ll_ctx* ctx, const float4* d_src, int n, unsigned char* 
   return LL_OK;
 }
 
-int upload_cloud(ll_ctx* ctx, const void* src, size_t n, int fmt, int where, float4* d_dst) {
+int upload_cloud(ll_ctx* ctx, cudaStream_t s, const void* src, size_t n, int fmt, int where, float4* d_dst) {
   if (n == 0) return LL_OK;
-  cudaStream_t s = ctx->stream;
   if (fmt == LL_FMT_XYZI16) {
     LL_CUDA(ctx, cudaMemcpyAsync(d_dst, src, n * 16, where == LL_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
   } else if (fmt == LL_FMT_PCL32) {

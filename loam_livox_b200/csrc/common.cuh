@@ -161,8 +161,15 @@ struct SyncEvents {
   cudaEvent_t fork = nullptr, join = nullptr;     // stream <-> stream2
   cudaEvent_t fork3 = nullptr, join3 = nullptr;   // stream <-> stream3
   cudaEvent_t it[2] = {nullptr, nullptr};         // ICP iteration `it` has been snapshot into PinnedStage::snap[it & 1]
-  template <typename F> void each(F&& f) { for (cudaEvent_t* e : {&fork, &join, &fork3, &join3, &it[0], &it[1]}) f(*e); }
+  // the sequence calls' front end (ll_ctx::fe_stream): fork / join of its own three streams, `ready` behind a whole front end, and `free[a]`
+  // behind the last copy of an input's features out of the front end's buffers (scans: [0], tmp_a / tmp_b; frames: [arena])
+  cudaEvent_t fe_fork = nullptr, fe_join = nullptr, fe_fork3 = nullptr, fe_join3 = nullptr, fe_ready = nullptr, fe_free[2] = {nullptr, nullptr};
+  template <typename F> void each(F&& f) {
+    for (cudaEvent_t* e : {&fork, &join, &fork3, &join3, &it[0], &it[1], &fe_fork, &fe_join, &fe_fork3, &fe_join3, &fe_ready, &fe_free[0], &fe_free[1]}) f(*e);
+  }
 };
+// The streams and ordering events one front end is enqueued on: the main chain, the corner VoxelGrid chain, the petal bookkeeping.
+struct FrontStreams { cudaStream_t main, corner, petals; cudaEvent_t fork, join, fork3, join3; };
 
 struct ll_ctx {
   int device = 0;
@@ -195,6 +202,11 @@ struct ll_ctx {
   int rank = 0, world = 1;
   cudaStream_t stream2 = nullptr;   // side stream: the corner halves of the front end and of the map side
   cudaStream_t stream3 = nullptr;   // second side stream: the petal bookkeeping of the extractor (whole_frame front end)
+  // The front end of ll_mapper_process_frames / _scans, which runs under the mapper step of the previous input: three streams of the least
+  // priority (stream / stream2 / stream3 have the greatest), sharing no stream and no event with the mapper step (main chain, corner chain, petals).
+  cudaStream_t fe_stream[3] = {nullptr, nullptr, nullptr};
+  FrontStreams own_front() const { return {stream, stream2, stream3, sev.fork, sev.join, sev.fork3, sev.join3}; }   // the single-input calls'
+  FrontStreams pipe_front() const { return {fe_stream[0], fe_stream[1], fe_stream[2], sev.fe_fork, sev.fe_join, sev.fe_fork3, sev.fe_join3}; }
   // The per-scan front end (extract + get_features + 4 VoxelGrids + count read-back) replayed as ONE CUDA graph: ~60 launches whose
   // enqueue cost on the host (CUB dispatch included) was longer than their execution.  Every buffer it touches is fixed at creation, so it is
   // re-captured only when the scan size or the pipeline config changes.

@@ -330,8 +330,8 @@ static ExtractParams extract_params(ll_ctx* ctx, int n) {
   return P;
 }
 // K1 + K2: the per-point part of projection_scan_3d_2d and compute_features (everything get_features needs)
-int launch_extract_points(ll_ctx* ctx, int n) {
-  ExtractState& e = ctx->ex; cudaStream_t s = ctx->stream;
+int launch_extract_points(ll_ctx* ctx, cudaStream_t s, int n) {
+  ExtractState& e = ctx->ex;
   const ExtractParams P = extract_params(ctx, n);
   const int blocks = ll_div_up(n, 256);
   ex_point_kernel<<<blocks, 256, 0, s>>>(e.raw, P, e.time_stamp, e.polar_dis_sq2, e.depth_sq2, e.self_mask);
@@ -360,9 +360,9 @@ int launch_extract_petals(ll_ctx* ctx, int n, cudaStream_t s, DevBuf& scratch) {
   return LL_OK;
 }
 
-int launch_piece_bounds(ll_ctx* ctx, int pieces, float* d_start_end) {
+int launch_piece_bounds(ll_ctx* ctx, cudaStream_t s, int pieces, float* d_start_end) {
   ExtractState& e = ctx->ex;
-  ex_piece_kernel<<<1, 32, 0, ctx->stream>>>(e.scan_first, e.scan_last, e.d_meta, e.n, pieces, d_start_end); ctx->launches++;
+  ex_piece_kernel<<<1, 32, 0, s>>>(e.scan_first, e.scan_last, e.d_meta, e.n, pieces, d_start_end); ctx->launches++;
   LL_CUDA(ctx, cudaGetLastError());
   return LL_OK;
 }

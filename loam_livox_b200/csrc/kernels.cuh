@@ -186,7 +186,7 @@ int launch_l1_exchange(ll_ctx* ctx, const double* d_l1, int M);
 int launch_count_exchange(ll_ctx* ctx);
 
 // ---------------------------------------------------------------------------------------------- clouds (cloud.cu)
-int upload_cloud(ll_ctx* ctx, const void* src, size_t n, int fmt, int where, float4* d_dst);   // async on ctx->stream
+int upload_cloud(ll_ctx* ctx, cudaStream_t s, const void* src, size_t n, int fmt, int where, float4* d_dst);   // async on s
 int launch_transform(ll_ctx* ctx, cudaStream_t s, const double* d_pose7, const float4* d_in, int n, float4* d_out);
 int launch_pack_strided(ll_ctx* ctx, const float4* d_src, int n, unsigned char* d_dst);   // 16-byte points -> PointCloud2 records (ctx->layout)
 // VoxelGrid on device: d_in [n] -> d_out [<= n], *d_n_out on device. n given by host, or by device count d_n_in (may be null).
@@ -198,11 +198,11 @@ size_t voxel_grid_bytes(int n_cap, int nseg = 1);   // what launch_voxel_grid(_s
 
 // ---------------------------------------------------------------------------------------------- extractor (extract.cu)
 int extract_alloc(ll_ctx* ctx);   // ExtractState arrays for max_scan_points (ll_ctx_create)
-int launch_extract_points(ll_ctx* ctx, int n);   // current_time is read from ctx->ex.d_time
+int launch_extract_points(ll_ctx* ctx, cudaStream_t s, int n);   // current_time is read from ctx->ex.d_time
 int launch_extract_petals(ll_ctx* ctx, int n, cudaStream_t s, DevBuf& scratch);
 int launch_get_features(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float* d_bounds /*min_blur,max_blur on device*/, float min_blur, float max_blur,
                         float4* d_corners, float4* d_surf, float4* d_full, int* d_counts /*3*/);
-int launch_piece_bounds(ll_ctx* ctx, int pieces, float* d_start_end /* 2*pieces */);
+int launch_piece_bounds(ll_ctx* ctx, cudaStream_t s, int pieces, float* d_start_end /* 2*pieces */);
 size_t petals_bytes(int n);         // what launch_extract_petals carves from `scratch`
 size_t get_features_bytes(int n);   // what launch_get_features carves from `scratch`
 
@@ -217,12 +217,22 @@ int launch_gather_pieces(ll_ctx* ctx, cudaStream_t s, FrameDev* dev, const Frame
 // ---------------------------------------------------------------------------------------------- host driver pieces (api.cu)
 // Registration of the features already resident in A.feat (corners then surfaces): the batch of one.  Core of ll_register / ll_scan_to_pose.
 int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg_state* in, ll_reg_result* out);
+// The per-scan front end in three parts: enqueue on `fs` (bookkeeping, upload, the front end replayed as a graph; its counts land in
+// ctx->pin->fe_counts / fe_meta), and, once that work has completed, finish (the counts, the drop rule, max_features, the features copied
+// from tmp_a / tmp_b into A.feat on `s`).  scan_front_end = both on the context's own streams with a synchronisation between them.
+int scan_front_end_enqueue(ll_ctx* ctx, const FrontStreams& fs, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc);
+int scan_front_end_finish(ll_ctx* ctx, cudaStream_t s, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);
 int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);
 // The device arrays of a piecewise frame front end (owned by the streaming mapper): gathered segments of cap points per class, the first
 // VoxelGrids' outputs, and the segmented VoxelGrids' scratch arenas (vg[0] on the context's stream, vg[1] on stream2).
-struct FrameArena { FrameDev* dev; float4* cls[2]; float4* mid[2]; int cap; DevBuf* vg[2]; };
+// The device part of a piecewise frame front end (everything after the uploads) replayed as one CUDA graph, one per arena: its buffers are
+// fixed, so it is re-captured only when the frame's shape changes (head count, per-head sizes, pieces, pipeline config).  The uploads and the
+// extractor's bookkeeping stay outside it, so the format and the caller's pointers do not enter the graph.
+struct FrameGraph { cudaGraphExec_t exec = nullptr; int n_heads = 0; size_t ns[LL_MAX_HEADS] = {}; int pieces = 0; ll_pipeline_cfg pc = {}; bool warm = false; uint64_t launches = 0; };
+struct FrameArena { FrameDev* dev; float4* cls[2]; float4* mid[2]; int cap; DevBuf* vg[2]; FrameGraph* graph; };
 // Every head through the extractor, the slices of every piece, the gathers and the four segmented VoxelGrids (laser_feature_extractor.hpp:
-// 303-380, laser_mapping.hpp:1367-1373), enqueued without a host synchronisation; dev->out lands in ctx->pin->frame.  Piece i's features
+// 303-380, laser_mapping.hpp:1367-1373), enqueued on `fs` without a host synchronisation (the device part replayed as fa.graph once the
+// shape repeats); dev->out lands in ctx->pin->frame.  Piece i's features
 // are then cls[0] / cls[1] [out_end[.][i - 1], out_end[.][i]).
-int frame_front_end(ll_ctx* ctx, const FrameArena& fa, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+int frame_front_end(ll_ctx* ctx, const FrontStreams& fs, const FrameArena& fa, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
                     int pieces, const ll_pipeline_cfg* pc);

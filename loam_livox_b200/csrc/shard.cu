@@ -101,8 +101,8 @@ int ll_map_build_sharded(ll_ctx* ctx, const void* corner, size_t nc, const void*
   // feat_buf: [corner cloud | surface cloud | compacted cloud]; scratch2: bbox, histogram / owner table, keep flags, CUB temp
   float4* d_c; float4* d_s; float4* d_k;
   LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) { d_c = c.take<float4>(nc); d_s = c.take<float4>(ns); d_k = c.take<float4>(nmax); }));
-  LL_TRY(upload_cloud(ctx, corner, nc, fmt, where, d_c));
-  LL_TRY(upload_cloud(ctx, surf, ns, fmt, where, d_s));
+  LL_TRY(upload_cloud(ctx, s, corner, nc, fmt, where, d_c));
+  LL_TRY(upload_cloud(ctx, s, surf, ns, fmt, where, d_s));
   // ---- grid over the bounding box of the whole map (identical on every rank: every rank sees the same two clouds)
   int* d_bbox = nullptr;
   LL_CUDA(ctx, ctx->scratch2.carve([&](Carve& c) { d_bbox = c.take<int>(16); }));

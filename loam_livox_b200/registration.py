@@ -448,6 +448,16 @@ class Points_cloud_map:
         return out[:n.value].copy(), nf.value
 
 
+class SequenceError(LoamLivoxError):
+    """An error that stopped process_new_frames / process_new_scans at input `done`: `results` holds what completed (per frame, the frames
+    before `done` and the pieces of frame `done` completed; per scan, the scans before `done`).  The mapper stands as after the one-by-one calls
+    up to and including the failing input, so the caller can go on from input done + 1."""
+
+    def __init__(self, status, message, done, results):
+        super().__init__(f"status {status}: {message} (input {done})")
+        self.status, self.done, self.results = status, done, results
+
+
 class Laser_mapping:
     """Streaming odometry: one call per raw scan (Laser_mapping::process_new_scan, loam_livox/source/laser_mapping.hpp:1316-1521, with the
     match-map refresh of update_buff_for_matching :460-566 in matching_mode 1).  All state stays on the device."""
@@ -509,6 +519,54 @@ class Laser_mapping:
         res, stats, n = (capi.RegResult * cap)(), (capi.MapperStats * cap)(), C.c_int()
         self.ctx.check(self.ctx._lib.ll_mapper_process_frame(self.h, k, ptrs, sizes, fmt, where, st, int(odom_mode), res, stats, cap, C.byref(n)))
         return [(res[i], stats[i]) for i in range(n.value)]
+
+    @staticmethod
+    def _clouds(clouds, where, ns, fmt):
+        """(void* array, size_t array, fmt, keepalive) of host clouds ([n,4] / [n,8] float32, or LL_FMT_STRIDED records with ns given) or of
+        device pointers (ns given)."""
+        if where == capi.LL_HOST and fmt != capi.LL_FMT_STRIDED:
+            arrs = [_pts(c) for c in clouds]
+            fmt = arrs[0][1] if arrs else capi.LL_FMT_XYZI16
+            keep = [a for a, _ in arrs]
+            ptrs, sizes = [a.ctypes.data for a in keep], [a.shape[0] for a in keep]
+        elif where == capi.LL_HOST:
+            keep = [np.ascontiguousarray(c) for c in clouds]
+            ptrs, sizes = [a.ctypes.data for a in keep], [int(n) for n in ns]
+        else:
+            keep, ptrs, sizes = None, [int(c) for c in clouds], [int(n) for n in ns]
+        k = len(ptrs)
+        return (C.c_void_p * k)(*ptrs), (C.c_size_t * k)(*sizes), fmt, keep
+
+    def process_new_frames(self, frames, stamps, odom_mode=1, where=capi.LL_HOST, ns=None, fmt=None):
+        """Several sensor frames in one call (frames[f]: the head clouds of frame f, the same number of heads in every frame; stamps[f]: their
+        time stamps; ns[f]: their sizes for device pointers): the results of process_new_frame on each frame in turn, while the front end of
+        frame f + 1 runs on the device under the registrations of frame f.  For recorded data; a live node keeps process_new_frame.
+        Returns one list of (RegResult, MapperStats) per frame."""
+        nf, nh = len(frames), len(frames[0])
+        assert all(len(f) == nh for f in frames) and len(stamps) == nf
+        flat_ns = [n for f in ns for n in f] if ns is not None else None
+        ptrs, sizes, fmt, _keep = self._clouds([h for f in frames for h in f], where, flat_ns, fmt)
+        st = (C.c_double * (nf * nh))(*[float(t) for f in stamps for t in f])
+        cap = capi.LL_MAX_PIECES_PER_FRAME
+        res, stats = (capi.RegResult * (nf * cap))(), (capi.MapperStats * (nf * cap))()
+        n_pieces, done = (C.c_int * nf)(), C.c_int()
+        status = self.ctx._lib.ll_mapper_process_frames(self.h, nf, nh, ptrs, sizes, fmt, where, st, int(odom_mode), res, stats, cap, n_pieces, C.byref(done))
+        out = [[(res[f * cap + i], stats[f * cap + i]) for i in range(n_pieces[f])] for f in range(nf)]
+        if status != capi.LL_OK:   # frames before `done` complete, frame `done` up to its failing piece
+            raise SequenceError(status, self.ctx._lib.ll_last_error(self.ctx.h).decode(), done.value, out[:done.value + 1] if done.value < nf else out)
+        return out
+
+    def process_new_scans(self, raws, stamps, where=capi.LL_HOST, ns=None, fmt=None):
+        """Several raw scans in one call: the results of process_new_scan on each in turn, the front end of scan k + 1 running on the device
+        under the mapper step of scan k.  Returns one (RegResult, MapperStats) per scan."""
+        k = len(raws)
+        ptrs, sizes, fmt, _keep = self._clouds(raws, where, ns, fmt)
+        st = (C.c_double * k)(*[float(t) for t in stamps])
+        res, stats, done = (capi.RegResult * k)(), (capi.MapperStats * k)(), C.c_int()
+        status = self.ctx._lib.ll_mapper_process_scans(self.h, k, ptrs, sizes, fmt, where, st, res, stats, C.byref(done))
+        if status != capi.LL_OK:
+            raise SequenceError(status, self.ctx._lib.ll_last_error(self.ctx.h).decode(), done.value, [(res[i], stats[i]) for i in range(done.value)])
+        return [(res[i], stats[i]) for i in range(k)]
 
     def pose(self):
         q, t, f = np.empty(4), np.empty(3), C.c_int()
