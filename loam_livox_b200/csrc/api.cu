@@ -871,41 +871,44 @@ static int front_end_enqueue(ll_ctx* ctx, const FrontStreams& fs, const ll_pipel
   return LL_OK;
 }
 
-// The graph is captured from, and replayed on, whichever streams the caller passes: it holds its own dependencies, so one cache serves both
-// the single-scan calls and the sequence calls.
-int scan_front_end_enqueue(ll_ctx* ctx, const FrontStreams& fs, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc) {
-  cudaStream_t s = fs.main;
-  LL_TRY(extract_prepare(ctx, s, raw, n, fmt, where, stamp));
-  const int ncap = (int)n;
-  ll_ctx::FrontGraph& g = ctx->fg;
-  const bool same = g.n == n && memcmp(&g.pc, pc, sizeof(*pc)) == 0;
+// `enqueue` (the device part of a front end, on stream s) eagerly on the first call with `key`, captured into g on the second when `capturable`,
+// replayed from the third.  The graph is captured from, and replayed on, whichever streams the caller passes: it holds its own dependencies,
+// so one cache serves both the single-input calls and the sequence calls.
+template <typename F>
+static int front_graph(ll_ctx* ctx, FrontGraph& g, cudaStream_t s, const FrontKey& key, bool capturable, F&& enqueue) {
+  const bool same = g.key == key;
   if (same && g.exec) {
     LL_CUDA(ctx, cudaGraphLaunch(g.exec, s));
     ctx->launches += g.launches;
-  } else if (same && g.warm && n >= 5) {
-    // second call with this shape: captured (every buffer the front end touches was laid out at creation)
-    if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
+    return LL_OK;
+  }
+  if (same && g.warm && capturable) {
     const uint64_t l0 = ctx->launches;
     cudaGraph_t graph = nullptr;
     LL_CUDA(ctx, cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-    const int st = front_end_enqueue(ctx, fs, pc, ncap);
-    const cudaError_t ce = cudaStreamEndCapture(s, &graph);
-    if (st != LL_OK || ce != cudaSuccess) {   // should not happen: fall back to eager launches
-      if (graph) cudaGraphDestroy(graph);
-      cudaGetLastError(); g.warm = false; g.n = 0;
-      LL_TRY(front_end_enqueue(ctx, fs, pc, ncap));
-    } else {
+    const int st = enqueue();
+    cudaError_t ce = cudaStreamEndCapture(s, &graph);
+    if (st == LL_OK && ce == cudaSuccess) ce = cudaGraphInstantiate(&g.exec, graph, 0);
+    if (graph) cudaGraphDestroy(graph);
+    if (st == LL_OK && ce == cudaSuccess) {
       g.launches = ctx->launches - l0;
-      LL_CUDA(ctx, cudaGraphInstantiate(&g.exec, graph, 0));
-      cudaGraphDestroy(graph);
       LL_CUDA(ctx, cudaGraphLaunch(g.exec, s));
+      return LL_OK;
     }
-  } else {
-    if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
-    LL_TRY(front_end_enqueue(ctx, fs, pc, ncap));
-    g.n = n; g.pc = *pc; g.warm = true;
+    // should not happen: the captured launches never ran, so they are not counted; eager launches, and the shape starts afresh
+    cudaGetLastError(); g.exec = nullptr; ctx->launches = l0; g.warm = false; g.key = FrontKey();
+    return enqueue();
   }
+  if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
+  LL_TRY(enqueue());
+  g.key = key; g.warm = true;
   return LL_OK;
+}
+
+int scan_front_end_enqueue(ll_ctx* ctx, const FrontStreams& fs, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc) {
+  LL_TRY(extract_prepare(ctx, fs.main, raw, n, fmt, where, stamp));
+  FrontKey key; key.n_heads = 1; key.ns[0] = n; key.pc = *pc;
+  return front_graph(ctx, ctx->fg, fs.main, key, n >= 5, [&] { return front_end_enqueue(ctx, fs, pc, (int)n); });
 }
 
 int scan_front_end_finish(ll_ctx* ctx, cudaStream_t s, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped) {
@@ -1024,34 +1027,8 @@ int frame_front_end(ll_ctx* ctx, const FrontStreams& fs, const FrameArena& fa, i
     LL_TRY(upload_cloud(ctx, s, raws[h], ns[h], fmt, where, ctx->ex.raw + base));
     base += ns[h];
   }
-  FrameGraph& g = *fa.graph;
-  const bool same = g.n_heads == n_heads && memcmp(g.ns, ns, (size_t)n_heads * sizeof(size_t)) == 0 && g.pieces == pieces && memcmp(&g.pc, pc, sizeof(*pc)) == 0;
-  if (same && g.exec) {
-    LL_CUDA(ctx, cudaGraphLaunch(g.exec, s));
-    ctx->launches += g.launches;
-  } else if (same && g.warm) {   // second frame of this shape: captured
-    const uint64_t l0 = ctx->launches;
-    cudaGraph_t graph = nullptr;
-    LL_CUDA(ctx, cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-    const int st = frame_front_end_device(ctx, fs, fa, n_heads, ns, pieces, pc);
-    const cudaError_t ce = cudaStreamEndCapture(s, &graph);
-    if (st != LL_OK || ce != cudaSuccess) {   // should not happen: fall back to eager launches
-      if (graph) cudaGraphDestroy(graph);
-      cudaGetLastError(); g.warm = false; g.n_heads = 0;
-      ctx->launches = l0;
-      LL_TRY(frame_front_end_device(ctx, fs, fa, n_heads, ns, pieces, pc));
-    } else {
-      g.launches = ctx->launches - l0;
-      LL_CUDA(ctx, cudaGraphInstantiate(&g.exec, graph, 0));
-      cudaGraphDestroy(graph);
-      LL_CUDA(ctx, cudaGraphLaunch(g.exec, s));
-    }
-  } else {
-    if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
-    LL_TRY(frame_front_end_device(ctx, fs, fa, n_heads, ns, pieces, pc));
-    g.n_heads = n_heads; memcpy(g.ns, ns, (size_t)n_heads * sizeof(size_t)); g.pieces = pieces; g.pc = *pc; g.warm = true;
-  }
-  return LL_OK;
+  FrontKey key; key.n_heads = n_heads; std::copy(ns, ns + n_heads, key.ns); key.pieces = pieces; key.pc = *pc;
+  return front_graph(ctx, *fa.graph, s, key, true, [&] { return frame_front_end_device(ctx, fs, fa, n_heads, ns, pieces, pc); });
 }
 
 extern "C" {

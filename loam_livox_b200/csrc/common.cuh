@@ -170,6 +170,21 @@ struct SyncEvents {
 };
 // The streams and ordering events one front end is enqueued on: the main chain, the corner VoxelGrid chain, the petal bookkeeping.
 struct FrontStreams { cudaStream_t main, corner, petals; cudaEvent_t fork, join, fork3, join3; };
+// The shape of a front end: what decides the work it enqueues (a scan: one head and pieces 0, the piece count being part of pc).  n_heads == 0
+// matches no call.
+#define LL_MAX_HEADS 8
+static_assert(sizeof(ll_pipeline_cfg) == 7 * 4, "ll_pipeline_cfg is compared bytewise: no padding");
+struct FrontKey {
+  int n_heads = 0, pieces = 0; size_t ns[LL_MAX_HEADS] = {}; ll_pipeline_cfg pc = {};
+  bool operator==(const FrontKey& o) const {
+    if (n_heads != o.n_heads || pieces != o.pieces || memcmp(&pc, &o.pc, sizeof(pc)) != 0) return false;
+    for (int h = 0; h < n_heads; h++) if (ns[h] != o.ns[h]) return false;
+    return true;
+  }
+};
+// The device part of a front end replayed as ONE CUDA graph: its enqueue cost on the host (CUB dispatch included) is longer than its execution.
+// Every buffer it touches is fixed, so it is captured at the second call of a shape and replayed from the third (front_graph, api.cu).
+struct FrontGraph { cudaGraphExec_t exec = nullptr; FrontKey key; bool warm = false; uint64_t launches = 0; };
 
 struct ll_ctx {
   int device = 0;
@@ -207,10 +222,7 @@ struct ll_ctx {
   cudaStream_t fe_stream[3] = {nullptr, nullptr, nullptr};
   FrontStreams own_front() const { return {stream, stream2, stream3, sev.fork, sev.join, sev.fork3, sev.join3}; }   // the single-input calls'
   FrontStreams pipe_front() const { return {fe_stream[0], fe_stream[1], fe_stream[2], sev.fe_fork, sev.fe_join, sev.fe_fork3, sev.fe_join3}; }
-  // The per-scan front end (extract + get_features + 4 VoxelGrids + count read-back) replayed as ONE CUDA graph: ~60 launches whose
-  // enqueue cost on the host (CUB dispatch included) was longer than their execution.  Every buffer it touches is fixed at creation, so it is
-  // re-captured only when the scan size or the pipeline config changes.
-  struct FrontGraph { cudaGraphExec_t exec = nullptr; size_t n = 0; ll_pipeline_cfg pc; bool warm = false; uint64_t launches = 0; } fg;
+  FrontGraph fg;   // the per-scan front end (extract + get_features + 4 VoxelGrids + count read-back)
   int reg_deblur = 0;                      // if_motion_deblur of the registration whose blocks are on the device
   int solve_world = 1;                     // world size the solver kernels all-reduce over (1 unless the map in use is sharded)
   void* comm_local = nullptr;              // this rank's staging slot (device memory, IPC-exported)

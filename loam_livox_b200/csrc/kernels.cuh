@@ -72,7 +72,6 @@ struct RegDevState {
 // The piecewise frame front end (frame_front_end).  get_features decides range membership per point and the class of a point does not
 // depend on the range, so the corner / surface / full clouds of piece i are contiguous slices of the whole-scan compaction (bounds 0 ... 1):
 // from the prefix count at the first index inside the piece's bounds to the prefix count past the last one.
-#define LL_MAX_HEADS 8
 #define LL_MAX_PIECES 16
 struct FrameSlices {                   // one head: per class (corner, surface, full) and piece, the slice of the head's compaction
   int off[3][LL_MAX_PIECES], len[3][LL_MAX_PIECES];
@@ -224,12 +223,9 @@ int scan_front_end_enqueue(ll_ctx* ctx, const FrontStreams& fs, const void* raw,
 int scan_front_end_finish(ll_ctx* ctx, cudaStream_t s, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);
 int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);
 // The device arrays of a piecewise frame front end (owned by the streaming mapper): gathered segments of cap points per class, the first
-// VoxelGrids' outputs, and the segmented VoxelGrids' scratch arenas (vg[0] on the context's stream, vg[1] on stream2).
-// The device part of a piecewise frame front end (everything after the uploads) replayed as one CUDA graph, one per arena: its buffers are
-// fixed, so it is re-captured only when the frame's shape changes (head count, per-head sizes, pieces, pipeline config).  The uploads and the
-// extractor's bookkeeping stay outside it, so the format and the caller's pointers do not enter the graph.
-struct FrameGraph { cudaGraphExec_t exec = nullptr; int n_heads = 0; size_t ns[LL_MAX_HEADS] = {}; int pieces = 0; ll_pipeline_cfg pc = {}; bool warm = false; uint64_t launches = 0; };
-struct FrameArena { FrameDev* dev; float4* cls[2]; float4* mid[2]; int cap; DevBuf* vg[2]; FrameGraph* graph; };
+// VoxelGrids' outputs, the segmented VoxelGrids' scratch arenas (vg[0] on the context's stream, vg[1] on stream2), and the graph of the
+// device part (everything after the uploads, so the format and the caller's pointers do not enter it), one per arena.
+struct FrameArena { FrameDev* dev; float4* cls[2]; float4* mid[2]; int cap; DevBuf* vg[2]; FrontGraph* graph; };
 // Every head through the extractor, the slices of every piece, the gathers and the four segmented VoxelGrids (laser_feature_extractor.hpp:
 // 303-380, laser_mapping.hpp:1367-1373), enqueued on `fs` without a host synchronisation (the device part replayed as fa.graph once the
 // shape repeats); dev->out lands in ctx->pin->frame.  Piece i's features

@@ -71,7 +71,7 @@ struct ll_mapper {
   // the piecewise front end (FrameLayout; segmented VoxelGrid scratch of its main / corner chain).  Two arenas: ll_mapper_process_frames reads
   // frame f's pieces out of frame[f & 1] while the front end of frame f + 1 fills the other; ll_mapper_process_frame uses frame[0].
   DevBuf frame[2], frame_vg[2];
-  FrameGraph frame_graph[2];   // the device part of the front end, replayed per arena
+  FrontGraph frame_graph[2];   // the device part of the front end, replayed per arena
   int frame_pieces = 0;        // the pieces `frame` was laid out for
 };
 
@@ -161,7 +161,7 @@ void ll_mapper_release(ll_mapper* m) {
   ll_cellmap_release(m->cells_corner); ll_cellmap_release(m->cells_surf);
   if (m->match_map) ll_map_release(m->match_map);
   m->work.release(); m->snap.release(); m->his_corner.release(); m->his_surf.release();
-  for (FrameGraph& g : m->frame_graph) if (g.exec) cudaGraphExecDestroy(g.exec);
+  for (FrontGraph& g : m->frame_graph) if (g.exec) cudaGraphExecDestroy(g.exec);
   m->frame[0].release(); m->frame[1].release(); m->frame_vg[0].release(); m->frame_vg[1].release(); delete m;
 }
 int ll_mapper_pose(const ll_mapper* m, double q_wxyz[4], double t[3], int* frame_index) {
