@@ -82,6 +82,7 @@ int ll_ctx_create(const ll_config* cfg, int device, ll_ctx** out) {
   // one registration state per batch item (d_reg[0]: ll_register and the parity hooks)
   void* dreg = nullptr; ok(cudaMalloc(&dreg, LL_MAX_BATCH * sizeof(RegDevState))); if (dreg) ok(cudaMemset(dreg, 0, LL_MAX_BATCH * sizeof(RegDevState))); ctx->d_reg = (RegDevState*)dreg;
   if (e == cudaSuccess && solve_prepare(ctx) != LL_OK) e = cudaErrorUnknown;   // per-function attributes of the solver kernels (no process-global flag: contexts are created from any thread)
+  if (e == cudaSuccess && voxel_grid_prepare(ctx) != LL_OK) e = cudaErrorUnknown;
   if (e == cudaSuccess && ctx_alloc(ctx) != LL_OK) e = cudaErrorMemoryAllocation;
   if (e != cudaSuccess) { cudaGetLastError(); ll_ctx_destroy(ctx); return LL_ERR_CUDA; }
   *out = ctx; return LL_OK;
@@ -832,20 +833,15 @@ int ll_debug_solver_cycles(ll_ctx* ctx, long long out8[16]) {
 // (laser_feature_extractor.hpp:285-380) and the mapping node's input VoxelGrids (laser_mapping.hpp:1367-1373).  Leaves the features in
 // A.feat (corners then surfaces).  *dropped = 1 when the frame has <= 5 petals (:287).
 // The four VoxelGrids of a frame's features (laser_feature_extractor.hpp:372-380 then laser_mapping.hpp:1367-1373): the corner chain
-// tmp_a -> tmp_d -> tmp_a on fs.corner (fe_corner), the surface chain tmp_b -> tmp_c -> tmp_b on fs.main (fe_main).  The input
-// counts are nc_cap / ns_cap, or the device counts d_nc / d_ns when given; the outputs land in counts[4..7].
+// tmp_a -> tmp_d -> tmp_a, the surface chain tmp_b -> tmp_c -> tmp_b, as one cluster launch on fs.main when they fit (launch_voxel_chains),
+// else the corner chain on fs.corner (fe_corner) and the surface chain on fs.main (fe_main).  The input counts are nc_cap / ns_cap, or the
+// device counts d_nc / d_ns when given; the outputs land in counts[4..7].
 static int voxel_chains(ll_ctx* ctx, const FrontStreams& fs, const ll_pipeline_cfg* pc, int nc_cap, const int* d_nc, int ns_cap, const int* d_ns) {
-  cudaStream_t s = fs.main, s2 = fs.corner;
   const RegArrays& A = ctx->A; int* cnt = A.counts;
-  LL_CUDA(ctx, cudaEventRecord(fs.fork, s));
-  LL_CUDA(ctx, cudaStreamWaitEvent(s2, fs.fork, 0));
-  LL_TRY(launch_voxel_grid(ctx, s2, ctx->fe_corner, A.tmp_a, nc_cap, d_nc, pc->extractor_leaf_corner, A.tmp_d, cnt + 4));
-  LL_TRY(launch_voxel_grid(ctx, s2, ctx->fe_corner, A.tmp_d, nc_cap, cnt + 4, pc->mapping_leaf_corner, A.tmp_a, cnt + 5));
-  LL_CUDA(ctx, cudaEventRecord(fs.join, s2));
-  LL_TRY(launch_voxel_grid(ctx, s, ctx->fe_main, A.tmp_b, ns_cap, d_ns, pc->extractor_leaf_surf, A.tmp_c, cnt + 6));
-  LL_TRY(launch_voxel_grid(ctx, s, ctx->fe_main, A.tmp_c, ns_cap, cnt + 6, pc->mapping_leaf_surf, A.tmp_b, cnt + 7));
-  LL_CUDA(ctx, cudaStreamWaitEvent(s, fs.join, 0));
-  return LL_OK;
+  const VgChain c[2] = {
+      {{A.tmp_a, nc_cap, d_nc, 2, {pc->extractor_leaf_corner, pc->mapping_leaf_corner}, {A.tmp_d, A.tmp_a}, {cnt + 4, cnt + 5}}, &ctx->fe_corner, fs.corner},
+      {{A.tmp_b, ns_cap, d_ns, 2, {pc->extractor_leaf_surf, pc->mapping_leaf_surf}, {A.tmp_c, A.tmp_b}, {cnt + 6, cnt + 7}}, &ctx->fe_main, fs.main}};
+  return launch_voxel_chains(ctx, fs.main, c, 2, fs.fork, fs.join);
 }
 
 // Everything of the front end that is enqueued on the device, in the order the reference runs it; counts land in pinned memory.

@@ -194,6 +194,14 @@ int launch_voxel_grid(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4
 // null when nseg == 1): each segment filtered as if alone, the outputs one segment after another, d_out_end[s] = the end of segment s's output.
 int launch_voxel_grid_segments(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_in, int n_cap, const int* d_end, int nseg, float leaf, float4* d_out, int* d_out_end);
 size_t voxel_grid_bytes(int n_cap, int nseg = 1);   // what launch_voxel_grid(_segments) carves from `scratch`
+// A chain of nvg (1 or 2) VoxelGrids, each on the previous one's output: in [n_cap points, or the device count *d_n_in clamped to n_cap]
+// -> out[0] (*d_n_out[0]) -> out[1] (*d_n_out[1]).
+struct VgChainDev { const float4* in; int n_cap; const int* d_n_in; int nvg; float leaf[2]; float4* out[2]; int* d_n_out[2]; };
+struct VgChain { VgChainDev d; DevBuf* scratch; cudaStream_t s; };   // scratch and stream of the CUB pass
+// nchains (1 or 2) chains ordered on stream s: one launch, one cluster per chain, when every n_cap is small enough, else each chain's CUB passes
+// on its own stream (at most one stream other than s: it forks from s through `fork` and s waits for it through `join`).
+int launch_voxel_chains(ll_ctx* ctx, cudaStream_t s, const VgChain* c, int nchains, cudaEvent_t fork, cudaEvent_t join);
+int voxel_grid_prepare(ll_ctx* ctx);   // once per context: opt the cluster VoxelGrid kernel in to its shared memory and its 16-CTA clusters
 
 // ---------------------------------------------------------------------------------------------- extractor (extract.cu)
 int extract_alloc(ll_ctx* ctx);   // ExtractState arrays for max_scan_points (ll_ctx_create)
