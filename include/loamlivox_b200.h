@@ -362,6 +362,65 @@ int  ll_mapper_process_scans(ll_mapper* mapper, int n_scans, const void* const* 
                              ll_reg_result* out, ll_mapper_stats* stats, int* n_scans_done);
 int  ll_mapper_pose(const ll_mapper* mapper, double q_wxyz[4], double t[3], int* frame_index);
 
+/* ---- checkpoint: the whole streaming mapper as one byte image ------------------------------------------------------------------------
+ * Stop a mapping run and resume it in another process or on another GPU, keep a map for the next session, move a stream between contexts.
+ * A mapper restored from an image continues bit for bit as the one that was saved: every ll_reg_result field except gpu_ms_*, every integer
+ * field of ll_mapper_stats and ll_mapper_pose.  (The reference persists its cell map as JSON, cell_map_keyframe.hpp:818-914; this is a
+ * binary image of the whole mapper instead.)
+ *
+ * Format (version 1), one little-endian byte string:
+ *   ll_mapper_image_header      magic "LLMAPIMG", version, config_bytes = sizeof(ll_mapper_config), total_bytes = the image's size, and
+ *                               one (offset, length) per section, in the order of the LL_IMAGE_* indices below
+ *   LL_IMAGE_CONFIG             the ll_mapper_config the mapper was created with, verbatim
+ *   LL_IMAGE_SCALARS            ll_mapper_image_scalars
+ *   LL_IMAGE_HISTORY_{CORNER,SURF}   the history window of one class (mode 0's match map):
+ *                               int64 n_segments, int64 n_points, int32 size[n_segments] (oldest first), ll_point points[n_points] (window order)
+ *   LL_IMAGE_SNAPSHOT_{CORNER,SURF}  the whole-map VoxelGrid output the current kNN index was built from (empty when have_map = 0):
+ *                               int64 n, ll_point points[n]
+ *   LL_IMAGE_CELLS_{CORNER,SURF}     one cell map: int32 current_frame_idx, int32 n_out_of_range, int64 n_cells, int64 n_points,
+ *                               ll_image_cell cells[n_cells] (every cell of the table, also cells without a live point, in ascending key),
+ *                               ll_image_cell_point points[n_points] (the live points only, in store order)
+ * A writer places the sections back to back after the header in index order.  The image is canonical: it depends only on the mapper's
+ * observable state, never on hash-slot placement, dead store entries, epochs, table capacity, reservations or arena offsets, so the same
+ * stream gives byte-identical images and load-then-save reproduces an image byte for byte.  Front-end graphs and launch counters are not
+ * saved (a restored mapper captures its graphs afresh).  Images are not portable across endianness. */
+#define LL_MAPPER_IMAGE_MAGIC "LLMAPIMG"
+#define LL_MAPPER_IMAGE_VERSION 1
+enum { LL_IMAGE_CONFIG = 0, LL_IMAGE_SCALARS = 1, LL_IMAGE_HISTORY_CORNER = 2, LL_IMAGE_HISTORY_SURF = 3, LL_IMAGE_SNAPSHOT_CORNER = 4,
+       LL_IMAGE_SNAPSHOT_SURF = 5, LL_IMAGE_CELLS_CORNER = 6, LL_IMAGE_CELLS_SURF = 7, LL_IMAGE_SECTIONS = 8 };
+typedef struct { uint64_t offset, length; } ll_image_section;
+typedef struct { char magic[8]; uint32_t version, config_bytes; uint64_t total_bytes; ll_image_section section[LL_IMAGE_SECTIONS]; } ll_mapper_image_header;   /* 152 B */
+typedef struct {
+  int32_t frame_index;                          /* m_current_frame_index                                                                  */
+  int32_t map_dirty, have_map;                  /* 0 / 1: the match map is refreshed at the next step / the kNN index exists             */
+  int32_t snap_n[2], fov[2];                    /* what the next ll_mapper_stats reports when map_dirty = 0 (map_*, cells_in_fov_*)      */
+  int32_t reserved;                             /* 0                                                                                      */
+  double  last_time_stamp;                      /* m_last_time_stamp                                                                      */
+  double  q_w_curr[4], t_w_curr[3];             /* the pose                                                                               */
+  double  last_his_add_q[4], last_his_add_t[3]; /* m_last_his_add_q / _t                                                                  */
+  double  first_receive_time, current_time, last_maximum_time_stamp;   /* the context's extractor time bookkeeping                       */
+} ll_mapper_image_scalars;                      /* 176 B */
+typedef struct { uint64_t key; int32_t create_frame, last_update; } ll_image_cell;   /* key: cell index (k, j, i) + 2^20 in 21 bits each, k highest */
+typedef struct { float x, y, z; int32_t cell; } ll_image_cell_point;               /* cell: index into the section's cell list */
+typedef struct {
+  uint64_t bytes;
+  int64_t  history_points[2], snapshot_points[2], cells[2], cell_points[2];   /* [0] corner, [1] surface; cell_points: live points */
+  uint32_t version;
+  int32_t  matching_mode, frame_index, have_map, map_dirty;
+  int32_t  history_segments[2], cell_frame_idx[2];
+  int32_t  reserved;
+} ll_image_info;                                /* 112 B */
+/* image NULL: *bytes = the size needed.  cap < needed: LL_ERR_CAPACITY, nothing written (*bytes = the size needed).  The mapper is not modified. */
+int  ll_mapper_save(ll_mapper* mapper, void* image, size_t cap, size_t* bytes);
+/* A new mapper on ctx in the image's state.  cfg NULL: the image's config.  Otherwise cfg must equal it in every field except max_cells,
+ * reserve_map_points and reserve_store_points (LL_ERR_INVALID), which size the new mapper's buffers only: its own images keep the image's
+ * config, so that load-then-save reproduces the image byte for byte.  Sets ctx's extractor time bookkeeping,
+ * as ll_mapper_create resets it.  The image is validated completely before anything touches the device: a refused image (LL_ERR_INVALID; a
+ * cell map with more cells than half the table of the effective max_cells: LL_ERR_CAPACITY) creates nothing and changes nothing. */
+int  ll_mapper_load(ll_ctx* ctx, const void* image, size_t bytes, const ll_mapper_config* cfg, ll_mapper** out);
+/* Host only, no context or GPU: validates an image completely (as ll_mapper_load with cfg NULL) and reports what is in it. */
+int  ll_mapper_image_info(const void* image, size_t bytes, ll_image_info* info);
+
 /* ---- wire formats (SURVEY 8(f) N3) ---------------------------------------------------------------------------------------------- */
 /* Layout of one point record of an LL_FMT_STRIDED input: what pcl::fromROSMsg (laser_feature_extractor.hpp:275) resolves by field name from a
  * sensor_msgs/PointCloud2 (point_step, the offsets of the little-endian fields x, y, z, intensity and intensity's datatype).  The payload is

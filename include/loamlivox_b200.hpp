@@ -10,7 +10,9 @@
 #pragma once
 #include <algorithm>
 #include <array>
+#include <cstdint>
 #include <cstring>
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -274,10 +276,28 @@ class Laser_mapping {
     std::vector<int> status; for (const ll_reg_result& x : r) status.push_back(x.status);
     return status;
   }
+  // the whole mapper as one byte image (ll_mapper_save; format in loamlivox_b200.h): load_from_image of it, on any context, continues bit for
+  // bit as this mapper does.  The mapper is not modified.
+  void save_to_image(std::vector<uint8_t>& image) const {
+    size_t n = 0;
+    ctx_.check(ll_mapper_save(mapper_, nullptr, 0, &n));
+    image.resize(n);
+    ctx_.check(ll_mapper_save(mapper_, image.data(), image.size(), &n));
+  }
+  // a mapper on ctx in the state of `image` (ll_mapper_load).  cfg NULL: the image's config; otherwise it may differ from it only in
+  // max_cells, reserve_map_points and reserve_store_points.  A refused image throws and creates nothing.
+  static std::unique_ptr<Laser_mapping> load_from_image(Context& ctx, const std::vector<uint8_t>& image, const ll_mapper_config* cfg = nullptr) {
+    ll_mapper* m = nullptr;
+    ctx.check(ll_mapper_load(ctx.get(), image.data(), image.size(), cfg, &m));
+    std::unique_ptr<Laser_mapping> out(new Laser_mapping(ctx, m));
+    ctx.check(ll_mapper_pose(m, out->m_q_w_curr.data(), out->m_t_w_curr.data(), &out->m_current_frame_index));
+    return out;
+  }
   std::array<double, 4> m_q_w_curr{{1, 0, 0, 0}};   // (w, x, y, z)
   std::array<double, 3> m_t_w_curr{{0, 0, 0}};
   int m_current_frame_index = 0;
  private:
+  Laser_mapping(Context& ctx, ll_mapper* m) : ctx_(ctx), mapper_(m) { ll_mapper_config_default(&cfg_); }
   Context& ctx_; ll_mapper_config cfg_; ll_mapper* mapper_ = nullptr;
 };
 

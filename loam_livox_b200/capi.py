@@ -20,6 +20,9 @@ LL_OK, LL_ERR_INVALID, LL_ERR_CUDA, LL_ERR_CAPACITY, LL_ERR_NO_BLOCKS, LL_ERR_CA
 LL_IPC_HANDLE_BYTES = 64
 LL_MAX_PIECES_PER_FRAME = 16
 LL_MAX_BATCH = 16
+LL_MAPPER_IMAGE_MAGIC, LL_MAPPER_IMAGE_VERSION = b"LLMAPIMG", 1
+(LL_IMAGE_CONFIG, LL_IMAGE_SCALARS, LL_IMAGE_HISTORY_CORNER, LL_IMAGE_HISTORY_SURF, LL_IMAGE_SNAPSHOT_CORNER, LL_IMAGE_SNAPSHOT_SURF, LL_IMAGE_CELLS_CORNER,
+ LL_IMAGE_CELLS_SURF, LL_IMAGE_SECTIONS) = range(9)
 
 EXPORTS = [
     "ll_config_default", "ll_ctx_create", "ll_ctx_destroy", "ll_ctx_warmup", "ll_last_error", "ll_ctx_stream", "ll_ctx_sync", "ll_extract", "ll_extract_reset", "ll_piece_bounds",
@@ -29,6 +32,7 @@ EXPORTS = [
     "ll_cellmap_assemble", "ll_cellmap_reserve", "ll_cellmap_stats", "ll_voxel_downsample_dev", "ll_transform_dev", "ll_last_features_dev", "ll_mapper_config_default", "ll_mapper_create", "ll_mapper_release",
     "ll_mapper_process_scan", "ll_mapper_pose", "ll_map_rebuild", "ll_debug_solver_cycles", "ll_state_snapshot_bytes", "ll_set_point_layout", "ll_format_pose_log", "ll_reg_state_yaml", "ll_cap_uniform", "ll_map_shard_info", "ll_shard_plan", "ll_align_cfg_default", "ll_scene_align", "ll_frame_to_pose", "ll_features_to_pointcloud2",
     "ll_mapper_process_frame", "ll_voxel_downsample_segments", "ll_register_batch", "ll_mapper_process_frames", "ll_mapper_process_scans",
+    "ll_mapper_save", "ll_mapper_load", "ll_mapper_image_info",
 ]
 
 
@@ -76,6 +80,13 @@ class MapperConfig(C.Structure):
 class MapperStats(C.Structure):
     _fields_ = [(n, C.c_int) for n in ("n_corner", "n_surf", "map_corner", "map_surf", "cells_in_fov_corner", "cells_in_fov_surf", "appended_corner", "appended_surf")] + \
                [(n, C.c_float) for n in ("ms_front_end", "ms_refresh", "ms_register", "ms_append")]
+
+
+class ImageInfo(C.Structure):
+    """ll_image_info: what ll_mapper_image_info reports about a mapper image ([0] corner, [1] surface)."""
+    _fields_ = [("bytes", C.c_uint64), ("history_points", C.c_int64 * 2), ("snapshot_points", C.c_int64 * 2), ("cells", C.c_int64 * 2), ("cell_points", C.c_int64 * 2),
+                ("version", C.c_uint32), ("matching_mode", C.c_int), ("frame_index", C.c_int), ("have_map", C.c_int), ("map_dirty", C.c_int),
+                ("history_segments", C.c_int * 2), ("cell_frame_idx", C.c_int * 2), ("reserved", C.c_int)]
 
 
 class ShardInfo(C.Structure):
@@ -172,6 +183,9 @@ def lib():
     L.ll_mapper_process_frames.argtypes = [vp, ci, ci, vp, vp, ci, ci, vp, ci, C.POINTER(RegResult), C.POINTER(MapperStats), ci, vp, C.POINTER(ci)]
     L.ll_mapper_process_scans.argtypes = [vp, ci, vp, vp, ci, ci, vp, C.POINTER(RegResult), C.POINTER(MapperStats), C.POINTER(ci)]
     L.ll_mapper_pose.argtypes = [vp, vp, vp, C.POINTER(ci)]
+    L.ll_mapper_save.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.ll_mapper_load.argtypes = [vp, vp, sz, C.POINTER(MapperConfig), C.POINTER(vp)]
+    L.ll_mapper_image_info.argtypes = [vp, sz, C.POINTER(ImageInfo)]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64
     _LIB = L

@@ -401,3 +401,149 @@ int ll_cellmap_assemble(ll_ctx* ctx, ll_cellmap* m, const double q_wxyz[4], cons
 }
 
 }  // extern "C"
+
+// ---- checkpoint (ll_mapper_save / ll_mapper_load) ---------------------------------------------------------------------------------
+// A map leaves as its cells in ascending key (key, create_frame, last_update) and its live points in store order (xyz, rank of the cell in
+// that list), and comes back into an empty table with every cell at epoch 0, bump -1 and every point at epoch 0.  Nothing a result depends on
+// changes: the assembly ranks cells by key and keeps store order inside a voxel, and liveness is only "point epoch == cell epoch".
+__global__ void cm_occupied_kernel(const unsigned long long* __restrict__ keys, int cap, unsigned char* __restrict__ flag) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s < cap) flag[s] = keys[s] != CM_EMPTY ? 1 : 0;
+}
+__global__ void cm_live_kernel(const int* __restrict__ pt_slot, const int* __restrict__ pt_epoch, int n, const int* __restrict__ epoch, unsigned char* __restrict__ flag) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const int s = pt_slot[t];
+  flag[t] = (s >= 0 && pt_epoch[t] == epoch[s]) ? 1 : 0;
+}
+__global__ void cm_export_cells_kernel(const unsigned long long* __restrict__ sorted_keys, const int* __restrict__ sorted_slots, int n, const int* __restrict__ create_frame,
+                                       const int* __restrict__ last_update, ll_image_cell* __restrict__ out) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const int s = sorted_slots[r];
+  ll_image_cell c; c.key = sorted_keys[r]; c.create_frame = create_frame[s]; c.last_update = last_update[s];
+  out[r] = c;
+}
+__global__ void cm_export_points_kernel(const float4* __restrict__ pts, const int* __restrict__ pt_slot, const int* __restrict__ idx, int n, const int* __restrict__ rank_of_slot,
+                                        ll_image_cell_point* __restrict__ out) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const int t = idx[r]; const float4 p = pts[t];
+  ll_image_cell_point o; o.x = p.x; o.y = p.y; o.z = p.z; o.cell = rank_of_slot[pt_slot[t]];
+  out[r] = o;
+}
+// one thread per cell: the probe sequence of cm_locate_kernel into an empty table (keys are distinct, so every CAS claims a fresh slot)
+__global__ void cm_import_cells_kernel(const ll_image_cell* __restrict__ in, int n, unsigned long long* keys, unsigned mask, int* create_frame, int* last_update, int* epoch, int* bump,
+                                       int* __restrict__ slot_of_rank) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const ll_image_cell c = in[r];
+  unsigned h = cm_hash(c.key, mask);
+  while (atomicCAS(&keys[h], CM_EMPTY, c.key) != CM_EMPTY) h = (h + 1) & mask;
+  create_frame[h] = c.create_frame; last_update[h] = c.last_update; epoch[h] = 0; bump[h] = -1;
+  slot_of_rank[r] = (int)h;
+}
+__global__ void cm_import_points_kernel(const ll_image_cell_point* __restrict__ in, int n, const int* __restrict__ slot_of_rank, float4* __restrict__ pts, int* __restrict__ pt_slot,
+                                        int* __restrict__ pt_epoch) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const ll_image_cell_point p = in[t];
+  pts[t] = make_float4(p.x, p.y, p.z, 0.f); pt_slot[t] = slot_of_rank[p.cell]; pt_epoch[t] = 0;
+}
+
+// The export's scratch over a table of T slots and a store of N points; rec = the cells then the live points, as the image holds them
+struct CmExport {
+  size_t cub_bytes = 0;
+  unsigned char* flag; int* slots; unsigned long long* keys; unsigned long long* keys2; int* slots2; int* rank; int* idx; int* cnt; char* cub_tmp; int4* rec;
+  CmExport(int T, int N) {
+    size_t cub_a = 0, cub_b = 0;
+    cub::DeviceSelect::Flagged(nullptr, cub_a, cub::CountingInputIterator<int>(0), (unsigned char*)nullptr, (int*)nullptr, (int*)nullptr, T > N ? T : N);
+    cub::DeviceRadixSort::SortPairs(nullptr, cub_b, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr, T, 0, 64);
+    cub_bytes = cub_a > cub_b ? cub_a : cub_b;
+  }
+  void layout(Carve& c, size_t T, size_t N, size_t n_rec) {
+    flag = c.take<unsigned char>(T > N ? T : N); slots = c.take<int>(T); keys = c.take<unsigned long long>(T); keys2 = c.take<unsigned long long>(T);
+    slots2 = c.take<int>(T); rank = c.take<int>(T); idx = c.take<int>(N); cnt = c.take<int>(16); cub_tmp = c.take<char>(cub_bytes); rec = c.take<int4>(n_rec);
+  }
+};
+
+// Cells in the table and live points in the store, the frame index and the out-of-range count (the map is only read)
+int cm_count(ll_ctx* ctx, ll_cellmap* m, int* n_cells, int* n_live, int* frame_idx, int* n_out_of_range) {
+  *frame_idx = m->current_frame_idx; *n_out_of_range = m->n_out_of_range;
+  cudaStream_t s = ctx->stream;
+  int* d = nullptr;
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { d = c.take<int>(1); }));
+  LL_CUDA(ctx, cudaMemsetAsync(d, 0, 4, s));
+  if (m->n_pts > 0) { cm_count_alive_kernel<<<ll_div_up(m->n_pts, 256), 256, 0, s>>>(m->pt_slot, m->pt_epoch, m->n_pts, m->epoch, d); ctx->launches++; }
+  int h[2] = {0, 0};
+  LL_CUDA(ctx, cudaMemcpyAsync(h, m->d_counters, 4, cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(h + 1, d, 4, cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  *n_cells = h[0]; *n_live = h[1];
+  return LL_OK;
+}
+
+// The map's cells (ascending key) and live points (store order) into out: n_cells ll_image_cell then n_live ll_image_cell_point, the counts
+// cm_count gave.  One copy to the host; the map's buffers are only read.
+int cm_export(ll_ctx* ctx, ll_cellmap* m, int n_cells, int n_live, void* out) {
+  cudaStream_t s = ctx->stream;
+  const int T = m->table_cap, N = m->n_pts;
+  if (n_cells + n_live == 0) return LL_OK;
+  CmExport a(T, N);
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { a.layout(c, T, N, (size_t)n_cells + n_live); }));
+  ll_image_cell* cells = (ll_image_cell*)a.rec; ll_image_cell_point* pts = (ll_image_cell_point*)(a.rec + n_cells);
+  size_t cub_c = a.cub_bytes;
+  LL_CUDA(ctx, cudaMemsetAsync(a.cnt, 0, 8, s));
+  // cells: occupied slots, sorted by key, and the rank of every slot
+  cm_occupied_kernel<<<ll_div_up(T, 256), 256, 0, s>>>(m->keys, T, a.flag);
+  LL_CUDA(ctx, cub::DeviceSelect::Flagged(a.cub_tmp, cub_c, cub::CountingInputIterator<int>(0), a.flag, a.slots, a.cnt + 0, T, s));
+  ctx->launches += 2;
+  if (n_cells > 0) {
+    cm_gather_keys_kernel<<<ll_div_up(n_cells, 256), 256, 0, s>>>(m->keys, a.slots, a.cnt + 0, a.keys);
+    LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(a.cub_tmp, cub_c, a.keys, a.keys2, a.slots, a.slots2, n_cells, 0, 64, s));
+    cm_rank_kernel<<<ll_div_up(n_cells, 256), 256, 0, s>>>(a.slots2, n_cells, a.rank);
+    cm_export_cells_kernel<<<ll_div_up(n_cells, 256), 256, 0, s>>>(a.keys2, a.slots2, n_cells, m->create_frame, m->last_update, cells);
+    ctx->launches += 4;
+  }
+  // live points in store order
+  if (N > 0) {
+    cm_live_kernel<<<ll_div_up(N, 256), 256, 0, s>>>(m->pt_slot, m->pt_epoch, N, m->epoch, a.flag);
+    LL_CUDA(ctx, cub::DeviceSelect::Flagged(a.cub_tmp, cub_c, cub::CountingInputIterator<int>(0), a.flag, a.idx, a.cnt + 1, N, s));
+    ctx->launches += 2;
+    if (n_live > 0) { cm_export_points_kernel<<<ll_div_up(n_live, 256), 256, 0, s>>>(m->pts, m->pt_slot, a.idx, n_live, a.rank, pts); ctx->launches++; }
+  }
+  LL_CUDA(ctx, cudaGetLastError());
+  int h[2] = {0, 0};
+  LL_CUDA(ctx, cudaMemcpyAsync(h, a.cnt, 8, cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(out, a.rec, ((size_t)n_cells + n_live) * 16, cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  if (h[0] != n_cells || h[1] != n_live) { ctx->set_error("cell map changed while it was saved"); return LL_ERR_INVALID; }
+  return LL_OK;
+}
+
+// An empty map (just created) in the state of an exported one: in = n_cells ll_image_cell (ascending key) then n_live ll_image_cell_point,
+// host memory, validated by the caller (distinct keys, ranks < n_cells).
+int cm_import(ll_ctx* ctx, ll_cellmap* m, int frame_idx, int n_out_of_range, const void* in, int n_cells, int n_live) {
+  cudaStream_t s = ctx->stream;
+  if (m->n_pts != 0 || m->n_cells != 0) { ctx->set_error("import into a cell map that is not empty"); return LL_ERR_INVALID; }
+  if (n_cells > m->table_cap / 2) { ctx->set_error("cell table more than half full: create the map with a larger max_cells"); return LL_ERR_CAPACITY; }
+  if (n_live > 0) LL_TRY(cm_reserve_store(ctx, m, n_live));
+  int4* rec = nullptr; int* slot_of_rank = nullptr;
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { rec = c.take<int4>((size_t)n_cells + n_live); slot_of_rank = c.take<int>(n_cells); }));
+  if (n_cells + n_live > 0) LL_CUDA(ctx, cudaMemcpyAsync(rec, in, ((size_t)n_cells + n_live) * 16, cudaMemcpyHostToDevice, s));
+  if (n_cells > 0) {
+    cm_import_cells_kernel<<<ll_div_up(n_cells, 256), 256, 0, s>>>((const ll_image_cell*)rec, n_cells, m->keys, (unsigned)(m->table_cap - 1), m->create_frame, m->last_update,
+                                                                   m->epoch, m->bump, slot_of_rank);
+    ctx->launches++;
+  }
+  if (n_live > 0) {
+    cm_import_points_kernel<<<ll_div_up(n_live, 256), 256, 0, s>>>((const ll_image_cell_point*)(rec + n_cells), n_live, slot_of_rank, m->pts, m->pt_slot, m->pt_epoch);
+    ctx->launches++;
+  }
+  const int c[3] = {n_cells, 0, n_out_of_range};   // d_counters: cells, scratch, points out of the key's range so far
+  LL_CUDA(ctx, cudaMemcpyAsync(m->d_counters, c, sizeof(c), cudaMemcpyHostToDevice, s));
+  LL_CUDA(ctx, cudaGetLastError());
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  m->n_pts = n_live; m->n_cells = n_cells; m->current_frame_idx = frame_idx; m->n_out_of_range = n_out_of_range;
+  return LL_OK;
+}

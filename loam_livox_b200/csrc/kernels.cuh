@@ -221,6 +221,15 @@ int launch_piece_slices(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const floa
 int launch_gather_pieces(ll_ctx* ctx, cudaStream_t s, FrameDev* dev, const FrameBases& B, int n_heads, int pieces, int max_head_n,
                          const float4* src_c, const float4* src_s, float4* dst_c, float4* dst_s);
 
+// ---------------------------------------------------------------------------------------------- cell-map checkpoint (cellmap.cu)
+// Cells in the table and live points in the store, current_frame_idx and n_out_of_range; the map is only read.
+int cm_count(ll_ctx* ctx, ll_cellmap* m, int* n_cells, int* n_live, int* frame_idx, int* n_out_of_range);
+// The cells in ascending key then the live points in store order, as the image's cell section holds them (n_cells ll_image_cell, n_live
+// ll_image_cell_point, the counts cm_count gave), copied once to host memory `out`; the map is only read.
+int cm_export(ll_ctx* ctx, ll_cellmap* m, int n_cells, int n_live, void* out);
+// An empty map in the state cm_export recorded (records validated by the caller: keys distinct, cell ranks < n_cells).
+int cm_import(ll_ctx* ctx, ll_cellmap* m, int frame_idx, int n_out_of_range, const void* in, int n_cells, int n_live);
+
 // ---------------------------------------------------------------------------------------------- host driver pieces (api.cu)
 // Registration of the features already resident in A.feat (corners then surfaces): the batch of one.  Core of ll_register / ll_scan_to_pose.
 int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg_state* in, ll_reg_result* out);

@@ -12,6 +12,7 @@
 // runs at the start of the next scan (same pose, same map content), so the result is the reference's with maximum_parallel_thread = 1.
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -511,4 +512,281 @@ extern "C" int ll_mapper_process_scans(ll_mapper* m, int n_scans, const void* co
   if (st != LL_OK) sequence_unwind(ctx, ahead);
   *n_scans_done = done;
   return st;
+}
+
+// ---------------------------------------------------------------------------------------------- checkpoint
+// The image (format: include/loamlivox_b200.h) holds what the next steps read: the config, the scalars, the history window, the snapshot
+// the kNN index was built from (the index's own copy of its input, BucketTree::src), both cell maps and the extractor's time bookkeeping.
+// One host validator serves ll_mapper_image_info and ll_mapper_load, before anything touches the device.
+namespace {
+
+template <typename T> T rd(const uint8_t* p) { T v; memcpy(&v, p, sizeof(T)); return v; }
+template <typename T> void wr(uint8_t* p, const T& v) { memcpy(p, &v, sizeof(T)); }
+
+const size_t HIS_HEAD = 16, SNAP_HEAD = 8, CELLS_HEAD = 24;   // the fixed part of a history, snapshot and cell-map section
+
+struct ImageView {   // a validated image
+  ll_mapper_image_header h; ll_mapper_config cfg; ll_mapper_image_scalars sc;
+  struct { int64_t n_seg = 0, n_pts = 0; const uint8_t* sizes = nullptr; const uint8_t* pts = nullptr; } his[2];
+  struct { int64_t n = 0; const uint8_t* pts = nullptr; } snap[2];
+  struct { int32_t frame_idx = 0, n_oor = 0; int64_t n_cells = 0, n_pts = 0; const uint8_t* rec = nullptr; } cells[2];
+};
+struct ImageCounts { int64_t his_seg[2], his_pts[2], snap[2], cells[2], cell_pts[2]; };
+
+// The canonical placement: the sections back to back after the header, in index order.  Returns the image's size.
+size_t image_layout(const ImageCounts& n, ll_mapper_image_header* h) {
+  memset(h, 0, sizeof(*h));
+  memcpy(h->magic, LL_MAPPER_IMAGE_MAGIC, 8); h->version = LL_MAPPER_IMAGE_VERSION; h->config_bytes = sizeof(ll_mapper_config);
+  const uint64_t len[LL_IMAGE_SECTIONS] = {sizeof(ll_mapper_config), sizeof(ll_mapper_image_scalars),
+                                           HIS_HEAD + 4 * (uint64_t)n.his_seg[0] + 16 * (uint64_t)n.his_pts[0], HIS_HEAD + 4 * (uint64_t)n.his_seg[1] + 16 * (uint64_t)n.his_pts[1],
+                                           SNAP_HEAD + 16 * (uint64_t)n.snap[0], SNAP_HEAD + 16 * (uint64_t)n.snap[1],
+                                           CELLS_HEAD + 16 * (uint64_t)(n.cells[0] + n.cell_pts[0]), CELLS_HEAD + 16 * (uint64_t)(n.cells[1] + n.cell_pts[1])};
+  uint64_t off = sizeof(*h);
+  for (int k = 0; k < LL_IMAGE_SECTIONS; k++) { h->section[k].offset = off; h->section[k].length = len[k]; off += len[k]; }
+  h->total_bytes = off;
+  return (size_t)off;
+}
+
+bool finite_xyz(const uint8_t* p) { float v[3]; memcpy(v, p, 12); return std::isfinite(v[0]) && std::isfinite(v[1]) && std::isfinite(v[2]); }
+// the hash-table capacity ll_cellmap_create gives a map of max_cells
+int64_t table_capacity(int max_cells) { int64_t cap = 1 << 12; const int64_t want = 2 * (int64_t)(max_cells > 0 ? max_cells : (1 << 20)); while (cap < want) cap <<= 1; return cap; }
+
+// LL_OK, or the code and what is wrong.  cfg: the caller's config for a load (NULL: the image's).
+int image_validate(const void* image, size_t bytes, const ll_mapper_config* cfg, ImageView* v, std::string* err) {
+  auto fail = [&](const char* msg, int code = LL_ERR_INVALID) { if (err) *err = msg; return code; };
+  const uint8_t* b = (const uint8_t*)image;
+  if (!b || bytes < sizeof(ll_mapper_image_header)) return fail("shorter than the image header");
+  memcpy(&v->h, b, sizeof(v->h));
+  if (memcmp(v->h.magic, LL_MAPPER_IMAGE_MAGIC, 8) != 0) return fail("not a mapper image (magic)");
+  if (v->h.version != LL_MAPPER_IMAGE_VERSION) return fail("unknown image version");
+  if (v->h.config_bytes != sizeof(ll_mapper_config)) return fail("config size differs from this library's ll_mapper_config");
+  if (v->h.total_bytes != bytes) return fail("image size differs from the header's total_bytes");
+  // structure: every section inside the image after the header, no two overlapping
+  int order[LL_IMAGE_SECTIONS];
+  for (int k = 0; k < LL_IMAGE_SECTIONS; k++) {
+    const ll_image_section& s = v->h.section[k];
+    if (s.offset < sizeof(ll_mapper_image_header) || s.offset > bytes || s.length > bytes - s.offset) return fail("section outside the image");
+    order[k] = k;
+  }
+  std::sort(order, order + LL_IMAGE_SECTIONS, [&](int a, int c) {
+    const ll_image_section &x = v->h.section[a], &y = v->h.section[c];
+    return x.offset != y.offset ? x.offset < y.offset : x.length < y.length;
+  });
+  for (int k = 1; k < LL_IMAGE_SECTIONS; k++) {
+    const ll_image_section &p = v->h.section[order[k - 1]], &q = v->h.section[order[k]];
+    if (p.offset + p.length > q.offset) return fail("overlapping sections");
+  }
+  auto sec = [&](int k) { return b + v->h.section[k].offset; };
+  auto len = [&](int k) { return (uint64_t)v->h.section[k].length; };
+  // config: ll_mapper_create's checks and a matching mode the mapper knows
+  if (len(LL_IMAGE_CONFIG) != sizeof(ll_mapper_config)) return fail("config section length");
+  memcpy(&v->cfg, sec(LL_IMAGE_CONFIG), sizeof(v->cfg));
+  if (!(v->cfg.cell_resolution > 0.f) || v->cfg.threshold_cell_revisit < 1) return fail("config: cell_resolution must be > 0 and threshold_cell_revisit >= 1");
+  if (v->cfg.matching_mode != 0 && v->cfg.matching_mode != 1) return fail("config: matching_mode must be 0 or 1");
+  // scalars
+  if (len(LL_IMAGE_SCALARS) != sizeof(ll_mapper_image_scalars)) return fail("scalars section length");
+  memcpy(&v->sc, sec(LL_IMAGE_SCALARS), sizeof(v->sc));
+  const ll_mapper_image_scalars& sc = v->sc;
+  {
+    const double d[] = {sc.last_time_stamp, sc.q_w_curr[0], sc.q_w_curr[1], sc.q_w_curr[2], sc.q_w_curr[3], sc.t_w_curr[0], sc.t_w_curr[1], sc.t_w_curr[2],
+                        sc.last_his_add_q[0], sc.last_his_add_q[1], sc.last_his_add_q[2], sc.last_his_add_q[3], sc.last_his_add_t[0], sc.last_his_add_t[1], sc.last_his_add_t[2],
+                        sc.first_receive_time, sc.current_time, sc.last_maximum_time_stamp};
+    for (double x : d) if (!std::isfinite(x)) return fail("non-finite pose or time stamp");
+  }
+  if (sc.frame_index < 0 || (sc.map_dirty != 0 && sc.map_dirty != 1) || (sc.have_map != 0 && sc.have_map != 1) || sc.reserved != 0 ||
+      sc.snap_n[0] < 0 || sc.snap_n[1] < 0 || sc.fov[0] < 0 || sc.fov[1] < 0)
+    return fail("scalars out of range");
+  if (sc.have_map && (sc.snap_n[0] == 0 || sc.snap_n[1] == 0)) return fail("have_map with an empty snapshot");
+  for (int c = 0; c < 2; c++) {
+    // history window: counts x element sizes = the length, segment sizes summing to the points, finite points
+    {
+      const uint8_t* p = sec(LL_IMAGE_HISTORY_CORNER + c); const uint64_t L = len(LL_IMAGE_HISTORY_CORNER + c);
+      if (L < HIS_HEAD) return fail("history section shorter than its counts");
+      const int64_t ns = rd<int64_t>(p), np = rd<int64_t>(p + 8);
+      if (ns < 0 || np < 0 || (uint64_t)ns > (L - HIS_HEAD) / 4 || (uint64_t)np > (L - HIS_HEAD) / 16 || HIS_HEAD + 4 * (uint64_t)ns + 16 * (uint64_t)np != L)
+        return fail("history counts disagree with the section length");
+      int64_t sum = 0;
+      for (int64_t k = 0; k < ns; k++) { const int32_t z = rd<int32_t>(p + HIS_HEAD + 4 * k); if (z < 0) return fail("negative history segment size"); sum += z; }
+      if (sum != np) return fail("history segment sizes do not sum to its points");
+      const uint8_t* pts = p + HIS_HEAD + 4 * ns;
+      for (int64_t k = 0; k < np; k++) if (!finite_xyz(pts + 16 * k)) return fail("non-finite history point");
+      v->his[c].n_seg = ns; v->his[c].n_pts = np; v->his[c].sizes = p + HIS_HEAD; v->his[c].pts = pts;
+    }
+    // snapshot: as many points as snap_n when the index exists, none otherwise
+    {
+      const uint8_t* p = sec(LL_IMAGE_SNAPSHOT_CORNER + c); const uint64_t L = len(LL_IMAGE_SNAPSHOT_CORNER + c);
+      if (L < SNAP_HEAD) return fail("snapshot section shorter than its count");
+      const int64_t n = rd<int64_t>(p);
+      if (n < 0 || (uint64_t)n > (L - SNAP_HEAD) / 16 || SNAP_HEAD + 16 * (uint64_t)n != L) return fail("snapshot count disagrees with the section length");
+      if (n != (sc.have_map ? sc.snap_n[c] : 0)) return fail("snapshot disagrees with have_map / snap_n");
+      for (int64_t k = 0; k < n; k++) if (!finite_xyz(p + SNAP_HEAD + 16 * k)) return fail("non-finite snapshot point");
+      v->snap[c].n = n; v->snap[c].pts = p + SNAP_HEAD;
+    }
+    // cell map: keys strictly ascending with bit 63 clear, stamps <= current_frame_idx, ranks < the cell count, finite points
+    {
+      const uint8_t* p = sec(LL_IMAGE_CELLS_CORNER + c); const uint64_t L = len(LL_IMAGE_CELLS_CORNER + c);
+      if (L < CELLS_HEAD) return fail("cell-map section shorter than its counts");
+      const int32_t fi = rd<int32_t>(p), oor = rd<int32_t>(p + 4);
+      const int64_t nc = rd<int64_t>(p + 8), np = rd<int64_t>(p + 16);
+      if (nc < 0 || np < 0 || (uint64_t)nc > (L - CELLS_HEAD) / 16 || (uint64_t)np > (L - CELLS_HEAD) / 16 || CELLS_HEAD + 16 * (uint64_t)(nc + np) != L)
+        return fail("cell-map counts disagree with the section length");
+      if (fi < 0 || oor < 0) return fail("cell-map frame index or out-of-range count negative");
+      const uint8_t* cells = p + CELLS_HEAD;
+      uint64_t prev = 0;
+      for (int64_t k = 0; k < nc; k++) {
+        const ll_image_cell e = rd<ll_image_cell>(cells + 16 * k);
+        if (e.key >> 63) return fail("cell key with bit 63 set");
+        if (k > 0 && e.key <= prev) return fail("cell keys not strictly ascending");
+        if (e.create_frame < 0 || e.create_frame > fi || e.last_update < 0 || e.last_update > fi) return fail("cell stamp outside 0 ... current_frame_idx");
+        prev = e.key;
+      }
+      const uint8_t* pts = cells + 16 * nc;
+      for (int64_t k = 0; k < np; k++) {
+        const ll_image_cell_point q = rd<ll_image_cell_point>(pts + 16 * k);
+        if (!(std::isfinite(q.x) && std::isfinite(q.y) && std::isfinite(q.z))) return fail("non-finite cell-map point");
+        if (q.cell < 0 || q.cell >= nc) return fail("cell-map point's cell rank >= the cell count");
+      }
+      v->cells[c].frame_idx = fi; v->cells[c].n_oor = oor; v->cells[c].n_cells = nc; v->cells[c].n_pts = np; v->cells[c].rec = cells;
+    }
+  }
+  // the caller's config: the image's but for the buffer sizes
+  if (cfg) {
+    ll_mapper_config x = *cfg;
+    x.max_cells = v->cfg.max_cells; x.reserve_map_points = v->cfg.reserve_map_points; x.reserve_store_points = v->cfg.reserve_store_points;
+    if (memcmp(&x, &v->cfg, sizeof(x)) != 0) return fail("cfg differs from the image's config in a field other than max_cells, reserve_map_points, reserve_store_points");
+  }
+  const int64_t cap = table_capacity(cfg ? cfg->max_cells : v->cfg.max_cells);
+  for (int c = 0; c < 2; c++) {
+    if (v->cells[c].n_cells > cap / 2) return fail("cell table more than half full: create the map with a larger max_cells", LL_ERR_CAPACITY);
+    if (v->cells[c].n_pts > ((int64_t)1 << 30) || v->his[c].n_pts > INT32_MAX || v->snap[c].n > INT32_MAX) return fail("more points than a map holds", LL_ERR_CAPACITY);
+  }
+  return LL_OK;
+}
+
+// The validated image's state into a mapper just created with its effective config.
+int mapper_restore(ll_mapper* m, const ImageView& v) {
+  ll_ctx* ctx = m->ctx;
+  cudaStream_t s = ctx->stream;
+  const ll_mapper_image_scalars& sc = v.sc;
+  m->frame_index = sc.frame_index; m->last_time_stamp = sc.last_time_stamp;
+  for (int k = 0; k < 4; k++) { m->q_w_curr[k] = sc.q_w_curr[k]; m->last_his_add_q[k] = sc.last_his_add_q[k]; }
+  for (int k = 0; k < 3; k++) { m->t_w_curr[k] = sc.t_w_curr[k]; m->last_his_add_t[k] = sc.last_his_add_t[k]; }
+  m->map_dirty = sc.map_dirty != 0;
+  for (int c = 0; c < 2; c++) { m->snap_n[c] = sc.snap_n[c]; m->fov[c] = sc.fov[c]; }
+  ctx->ex.first_receive_time = sc.first_receive_time; ctx->ex.current_time = sc.current_time; ctx->ex.last_maximum_time_stamp = sc.last_maximum_time_stamp;
+  // the history window, pushed segment by segment from one upload
+  HistoryWindow* his[2] = {&m->his_corner, &m->his_surf};
+  for (int c = 0; c < 2; c++) {
+    float4* d = nullptr;
+    const size_t np = (size_t)v.his[c].n_pts;
+    if (np) {
+      LL_CUDA(ctx, ctx->scratch.carve([&](Carve& k) { d = k.take<float4>(np); }));
+      LL_CUDA(ctx, cudaMemcpyAsync(d, v.his[c].pts, np * 16, cudaMemcpyHostToDevice, s));
+    }
+    size_t off = 0;
+    for (int64_t k = 0; k < v.his[c].n_seg; k++) {
+      const size_t n = (size_t)rd<int32_t>(v.his[c].sizes + 4 * k);
+      LL_TRY(his[c]->push(ctx, d ? d + off : nullptr, n));
+      off += n;
+    }
+    LL_CUDA(ctx, cudaStreamSynchronize(s));   // (the scratch upload may be reallocated by the next carve)
+  }
+  // both cell maps
+  ll_cellmap* cm[2] = {m->cells_corner, m->cells_surf};
+  for (int c = 0; c < 2; c++) LL_TRY(cm_import(ctx, cm[c], v.cells[c].frame_idx, v.cells[c].n_oor, v.cells[c].rec, (int)v.cells[c].n_cells, (int)v.cells[c].n_pts));
+  // the snapshot and its index (the build is deterministic: the kNN answers are the saved mapper's)
+  m->have_map = false;
+  if (sc.have_map) {
+    const size_t n0 = (size_t)v.snap[0].n, n1 = (size_t)v.snap[1].n;
+    SnapLayout sn; LL_CUDA(ctx, m->snap.carve([&](Carve& k) { sn.layout(k, n0, n1); }));
+    LL_CUDA(ctx, cudaMemcpyAsync(sn.c, v.snap[0].pts, n0 * 16, cudaMemcpyHostToDevice, s));
+    LL_CUDA(ctx, cudaMemcpyAsync(sn.s, v.snap[1].pts, n1 * 16, cudaMemcpyHostToDevice, s));
+    LL_TRY(ll_map_rebuild(ctx, m->match_map, sn.c, n0, sn.s, n1, LL_FMT_XYZI16, LL_DEVICE));
+    m->have_map = true;
+  }
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  return LL_OK;
+}
+
+}  // namespace
+
+extern "C" int ll_mapper_save(ll_mapper* m, void* image, size_t cap, size_t* bytes) {
+  if (!m || !bytes) return LL_ERR_INVALID;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  cudaStream_t s = ctx->stream;
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  HistoryWindow* his[2] = {&m->his_corner, &m->his_surf};
+  ll_cellmap* cm[2] = {m->cells_corner, m->cells_surf};
+  const BucketTree* snap[2] = {&m->match_map->corner, &m->match_map->surf};
+  ImageCounts n; int frame_idx[2], oor[2];
+  for (int c = 0; c < 2; c++) {
+    n.his_seg[c] = (int64_t)his[c]->segs.size(); n.his_pts[c] = (int64_t)his[c]->live();
+    n.snap[c] = m->have_map ? snap[c]->n_src : 0;
+    if (m->have_map && n.snap[c] != m->snap_n[c]) { ctx->set_error("match-map index and snapshot disagree"); return LL_ERR_INVALID; }
+    int cells = 0, live = 0;
+    LL_TRY(cm_count(ctx, cm[c], &cells, &live, &frame_idx[c], &oor[c]));
+    n.cells[c] = cells; n.cell_pts[c] = live;
+  }
+  ll_mapper_image_header h;
+  const size_t total = image_layout(n, &h);
+  *bytes = total;
+  if (!image) return LL_OK;
+  if (cap < total) { ctx->set_error("image buffer smaller than the image (query the size with image = NULL)"); return LL_ERR_CAPACITY; }
+  uint8_t* b = (uint8_t*)image;
+  memcpy(b, &h, sizeof(h));
+  memcpy(b + h.section[LL_IMAGE_CONFIG].offset, &m->cfg, sizeof(m->cfg));
+  ll_mapper_image_scalars sc; memset(&sc, 0, sizeof(sc));
+  sc.frame_index = m->frame_index; sc.map_dirty = m->map_dirty ? 1 : 0; sc.have_map = m->have_map ? 1 : 0;
+  for (int c = 0; c < 2; c++) { sc.snap_n[c] = m->snap_n[c]; sc.fov[c] = m->fov[c]; }
+  sc.last_time_stamp = m->last_time_stamp;
+  for (int k = 0; k < 4; k++) { sc.q_w_curr[k] = m->q_w_curr[k]; sc.last_his_add_q[k] = m->last_his_add_q[k]; }
+  for (int k = 0; k < 3; k++) { sc.t_w_curr[k] = m->t_w_curr[k]; sc.last_his_add_t[k] = m->last_his_add_t[k]; }
+  sc.first_receive_time = ctx->ex.first_receive_time; sc.current_time = ctx->ex.current_time; sc.last_maximum_time_stamp = ctx->ex.last_maximum_time_stamp;
+  memcpy(b + h.section[LL_IMAGE_SCALARS].offset, &sc, sizeof(sc));
+  for (int c = 0; c < 2; c++) {
+    uint8_t* p = b + h.section[LL_IMAGE_HISTORY_CORNER + c].offset;
+    wr<int64_t>(p, n.his_seg[c]); wr<int64_t>(p + 8, n.his_pts[c]); p += HIS_HEAD;
+    for (const auto& sg : his[c]->segs) { wr<int32_t>(p, (int32_t)sg.second); p += 4; }
+    if (n.his_pts[c]) LL_CUDA(ctx, cudaMemcpyAsync(p, his[c]->data(), (size_t)n.his_pts[c] * 16, cudaMemcpyDeviceToHost, s));
+    p = b + h.section[LL_IMAGE_SNAPSHOT_CORNER + c].offset;
+    wr<int64_t>(p, n.snap[c]);
+    if (n.snap[c]) LL_CUDA(ctx, cudaMemcpyAsync(p + SNAP_HEAD, snap[c]->src, (size_t)n.snap[c] * 16, cudaMemcpyDeviceToHost, s));
+    p = b + h.section[LL_IMAGE_CELLS_CORNER + c].offset;
+    wr<int32_t>(p, frame_idx[c]); wr<int32_t>(p + 4, oor[c]); wr<int64_t>(p + 8, n.cells[c]); wr<int64_t>(p + 16, n.cell_pts[c]);
+    LL_TRY(cm_export(ctx, cm[c], (int)n.cells[c], (int)n.cell_pts[c], p + CELLS_HEAD));
+  }
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  return LL_OK;
+}
+
+extern "C" int ll_mapper_load(ll_ctx* ctx, const void* image, size_t bytes, const ll_mapper_config* cfg, ll_mapper** out) {
+  if (!ctx || !out) return LL_ERR_INVALID;
+  *out = nullptr;
+  ImageView v; std::string err;
+  const int st = image_validate(image, bytes, cfg, &v, &err);
+  if (st != LL_OK) { ctx->set_error("mapper image refused: " + err); return st; }
+  cudaSetDevice(ctx->device);
+  ll_mapper* m = nullptr;
+  LL_TRY(ll_mapper_create(ctx, cfg ? cfg : &v.cfg, &m));
+  const int rs = mapper_restore(m, v);
+  if (rs != LL_OK) { ll_mapper_release(m); return rs; }
+  // The buffer sizes of cfg sized this mapper's allocations (they are read at creation only); its images keep the stream's config, so that
+  // load-then-save reproduces an image whatever sizes the load chose.
+  m->cfg = v.cfg;
+  *out = m;
+  return LL_OK;
+}
+
+extern "C" int ll_mapper_image_info(const void* image, size_t bytes, ll_image_info* info) {
+  if (!info) return LL_ERR_INVALID;
+  ImageView v;
+  LL_TRY(image_validate(image, bytes, nullptr, &v, nullptr));
+  memset(info, 0, sizeof(*info));
+  info->bytes = bytes; info->version = v.h.version; info->matching_mode = v.cfg.matching_mode;
+  info->frame_index = v.sc.frame_index; info->have_map = v.sc.have_map; info->map_dirty = v.sc.map_dirty;
+  for (int c = 0; c < 2; c++) {
+    info->history_points[c] = v.his[c].n_pts; info->history_segments[c] = (int32_t)v.his[c].n_seg; info->snapshot_points[c] = v.snap[c].n;
+    info->cells[c] = v.cells[c].n_cells; info->cell_points[c] = v.cells[c].n_pts; info->cell_frame_idx[c] = v.cells[c].frame_idx;
+  }
+  return LL_OK;
 }

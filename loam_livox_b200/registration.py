@@ -572,3 +572,49 @@ class Laser_mapping:
         q, t, f = np.empty(4), np.empty(3), C.c_int()
         self.ctx.check(self.ctx._lib.ll_mapper_pose(self.h, q.ctypes.data, t.ctypes.data, C.byref(f)))
         return q, t, f.value
+
+    def save(self) -> bytes:
+        """The whole mapper as one byte image (ll_mapper_save; the format is specified in include/loamlivox_b200.h): Laser_mapping.load of
+        it, on any context, continues bit for bit as this mapper does.  The mapper is not modified."""
+        n = C.c_size_t()
+        self.ctx.check(self.ctx._lib.ll_mapper_save(self.h, None, 0, C.byref(n)))
+        buf = bytearray(n.value)
+        self.ctx.check(self.ctx._lib.ll_mapper_save(self.h, (C.c_char * len(buf)).from_buffer(buf), len(buf), C.byref(n)))
+        return bytes(buf)
+
+    @classmethod
+    def load(cls, ctx: Context, image, **alloc) -> "Laser_mapping":
+        """A mapper on ctx in the state of `image` (ll_mapper_load).  alloc may set max_cells, reserve_map_points and reserve_store_points,
+        which size the new mapper's buffers; everything else is the image's config.  A refused image raises and creates nothing."""
+        img = np.frombuffer(image, np.uint8)
+        cfg = None
+        if alloc:
+            image_info(image)   # validated before its config is read
+            cfg = image_config(image)
+            for k, v in alloc.items():
+                if k not in ("max_cells", "reserve_map_points", "reserve_store_points"):
+                    raise AttributeError(f"{k}: only the buffer sizes can differ from the image's config")
+                setattr(cfg, k, v)
+        h = C.c_void_p()
+        ctx.check(ctx._lib.ll_mapper_load(ctx.h, img.ctypes.data, img.shape[0], C.byref(cfg) if cfg is not None else None, C.byref(h)))
+        self = cls.__new__(cls)
+        self.ctx, self.h = ctx, h
+        self.cfg = image_config(image)   # what the mapper saves; alloc only sized its buffers
+        return self
+
+
+def image_config(image) -> capi.MapperConfig:
+    """The ll_mapper_config recorded in a mapper image (section LL_IMAGE_CONFIG; the image is not validated here)."""
+    off = int(np.frombuffer(image, np.uint64, count=1, offset=24 + 16 * capi.LL_IMAGE_CONFIG)[0])
+    return capi.MapperConfig.from_buffer_copy(bytes(image[off:off + C.sizeof(capi.MapperConfig)]))
+
+
+def image_info(image) -> dict:
+    """Validate a mapper image completely on the host (no context, no GPU) and report what is in it (ll_mapper_image_info): per class
+    ([corner, surface]) the history window's segments and points, the snapshot's points, the cell maps' cells, live points and frame index."""
+    img = np.frombuffer(image, np.uint8)
+    info = capi.ImageInfo()
+    st = capi.lib().ll_mapper_image_info(img.ctypes.data, img.shape[0], C.byref(info))
+    if st != capi.LL_OK:
+        raise LoamLivoxError(f"status {st}: mapper image refused")
+    return {n: (list(getattr(info, n)) if isinstance(getattr(info, n), C.Array) else getattr(info, n)) for n, _ in capi.ImageInfo._fields_ if n != "reserved"}
