@@ -421,7 +421,64 @@ int  ll_mapper_load(ll_ctx* ctx, const void* image, size_t bytes, const ll_mappe
 /* Host only, no context or GPU: validates an image completely (as ll_mapper_load with cfg NULL) and reports what is in it. */
 int  ll_mapper_image_info(const void* image, size_t bytes, ll_image_info* info);
 
-/* ---- wire formats (SURVEY 8(f) N3) ---------------------------------------------------------------------------------------------- */
+/* ---- relocalization: a scan's pose in a prior map without an initial guess (beyond the reference; DESIGN.md §4.3) ------------------
+ * Every other entry point needs a guess inside the basin of ICP (about the +-para_max_speed box and a few degrees).  These find one: an
+ * occupancy index of the map, every hypothesis of a rotation set x translation lattice scored against it on the device, the first K local maxima
+ * of the score (peaks) refined as the items of one ll_register_batch, the best accepted item chosen. */
+typedef struct ll_reloc_index ll_reloc_index;
+/* The occupancy index of `map` (not sharded: LL_ERR_INVALID), built from its own device clouds (corners and surfaces, finite points only).  The
+ * anchor lo is the finite bounding box the map keeps; a point's cell on axis a is floor(((double)x_a - (double)lo_a) / (double)res) + dilate,
+ * computed in fp64 and compared as a double before it becomes an integer; dims_a = floor(((double)hi_a - lo_a) / res) + 1 + 2 dilate.  A voxel is
+ * set iff an occupied voxel lies within Chebyshev distance `dilate` of it.  res <= 0 (or not finite), dilate outside 0 ... 4 or max_hypotheses
+ * outside 1 ... 2^24: LL_ERR_INVALID; more than 2^30 voxels: LL_ERR_CAPACITY; a map without a finite point: LL_ERR_INVALID; all before anything is
+ * enqueued.  Everything a relocalization needs is allocated here once (the bitmask, 44 bytes per hypothesis of max_hypotheses, the score
+ * points): ll_relocalize allocates nothing.  The index belongs to this map as it is now (ll_map_rebuild of it invalidates the index), and is used
+ * by one call at a time. */
+int  ll_reloc_index_build(ll_ctx* ctx, const ll_map* map, float res, int dilate, int max_hypotheses, ll_reloc_index** out);
+void ll_reloc_index_release(ll_reloc_index* idx);
+/* Parity hook: dims[3], lo[3] (the grid's fp32 anchor) and the dilated bitmask, voxel v = x + dims0 (y + dims1 z) in bit v & 31 of word v >> 5
+ * (ceil(dims0 dims1 dims2 / 32) words; words NULL: only dims and lo; cap_words too small: LL_ERR_CAPACITY). */
+int  ll_reloc_index_read(const ll_reloc_index* idx, int dims[3], float lo[3], uint32_t* words, size_t cap_words);
+typedef struct {
+  int           n_rot;  const double* rot_wxyz;   /* hypothesis rotations, host, n_rot x 4 (w,x,y,z), unit norm within 1e-6             */
+  int           rot_cyclic;                       /* rotation r's neighbours are r-1 and r+1 mod n_rot (a yaw circle)                    */
+  double        t0[3], step[3]; int nt[3];        /* translation lattice: t = t0 + i*step per axis, i in 0 .. nt-1                       */
+  int           max_candidates;                   /* K, 1 .. LL_MAX_BATCH                                                                */
+} ll_reloc_cfg;
+typedef struct { double q_wxyz[4], t[3]; int32_t score, hypothesis; } ll_reloc_candidate;
+/* Score points that ll_relocalize accepts at most (LL_ERR_CAPACITY above). */
+#define LL_RELOC_MAX_SCORE_POINTS 8192
+/* Hypothesis h = i + nt0 (j + nt1 (k + nt2 r)) (x fastest, rotation slowest) is the pose (rot_wxyz[r], t0 + (i, j, k) * step).  Its score is the
+ * number of score points p (scan frame, finite xyz) whose p_w = (float)(q_r * p + t) (fp64 rotation, the association of ll_transform, rounded to
+ * fp32 per component) falls on a set voxel inside the grid.  h is a peak iff score(h) >= 1 and h comes first in (score descending, index
+ * ascending) among its lattice Chebyshev-1 neighbours (clipped at the border) at rotations r - 1, r, r + 1 (wrapped when rot_cyclic and
+ * n_rot >= 3).  The candidates are the first K peaks in that order (*n_cand <= K of them, cand[0 .. *n_cand)).  Each is refined as one item of
+ * ll_register_batch over corner / surf with tmpl, its q_w_last = q_w_curr and t_w_last = t_w_curr set to the candidate and
+ * para_buffer_incremental to identity: refined[j] and item_status[j] are what ll_register_batch returns for it.  *best = the rank j with
+ * item_status LL_OK, registered 1 and status 1 of the smallest inlier_threshold (:559, the score Scene_alignment uses), ties to the lower rank;
+ * -1 when none qualifies (the call still returns LL_OK).  cand / refined / item_status hold max_candidates entries.
+ * Before anything is enqueued: a null pointer, a non-unit quaternion, n_rot or nt < 1, more hypotheses than the index's max_hypotheses, K outside
+ * 1 ... LL_MAX_BATCH, a sharded map, an index built on another map, an unknown fmt / where or a tmpl whose frame index is at or below
+ * mapping_init_accumulate_frames (the :199 gate would skip every refinement): LL_ERR_INVALID; more than LL_RELOC_MAX_SCORE_POINTS score points,
+ * or K items of these features failing the batch's capacity check: LL_ERR_CAPACITY. */
+int ll_relocalize(ll_ctx* ctx, const ll_map* map, const ll_reloc_index* idx,
+                  const void* score_pts, size_t n_score,
+                  const void* corner, size_t n_corner, const void* surf, size_t n_surf, int fmt, int where,
+                  const ll_reloc_cfg* cfg, const ll_reg_state* tmpl,
+                  ll_reloc_candidate* cand, ll_reg_result* refined, int* item_status, int* n_cand, int* best);
+/* Parity hook: the scores of all n_rot x nt0 x nt1 x nt2 hypotheses (hypothesis order), validated as ll_relocalize validates them. */
+int ll_reloc_scores(ll_ctx* ctx, const ll_reloc_index* idx, const void* score_pts, size_t n_score, int fmt, int where,
+                    const ll_reloc_cfg* cfg, int32_t* scores);
+/* A new ll_map of the mapper's whole map: mode 0 = VoxelGrid (line / plane resolution) of the live history window, exactly what the next
+ * refresh indexes; mode 1 = VoxelGrid of every live point of each cell map in store order (no FOV, no radius, no down-sample-and-replace).
+ * The mapper's state does not change.  LL_ERR_INVALID when either class is empty (the mapper has no map yet).  Release with ll_map_release. */
+int ll_mapper_whole_map(ll_mapper* mapper, ll_map** out);
+/* The pose the next step seeds from (a relocalized pose, or any other).  Setting the pose the mapper already has (bitwise) changes nothing;
+ * otherwise in matching mode 1 the match map is marked for refresh (the assembly is around the pose).  Frame index, time stamps and history
+ * bookkeeping are untouched.  A non-finite value: LL_ERR_INVALID. */
+int ll_mapper_set_pose(ll_mapper* mapper, const double q_wxyz[4], const double t[3]);
+
+/* ---- wire formats (SURVEY 8(f) N3)---------------------------------------------------------------------------------------------- */
 /* Layout of one point record of an LL_FMT_STRIDED input: what pcl::fromROSMsg (laser_feature_extractor.hpp:275) resolves by field name from a
  * sensor_msgs/PointCloud2 (point_step, the offsets of the little-endian fields x, y, z, intensity and intensity's datatype).  The payload is
  * copied to the device as it is and unpacked there into 16-byte points; n = width * height. */

@@ -20,6 +20,7 @@ LL_OK, LL_ERR_INVALID, LL_ERR_CUDA, LL_ERR_CAPACITY, LL_ERR_NO_BLOCKS, LL_ERR_CA
 LL_IPC_HANDLE_BYTES = 64
 LL_MAX_PIECES_PER_FRAME = 16
 LL_MAX_BATCH = 16
+LL_RELOC_MAX_SCORE_POINTS = 8192
 LL_MAPPER_IMAGE_MAGIC, LL_MAPPER_IMAGE_VERSION = b"LLMAPIMG", 1
 (LL_IMAGE_CONFIG, LL_IMAGE_SCALARS, LL_IMAGE_HISTORY_CORNER, LL_IMAGE_HISTORY_SURF, LL_IMAGE_SNAPSHOT_CORNER, LL_IMAGE_SNAPSHOT_SURF, LL_IMAGE_CELLS_CORNER,
  LL_IMAGE_CELLS_SURF, LL_IMAGE_SECTIONS) = range(9)
@@ -33,6 +34,7 @@ EXPORTS = [
     "ll_mapper_process_scan", "ll_mapper_pose", "ll_map_rebuild", "ll_debug_solver_cycles", "ll_state_snapshot_bytes", "ll_set_point_layout", "ll_format_pose_log", "ll_reg_state_yaml", "ll_cap_uniform", "ll_map_shard_info", "ll_shard_plan", "ll_align_cfg_default", "ll_scene_align", "ll_frame_to_pose", "ll_features_to_pointcloud2",
     "ll_mapper_process_frame", "ll_voxel_downsample_segments", "ll_register_batch", "ll_mapper_process_frames", "ll_mapper_process_scans",
     "ll_mapper_save", "ll_mapper_load", "ll_mapper_image_info",
+    "ll_reloc_index_build", "ll_reloc_index_release", "ll_reloc_index_read", "ll_relocalize", "ll_reloc_scores", "ll_mapper_whole_map", "ll_mapper_set_pose",
 ]
 
 
@@ -97,6 +99,16 @@ class ShardInfo(C.Structure):
 class AlignCfg(C.Structure):
     _fields_ = [("line_res", C.c_float), ("plane_res", C.c_float), ("maximum_icp_iteration", C.c_int), ("maximum_residual_block", C.c_int),
                 ("accepted_threshold", C.c_float), ("rng_seed", C.c_int), ("t_init", C.c_double * 3)]
+
+
+class RelocCfg(C.Structure):
+    """ll_reloc_cfg: the hypotheses of a relocalization (rotations x translation lattice) and the candidate count K."""
+    _fields_ = [("n_rot", C.c_int), ("rot_wxyz", C.POINTER(C.c_double)), ("rot_cyclic", C.c_int), ("t0", C.c_double * 3), ("step", C.c_double * 3),
+                ("nt", C.c_int * 3), ("max_candidates", C.c_int)]
+
+
+class RelocCandidate(C.Structure):
+    _fields_ = [("q_wxyz", C.c_double * 4), ("t", C.c_double * 3), ("score", C.c_int32), ("hypothesis", C.c_int32)]
 
 
 class LoamLivoxError(RuntimeError):
@@ -186,6 +198,14 @@ def lib():
     L.ll_mapper_save.argtypes = [vp, vp, sz, C.POINTER(sz)]
     L.ll_mapper_load.argtypes = [vp, vp, sz, C.POINTER(MapperConfig), C.POINTER(vp)]
     L.ll_mapper_image_info.argtypes = [vp, sz, C.POINTER(ImageInfo)]
+    L.ll_reloc_index_build.argtypes = [vp, vp, cf, ci, ci, C.POINTER(vp)]
+    L.ll_reloc_index_release.argtypes = [vp]
+    L.ll_reloc_index_read.argtypes = [vp, vp, vp, vp, sz]
+    L.ll_relocalize.argtypes = [vp, vp, vp, vp, sz, vp, sz, vp, sz, ci, ci, C.POINTER(RelocCfg), C.POINTER(RegState), C.POINTER(RelocCandidate),
+                                C.POINTER(RegResult), vp, C.POINTER(ci), C.POINTER(ci)]
+    L.ll_reloc_scores.argtypes = [vp, vp, vp, sz, ci, ci, C.POINTER(RelocCfg), vp]
+    L.ll_mapper_whole_map.argtypes = [vp, C.POINTER(vp)]
+    L.ll_mapper_set_pose.argtypes = [vp, vp, vp]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64
     _LIB = L

@@ -483,6 +483,16 @@ int cm_count(ll_ctx* ctx, ll_cellmap* m, int* n_cells, int* n_live, int* frame_i
   return LL_OK;
 }
 
+// The store indices of the live points in store order into a.idx (their count into a.cnt[1]), on the context's stream.
+static int cm_select_live(ll_ctx* ctx, ll_cellmap* m, CmExport& a) {
+  size_t cub_c = a.cub_bytes;
+  const int N = m->n_pts;
+  cm_live_kernel<<<ll_div_up(N, 256), 256, 0, ctx->stream>>>(m->pt_slot, m->pt_epoch, N, m->epoch, a.flag);
+  LL_CUDA(ctx, cub::DeviceSelect::Flagged(a.cub_tmp, cub_c, cub::CountingInputIterator<int>(0), a.flag, a.idx, a.cnt + 1, N, ctx->stream));
+  ctx->launches += 2;
+  return LL_OK;
+}
+
 // The map's cells (ascending key) and live points (store order) into out: n_cells ll_image_cell then n_live ll_image_cell_point, the counts
 // cm_count gave.  One copy to the host; the map's buffers are only read.
 int cm_export(ll_ctx* ctx, ll_cellmap* m, int n_cells, int n_live, void* out) {
@@ -507,9 +517,7 @@ int cm_export(ll_ctx* ctx, ll_cellmap* m, int n_cells, int n_live, void* out) {
   }
   // live points in store order
   if (N > 0) {
-    cm_live_kernel<<<ll_div_up(N, 256), 256, 0, s>>>(m->pt_slot, m->pt_epoch, N, m->epoch, a.flag);
-    LL_CUDA(ctx, cub::DeviceSelect::Flagged(a.cub_tmp, cub_c, cub::CountingInputIterator<int>(0), a.flag, a.idx, a.cnt + 1, N, s));
-    ctx->launches += 2;
+    LL_TRY(cm_select_live(ctx, m, a));
     if (n_live > 0) { cm_export_points_kernel<<<ll_div_up(n_live, 256), 256, 0, s>>>(m->pts, m->pt_slot, a.idx, n_live, a.rank, pts); ctx->launches++; }
   }
   LL_CUDA(ctx, cudaGetLastError());
@@ -518,6 +526,17 @@ int cm_export(ll_ctx* ctx, ll_cellmap* m, int n_cells, int n_live, void* out) {
   LL_CUDA(ctx, cudaMemcpyAsync(out, a.rec, ((size_t)n_cells + n_live) * 16, cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   if (h[0] != n_cells || h[1] != n_live) { ctx->set_error("cell map changed while it was saved"); return LL_ERR_INVALID; }
+  return LL_OK;
+}
+
+int cm_live_points(ll_ctx* ctx, ll_cellmap* m, int n_live, float4* dst) {
+  const int T = m->table_cap, N = m->n_pts;
+  if (n_live <= 0 || N <= 0) return LL_OK;
+  CmExport a(T, N);
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { a.layout(c, T, N, 0); }));
+  LL_TRY(cm_select_live(ctx, m, a));
+  LL_TRY(launch_gather_points(ctx, ctx->stream, m->pts, a.idx, n_live, dst));
+  LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // (a lives in the scratch arena, which the next carve may reallocate)
   return LL_OK;
 }
 

@@ -229,6 +229,12 @@ int cm_count(ll_ctx* ctx, ll_cellmap* m, int* n_cells, int* n_live, int* frame_i
 int cm_export(ll_ctx* ctx, ll_cellmap* m, int n_cells, int n_live, void* out);
 // An empty map in the state cm_export recorded (records validated by the caller: keys distinct, cell ranks < n_cells).
 int cm_import(ll_ctx* ctx, ll_cellmap* m, int frame_idx, int n_out_of_range, const void* in, int n_cells, int n_live);
+// The n_live live points (the count cm_count gave) in store order, as the map stores them, into the device array dst on the context's stream,
+// by the export's live-point selection; the map is only read.
+int cm_live_points(ll_ctx* ctx, ll_cellmap* m, int n_live, float4* dst);
+
+// ---------------------------------------------------------------------------------------------- relocalization (reloc.cu)
+int launch_gather_points(ll_ctx* ctx, cudaStream_t s, const float4* src, const int* idx, int n, float4* dst);   // dst[i] = src[idx[i]]
 
 // ---------------------------------------------------------------------------------------------- host driver pieces (api.cu)
 // Registration of the features already resident in A.feat (corners then surfaces): the batch of one.  Core of ll_register / ll_scan_to_pose.

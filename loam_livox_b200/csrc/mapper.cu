@@ -790,3 +790,52 @@ extern "C" int ll_mapper_image_info(const void* image, size_t bytes, ll_image_in
   }
   return LL_OK;
 }
+
+// ---------------------------------------------------------------------------------------------- relocalization glue
+// The whole map as a new ll_map: the clouds (mode 0: the live history window; mode 1: every live point of each cell map in store order) into
+// the context's feat_buf, their VoxelGrids at the line / plane resolution, and an index built in place.  Nothing of the mapper is written.
+extern "C" int ll_mapper_whole_map(ll_mapper* m, ll_map** out) {
+  if (!m || !out) return LL_ERR_INVALID;
+  *out = nullptr;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  cudaStream_t s = ctx->stream;
+  size_t n[2] = {0, 0};
+  ll_cellmap* cm[2] = {m->cells_corner, m->cells_surf};
+  const HistoryWindow* his[2] = {&m->his_corner, &m->his_surf};
+  if (m->cfg.matching_mode == 0) {
+    for (int c = 0; c < 2; c++) n[c] = his[c]->live();
+  } else {
+    for (int c = 0; c < 2; c++) { int cells = 0, live = 0, fi = 0, oor = 0; LL_TRY(cm_count(ctx, cm[c], &cells, &live, &fi, &oor)); n[c] = (size_t)live; }
+  }
+  if (n[0] == 0 || n[1] == 0) { ctx->set_error("the mapper has no map yet (a class is empty)"); return LL_ERR_INVALID; }
+  float4* in[2] = {nullptr, nullptr}; float4* vg[2]; int* d_cnt;
+  LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) {
+    if (m->cfg.matching_mode == 1) { in[0] = c.take<float4>(n[0]); in[1] = c.take<float4>(n[1]); }
+    vg[0] = c.take<float4>(n[0]); vg[1] = c.take<float4>(n[1]); d_cnt = c.take<int>(2);
+  }));
+  const float leaf[2] = {m->cfg.line_resolution, m->cfg.plane_resolution};
+  for (int c = 0; c < 2; c++) {
+    const float4* src = his[c]->data();
+    if (m->cfg.matching_mode == 1) { LL_TRY(cm_live_points(ctx, cm[c], (int)n[c], in[c])); src = in[c]; }
+    LL_TRY(launch_voxel_grid(ctx, s, ctx->scratch, src, (int)n[c], nullptr, leaf[c], vg[c], d_cnt + c));
+  }
+  int hc[2] = {0, 0};
+  LL_CUDA(ctx, cudaMemcpyAsync(hc, d_cnt, sizeof(hc), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  ll_map* map = nullptr;
+  LL_TRY(ll_map_build(ctx, vg[0], (size_t)hc[0], vg[1], (size_t)hc[1], LL_FMT_XYZI16, LL_DEVICE, &map));
+  if (cudaStreamSynchronize(s) != cudaSuccess) { ll_map_release(map); ctx->set_error("whole-map index build failed"); return LL_ERR_CUDA; }
+  *out = map;
+  return LL_OK;
+}
+
+extern "C" int ll_mapper_set_pose(ll_mapper* m, const double q_wxyz[4], const double t[3]) {
+  if (!m || !q_wxyz || !t) return LL_ERR_INVALID;
+  for (int k = 0; k < 4; k++) if (!std::isfinite(q_wxyz[k])) return LL_ERR_INVALID;
+  for (int k = 0; k < 3; k++) if (!std::isfinite(t[k])) return LL_ERR_INVALID;
+  if (memcmp(q_wxyz, m->q_w_curr, sizeof(m->q_w_curr)) == 0 && memcmp(t, m->t_w_curr, sizeof(m->t_w_curr)) == 0) return LL_OK;
+  for (int k = 0; k < 4; k++) m->q_w_curr[k] = q_wxyz[k];
+  for (int k = 0; k < 3; k++) m->t_w_curr[k] = t[k];
+  if (m->cfg.matching_mode == 1) m->map_dirty = true;   // the assembly of mode 1 is around the pose
+  return LL_OK;
+}

@@ -1,0 +1,419 @@
+// Relocalization (include/loamlivox_b200.h, ll_reloc_*; DESIGN.md §4.3): the pose of a scan in a prior map without an initial guess.
+// An occupancy bitmask of the map's own device clouds, dilated; every hypothesis of a rotation set x translation lattice scored by how many
+// score points land on set voxels; the first K local maxima (peaks) of the score field refined by the batched registration (ll_register_batch).
+// Beyond the reference, which has no relocalization: its only answer to a lost track is to drop the scan (laser_mapping.hpp:1413-1416).
+//
+// Built -fmad=false: the cell of a point and the transform of a score point are restated bit for bit by tests/reloc_reference.py.
+#include <cmath>
+#include <algorithm>
+#include "common.cuh"
+#include "kernels.cuh"
+#include "exact_math.cuh"
+#include <math_constants.h>
+
+#define RELOC_MAX_DILATE 4
+#define RELOC_MAX_HYP (1 << 24)
+#define RELOC_MAX_VOXELS (1ll << 30)
+#define RELOC_TILE 1024    // score points rotated into shared memory per pass (3 x 8 KB)
+#define RELOC_GROUP 64     // lattice translations per CTA (8 warps x 8)
+
+struct ll_reloc_index {
+  int device = 0;
+  const ll_map* map = nullptr; const float4* src[2] = {nullptr, nullptr}; int n_src[2] = {0, 0};   // the map it was built on
+  float res = 0.f; int dilate = 0; int max_hyp = 0;
+  int dims[3] = {0, 0, 0}; float lo[3] = {0, 0, 0};
+  long long n_vox = 0, n_words = 0;
+  DevBuf storage;   // everything below, allocated once by ll_reloc_index_build
+  uint32_t* bits = nullptr;             // [n_words] the dilated occupancy, x fastest, bit v & 31 of word v >> 5
+  int32_t* scores = nullptr;            // [max_hyp]
+  unsigned long long* peaks = nullptr;  // [max_hyp] peak keys (score << 32 | ~h), unordered
+  int* counts = nullptr;                // [0] peaks, [1] candidates
+  unsigned long long* cand = nullptr;   // [LL_MAX_BATCH] the first K peaks
+  float4* pts = nullptr;                // [LL_RELOC_MAX_SCORE_POINTS] score points (scan frame)
+  double* rot = nullptr;                // [max_hyp x 4] hypothesis rotations (w, x, y, z)
+};
+
+namespace {
+
+struct RelocGrid { const uint32_t* bits; int dims[3]; double lo[3]; double res; int dilate; };
+
+// Cell of p on axis a = floor((p_a - lo_a) / res) + dilate in fp64, compared as a double before it becomes an integer.
+__device__ __forceinline__ bool grid_cell(const RelocGrid& g, float x, float y, float z, long long* v) {
+  const float p[3] = {x, y, z};
+  long long c[3];
+  for (int a = 0; a < 3; a++) {
+    const double d = floor(((double)p[a] - g.lo[a]) / g.res) + (double)g.dilate;
+    if (!(d >= 0.0 && d < (double)g.dims[a])) return false;
+    c[a] = (long long)d;
+  }
+  *v = c[0] + (long long)g.dims[0] * (c[1] + (long long)g.dims[1] * c[2]);
+  return true;
+}
+
+__global__ void reloc_mark_kernel(const float4* __restrict__ src, int n, RelocGrid g, uint32_t* __restrict__ bits) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 p = src[i];
+  if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z))) return;
+  long long v;
+  if (grid_cell(g, p.x, p.y, p.z, &v)) atomicOr(&bits[v >> 5], 1u << (v & 31));
+}
+
+// One separable pass of the Chebyshev dilation along `axis` (radius r, clipped at the border): one thread per voxel, one ballot per word.
+__global__ void reloc_dilate_kernel(const uint32_t* __restrict__ in, uint32_t* __restrict__ out, int d0, int d1, int d2, int axis, int r, long long n_vox,
+                                    long long n_words) {
+  const long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  bool set = false;
+  if (v < n_vox) {
+    const long long yz = v / d0;
+    const int x = (int)(v - yz * d0), y = (int)(yz % d1), z = (int)(yz / d1);
+    const int c = axis == 0 ? x : (axis == 1 ? y : z), D = axis == 0 ? d0 : (axis == 1 ? d1 : d2);
+    const long long stride = axis == 0 ? 1 : (axis == 1 ? (long long)d0 : (long long)d0 * d1);
+    const int a = max(c - r, 0), b = min(c + r, D - 1);
+    for (int k = a; k <= b && !set; k++) { const long long u = v + (long long)(k - c) * stride; set = (in[u >> 5] >> (u & 31)) & 1u; }
+  }
+  const unsigned w = __ballot_sync(0xffffffffu, set);
+  if ((threadIdx.x & 31) == 0 && (v >> 5) < n_words) out[v >> 5] = w;
+}
+
+struct ScoreArgs {
+  RelocGrid g; const float4* pts; int n_pts; const double* rot;
+  double t0[3], step[3]; int nt[3]; int n_lat, blocks_per_rot;
+  int32_t* scores;
+};
+// CTA = one rotation x RELOC_GROUP consecutive lattice points.  Per tile, the score points are rotated once (qrot_d, fp64) into shared memory;
+// then one warp per translation counts, its lanes striding over the tile.  score(h) with h = l + n_lat * r, l = i + nt0 (j + nt1 k).
+__global__ void __launch_bounds__(256) reloc_score_kernel(ScoreArgs a) {
+  __shared__ double sx[RELOC_TILE], sy[RELOC_TILE], sz[RELOC_TILE];
+  __shared__ int cnt[RELOC_GROUP];
+  const int r = blockIdx.x / a.blocks_per_rot, l0 = (blockIdx.x - r * a.blocks_per_rot) * RELOC_GROUP;
+  const double q[4] = {a.rot[4 * r], a.rot[4 * r + 1], a.rot[4 * r + 2], a.rot[4 * r + 3]};
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
+  if (threadIdx.x < RELOC_GROUP) cnt[threadIdx.x] = 0;
+  for (int base = 0; base < a.n_pts; base += RELOC_TILE) {
+    const int nt = min(RELOC_TILE, a.n_pts - base);
+    __syncthreads();
+    for (int i = threadIdx.x; i < nt; i += blockDim.x) {
+      const float4 p = a.pts[base + i];
+      double ox = CUDART_NAN, oy = CUDART_NAN, oz = CUDART_NAN;   // a point with a non-finite coordinate never scores
+      if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) qrot_d(q, (double)p.x, (double)p.y, (double)p.z, ox, oy, oz);
+      sx[i] = ox; sy[i] = oy; sz[i] = oz;
+    }
+    __syncthreads();
+    for (int j = warp; j < RELOC_GROUP; j += n_warps) {
+      const int l = l0 + j;
+      if (l >= a.n_lat) break;
+      const int i0 = l % a.nt[0], i1 = (l / a.nt[0]) % a.nt[1], i2 = l / (a.nt[0] * a.nt[1]);
+      const double tx = a.t0[0] + (double)i0 * a.step[0], ty = a.t0[1] + (double)i1 * a.step[1], tz = a.t0[2] + (double)i2 * a.step[2];
+      int c = 0;
+      for (int p = lane; p < nt; p += 32) {
+        long long v;
+        if (grid_cell(a.g, (float)(sx[p] + tx), (float)(sy[p] + ty), (float)(sz[p] + tz), &v)) c += (int)((__ldg(&a.g.bits[v >> 5]) >> (v & 31)) & 1u);
+      }
+      for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+      if (lane == 0) cnt[j] += c;   // (translation j belongs to this warp alone)
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < RELOC_GROUP && l0 + (int)threadIdx.x < a.n_lat) a.scores[(size_t)r * a.n_lat + l0 + threadIdx.x] = cnt[threadIdx.x];
+}
+
+// h is a peak iff score(h) >= 1 and h comes first in (score descending, index ascending) among its lattice Chebyshev-1 neighbours (clipped at the
+// border) at rotations r - 1, r, r + 1 (wrapped when cyclic and n_rot >= 3).  Peaks are appended as keys score << 32 | (2^32 - 1 - h).
+__global__ void reloc_peak_kernel(const int32_t* __restrict__ scores, int nt0, int nt1, int nt2, int n_rot, int cyclic, int H, unsigned long long* __restrict__ peaks,
+                                  int* __restrict__ count) {
+  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  if (h >= H) return;
+  const int s = scores[h];
+  if (s < 1) return;
+  const int n_lat = nt0 * nt1 * nt2;
+  const int r = h / n_lat, l = h - r * n_lat, i = l % nt0, j = (l / nt0) % nt1, k = l / (nt0 * nt1);
+  const bool wrap = cyclic && n_rot >= 3;
+  for (int dr = -1; dr <= 1; dr++) {
+    int rr = r + dr;
+    if (wrap) rr = (rr + n_rot) % n_rot;
+    else if (rr < 0 || rr >= n_rot) continue;
+    for (int dk = -1; dk <= 1; dk++) {
+      const int kk = k + dk; if (kk < 0 || kk >= nt2) continue;
+      for (int dj = -1; dj <= 1; dj++) {
+        const int jj = j + dj; if (jj < 0 || jj >= nt1) continue;
+        for (int di = -1; di <= 1; di++) {
+          const int ii = i + di; if (ii < 0 || ii >= nt0) continue;
+          const int h2 = ii + nt0 * (jj + nt1 * kk) + n_lat * rr;
+          if (h2 == h) continue;
+          const int s2 = scores[h2];
+          if (s2 > s || (s2 == s && h2 < h)) return;
+        }
+      }
+    }
+  }
+  peaks[atomicAdd(count, 1)] = ((unsigned long long)(unsigned)s << 32) | (unsigned long long)(0xffffffffu - (unsigned)h);
+}
+
+// The first K peaks in (score descending, index ascending) order, i.e. the K largest keys: K rounds of a block-wide maximum below the last one.
+__global__ void __launch_bounds__(1024) reloc_select_kernel(const unsigned long long* __restrict__ peaks, int* __restrict__ counts, int K, unsigned long long* __restrict__ cand) {
+  __shared__ unsigned long long red[32];
+  const int n = counts[0];
+  unsigned long long bound = ~0ull;
+  int k = 0;
+  for (; k < K; k++) {
+    unsigned long long best = 0;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) { const unsigned long long v = peaks[i]; if (v < bound && v > best) best = v; }
+    for (int o = 16; o > 0; o >>= 1) { const unsigned long long w = __shfl_xor_sync(0xffffffffu, best, o); best = w > best ? w : best; }
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = best;
+    __syncthreads();
+    best = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); w++) best = red[w] > best ? red[w] : best;
+    if (best == 0) break;   // (keys of peaks are > 0: score >= 1)
+    if (threadIdx.x == 0) cand[k] = best;
+    bound = best;
+  }
+  if (threadIdx.x == 0) counts[1] = k;
+}
+
+__global__ void reloc_gather_kernel(const float4* __restrict__ src, const int* __restrict__ idx, int n, float4* __restrict__ dst) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = src[idx[i]];
+}
+
+RelocGrid grid_of(const ll_reloc_index* x) {
+  RelocGrid g; g.bits = x->bits; g.res = (double)x->res; g.dilate = x->dilate;
+  for (int a = 0; a < 3; a++) { g.dims[a] = x->dims[a]; g.lo[a] = (double)x->lo[a]; }
+  return g;
+}
+
+void index_layout(ll_reloc_index* x, Carve& c) {
+  x->bits = c.take<uint32_t>((size_t)x->n_words); x->scores = c.take<int32_t>(x->max_hyp); x->peaks = c.take<unsigned long long>(x->max_hyp);
+  x->counts = c.take<int>(2); x->cand = c.take<unsigned long long>(LL_MAX_BATCH); x->pts = c.take<float4>(LL_RELOC_MAX_SCORE_POINTS);
+  x->rot = c.take<double>((size_t)x->max_hyp * 4);
+}
+
+int check_map(ll_ctx* ctx, const ll_map* map) {
+  if (map->world > 1) { ctx->set_error("relocalization needs the whole map: a sharded map is refused"); return LL_ERR_INVALID; }
+  return LL_OK;
+}
+
+// The configuration's hypothesis count (*H) after every check of ll_reloc_cfg except max_candidates.
+int check_cfg(ll_ctx* ctx, const ll_reloc_index* idx, const ll_reloc_cfg* cfg, long long* H) {
+  if (!cfg->rot_wxyz) { ctx->set_error("null rotation array"); return LL_ERR_INVALID; }
+  if (cfg->n_rot < 1 || cfg->nt[0] < 1 || cfg->nt[1] < 1 || cfg->nt[2] < 1) { ctx->set_error("n_rot and nt must be >= 1"); return LL_ERR_INVALID; }
+  for (int a = 0; a < 3; a++)
+    if (!std::isfinite(cfg->t0[a]) || !std::isfinite(cfg->step[a])) { ctx->set_error("non-finite lattice origin or step"); return LL_ERR_INVALID; }
+  const long long h = (long long)cfg->n_rot * cfg->nt[0] * cfg->nt[1] * cfg->nt[2];
+  if ((long long)cfg->nt[0] * cfg->nt[1] * cfg->nt[2] > idx->max_hyp || h > idx->max_hyp) {
+    ctx->set_error("more hypotheses than the index's max_hypotheses (" + std::to_string(idx->max_hyp) + ")"); return LL_ERR_INVALID;
+  }
+  for (int r = 0; r < cfg->n_rot; r++) {
+    const double* q = cfg->rot_wxyz + 4 * r;
+    const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+    if (!(std::fabs(std::sqrt(n2) - 1.0) <= 1e-6)) { ctx->set_error("rotation " + std::to_string(r) + " is not a unit quaternion"); return LL_ERR_INVALID; }
+  }
+  *H = h;
+  return LL_OK;
+}
+
+int check_points(ll_ctx* ctx, const void* pts, size_t n, int fmt, int where, const char* what) {
+  if (fmt != LL_FMT_XYZI16 && fmt != LL_FMT_PCL32 && fmt != LL_FMT_STRIDED) { ctx->set_error("unknown point format"); return LL_ERR_INVALID; }
+  if (where != LL_HOST && where != LL_DEVICE) { ctx->set_error("unknown memory kind"); return LL_ERR_INVALID; }
+  if (!pts && n) { ctx->set_error(std::string("null ") + what); return LL_ERR_INVALID; }
+  return LL_OK;
+}
+
+// Upload of the score points and the rotations, then the score kernel: scores[0 .. H) of the index, on the context's stream.
+int enqueue_scores(ll_ctx* ctx, ll_reloc_index* idx, const void* pts, size_t n, int fmt, int where, const ll_reloc_cfg* cfg) {
+  cudaStream_t s = ctx->stream;
+  LL_TRY(upload_cloud(ctx, s, pts, n, fmt, where, idx->pts));
+  LL_CUDA(ctx, cudaMemcpyAsync(idx->rot, cfg->rot_wxyz, (size_t)cfg->n_rot * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
+  ScoreArgs a;
+  a.g = grid_of(idx); a.pts = idx->pts; a.n_pts = (int)n; a.rot = idx->rot; a.scores = idx->scores;
+  for (int k = 0; k < 3; k++) { a.t0[k] = cfg->t0[k]; a.step[k] = cfg->step[k]; a.nt[k] = cfg->nt[k]; }
+  a.n_lat = cfg->nt[0] * cfg->nt[1] * cfg->nt[2];
+  a.blocks_per_rot = ll_div_up(a.n_lat, RELOC_GROUP);
+  const long long blocks = (long long)cfg->n_rot * a.blocks_per_rot;
+  reloc_score_kernel<<<(unsigned)blocks, 256, 0, s>>>(a); ctx->launches++;
+  LL_CUDA(ctx, cudaGetLastError());
+  return LL_OK;
+}
+
+}  // namespace
+
+// The live points of a cell map in store order (cm_live_points, cellmap.cu) are gathered here.
+int launch_gather_points(ll_ctx* ctx, cudaStream_t s, const float4* src, const int* idx, int n, float4* dst) {
+  if (n <= 0) return LL_OK;
+  reloc_gather_kernel<<<ll_div_up(n, 256), 256, 0, s>>>(src, idx, n, dst); ctx->launches++;
+  LL_CUDA(ctx, cudaGetLastError());
+  return LL_OK;
+}
+
+extern "C" {
+
+int ll_reloc_index_build(ll_ctx* ctx, const ll_map* map, float res, int dilate, int max_hypotheses, ll_reloc_index** out) {
+  if (!ctx || !map || !out) return LL_ERR_INVALID;
+  *out = nullptr;
+  LL_TRY(check_map(ctx, map));
+  if (!(res > 0.f) || !std::isfinite(res)) { ctx->set_error("res must be a finite value > 0"); return LL_ERR_INVALID; }
+  if (dilate < 0 || dilate > RELOC_MAX_DILATE) { ctx->set_error("dilate must be 0 ... 4"); return LL_ERR_INVALID; }
+  if (max_hypotheses < 1 || max_hypotheses > RELOC_MAX_HYP) { ctx->set_error("max_hypotheses must be 1 ... 2^24"); return LL_ERR_INVALID; }
+  cudaSetDevice(ctx->device);
+  cudaStream_t s = ctx->stream;
+  // the anchor: the finite bounding box both trees keep (d_bbox); read before anything is enqueued
+  const BucketTree* tr[2] = {&map->corner, &map->surf};
+  float bb[2][6];
+  for (int c = 0; c < 2; c++) if (tr[c]->n_src > 0) LL_CUDA(ctx, cudaMemcpyAsync(bb[c], tr[c]->d_bbox, sizeof(bb[c]), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
+  bool any = false;
+  for (int c = 0; c < 2; c++) {
+    if (tr[c]->n_src <= 0) continue;
+    bool ok = true;
+    for (int a = 0; a < 3; a++) ok = ok && std::isfinite(bb[c][a]) && std::isfinite(bb[c][3 + a]) && bb[c][a] <= bb[c][3 + a];
+    if (!ok) continue;   // no finite point in this cloud
+    any = true;
+    for (int a = 0; a < 3; a++) { lo[a] = std::min(lo[a], bb[c][a]); hi[a] = std::max(hi[a], bb[c][3 + a]); }
+  }
+  if (!any) { ctx->set_error("the map has no finite point"); return LL_ERR_INVALID; }
+  int dims[3]; double nv = 1.0;
+  for (int a = 0; a < 3; a++) {
+    const double d = std::floor(((double)hi[a] - (double)lo[a]) / (double)res) + 1.0 + 2.0 * dilate;
+    if (!(d <= (double)RELOC_MAX_VOXELS)) { ctx->set_error("more than 2^30 voxels"); return LL_ERR_CAPACITY; }
+    dims[a] = (int)d; nv *= d;
+  }
+  if (nv > (double)RELOC_MAX_VOXELS) { ctx->set_error("more than 2^30 voxels"); return LL_ERR_CAPACITY; }
+  ll_reloc_index* x = new ll_reloc_index();
+  x->device = ctx->device; x->map = map; x->res = res; x->dilate = dilate; x->max_hyp = max_hypotheses;
+  for (int c = 0; c < 2; c++) { x->src[c] = tr[c]->src; x->n_src[c] = tr[c]->n_src; }
+  for (int a = 0; a < 3; a++) { x->dims[a] = dims[a]; x->lo[a] = lo[a]; }
+  x->n_vox = (long long)dims[0] * dims[1] * dims[2]; x->n_words = (x->n_vox + 31) / 32;
+  auto fail = [&](int st) { x->storage.release(); delete x; return st; };
+  { const cudaError_t e = x->storage.carve([&](Carve& c) { index_layout(x, c); });
+    if (e != cudaSuccess) { ctx->set_error(std::string("index allocation: ") + cudaGetErrorString(e)); return fail(LL_ERR_CUDA); } }
+  // occupancy into `occ` (the index itself when nothing is dilated), then x, y, z passes ping-ponging with the context's scratch
+  uint32_t* tmp = nullptr;
+  if (dilate > 0) {
+    const cudaError_t e = ctx->scratch.carve([&](Carve& c) { tmp = c.take<uint32_t>((size_t)x->n_words); });
+    if (e != cudaSuccess) { ctx->set_error(std::string("index scratch: ") + cudaGetErrorString(e)); return fail(LL_ERR_CUDA); }
+  }
+  uint32_t* occ = dilate > 0 ? tmp : x->bits;
+  int st = LL_OK;
+  auto cu = [&](cudaError_t e) { if (e != cudaSuccess && st == LL_OK) { ctx->set_error(std::string("index build: ") + cudaGetErrorString(e)); st = LL_ERR_CUDA; } };
+  cu(cudaMemsetAsync(occ, 0, (size_t)x->n_words * 4, s));
+  RelocGrid g = grid_of(x); g.bits = nullptr;
+  for (int c = 0; c < 2; c++) if (x->n_src[c] > 0) { reloc_mark_kernel<<<ll_div_up(x->n_src[c], 256), 256, 0, s>>>(x->src[c], x->n_src[c], g, occ); ctx->launches++; }
+  if (dilate > 0) {
+    const long long threads = x->n_words * 32;
+    const unsigned blocks = (unsigned)((threads + 255) / 256);
+    uint32_t* io[3][2] = {{tmp, x->bits}, {x->bits, tmp}, {tmp, x->bits}};
+    for (int a = 0; a < 3; a++) { reloc_dilate_kernel<<<blocks, 256, 0, s>>>(io[a][0], io[a][1], dims[0], dims[1], dims[2], a, dilate, x->n_vox, x->n_words); ctx->launches++; }
+  }
+  cu(cudaGetLastError());
+  cu(cudaStreamSynchronize(s));
+  if (st != LL_OK) return fail(st);
+  *out = x;
+  return LL_OK;
+}
+
+void ll_reloc_index_release(ll_reloc_index* idx) {
+  if (!idx) return;
+  cudaSetDevice(idx->device);
+  idx->storage.release();
+  delete idx;
+}
+
+int ll_reloc_index_read(const ll_reloc_index* idx, int dims[3], float lo[3], uint32_t* words, size_t cap_words) {
+  if (!idx) return LL_ERR_INVALID;
+  if (dims) for (int a = 0; a < 3; a++) dims[a] = idx->dims[a];
+  if (lo) for (int a = 0; a < 3; a++) lo[a] = idx->lo[a];
+  if (!words) return LL_OK;
+  if (cap_words < (size_t)idx->n_words) return LL_ERR_CAPACITY;
+  cudaSetDevice(idx->device);
+  if (cudaMemcpy(words, idx->bits, (size_t)idx->n_words * 4, cudaMemcpyDeviceToHost) != cudaSuccess) return LL_ERR_CUDA;
+  return LL_OK;
+}
+
+int ll_reloc_scores(ll_ctx* ctx, const ll_reloc_index* cidx, const void* score_pts, size_t n_score, int fmt, int where, const ll_reloc_cfg* cfg, int32_t* scores) {
+  if (!ctx || !cidx || !cfg || !scores) return LL_ERR_INVALID;
+  ll_reloc_index* idx = const_cast<ll_reloc_index*>(cidx);   // (its work buffers; the index itself is not changed)
+  LL_TRY(check_points(ctx, score_pts, n_score, fmt, where, "score points"));
+  long long H = 0;
+  LL_TRY(check_cfg(ctx, idx, cfg, &H));
+  if (n_score > LL_RELOC_MAX_SCORE_POINTS) { ctx->set_error("more than LL_RELOC_MAX_SCORE_POINTS score points"); return LL_ERR_CAPACITY; }
+  if (idx->device != ctx->device) { ctx->set_error("index and context are on different devices"); return LL_ERR_INVALID; }
+  cudaSetDevice(ctx->device);
+  LL_TRY(enqueue_scores(ctx, idx, score_pts, n_score, fmt, where, cfg));
+  LL_CUDA(ctx, cudaMemcpyAsync(scores, idx->scores, (size_t)H * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return LL_OK;
+}
+
+int ll_relocalize(ll_ctx* ctx, const ll_map* map, const ll_reloc_index* cidx, const void* score_pts, size_t n_score, const void* corner, size_t n_corner,
+                  const void* surf, size_t n_surf, int fmt, int where, const ll_reloc_cfg* cfg, const ll_reg_state* tmpl, ll_reloc_candidate* cand,
+                  ll_reg_result* refined, int* item_status, int* n_cand, int* best) {
+  if (!ctx || !map || !cidx || !cfg || !tmpl || !cand || !refined || !item_status || !n_cand || !best) return LL_ERR_INVALID;
+  ll_reloc_index* idx = const_cast<ll_reloc_index*>(cidx);
+  *n_cand = 0; *best = -1;
+  LL_TRY(check_map(ctx, map));
+  if (idx->map != map || idx->src[0] != map->corner.src || idx->src[1] != map->surf.src || idx->n_src[0] != map->corner.n_src || idx->n_src[1] != map->surf.n_src) {
+    ctx->set_error("the index was built on another map (or the map was rebuilt since)"); return LL_ERR_INVALID;
+  }
+  if (idx->device != ctx->device) { ctx->set_error("index and context are on different devices"); return LL_ERR_INVALID; }
+  LL_TRY(check_points(ctx, score_pts, n_score, fmt, where, "score points"));
+  LL_TRY(check_points(ctx, corner, n_corner, fmt, where, "corner features"));
+  LL_TRY(check_points(ctx, surf, n_surf, fmt, where, "surface features"));
+  long long H = 0;
+  LL_TRY(check_cfg(ctx, idx, cfg, &H));
+  const int K = cfg->max_candidates;
+  if (K < 1 || K > LL_MAX_BATCH) { ctx->set_error("max_candidates must be 1 ... LL_MAX_BATCH"); return LL_ERR_INVALID; }
+  if (tmpl->current_frame_index <= tmpl->mapping_init_accumulate_frames) {
+    ctx->set_error("the template's frame index is at or below mapping_init_accumulate_frames: every refinement would skip the ICP (:199)"); return LL_ERR_INVALID;
+  }
+  if (n_score > LL_RELOC_MAX_SCORE_POINTS) { ctx->set_error("more than LL_RELOC_MAX_SCORE_POINTS score points"); return LL_ERR_CAPACITY; }
+  // the batch's own capacity check, for the largest batch this call can run (K items of the same features)
+  const size_t M = n_corner + n_surf;
+  if ((size_t)K * M > (size_t)ctx->cfg.max_features) { ctx->set_error("K x the features (" + std::to_string((size_t)K * M) + ") exceed max_features"); return LL_ERR_CAPACITY; }
+  { int Ms[LL_MAX_BATCH]; for (int j = 0; j < K; j++) Ms[j] = (int)M;
+    LL_TRY(solve_capacity(ctx, K, Ms, tmpl->if_motion_deblur ? 1 : 0)); }
+  cudaSetDevice(ctx->device);
+  cudaStream_t s = ctx->stream;
+  // scores -> peaks -> the first K peaks
+  LL_TRY(enqueue_scores(ctx, idx, score_pts, n_score, fmt, where, cfg));
+  LL_CUDA(ctx, cudaMemsetAsync(idx->counts, 0, 2 * sizeof(int), s));
+  reloc_peak_kernel<<<(unsigned)((H + 255) / 256), 256, 0, s>>>(idx->scores, cfg->nt[0], cfg->nt[1], cfg->nt[2], cfg->n_rot, cfg->rot_cyclic ? 1 : 0, (int)H, idx->peaks, idx->counts);
+  reloc_select_kernel<<<1, 1024, 0, s>>>(idx->peaks, idx->counts, K, idx->cand);
+  ctx->launches += 2;
+  LL_CUDA(ctx, cudaGetLastError());
+  unsigned long long keys[LL_MAX_BATCH]; int cnt[2] = {0, 0};
+  LL_CUDA(ctx, cudaMemcpyAsync(cnt, idx->counts, sizeof(cnt), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(keys, idx->cand, sizeof(keys), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  const int n = cnt[1];
+  if (n == 0) return LL_OK;
+  // refinement: the candidates as the items of one registration batch, each seeded at its hypothesis
+  const int n_lat = cfg->nt[0] * cfg->nt[1] * cfg->nt[2];
+  ll_reg_state in[LL_MAX_BATCH];
+  const void* cs[LL_MAX_BATCH]; const void* ss[LL_MAX_BATCH]; size_t ncs[LL_MAX_BATCH], nss[LL_MAX_BATCH];
+  for (int j = 0; j < n; j++) {
+    const int h = (int)(0xffffffffu - (unsigned)(keys[j] & 0xffffffffu));
+    const int r = h / n_lat, l = h - r * n_lat, li[3] = {l % cfg->nt[0], (l / cfg->nt[0]) % cfg->nt[1], l / (cfg->nt[0] * cfg->nt[1])};
+    ll_reloc_candidate& c = cand[j];
+    c.score = (int32_t)(keys[j] >> 32); c.hypothesis = h;
+    for (int k = 0; k < 4; k++) c.q_wxyz[k] = cfg->rot_wxyz[4 * r + k];
+    for (int k = 0; k < 3; k++) c.t[k] = cfg->t0[k] + (double)li[k] * cfg->step[k];
+    in[j] = *tmpl;
+    for (int k = 0; k < 4; k++) { in[j].q_w_last[k] = c.q_wxyz[k]; in[j].q_w_curr[k] = c.q_wxyz[k]; }
+    for (int k = 0; k < 3; k++) { in[j].t_w_last[k] = c.t[k]; in[j].t_w_curr[k] = c.t[k]; }
+    for (int k = 0; k < 7; k++) in[j].para_buffer_incremental[k] = k == 3 ? 1.0 : 0.0;
+    cs[j] = corner; ss[j] = surf; ncs[j] = n_corner; nss[j] = n_surf;
+  }
+  *n_cand = n;
+  LL_TRY(ll_register_batch(ctx, map, n, cs, ncs, ss, nss, fmt, where, in, refined, item_status));
+  // the choice: the smallest inlier_threshold (:559) among the accepted registrations, ties to the lower rank
+  for (int j = 0; j < n; j++) {
+    const ll_reg_result& r = refined[j];
+    if (item_status[j] != LL_OK || r.registered != 1 || r.status != 1) continue;
+    if (*best < 0 || r.inlier_threshold < refined[*best].inlier_threshold) *best = j;
+  }
+  return LL_OK;
+}
+
+}  // extern "C"

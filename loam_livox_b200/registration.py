@@ -373,6 +373,126 @@ def features_to_pointcloud2(ctx: Context, which: int) -> bytes:
     return buf.tobytes()
 
 
+def yaw_circle(yaw_step_deg: float, tilt_q=None):
+    """Rotations of a yaw circle (n = round(360 / yaw_step_deg) yaws k * step about z, k = 0 ... n - 1), each composed with an optional tilt
+    applied first: q_k = q_yaw(k) * tilt_q.  [n, 4] (w, x, y, z), fp64."""
+    n = int(round(360.0 / float(yaw_step_deg)))
+    if n < 1:
+        raise ValueError("yaw_step_deg must be in (0, 360]")
+    a = np.radians(np.arange(n) * (360.0 / n)) * 0.5
+    q = np.stack([np.cos(a), np.zeros(n), np.zeros(n), np.sin(a)], axis=1)
+    if tilt_q is not None:
+        b = np.asarray(tilt_q, np.float64)
+        b = b / np.linalg.norm(b)
+        w1, x1, y1, z1 = q.T
+        w2, x2, y2, z2 = b
+        q = np.stack([w1 * w2 - x1 * x2 - y1 * y2 - z1 * z2, w1 * x2 + x1 * w2 + y1 * z2 - z1 * y2,
+                      w1 * y2 - x1 * z2 + y1 * w2 + z1 * x2, w1 * z2 + x1 * y2 - y1 * x2 + z1 * w2], axis=1)
+    return np.ascontiguousarray(q)
+
+
+def reloc_cfg(rot_wxyz, t0, step, nt, k=8, cyclic=True):
+    """(capi.RelocCfg, keepalive) of rotations [n, 4] and the lattice t = t0 + i * step, i in 0 ... nt - 1 per axis."""
+    rot = np.ascontiguousarray(rot_wxyz, np.float64).reshape(-1, 4)
+    cfg = capi.RelocCfg()
+    cfg.n_rot = rot.shape[0]
+    cfg.rot_wxyz = rot.ctypes.data_as(C.POINTER(C.c_double))
+    cfg.rot_cyclic = int(bool(cyclic))
+    cfg.t0[:] = [float(v) for v in t0]
+    cfg.step[:] = [float(v) for v in step]
+    cfg.nt[:] = [int(v) for v in nt]
+    cfg.max_candidates = int(k)
+    return cfg, rot
+
+
+def window_lattice(window):
+    """((x0, x1, dx), (y0, y1, dy), (z0, z1, dz)) -> (t0, step, nt): every lattice point t0 + i * step inside [lo, hi] per axis (dz may be 0 for one
+    height)."""
+    t0, step, nt = [], [], []
+    for lo, hi, d in window:
+        n = 1 if d == 0 or hi == lo else int(np.floor((hi - lo) / d + 1e-9)) + 1
+        t0.append(float(lo)); step.append(float(d) if d else 1.0); nt.append(n)
+    return t0, step, nt
+
+
+class RelocIndex:
+    """The occupancy index of a map for relocalization (ll_reloc_index_build): the map's own clouds voxelised at `res`, dilated by `dilate`
+    voxels (Chebyshev), with the buffers of up to max_hypotheses hypotheses allocated once."""
+
+    def __init__(self, ctx: Context, match_map: Map, res: float = 0.2, dilate: int = 1, max_hypotheses: int = 1 << 20):
+        self.ctx, self.map = ctx, match_map
+        h = C.c_void_p()
+        ctx.check(ctx._lib.ll_reloc_index_build(ctx.h, match_map.h, float(res), int(dilate), int(max_hypotheses), C.byref(h)))
+        self.h = h
+
+    def read(self):
+        """(dims [3] int, lo [3] float32, words uint32): the bitmask, voxel x + dims0 (y + dims1 z) in bit v & 31 of word v >> 5."""
+        dims, lo = np.zeros(3, np.int32), np.zeros(3, np.float32)
+        st = self.ctx._lib.ll_reloc_index_read(self.h, dims.ctypes.data, lo.ctypes.data, None, 0)
+        if st != capi.LL_OK:
+            raise LoamLivoxError(f"ll_reloc_index_read: status {st}")
+        words = np.zeros((int(np.prod(dims.astype(np.int64))) + 31) // 32, np.uint32)
+        st = self.ctx._lib.ll_reloc_index_read(self.h, dims.ctypes.data, lo.ctypes.data, words.ctypes.data, words.shape[0])
+        if st != capi.LL_OK:
+            raise LoamLivoxError(f"ll_reloc_index_read: status {st}")
+        return dims, lo, words
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx._lib.ll_reloc_index_release(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def reloc_scores(ctx: Context, index: RelocIndex, score_pts, rot_wxyz, t0, step, nt, cyclic=True):
+    """The score of every hypothesis (ll_reloc_scores), int32 in hypothesis order h = i + nt0 (j + nt1 (k + nt2 r))."""
+    p, fmt = _pts(score_pts)
+    cfg, _keep = reloc_cfg(rot_wxyz, t0, step, nt, 1, cyclic)
+    out = np.zeros(cfg.n_rot * int(np.prod(nt)), np.int32)
+    ctx.check(ctx._lib.ll_reloc_scores(ctx.h, index.h, p.ctypes.data, p.shape[0], fmt, capi.LL_HOST, C.byref(cfg), out.ctypes.data))
+    return out
+
+
+def relocalize(ctx: Context, match_map: Map, index: RelocIndex, corners, surfs, score_leaf: float = 0.5, window=((-1.0, 1.0, 1.0), (-1.0, 1.0, 1.0), (0.0, 0.0, 0.0)),
+               yaw_step_deg: float = 10.0, tilt_q=None, k: int = 8, state: capi.RegState | None = None, score_pts=None):
+    """Find the pose of a scan (its scan-frame corner / surface features) in `match_map` without an initial guess (ll_relocalize).
+
+    The score points are a VoxelGrid of both feature clouds at score_leaf (through the library), unless score_pts is given.  The hypotheses are a
+    yaw circle of yaw_step_deg (composed with tilt_q, the sensor's roll / pitch, when given) times the translation lattice of `window`
+    (((x0, x1, dx), (y0, y1, dy), (z0, z1, dz))).  The first k peaks of the score are refined by the batched registration with `state` (default:
+    capi.default_reg_state past the initialisation gate).  Returns {"candidates": [{hypothesis, score, q, t}], "refined": [RegResult],
+    "item_status": [int], "best": rank or -1, "n_score": int}."""
+    c, fmt = _pts(corners)
+    s, fmt2 = _pts(surfs)
+    if fmt != fmt2:
+        raise ValueError("corners and surfaces in one point format")
+    if score_pts is None:
+        both = np.concatenate([c[:, :4], s[:, :4]] if fmt == capi.LL_FMT_XYZI16 else [c[:, [0, 1, 2, 4]], s[:, [0, 1, 2, 4]]], axis=0)
+        score_pts = voxel_grid_filter(ctx, both, float(score_leaf))
+    sp, sfmt = _pts(score_pts)
+    if sfmt != fmt:
+        sp = np.ascontiguousarray(sp[:, [0, 1, 2, 4]] if sfmt == capi.LL_FMT_PCL32 else np.concatenate([sp, np.zeros((sp.shape[0], 4), np.float32)], axis=1))
+    if state is None:
+        state = capi.default_reg_state()
+        state.current_frame_index = state.mapping_init_accumulate_frames + 1
+    rot = yaw_circle(yaw_step_deg, tilt_q)
+    t0, step, nt = window_lattice(window)
+    cfg, _keep = reloc_cfg(rot, t0, step, nt, k, cyclic=True)
+    K = int(k)
+    cand, res, status = (capi.RelocCandidate * K)(), (capi.RegResult * K)(), (C.c_int * K)()
+    n, best = C.c_int(), C.c_int()
+    ctx.check(ctx._lib.ll_relocalize(ctx.h, match_map.h, index.h, sp.ctypes.data, sp.shape[0], c.ctypes.data, c.shape[0], s.ctypes.data, s.shape[0], fmt, capi.LL_HOST,
+                                     C.byref(cfg), C.byref(state), cand, res, status, C.byref(n), C.byref(best)))
+    cands = [{"hypothesis": int(cand[i].hypothesis), "score": int(cand[i].score), "q": np.array(cand[i].q_wxyz), "t": np.array(cand[i].t)} for i in range(n.value)]
+    return {"candidates": cands, "refined": [res[i] for i in range(n.value)], "item_status": [int(status[i]) for i in range(n.value)], "best": int(best.value),
+            "n_score": int(sp.shape[0])}
+
+
 class Scene_alignment:
     """Mirror of Scene_alignment::find_tranfrom_of_two_mappings from the point where the four feature clouds exist
     (loam_livox/source/scene_alignment.hpp:269-353): coarse-to-fine registration of keyframe b's features onto keyframe a's."""
@@ -572,6 +692,21 @@ class Laser_mapping:
         q, t, f = np.empty(4), np.empty(3), C.c_int()
         self.ctx.check(self.ctx._lib.ll_mapper_pose(self.h, q.ctypes.data, t.ctypes.data, C.byref(f)))
         return q, t, f.value
+
+    def whole_map(self) -> Map:
+        """A new Map of the mapper's whole map (ll_mapper_whole_map): matching mode 0, the VoxelGrid of the live history window (what the next
+        refresh indexes); mode 1, the VoxelGrid of every live point of the cell maps.  The mapper is not modified."""
+        h = C.c_void_p()
+        self.ctx.check(self.ctx._lib.ll_mapper_whole_map(self.h, C.byref(h)))
+        m = Map.__new__(Map)
+        m.ctx, m.h = self.ctx, h
+        return m
+
+    def set_pose(self, q_wxyz, t):
+        """The pose the next step seeds from (ll_mapper_set_pose): e.g. a relocalized pose after a load or a tracking loss."""
+        q = np.ascontiguousarray(q_wxyz, np.float64)
+        tt = np.ascontiguousarray(t, np.float64)
+        self.ctx.check(self.ctx._lib.ll_mapper_set_pose(self.h, q.ctypes.data, tt.ctypes.data))
 
     def save(self) -> bytes:
         """The whole mapper as one byte image (ll_mapper_save; the format is specified in include/loamlivox_b200.h): Laser_mapping.load of
