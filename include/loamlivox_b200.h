@@ -469,6 +469,61 @@ int ll_relocalize(ll_ctx* ctx, const ll_map* map, const ll_reloc_index* idx,
 /* Parity hook: the scores of all n_rot x nt0 x nt1 x nt2 hypotheses (hypothesis order), validated as ll_relocalize validates them. */
 int ll_reloc_scores(ll_ctx* ctx, const ll_reloc_index* idx, const void* score_pts, size_t n_score, int fmt, int where,
                     const ll_reloc_cfg* cfg, int32_t* scores);
+
+/* ---- relocalization by class-aware distance fields (DESIGN.md §4.3.1) -----------------------------------------------------------
+ * The same search with a graded, class-aware score, a fine search around every candidate and a choice that sees the points an alias leaves
+ * outside the map: coarse peaks of the field score, each refined by a fine lattice of its own, the fine picks registered as one
+ * ll_register_batch, the accepted item of the largest field score at its refined pose chosen. */
+typedef struct ll_reloc_field ll_reloc_field;
+/* One truncated squared distance field per class of `map` (not sharded: LL_ERR_INVALID), from its own device clouds (finite points only).  The
+ * grid is that of ll_reloc_index_build with T = trunc in place of dilate: lo the map's finite bounding-box minimum, a point's cell on axis a
+ * floor(((double)x_a - (double)lo_a) / (double)res) + T in fp64, dims_a = floor(((double)hi_a - lo_a) / res) + 1 + 2 T.  D_c(v) = min(T^2, the
+ * smallest squared voxel distance |u - v|^2 from v to a voxel u holding a point of class c), one byte per voxel (a class without a point: T^2
+ * everywhere).  Built by three separable integer passes, so it is deterministic.  res <= 0 (or not finite), trunc outside 1 ... 15 or
+ * max_hypotheses outside 1 ... 2^24: LL_ERR_INVALID; more than 2^30 voxels: LL_ERR_CAPACITY; a map without a finite point: LL_ERR_INVALID; all
+ * before anything is enqueued.  Everything ll_relocalize_field needs is allocated here once (2 bytes per voxel, 48 bytes per hypothesis of
+ * max_hypotheses, the score points of both classes): ll_relocalize_field allocates no device memory.  The field belongs to this map as it is now
+ * (ll_map_rebuild of it invalidates the field), and is used by one call at a time. */
+int  ll_reloc_field_build(ll_ctx* ctx, const ll_map* map, float res, int trunc, int max_hypotheses, ll_reloc_field** out);
+void ll_reloc_field_release(ll_reloc_field* field);
+/* Parity hook: dims[3], lo[3] and the field of class `which` (0 corner, 1 surface), voxel v = x + dims0 (y + dims1 z) in byte v (dims0 dims1 dims2
+ * bytes; d2 NULL: only dims and lo; cap too small: LL_ERR_CAPACITY; which not 0 / 1: LL_ERR_INVALID). */
+int  ll_reloc_field_read(const ll_reloc_field* field, int which, int dims[3], float lo[3], uint8_t* d2, size_t cap);
+typedef struct {
+  int           n_rot;  const double* rot_wxyz;   /* offsets dq, host, n_rot x 4 (w,x,y,z), unit norm within 1e-6                          */
+  double        step[3]; int nt[3];               /* lattice per candidate: nt odd per axis, centred on the candidate's translation         */
+} ll_reloc_fine_cfg;
+typedef struct {
+  double  q_wxyz[4], t[3]; int32_t score, hypothesis;                /* the coarse peak: pose, field score, hypothesis (as ll_reloc_candidate) */
+  double  fine_q_wxyz[4], fine_t[3]; int32_t fine_score, fine_index; /* the fine pick: pose, field score, index r * n_lat + l in its group    */
+  int32_t verify_score, reserved;                                    /* the field score at refined[j]'s pose; reserved = 0                   */
+} ll_reloc_field_candidate;                                          /* 136 B */
+/* The field score of pose (q, t): every score point p of class c with finite xyz, p_w = (float)(q * p + t) (fp64 rotation, the association of
+ * ll_transform, rounded to fp32 per component) adds T^2 - D_c(cell(p_w)) when the cell is inside the grid, 0 otherwise; int32, corner points
+ * read only the corner field and surface points only the surface field.
+ * 1. Coarse: hypothesis h of `coarse` (as ll_relocalize) scored by the field score; the candidates are the first K = coarse->max_candidates peaks
+ *    (the peak definition of ll_relocalize; *n_cand <= K of them).
+ * 2. Fine: candidate j with pose (q_j, t_j) gets the group of rotations q_j (x) dq_r (Hamilton product in fp64, q_j on the left, each component
+ *    summed left to right: w = w1 w2 - x1 x2 - y1 y2 - z1 z2, x = w1 x2 + x1 w2 + y1 z2 - z1 y2, y = w1 y2 - x1 z2 + y1 w2 + z1 x2,
+ *    z = w1 z2 + x1 y2 - y1 x2 + z1 w2) times the lattice t = o_j + (i, j, k) * step, o_j = t_j - ((nt - 1) / 2) * step, fine index
+ *    l + n_lat * r as in the coarse order.  Its pick is its first index in (score descending, index ascending).
+ * 3. Refine: each pick seeds one item of ll_register_batch exactly as ll_relocalize seeds its candidates; refined[j] / item_status[j] are what
+ *    the batch returns for it.
+ * 4. Verify: cand[j].verify_score = the field score at (refined[j].q_w_curr, refined[j].t_w_curr).  *best = the rank j with item_status LL_OK,
+ *    registered 1 and status 1 of the largest verify score, ties to the smaller inlier_threshold, then to the lower rank; -1 when none qualifies
+ *    (the call still returns LL_OK).  cand / refined / item_status hold max_candidates entries.
+ * Before anything is enqueued, everything ll_relocalize refuses (with this field in place of the index; more than LL_RELOC_MAX_SCORE_POINTS
+ * score points in either class: LL_ERR_CAPACITY), and: a null fine cfg or fine rotation array, fine n_rot or nt < 1, an even fine nt, a
+ * non-finite fine step, a non-unit dq, K x the fine hypotheses above max_hypotheses, a field on another device: LL_ERR_INVALID. */
+int ll_relocalize_field(ll_ctx* ctx, const ll_map* map, const ll_reloc_field* field,
+                        const void* score_corner, size_t n_score_corner, const void* score_surf, size_t n_score_surf,
+                        const void* corner, size_t n_corner, const void* surf, size_t n_surf, int fmt, int where,
+                        const ll_reloc_cfg* coarse, const ll_reloc_fine_cfg* fine, const ll_reg_state* tmpl,
+                        ll_reloc_field_candidate* cand, ll_reg_result* refined, int* item_status, int* n_cand, int* best);
+/* Parity hook: the field scores of all n_rot x nt0 x nt1 x nt2 hypotheses of cfg (hypothesis order), validated as ll_relocalize_field
+ * validates them (max_candidates is not used). */
+int ll_reloc_field_scores(ll_ctx* ctx, const ll_reloc_field* field, const void* score_corner, size_t n_score_corner, const void* score_surf,
+                          size_t n_score_surf, int fmt, int where, const ll_reloc_cfg* cfg, int32_t* scores);
 /* A new ll_map of the mapper's whole map: mode 0 = VoxelGrid (line / plane resolution) of the live history window, exactly what the next
  * refresh indexes; mode 1 = VoxelGrid of every live point of each cell map in store order (no FOV, no radius, no down-sample-and-replace).
  * The mapper's state does not change.  LL_ERR_INVALID when either class is empty (the mapper has no map yet).  Release with ll_map_release. */

@@ -35,6 +35,7 @@ EXPORTS = [
     "ll_mapper_process_frame", "ll_voxel_downsample_segments", "ll_register_batch", "ll_mapper_process_frames", "ll_mapper_process_scans",
     "ll_mapper_save", "ll_mapper_load", "ll_mapper_image_info",
     "ll_reloc_index_build", "ll_reloc_index_release", "ll_reloc_index_read", "ll_relocalize", "ll_reloc_scores", "ll_mapper_whole_map", "ll_mapper_set_pose",
+    "ll_reloc_field_build", "ll_reloc_field_release", "ll_reloc_field_read", "ll_relocalize_field", "ll_reloc_field_scores",
 ]
 
 
@@ -109,6 +110,18 @@ class RelocCfg(C.Structure):
 
 class RelocCandidate(C.Structure):
     _fields_ = [("q_wxyz", C.c_double * 4), ("t", C.c_double * 3), ("score", C.c_int32), ("hypothesis", C.c_int32)]
+
+
+class RelocFineCfg(C.Structure):
+    """ll_reloc_fine_cfg: the fine search around every candidate (rotation offsets x an odd lattice centred on the candidate)."""
+    _fields_ = [("n_rot", C.c_int), ("rot_wxyz", C.POINTER(C.c_double)), ("step", C.c_double * 3), ("nt", C.c_int * 3)]
+
+
+class RelocFieldCandidate(C.Structure):
+    """ll_reloc_field_candidate: a coarse peak, its fine pick and the field score at its refined pose."""
+    _fields_ = [("q_wxyz", C.c_double * 4), ("t", C.c_double * 3), ("score", C.c_int32), ("hypothesis", C.c_int32),
+                ("fine_q_wxyz", C.c_double * 4), ("fine_t", C.c_double * 3), ("fine_score", C.c_int32), ("fine_index", C.c_int32),
+                ("verify_score", C.c_int32), ("reserved", C.c_int32)]
 
 
 class LoamLivoxError(RuntimeError):
@@ -204,6 +217,12 @@ def lib():
     L.ll_relocalize.argtypes = [vp, vp, vp, vp, sz, vp, sz, vp, sz, ci, ci, C.POINTER(RelocCfg), C.POINTER(RegState), C.POINTER(RelocCandidate),
                                 C.POINTER(RegResult), vp, C.POINTER(ci), C.POINTER(ci)]
     L.ll_reloc_scores.argtypes = [vp, vp, vp, sz, ci, ci, C.POINTER(RelocCfg), vp]
+    L.ll_reloc_field_build.argtypes = [vp, vp, cf, ci, ci, C.POINTER(vp)]
+    L.ll_reloc_field_release.argtypes = [vp]
+    L.ll_reloc_field_read.argtypes = [vp, ci, vp, vp, vp, sz]
+    L.ll_relocalize_field.argtypes = [vp, vp, vp, vp, sz, vp, sz, vp, sz, vp, sz, ci, ci, C.POINTER(RelocCfg), C.POINTER(RelocFineCfg), C.POINTER(RegState),
+                                      C.POINTER(RelocFieldCandidate), C.POINTER(RegResult), vp, C.POINTER(ci), C.POINTER(ci)]
+    L.ll_reloc_field_scores.argtypes = [vp, vp, vp, sz, vp, sz, ci, ci, C.POINTER(RelocCfg), vp]
     L.ll_mapper_whole_map.argtypes = [vp, C.POINTER(vp)]
     L.ll_mapper_set_pose.argtypes = [vp, vp, vp]
     L.ll_launch_count.argtypes = [vp]

@@ -3,7 +3,8 @@
 // score points land on set voxels; the first K local maxima (peaks) of the score field refined by the batched registration (ll_register_batch).
 // Beyond the reference, which has no relocalization: its only answer to a lost track is to drop the scan (laser_mapping.hpp:1413-1416).
 //
-// Built -fmad=false: the cell of a point and the transform of a score point are restated bit for bit by tests/reloc_reference.py.
+// Built -fmad=false: the cell of a point and the transform of a score point are restated bit for bit by tests/reloc_reference.py
+// (the occupancy index) and tests/reloc_field_reference.py (the distance fields).
 #include <cmath>
 #include <algorithm>
 #include "common.cuh"
@@ -31,6 +32,28 @@ struct ll_reloc_index {
   unsigned long long* cand = nullptr;   // [LL_MAX_BATCH] the first K peaks
   float4* pts = nullptr;                // [LL_RELOC_MAX_SCORE_POINTS] score points (scan frame)
   double* rot = nullptr;                // [max_hyp x 4] hypothesis rotations (w, x, y, z)
+};
+
+#define RELOC_MAX_TRUNC 15   // T^2 <= 225 fits a byte
+
+struct ll_reloc_field {
+  int device = 0;
+  const ll_map* map = nullptr; const float4* src[2] = {nullptr, nullptr}; int n_src[2] = {0, 0};   // the map it was built on
+  float res = 0.f; int trunc = 0; int max_hyp = 0;
+  int dims[3] = {0, 0, 0}; float lo[3] = {0, 0, 0};
+  long long n_vox = 0;
+  DevBuf storage;   // everything below, allocated once by ll_reloc_field_build
+  uint8_t* d2[2] = {nullptr, nullptr};  // [n_vox] per class ([0] corner, [1] surface): min(T^2, squared voxel distance to the class's nearest point)
+  int32_t* scores = nullptr;            // [max_hyp] coarse scores
+  unsigned long long* peaks = nullptr;  // [max_hyp] peak keys (score << 32 | ~h), unordered
+  int* counts = nullptr;                // [0] peaks, [1] candidates
+  unsigned long long* cand = nullptr;   // [LL_MAX_BATCH] the first K peaks
+  int32_t* fine = nullptr;              // [max_hyp] the fine groups' scores, group-major
+  unsigned long long* picks = nullptr;  // [LL_MAX_BATCH] each fine group's pick key (score << 32 | ~index)
+  int32_t* verify = nullptr;            // [LL_MAX_BATCH] the score of each refined pose
+  float4* pts[2] = {nullptr, nullptr};  // [LL_RELOC_MAX_SCORE_POINTS] score points per class (scan frame)
+  double* rot = nullptr;                // [max_hyp x 4] the rotations of every group, group-major
+  double* t0 = nullptr;                 // [LL_MAX_BATCH x 3] each group's lattice origin
 };
 
 namespace {
@@ -194,21 +217,56 @@ int check_map(ll_ctx* ctx, const ll_map* map) {
   return LL_OK;
 }
 
+// The grid of a map: lo = the minimum of the finite bounding box both trees keep (d_bbox, read before anything is enqueued) and
+// dims_a = floor((hi_a - lo_a) / res) + 1 + 2 pad.  A map without a finite point: LL_ERR_INVALID; more than 2^30 voxels: LL_ERR_CAPACITY.
+int map_grid(ll_ctx* ctx, const ll_map* map, float res, int pad, int dims[3], float lo[3]) {
+  cudaStream_t s = ctx->stream;
+  const BucketTree* tr[2] = {&map->corner, &map->surf};
+  float bb[2][6];
+  for (int c = 0; c < 2; c++) if (tr[c]->n_src > 0) LL_CUDA(ctx, cudaMemcpyAsync(bb[c], tr[c]->d_bbox, sizeof(bb[c]), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  float hi[3] = {-INFINITY, -INFINITY, -INFINITY};
+  for (int a = 0; a < 3; a++) lo[a] = INFINITY;
+  bool any = false;
+  for (int c = 0; c < 2; c++) {
+    if (tr[c]->n_src <= 0) continue;
+    bool ok = true;
+    for (int a = 0; a < 3; a++) ok = ok && std::isfinite(bb[c][a]) && std::isfinite(bb[c][3 + a]) && bb[c][a] <= bb[c][3 + a];
+    if (!ok) continue;   // no finite point in this cloud
+    any = true;
+    for (int a = 0; a < 3; a++) { lo[a] = std::min(lo[a], bb[c][a]); hi[a] = std::max(hi[a], bb[c][3 + a]); }
+  }
+  if (!any) { ctx->set_error("the map has no finite point"); return LL_ERR_INVALID; }
+  double nv = 1.0;
+  for (int a = 0; a < 3; a++) {
+    const double d = std::floor(((double)hi[a] - (double)lo[a]) / (double)res) + 1.0 + 2.0 * pad;
+    if (!(d <= (double)RELOC_MAX_VOXELS)) { ctx->set_error("more than 2^30 voxels"); return LL_ERR_CAPACITY; }
+    dims[a] = (int)d; nv *= d;
+  }
+  if (nv > (double)RELOC_MAX_VOXELS) { ctx->set_error("more than 2^30 voxels"); return LL_ERR_CAPACITY; }
+  return LL_OK;
+}
+
+bool unit_quaternions(ll_ctx* ctx, const double* rot, int n, const char* what) {
+  for (int r = 0; r < n; r++) {
+    const double* q = rot + 4 * r;
+    const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+    if (!(std::fabs(std::sqrt(n2) - 1.0) <= 1e-6)) { ctx->set_error(std::string(what) + " " + std::to_string(r) + " is not a unit quaternion"); return false; }
+  }
+  return true;
+}
+
 // The configuration's hypothesis count (*H) after every check of ll_reloc_cfg except max_candidates.
-int check_cfg(ll_ctx* ctx, const ll_reloc_index* idx, const ll_reloc_cfg* cfg, long long* H) {
+int check_cfg(ll_ctx* ctx, int max_hyp, const ll_reloc_cfg* cfg, long long* H) {
   if (!cfg->rot_wxyz) { ctx->set_error("null rotation array"); return LL_ERR_INVALID; }
   if (cfg->n_rot < 1 || cfg->nt[0] < 1 || cfg->nt[1] < 1 || cfg->nt[2] < 1) { ctx->set_error("n_rot and nt must be >= 1"); return LL_ERR_INVALID; }
   for (int a = 0; a < 3; a++)
     if (!std::isfinite(cfg->t0[a]) || !std::isfinite(cfg->step[a])) { ctx->set_error("non-finite lattice origin or step"); return LL_ERR_INVALID; }
   const long long h = (long long)cfg->n_rot * cfg->nt[0] * cfg->nt[1] * cfg->nt[2];
-  if ((long long)cfg->nt[0] * cfg->nt[1] * cfg->nt[2] > idx->max_hyp || h > idx->max_hyp) {
-    ctx->set_error("more hypotheses than the index's max_hypotheses (" + std::to_string(idx->max_hyp) + ")"); return LL_ERR_INVALID;
+  if ((long long)cfg->nt[0] * cfg->nt[1] * cfg->nt[2] > max_hyp || h > max_hyp) {
+    ctx->set_error("more hypotheses than the index's max_hypotheses (" + std::to_string(max_hyp) + ")"); return LL_ERR_INVALID;
   }
-  for (int r = 0; r < cfg->n_rot; r++) {
-    const double* q = cfg->rot_wxyz + 4 * r;
-    const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
-    if (!(std::fabs(std::sqrt(n2) - 1.0) <= 1e-6)) { ctx->set_error("rotation " + std::to_string(r) + " is not a unit quaternion"); return LL_ERR_INVALID; }
-  }
+  if (!unit_quaternions(ctx, cfg->rot_wxyz, cfg->n_rot, "rotation")) return LL_ERR_INVALID;
   *H = h;
   return LL_OK;
 }
@@ -236,6 +294,169 @@ int enqueue_scores(ll_ctx* ctx, ll_reloc_index* idx, const void* pts, size_t n, 
   return LL_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ class-aware distance fields
+__global__ void reloc_field_mark_kernel(const float4* __restrict__ src, int n, RelocGrid g, uint8_t* __restrict__ occ) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 p = src[i];
+  if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z))) return;
+  long long v;
+  if (grid_cell(g, p.x, p.y, p.z, &v)) occ[v] = 1;
+}
+
+// One separable pass of the truncated squared distance transform along `axis`, one thread per voxel.  The first pass reads occupancy:
+// min over |k| <= T of (occ(v + k e) ? k^2 : T^2); each later pass min over |k| <= T of in(v + k e) + k^2.  Voxels past the border are absent,
+// every result is clamped to T^2.  A term with |k| > T is at least T^2 + 1, so the truncated window gives the exact transform.
+__global__ void reloc_edt_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, int d0, int d1, int d2, int axis, int T, int first, long long n_vox) {
+  const long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n_vox) return;
+  const long long yz = v / d0;
+  const int x = (int)(v - yz * d0), y = (int)(yz % d1), z = (int)(yz / d1);
+  const int c = axis == 0 ? x : (axis == 1 ? y : z), D = axis == 0 ? d0 : (axis == 1 ? d1 : d2);
+  const long long stride = axis == 0 ? 1 : (axis == 1 ? (long long)d0 : (long long)d0 * d1);
+  const int T2 = T * T;
+  int best = T2;
+  for (int k = max(c - T, 0) - c; k <= min(c + T, D - 1) - c; k++) {
+    const int g = (int)in[v + (long long)k * stride];
+    best = min(best, first ? (g ? k * k : T2) : g + k * k);
+  }
+  out[v] = (uint8_t)best;
+}
+
+struct FieldScoreArgs {
+  RelocGrid g; const uint8_t* d2[2]; const float4* pts[2]; int n_pts[2];
+  const double* rot;   // [n_groups x n_rot x 4]
+  const double* t0;    // [n_groups x 3]
+  double step[3]; int nt[3]; int n_rot, n_lat, blocks_per_rot;
+  int32_t* scores;     // [n_groups x n_rot x n_lat]
+};
+// The layout of reloc_score_kernel with groups: CTA = one rotation of one group x RELOC_GROUP consecutive lattice points of that group's lattice.
+// A score point of class c adds T^2 - D_c(cell) where its p_w lands inside the grid.  Global rotation gr = r + n_rot * group; the score of
+// hypothesis l + n_lat * r of the group is at scores[gr * n_lat + l].
+__global__ void __launch_bounds__(256) reloc_field_score_kernel(FieldScoreArgs a) {
+  __shared__ double sx[RELOC_TILE], sy[RELOC_TILE], sz[RELOC_TILE];
+  __shared__ int acc[RELOC_GROUP];
+  const int gr = blockIdx.x / a.blocks_per_rot, l0 = (blockIdx.x - gr * a.blocks_per_rot) * RELOC_GROUP, grp = gr / a.n_rot;
+  const double q[4] = {a.rot[4 * gr], a.rot[4 * gr + 1], a.rot[4 * gr + 2], a.rot[4 * gr + 3]};
+  const double o[3] = {a.t0[3 * grp], a.t0[3 * grp + 1], a.t0[3 * grp + 2]};
+  const int T2 = a.g.dilate * a.g.dilate;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
+  if (threadIdx.x < RELOC_GROUP) acc[threadIdx.x] = 0;
+  for (int cls = 0; cls < 2; cls++) {
+    const uint8_t* __restrict__ f = a.d2[cls];
+    const float4* __restrict__ pts = a.pts[cls];
+    for (int base = 0; base < a.n_pts[cls]; base += RELOC_TILE) {
+      const int nt = min(RELOC_TILE, a.n_pts[cls] - base);
+      __syncthreads();
+      for (int i = threadIdx.x; i < nt; i += blockDim.x) {
+        const float4 p = pts[base + i];
+        double ox = CUDART_NAN, oy = CUDART_NAN, oz = CUDART_NAN;   // a point with a non-finite coordinate never scores
+        if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) qrot_d(q, (double)p.x, (double)p.y, (double)p.z, ox, oy, oz);
+        sx[i] = ox; sy[i] = oy; sz[i] = oz;
+      }
+      __syncthreads();
+      for (int j = warp; j < RELOC_GROUP; j += n_warps) {
+        const int l = l0 + j;
+        if (l >= a.n_lat) break;
+        const int i0 = l % a.nt[0], i1 = (l / a.nt[0]) % a.nt[1], i2 = l / (a.nt[0] * a.nt[1]);
+        const double tx = o[0] + (double)i0 * a.step[0], ty = o[1] + (double)i1 * a.step[1], tz = o[2] + (double)i2 * a.step[2];
+        int s = 0;
+        for (int p = lane; p < nt; p += 32) {
+          long long v;
+          if (grid_cell(a.g, (float)(sx[p] + tx), (float)(sy[p] + ty), (float)(sz[p] + tz), &v)) s += T2 - (int)__ldg(&f[v]);
+        }
+        for (int k = 16; k > 0; k >>= 1) s += __shfl_xor_sync(0xffffffffu, s, k);
+        if (lane == 0) acc[j] += s;   // (translation j belongs to this warp alone)
+      }
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < RELOC_GROUP && l0 + (int)threadIdx.x < a.n_lat) a.scores[(size_t)gr * a.n_lat + l0 + threadIdx.x] = acc[threadIdx.x];
+}
+
+// Each group's pick: its first hypothesis in (score descending, index ascending), as the key score << 32 | (2^32 - 1 - index).  One CTA per group
+// of `per_group` scores (all >= 0, so every key is > 0).
+__global__ void __launch_bounds__(1024) reloc_pick_kernel(const int32_t* __restrict__ scores, int per_group, unsigned long long* __restrict__ picks) {
+  __shared__ unsigned long long red[32];
+  const int32_t* s = scores + (size_t)blockIdx.x * per_group;
+  unsigned long long best = 0;
+  for (int i = threadIdx.x; i < per_group; i += blockDim.x) {
+    const unsigned long long k = ((unsigned long long)(unsigned)s[i] << 32) | (unsigned long long)(0xffffffffu - (unsigned)i);
+    best = k > best ? k : best;
+  }
+  for (int o = 16; o > 0; o >>= 1) { const unsigned long long w = __shfl_xor_sync(0xffffffffu, best, o); best = w > best ? w : best; }
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = best;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 0; w < (int)(blockDim.x >> 5); w++) best = red[w] > best ? red[w] : best;
+    picks[blockIdx.x] = best;
+  }
+}
+
+RelocGrid field_grid(const ll_reloc_field* f) {
+  RelocGrid g; g.bits = nullptr; g.res = (double)f->res; g.dilate = f->trunc;
+  for (int a = 0; a < 3; a++) { g.dims[a] = f->dims[a]; g.lo[a] = (double)f->lo[a]; }
+  return g;
+}
+
+void field_layout(ll_reloc_field* f, Carve& c) {
+  for (int k = 0; k < 2; k++) f->d2[k] = c.take<uint8_t>((size_t)f->n_vox);
+  f->scores = c.take<int32_t>(f->max_hyp); f->peaks = c.take<unsigned long long>(f->max_hyp); f->counts = c.take<int>(2);
+  f->cand = c.take<unsigned long long>(LL_MAX_BATCH); f->fine = c.take<int32_t>(f->max_hyp); f->picks = c.take<unsigned long long>(LL_MAX_BATCH);
+  f->verify = c.take<int32_t>(LL_MAX_BATCH);
+  for (int k = 0; k < 2; k++) f->pts[k] = c.take<float4>(LL_RELOC_MAX_SCORE_POINTS);
+  f->rot = c.take<double>((size_t)f->max_hyp * 4); f->t0 = c.take<double>(LL_MAX_BATCH * 3);
+}
+
+// Everything ll_reloc_field_scores and ll_relocalize_field check about the field and the score points.
+int check_field_use(ll_ctx* ctx, const ll_reloc_field* f, const void* sc, size_t n_sc, const void* ss, size_t n_ss, int fmt, int where) {
+  if (f->device != ctx->device) { ctx->set_error("field and context are on different devices"); return LL_ERR_INVALID; }
+  LL_TRY(check_points(ctx, sc, n_sc, fmt, where, "corner score points"));
+  LL_TRY(check_points(ctx, ss, n_ss, fmt, where, "surface score points"));
+  return LL_OK;
+}
+
+int check_score_counts(ll_ctx* ctx, size_t n_sc, size_t n_ss) {
+  if (n_sc > LL_RELOC_MAX_SCORE_POINTS || n_ss > LL_RELOC_MAX_SCORE_POINTS) {
+    ctx->set_error("more than LL_RELOC_MAX_SCORE_POINTS score points in a class"); return LL_ERR_CAPACITY;
+  }
+  return LL_OK;
+}
+
+// The rotations (n_groups x n_rot, host) and origins (n_groups, host) of the groups uploaded, then the score kernel: out[0 .. n_groups x n_rot x
+// n_lat) on the context's stream.  The score points are already on the device.
+int enqueue_field_scores(ll_ctx* ctx, ll_reloc_field* f, int n_sc, int n_ss, int n_groups, const double* rot, int n_rot, const double* t0,
+                         const double step[3], const int nt[3], int32_t* out) {
+  cudaStream_t s = ctx->stream;
+  LL_CUDA(ctx, cudaMemcpyAsync(f->rot, rot, (size_t)n_groups * n_rot * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(f->t0, t0, (size_t)n_groups * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
+  FieldScoreArgs a;
+  a.g = field_grid(f);
+  for (int c = 0; c < 2; c++) { a.d2[c] = f->d2[c]; a.pts[c] = f->pts[c]; }
+  a.n_pts[0] = n_sc; a.n_pts[1] = n_ss; a.rot = f->rot; a.t0 = f->t0; a.scores = out;
+  for (int k = 0; k < 3; k++) { a.step[k] = step[k]; a.nt[k] = nt[k]; }
+  a.n_rot = n_rot; a.n_lat = nt[0] * nt[1] * nt[2];
+  a.blocks_per_rot = ll_div_up(a.n_lat, RELOC_GROUP);
+  const long long blocks = (long long)n_groups * n_rot * a.blocks_per_rot;
+  reloc_field_score_kernel<<<(unsigned)blocks, 256, 0, s>>>(a); ctx->launches++;
+  LL_CUDA(ctx, cudaGetLastError());
+  return LL_OK;
+}
+
+int upload_score_points(ll_ctx* ctx, ll_reloc_field* f, const void* sc, size_t n_sc, const void* ss, size_t n_ss, int fmt, int where) {
+  LL_TRY(upload_cloud(ctx, ctx->stream, sc, n_sc, fmt, where, f->pts[0]));
+  LL_TRY(upload_cloud(ctx, ctx->stream, ss, n_ss, fmt, where, f->pts[1]));
+  return LL_OK;
+}
+
+// q1 (x) q2, the Hamilton product in fp64, each component summed left to right as written.
+void quat_mul(const double* a, const double* b, double* o) {
+  o[0] = a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3];
+  o[1] = a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2];
+  o[2] = a[0] * b[2] - a[1] * b[3] + a[2] * b[0] + a[3] * b[1];
+  o[3] = a[0] * b[3] + a[1] * b[2] - a[2] * b[1] + a[3] * b[0];
+}
+
 }  // namespace
 
 // The live points of a cell map in store order (cm_live_points, cellmap.cu) are gathered here.
@@ -257,29 +478,9 @@ int ll_reloc_index_build(ll_ctx* ctx, const ll_map* map, float res, int dilate, 
   if (max_hypotheses < 1 || max_hypotheses > RELOC_MAX_HYP) { ctx->set_error("max_hypotheses must be 1 ... 2^24"); return LL_ERR_INVALID; }
   cudaSetDevice(ctx->device);
   cudaStream_t s = ctx->stream;
-  // the anchor: the finite bounding box both trees keep (d_bbox); read before anything is enqueued
+  int dims[3]; float lo[3];
+  LL_TRY(map_grid(ctx, map, res, dilate, dims, lo));
   const BucketTree* tr[2] = {&map->corner, &map->surf};
-  float bb[2][6];
-  for (int c = 0; c < 2; c++) if (tr[c]->n_src > 0) LL_CUDA(ctx, cudaMemcpyAsync(bb[c], tr[c]->d_bbox, sizeof(bb[c]), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaStreamSynchronize(s));
-  float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-  bool any = false;
-  for (int c = 0; c < 2; c++) {
-    if (tr[c]->n_src <= 0) continue;
-    bool ok = true;
-    for (int a = 0; a < 3; a++) ok = ok && std::isfinite(bb[c][a]) && std::isfinite(bb[c][3 + a]) && bb[c][a] <= bb[c][3 + a];
-    if (!ok) continue;   // no finite point in this cloud
-    any = true;
-    for (int a = 0; a < 3; a++) { lo[a] = std::min(lo[a], bb[c][a]); hi[a] = std::max(hi[a], bb[c][3 + a]); }
-  }
-  if (!any) { ctx->set_error("the map has no finite point"); return LL_ERR_INVALID; }
-  int dims[3]; double nv = 1.0;
-  for (int a = 0; a < 3; a++) {
-    const double d = std::floor(((double)hi[a] - (double)lo[a]) / (double)res) + 1.0 + 2.0 * dilate;
-    if (!(d <= (double)RELOC_MAX_VOXELS)) { ctx->set_error("more than 2^30 voxels"); return LL_ERR_CAPACITY; }
-    dims[a] = (int)d; nv *= d;
-  }
-  if (nv > (double)RELOC_MAX_VOXELS) { ctx->set_error("more than 2^30 voxels"); return LL_ERR_CAPACITY; }
   ll_reloc_index* x = new ll_reloc_index();
   x->device = ctx->device; x->map = map; x->res = res; x->dilate = dilate; x->max_hyp = max_hypotheses;
   for (int c = 0; c < 2; c++) { x->src[c] = tr[c]->src; x->n_src[c] = tr[c]->n_src; }
@@ -336,7 +537,7 @@ int ll_reloc_scores(ll_ctx* ctx, const ll_reloc_index* cidx, const void* score_p
   ll_reloc_index* idx = const_cast<ll_reloc_index*>(cidx);   // (its work buffers; the index itself is not changed)
   LL_TRY(check_points(ctx, score_pts, n_score, fmt, where, "score points"));
   long long H = 0;
-  LL_TRY(check_cfg(ctx, idx, cfg, &H));
+  LL_TRY(check_cfg(ctx, idx->max_hyp, cfg, &H));
   if (n_score > LL_RELOC_MAX_SCORE_POINTS) { ctx->set_error("more than LL_RELOC_MAX_SCORE_POINTS score points"); return LL_ERR_CAPACITY; }
   if (idx->device != ctx->device) { ctx->set_error("index and context are on different devices"); return LL_ERR_INVALID; }
   cudaSetDevice(ctx->device);
@@ -361,7 +562,7 @@ int ll_relocalize(ll_ctx* ctx, const ll_map* map, const ll_reloc_index* cidx, co
   LL_TRY(check_points(ctx, corner, n_corner, fmt, where, "corner features"));
   LL_TRY(check_points(ctx, surf, n_surf, fmt, where, "surface features"));
   long long H = 0;
-  LL_TRY(check_cfg(ctx, idx, cfg, &H));
+  LL_TRY(check_cfg(ctx, idx->max_hyp, cfg, &H));
   const int K = cfg->max_candidates;
   if (K < 1 || K > LL_MAX_BATCH) { ctx->set_error("max_candidates must be 1 ... LL_MAX_BATCH"); return LL_ERR_INVALID; }
   if (tmpl->current_frame_index <= tmpl->mapping_init_accumulate_frames) {
@@ -412,6 +613,196 @@ int ll_relocalize(ll_ctx* ctx, const ll_map* map, const ll_reloc_index* cidx, co
     const ll_reg_result& r = refined[j];
     if (item_status[j] != LL_OK || r.registered != 1 || r.status != 1) continue;
     if (*best < 0 || r.inlier_threshold < refined[*best].inlier_threshold) *best = j;
+  }
+  return LL_OK;
+}
+
+int ll_reloc_field_build(ll_ctx* ctx, const ll_map* map, float res, int trunc, int max_hypotheses, ll_reloc_field** out) {
+  if (!ctx || !map || !out) return LL_ERR_INVALID;
+  *out = nullptr;
+  LL_TRY(check_map(ctx, map));
+  if (!(res > 0.f) || !std::isfinite(res)) { ctx->set_error("res must be a finite value > 0"); return LL_ERR_INVALID; }
+  if (trunc < 1 || trunc > RELOC_MAX_TRUNC) { ctx->set_error("trunc must be 1 ... 15"); return LL_ERR_INVALID; }
+  if (max_hypotheses < 1 || max_hypotheses > RELOC_MAX_HYP) { ctx->set_error("max_hypotheses must be 1 ... 2^24"); return LL_ERR_INVALID; }
+  cudaSetDevice(ctx->device);
+  cudaStream_t s = ctx->stream;
+  int dims[3]; float lo[3];
+  LL_TRY(map_grid(ctx, map, res, trunc, dims, lo));
+  const BucketTree* tr[2] = {&map->corner, &map->surf};
+  ll_reloc_field* f = new ll_reloc_field();
+  f->device = ctx->device; f->map = map; f->res = res; f->trunc = trunc; f->max_hyp = max_hypotheses;
+  for (int c = 0; c < 2; c++) { f->src[c] = tr[c]->src; f->n_src[c] = tr[c]->n_src; }
+  for (int a = 0; a < 3; a++) { f->dims[a] = dims[a]; f->lo[a] = lo[a]; }
+  f->n_vox = (long long)dims[0] * dims[1] * dims[2];
+  auto fail = [&](int st) { f->storage.release(); delete f; return st; };
+  { const cudaError_t e = f->storage.carve([&](Carve& c) { field_layout(f, c); });
+    if (e != cudaSuccess) { ctx->set_error(std::string("field allocation: ") + cudaGetErrorString(e)); return fail(LL_ERR_CUDA); } }
+  uint8_t* tmp = nullptr;   // occupancy, then the pass between y and z
+  { const cudaError_t e = ctx->scratch.carve([&](Carve& c) { tmp = c.take<uint8_t>((size_t)f->n_vox); });
+    if (e != cudaSuccess) { ctx->set_error(std::string("field scratch: ") + cudaGetErrorString(e)); return fail(LL_ERR_CUDA); } }
+  int st = LL_OK;
+  auto cu = [&](cudaError_t e) { if (e != cudaSuccess && st == LL_OK) { ctx->set_error(std::string("field build: ") + cudaGetErrorString(e)); st = LL_ERR_CUDA; } };
+  const RelocGrid g = field_grid(f);
+  const unsigned blocks = (unsigned)((f->n_vox + 255) / 256);
+  for (int c = 0; c < 2; c++) {
+    cu(cudaMemsetAsync(tmp, 0, (size_t)f->n_vox, s));
+    if (f->n_src[c] > 0) { reloc_field_mark_kernel<<<ll_div_up(f->n_src[c], 256), 256, 0, s>>>(f->src[c], f->n_src[c], g, tmp); ctx->launches++; }
+    uint8_t* io[3][2] = {{tmp, f->d2[c]}, {f->d2[c], tmp}, {tmp, f->d2[c]}};
+    for (int a = 0; a < 3; a++) { reloc_edt_kernel<<<blocks, 256, 0, s>>>(io[a][0], io[a][1], dims[0], dims[1], dims[2], a, trunc, a == 0 ? 1 : 0, f->n_vox); ctx->launches++; }
+  }
+  cu(cudaGetLastError());
+  cu(cudaStreamSynchronize(s));
+  if (st != LL_OK) return fail(st);
+  *out = f;
+  return LL_OK;
+}
+
+void ll_reloc_field_release(ll_reloc_field* field) {
+  if (!field) return;
+  cudaSetDevice(field->device);
+  field->storage.release();
+  delete field;
+}
+
+int ll_reloc_field_read(const ll_reloc_field* field, int which, int dims[3], float lo[3], uint8_t* d2, size_t cap) {
+  if (!field || (which != 0 && which != 1)) return LL_ERR_INVALID;
+  if (dims) for (int a = 0; a < 3; a++) dims[a] = field->dims[a];
+  if (lo) for (int a = 0; a < 3; a++) lo[a] = field->lo[a];
+  if (!d2) return LL_OK;
+  if (cap < (size_t)field->n_vox) return LL_ERR_CAPACITY;
+  cudaSetDevice(field->device);
+  if (cudaMemcpy(d2, field->d2[which], (size_t)field->n_vox, cudaMemcpyDeviceToHost) != cudaSuccess) return LL_ERR_CUDA;
+  return LL_OK;
+}
+
+int ll_reloc_field_scores(ll_ctx* ctx, const ll_reloc_field* cfield, const void* score_corner, size_t n_sc, const void* score_surf, size_t n_ss, int fmt,
+                          int where, const ll_reloc_cfg* cfg, int32_t* scores) {
+  if (!ctx || !cfield || !cfg || !scores) return LL_ERR_INVALID;
+  ll_reloc_field* f = const_cast<ll_reloc_field*>(cfield);   // (its work buffers; the fields themselves are not changed)
+  LL_TRY(check_field_use(ctx, f, score_corner, n_sc, score_surf, n_ss, fmt, where));
+  long long H = 0;
+  LL_TRY(check_cfg(ctx, f->max_hyp, cfg, &H));
+  LL_TRY(check_score_counts(ctx, n_sc, n_ss));
+  cudaSetDevice(ctx->device);
+  LL_TRY(upload_score_points(ctx, f, score_corner, n_sc, score_surf, n_ss, fmt, where));
+  LL_TRY(enqueue_field_scores(ctx, f, (int)n_sc, (int)n_ss, 1, cfg->rot_wxyz, cfg->n_rot, cfg->t0, cfg->step, cfg->nt, f->scores));
+  LL_CUDA(ctx, cudaMemcpyAsync(scores, f->scores, (size_t)H * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return LL_OK;
+}
+
+int ll_relocalize_field(ll_ctx* ctx, const ll_map* map, const ll_reloc_field* cfield, const void* score_corner, size_t n_sc, const void* score_surf,
+                        size_t n_ss, const void* corner, size_t n_corner, const void* surf, size_t n_surf, int fmt, int where, const ll_reloc_cfg* coarse,
+                        const ll_reloc_fine_cfg* fine, const ll_reg_state* tmpl, ll_reloc_field_candidate* cand, ll_reg_result* refined, int* item_status,
+                        int* n_cand, int* best) {
+  if (!ctx || !map || !cfield || !coarse || !fine || !tmpl || !cand || !refined || !item_status || !n_cand || !best) return LL_ERR_INVALID;
+  ll_reloc_field* f = const_cast<ll_reloc_field*>(cfield);
+  *n_cand = 0; *best = -1;
+  LL_TRY(check_map(ctx, map));
+  if (f->map != map || f->src[0] != map->corner.src || f->src[1] != map->surf.src || f->n_src[0] != map->corner.n_src || f->n_src[1] != map->surf.n_src) {
+    ctx->set_error("the field was built on another map (or the map was rebuilt since)"); return LL_ERR_INVALID;
+  }
+  LL_TRY(check_field_use(ctx, f, score_corner, n_sc, score_surf, n_ss, fmt, where));
+  LL_TRY(check_points(ctx, corner, n_corner, fmt, where, "corner features"));
+  LL_TRY(check_points(ctx, surf, n_surf, fmt, where, "surface features"));
+  long long H = 0;
+  LL_TRY(check_cfg(ctx, f->max_hyp, coarse, &H));
+  const int K = coarse->max_candidates;
+  if (K < 1 || K > LL_MAX_BATCH) { ctx->set_error("max_candidates must be 1 ... LL_MAX_BATCH"); return LL_ERR_INVALID; }
+  // the fine search: K groups of n_rot x nt0 x nt1 x nt2 hypotheses, centred on each candidate
+  if (!fine->rot_wxyz) { ctx->set_error("null fine rotation array"); return LL_ERR_INVALID; }
+  if (fine->n_rot < 1 || fine->nt[0] < 1 || fine->nt[1] < 1 || fine->nt[2] < 1) { ctx->set_error("fine n_rot and nt must be >= 1"); return LL_ERR_INVALID; }
+  for (int a = 0; a < 3; a++) {
+    if (fine->nt[a] % 2 == 0) { ctx->set_error("fine nt must be odd (a lattice centred on the candidate)"); return LL_ERR_INVALID; }
+    if (!std::isfinite(fine->step[a])) { ctx->set_error("non-finite fine step"); return LL_ERR_INVALID; }
+  }
+  const long long n_lat_f = (long long)fine->nt[0] * fine->nt[1] * fine->nt[2], H_f = n_lat_f * fine->n_rot;
+  if (n_lat_f > f->max_hyp || H_f > f->max_hyp || (long long)K * H_f > f->max_hyp) {
+    ctx->set_error("max_candidates x the fine hypotheses exceed the field's max_hypotheses (" + std::to_string(f->max_hyp) + ")"); return LL_ERR_INVALID;
+  }
+  if (!unit_quaternions(ctx, fine->rot_wxyz, fine->n_rot, "fine rotation")) return LL_ERR_INVALID;
+  if (tmpl->current_frame_index <= tmpl->mapping_init_accumulate_frames) {
+    ctx->set_error("the template's frame index is at or below mapping_init_accumulate_frames: every refinement would skip the ICP (:199)"); return LL_ERR_INVALID;
+  }
+  LL_TRY(check_score_counts(ctx, n_sc, n_ss));
+  // the batch's own capacity check, for the largest batch this call can run (K items of the same features)
+  const size_t M = n_corner + n_surf;
+  if ((size_t)K * M > (size_t)ctx->cfg.max_features) { ctx->set_error("K x the features (" + std::to_string((size_t)K * M) + ") exceed max_features"); return LL_ERR_CAPACITY; }
+  { int Ms[LL_MAX_BATCH]; for (int j = 0; j < K; j++) Ms[j] = (int)M;
+    LL_TRY(solve_capacity(ctx, K, Ms, tmpl->if_motion_deblur ? 1 : 0)); }
+  cudaSetDevice(ctx->device);
+  cudaStream_t s = ctx->stream;
+  // 1. coarse: scores -> peaks -> the first K peaks
+  LL_TRY(upload_score_points(ctx, f, score_corner, n_sc, score_surf, n_ss, fmt, where));
+  LL_TRY(enqueue_field_scores(ctx, f, (int)n_sc, (int)n_ss, 1, coarse->rot_wxyz, coarse->n_rot, coarse->t0, coarse->step, coarse->nt, f->scores));
+  LL_CUDA(ctx, cudaMemsetAsync(f->counts, 0, 2 * sizeof(int), s));
+  reloc_peak_kernel<<<(unsigned)((H + 255) / 256), 256, 0, s>>>(f->scores, coarse->nt[0], coarse->nt[1], coarse->nt[2], coarse->n_rot, coarse->rot_cyclic ? 1 : 0, (int)H,
+                                                                f->peaks, f->counts);
+  reloc_select_kernel<<<1, 1024, 0, s>>>(f->peaks, f->counts, K, f->cand);
+  ctx->launches += 2;
+  LL_CUDA(ctx, cudaGetLastError());
+  unsigned long long keys[LL_MAX_BATCH]; int cnt[2] = {0, 0};
+  LL_CUDA(ctx, cudaMemcpyAsync(cnt, f->counts, sizeof(cnt), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(keys, f->cand, sizeof(keys), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  const int n = cnt[1];
+  if (n == 0) return LL_OK;
+  // 2. fine: group j = the rotations q_j (x) dq_r and the lattice origin t_j - ((nt - 1) / 2) step; its pick is its best hypothesis
+  const int n_lat = coarse->nt[0] * coarse->nt[1] * coarse->nt[2];
+  std::vector<double> rot_f((size_t)n * fine->n_rot * 4);
+  double t0_f[LL_MAX_BATCH * 3];
+  for (int j = 0; j < n; j++) {
+    const int h = (int)(0xffffffffu - (unsigned)(keys[j] & 0xffffffffu));
+    const int r = h / n_lat, l = h - r * n_lat, li[3] = {l % coarse->nt[0], (l / coarse->nt[0]) % coarse->nt[1], l / (coarse->nt[0] * coarse->nt[1])};
+    ll_reloc_field_candidate& c = cand[j];
+    c.score = (int32_t)(keys[j] >> 32); c.hypothesis = h;
+    for (int k = 0; k < 4; k++) c.q_wxyz[k] = coarse->rot_wxyz[4 * r + k];
+    for (int k = 0; k < 3; k++) c.t[k] = coarse->t0[k] + (double)li[k] * coarse->step[k];
+    for (int rr = 0; rr < fine->n_rot; rr++) quat_mul(c.q_wxyz, fine->rot_wxyz + 4 * rr, &rot_f[((size_t)j * fine->n_rot + rr) * 4]);
+    for (int k = 0; k < 3; k++) t0_f[3 * j + k] = c.t[k] - (double)((fine->nt[k] - 1) / 2) * fine->step[k];
+  }
+  LL_TRY(enqueue_field_scores(ctx, f, (int)n_sc, (int)n_ss, n, rot_f.data(), fine->n_rot, t0_f, fine->step, fine->nt, f->fine));
+  reloc_pick_kernel<<<n, 1024, 0, s>>>(f->fine, (int)H_f, f->picks); ctx->launches++;
+  LL_CUDA(ctx, cudaGetLastError());
+  unsigned long long picks[LL_MAX_BATCH];
+  LL_CUDA(ctx, cudaMemcpyAsync(picks, f->picks, (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  // 3. refinement: the picks as the items of one registration batch, seeded as ll_relocalize seeds its candidates
+  ll_reg_state in[LL_MAX_BATCH];
+  const void* cs[LL_MAX_BATCH]; const void* ss[LL_MAX_BATCH]; size_t ncs[LL_MAX_BATCH], nss[LL_MAX_BATCH];
+  for (int j = 0; j < n; j++) {
+    ll_reloc_field_candidate& c = cand[j];
+    const int i = (int)(0xffffffffu - (unsigned)(picks[j] & 0xffffffffu));
+    const int r = i / (int)n_lat_f, l = i - r * (int)n_lat_f, li[3] = {l % fine->nt[0], (l / fine->nt[0]) % fine->nt[1], l / (fine->nt[0] * fine->nt[1])};
+    c.fine_score = (int32_t)(picks[j] >> 32); c.fine_index = i;
+    for (int k = 0; k < 4; k++) c.fine_q_wxyz[k] = rot_f[((size_t)j * fine->n_rot + r) * 4 + k];
+    for (int k = 0; k < 3; k++) c.fine_t[k] = t0_f[3 * j + k] + (double)li[k] * fine->step[k];
+    c.verify_score = 0; c.reserved = 0;
+    in[j] = *tmpl;
+    for (int k = 0; k < 4; k++) { in[j].q_w_last[k] = c.fine_q_wxyz[k]; in[j].q_w_curr[k] = c.fine_q_wxyz[k]; }
+    for (int k = 0; k < 3; k++) { in[j].t_w_last[k] = c.fine_t[k]; in[j].t_w_curr[k] = c.fine_t[k]; }
+    for (int k = 0; k < 7; k++) in[j].para_buffer_incremental[k] = k == 3 ? 1.0 : 0.0;
+    cs[j] = corner; ss[j] = surf; ncs[j] = n_corner; nss[j] = n_surf;
+  }
+  *n_cand = n;
+  LL_TRY(ll_register_batch(ctx, map, n, cs, ncs, ss, nss, fmt, where, in, refined, item_status));
+  // 4. verify: the same score at every refined pose (one group of one rotation and one translation each)
+  double rot_v[LL_MAX_BATCH * 4], t0_v[LL_MAX_BATCH * 3];
+  for (int j = 0; j < n; j++) {
+    for (int k = 0; k < 4; k++) rot_v[4 * j + k] = refined[j].q_w_curr[k];
+    for (int k = 0; k < 3; k++) t0_v[3 * j + k] = refined[j].t_w_curr[k];
+  }
+  const double step_v[3] = {0.0, 0.0, 0.0}; const int nt_v[3] = {1, 1, 1};
+  LL_TRY(enqueue_field_scores(ctx, f, (int)n_sc, (int)n_ss, n, rot_v, 1, t0_v, step_v, nt_v, f->verify));
+  int32_t ver[LL_MAX_BATCH];
+  LL_CUDA(ctx, cudaMemcpyAsync(ver, f->verify, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  // the choice: the accepted item of the largest verify score, ties to the smaller inlier_threshold, then to the lower rank
+  for (int j = 0; j < n; j++) {
+    cand[j].verify_score = ver[j];
+    const ll_reg_result& r = refined[j];
+    if (item_status[j] != LL_OK || r.registered != 1 || r.status != 1) continue;
+    if (*best < 0 || ver[j] > ver[*best] || (ver[j] == ver[*best] && r.inlier_threshold < refined[*best].inlier_threshold)) *best = j;
   }
   return LL_OK;
 }

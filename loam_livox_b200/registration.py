@@ -493,6 +493,124 @@ def relocalize(ctx: Context, match_map: Map, index: RelocIndex, corners, surfs, 
             "n_score": int(sp.shape[0])}
 
 
+class RelocField:
+    """The class-aware distance fields of a map for relocalization (ll_reloc_field_build): per class, the squared voxel distance at `res` to the
+    class's nearest map point, truncated at trunc^2, with the buffers of up to max_hypotheses hypotheses allocated once.  The defaults (0.2 m,
+    T = 2) are the setting that found every measured case (DESIGN.md §4.3.1)."""
+
+    def __init__(self, ctx: Context, match_map: Map, res: float = 0.2, trunc: int = 2, max_hypotheses: int = 1 << 20):
+        self.ctx, self.map = ctx, match_map
+        h = C.c_void_p()
+        ctx.check(ctx._lib.ll_reloc_field_build(ctx.h, match_map.h, float(res), int(trunc), int(max_hypotheses), C.byref(h)))
+        self.h = h
+
+    def read(self, which: int):
+        """(dims [3] int, lo [3] float32, d2 uint8 [dims2, dims1, dims0]): the field of class `which` (0 corner, 1 surface)."""
+        dims, lo = np.zeros(3, np.int32), np.zeros(3, np.float32)
+        st = self.ctx._lib.ll_reloc_field_read(self.h, int(which), dims.ctypes.data, lo.ctypes.data, None, 0)
+        if st != capi.LL_OK:
+            raise LoamLivoxError(f"ll_reloc_field_read: status {st}")
+        d2 = np.zeros((int(dims[2]), int(dims[1]), int(dims[0])), np.uint8)
+        st = self.ctx._lib.ll_reloc_field_read(self.h, int(which), dims.ctypes.data, lo.ctypes.data, d2.ctypes.data, d2.size)
+        if st != capi.LL_OK:
+            raise LoamLivoxError(f"ll_reloc_field_read: status {st}")
+        return dims, lo, d2
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx._lib.ll_reloc_field_release(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def fine_cfg(rot_wxyz, step, nt):
+    """(capi.RelocFineCfg, keepalive) of rotation offsets [n, 4] and the odd lattice nt x step centred on each candidate."""
+    rot = np.ascontiguousarray(rot_wxyz, np.float64).reshape(-1, 4)
+    cfg = capi.RelocFineCfg()
+    cfg.n_rot = rot.shape[0]
+    cfg.rot_wxyz = rot.ctypes.data_as(C.POINTER(C.c_double))
+    cfg.step[:] = [float(v) for v in step]
+    cfg.nt[:] = [int(v) for v in nt]
+    return cfg, rot
+
+
+def fine_search(yaw_step_deg: float, window, fine_yaw_step_deg: float = 1.0, fine_t_step: float = 0.1, fine_t_half: float = 1.5):
+    """The fine search of a coarse yaw circle and window: yaw offsets of +-half the coarse yaw step at fine_yaw_step_deg, and on every axis the
+    window steps along, +-fine_t_half coarse steps at fine_t_step (one point on an axis of one height).  Returns (dq [n, 4], step [3], nt [3]).
+    Half a coarse step is not enough: at a yaw 4.5 deg off, the coarse peaks of the C2 room lie about 1.5 m to either side of the truth
+    (DESIGN.md §4.3.1)."""
+    ny = int(np.floor(0.5 * float(yaw_step_deg) / float(fine_yaw_step_deg) + 1e-9))
+    a = np.radians(np.arange(-ny, ny + 1) * float(fine_yaw_step_deg)) * 0.5
+    dq = np.ascontiguousarray(np.stack([np.cos(a), np.zeros_like(a), np.zeros_like(a), np.sin(a)], axis=1))
+    _, coarse_step, coarse_nt = window_lattice(window)
+    nt = [1 if n == 1 else 2 * int(np.floor(float(fine_t_half) * d / float(fine_t_step) + 1e-9)) + 1 for d, n in zip(coarse_step, coarse_nt)]
+    return dq, [float(fine_t_step)] * 3, nt
+
+
+def _score_pair(fmt, score_corner, score_surf):
+    c, cf = _pts(score_corner)
+    s, sf = _pts(score_surf)
+    if cf != fmt or sf != fmt:
+        raise ValueError("score points in the features' point format")
+    return c, s
+
+
+def reloc_field_scores(ctx: Context, field: RelocField, score_corner, score_surf, rot_wxyz, t0, step, nt):
+    """The field score of every hypothesis (ll_reloc_field_scores), int32 in hypothesis order h = i + nt0 (j + nt1 (k + nt2 r))."""
+    c, s = _score_pair(_pts(score_corner)[1], score_corner, score_surf)
+    fmt = _pts(c)[1]
+    cfg, _keep = reloc_cfg(rot_wxyz, t0, step, nt, 1)
+    out = np.zeros(cfg.n_rot * int(np.prod(nt)), np.int32)
+    ctx.check(ctx._lib.ll_reloc_field_scores(ctx.h, field.h, c.ctypes.data, c.shape[0], s.ctypes.data, s.shape[0], fmt, capi.LL_HOST, C.byref(cfg), out.ctypes.data))
+    return out
+
+
+def relocalize_field(ctx: Context, match_map: Map, field: RelocField, corners, surfs, score_leaf: float = 0.5,
+                     window=((-1.0, 1.0, 1.0), (-1.0, 1.0, 1.0), (0.0, 0.0, 0.0)), yaw_step_deg: float = 10.0, tilt_q=None, k: int = 8,
+                     state: capi.RegState | None = None, score_pts=None, fine_yaw_step_deg: float = 1.0, fine_t_step: float = 0.1,
+                     fine_t_half: float = 1.5):
+    """Find the pose of a scan (its scan-frame corner / surface features) in `match_map` without an initial guess (ll_relocalize_field).
+
+    The score points are each class's VoxelGrid at score_leaf (through the library), unless score_pts = (corner, surface) is given.  The coarse
+    hypotheses are those of `relocalize`; every one of the first k peaks gets the fine search of `fine_search` around it, the best fine hypothesis
+    of each is refined by the batched registration with `state`, and the accepted item of the largest field score at its refined pose wins.
+    Returns {"candidates": [{hypothesis, score, q, t, fine_index, fine_score, fine_q, fine_t, verify_score}], "refined": [RegResult],
+    "item_status": [int], "best": rank or -1, "n_score": (corner, surface)}."""
+    c, fmt = _pts(corners)
+    s, fmt2 = _pts(surfs)
+    if fmt != fmt2:
+        raise ValueError("corners and surfaces in one point format")
+    if score_pts is None:
+        score_pts = (voxel_grid_filter(ctx, c, float(score_leaf)), voxel_grid_filter(ctx, s, float(score_leaf)))
+        if fmt == capi.LL_FMT_PCL32:
+            score_pts = tuple(np.concatenate([p, np.zeros((p.shape[0], 4), np.float32)], axis=1) for p in score_pts)
+    sc, ss = _score_pair(fmt, *score_pts)
+    if state is None:
+        state = capi.default_reg_state()
+        state.current_frame_index = state.mapping_init_accumulate_frames + 1
+    rot = yaw_circle(yaw_step_deg, tilt_q)
+    t0, step, nt = window_lattice(window)
+    cfg, _keep = reloc_cfg(rot, t0, step, nt, k, cyclic=True)
+    dq, fstep, fnt = fine_search(yaw_step_deg, window, fine_yaw_step_deg, fine_t_step, fine_t_half)
+    fcfg, _keep2 = fine_cfg(dq, fstep, fnt)
+    K = int(k)
+    cand, res, status = (capi.RelocFieldCandidate * K)(), (capi.RegResult * K)(), (C.c_int * K)()
+    n, best = C.c_int(), C.c_int()
+    ctx.check(ctx._lib.ll_relocalize_field(ctx.h, match_map.h, field.h, sc.ctypes.data, sc.shape[0], ss.ctypes.data, ss.shape[0], c.ctypes.data, c.shape[0],
+                                           s.ctypes.data, s.shape[0], fmt, capi.LL_HOST, C.byref(cfg), C.byref(fcfg), C.byref(state), cand, res, status,
+                                           C.byref(n), C.byref(best)))
+    cands = [{"hypothesis": int(x.hypothesis), "score": int(x.score), "q": np.array(x.q_wxyz), "t": np.array(x.t), "fine_index": int(x.fine_index),
+              "fine_score": int(x.fine_score), "fine_q": np.array(x.fine_q_wxyz), "fine_t": np.array(x.fine_t), "verify_score": int(x.verify_score)}
+             for x in (cand[i] for i in range(n.value))]
+    return {"candidates": cands, "refined": [res[i] for i in range(n.value)], "item_status": [int(status[i]) for i in range(n.value)], "best": int(best.value),
+            "n_score": (int(sc.shape[0]), int(ss.shape[0]))}
+
+
 class Scene_alignment:
     """Mirror of Scene_alignment::find_tranfrom_of_two_mappings from the point where the four feature clouds exist
     (loam_livox/source/scene_alignment.hpp:269-353): coarse-to-fine registration of keyframe b's features onto keyframe a's."""
