@@ -533,6 +533,80 @@ int ll_mapper_whole_map(ll_mapper* mapper, ll_map** out);
  * bookkeeping are untouched.  A non-finite value: LL_ERR_INVALID. */
 int ll_mapper_set_pose(ll_mapper* mapper, const double q_wxyz[4], const double t[3]);
 
+/* ---- tracking-loss recovery inside the streaming mapper (beyond the reference; DESIGN.md §4.3.2) -----------------------------------------
+ * Off by default.  When on, every mapper step (every scan, every published piece of a frame, also inside the sequence calls) judges its own
+ * registration: a registered step (registered 1) is bad when it is rejected (status 0) or its inlier_threshold (:559) exceeds
+ * max_inlier_threshold.  A bad step is held back: nothing is appended and its pose is not adopted (as a rejected scan).  After lost_after
+ * consecutive bad steps the mapper is lost; from then on every step registers as usual first, a good registration ends the loss, and a bad one
+ * runs a relocalization of the step's own features in the mapper's own whole map (ll_relocalize_field's path):
+ *   map     mode 0: the match map the mapper holds (the VoxelGrid of the live window, nothing appended since the first bad step); mode 1: the
+ *           whole map of ll_mapper_whole_map rebuilt into a mapper-owned map.  The field is built once per loss episode.
+ *   score   each class of the step's features through one VoxelGrid at score_leaf, the leaf doubled until a class fits
+ *           LL_RELOC_MAX_SCORE_POINTS.
+ *   coarse  the yaw circle of yaw_step_deg composed with the tilt of the mapper's pose (its yaw removed); the x / y lattice of t_step centred on
+ *           the mapper's translation, half-width window_base + window_growth x the consecutive bad steps, clipped to the field's grid and to
+ *           max_hypotheses; z the mapper's z.
+ *   fine    yaw offsets +-yaw_step_deg / 2 at fine_yaw_step_deg, x / y +-fine_t_half coarse steps at fine_t_step (the Python defaults).
+ *   adopt   best >= 0, verify_score / (T^2 (n_score_corner + n_score_surf)) >= min_verify_fraction and the refined inlier_threshold
+ *           <= max_inlier_threshold: the pose is set as ll_mapper_set_pose sets it; the step itself is not appended.
+ * The mapper's pose is the last good pose (or the last adopted one): the search is centred on it.  An attempt's error other than LL_ERR_CUDA is
+ * logged and the step counts as bad; LL_ERR_CUDA is returned.  Recovery is a runtime setting: it is not part of a mapper image, and a loaded
+ * mapper has it off until it is turned on again. */
+typedef struct {
+  double max_inlier_threshold;   /* the detection bound on inlier_threshold (m)                                                           */
+  int    lost_after;             /* consecutive bad steps that make the mapper lost (>= 1)                                                */
+  int    trunc;                  /* field truncation T (1 ... 15)                                                                         */
+  float  res;                    /* field voxel (m)                                                                                       */
+  float  score_leaf;             /* VoxelGrid leaf of the score points (m)                                                                */
+  double yaw_step_deg, t_step;   /* coarse yaw step (deg, a divisor of 360 up to rounding) and translation step (m)                      */
+  double window_base, window_growth;   /* lattice half-width (m) = window_base + window_growth x consecutive bad steps                    */
+  int    max_candidates;         /* K, 1 ... LL_MAX_BATCH                                                                                 */
+  int    max_hypotheses;         /* the field's hypothesis buffers (1 ... 2^24); must hold K x the fine hypotheses                        */
+  double fine_yaw_step_deg, fine_t_step, fine_t_half;   /* fine search: yaw step (deg), translation step (m), half-width in coarse steps  */
+  double min_verify_fraction;    /* adoption floor of verify_score / (T^2 x score points), 0 ... 1                                      */
+  long long reserve_field_voxels;      /* field voxels allocated by ll_mapper_set_recovery                                                */
+  long long reserve_whole_map_points;  /* mode 1: points per class of the whole map allocated by ll_mapper_set_recovery                   */
+} ll_recovery_cfg;
+void ll_mapper_recovery_default(ll_recovery_cfg* cfg);
+/* cfg NULL: recovery off (its buffers released, the state back to tracking; the log keeps its entries).  Otherwise every value is checked
+ * (LL_ERR_INVALID, the mapper unchanged) and everything an attempt needs is allocated now: the field (reserve_field_voxels, max_hypotheses),
+ * the step's features and score points, the mode-1 whole map (reserve_whole_map_points).  Past these an attempt's buffers grow, and its log
+ * entry says so.  Turning recovery on (again) starts in the tracking state. */
+int  ll_mapper_set_recovery(ll_mapper* mapper, const ll_recovery_cfg* cfg);
+enum { LL_TRACKING = 0, LL_SUSPECT = 1, LL_LOST = 2 };
+enum { LL_BAD_NONE = 0, LL_BAD_REJECTED = 1, LL_BAD_INLIER = 2 };
+/* One mapper step while recovery is on. */
+typedef struct {
+  int32_t frame_index;                 /* the registration's current_frame_index                                                        */
+  int32_t state_before, state_after;   /* LL_TRACKING / LL_SUSPECT / LL_LOST                                                            */
+  int32_t bad;                         /* LL_BAD_NONE, LL_BAD_REJECTED (status 0) or LL_BAD_INLIER (inlier_threshold over the bound)    */
+  int32_t bad_steps;                   /* consecutive bad steps after this one                                                          */
+  int32_t appended;                    /* 1 when the step's features were appended                                                     */
+  int32_t attempted;                   /* 1 when a relocalization ran; the fields below describe it                                     */
+  int32_t attempt_status;              /* LL_OK or the attempt's LL_ERR_*                                                               */
+  int32_t nt[3], n_yaw;                /* the coarse lattice and yaw count                                                              */
+  int32_t n_cand, best, adopted, grew; /* as ll_relocalize_field; adopted 1 when the pose was set; grew 1 when a buffer was reallocated */
+  int32_t n_score[2];                  /* score points per class                                                                        */
+  float   score_leaf[2];               /* the leaf each class was filtered with                                                         */
+  double  t0[3], step[3];              /* the coarse lattice                                                                            */
+  double  tilt_wxyz[4];                /* the tilt composed with the yaw circle                                                         */
+  double  verify_fraction;             /* best's verify_score / (T^2 (n_score[0] + n_score[1])); 0 when best = -1                       */
+  double  q_wxyz[4], t[3];             /* best's refined pose (the mapper's pose when best = -1)                                        */
+  double  inlier_threshold;            /* best's refined inlier_threshold                                                               */
+  double  ms_map, ms_search;           /* host wall clock: map + field build (0 when the episode's field was reused), the search        */
+} ll_recovery_step;
+#define LL_RECOVERY_LOG 1024
+/* Drains up to cap entries, oldest first, from a ring of LL_RECOVERY_LOG entries (entries past cap stay for the next read).  *n_dropped = the
+ * entries overwritten since the last read because the ring was full. */
+int  ll_mapper_recovery_read(ll_mapper* mapper, ll_recovery_step* out, int cap, int* n, int* n_dropped);
+/* Parity hook: what the last attempt passed to the search (LL_ERR_INVALID before any attempt).  n[4] = features (corner, surface) and score
+ * points (corner, surface); coarse / fine as given to the search, rot_wxyz pointing at rot_coarse / rot_fine (n_rot x 4 each; NULL arrays:
+ * counts only); tmpl = the step's registration state.  Point arrays hold cap_points, rotation arrays cap_rot rotations (LL_ERR_CAPACITY, nothing
+ * written, when short). */
+int  ll_mapper_recovery_last_inputs(ll_mapper* mapper, ll_reloc_cfg* coarse, ll_reloc_fine_cfg* fine, ll_reg_state* tmpl, size_t n[4],
+                                    ll_point* corner, ll_point* surf, ll_point* score_corner, ll_point* score_surf, size_t cap_points,
+                                    double* rot_coarse, double* rot_fine, int cap_rot);
+
 /* ---- wire formats (SURVEY 8(f) N3)---------------------------------------------------------------------------------------------- */
 /* Layout of one point record of an LL_FMT_STRIDED input: what pcl::fromROSMsg (laser_feature_extractor.hpp:275) resolves by field name from a
  * sensor_msgs/PointCloud2 (point_step, the offsets of the little-endian fields x, y, z, intensity and intensity's datatype).  The payload is

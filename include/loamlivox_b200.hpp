@@ -293,6 +293,20 @@ class Laser_mapping {
     ctx.check(ll_mapper_pose(m, out->m_q_w_curr.data(), out->m_t_w_curr.data(), &out->m_current_frame_index));
     return out;
   }
+  // tracking-loss recovery (ll_mapper_set_recovery): cfg NULL turns it off; a bad value throws and leaves the mapper unchanged.  Recovery is not
+  // part of an image: a mapper from load_from_image has it off.
+  void set_recovery(const ll_recovery_cfg* cfg) { ctx_.check(ll_mapper_set_recovery(mapper_, cfg)); }
+  // the recovery log entries since the last read, oldest first (ll_mapper_recovery_read); *dropped = entries overwritten unread
+  std::vector<ll_recovery_step> recovery_log(int* dropped = nullptr) {
+    std::vector<ll_recovery_step> out, buf(LL_RECOVERY_LOG);
+    int n = 0, d = 0, total = 0;
+    do {
+      ctx_.check(ll_mapper_recovery_read(mapper_, buf.data(), (int)buf.size(), &n, &d));
+      out.insert(out.end(), buf.begin(), buf.begin() + n); total += d;
+    } while (n == (int)buf.size());
+    if (dropped) *dropped = total;
+    return out;
+  }
   std::array<double, 4> m_q_w_curr{{1, 0, 0, 0}};   // (w, x, y, z)
   std::array<double, 3> m_t_w_curr{{0, 0, 0}};
   int m_current_frame_index = 0;

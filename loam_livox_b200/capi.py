@@ -21,6 +21,9 @@ LL_IPC_HANDLE_BYTES = 64
 LL_MAX_PIECES_PER_FRAME = 16
 LL_MAX_BATCH = 16
 LL_RELOC_MAX_SCORE_POINTS = 8192
+LL_RECOVERY_LOG = 1024
+LL_TRACKING, LL_SUSPECT, LL_LOST = 0, 1, 2
+LL_BAD_NONE, LL_BAD_REJECTED, LL_BAD_INLIER = 0, 1, 2
 LL_MAPPER_IMAGE_MAGIC, LL_MAPPER_IMAGE_VERSION = b"LLMAPIMG", 1
 (LL_IMAGE_CONFIG, LL_IMAGE_SCALARS, LL_IMAGE_HISTORY_CORNER, LL_IMAGE_HISTORY_SURF, LL_IMAGE_SNAPSHOT_CORNER, LL_IMAGE_SNAPSHOT_SURF, LL_IMAGE_CELLS_CORNER,
  LL_IMAGE_CELLS_SURF, LL_IMAGE_SECTIONS) = range(9)
@@ -36,6 +39,7 @@ EXPORTS = [
     "ll_mapper_save", "ll_mapper_load", "ll_mapper_image_info",
     "ll_reloc_index_build", "ll_reloc_index_release", "ll_reloc_index_read", "ll_relocalize", "ll_reloc_scores", "ll_mapper_whole_map", "ll_mapper_set_pose",
     "ll_reloc_field_build", "ll_reloc_field_release", "ll_reloc_field_read", "ll_relocalize_field", "ll_reloc_field_scores",
+    "ll_mapper_recovery_default", "ll_mapper_set_recovery", "ll_mapper_recovery_read", "ll_mapper_recovery_last_inputs",
 ]
 
 
@@ -122,6 +126,24 @@ class RelocFieldCandidate(C.Structure):
     _fields_ = [("q_wxyz", C.c_double * 4), ("t", C.c_double * 3), ("score", C.c_int32), ("hypothesis", C.c_int32),
                 ("fine_q_wxyz", C.c_double * 4), ("fine_t", C.c_double * 3), ("fine_score", C.c_int32), ("fine_index", C.c_int32),
                 ("verify_score", C.c_int32), ("reserved", C.c_int32)]
+
+
+class RecoveryCfg(C.Structure):
+    """ll_recovery_cfg: the streaming mapper's tracking-loss detection, relocalization search, acceptance floor and reservations."""
+    _fields_ = [("max_inlier_threshold", C.c_double), ("lost_after", C.c_int), ("trunc", C.c_int), ("res", C.c_float), ("score_leaf", C.c_float),
+                ("yaw_step_deg", C.c_double), ("t_step", C.c_double), ("window_base", C.c_double), ("window_growth", C.c_double),
+                ("max_candidates", C.c_int), ("max_hypotheses", C.c_int), ("fine_yaw_step_deg", C.c_double), ("fine_t_step", C.c_double),
+                ("fine_t_half", C.c_double), ("min_verify_fraction", C.c_double), ("reserve_field_voxels", C.c_longlong),
+                ("reserve_whole_map_points", C.c_longlong)]
+
+
+class RecoveryStep(C.Structure):
+    """ll_recovery_step: one mapper step while recovery is on (state, detection, and the relocalization attempt when there was one)."""
+    _fields_ = [(n, C.c_int32) for n in ("frame_index", "state_before", "state_after", "bad", "bad_steps", "appended", "attempted", "attempt_status")] + \
+               [("nt", C.c_int32 * 3), ("n_yaw", C.c_int32)] + [(n, C.c_int32) for n in ("n_cand", "best", "adopted", "grew")] + \
+               [("n_score", C.c_int32 * 2), ("score_leaf", C.c_float * 2), ("t0", C.c_double * 3), ("step", C.c_double * 3), ("tilt_wxyz", C.c_double * 4),
+                ("verify_fraction", C.c_double), ("q_wxyz", C.c_double * 4), ("t", C.c_double * 3), ("inlier_threshold", C.c_double),
+                ("ms_map", C.c_double), ("ms_search", C.c_double)]
 
 
 class LoamLivoxError(RuntimeError):
@@ -225,6 +247,10 @@ def lib():
     L.ll_reloc_field_scores.argtypes = [vp, vp, vp, sz, vp, sz, ci, ci, C.POINTER(RelocCfg), vp]
     L.ll_mapper_whole_map.argtypes = [vp, C.POINTER(vp)]
     L.ll_mapper_set_pose.argtypes = [vp, vp, vp]
+    L.ll_mapper_recovery_default.argtypes = [C.POINTER(RecoveryCfg)]
+    L.ll_mapper_set_recovery.argtypes = [vp, C.POINTER(RecoveryCfg)]
+    L.ll_mapper_recovery_read.argtypes = [vp, C.POINTER(RecoveryStep), ci, C.POINTER(ci), C.POINTER(ci)]
+    L.ll_mapper_recovery_last_inputs.argtypes = [vp, C.POINTER(RelocCfg), C.POINTER(RelocFineCfg), C.POINTER(RegState), vp, vp, vp, vp, vp, sz, vp, vp, ci]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64
     _LIB = L

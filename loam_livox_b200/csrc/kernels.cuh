@@ -235,6 +235,12 @@ int cm_live_points(ll_ctx* ctx, ll_cellmap* m, int n_live, float4* dst);
 
 // ---------------------------------------------------------------------------------------------- relocalization (reloc.cu)
 int launch_gather_points(ll_ctx* ctx, cudaStream_t s, const float4* src, const int* idx, int n, float4* dst);   // dst[i] = src[idx[i]]
+// The field build ll_reloc_field_build and the streaming mapper's recovery share: a field object without storage, its storage (and the build's
+// scratch) allocated for n_vox voxels and max_hyp hypotheses, and a build into it that reuses that storage (release: ll_reloc_field_release).
+ll_reloc_field* reloc_field_create(int device);
+size_t reloc_field_storage_cap(const ll_reloc_field* f);   // bytes its storage holds
+int reloc_field_reserve(ll_ctx* ctx, ll_reloc_field* f, long long n_vox, int max_hyp);
+int reloc_field_build_into(ll_ctx* ctx, const ll_map* map, float res, int trunc, int max_hypotheses, ll_reloc_field* f);
 
 // ---------------------------------------------------------------------------------------------- host driver pieces (api.cu)
 // Registration of the features already resident in A.feat (corners then surfaces): the batch of one.  Core of ll_register / ll_scan_to_pose.

@@ -53,6 +53,30 @@ struct HistoryWindow {
   void release() { buf[0].release(); buf[1].release(); segs.clear(); tail = 0; }
 };
 
+// Tracking-loss recovery (ll_mapper_set_recovery; DESIGN.md §4.3.2): the detection state, the attempt's own buffers (allocated when it is
+// turned on), the step log and what the last attempt passed to the search.
+struct Recovery {
+  bool on = false;
+  ll_recovery_cfg cfg;
+  int state = LL_TRACKING, bad = 0;   // bad: consecutive bad steps
+  bool field_valid = false;           // the field belongs to the map as it is in this loss episode
+  ll_reloc_field* field = nullptr;
+  ll_map* whole = nullptr;            // mode 1: the whole map, rebuilt in place once per episode
+  DevBuf buf;                         // the step's features and the score points of each class (RecoveryLayout)
+  std::vector<ll_recovery_step> ring; size_t first = 0, count = 0; int dropped = 0;   // the log: count entries from ring[first]
+  size_t cur = 0;                     // the ring slot of the current step's entry
+  // the last attempt's inputs (the parity hook): host copies of the rotations and cfgs, the device features and score points in buf
+  bool have_last = false;
+  std::vector<double> rot_c, rot_f;
+  ll_reloc_cfg coarse; ll_reloc_fine_cfg fine; ll_reg_state tmpl;
+  size_t n_last[4] = {0, 0, 0, 0};
+};
+// buf: a step's features (corners then surfaces, scan frame), the score points of each class, their counts
+struct RecoveryLayout {
+  float4* feat; float4* score[2]; int* cnt;
+  void layout(Carve& k, size_t n) { feat = k.take<float4>(n); score[0] = k.take<float4>(n); score[1] = k.take<float4>(n); cnt = k.take<int>(2); }
+};
+
 struct ll_mapper {
   ll_ctx* ctx = nullptr;
   HistoryWindow his_corner, his_surf;
@@ -74,6 +98,7 @@ struct ll_mapper {
   DevBuf frame[2], frame_vg[2];
   FrontGraph frame_graph[2];   // the device part of the front end, replayed per arena
   int frame_pieces = 0;        // the pieces `frame` was laid out for
+  Recovery rec;                // tracking-loss recovery (off unless ll_mapper_set_recovery turned it on)
 };
 
 // frame: the front end's device record and, per class, the gathered piece segments and the first VoxelGrid's outputs
@@ -163,7 +188,9 @@ void ll_mapper_release(ll_mapper* m) {
   if (m->match_map) ll_map_release(m->match_map);
   m->work.release(); m->snap.release(); m->his_corner.release(); m->his_surf.release();
   for (FrontGraph& g : m->frame_graph) if (g.exec) cudaGraphExecDestroy(g.exec);
-  m->frame[0].release(); m->frame[1].release(); m->frame_vg[0].release(); m->frame_vg[1].release(); delete m;
+  m->frame[0].release(); m->frame[1].release(); m->frame_vg[0].release(); m->frame_vg[1].release();
+  ll_reloc_field_release(m->rec.field); if (m->rec.whole) ll_map_release(m->rec.whole); m->rec.buf.release();
+  delete m;
 }
 int ll_mapper_pose(const ll_mapper* m, double q_wxyz[4], double t[3], int* frame_index) {
   if (!m) return LL_ERR_INVALID;
@@ -176,6 +203,8 @@ static void out_init(const ll_mapper* m, ll_reg_result* out) {
   memset(out, 0, sizeof(*out)); out->status = 1;
   for (int k = 0; k < 4; k++) out->q_w_curr[k] = m->q_w_curr[k]; for (int k = 0; k < 3; k++) out->t_w_curr[k] = m->t_w_curr[k];
 }
+
+static int recovery_step(ll_mapper* m, int nc, int ns, const ll_reg_state& st, const ll_reg_result* out, bool* hold);
 
 // One mapper step on features already in A.feat (nc corners, then ns surfaces) whose full cloud's largest time stamp is max_t: (refresh the
 // match map) -> registration -> world-frame features -> VoxelGrid -> history window and cell maps -> pose.  Every registered scan of
@@ -238,6 +267,11 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
   tp = now_ms();
   if (m->have_map) LL_TRY(register_device(ctx, m->match_map, nc, ns, &st, out));
   if (stats) stats->ms_register = (float)(now_ms() - tp);
+  if (m->rec.on) {   // a bad step is held back (and, once lost, relocalized)
+    bool hold = false;
+    LL_TRY(recovery_step(m, nc, ns, st, out, &hold));
+    if (hold) return LL_OK;
+  }
   tp = now_ms();   // no map yet: the gate of :199 returns 1
   if (out->status == 0) return LL_OK;                                           // rejected: frame discarded (:1413-1416)
   // ---- new features to the world frame (:1422-1432), VoxelGrid (:1434-1437), cell maps (:1492-1493)
@@ -278,6 +312,7 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
     fprintf(stderr, "ll_mapper trace: frame %d append %.2f ms = features %.2f + history %.2f + cells %.2f + %.2f\n", m->frame_index, now_ms() - tp, tr0 - tp, tr1 - tr0, tr2 - tr1, now_ms() - tr2);
   m->map_dirty = true;                                                           // m_if_mapping_updated_* (:1490-1491)
   if (stats) { stats->appended_corner = hc[0]; stats->appended_surf = hc[1]; stats->ms_append = (float)(now_ms() - tp); }
+  if (m->rec.on) m->rec.ring[m->rec.cur].appended = 1;
   for (int k = 0; k < 4; k++) m->q_w_curr[k] = out->q_w_curr[k]; for (int k = 0; k < 3; k++) m->t_w_curr[k] = out->t_w_curr[k];   // :1496-1505
   return LL_OK;
 }
@@ -794,10 +829,9 @@ extern "C" int ll_mapper_image_info(const void* image, size_t bytes, ll_image_in
 // ---------------------------------------------------------------------------------------------- relocalization glue
 // The whole map as a new ll_map: the clouds (mode 0: the live history window; mode 1: every live point of each cell map in store order) into
 // the context's feat_buf, their VoxelGrids at the line / plane resolution, and an index built in place.  Nothing of the mapper is written.
-extern "C" int ll_mapper_whole_map(ll_mapper* m, ll_map** out) {
-  if (!m || !out) return LL_ERR_INVALID;
-  *out = nullptr;
-  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+// The whole map's two VoxelGrid outputs in the context's feat_buf: vg[c], hc[c] points (on the device once this returns).
+static int whole_map_clouds(ll_mapper* m, float4* vg[2], int hc[2]) {
+  ll_ctx* ctx = m->ctx;
   cudaStream_t s = ctx->stream;
   size_t n[2] = {0, 0};
   ll_cellmap* cm[2] = {m->cells_corner, m->cells_surf};
@@ -808,7 +842,7 @@ extern "C" int ll_mapper_whole_map(ll_mapper* m, ll_map** out) {
     for (int c = 0; c < 2; c++) { int cells = 0, live = 0, fi = 0, oor = 0; LL_TRY(cm_count(ctx, cm[c], &cells, &live, &fi, &oor)); n[c] = (size_t)live; }
   }
   if (n[0] == 0 || n[1] == 0) { ctx->set_error("the mapper has no map yet (a class is empty)"); return LL_ERR_INVALID; }
-  float4* in[2] = {nullptr, nullptr}; float4* vg[2]; int* d_cnt;
+  float4* in[2] = {nullptr, nullptr}; int* d_cnt;
   LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) {
     if (m->cfg.matching_mode == 1) { in[0] = c.take<float4>(n[0]); in[1] = c.take<float4>(n[1]); }
     vg[0] = c.take<float4>(n[0]); vg[1] = c.take<float4>(n[1]); d_cnt = c.take<int>(2);
@@ -819,9 +853,18 @@ extern "C" int ll_mapper_whole_map(ll_mapper* m, ll_map** out) {
     if (m->cfg.matching_mode == 1) { LL_TRY(cm_live_points(ctx, cm[c], (int)n[c], in[c])); src = in[c]; }
     LL_TRY(launch_voxel_grid(ctx, s, ctx->scratch, src, (int)n[c], nullptr, leaf[c], vg[c], d_cnt + c));
   }
-  int hc[2] = {0, 0};
-  LL_CUDA(ctx, cudaMemcpyAsync(hc, d_cnt, sizeof(hc), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(hc, d_cnt, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
+  return LL_OK;
+}
+
+extern "C" int ll_mapper_whole_map(ll_mapper* m, ll_map** out) {
+  if (!m || !out) return LL_ERR_INVALID;
+  *out = nullptr;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  cudaStream_t s = ctx->stream;
+  float4* vg[2]; int hc[2] = {0, 0};
+  LL_TRY(whole_map_clouds(m, vg, hc));
   ll_map* map = nullptr;
   LL_TRY(ll_map_build(ctx, vg[0], (size_t)hc[0], vg[1], (size_t)hc[1], LL_FMT_XYZI16, LL_DEVICE, &map));
   if (cudaStreamSynchronize(s) != cudaSuccess) { ll_map_release(map); ctx->set_error("whole-map index build failed"); return LL_ERR_CUDA; }
@@ -829,13 +872,296 @@ extern "C" int ll_mapper_whole_map(ll_mapper* m, ll_map** out) {
   return LL_OK;
 }
 
+// ll_mapper_set_pose after its checks (also the adoption of a relocalized pose).
+static void mapper_set_pose(ll_mapper* m, const double q_wxyz[4], const double t[3]) {
+  if (memcmp(q_wxyz, m->q_w_curr, sizeof(m->q_w_curr)) == 0 && memcmp(t, m->t_w_curr, sizeof(m->t_w_curr)) == 0) return;
+  for (int k = 0; k < 4; k++) m->q_w_curr[k] = q_wxyz[k];
+  for (int k = 0; k < 3; k++) m->t_w_curr[k] = t[k];
+  if (m->cfg.matching_mode == 1) m->map_dirty = true;   // the assembly of mode 1 is around the pose
+}
+
 extern "C" int ll_mapper_set_pose(ll_mapper* m, const double q_wxyz[4], const double t[3]) {
   if (!m || !q_wxyz || !t) return LL_ERR_INVALID;
   for (int k = 0; k < 4; k++) if (!std::isfinite(q_wxyz[k])) return LL_ERR_INVALID;
   for (int k = 0; k < 3; k++) if (!std::isfinite(t[k])) return LL_ERR_INVALID;
-  if (memcmp(q_wxyz, m->q_w_curr, sizeof(m->q_w_curr)) == 0 && memcmp(t, m->t_w_curr, sizeof(m->t_w_curr)) == 0) return LL_OK;
-  for (int k = 0; k < 4; k++) m->q_w_curr[k] = q_wxyz[k];
-  for (int k = 0; k < 3; k++) m->t_w_curr[k] = t[k];
-  if (m->cfg.matching_mode == 1) m->map_dirty = true;   // the assembly of mode 1 is around the pose
+  mapper_set_pose(m, q_wxyz, t);
   return LL_OK;
 }
+
+// ---------------------------------------------------------------------------------------------- tracking-loss recovery
+// DESIGN.md §4.3.2.  Detection runs on the host from the step's ll_reg_result; the attempt is the library's own path: the whole map, the field
+// build shared with ll_reloc_field_build, the VoxelGrid launcher for the score points and ll_relocalize_field on device inputs.
+namespace {
+
+void qmul(const double* a, const double* b, double* o) {   // Hamilton product, as reloc.cu forms the fine rotations
+  o[0] = a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3];
+  o[1] = a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2];
+  o[2] = a[0] * b[2] - a[1] * b[3] + a[2] * b[0] + a[3] * b[1];
+  o[3] = a[0] * b[3] + a[1] * b[2] - a[2] * b[1] + a[3] * b[0];
+}
+void yaw_quat(double deg, double* q) { const double a = deg * (M_PI / 180.0) * 0.5; q[0] = cos(a); q[1] = 0; q[2] = 0; q[3] = sin(a); }
+int coarse_yaws(const ll_recovery_cfg& c) { return (int)std::lround(360.0 / c.yaw_step_deg); }
+int fine_yaws(const ll_recovery_cfg& c) { return 2 * (int)std::floor(0.5 * c.yaw_step_deg / c.fine_yaw_step_deg + 1e-9) + 1; }
+int fine_nt(const ll_recovery_cfg& c) { return 2 * (int)std::floor(c.fine_t_half * c.t_step / c.fine_t_step + 1e-9) + 1; }
+
+const char* recovery_cfg_error(const ll_recovery_cfg& c) {
+  auto pos = [](double x) { return std::isfinite(x) && x > 0.0; };
+  auto nonneg = [](double x) { return std::isfinite(x) && x >= 0.0; };
+  if (!nonneg(c.max_inlier_threshold)) return "max_inlier_threshold must be finite and >= 0";
+  if (c.lost_after < 1) return "lost_after must be >= 1";
+  if (c.trunc < 1 || c.trunc > 15) return "trunc must be 1 ... 15";
+  if (!pos(c.res)) return "res must be finite and > 0";
+  if (!pos(c.score_leaf)) return "score_leaf must be finite and > 0";
+  if (!pos(c.yaw_step_deg) || c.yaw_step_deg > 360.0) return "yaw_step_deg must be in (0, 360]";
+  if (!pos(c.t_step)) return "t_step must be finite and > 0";
+  if (!nonneg(c.window_base) || !nonneg(c.window_growth)) return "window_base and window_growth must be finite and >= 0";
+  if (c.max_candidates < 1 || c.max_candidates > LL_MAX_BATCH) return "max_candidates must be 1 ... LL_MAX_BATCH";
+  if (c.max_hypotheses < 1 || c.max_hypotheses > (1 << 24)) return "max_hypotheses must be 1 ... 2^24";
+  if (!pos(c.fine_yaw_step_deg) || !pos(c.fine_t_step) || !nonneg(c.fine_t_half)) return "fine steps must be finite and > 0, fine_t_half >= 0";
+  if (!(c.min_verify_fraction >= 0.0 && c.min_verify_fraction <= 1.0)) return "min_verify_fraction must be 0 ... 1";
+  if (c.reserve_field_voxels < 0 || c.reserve_field_voxels > (1ll << 30) || c.reserve_whole_map_points < 0 || c.reserve_whole_map_points > INT32_MAX)
+    return "reservations must be >= 0 (field voxels <= 2^30, whole-map points <= 2^31 - 1)";
+  if (coarse_yaws(c) > c.max_hypotheses) return "the yaw circle alone exceeds max_hypotheses";
+  const double fine = (double)c.max_candidates * fine_yaws(c) * fine_nt(c) * fine_nt(c);
+  if (fine > c.max_hypotheses) return "max_candidates x the fine hypotheses exceed max_hypotheses";
+  return nullptr;
+}
+
+size_t buf_caps(ll_mapper* m) {   // the bytes held by every buffer an attempt may grow
+  ll_ctx* ctx = m->ctx;
+  size_t b = ctx->scratch.cap + ctx->scratch2.cap + ctx->feat_buf.cap + ctx->stage_in.cap + m->rec.buf.cap;
+  if (m->rec.field) b += reloc_field_storage_cap(m->rec.field);
+  if (m->rec.whole) b += m->rec.whole->corner.storage.cap + m->rec.whole->surf.storage.cap;
+  return b;
+}
+
+// One class of the step's features through one VoxelGrid at the score leaf, the leaf doubled until the output fits LL_RELOC_MAX_SCORE_POINTS.
+int score_points(ll_ctx* ctx, const float4* src, int n, float leaf, float4* dst, int* d_cnt, int* n_out, float* leaf_out) {
+  *n_out = 0; *leaf_out = leaf;
+  if (n <= 0) return LL_OK;
+  for (;;) {
+    LL_TRY(launch_voxel_grid(ctx, ctx->stream, ctx->scratch, src, n, nullptr, leaf, dst, d_cnt));
+    int h = 0;
+    LL_CUDA(ctx, cudaMemcpyAsync(&h, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    *n_out = h; *leaf_out = leaf;
+    if (h <= LL_RELOC_MAX_SCORE_POINTS) return LL_OK;
+    leaf *= 2.f;
+  }
+}
+
+}  // namespace
+
+// The relocalization of one lost step (features nc + ns in A.feat, registration state st) into the log entry e; the pose is adopted when the
+// choice passes the acceptance rule.
+static int recovery_attempt(ll_mapper* m, int nc, int ns, const ll_reg_state& st, ll_recovery_step* e) {
+  ll_ctx* ctx = m->ctx;
+  Recovery& R = m->rec;
+  const ll_recovery_cfg& c = R.cfg;
+  cudaStream_t s = ctx->stream;
+  // the map and its field, once per loss episode
+  double t0 = now_ms();
+  const ll_map* map = m->match_map;   // mode 0: the VoxelGrid of the live window, nothing appended since the first bad step
+  if (!R.field_valid) {
+    if (m->cfg.matching_mode == 1) {
+      float4* vg[2]; int hc[2] = {0, 0};
+      LL_TRY(whole_map_clouds(m, vg, hc));
+      LL_TRY(ll_map_rebuild(ctx, R.whole, vg[0], (size_t)hc[0], vg[1], (size_t)hc[1], LL_FMT_XYZI16, LL_DEVICE));
+    }
+    if (m->cfg.matching_mode == 1) map = R.whole;
+    LL_TRY(reloc_field_build_into(ctx, map, c.res, c.trunc, c.max_hypotheses, R.field));
+    R.field_valid = true;
+    e->ms_map = now_ms() - t0;
+  }
+  if (m->cfg.matching_mode == 1) map = R.whole;
+  t0 = now_ms();
+  // the step's features out of A.feat (the next step overwrites them) and the score points of each class
+  RecoveryLayout rl; LL_CUDA(ctx, R.buf.carve([&](Carve& k) { rl.layout(k, (size_t)ctx->cfg.max_features); }));
+  if (nc + ns > 0) LL_CUDA(ctx, cudaMemcpyAsync(rl.feat, ctx->A.feat, (size_t)(nc + ns) * 16, cudaMemcpyDeviceToDevice, s));
+  int n_sc = 0, n_ss = 0;
+  LL_TRY(score_points(ctx, rl.feat, nc, c.score_leaf, rl.score[0], rl.cnt, &n_sc, &e->score_leaf[0]));
+  LL_TRY(score_points(ctx, rl.feat + nc, ns, c.score_leaf, rl.score[1], rl.cnt + 1, &n_ss, &e->score_leaf[1]));
+  e->n_score[0] = n_sc; e->n_score[1] = n_ss;
+  // coarse: the yaw circle x the tilt of the mapper's pose; the x / y lattice around its translation, clipped to the grid and max_hypotheses
+  const double* q = m->q_w_curr; const double* t = m->t_w_curr;
+  const double yaw = atan2(2.0 * (q[0] * q[3] + q[1] * q[2]), 1.0 - 2.0 * (q[2] * q[2] + q[3] * q[3]));
+  double qy[4], qyc[4], tilt[4];
+  yaw_quat(yaw * (180.0 / M_PI), qy);
+  qyc[0] = qy[0]; qyc[1] = -qy[1]; qyc[2] = -qy[2]; qyc[3] = -qy[3];
+  qmul(qyc, q, tilt);
+  { const double nn = sqrt(tilt[0] * tilt[0] + tilt[1] * tilt[1] + tilt[2] * tilt[2] + tilt[3] * tilt[3]); for (int k = 0; k < 4; k++) tilt[k] /= nn; }
+  const int n_yaw = coarse_yaws(c);
+  R.rot_c.resize((size_t)n_yaw * 4);
+  for (int k = 0; k < n_yaw; k++) { double a[4]; yaw_quat(k * (360.0 / n_yaw), a); qmul(a, tilt, &R.rot_c[(size_t)k * 4]); }
+  int dims[3]; float lo[3];
+  LL_TRY(ll_reloc_field_read(R.field, 0, dims, lo, nullptr, 0));
+  const double W = c.window_base + c.window_growth * R.bad;
+  const int h = (int)std::floor(W / c.t_step + 1e-9);
+  int i0[2], i1[2];
+  for (int a = 0; a < 2; a++) {
+    const double glo = (double)lo[a], ghi = (double)lo[a] + (double)(dims[a] - 2 * c.trunc) * (double)c.res;
+    i0[a] = std::max(-h, (int)std::ceil((glo - t[a]) / c.t_step));
+    i1[a] = std::min(h, (int)std::floor((ghi - t[a]) / c.t_step));
+    if (i0[a] > i1[a]) { i0[a] = i1[a] = 0; }   // the pose off the grid on this axis: its own coordinate only
+  }
+  const long long max_lat = c.max_hypotheses / n_yaw;
+  while ((long long)(i1[0] - i0[0] + 1) * (i1[1] - i0[1] + 1) > max_lat) {   // shrink the wider axis at its end farther from the pose
+    const int a = (i1[0] - i0[0]) >= (i1[1] - i0[1]) ? 0 : 1;
+    if (-i0[a] > i1[a]) i0[a]++; else i1[a]--;
+  }
+  ll_reloc_cfg& co = R.coarse;
+  memset(&co, 0, sizeof(co));
+  co.n_rot = n_yaw; co.rot_wxyz = R.rot_c.data(); co.rot_cyclic = 1; co.max_candidates = c.max_candidates;
+  for (int a = 0; a < 2; a++) { co.t0[a] = t[a] + i0[a] * c.t_step; co.step[a] = c.t_step; co.nt[a] = i1[a] - i0[a] + 1; }
+  co.t0[2] = t[2]; co.step[2] = c.t_step; co.nt[2] = 1;
+  // fine: the Python defaults (fine_search): yaw offsets +-yaw_step / 2, x / y +-fine_t_half coarse steps, one height
+  const int nfy = fine_yaws(c), ny = nfy / 2;
+  R.rot_f.resize((size_t)nfy * 4);
+  for (int k = -ny; k <= ny; k++) yaw_quat(k * c.fine_yaw_step_deg, &R.rot_f[(size_t)(k + ny) * 4]);
+  ll_reloc_fine_cfg& fi = R.fine;
+  memset(&fi, 0, sizeof(fi));
+  fi.n_rot = nfy; fi.rot_wxyz = R.rot_f.data();
+  for (int a = 0; a < 3; a++) { fi.step[a] = c.fine_t_step; fi.nt[a] = a < 2 && co.nt[a] > 1 ? fine_nt(c) : 1; }
+  R.tmpl = st;
+  for (int a = 0; a < 3; a++) { e->t0[a] = co.t0[a]; e->step[a] = co.step[a]; e->nt[a] = co.nt[a]; }
+  e->n_yaw = n_yaw;
+  for (int k = 0; k < 4; k++) e->tilt_wxyz[k] = tilt[k];
+  // K items of the step's features must fit max_features
+  const int M = nc + ns;
+  if (M > 0 && co.max_candidates * M > ctx->cfg.max_features) co.max_candidates = std::max(1, ctx->cfg.max_features / M);
+  R.n_last[0] = (size_t)nc; R.n_last[1] = (size_t)ns; R.n_last[2] = (size_t)n_sc; R.n_last[3] = (size_t)n_ss;
+  R.have_last = true;
+  ll_reloc_field_candidate cand[LL_MAX_BATCH]; ll_reg_result refined[LL_MAX_BATCH]; int item_status[LL_MAX_BATCH]; int n_cand = 0, best = -1;
+  const int rs = ll_relocalize_field(ctx, map, R.field, rl.score[0], (size_t)n_sc, rl.score[1], (size_t)n_ss, rl.feat, (size_t)nc, rl.feat + nc, (size_t)ns,
+                                     LL_FMT_XYZI16, LL_DEVICE, &co, &fi, &R.tmpl, cand, refined, item_status, &n_cand, &best);
+  e->ms_search = now_ms() - t0;
+  LL_TRY(rs);
+  e->n_cand = n_cand; e->best = best;
+  if (best < 0) return LL_OK;
+  const ll_reg_result& r = refined[best];
+  const double T2 = (double)c.trunc * c.trunc;
+  e->verify_fraction = n_sc + n_ss > 0 ? cand[best].verify_score / (T2 * (n_sc + n_ss)) : 0.0;
+  for (int k = 0; k < 4; k++) e->q_wxyz[k] = r.q_w_curr[k];
+  for (int k = 0; k < 3; k++) e->t[k] = r.t_w_curr[k];
+  e->inlier_threshold = r.inlier_threshold;
+  if (e->verify_fraction >= c.min_verify_fraction && r.inlier_threshold <= c.max_inlier_threshold) {
+    mapper_set_pose(m, r.q_w_curr, r.t_w_curr);
+    e->adopted = 1;
+  }
+  return LL_OK;
+}
+
+// The judgement of one registered step and, when the mapper is lost and the step is bad, an attempt.  *hold: the step is not appended.
+static int recovery_step(ll_mapper* m, int nc, int ns, const ll_reg_state& st, const ll_reg_result* out, bool* hold) {
+  Recovery& R = m->rec;
+  const ll_recovery_cfg& c = R.cfg;
+  if (R.count == R.ring.size()) { R.first = (R.first + 1) % R.ring.size(); R.count--; R.dropped++; }   // the oldest unread entry is overwritten
+  R.cur = (R.first + R.count) % R.ring.size(); R.count++;
+  ll_recovery_step* e = &R.ring[R.cur];
+  memset(e, 0, sizeof(*e));
+  e->frame_index = st.current_frame_index; e->state_before = R.state; e->best = -1;
+  for (int k = 0; k < 4; k++) e->q_wxyz[k] = m->q_w_curr[k];
+  for (int k = 0; k < 3; k++) e->t[k] = m->t_w_curr[k];
+  if (out->registered == 1) {   // (a step that did not register, before the map exists or under :199, is not judged)
+    if (out->status == 0) e->bad = LL_BAD_REJECTED;
+    else if (!(out->inlier_threshold <= c.max_inlier_threshold)) e->bad = LL_BAD_INLIER;
+    if (e->bad == LL_BAD_NONE) { R.bad = 0; R.state = LL_TRACKING; R.field_valid = false; }
+    else {
+      *hold = true;
+      R.bad++;
+      R.state = R.state == LL_LOST || R.bad >= c.lost_after ? LL_LOST : LL_SUSPECT;
+      if (R.state == LL_LOST) {
+        e->attempted = 1;
+        const size_t b0 = buf_caps(m);
+        const int as = recovery_attempt(m, nc, ns, st, e);
+        e->grew = buf_caps(m) != b0 ? 1 : 0;
+        e->attempt_status = as;
+        if (as == LL_ERR_CUDA) return as;
+      }
+    }
+  }
+  e->bad_steps = R.bad; e->state_after = R.state;
+  return LL_OK;
+}
+
+extern "C" {
+
+void ll_mapper_recovery_default(ll_recovery_cfg* c) {
+  if (!c) return;
+  memset(c, 0, sizeof(*c));
+  c->max_inlier_threshold = 0.1; c->lost_after = 3;           // DESIGN.md §4.3.2: normal C3-style scans stay below 0.045, kidnapped ones above 0.18
+  c->res = 0.2f; c->trunc = 2; c->score_leaf = 0.5f;          // the field defaults of §4.3.1
+  c->yaw_step_deg = 10.0; c->t_step = 1.0; c->window_base = 2.0; c->window_growth = 1.0; c->max_candidates = 8;
+  c->fine_yaw_step_deg = 1.0; c->fine_t_step = 0.1; c->fine_t_half = 1.5;
+  c->min_verify_fraction = 0.3;                               // the truth of a covered view scores 0.46 ... 0.76 (§4.3.2)
+  c->max_hypotheses = 1 << 18;
+  c->reserve_field_voxels = 1 << 22; c->reserve_whole_map_points = 1 << 20;
+}
+
+int ll_mapper_set_recovery(ll_mapper* m, const ll_recovery_cfg* cfg) {
+  if (!m) return LL_ERR_INVALID;
+  ll_ctx* ctx = m->ctx;
+  Recovery& R = m->rec;
+  if (!cfg) {
+    R.on = false; R.state = LL_TRACKING; R.bad = 0; R.field_valid = false; R.have_last = false;
+    ll_reloc_field_release(R.field); R.field = nullptr;
+    if (R.whole) ll_map_release(R.whole);
+    R.whole = nullptr; R.buf.release();
+    return LL_OK;
+  }
+  if (const char* err = recovery_cfg_error(*cfg)) { ctx->set_error(std::string("recovery config: ") + err); return LL_ERR_INVALID; }
+  cudaSetDevice(ctx->device);
+  if (!R.field) R.field = reloc_field_create(ctx->device);
+  if (!R.whole) { R.whole = new ll_map(); R.whole->device = ctx->device; }
+  LL_TRY(reloc_field_reserve(ctx, R.field, cfg->reserve_field_voxels, cfg->max_hypotheses));
+  RecoveryLayout rl; LL_CUDA(ctx, R.buf.reserve_floor(layout_bytes([&](Carve& k) { rl.layout(k, (size_t)ctx->cfg.max_features); })));
+  if (m->cfg.matching_mode == 1 && cfg->reserve_whole_map_points > 0) {   // whole_map_clouds' feat_buf, VoxelGrid and index build
+    const int W = (int)cfg->reserve_whole_map_points;
+    LL_CUDA(ctx, ctx->feat_buf.reserve_floor((size_t)W * 4 * 16 + 64));
+    const size_t side = std::max(voxel_grid_bytes(W), tree_scratch_bytes(W));
+    LL_CUDA(ctx, ctx->scratch.reserve_floor(side)); LL_CUDA(ctx, ctx->scratch2.reserve_floor(side));
+    for (BucketTree* t : {&R.whole->corner, &R.whole->surf}) LL_CUDA(ctx, t->storage.reserve_floor(tree_storage_bytes(W)));
+  }
+  if (R.ring.empty()) R.ring.resize(LL_RECOVERY_LOG);
+  R.cfg = *cfg; R.on = true; R.state = LL_TRACKING; R.bad = 0; R.field_valid = false;
+  return LL_OK;
+}
+
+int ll_mapper_recovery_read(ll_mapper* m, ll_recovery_step* out, int cap, int* n, int* n_dropped) {
+  if (!m || !n || cap < 0 || (cap > 0 && !out)) return LL_ERR_INVALID;
+  Recovery& R = m->rec;
+  const int k = (int)std::min((size_t)cap, R.count);
+  for (int i = 0; i < k; i++) out[i] = R.ring[(R.first + i) % R.ring.size()];
+  if (k > 0) { R.first = (R.first + k) % R.ring.size(); R.count -= k; }
+  *n = k;
+  if (n_dropped) *n_dropped = R.dropped;
+  R.dropped = 0;
+  return LL_OK;
+}
+
+int ll_mapper_recovery_last_inputs(ll_mapper* m, ll_reloc_cfg* coarse, ll_reloc_fine_cfg* fine, ll_reg_state* tmpl, size_t n[4], ll_point* corner, ll_point* surf,
+                                   ll_point* score_corner, ll_point* score_surf, size_t cap_points, double* rot_coarse, double* rot_fine, int cap_rot) {
+  if (!m || !n) return LL_ERR_INVALID;
+  ll_ctx* ctx = m->ctx;
+  Recovery& R = m->rec;
+  if (!R.have_last) { ctx->set_error("no relocalization attempt yet"); return LL_ERR_INVALID; }
+  for (int k = 0; k < 4; k++) n[k] = R.n_last[k];
+  const int nrc = R.coarse.n_rot, nrf = R.fine.n_rot;
+  ll_point* dst[4] = {corner, surf, score_corner, score_surf};
+  for (int k = 0; k < 4; k++) if (dst[k] && cap_points < R.n_last[k]) return LL_ERR_CAPACITY;
+  if ((rot_coarse && cap_rot < nrc) || (rot_fine && cap_rot < nrf)) return LL_ERR_CAPACITY;
+  if (coarse) { *coarse = R.coarse; coarse->rot_wxyz = rot_coarse; }
+  if (fine) { *fine = R.fine; fine->rot_wxyz = rot_fine; }
+  if (tmpl) *tmpl = R.tmpl;
+  if (rot_coarse) memcpy(rot_coarse, R.rot_c.data(), (size_t)nrc * 4 * sizeof(double));
+  if (rot_fine) memcpy(rot_fine, R.rot_f.data(), (size_t)nrf * 4 * sizeof(double));
+  cudaSetDevice(ctx->device);
+  RecoveryLayout rl; LL_CUDA(ctx, R.buf.carve([&](Carve& k) { rl.layout(k, (size_t)ctx->cfg.max_features); }));   // (reserved: no reallocation)
+  const float4* src[4] = {rl.feat, rl.feat + R.n_last[0], rl.score[0], rl.score[1]};
+  for (int k = 0; k < 4; k++)
+    if (dst[k] && R.n_last[k]) LL_CUDA(ctx, cudaMemcpyAsync(dst[k], src[k], R.n_last[k] * 16, cudaMemcpyDeviceToHost, ctx->stream));
+  LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return LL_OK;
+}
+
+}  // extern "C"

@@ -467,6 +467,57 @@ int launch_gather_points(ll_ctx* ctx, cudaStream_t s, const float4* src, const i
   return LL_OK;
 }
 
+ll_reloc_field* reloc_field_create(int device) { ll_reloc_field* f = new ll_reloc_field(); f->device = device; return f; }
+size_t reloc_field_storage_cap(const ll_reloc_field* f) { return f->storage.cap; }
+
+// The storage of a field of n_vox voxels and max_hyp hypotheses, and the context's scratch for its build: allocated now, so that a build into f
+// within these sizes allocates nothing.
+int reloc_field_reserve(ll_ctx* ctx, ll_reloc_field* f, long long n_vox, int max_hyp) {
+  ll_reloc_field x; x.n_vox = n_vox; x.max_hyp = max_hyp;
+  LL_CUDA(ctx, f->storage.reserve_floor(layout_bytes([&](Carve& c) { field_layout(&x, c); })));
+  LL_CUDA(ctx, ctx->scratch.reserve_floor((size_t)n_vox));
+  return LL_OK;
+}
+
+// ll_reloc_field_build into an existing field, reusing its storage when it is large enough (ll_reloc_field_build: a new one; the streaming
+// mapper's recovery: its own, once per loss episode).  On an error f holds no field (its map is cleared).
+int reloc_field_build_into(ll_ctx* ctx, const ll_map* map, float res, int trunc, int max_hypotheses, ll_reloc_field* f) {
+  f->map = nullptr; f->src[0] = f->src[1] = nullptr; f->n_src[0] = f->n_src[1] = 0;
+  LL_TRY(check_map(ctx, map));
+  if (!(res > 0.f) || !std::isfinite(res)) { ctx->set_error("res must be a finite value > 0"); return LL_ERR_INVALID; }
+  if (trunc < 1 || trunc > RELOC_MAX_TRUNC) { ctx->set_error("trunc must be 1 ... 15"); return LL_ERR_INVALID; }
+  if (max_hypotheses < 1 || max_hypotheses > RELOC_MAX_HYP) { ctx->set_error("max_hypotheses must be 1 ... 2^24"); return LL_ERR_INVALID; }
+  cudaSetDevice(ctx->device);
+  cudaStream_t s = ctx->stream;
+  int dims[3]; float lo[3];
+  LL_TRY(map_grid(ctx, map, res, trunc, dims, lo));
+  const BucketTree* tr[2] = {&map->corner, &map->surf};
+  f->device = ctx->device; f->res = res; f->trunc = trunc; f->max_hyp = max_hypotheses;
+  for (int a = 0; a < 3; a++) { f->dims[a] = dims[a]; f->lo[a] = lo[a]; }
+  f->n_vox = (long long)dims[0] * dims[1] * dims[2];
+  { const cudaError_t e = f->storage.carve([&](Carve& c) { field_layout(f, c); });
+    if (e != cudaSuccess) { ctx->set_error(std::string("field allocation: ") + cudaGetErrorString(e)); return LL_ERR_CUDA; } }
+  uint8_t* tmp = nullptr;   // occupancy, then the pass between y and z
+  { const cudaError_t e = ctx->scratch.carve([&](Carve& c) { tmp = c.take<uint8_t>((size_t)f->n_vox); });
+    if (e != cudaSuccess) { ctx->set_error(std::string("field scratch: ") + cudaGetErrorString(e)); return LL_ERR_CUDA; } }
+  int st = LL_OK;
+  auto cu = [&](cudaError_t e) { if (e != cudaSuccess && st == LL_OK) { ctx->set_error(std::string("field build: ") + cudaGetErrorString(e)); st = LL_ERR_CUDA; } };
+  const RelocGrid g = field_grid(f);
+  const unsigned blocks = (unsigned)((f->n_vox + 255) / 256);
+  for (int c = 0; c < 2; c++) {
+    cu(cudaMemsetAsync(tmp, 0, (size_t)f->n_vox, s));
+    if (tr[c]->n_src > 0) { reloc_field_mark_kernel<<<ll_div_up(tr[c]->n_src, 256), 256, 0, s>>>(tr[c]->src, tr[c]->n_src, g, tmp); ctx->launches++; }
+    uint8_t* io[3][2] = {{tmp, f->d2[c]}, {f->d2[c], tmp}, {tmp, f->d2[c]}};
+    for (int a = 0; a < 3; a++) { reloc_edt_kernel<<<blocks, 256, 0, s>>>(io[a][0], io[a][1], dims[0], dims[1], dims[2], a, trunc, a == 0 ? 1 : 0, f->n_vox); ctx->launches++; }
+  }
+  cu(cudaGetLastError());
+  cu(cudaStreamSynchronize(s));
+  if (st != LL_OK) return st;
+  f->map = map;
+  for (int c = 0; c < 2; c++) { f->src[c] = tr[c]->src; f->n_src[c] = tr[c]->n_src; }
+  return LL_OK;
+}
+
 extern "C" {
 
 int ll_reloc_index_build(ll_ctx* ctx, const ll_map* map, float res, int dilate, int max_hypotheses, ll_reloc_index** out) {
@@ -620,39 +671,9 @@ int ll_relocalize(ll_ctx* ctx, const ll_map* map, const ll_reloc_index* cidx, co
 int ll_reloc_field_build(ll_ctx* ctx, const ll_map* map, float res, int trunc, int max_hypotheses, ll_reloc_field** out) {
   if (!ctx || !map || !out) return LL_ERR_INVALID;
   *out = nullptr;
-  LL_TRY(check_map(ctx, map));
-  if (!(res > 0.f) || !std::isfinite(res)) { ctx->set_error("res must be a finite value > 0"); return LL_ERR_INVALID; }
-  if (trunc < 1 || trunc > RELOC_MAX_TRUNC) { ctx->set_error("trunc must be 1 ... 15"); return LL_ERR_INVALID; }
-  if (max_hypotheses < 1 || max_hypotheses > RELOC_MAX_HYP) { ctx->set_error("max_hypotheses must be 1 ... 2^24"); return LL_ERR_INVALID; }
-  cudaSetDevice(ctx->device);
-  cudaStream_t s = ctx->stream;
-  int dims[3]; float lo[3];
-  LL_TRY(map_grid(ctx, map, res, trunc, dims, lo));
-  const BucketTree* tr[2] = {&map->corner, &map->surf};
-  ll_reloc_field* f = new ll_reloc_field();
-  f->device = ctx->device; f->map = map; f->res = res; f->trunc = trunc; f->max_hyp = max_hypotheses;
-  for (int c = 0; c < 2; c++) { f->src[c] = tr[c]->src; f->n_src[c] = tr[c]->n_src; }
-  for (int a = 0; a < 3; a++) { f->dims[a] = dims[a]; f->lo[a] = lo[a]; }
-  f->n_vox = (long long)dims[0] * dims[1] * dims[2];
-  auto fail = [&](int st) { f->storage.release(); delete f; return st; };
-  { const cudaError_t e = f->storage.carve([&](Carve& c) { field_layout(f, c); });
-    if (e != cudaSuccess) { ctx->set_error(std::string("field allocation: ") + cudaGetErrorString(e)); return fail(LL_ERR_CUDA); } }
-  uint8_t* tmp = nullptr;   // occupancy, then the pass between y and z
-  { const cudaError_t e = ctx->scratch.carve([&](Carve& c) { tmp = c.take<uint8_t>((size_t)f->n_vox); });
-    if (e != cudaSuccess) { ctx->set_error(std::string("field scratch: ") + cudaGetErrorString(e)); return fail(LL_ERR_CUDA); } }
-  int st = LL_OK;
-  auto cu = [&](cudaError_t e) { if (e != cudaSuccess && st == LL_OK) { ctx->set_error(std::string("field build: ") + cudaGetErrorString(e)); st = LL_ERR_CUDA; } };
-  const RelocGrid g = field_grid(f);
-  const unsigned blocks = (unsigned)((f->n_vox + 255) / 256);
-  for (int c = 0; c < 2; c++) {
-    cu(cudaMemsetAsync(tmp, 0, (size_t)f->n_vox, s));
-    if (f->n_src[c] > 0) { reloc_field_mark_kernel<<<ll_div_up(f->n_src[c], 256), 256, 0, s>>>(f->src[c], f->n_src[c], g, tmp); ctx->launches++; }
-    uint8_t* io[3][2] = {{tmp, f->d2[c]}, {f->d2[c], tmp}, {tmp, f->d2[c]}};
-    for (int a = 0; a < 3; a++) { reloc_edt_kernel<<<blocks, 256, 0, s>>>(io[a][0], io[a][1], dims[0], dims[1], dims[2], a, trunc, a == 0 ? 1 : 0, f->n_vox); ctx->launches++; }
-  }
-  cu(cudaGetLastError());
-  cu(cudaStreamSynchronize(s));
-  if (st != LL_OK) return fail(st);
+  ll_reloc_field* f = reloc_field_create(ctx->device);
+  const int st = reloc_field_build_into(ctx, map, res, trunc, max_hypotheses, f);
+  if (st != LL_OK) { ll_reloc_field_release(f); return st; }
   *out = f;
   return LL_OK;
 }

@@ -826,6 +826,55 @@ class Laser_mapping:
         tt = np.ascontiguousarray(t, np.float64)
         self.ctx.check(self.ctx._lib.ll_mapper_set_pose(self.h, q.ctypes.data, tt.ctypes.data))
 
+    def set_recovery(self, enable: bool = True, **kw):
+        """Tracking-loss recovery (ll_mapper_set_recovery; DESIGN.md §4.3.2): from now on a bad step (rejected, or inlier_threshold above
+        max_inlier_threshold) is held back, and after lost_after of them in a row every bad step relocalizes the step's features in the mapper's
+        own map.  kw overrides fields of ll_mapper_recovery_default; enable=False turns recovery off.  Returns the capi.RecoveryCfg in force."""
+        if not enable:
+            self.ctx.check(self.ctx._lib.ll_mapper_set_recovery(self.h, None))
+            return None
+        cfg = capi.RecoveryCfg()
+        self.ctx._lib.ll_mapper_recovery_default(C.byref(cfg))
+        for k, v in kw.items():
+            if not hasattr(cfg, k):
+                raise AttributeError(k)
+            setattr(cfg, k, v)
+        self.ctx.check(self.ctx._lib.ll_mapper_set_recovery(self.h, C.byref(cfg)))
+        return cfg
+
+    def recovery_log(self):
+        """The recovery log entries since the last read (capi.RecoveryStep, oldest first) and how many were overwritten unread."""
+        out, total = [], 0
+        buf, n, dropped = (capi.RecoveryStep * capi.LL_RECOVERY_LOG)(), C.c_int(), C.c_int()
+        while True:
+            self.ctx.check(self.ctx._lib.ll_mapper_recovery_read(self.h, buf, capi.LL_RECOVERY_LOG, C.byref(n), C.byref(dropped)))
+            total += dropped.value
+            out += [capi.RecoveryStep.from_buffer_copy(buf[i]) for i in range(n.value)]
+            if n.value < capi.LL_RECOVERY_LOG:
+                return out, total
+
+    def recovery_last_inputs(self):
+        """What the last relocalization attempt passed to the search (ll_mapper_recovery_last_inputs): {"corner", "surf", "score_corner",
+        "score_surf": float32 [n, 4]; "rot_coarse", "rot_fine": [n, 4]; "coarse": RelocCfg; "fine": RelocFineCfg; "tmpl": RegState}; the cfgs point
+        at the returned rotation arrays."""
+        L = self.ctx._lib
+        n = (C.c_size_t * 4)()
+        coarse, fine, tmpl = capi.RelocCfg(), capi.RelocFineCfg(), capi.RegState()
+        self.ctx.check(L.ll_mapper_recovery_last_inputs(self.h, C.byref(coarse), C.byref(fine), C.byref(tmpl), n, None, None, None, None, 0, None, None, 0))
+        cap = max(max(n), 1)
+        pts = [np.zeros((cap, 4), np.float32) for _ in range(4)]
+        nrot = max(coarse.n_rot, fine.n_rot)
+        rc, rf = np.zeros((nrot, 4)), np.zeros((nrot, 4))
+        self.ctx.check(L.ll_mapper_recovery_last_inputs(self.h, C.byref(coarse), C.byref(fine), C.byref(tmpl), n, *[p.ctypes.data for p in pts], cap,
+                                                        rc.ctypes.data, rf.ctypes.data, nrot))
+        rc, rf = np.ascontiguousarray(rc[:coarse.n_rot]), np.ascontiguousarray(rf[:fine.n_rot])
+        coarse.rot_wxyz = rc.ctypes.data_as(C.POINTER(C.c_double))
+        fine.rot_wxyz = rf.ctypes.data_as(C.POINTER(C.c_double))
+        names = ("corner", "surf", "score_corner", "score_surf")
+        out = {k: pts[i][:n[i]].copy() for i, k in enumerate(names)}
+        out.update(rot_coarse=rc, rot_fine=rf, coarse=coarse, fine=fine, tmpl=tmpl)
+        return out
+
     def save(self) -> bytes:
         """The whole mapper as one byte image (ll_mapper_save; the format is specified in include/loamlivox_b200.h): Laser_mapping.load of
         it, on any context, continues bit for bit as this mapper does.  The mapper is not modified."""
