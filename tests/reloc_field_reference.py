@@ -1,9 +1,10 @@
 """NumPy restatement of relocalization by class-aware distance fields (ll_reloc_field_build, ll_reloc_field_scores, the fine groups and picks of
 ll_relocalize_field; include/loamlivox_b200.h, DESIGN.md §4.3.1), bit for bit.  The grid, the cells, the lattice, the score transform and the
-peaks are those of the occupancy relocalization (tests/reloc_reference.py)."""
+peaks are those of the occupancy relocalization (tests/reloc_reference.py).  `field_scores` loops over hypotheses; `field_scores_vec` and the
+one-call pipeline `relocalize_field` are fast enough for the shipped search sizes."""
 import numpy as np
 
-from reloc_reference import cells, dims_of, finite_bbox, lattice, qrot
+from reloc_reference import candidate_pose, cells, dims_of, finite_bbox, finite_points, lattice, lattice_sums, peaks, qrot
 
 
 def class_occupancy(clouds, res, T):
@@ -63,6 +64,41 @@ def field_scores(d2, dims, lo, res, T, pts, rot, t0, step, nt):
                 v = c[ok, 0] + dims[0] * (c[ok, 1] + dims[1] * c[ok, 2])
                 out[r * Tl.shape[0] + l] += int(np.sum(T2 - flat[v]))
     return out.astype(np.int32)
+
+
+def field_scores_vec(d2, dims, lo, res, T, pts, rot, t0, step, nt, chunk=None):
+    """`field_scores`, vectorised over chunks of translations x score points (reloc_reference.lattice_sums)."""
+    Tl = lattice(t0, step, nt)
+    out = np.zeros(len(rot) * Tl.shape[0], np.int64)
+    for cls in range(2):
+        p = finite_points(pts[cls])
+        value = T * T - d2[cls].reshape(-1).astype(np.int64)
+        for r, q in enumerate(rot):
+            out[r * Tl.shape[0]:(r + 1) * Tl.shape[0]] += lattice_sums(qrot(q, p), Tl, value, lo, res, T, dims, chunk)
+    return out.astype(np.int32)
+
+
+def relocalize_field(d2, dims, lo, res, T, pts, rot, t0, step, nt, K, dq, fstep, fnt, cyclic=True, chunk=None):
+    """One ll_relocalize_field call up to the refinement: coarse scores -> peaks -> the first K -> their fine groups -> each group's pick -> the
+    fine poses.  {"scores", "n_peaks", "fine": [each group's scores], "candidates": [{hypothesis, score, q, t, fine_index, fine_score, fine_q,
+    fine_t}]}."""
+    sc = field_scores_vec(d2, dims, lo, res, T, pts, rot, t0, step, nt, chunk)
+    hs, ss = peaks(sc, len(rot), nt, cyclic)
+    fine, cands = [], []
+    for h, s in zip(hs[:K], ss[:K]):
+        q, t = candidate_pose(h, rot, t0, step, nt)
+        rf, o = fine_group(q, t, dq, fstep, fnt)
+        fs = field_scores_vec(d2, dims, lo, res, T, pts, rf, o, fstep, fnt, chunk)
+        i, s_f = pick(fs)
+        fq, ft = fine_pose(rf, o, fstep, fnt, i)
+        fine.append(fs)
+        cands.append({"hypothesis": int(h), "score": int(s), "q": q, "t": t, "fine_index": i, "fine_score": s_f, "fine_q": fq, "fine_t": ft})
+    return {"scores": sc, "n_peaks": int(hs.shape[0]), "fine": fine, "candidates": cands}
+
+
+def verify_scores(d2, dims, lo, res, T, pts, poses):
+    """The field score at each (q, t) of `poses`: ll_relocalize_field's verify step at the refined poses."""
+    return [int(field_scores_vec(d2, dims, lo, res, T, pts, np.asarray(q, np.float64)[None], tuple(t), (0.0, 0.0, 0.0), (1, 1, 1))[0]) for q, t in poses]
 
 
 def field_scores_loop(d2, dims, lo, res, T, pts, rot, t0, step, nt):

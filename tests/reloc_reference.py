@@ -1,5 +1,6 @@
-"""NumPy restatement of relocalization (ll_reloc_index_build, ll_reloc_scores, the peaks of ll_relocalize; include/loamlivox_b200.h, DESIGN.md
-§4.3), bit for bit: the cells in fp64, the score transform in fp64 with Eigen's association (exact_math.cuh qrot_d), rounded to fp32."""
+"""NumPy restatement of relocalization (ll_reloc_index_build, ll_reloc_scores, the peaks and candidates of ll_relocalize; include/loamlivox_b200.h,
+DESIGN.md §4.3), bit for bit: the cells in fp64, the score transform in fp64 with Eigen's association (exact_math.cuh qrot_d), rounded to fp32.
+`scores` loops over hypotheses; `scores_vec` computes the same over chunks of translations x score points, fast enough for the shipped search sizes."""
 import numpy as np
 
 
@@ -115,6 +116,61 @@ def scores(grid, dims, lo, res, dilate, pts, rot, t0, step, nt):
             v = c[ok, 0] + dims[0] * (c[ok, 1] + dims[1] * c[ok, 2])
             out[r * T.shape[0] + l] = int(np.count_nonzero(flat[v]))
     return out
+
+
+CHUNK_ELEMS = 1 << 20   # lattice points x score points per chunk of the vectorised scorers: each [chunk, n, 3] fp64 temporary is 24 MB
+
+
+def finite_points(pts):
+    """The score points with three finite coordinates, fp64 [n, 3] (the kernels rotate a non-finite point to NaN, which never scores)."""
+    p = np.asarray(pts, np.float32).reshape(-1, 4)[:, :3]
+    return p[np.all(np.isfinite(p), axis=1)].astype(np.float64)
+
+
+def flat_cells(pw, lo, res, pad, dims):
+    """`cells` over fp32 points [..., 3] of any shape, as flat voxels v = x + dims0 (y + dims1 z) ([...] int64, 0 outside) and the mask of those
+    inside the grid."""
+    dims = np.asarray(dims, np.int64)
+    with np.errstate(invalid="ignore", over="ignore"):
+        d = np.floor((pw.astype(np.float64) - np.asarray(lo, np.float32).astype(np.float64)) / float(np.float32(res))) + float(pad)
+        ok = np.all((d >= 0.0) & (d < dims.astype(np.float64)), axis=-1)
+    c = np.where(ok[..., None], d, 0.0).astype(np.int64)
+    return c[..., 0] + dims[0] * (c[..., 1] + dims[1] * c[..., 2]), ok
+
+
+def lattice_sums(rp, T, value, lo, res, pad, dims, chunk=None):
+    """[n_lat] int64: for every translation T[l] (fp64), the sum of value[v] over the rotated points rp [n, 3] (fp64) whose p_w = fp32(rp + T[l])
+    lands in voxel v of the grid.  `chunk` translations at a time (default CHUNK_ELEMS / n): the per-hypothesis loop of `scores`, vectorised with
+    the same arithmetic element for element."""
+    out = np.zeros(T.shape[0], np.int64)
+    if rp.shape[0] == 0 or T.shape[0] == 0:
+        return out
+    c = int(chunk) if chunk else max(1, CHUNK_ELEMS // rp.shape[0])
+    for l0 in range(0, T.shape[0], c):
+        v, ok = flat_cells((rp[None, :, :] + T[l0:l0 + c, None, :]).astype(np.float32), lo, res, pad, dims)
+        out[l0:l0 + c] = np.where(ok, value[v], 0).sum(axis=1)
+    return out
+
+
+def scores_vec(grid, dims, lo, res, dilate, pts, rot, t0, step, nt, chunk=None):
+    """`scores`, vectorised over chunks of translations x score points."""
+    p = finite_points(pts)
+    T = lattice(t0, step, nt)
+    flat = grid.reshape(-1).astype(np.int64)
+    out = [lattice_sums(qrot(q, p), T, flat, lo, res, dilate, dims, chunk) for q in rot]
+    return np.concatenate(out).astype(np.int32) if out else np.zeros(0, np.int32)
+
+
+def relocalize(grid, dims, lo, res, dilate, pts, rot, t0, step, nt, K, cyclic=True, chunk=None):
+    """One ll_relocalize call up to the refinement: coarse scores -> peaks -> the first K.  {"scores", "n_peaks", "candidates": [{hypothesis,
+    score, q, t}]}."""
+    sc = scores_vec(grid, dims, lo, res, dilate, pts, rot, t0, step, nt, chunk)
+    hs, ss = peaks(sc, len(rot), nt, cyclic)
+    cands = []
+    for h, s in zip(hs[:K], ss[:K]):
+        q, t = candidate_pose(h, rot, t0, step, nt)
+        cands.append({"hypothesis": int(h), "score": int(s), "q": q, "t": t})
+    return {"scores": sc, "n_peaks": int(hs.shape[0]), "candidates": cands}
 
 
 def scores_loop(grid, dims, lo, res, dilate, pts, rot, t0, step, nt):

@@ -12,7 +12,6 @@ import pytest
 sys.path.insert(0, os.path.dirname(__file__))
 from loam_livox_b200 import synthetic as S  # noqa: E402
 import reloc_field_reference as F  # noqa: E402
-import reloc_reference as R  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -119,20 +118,6 @@ def test_field_scores_equal_numpy(ctxs):
     f.close()
 
 
-def _numpy_call(d2, dims, lo, res, T, pts, rot, t0, step, nt, K, dq, fstep, fnt):
-    """NumPy's candidates [(h, score, q, t, fine index, fine score, fine q, fine t)] of one ll_relocalize_field call."""
-    sc = F.field_scores(d2, dims, lo, res, T, pts, rot, t0, step, nt)
-    hs, ss = R.peaks(sc, rot.shape[0], nt, True)
-    out = []
-    for h, s in zip(hs[:K], ss[:K]):
-        q, t = R.candidate_pose(h, rot, t0, step, nt)
-        rf, o = F.fine_group(q, t, dq, fstep, fnt)
-        i, fs = F.pick(F.field_scores(d2, dims, lo, res, T, pts, rf, o, fstep, fnt))
-        fq, ft = F.fine_pose(rf, o, fstep, fnt, i)
-        out.append((int(h), int(s), q, t, i, fs, fq, ft))
-    return out
-
-
 def test_one_call_equals_numpy_and_the_batch(ctxs):
     from loam_livox_b200 import capi
     from loam_livox_b200.registration import fine_search, register_batch, relocalize_field, window_lattice, yaw_circle
@@ -146,11 +131,11 @@ def test_one_call_equals_numpy_and_the_batch(ctxs):
     rot = yaw_circle(5.0)
     t0, step, nt = window_lattice(window)
     dq, fstep, fnt = fine_search(5.0, window, 1.0, 0.05, 0.5)
-    want = _numpy_call(d2, dims, lo, 0.3, 5, pts, rot, t0, step, nt, 6, dq, fstep, fnt)
+    want = F.relocalize_field(d2, dims, lo, 0.3, 5, pts, rot, t0, step, nt, 6, dq, fstep, fnt)["candidates"]
     assert len(out["candidates"]) == len(want) > 1
-    for c, (h, s, q, tt, i, fsc, fq, ft) in zip(out["candidates"], want):
-        assert (c["hypothesis"], c["score"], c["fine_index"], c["fine_score"]) == (h, s, i, fsc)
-        assert np.array_equal(c["q"], q) and np.array_equal(c["t"], tt) and np.array_equal(c["fine_q"], fq) and np.array_equal(c["fine_t"], ft)
+    for c, w in zip(out["candidates"], want):
+        assert (c["hypothesis"], c["score"], c["fine_index"], c["fine_score"]) == (w["hypothesis"], w["score"], w["fine_index"], w["fine_score"])
+        assert all(np.array_equal(c[k], w[k]) for k in ("q", "t", "fine_q", "fine_t"))
     # the refined items: one ll_register_batch from the same seeds on another context
     state0 = capi.default_reg_state()
     state0.current_frame_index = state0.mapping_init_accumulate_frames + 1

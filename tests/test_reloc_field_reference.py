@@ -92,6 +92,54 @@ def test_field_scores_equal_a_plain_loop_for_coarse_fine_and_verify_groups(T):
         assert x.dtype == np.int32 and np.array_equal(x, y) and x.max() > 0
 
 
+@pytest.mark.parametrize("chunk", [1, 3, None])
+def test_vectorised_field_scores_equal_the_per_hypothesis_scores_and_the_loop(chunk):
+    from test_reloc_reference import vec_case
+    cloud, pts, rot = vec_case(23)
+    surf = np.concatenate([cloud[200:], np.float32([[0.25, 0.5, -0.75, 0]])])
+    dims, lo, d2 = F.field([cloud[:200], surf], 0.5, 3)
+    sp = [pts[:30], pts[30:]]
+    sp[1][0, :3] = (0.25, 0.5, -0.75)   # on the surface class's own voxel face
+    for t0, step, nt in (((-1.0, -0.5, 0.0), (0.5, 0.5, 0.5), (5, 3, 2)), ((0.3, 0.2, -0.1), (0.0, 0.0, 0.0), (3, 2, 2)),
+                         ((2.0, 1.0, 0.5), (-0.35, -0.5, -0.25), (7, 4, 3))):
+        a = F.field_scores_vec(d2, dims, lo, 0.5, 3, sp, rot, t0, step, nt, chunk=chunk)
+        b = F.field_scores(d2, dims, lo, 0.5, 3, sp, rot, t0, step, nt)
+        assert a.dtype == np.int32 and np.array_equal(a, b) and a.max() > 0
+        if chunk == 1:
+            assert np.array_equal(a, F.field_scores_loop(d2, dims, lo, 0.5, 3, sp, rot, t0, step, nt))
+    # a class without points next to one with points, and no finite point at all
+    none = np.zeros((0, 4), np.float32)
+    for p in ([none, sp[1]], [sp[0], none], [none, none], [pts[12:15], pts[12:15]]):
+        assert np.array_equal(F.field_scores_vec(d2, dims, lo, 0.5, 3, p, rot, (0, 0, 0), (0.5, 0.5, 0.5), (3, 2, 1)),
+                              F.field_scores(d2, dims, lo, 0.5, 3, p, rot, (0, 0, 0), (0.5, 0.5, 0.5), (3, 2, 1)))
+
+
+def test_one_call_pipeline_is_coarse_peaks_fine_groups_and_picks():
+    from test_reloc_reference import vec_case
+    cloud, pts, rot = vec_case(29)
+    dims, lo, d2 = F.field([cloud[:40], cloud[40:100]], 0.5, 1)
+    sp = [pts[:20], pts[20:]]
+    t0, step, nt = (-2.5, -2.0, 0.0), (0.6, 0.6, 0.5), (9, 9, 1)
+    a = np.radians([-4.0, 0.0, 4.0]) * 0.5
+    dq = np.stack([np.cos(a), 0 * a, 0 * a, np.sin(a)], axis=1)
+    fstep, fnt = (0.1, 0.2, 0.1), (5, 3, 1)
+    out = F.relocalize_field(d2, dims, lo, 0.5, 1, sp, rot, t0, step, nt, 5, dq, fstep, fnt)
+    sc = F.field_scores(d2, dims, lo, 0.5, 1, sp, rot, t0, step, nt)
+    hs, ss = R.peaks_brute(sc, 3, nt, True)
+    assert np.array_equal(out["scores"], sc) and out["n_peaks"] == hs.shape[0] > 5 and len(out["candidates"]) == 5
+    for j, c in enumerate(out["candidates"]):
+        assert (c["hypothesis"], c["score"]) == (hs[j], ss[j])
+        q, t = R.candidate_pose(hs[j], rot, t0, step, nt)
+        rf, o = F.fine_group(q, t, dq, fstep, fnt)
+        fs = F.field_scores(d2, dims, lo, 0.5, 1, sp, rf, o, fstep, fnt)
+        i = max(range(fs.shape[0]), key=lambda k: (fs[k], -k))
+        fq, ft = F.fine_pose(rf, o, fstep, fnt, i)
+        assert np.array_equal(out["fine"][j], fs) and (c["fine_index"], c["fine_score"]) == (i, fs[i])
+        assert np.array_equal(c["q"], q) and np.array_equal(c["t"], t) and np.array_equal(c["fine_q"], fq) and np.array_equal(c["fine_t"], ft)
+    v = F.verify_scores(d2, dims, lo, 0.5, 1, sp, [(c["fine_q"], c["fine_t"]) for c in out["candidates"]])
+    assert v == [c["fine_score"] for c in out["candidates"]]   # the verify score of a fine pose is its fine score
+
+
 def test_field_score_is_class_aware():
     T = 3
     corner = np.array([[0.0, 0.0, 0.0, 0]], np.float32)

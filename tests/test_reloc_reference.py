@@ -63,6 +63,61 @@ def test_scores_equal_a_plain_loop():
     assert np.array_equal(a, b) and a.max() > a.min()
 
 
+def vec_case(seed):
+    """A small grid anchored at (-3, -2, -1.5) (res 0.5: voxel faces at exact multiples) and score points with non-finite ones, points on voxel
+    faces and at negative coordinates; rotations with the identity, a 180 deg yaw (w = 0 exactly) and a tilted one."""
+    rng = np.random.default_rng(seed)
+    cloud = rng.uniform(-3, 3, (400, 4)).astype(np.float32)
+    cloud[0, :3] = (-3.0, -2.0, -1.5)
+    cloud[1, :3] = (3.0, 2.5, 1.5)
+    pts = rng.uniform(-2.5, 2.5, (60, 4)).astype(np.float32)
+    pts[:12, :3] = rng.integers(-8, 8, (12, 3)) * 0.25   # on voxel faces (and on them again after the lattice's steps of 0.5)
+    pts[12, :3] = np.nan
+    pts[13, 1] = np.inf
+    pts[14, 2] = -np.inf
+    pts[15, :3] = 0.0
+    tilt = np.array([0.995, 0.05, -0.08, 0.02]); tilt /= np.linalg.norm(tilt)
+    rot = np.array([[1.0, 0, 0, 0], [0.0, 0, 0, 1.0], tilt])
+    return cloud, pts, rot
+
+
+@pytest.mark.parametrize("t0,step,nt", [((-1.0, -0.5, 0.0), (0.5, 0.5, 0.5), (5, 3, 2)),     # steps landing every face on a face again
+                                        ((0.3, 0.2, -0.1), (0.0, 0.0, 0.0), (3, 2, 2)),     # step 0: identical translations
+                                        ((2.0, 1.0, 0.5), (-0.35, -0.5, -0.25), (7, 4, 3)),  # negative steps, points leaving the grid
+                                        ((0.0, 0.0, 0.0), (1.0, 1.0, 1.0), (1, 1, 1))])
+@pytest.mark.parametrize("chunk", [1, 2, 7, None])
+def test_vectorised_scores_equal_the_per_hypothesis_scores_and_the_loop(t0, step, nt, chunk):
+    cloud, pts, rot = vec_case(17)
+    dims, lo, g, _ = R.index([cloud], 0.5, 1)
+    a = R.scores_vec(g, dims, lo, 0.5, 1, pts, rot, t0, step, nt, chunk=chunk)
+    b = R.scores(g, dims, lo, 0.5, 1, pts, rot, t0, step, nt)
+    assert a.dtype == np.int32 and np.array_equal(a, b) and a.max() > 0
+    if chunk == 1:
+        assert np.array_equal(a, R.scores_loop(g, dims, lo, 0.5, 1, pts, rot, t0, step, nt))
+
+
+def test_vectorised_scores_of_no_point_and_of_non_finite_points_only():
+    cloud, pts, rot = vec_case(3)
+    dims, lo, g, _ = R.index([cloud], 0.5, 0)
+    for p in (pts[:0], pts[12:15]):
+        assert np.array_equal(R.scores_vec(g, dims, lo, 0.5, 0, p, rot, (0, 0, 0), (0.5, 0.5, 0.5), (3, 2, 1)), np.zeros(18, np.int32))
+
+
+def test_one_call_pipeline_is_scores_peaks_and_the_first_k():
+    cloud, pts, rot = vec_case(5)
+    dims, lo, g, _ = R.index([cloud[:150]], 0.5, 0)
+    t0, step, nt = (-2.5, -2.0, 0.0), (0.6, 0.6, 0.5), (9, 9, 1)
+    for K, cyclic in ((4, True), (16, False)):
+        out = R.relocalize(g, dims, lo, 0.5, 0, pts, rot, t0, step, nt, K, cyclic=cyclic)
+        sc = R.scores(g, dims, lo, 0.5, 0, pts, rot, t0, step, nt)
+        hs, ss = R.peaks_brute(sc, 3, nt, cyclic)
+        assert np.array_equal(out["scores"], sc) and out["n_peaks"] == hs.shape[0] > 4
+        assert [(c["hypothesis"], c["score"]) for c in out["candidates"]] == list(zip(hs[:K].tolist(), ss[:K].tolist()))
+        for c in out["candidates"]:
+            q, t = R.candidate_pose(c["hypothesis"], rot, t0, step, nt)
+            assert np.array_equal(c["q"], q) and np.array_equal(c["t"], t)
+
+
 @pytest.mark.parametrize("n_rot", [1, 2, 3, 5])
 @pytest.mark.parametrize("cyclic", [False, True])
 def test_peaks_equal_a_brute_force_neighbourhood(n_rot, cyclic):
