@@ -23,6 +23,7 @@ static int ctx_alloc(ll_ctx* ctx) {
     A.k10_n_distinct = c.take<int>(1); A.counts = c.take<int>(16); A.bounds = c.take<float>(32);
     A.knn_idx = c.take<int>(cap * LL_KNN); A.knn_d = c.take<float>(cap * LL_KNN); A.perm = c.take<int>(cap);
     A.tmp_a = c.take<float4>(scap); A.tmp_b = c.take<float4>(scap); A.tmp_c = c.take<float4>(scap); A.tmp_d = c.take<float4>(scap);
+    A.dev_counts = c.take<int>(2);
   }));
   LL_TRY(extract_alloc(ctx));
   // the front end: extraction + get_features + the surface VoxelGrids on fe_main, the corner VoxelGrids on fe_corner, the petals on fe_petals
@@ -402,6 +403,7 @@ static KnnBlocksArgs knn_args(ll_ctx* ctx, const ll_map* map, const RegBatch& b,
   ctx->solve_world = (map->world > 1 && ctx->world > 1) ? ctx->world : 1;   // replicas of the whole map never exchange anything
   a.st = ctx->d_reg; a.deblur = b.in[0]->if_motion_deblur ? 1 : 0; ctx->reg_deblur = a.deblur;   // (the items of a batch agree on it)
   a.rank = map->rank; a.world = map->world; a.grid = map->grid; a.shard_owner = (const int*)map->shard_owner.p;
+  a.dev_counts = nullptr;
   return a;
 }
 static RegBatch single_batch(int nc, int ns, const ll_reg_state* in) {
@@ -414,7 +416,7 @@ static SolveArgs solve_args(ll_ctx* ctx, int M, SolveMode mode, int max_iter) {
   SolveArgs s; s.st = ctx->d_reg; s.sync = ctx->d_sync; s.feat = A.feat; s.blk_a = A.blk_a; s.blk_v = A.blk_v; s.l1 = A.l1; s.k10_value = A.k10_value; s.k10_n_distinct = A.k10_n_distinct;
   s.mode = mode; s.rank = ctx->rank; s.world = ctx->solve_world; s.comm_local = (double*)ctx->comm_local;
   for (int i = 0; i < 8; i++) s.comm_peer[i] = (double*)ctx->comm_peers[i];
-  s.deblur = ctx->reg_deblur; s.n_items = 1;
+  s.deblur = ctx->reg_deblur; s.n_items = 1; s.dev_counts = nullptr; s.snap = nullptr;
   SolveItem& I = s.item[0];
   I.off = 0; I.M = M; I.max_iterations = max_iter; I.prerun_iterations = 0; I.cap_check = 0; I.table = nullptr; I.table_mask = 0;
   return s;
@@ -422,6 +424,10 @@ static SolveArgs solve_args(ll_ctx* ctx, int M, SolveMode mode, int max_iter) {
 
 }  // extern "C"
 
+// The gate (:199): CORNER_MIN_MAP_NUM 0, SURFACE_MIN_MAP_NUM 50.
+static bool reg_gate(const ll_map* map, const ll_reg_state* in) {
+  return map->corner.n_src > 0 && map->surf.n_src > 50 && in->current_frame_index > in->mapping_init_accumulate_frames;
+}
 // What an item returns before any device work: the result initialised from its state, the gate (:199) and the empty item.  Returns 1 when the
 // item goes on to the device; else *status is its outcome (LL_OK with registered = 0 under the gate, LL_ERR_NO_BLOCKS without features).
 static int item_prologue(ll_ctx* ctx, const ll_map* map, int M, const ll_reg_state* in, ll_reg_result* out, int* status) {
@@ -430,26 +436,35 @@ static int item_prologue(ll_ctx* ctx, const ll_map* map, int M, const ll_reg_sta
   for (int k = 0; k < 4; k++) { out->q_w_curr[k] = in->q_w_curr[k]; out->q_w_incre[k] = k == 0 ? in->para_buffer_incremental[3] : in->para_buffer_incremental[k - 1]; }
   for (int k = 0; k < 3; k++) { out->t_w_curr[k] = in->t_w_curr[k]; out->t_w_incre[k] = in->para_buffer_incremental[4 + k]; }
   *status = LL_OK;
-  // gate (:199): CORNER_MIN_MAP_NUM 0, SURFACE_MIN_MAP_NUM 50
-  if (!(map->corner.n_src > 0 && map->surf.n_src > 50 && in->current_frame_index > in->mapping_init_accumulate_frames)) return 0;
+  if (!reg_gate(map, in)) return 0;
   if (M == 0) { ctx->set_error("no features"); *status = LL_ERR_NO_BLOCKS; return 0; }
   return 1;
 }
 
+// ll_scan_to_pose's registration of the front end's features on the device counts (A.dev_counts), with no host read in between: the one item's
+// slot count in the RegBatch is the capacity, and the host learns the counts at its first wait in the ICP loop.  Then, from the front end's
+// counts in pinned memory: st = scan_front_end_finish's outcome for them (LL_OK or LL_ERR_CAPACITY), nc / ns, dropped; `stopped` when the
+// device counts were zero (dropped, over capacity, or no feature), so that nothing ran and the caller reports the outcome.
+struct DevHandoff { const ll_pipeline_cfg* pc; int st, nc, ns, dropped, stopped; };
+static int front_end_counts(ll_ctx* ctx, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);
+
 // The ICP loops of the batch's items on the device (every item has passed item_prologue and the capacity check): one kNN launch and one solver
-// launch per ICP iteration for all of them.  outs[j] / status[j] belong to item j.
-static int register_batch(ll_ctx* ctx, const ll_map* map, const RegBatch& b, ll_reg_result* const* outs, int* const* status) {
+// launch per ICP iteration for all of them.  outs[j] / status[j] belong to item j.  With `hand` (one item), the caller has uploaded the state.
+static int register_batch(ll_ctx* ctx, const ll_map* map, const RegBatch& b, ll_reg_result* const* outs, int* const* status, DevHandoff* hand = nullptr) {
   cudaStream_t s = ctx->stream;
   const RegArrays& A = ctx->A;
   RegEvents& ev = ctx->ev;
   const int n = b.n, Mtot = b.off[n];
-  ctx->last_nc = b.nc[0]; ctx->last_ns = b.ns[0];
-  RegDevState* h = ctx->pin->state_in;
-  for (int j = 0; j < n; j++) fill_state(&h[j], b.in[j]);
-  LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, n * sizeof(RegDevState), cudaMemcpyHostToDevice, s));
+  if (!hand) {
+    ctx->last_nc = b.nc[0]; ctx->last_ns = b.ns[0];
+    RegDevState* h = ctx->pin->state_in;
+    for (int j = 0; j < n; j++) fill_state(&h[j], b.in[j]);
+    LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, n * sizeof(RegDevState), cudaMemcpyHostToDevice, s));
+  }
   LL_CUDA(ctx, cudaEventRecord(ev.total[0], s));
   for (int j = 0; j < n; j++) outs[j]->registered = 1;
   KnnBlocksArgs ka = knn_args(ctx, map, b, false);
+  if (hand) ka.dev_counts = A.dev_counts;
   LL_CUDA(ctx, cudaMemsetAsync(A.knn_idx, 0xff, (size_t)Mtot * LL_KNN * 4, s));   // no seeds for the first ICP iteration
   LL_CUDA(ctx, cudaEventRecord(ev.sort[0], s));
   LL_TRY(launch_query_sort(ctx, s, ctx->scratch, ka, A.perm));   // spatial tiles of features (Hilbert order at the initial poses)
@@ -469,13 +484,13 @@ static int register_batch(ll_ctx* ctx, const ll_map* map, const RegBatch& b, ll_
   double* x_l1 = sharded ? (double*)((char*)ctx->comm_local + LL_COMM_X_OFF) : nullptr;
   unsigned long long* set_table[LL_MAX_BATCH];   // hash set of each item's L1 norms (K10)
   LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { for (int j = 0; j < n; j++) set_table[j] = l1_set_layout(c, b.nc[j] + b.ns[j]); }));
-  // One ICP iteration's device work + a snapshot of the n 1.7 KB states into pinned slot `it & 1`.
+  // One ICP iteration's device work + a snapshot of the n 1.7 KB states into pinned slot `it & 1` (written by the fused solver launch).
   RegDevState (*slots)[LL_MAX_BATCH] = ctx->pin->snap;
   auto enqueue_iteration = [&](int it) -> int {
     cudaEvent_t* e = it < LL_TIMED_ITERS ? ev.phase[it] : nullptr;
-    // corner_avail, surf_avail, n_blocks of every item (one item: the plain memset, cheaper to enqueue than the strided one)
-    if (n == 1) LL_CUDA(ctx, cudaMemsetAsync(&ctx->d_reg->corner_avail, 0, 3 * sizeof(int), s));
-    else LL_CUDA(ctx, cudaMemset2DAsync(&ctx->d_reg->corner_avail, sizeof(RegDevState), 0, 3 * sizeof(int), n, s));
+    // corner_avail, surf_avail, n_blocks of every item: zero in the uploaded state, and cleared by the fused solver launch of every iteration
+    // (SolveArgs::snap); the sharded mode clears them here
+    if (sharded) LL_CUDA(ctx, cudaMemsetAsync(&ctx->d_reg->corner_avail, 0, 3 * sizeof(int), s));
     if (sharded) LL_CUDA(ctx, cudaMemsetAsync(x_l1, 0xff, (size_t)M * sizeof(double), s));   // NaN = nobody owns a block here (peers fill it after solve #1)
     if (it == 0) LL_CUDA(ctx, cudaEventRecord(ev.knn_first[0], s));
     if (e) LL_CUDA(ctx, cudaEventRecord(e[0], s));
@@ -485,7 +500,7 @@ static int register_batch(ll_ctx* ctx, const ll_map* map, const RegBatch& b, ll_
     if (!sharded) {
       // one launch: per item, solve #1 -> L1 norms -> de-duplication + order statistic -> outlier drop -> solve #2 -> pose
       SolveArgs sa = solve_args(ctx, M, SOLVE_FUSED, 0);
-      sa.n_items = n;
+      sa.n_items = n; sa.dev_counts = ka.dev_counts; sa.snap = slots[it & 1];
       for (int j = 0; j < n; j++) {
         SolveItem& I = sa.item[j]; const int Mj = b.nc[j] + b.ns[j];
         I.off = b.off[j]; I.M = Mj; I.max_iterations = b.in[j]->cere_max_iterations; I.prerun_iterations = b.in[j]->cere_prerun_times;
@@ -503,7 +518,7 @@ static int register_batch(ll_ctx* ctx, const ll_map* map, const RegBatch& b, ll_
       { SolveArgs sa = solve_args(ctx, M, SOLVE_SECOND, in->cere_max_iterations); sa.item[0].cap_check = cap_check; LL_TRY(launch_solve(ctx, sa)); }
     }
     if (e) LL_CUDA(ctx, cudaEventRecord(e[4], s));
-    LL_CUDA(ctx, cudaMemcpyAsync(slots[it & 1], ctx->d_reg, n * sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
+    if (sharded) LL_CUDA(ctx, cudaMemcpyAsync(slots[it & 1], ctx->d_reg, n * sizeof(RegDevState), cudaMemcpyDeviceToHost, s));
     LL_CUDA(ctx, cudaEventRecord(ctx->sev.it[it & 1], s));
     return LL_OK;
   };
@@ -518,6 +533,12 @@ static int register_batch(ll_ctx* ctx, const ll_map* map, const RegBatch& b, ll_
   for (iter = 0; iter < max_iters; iter++) {
     if (speculate && iter + 1 < max_iters) LL_TRY(enqueue_iteration(iter + 1));
     LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.it[iter & 1]));
+    if (hand && iter == 0) {   // the front end has completed: its counts are in pinned memory
+      hand->st = front_end_counts(ctx, hand->pc, &hand->nc, &hand->ns, &hand->dropped);
+      hand->stopped = hand->st != LL_OK || hand->dropped || hand->nc + hand->ns == 0;
+      if (hand->stopped) break;
+      ctx->last_nc = hand->nc; ctx->last_ns = hand->ns;
+    }
     for (int j = 0; j < n; j++) {
       if (done[j]) continue;
       const RegDevState* hs = &slots[iter & 1][j];
@@ -533,6 +554,7 @@ static int register_batch(ll_ctx* ctx, const ll_map* map, const RegBatch& b, ll_
   // (an iteration enqueued ahead returns at once; it is drained here, before the arena is reused)
   LL_CUDA(ctx, cudaEventRecord(ev.total[1], s));
   LL_CUDA(ctx, cudaEventSynchronize(ev.total[1]));
+  if (hand && hand->stopped) return LL_OK;
   ll_reg_result t; memset(&t, 0, sizeof(t));   // the batch's timings, given to every item
   cudaEventElapsedTime(&t.gpu_ms_total, ev.total[0], ev.total[1]); cudaEventElapsedTime(&t.gpu_ms_knn, ev.knn_first[0], ev.knn_first[1]);
   cudaEventElapsedTime(&t.gpu_ms_sort, ev.sort[0], ev.sort[1]);
@@ -907,8 +929,9 @@ int scan_front_end_enqueue(ll_ctx* ctx, const FrontStreams& fs, const void* raw,
   return front_graph(ctx, ctx->fg, fs.main, key, n >= 5, [&] { return front_end_enqueue(ctx, fs, pc, (int)n); });
 }
 
-int scan_front_end_finish(ll_ctx* ctx, cudaStream_t s, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped) {
-  const RegArrays& A = ctx->A;
+// The front end's outcome from its counts in pinned memory, once it has completed: the time-stamp range, the feature counts, the drop rule
+// (<= 5 petals, :287) and max_features.
+static int front_end_counts(ll_ctx* ctx, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped) {
   const int* h = ctx->pin->fe_counts;
   const int nc = h[5], ns = h[7], meta_scans = ctx->pin->fe_meta[1];
   ctx->last_full_min_t = ll_ord2f(h[10]); ctx->last_full_max_t = ll_ord2f(h[11]);
@@ -916,6 +939,14 @@ int scan_front_end_finish(ll_ctx* ctx, cudaStream_t s, const ll_pipeline_cfg* pc
   *dropped = (meta_scans <= 5 && !pc->whole_frame) ? 1 : 0;
   if (*dropped) return LL_OK;
   if (nc + ns > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
+  return LL_OK;
+}
+
+int scan_front_end_finish(ll_ctx* ctx, cudaStream_t s, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped) {
+  const RegArrays& A = ctx->A;
+  LL_TRY(front_end_counts(ctx, pc, nc_out, ns_out, dropped));
+  if (*dropped) return LL_OK;
+  const int nc = *nc_out, ns = *ns_out;
   LL_CUDA(ctx, cudaMemcpyAsync(A.feat, A.tmp_a, (size_t)nc * 16, cudaMemcpyDeviceToDevice, s));
   LL_CUDA(ctx, cudaMemcpyAsync(A.feat + nc, A.tmp_b, (size_t)ns * 16, cudaMemcpyDeviceToDevice, s));
   return LL_OK;
@@ -927,11 +958,63 @@ int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, d
   return scan_front_end_finish(ctx, ctx->stream, pc, nc_out, ns_out, dropped);
 }
 
+// The front end's features into A.feat on the device: corners (counts[5], from tmp_a) then surfaces (counts[7], from tmp_b), and the counts
+// the registration reads, dc = {corners, surfaces}.  dc = {0, 0} and nothing is copied when the frame is dropped (meta[1] <= 5 petals and not
+// whole_frame, :287) or has more features than max_features: scan_front_end_finish's rules.
+__global__ void feature_handoff_kernel(const int* __restrict__ counts, const int* __restrict__ meta, int whole_frame, int max_features, const float4* __restrict__ corner,
+                                       const float4* __restrict__ surf, float4* __restrict__ feat, int* __restrict__ dc) {
+  const int nc = counts[5], ns = counts[7];
+  const bool keep = !(meta[1] <= 5 && !whole_frame) && nc + ns <= max_features;
+  if (blockIdx.x == 0 && threadIdx.x == 0) { dc[0] = keep ? nc : 0; dc[1] = keep ? ns : 0; }
+  if (!keep) return;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nc + ns; i += gridDim.x * blockDim.x) feat[i] = i < nc ? corner[i] : surf[i - nc];
+}
+
+// ll_scan_to_pose without a host read between the front end and the registration: the state goes up before the front end, the features move
+// into A.feat and the spatial sort and the first two ICP iterations are enqueued behind the front end at once, all sized for max_features and
+// reading the counts on the device; the host reads the counts at its first wait in the ICP loop.  The outcomes and the results are those of
+// the host-sized path (scan_front_end + register_device), which is taken instead when the capacity does not bound the feature count
+// (max_features < max_scan_points), when the solver's shared memory cannot hold max_features slots, for a sharded map or context, under
+// the gate (:199), where no registration runs, and with no ICP iteration to read the counts at.
+static bool device_handoff(ll_ctx* ctx, const ll_map* map, const ll_reg_state* in) {
+  if (ctx->cfg.max_features < ctx->cfg.max_scan_points || ctx->world > 1 || map->world > 1 || !reg_gate(map, in) || in->icp_max_iterations < 1) return false;
+  const std::string err = ctx->err;
+  if (solve_capacity(ctx, 1, &ctx->cfg.max_features, in->if_motion_deblur ? 1 : 0) != LL_OK) { ctx->err = err; return false; }
+  return true;
+}
+static int scan_to_pose_device(ll_ctx* ctx, const ll_map* map, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc,
+                               const ll_reg_state* in, ll_reg_result* out, int* nc, int* ns, int* dropped) {
+  cudaStream_t s = ctx->stream;
+  const RegArrays& A = ctx->A;
+  const int cap = ctx->cfg.max_features;
+  RegDevState* h = ctx->pin->state_in; fill_state(h, in);
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, sizeof(RegDevState), cudaMemcpyHostToDevice, s));
+  LL_TRY(scan_front_end_enqueue(ctx, ctx->own_front(), raw, n, fmt, where, stamp, pc));
+  feature_handoff_kernel<<<ctx->num_sms * 2, 256, 0, s>>>(A.counts, ctx->ex.d_meta, pc->whole_frame, cap, A.tmp_a, A.tmp_b, A.feat, A.dev_counts); ctx->launches++;
+  LL_CUDA(ctx, cudaGetLastError());
+  int st = LL_OK;
+  item_prologue(ctx, map, cap, in, out, &st);   // (the gate has passed and cap > 0: the result initialised from the state)
+  DevHandoff hand = {pc, LL_OK, 0, 0, 0, 0};
+  int* stp = &st;
+  LL_TRY(register_batch(ctx, map, single_batch(cap, 0, in), &out, &stp, &hand));
+  *nc = hand.nc; *ns = hand.ns; *dropped = hand.dropped;
+  if (hand.st != LL_OK || hand.dropped) return hand.st;
+  if (hand.nc + hand.ns == 0) { item_prologue(ctx, map, 0, in, out, &st); ctx->last_nc = 0; ctx->last_ns = 0; }   // as register_device reports it
+  return st;
+}
+
 extern "C" int ll_scan_to_pose(ll_ctx* ctx, const ll_map* map, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc, const ll_reg_state* in,
                     ll_reg_result* out, int* n_corner_used, int* n_surf_used) {
   if (!ctx || !map || !pc || !in || !out) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
   int nc = 0, ns = 0, dropped = 0;
+  if (device_handoff(ctx, map, in)) {
+    const int st = scan_to_pose_device(ctx, map, raw, n, fmt, where, stamp, pc, in, out, &nc, &ns, &dropped);
+    if (st != LL_OK && !(st == LL_ERR_NO_BLOCKS && !dropped)) return st;
+    if (n_corner_used) *n_corner_used = nc; if (n_surf_used) *n_surf_used = ns;
+    if (dropped) { memset(out, 0, sizeof(*out)); out->status = 1; ctx->set_error("frame dropped: <= 5 petals"); return LL_OK; }
+    return st;
+  }
   LL_TRY(scan_front_end(ctx, raw, n, fmt, where, stamp, pc, &nc, &ns, &dropped));
   if (n_corner_used) *n_corner_used = nc; if (n_surf_used) *n_surf_used = ns;
   if (dropped) { memset(out, 0, sizeof(*out)); out->status = 1; ctx->set_error("frame dropped: <= 5 petals"); return LL_OK; }

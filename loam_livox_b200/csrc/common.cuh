@@ -140,6 +140,7 @@ struct ExtractState {
 struct RegArrays {
   float4* feat; float4* blk_a; double* blk_v; double* l1; double* k10_value;
   int* k10_n_distinct; int* knn_idx; float* knn_d; int* perm; float4* tmp_a; float4* tmp_b; float4* tmp_c; float4* tmp_d; int* counts; float* bounds;
+  int* dev_counts;      // ll_scan_to_pose: {corners, surfaces} of the front end as the registration reads them (KnnBlocksArgs::dev_counts)
 };
 
 // Solver / registration device state shared between kernels (lives in global memory)

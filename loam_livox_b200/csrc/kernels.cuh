@@ -40,6 +40,9 @@ struct KnnBlocksArgs {
   RegDevState* st;              // [n_items]: the pose, the deblur terms, icp_done, and the counters corner_avail / surf_avail / n_blocks
                                 // (cleared before every launch)
   int deblur;
+  // One item whose counts only the device knows (ll_scan_to_pose): {n_corner, n_surf} of item 0, the front end's counts; M and item 0's
+  // counts above are then the capacity the launches are sized for.  Null: the counts above are the item's.
+  const int* dev_counts;
 };
 int launch_knn_query(ll_ctx* ctx, const BucketTree& t, const float4* d_q, int nq, int* d_idx, float* d_d);
 int launch_knn_blocks(ll_ctx* ctx, const KnnBlocksArgs& a);
@@ -95,7 +98,8 @@ struct FrameDev {
 // snap[it & 1] only after the event recorded behind its copy).
 struct PinnedStage {
   RegDevState state_in[LL_MAX_BATCH];   // the registration states uploaded by register_batch / ll_build_blocks / ll_set_blocks (item order)
-  RegDevState snap[2][LL_MAX_BATCH];    // state read-backs: ICP iteration `it` of every item into snap[it & 1]; the solver parity hooks use snap[0][0]
+  RegDevState snap[2][LL_MAX_BATCH];    // state read-backs: ICP iteration `it` of every item into snap[it & 1], written by the fused solver launch itself
+                                        // (SolveArgs::snap; copied in the sharded mode); the solver parity hooks use snap[0][0]
   double x[7];            // x of the solver parity hooks
   double pose[7];         // ll_transform / ll_transform_dev
   double mapper_pose[7];  // the mapper's world-frame transform of the new features
@@ -156,6 +160,13 @@ struct SolveArgs {
   int deblur;                // 1: *_mb functors (ceres_icp.hpp:81-233), s per block from the feature's time stamp
   int n_items;               // 1 ... LL_MAX_BATCH; more than one only in SOLVE_FUSED
   SolveItem item[LL_MAX_BATCH];
+  // SOLVE_FUSED of one item whose slot count only the device knows (KnnBlocksArgs::dev_counts): M = dev_counts[0] + dev_counts[1]; the launch
+  // is sized for item 0's M as a capacity, and the kernel derives the CTA split, cap_check and the hash set's mask from the device M.
+  const int* dev_counts;
+  // SOLVE_FUSED of an ICP loop (register_batch): pinned host memory [n_items] that each item's master CTA fills with the item's state at the end
+  // of the launch (the iteration's snapshot, without a copy of its own), then it clears the item's kNN counters corner_avail / surf_avail /
+  // n_blocks for the next iteration's kNN launch.  Null: neither.
+  RegDevState* snap;
 };
 // Layout of the IPC-exported staging buffer of a rank (ll_comm_local_handle):
 //   [0, 8192)            2 parities x 8 ranks x 64 doubles: the 29 sums of one evaluation + a generation flag at double index 32
@@ -175,7 +186,7 @@ int solve_prepare(ll_ctx* ctx);   // once per context: opt the solver kernels in
 // The sharded mode's select over the exchanged L1 norms, and the parity hook ll_inlier_select.
 int launch_k10_select(ll_ctx* ctx, const double* d_l1, int n, const double* d_ratio, unsigned long long* table, unsigned table_mask, double* d_value, int* d_n_distinct);
 // Slots of the hash set of M L1 norms (K10): a power of two >= 2 M.
-inline unsigned l1_set_capacity(int M) { unsigned cap = 1024; while (cap < (unsigned)(2 * M)) cap <<= 1; return cap; }
+__host__ __device__ inline unsigned l1_set_capacity(int M) { unsigned cap = 1024; while (cap < (unsigned)(2 * M)) cap <<= 1; return cap; }
 // The hash set's place at the start of a scratch arena.
 inline unsigned long long* l1_set_layout(Carve& c, int M) { return c.take<unsigned long long>(l1_set_capacity(M)); }
 // Sharded mode, K10: every rank pushes the loss-corrected L1 norms of the slots it owns into every peer's X buffer (NVLink stores), then a

@@ -354,11 +354,19 @@ static int item_key_bits(int n_items) { int b = 0; while ((1 << b) < n_items) b+
 
 // Spatial sort key of a feature at its item's current pose: item index | class bit (corner/surface) | 21-bit Hilbert index (7 bits per axis)
 // inside the tree's box.  Neighbouring queries then sit in the same warp / CTA, walk the same tree nodes and buckets, and hit them in L1.
+// With device counts (KnnBlocksArgs::dev_counts) the keys cover the capacity a.M and the slots past the device M get 0xffffffff: no real key
+// is above it in the bits the sort sees, the sort is stable and those slots come after every real one, so perm[0 .. M) is the one a sort of
+// the M real keys gives.
 __global__ void query_key_kernel(KnnBlocksArgs a, unsigned* __restrict__ keys, int* __restrict__ vals) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.M) return;
+  int n_corner0 = a.item[0].n_corner;
+  if (a.dev_counts) {
+    n_corner0 = a.dev_counts[0];
+    if (i >= n_corner0 + a.dev_counts[1]) { keys[i] = 0xffffffffu; vals[i] = i; return; }
+  }
   const int it = knn_item_of(a, i);
-  const bool is_corner = i - a.item[it].off < a.item[it].n_corner;
+  const bool is_corner = i - a.item[it].off < (it == 0 ? n_corner0 : a.item[it].n_corner);
   const double* pose = a.st[it].pose_curr;
   const float4 f = __ldg(&a.feat[i]);
   double wx, wy, wz; qrot_d(pose, (double)f.x, (double)f.y, (double)f.z, wx, wy, wz);
@@ -414,20 +422,22 @@ __device__ __forceinline__ void emit_block(const KnnBlocksArgs& a, const KnnItem
 // K6 + K7 fused, one warp per scan feature, features taken in spatially sorted order (perm), each against the pose of its batch item.
 // Writes one residual-block slot per feature (indexed by the ORIGINAL feature order): blk_a[slot] = (a.x, a.y, a.z, type) with
 // type 0 invalid / 1 line / 2 plane, blk_v[slot*3..] = unit line direction or (un-normalised) plane normal, in fp64.
+// DEV (dev_counts set): the launch covers the capacity a.M and the warps past the device M return at once.
 // (5 CTAs of 256 threads per SM: at most 48 registers.  The search is latency-bound; one register more is 56 with the allocation granularity,
 // 4 CTAs per SM, and the kernel ~9 % slower on an H100.)
+template <bool DEV>
 __global__ void __launch_bounds__(KNN_THREADS, 5) knn_blocks_kernel(KnnBlocksArgs a) {
   __shared__ WarpWalk walks[WARPS_PER_CTA];
   const int j = blockIdx.x * WARPS_PER_CTA + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  if (j >= a.M) return;
+  if (j >= (DEV ? a.dev_counts[0] + a.dev_counts[1] : a.M)) return;
   const int w = a.perm ? a.perm[j] : j;      // original feature index
   const int it = knn_item_of(a, w);
   const KnnItem& I = a.item[it];
   RegDevState* st = a.st + it;
   if (st->icp_done) return;   // (warp-uniform) launched ahead of the termination test by the host: this item's ICP loop has already ended
   const int lw = w - I.off;   // item-local feature index
-  const bool is_corner = lw < I.n_corner;
+  const bool is_corner = lw < (DEV ? __ldg(a.dev_counts) : I.n_corner);   // (DEV: one item; the counts are read where they are used)
   const TreeView& tv = is_corner ? a.corner : a.surf;
   const float4 f = __ldg(&a.feat[w]);
   // pointAssociateToMap (non-deblur branch): p_w = q_curr * p + t_curr in fp64, stored as fp32
@@ -457,8 +467,8 @@ __global__ void __launch_bounds__(KNN_THREADS, 5) knn_blocks_kernel(KnnBlocksArg
   // Residual-block cap, pre-skip (:232-238 corners, :339-345 surfaces): with N features of this class and N > 2 cap, a feature is skipped when
   // rand * N > 2 cap (float arithmetic, like m_rand_float), before it is transformed or searched.  Drawn per (seed, ICP iteration, class, index).
   bool skipped = false;
-  { const int ncls = is_corner ? I.n_corner : I.n_surf;
-    if (ncls > 2 * I.cap) skipped = ll_cap_uniform_f(I.rng_seed, st->icp_iter, is_corner ? 0 : 1, is_corner ? lw : lw - I.n_corner) * (float)ncls > (float)(2 * I.cap); }
+  { const int n_corner = DEV ? __ldg(a.dev_counts) : I.n_corner, ncls = is_corner ? n_corner : (DEV ? __ldg(a.dev_counts + 1) : I.n_surf);
+    if (ncls > 2 * I.cap) skipped = ll_cap_uniform_f(I.rng_seed, st->icp_iter, is_corner ? 0 : 1, is_corner ? lw : lw - n_corner) * (float)ncls > (float)(2 * I.cap); }
   const bool active = owned && finite_in && !skipped;
   LaneTop t;
   warp_knn5(tv, walks[threadIdx.x >> 5], active, qx, qy, qz, t, a.seed_ids ? a.seed_ids + (size_t)w * LL_KNN : nullptr);
@@ -500,7 +510,8 @@ int launch_query_sort(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const KnnBlo
 int launch_knn_blocks(ll_ctx* ctx, const KnnBlocksArgs& a) {
   const int M = a.M;
   if (M == 0) return LL_OK;
-  knn_blocks_kernel<<<ll_div_up(M, WARPS_PER_CTA), KNN_THREADS, 0, ctx->stream>>>(a);
+  if (a.dev_counts) knn_blocks_kernel<true><<<ll_div_up(M, WARPS_PER_CTA), KNN_THREADS, 0, ctx->stream>>>(a);
+  else knn_blocks_kernel<false><<<ll_div_up(M, WARPS_PER_CTA), KNN_THREADS, 0, ctx->stream>>>(a);
   ctx->launches++;
   LL_CUDA(ctx, cudaGetLastError());
   return LL_OK;

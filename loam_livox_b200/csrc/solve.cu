@@ -364,6 +364,21 @@ __device__ __forceinline__ void k10_select(K10Smem& s_k10, SolveSync* Y, K10Area
   }
 }
 
+// How M slots are spread over `ncta` persistent CTAs: CTA b owns the tiles b, b + grid, b + 2 grid, ... of `tile` slots each.  The host
+// sizes its launches with it; a launch of device counts (SolveArgs::dev_counts) computes the same split on the device.
+struct SolveGrid { int tile, tiles_per_cta, grid; };
+__host__ __device__ inline SolveGrid solve_grid(int ncta, int M) {
+  // The evaluation is fp64-throughput bound (64 DFMA/clk/SM): spread the slots over ALL the CTAs, even when that leaves CTAs partly empty.
+  // tile = slots per CTA and pass (a multiple of 32, <= SOLVE_THREADS); partly empty CTAs on every SM evaluate faster than fewer full ones.
+  const int M1 = M > 0 ? M : 1;
+  SolveGrid g;
+  g.tile = (((M1 + ncta - 1) / ncta + 31) / 32) * 32; if (g.tile > SOLVE_THREADS) g.tile = SOLVE_THREADS;
+  const int tiles = (M1 + g.tile - 1) / g.tile;
+  g.grid = tiles < ncta ? tiles : ncta;
+  g.tiles_per_cta = (tiles + g.grid - 1) / g.grid;
+  return g;
+}
+
 // BATCH: the launch has several items (CTA groups).  A launch of one item is the instance without: its group is the whole grid, its slots start
 // at 0 and its fields are plain kernel parameters, as in a launch that knows nothing of batches.
 template <bool MB, bool BATCH>
@@ -382,11 +397,20 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a)
   int item = 0;
   if (BATCH) while (item + 1 < a.n_items && (int)blockIdx.x >= a.item[item + 1].first) item++;
   const SolveItem& I = a.item[item];
-  const CtaGroup grp = {BATCH ? I.first : 0, BATCH ? I.n_cta : (int)gridDim.x};
-  const int cta = BATCH ? (int)blockIdx.x - grp.first : (int)blockIdx.x, tiles_per_cta = I.tiles_per_cta, tile = I.tile, M = I.M;
+  RegDevState* st = a.st + item;
+  int M = I.M, tile = I.tile, tiles_per_cta = I.tiles_per_cta, n_cta = BATCH ? I.n_cta : (int)gridDim.x, cap_check = I.cap_check;
+  unsigned table_mask = I.table_mask;
+  if (!BATCH && a.dev_counts) {   // the host's split of the device M over the launched grid, and the host's rules for cap_check and the hash set
+    M = a.dev_counts[0] + a.dev_counts[1];
+    const SolveGrid g = solve_grid((int)gridDim.x, M);
+    if (M == 0 || (int)blockIdx.x >= g.grid) return;   // no feature (the host reports it) / past the CTAs the split uses: before any exchange
+    tile = g.tile; tiles_per_cta = g.tiles_per_cta; n_cta = g.grid;
+    cap_check = M > st->cap ? 1 : 0; table_mask = l1_set_capacity(M) - 1;
+  }
+  const CtaGroup grp = {BATCH ? I.first : 0, n_cta};
+  const int cta = BATCH ? (int)blockIdx.x - grp.first : (int)blockIdx.x;
   const int off = BATCH ? I.off : 0;
   const float4* feat = a.feat + off; const float4* blk_a = a.blk_a + off; const double* blk_v = a.blk_v + (size_t)off * 3; double* l1 = a.l1 + off;
-  RegDevState* st = a.st + item;
   SolveSync* Y = a.sync;
   K10Area* K = &Y->k10[item];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -408,7 +432,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a)
   // exchange orders the clear before any insert.
   const bool fused = a.mode == SOLVE_FUSED;
   SolveMode cur_mode = fused ? SOLVE_FIRST : a.mode;
-  if (fused) k10_clear(I.table, I.table_mask, K, grp);
+  if (fused) k10_clear(I.table, table_mask, K, grp);
   // ---- stage this CTA's residual blocks
   double thr = 0;
   if (a.mode == SOLVE_SECOND) {   // K10 tail: the threshold from the order statistic and distinct count launch_k10_select left on the device
@@ -417,7 +441,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a)
   }
   // Residual-block cap, drop rule (:434-458): with M blocks and M > cap, block i leaves the problem when rand_i > (float)cap / (float)M.
   float cap_keep = 2.0f; int cap_iter = 0, cap_seed = 0;
-  if (I.cap_check) {
+  if (cap_check) {
     const int nb = a.world > 1 ? st->n_blocks_all : st->n_blocks;
     if (nb > st->cap) cap_keep = (float)st->cap / (float)nb;
     cap_iter = st->icp_iter; cap_seed = st->rng_seed;
@@ -672,7 +696,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a)
         my_l1 = l1v;
       }
       // std::set de-duplication: the thread whose insert created the entry represents the value from here on (bit 8 of its slot's type)
-      if (fused && l1_set_insert_flag(I.table, I.table_mask, my_l1, my_l1 < INFINITY)) S.type[li] |= 0x100;
+      if (fused && l1_set_insert_flag(I.table, table_mask, my_l1, my_l1 < INFINITY)) S.type[li] |= 0x100;
     }
   }
   if (fused && ph == 0) {
@@ -693,6 +717,14 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) lm_solve_kernel(SolveArgs a)
   if (master && tid == 0) s_prof[7] += clock64() - t_p0;
   }   // phase
   if (master && tid == 0) for (int k = 0; k < 16; k++) st->prof[k] += s_prof[k];
+  if (a.snap && master) {   // the snapshot straight into pinned host memory (visible to the host once the launch has completed), then the counters
+    __syncthreads();
+    const long long* src = (const long long*)st; long long* dst = (long long*)(a.snap + item);
+    static_assert(sizeof(RegDevState) % 8 == 0, "the state is copied in 8-byte words");
+    for (int k = tid; k < (int)(sizeof(RegDevState) / 8); k += SOLVE_THREADS) dst[k] = __ldcg(src + k);
+    __syncthreads();
+    if (tid == 0) { st->corner_avail = 0; st->surf_avail = 0; st->n_blocks = 0; }
+  }
   if (tid == 0) hand_over_gen(Y, gen, n_groups);
 }
 template <bool MB>
@@ -709,19 +741,6 @@ int solve_prepare(ll_ctx* ctx) {
     void* p = nullptr; LL_CUDA(ctx, cudaMalloc(&p, sizeof(SolveSync))); LL_CUDA(ctx, cudaMemset(p, 0, sizeof(SolveSync))); ctx->d_sync = (SolveSync*)p;
   }
   return LL_OK;
-}
-// How M slots are spread over `ncta` persistent CTAs: CTA b owns the tiles b, b + grid, b + 2 grid, ... of `tile` slots each.
-struct SolveGrid { int tile, tiles_per_cta, grid; };
-static SolveGrid solve_grid(int ncta, int M) {
-  // The evaluation is fp64-throughput bound (64 DFMA/clk/SM): spread the slots over ALL the CTAs, even when that leaves CTAs partly empty.
-  // tile = slots per CTA and pass (a multiple of 32, <= SOLVE_THREADS); partly empty CTAs on every SM evaluate faster than fewer full ones.
-  const int M1 = M > 0 ? M : 1;
-  SolveGrid g;
-  g.tile = ((ll_div_up(M1, ncta) + 31) / 32) * 32; if (g.tile > SOLVE_THREADS) g.tile = SOLVE_THREADS;
-  const int tiles = ll_div_up(M1, g.tile);
-  g.grid = tiles < ncta ? tiles : ncta;
-  g.tiles_per_cta = ll_div_up(tiles, g.grid);
-  return g;
 }
 // The CTA groups of a launch of n items with M[i] slots (a pure function of the slot counts and the SM count): T = min(SMs, LL_SYNC_ROWS) CTAs
 // at most, every group at least one, the rest shared in proportion to the slots; within group i the rule of solve_grid with its CTA count.  One
@@ -750,6 +769,9 @@ int launch_solve(ll_ctx* ctx, const SolveArgs& a) {
   for (int i = 0; i < a.n_items; i++) M[i] = a.item[i].M;
   LL_TRY(solve_capacity(ctx, a.n_items, M, mb));
   batch_grid(ctx->num_sms, a.n_items, M, g);
+  // Device counts: item 0's M is a capacity.  solve_grid(T, m).grid <= T for every m, and tiles_per_cta grows with m (1 while tile < 256, then
+  // ceil(ceil(m / 256) / T)), so the grid of T CTAs and the capacity's shared memory hold the split of any m up to the capacity.
+  if (a.dev_counts) g[0].grid = std::min(ctx->num_sms, LL_SYNC_ROWS);
   SolveArgs args = a; args.sync = ctx->d_sync;
   int grid = 0; size_t smem = 0;
   for (int i = 0; i < a.n_items; i++) {
