@@ -633,6 +633,55 @@ int ll_transform_dev(ll_ctx* ctx, const double q_wxyz[4], const double t[3], con
 /* Device pointers to the features of the last ll_register / ll_scan_to_pose on this context (scan frame, corners then surfaces). */
 int ll_last_features_dev(ll_ctx* ctx, const ll_point** corner_dev, size_t* n_corner, const ll_point** surf_dev, size_t* n_surf);
 
+/* ---- loop closure back end: the pose graph ----------------------------------------------------------- */
+/* Replaces Ceres_pose_graph_3d::pose_graph_optimization (ceres_pose_graph_3d.hpp:282-352) as laser_mapping.hpp:1058-1089 calls it.
+ * Poses 0 .. n-1; pose 0 is held constant (SetParameterBlockConstant on poses->begin()).  Edge (id_begin = a, id_end = b, t_be = (p^, q^),
+ * information W): residual L [conj(q_a) (p_b - p_a) - p^ ; 2 vec(q^ (conj(q_a) q_b)^*)], L the lower Cholesky factor of W
+ * (PoseGraph3dErrorTerm, :205-239).  Quaternions move by ceres' EigenQuaternionParameterization; the solver is ceres 1.14's
+ * Levenberg-Marquardt trust region with Jacobi scaling, exact linear solves and max_num_iterations 200. */
+typedef struct { double q_wxyz[4]; double t[3]; } ll_pose;
+typedef struct { int id_begin, id_end; double q_wxyz[4]; double t[3]; double information[36]; /* row-major, symmetric positive definite */ } ll_pg_edge;
+typedef struct {
+  double initial_cost, final_cost;   /* 1/2 sum r^2 before, and the least cost an iteration reached (ceres' Summary) */
+  int iterations, evaluations;       /* LM iterations (iteration zero not counted), residual + Jacobian evaluations */
+  int termination;                   /* 0 iteration limit, 1 gradient, 2 parameter, 3 function tolerance, 4 failure (5 invalid steps), 5 radius */
+  int border_nodes, segments, levels, free_nodes, reserved;   /* the elimination plan (see ll_pose_graph_optimize) */
+  long long cycles_eval, cycles_elim, cycles_border, cycles_total;   /* SM clock cycles spent by the solve's phases (clock64) */
+} ll_pg_summary;
+/* Largest border the device solve accepts: the free endpoints of all loop edges (edges between non-consecutive free poses). */
+#define LL_PG_MAX_BORDER 64
+typedef struct ll_pose_graph ll_pose_graph;
+/* A pose-graph solver on ctx's device and stream, with everything a solve of reserve_nodes poses and reserve_edges edges needs allocated now:
+ * such a solve allocates no device memory; a larger one grows the buffers. */
+int  ll_pose_graph_create(ll_ctx* ctx, int reserve_nodes, int reserve_edges, ll_pose_graph** out);
+void ll_pose_graph_release(ll_pose_graph* pg);
+/* Optimizes poses[0 .. n-1] in place (max_iterations <= 0: the reference's 200).  One kernel launch, the whole LM loop on the device:
+ * odometry-chain segments are eliminated by block cyclic reduction, the border (free endpoints of the loop edges, at most LL_PG_MAX_BORDER,
+ * else LL_ERR_CAPACITY) by a dense Cholesky factorization.  Poses no edge touches and pose 0 come back bit-unchanged.  m = 0 changes nothing
+ * and reports 0 iterations.  LL_ERR_INVALID, with nothing changed or enqueued: an id outside 0 .. n-1, id_begin == id_end, a non-finite
+ * value, an information matrix that is not symmetric positive definite. */
+int  ll_pose_graph_optimize(ll_pose_graph* pg, ll_pose* poses, int n, const ll_pg_edge* edges, int m, int max_iterations, ll_pg_summary* summary);
+/* Test hook: one LM step solve at the given poses and trust-region radius, with the Jacobi scaling s of these poses' Jacobian.  Per pose
+ * (6 values: position, then rotation tangent; zero for poses that are not free): the gradient g = J^T r, the scaling s and the solution
+ * `step` of (S J^T J S + D / radius) step = -S g, D = clamp(diag(S J^T J S), 1e-6, 1e32).  *valid = 0 when the factorization failed. */
+int  ll_pose_graph_step(ll_pose_graph* pg, const ll_pose* poses, int n, const ll_pg_edge* edges, int m, double radius, double* cost, double* gradient,
+                        double* scaling, double* step, int* valid);
+/* The loop edge of Scene_alignment::add_constrain_of_loop (scene_alignment.hpp:97-127) with the inversion of laser_mapping.hpp:1065-1066:
+ * icp = the pose ll_scene_align returned for the pair, a = the older keyframe (id_end), b = the newer one (id_begin).  icp is inverted
+ * (Eigen's inverse(): conjugate / squared norm), then q = q_b^-1 icp^-1 q_a, t = q_b^-1 (icp^-1 (t_a - t_icp) - t_b), information = I. */
+void ll_pose_graph_loop_edge(const double icp_q_wxyz[4], const double icp_t[3], const ll_pose* pose_a, int id_a, const ll_pose* pose_b, int id_b,
+                             ll_pg_edge* out);
+/* The corrected map the reference publishes after a loop closure (Mapping_refine::refine_pointcloud / refine_pts, ceres_pose_graph_3d.hpp:437-500,
+ * its if_save == 0 path): keyframe k is clouds[seg_end[k - 1] .. seg_end[k]) (seg_end[-1] = 0), at most 256 keyframes per call.  Each keyframe is
+ * down-sampled by a VoxelGrid at `leaf` (as ll_voxel_downsample_segments), then moved by the float transform R_aff p + T_aff with
+ * R_aff = (R_opt R_ori^T) cast to float and T_aff = (double(R_aff) (-t_ori) + t_opt) cast to float (rotations by toRotationMatrix), from its pose
+ * before (poses_ori[k]) and after (poses_opt[k]) the optimization.  The intensity of the output is 0.  out: the keyframes one after another
+ * (at most n points), n_out_per_seg[k] their counts. */
+int  ll_keyframes_repose(ll_ctx* ctx, const ll_point* clouds, size_t n, const size_t* seg_end, int n_kf, const ll_pose* poses_ori, const ll_pose* poses_opt,
+                         float leaf, ll_point* out, size_t* n_out_per_seg);
+/* R_aff (row-major) and T_aff of ll_keyframes_repose for one keyframe, as the host computes them. */
+void ll_keyframe_affine(const ll_pose* pose_ori, const ll_pose* pose_opt, float R_aff[9], float T_aff[3]);
+
 /* ---- multi-GPU ------------------------------------------------------------------------------------- */
 /* One process per GPU.  The 28-double normal equations (+4 counters) are all-reduced inside the solver kernel
  * through peer-mapped staging buffers (CUDA IPC over NVLink); the host only exchanges the IPC handles once. */

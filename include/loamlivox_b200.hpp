@@ -12,6 +12,7 @@
 #include <array>
 #include <cstdint>
 #include <cstring>
+#include <map>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -314,5 +315,73 @@ class Laser_mapping {
   Laser_mapping(Context& ctx, ll_mapper* m) : ctx_(ctx), mapper_(m) { ll_mapper_config_default(&cfg_); }
   Context& ctx_; ll_mapper_config cfg_; ll_mapper* mapper_ = nullptr;
 };
+
+// ---- Ceres_pose_graph_3d (ceres_pose_graph_3d.hpp:198-352), Scene_alignment::add_constrain_of_loop (scene_alignment.hpp:97-127) and
+// ---- Mapping_refine::refine_pointcloud (ceres_pose_graph_3d.hpp:437-500), without Eigen: quaternions as (w, x, y, z) ----------------------
+struct Pose3d { std::array<double, 4> q{{1, 0, 0, 0}}; std::array<double, 3> p{{0, 0, 0}}; };
+struct Constraint3d {
+  int id_begin = 0, id_end = 0; Pose3d t_be; std::array<double, 36> information{};
+  Constraint3d() { for (int k = 0; k < 6; k++) information[7 * k] = 1.0; }
+};
+typedef std::map<int, Pose3d> MapOfPoses;   // keyframe order: ids 0 .. n-1
+typedef std::vector<Constraint3d> VectorOfConstraints;
+
+class Pose_graph {
+ public:
+  Pose_graph(Context& ctx, int reserve_nodes = 1024, int reserve_edges = 2048) : ctx_(ctx) { ctx_.check(ll_pose_graph_create(ctx.get(), reserve_nodes, reserve_edges, &pg_)); }
+  ~Pose_graph() { ll_pose_graph_release(pg_); }
+  Pose_graph(const Pose_graph&) = delete; Pose_graph& operator=(const Pose_graph&) = delete;
+  // pose_graph_optimization(poses, constraints): poses optimized in place; the lowest id is held constant, as SetParameterBlockConstant on poses->begin()
+  ll_pg_summary pose_graph_optimization(MapOfPoses& poses, const VectorOfConstraints& constraints, int max_iterations = 200) {
+    std::vector<ll_pose> x; x.reserve(poses.size());
+    int expect = 0;
+    for (const auto& kv : poses) {
+      if (kv.first != expect++) throw Error(LL_ERR_INVALID, "pose ids must be 0 .. n-1");
+      ll_pose p; for (int k = 0; k < 4; k++) p.q_wxyz[k] = kv.second.q[k]; for (int k = 0; k < 3; k++) p.t[k] = kv.second.p[k];
+      x.push_back(p);
+    }
+    std::vector<ll_pg_edge> e(constraints.size());
+    for (size_t i = 0; i < constraints.size(); i++) {
+      const Constraint3d& c = constraints[i];
+      e[i].id_begin = c.id_begin; e[i].id_end = c.id_end;
+      for (int k = 0; k < 4; k++) e[i].q_wxyz[k] = c.t_be.q[k]; for (int k = 0; k < 3; k++) e[i].t[k] = c.t_be.p[k];
+      for (int k = 0; k < 36; k++) e[i].information[k] = c.information[k];
+    }
+    ll_pg_summary s;
+    ctx_.check(ll_pose_graph_optimize(pg_, x.data(), (int)x.size(), e.empty() ? nullptr : e.data(), (int)e.size(), max_iterations, &s));
+    for (auto& kv : poses) { for (int k = 0; k < 4; k++) kv.second.q[k] = x[kv.first].q_wxyz[k]; for (int k = 0; k < 3; k++) kv.second.p[k] = x[kv.first].t[k]; }
+    return s;
+  }
+  // Scene_alignment::add_constrain_of_loop(s_idx, t_idx, q_a, t_a, q_b, t_b, icp_q, icp_t) with laser_mapping.hpp:1065-1066's inversion of the
+  // ll_scene_align pose (icp) first: the edge runs from id_b (the newer keyframe) to id_a (the older one)
+  static Constraint3d add_constrain_of_loop(int id_b, int id_a, const Pose3d& a, const Pose3d& b, const std::array<double, 4>& icp_q, const std::array<double, 3>& icp_t) {
+    ll_pose pa, pb; ll_pg_edge e;
+    for (int k = 0; k < 4; k++) { pa.q_wxyz[k] = a.q[k]; pb.q_wxyz[k] = b.q[k]; }
+    for (int k = 0; k < 3; k++) { pa.t[k] = a.p[k]; pb.t[k] = b.p[k]; }
+    ll_pose_graph_loop_edge(icp_q.data(), icp_t.data(), &pa, id_a, &pb, id_b, &e);
+    Constraint3d c; c.id_begin = e.id_begin; c.id_end = e.id_end;
+    for (int k = 0; k < 4; k++) c.t_be.q[k] = e.q_wxyz[k]; for (int k = 0; k < 3; k++) c.t_be.p[k] = e.t[k];
+    for (int k = 0; k < 36; k++) c.information[k] = e.information[k];
+    return c;
+  }
+ private:
+  Context& ctx_; ll_pose_graph* pg_ = nullptr;
+};
+
+// Mapping_refine::refine_pointcloud with if_save == 0 for every keyframe (at most 256 per call): VoxelGrid at leaf, then the float re-pose
+inline std::vector<PointCloud> refine_pointclouds(Context& ctx, const std::vector<PointCloud>& clouds, const MapOfPoses& ori, const MapOfPoses& opt, float leaf) {
+  std::vector<ll_point> in; std::vector<size_t> ends; std::vector<ll_pose> po, pp;
+  for (const PointCloud& c : clouds) { for (const PointXYZI& p : c) in.push_back({p.x, p.y, p.z, p.intensity}); ends.push_back(in.size()); }
+  for (size_t k = 0; k < clouds.size(); k++) {
+    const Pose3d &a = ori.at((int)k), &b = opt.at((int)k); ll_pose x, y;
+    for (int j = 0; j < 4; j++) { x.q_wxyz[j] = a.q[j]; y.q_wxyz[j] = b.q[j]; } for (int j = 0; j < 3; j++) { x.t[j] = a.p[j]; y.t[j] = b.p[j]; }
+    po.push_back(x); pp.push_back(y);
+  }
+  std::vector<ll_point> out(in.size()); std::vector<size_t> cnt(clouds.size());
+  ctx.check(ll_keyframes_repose(ctx.get(), in.data(), in.size(), ends.data(), (int)clouds.size(), po.data(), pp.data(), leaf, out.data(), cnt.data()));
+  std::vector<PointCloud> res(clouds.size()); size_t w = 0;
+  for (size_t k = 0; k < clouds.size(); k++) { res[k] = to_cloud(std::vector<ll_point>(out.begin() + w, out.begin() + w + cnt[k])); w += cnt[k]; }
+  return res;
+}
 
 }  // namespace ll200

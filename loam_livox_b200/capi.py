@@ -24,6 +24,7 @@ LL_RELOC_MAX_SCORE_POINTS = 8192
 LL_RECOVERY_LOG = 1024
 LL_TRACKING, LL_SUSPECT, LL_LOST = 0, 1, 2
 LL_BAD_NONE, LL_BAD_REJECTED, LL_BAD_INLIER = 0, 1, 2
+LL_PG_MAX_BORDER = 64
 LL_MAPPER_IMAGE_MAGIC, LL_MAPPER_IMAGE_VERSION = b"LLMAPIMG", 1
 (LL_IMAGE_CONFIG, LL_IMAGE_SCALARS, LL_IMAGE_HISTORY_CORNER, LL_IMAGE_HISTORY_SURF, LL_IMAGE_SNAPSHOT_CORNER, LL_IMAGE_SNAPSHOT_SURF, LL_IMAGE_CELLS_CORNER,
  LL_IMAGE_CELLS_SURF, LL_IMAGE_SECTIONS) = range(9)
@@ -40,6 +41,8 @@ EXPORTS = [
     "ll_reloc_index_build", "ll_reloc_index_release", "ll_reloc_index_read", "ll_relocalize", "ll_reloc_scores", "ll_mapper_whole_map", "ll_mapper_set_pose",
     "ll_reloc_field_build", "ll_reloc_field_release", "ll_reloc_field_read", "ll_relocalize_field", "ll_reloc_field_scores",
     "ll_mapper_recovery_default", "ll_mapper_set_recovery", "ll_mapper_recovery_read", "ll_mapper_recovery_last_inputs",
+    "ll_pose_graph_create", "ll_pose_graph_release", "ll_pose_graph_optimize", "ll_pose_graph_step", "ll_pose_graph_loop_edge",
+    "ll_keyframes_repose", "ll_keyframe_affine",
 ]
 
 
@@ -144,6 +147,22 @@ class RecoveryStep(C.Structure):
                [("n_score", C.c_int32 * 2), ("score_leaf", C.c_float * 2), ("t0", C.c_double * 3), ("step", C.c_double * 3), ("tilt_wxyz", C.c_double * 4),
                 ("verify_fraction", C.c_double), ("q_wxyz", C.c_double * 4), ("t", C.c_double * 3), ("inlier_threshold", C.c_double),
                 ("ms_map", C.c_double), ("ms_search", C.c_double)]
+
+
+class Pose(C.Structure):
+    """ll_pose: a pose graph vertex (q as w, x, y, z)."""
+    _fields_ = [("q_wxyz", C.c_double * 4), ("t", C.c_double * 3)]
+
+
+class PgEdge(C.Structure):
+    """ll_pg_edge: a pose graph constraint t_be = (q, t) from id_begin to id_end with its information matrix (row-major)."""
+    _fields_ = [("id_begin", C.c_int), ("id_end", C.c_int), ("q_wxyz", C.c_double * 4), ("t", C.c_double * 3), ("information", C.c_double * 36)]
+
+
+class PgSummary(C.Structure):
+    _fields_ = [("initial_cost", C.c_double), ("final_cost", C.c_double)] + \
+               [(n, C.c_int) for n in ("iterations", "evaluations", "termination", "border_nodes", "segments", "levels", "free_nodes", "reserved")] + \
+               [(n, C.c_longlong) for n in ("cycles_eval", "cycles_elim", "cycles_border", "cycles_total")]
 
 
 class LoamLivoxError(RuntimeError):
@@ -251,6 +270,13 @@ def lib():
     L.ll_mapper_set_recovery.argtypes = [vp, C.POINTER(RecoveryCfg)]
     L.ll_mapper_recovery_read.argtypes = [vp, C.POINTER(RecoveryStep), ci, C.POINTER(ci), C.POINTER(ci)]
     L.ll_mapper_recovery_last_inputs.argtypes = [vp, C.POINTER(RelocCfg), C.POINTER(RelocFineCfg), C.POINTER(RegState), vp, vp, vp, vp, vp, sz, vp, vp, ci]
+    L.ll_pose_graph_create.argtypes = [vp, ci, ci, C.POINTER(vp)]
+    L.ll_pose_graph_release.argtypes = [vp]
+    L.ll_pose_graph_optimize.argtypes = [vp, vp, ci, vp, ci, ci, C.POINTER(PgSummary)]
+    L.ll_pose_graph_step.argtypes = [vp, vp, ci, vp, ci, cd, C.POINTER(cd), vp, vp, vp, C.POINTER(ci)]
+    L.ll_pose_graph_loop_edge.argtypes = [vp, vp, C.POINTER(Pose), ci, C.POINTER(Pose), ci, C.POINTER(PgEdge)]
+    L.ll_keyframes_repose.argtypes = [vp, vp, sz, vp, ci, vp, vp, cf, vp, vp]
+    L.ll_keyframe_affine.argtypes = [C.POINTER(Pose), C.POINTER(Pose), vp, vp]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64
     _LIB = L

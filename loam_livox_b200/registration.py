@@ -637,6 +637,88 @@ class Scene_alignment:
         return res
 
 
+def pg_edges(id_begin, id_end, q_wxyz, t, information=None):
+    """An array of capi.PgEdge (Ceres_pose_graph_3d::Constraint3d): information defaults to the identity, as the reference always passes."""
+    id_begin, id_end = np.atleast_1d(id_begin), np.atleast_1d(id_end)
+    q, t = np.asarray(q_wxyz, np.float64).reshape(-1, 4), np.asarray(t, np.float64).reshape(-1, 3)
+    W = np.broadcast_to(np.eye(6) if information is None else np.asarray(information, np.float64), (len(id_begin), 6, 6))
+    out = (capi.PgEdge * len(id_begin))()
+    for k in range(len(id_begin)):
+        out[k].id_begin, out[k].id_end = int(id_begin[k]), int(id_end[k])
+        out[k].q_wxyz[:], out[k].t[:], out[k].information[:] = list(q[k]), list(t[k]), list(W[k].reshape(36))
+    return out
+
+
+def pg_loop_edge(icp_q_wxyz, icp_t, pose_a, id_a: int, pose_b, id_b: int) -> capi.PgEdge:
+    """Scene_alignment::add_constrain_of_loop on the pose ll_scene_align returned (laser_mapping.hpp:1062-1078): a = the older keyframe
+    (id_end), b = the newer one (id_begin); poses as (q_wxyz, t) rows of 7."""
+    e = capi.PgEdge()
+    pa, pb = capi.Pose(), capi.Pose()
+    pa.q_wxyz[:], pa.t[:] = list(pose_a[:4]), list(pose_a[4:7])
+    pb.q_wxyz[:], pb.t[:] = list(pose_b[:4]), list(pose_b[4:7])
+    q, t = np.ascontiguousarray(icp_q_wxyz, np.float64), np.ascontiguousarray(icp_t, np.float64)
+    capi.lib().ll_pose_graph_loop_edge(q.ctypes.data, t.ctypes.data, C.byref(pa), id_a, C.byref(pb), id_b, C.byref(e))
+    return e
+
+
+def keyframes_repose(ctx: Context, clouds, poses_ori, poses_opt, leaf: float):
+    """Mapping_refine::refine_pointcloud (ceres_pose_graph_3d.hpp:437-500, if_save == 0) for every keyframe: clouds is a list of [n_k, 4] arrays,
+    poses rows of 7 (q_wxyz, t) before / after the optimization.  Returns the list of re-posed, down-sampled clouds (intensity 0)."""
+    arrs = [np.ascontiguousarray(c, np.float32).reshape(-1, 4) for c in clouds]
+    allp = np.concatenate(arrs) if arrs else np.zeros((0, 4), np.float32)
+    allp = np.ascontiguousarray(allp)
+    ends = np.cumsum([a.shape[0] for a in arrs]).astype(np.uint64)
+    po, pp = np.ascontiguousarray(poses_ori, np.float64).reshape(-1, 7), np.ascontiguousarray(poses_opt, np.float64).reshape(-1, 7)
+    out, cnt = np.zeros((max(allp.shape[0], 1), 4), np.float32), np.zeros(len(arrs), np.uint64)
+    ctx.check(ctx._lib.ll_keyframes_repose(ctx.h, allp.ctypes.data, allp.shape[0], ends.ctypes.data, len(arrs), po.ctypes.data, pp.ctypes.data, leaf,
+                                           out.ctypes.data, cnt.ctypes.data))
+    res, w = [], 0
+    for c in cnt:
+        res.append(out[w:w + int(c)].copy())
+        w += int(c)
+    return res
+
+
+class PoseGraph:
+    """Mirror of Ceres_pose_graph_3d::pose_graph_optimization (ceres_pose_graph_3d.hpp:282-352) on the device.  Poses are an [n, 7] array of
+    rows (qw, qx, qy, qz, tx, ty, tz), keyframe order; pose 0 is held constant."""
+
+    def __init__(self, ctx: Context, reserve_nodes: int = 1024, reserve_edges: int = 2048):
+        self.ctx = ctx
+        h = C.c_void_p()
+        ctx.check(ctx._lib.ll_pose_graph_create(ctx.h, reserve_nodes, reserve_edges, C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx._lib.ll_pose_graph_release(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def optimize(self, poses, edges, max_iterations: int = 200):
+        """Returns (optimized poses, capi.PgSummary); `poses` is not modified."""
+        x = np.ascontiguousarray(poses, np.float64).reshape(-1, 7).copy()
+        s = capi.PgSummary()
+        self.ctx.check(self.ctx._lib.ll_pose_graph_optimize(self.h, x.ctypes.data, x.shape[0], C.cast(edges, C.c_void_p) if len(edges) else None, len(edges),
+                                                            max_iterations, C.byref(s)))
+        return x, s
+
+    def step(self, poses, edges, radius: float):
+        """The LM step solve at `poses` (ll_pose_graph_step): (cost, gradient [n,6], scaling [n,6], step [n,6], valid)."""
+        x = np.ascontiguousarray(poses, np.float64).reshape(-1, 7)
+        n = x.shape[0]
+        g, s, st = np.zeros((n, 6)), np.zeros((n, 6)), np.zeros((n, 6))
+        cost, valid = C.c_double(), C.c_int()
+        self.ctx.check(self.ctx._lib.ll_pose_graph_step(self.h, x.ctypes.data, n, C.cast(edges, C.c_void_p), len(edges), radius, C.byref(cost), g.ctypes.data,
+                                                        s.ctypes.data, st.ctypes.data, C.byref(valid)))
+        return cost.value, g, s, st, bool(valid.value)
+
+
 class Points_cloud_map:
     """Device-resident voxel-cell map as the matching path uses it (Points_cloud_map<float>, loam_livox/source/cell_map_keyframe.hpp:264;
     append_cloud :619, find_cells_in_radius :761; the consumer is update_buff_for_matching, loam_livox/source/laser_mapping.hpp:471-516)."""
