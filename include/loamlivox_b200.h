@@ -230,6 +230,13 @@ int ll_set_blocks(ll_ctx* ctx, const ll_reg_state* in, size_t n, const int32_t* 
  * l1_out[n] (or NULL) = the L1 norms (+inf for invalid slots), iterations[2] = LM iterations of solve #1 and #2. */
 int ll_solve_fused(ll_ctx* ctx, int prerun, int max_iterations, double x_io[7], double* threshold, int* n_distinct, int* n_kept, double* l1_out,
                    int iterations[2]);
+/* ... and caller-given features through ll_scan_to_pose's registration on the front end's device-side counts (the capacity-sized sort, kNN and
+ * solver launches that read the counts on the device), for a whole frame: the features go where the front end leaves them and that same path
+ * runs.  Returns and fills `out` as ll_register on the same features would, except: LL_ERR_INVALID when ll_scan_to_pose would take the
+ * host-sized path for this context, map and state; LL_ERR_CAPACITY when n_corner or n_surf exceeds max_scan_points (both with nothing
+ * enqueued).  n_corner + n_surf > max_features is refused on the device as a front end's counts are: LL_ERR_CAPACITY. */
+int ll_register_dev_counts(ll_ctx* ctx, const ll_map* map, const void* scan_corner, size_t n_corner, const void* scan_surf, size_t n_surf,
+                           int fmt, int where, const ll_reg_state* in, ll_reg_result* out);
 
 /* ---- N4: loop-closure reuse of S3 ----------------------------------------------------------------------- */
 /* Replaces Scene_alignment::find_tranfrom_of_two_mappings (scene_alignment.hpp:269-353) from the point where the four feature clouds exist:

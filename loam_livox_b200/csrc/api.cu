@@ -866,6 +866,13 @@ static int voxel_chains(ll_ctx* ctx, const FrontStreams& fs, const ll_pipeline_c
   return launch_voxel_chains(ctx, fs.main, c, 2, fs.fork, fs.join);
 }
 
+// The front end's counts and the extractor's meta into pinned memory, where front_end_counts reads them.
+static int front_end_counts_d2h(ll_ctx* ctx, cudaStream_t s) {
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->pin->fe_counts, ctx->A.counts, sizeof(ctx->pin->fe_counts), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->pin->fe_meta, ctx->ex.d_meta, sizeof(ctx->pin->fe_meta), cudaMemcpyDeviceToHost, s));
+  return LL_OK;
+}
+
 // Everything of the front end that is enqueued on the device, in the order the reference runs it; counts land in pinned memory.
 static int front_end_enqueue(ll_ctx* ctx, const FrontStreams& fs, const ll_pipeline_cfg* pc, int ncap) {
   cudaStream_t s = fs.main;
@@ -884,9 +891,7 @@ static int front_end_enqueue(ll_ctx* ctx, const FrontStreams& fs, const ll_pipel
   LL_TRY(voxel_chains(ctx, fs, pc, ncap, A.counts + 0, ncap, A.counts + 1));   // counts: [0] corners [1] surf [2] full
   if (petals_aside) LL_CUDA(ctx, cudaStreamWaitEvent(s, fs.join3, 0));
   // [10], [11]: min / max time stamp of the full cloud
-  LL_CUDA(ctx, cudaMemcpyAsync(ctx->pin->fe_counts, A.counts, sizeof(ctx->pin->fe_counts), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaMemcpyAsync(ctx->pin->fe_meta, ctx->ex.d_meta, sizeof(ctx->pin->fe_meta), cudaMemcpyDeviceToHost, s));
-  return LL_OK;
+  return front_end_counts_d2h(ctx, s);
 }
 
 // `enqueue` (the device part of a front end, on stream s) eagerly on the first call with `key`, captured into g on the second when `capturable`,
@@ -982,14 +987,18 @@ static bool device_handoff(ll_ctx* ctx, const ll_map* map, const ll_reg_state* i
   if (solve_capacity(ctx, 1, &ctx->cfg.max_features, in->if_motion_deblur ? 1 : 0) != LL_OK) { ctx->err = err; return false; }
   return true;
 }
-static int scan_to_pose_device(ll_ctx* ctx, const ll_map* map, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc,
-                               const ll_reg_state* in, ll_reg_result* out, int* nc, int* ns, int* dropped) {
+// The registration on the device counts (device_handoff has passed): the state goes up, `front` enqueues what leaves the features in tmp_a /
+// tmp_b, their counts in counts[5] / [7] and those on their way into pin->fe_counts / fe_meta (front_end_enqueue's end), then the hand-over,
+// the registration and the outcome.  ll_scan_to_pose runs the front end here, ll_register_dev_counts uploads caller-given features.
+template <typename F>
+static int register_dev_counts(ll_ctx* ctx, const ll_map* map, const ll_pipeline_cfg* pc, const ll_reg_state* in, ll_reg_result* out, int* nc, int* ns,
+                               int* dropped, F&& front) {
   cudaStream_t s = ctx->stream;
   const RegArrays& A = ctx->A;
   const int cap = ctx->cfg.max_features;
   RegDevState* h = ctx->pin->state_in; fill_state(h, in);
   LL_CUDA(ctx, cudaMemcpyAsync(ctx->d_reg, h, sizeof(RegDevState), cudaMemcpyHostToDevice, s));
-  LL_TRY(scan_front_end_enqueue(ctx, ctx->own_front(), raw, n, fmt, where, stamp, pc));
+  LL_TRY(front());
   feature_handoff_kernel<<<ctx->num_sms * 2, 256, 0, s>>>(A.counts, ctx->ex.d_meta, pc->whole_frame, cap, A.tmp_a, A.tmp_b, A.feat, A.dev_counts); ctx->launches++;
   LL_CUDA(ctx, cudaGetLastError());
   int st = LL_OK;
@@ -1009,7 +1018,8 @@ extern "C" int ll_scan_to_pose(ll_ctx* ctx, const ll_map* map, const void* raw, 
   cudaSetDevice(ctx->device);
   int nc = 0, ns = 0, dropped = 0;
   if (device_handoff(ctx, map, in)) {
-    const int st = scan_to_pose_device(ctx, map, raw, n, fmt, where, stamp, pc, in, out, &nc, &ns, &dropped);
+    const int st = register_dev_counts(ctx, map, pc, in, out, &nc, &ns, &dropped,
+                                       [&] { return scan_front_end_enqueue(ctx, ctx->own_front(), raw, n, fmt, where, stamp, pc); });
     if (st != LL_OK && !(st == LL_ERR_NO_BLOCKS && !dropped)) return st;
     if (n_corner_used) *n_corner_used = nc; if (n_surf_used) *n_surf_used = ns;
     if (dropped) { memset(out, 0, sizeof(*out)); out->status = 1; ctx->set_error("frame dropped: <= 5 petals"); return LL_OK; }
@@ -1019,6 +1029,30 @@ extern "C" int ll_scan_to_pose(ll_ctx* ctx, const ll_map* map, const void* raw, 
   if (n_corner_used) *n_corner_used = nc; if (n_surf_used) *n_surf_used = ns;
   if (dropped) { memset(out, 0, sizeof(*out)); out->status = 1; ctx->set_error("frame dropped: <= 5 petals"); return LL_OK; }
   return register_device(ctx, map, nc, ns, in, out);
+}
+
+// Caller-given features where the front end leaves them (tmp_a / tmp_b, counts[5] / [7]), then ll_scan_to_pose's registration on the device
+// counts for a whole frame.  n_corner + n_surf > max_features reaches the hand-over kernel's rule, as a front end's counts would.
+extern "C" int ll_register_dev_counts(ll_ctx* ctx, const ll_map* map, const void* scan_corner, size_t n_corner, const void* scan_surf, size_t n_surf, int fmt,
+                                      int where, const ll_reg_state* in, ll_reg_result* out) {
+  if (!ctx || !map || !in || !out || (!scan_corner && n_corner) || (!scan_surf && n_surf)) return LL_ERR_INVALID;
+  cudaSetDevice(ctx->device);
+  if (!device_handoff(ctx, map, in)) { ctx->set_error("ll_scan_to_pose would register on host-sized counts here"); return LL_ERR_INVALID; }
+  if (n_corner > (size_t)ctx->cfg.max_scan_points || n_surf > (size_t)ctx->cfg.max_scan_points) {
+    ctx->set_error("more corner or surface features than max_scan_points"); return LL_ERR_CAPACITY;
+  }
+  static const ll_pipeline_cfg whole = {1, 0, 0.f, 0.f, 0.f, 0.f, 1};   // (only whole_frame is read: no piece is dropped)
+  cudaStream_t s = ctx->stream;
+  const RegArrays& A = ctx->A;
+  const int cnt[2] = {(int)n_corner, (int)n_surf};
+  int nc = 0, ns = 0, dropped = 0;
+  return register_dev_counts(ctx, map, &whole, in, out, &nc, &ns, &dropped, [&]() -> int {
+    LL_TRY(upload_cloud(ctx, s, scan_corner, n_corner, fmt, where, A.tmp_a));
+    LL_TRY(upload_cloud(ctx, s, scan_surf, n_surf, fmt, where, A.tmp_b));
+    LL_CUDA(ctx, cudaMemcpyAsync(A.counts + 5, &cnt[0], sizeof(int), cudaMemcpyHostToDevice, s));
+    LL_CUDA(ctx, cudaMemcpyAsync(A.counts + 7, &cnt[1], sizeof(int), cudaMemcpyHostToDevice, s));
+    return front_end_counts_d2h(ctx, s);
+  });
 }
 
 // Multi-head frame (Mid-100: three Mid-40 heads, launch/rosbag_mid100.launch): Laser_feature::laserCloudHandler runs ONE Livox_laser object over
