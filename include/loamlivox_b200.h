@@ -689,6 +689,62 @@ int  ll_keyframes_repose(ll_ctx* ctx, const ll_point* clouds, size_t n, const si
 /* R_aff (row-major) and T_aff of ll_keyframes_repose for one keyframe, as the host computes them. */
 void ll_keyframe_affine(const ll_pose* pose_ori, const ll_pose* pose_opt, float R_aff[9], float T_aff[3]);
 
+/* ---- loop detection: keyframes over the full-resolution cell map and the candidate search ------------------------------------------------ */
+/* A keyframe (Maps_keyframe<float>, cell_map_keyframe.hpp:1002-1494) is a set of cells of one ll_cellmap, the caller's full-resolution map
+ * (m_pt_cell_map_full, laser_mapping.hpp:617-618).  A cell here is one incarnation of a map cell: a revisit replaces a cell by an empty one
+ * (find_cell, :716-758) and a keyframe that held the old one keeps it with its points.  Cells are ordered by ascending cell key (k, j, i), then
+ * incarnation; that order replaces the reference's std::set of pointers (address order) in every sum and in the typed clouds.  A keyframe refers to
+ * the map's point store: after a down-sample-and-replace assembly of the map, appends and analyses of the keyframes that held its cells before are
+ * refused (LL_ERR_INVALID).  The accumulated cloud (m_accumulated_point_cloud) stays the caller's. */
+typedef struct ll_keyframe ll_keyframe;
+enum { LL_CELL_SPHERE = 0, LL_CELL_LINE = 1, LL_CELL_PLANE = 2, LL_CELL_ALL = -1 };   /* Feature_type (cell_map_keyframe.hpp:46-51); ALL: every cell */
+typedef struct {
+  int    cells, line_cells, plane_cells, accumulate_frames;
+  float  center[3];                          /* get_center(): the mean of the cell centres (:1292-1302)                                     */
+  float  roi_range;                          /* m_roi_range: 0.9 quantile of the distinct centre distances (:1304-1319); 0 without cells       */
+  float  ratio_nonzero_line, ratio_nonzero_plane;   /* m_ratio_nonzero_*: image pixels >= 1 before the blur (:1423-1424)                    */
+  size_t line_points, plane_points, all_points;     /* sizes of the typed clouds                                                          */
+} ll_keyframe_info;
+int  ll_keyframe_create(ll_ctx* ctx, ll_keyframe** out);
+void ll_keyframe_release(ll_keyframe* kf);
+/* laser_mapping.hpp:1527-1533: m_pt_cell_map_full.append_cloud(pts, &cell_vec), then add_cells(cell_vec) and m_accumulate_frames++ on each of the
+ * n_open keyframes.  The append is ll_cellmap_append itself (same map state, same return codes); the cell set follows :585-665: every cell the
+ * points reach on the first append into an empty map (set_point_cloud), afterwards the cells that received at least 3 of this call's points. */
+int  ll_keyframe_append(ll_ctx* ctx, ll_cellmap* map, const void* pts, size_t n, int fmt, int where, ll_keyframe* const* open, int n_open);
+/* Maps_keyframe::analyze (:1487-1494) over the keyframe's cells as `map` holds them now: per cell the mean and covariance (COMP_TYPE float,
+ * IF_COV_INIT_IDENTITY 0, N - 1 divisor) and determine_feature (:436-473; sphere below 5 points or when |centre - mean| > 0.75 res, plane when
+ * l1 / 3 > l0, line when l2 / 3 > l1, eigen-decomposition in fp64); then the centre, the ROI range, the 60 x 60 line / plane direction images
+ * of generate_feature_img (:1385-1427) with their nonzero ratios, the Gaussian blur (9 x 9, sigma 4, wrap padding) and the typed clouds.
+ * incremental_cov: common/if_update_mean_and_cov_incrementally of the map (1 in performance_precision.yaml, 0 in performance_realtime.yaml), one
+ * value for the map's lifetime; the per-point recurrence of append_pt (:392-414) is replayed over each cell's points in append order. */
+int  ll_keyframe_analyze(ll_ctx* ctx, ll_cellmap* map, ll_keyframe* kf, int incremental_cov, ll_keyframe_info* info);
+int  ll_keyframe_get_info(const ll_keyframe* kf, ll_keyframe_info* info);
+/* The analyzed keyframe's cells (at most cap): key (as ll_image_cell::key), incarnation, type and feature vector (3 floats; zero for spheres).
+ * Any output may be NULL; *n = the keyframe's cell count.  keys and epochs are also available before an analysis. */
+int  ll_keyframe_cells(ll_ctx* ctx, const ll_keyframe* kf, uint64_t* keys, int* epochs, int* types, float* vecs, int cap, int* n);
+/* 60 x 60 row-major images [phi][theta]: direction counts before the blur and the blurred images; any may be NULL. */
+int  ll_keyframe_images(ll_ctx* ctx, const ll_keyframe* kf, float* count_line, float* count_plane, float* line, float* plane);
+/* extract_specify_points(e_feature_line / e_feature_plane) or get_all_pointcloud() (which = LL_CELL_LINE / LL_CELL_PLANE / LL_CELL_ALL,
+ * :1263-1290): the points of those cells in cell order, append order inside a cell, intensity 0.  The cloud stays on the device (*out_dev, valid
+ * until the next analysis of this keyframe), ready for ll_scene_align with LL_DEVICE; copied to out_host (cap points) when that is not NULL. */
+int  ll_keyframe_cloud(ll_ctx* ctx, const ll_keyframe* kf, int which, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev);
+typedef struct {
+  int   minimum_keyframe_differen;   /* loop_closure/minimum_keyframe_differen (200)                                                      */
+  float avail_ratio_plane, avail_ratio_line;   /* laser_mapping.hpp:894-895 (0.05, 0.03)                                              */
+  float maximum_roi_difference;      /* :1004 (5.0)                                                                                      */
+  float minimum_similarity_linear, minimum_similarity_planar;   /* loop_closure/minimum_similarity_* (YAMLs: 0.65, 0.94)              */
+  double plane_with_line;            /* :1012 (0.92, a double literal against the float similarity)                                      */
+} ll_loop_cfg;
+void ll_loop_cfg_default(ll_loop_cfg* cfg);
+/* service_loop_detection's search (laser_mapping.hpp:988-1033) for kfs[newest] against kfs[0 .. newest - 1], every keyframe analyzed.  One launch
+ * computes max_similiarity_of_two_image (matchTemplate CCORR_NORMED of the newest image against the earlier one wrap-padded by 30, max over
+ * 61 x 61 positions) for the plane and the line images of every pair; sim_plane / sim_line[his] (newest entries, may be NULL).  candidates (his
+ * ascending, at most newest) are the pairs that pass the keyframe-difference, nonzero-ratio, ROI-range (|d| > 5 in float), similarity and
+ * cell-count gates; the cell-count gate is (a - b) / (a + b) * 0.1 in size_t (:1030), so a pair passes it only when the newest keyframe has at
+ * least as many cells and the earlier one has some.  Alignment, `his += 10` (:1048-1052) and the stop after a true loop stay the caller's. */
+int  ll_loop_search(ll_ctx* ctx, const ll_keyframe* const* kfs, int n, int newest, const ll_loop_cfg* cfg, float* sim_plane, float* sim_line, int* candidates,
+                    int* n_candidates);
+
 /* ---- multi-GPU ------------------------------------------------------------------------------------- */
 /* One process per GPU.  The 28-double normal equations (+4 counters) are all-reduced inside the solver kernel
  * through peer-mapped staging buffers (CUDA IPC over NVLink); the host only exchanges the IPC handles once. */

@@ -5,6 +5,8 @@
 //                                                                                               pointcloudAssociateToMap :673)
 //   Points_cloud_map                 loam_livox/source/cell_map_keyframe.hpp:264        (append_cloud :619, cells in radius + FOV :761, laser_mapping.hpp:475-516)
 //   Laser_mapping::process_new_scan  loam_livox/source/laser_mapping.hpp:1316
+//   Maps_keyframe                    loam_livox/source/cell_map_keyframe.hpp:1002   (analyze :1488, extract_specify_points :1263, get_center :1292,
+//                                                                                               max_similiarity_of_two_image :1157)
 // so that laser_feature_extractor.hpp / laser_mapping.hpp can switch with the small adapter shown in INTEGRATION.md.
 // No PCL / Eigen / Ceres needed: clouds are std::vector<ll200::PointXYZI> (layout-identical to pcl::PointXYZI, 32 bytes).
 #pragma once
@@ -382,6 +384,53 @@ inline std::vector<PointCloud> refine_pointclouds(Context& ctx, const std::vecto
   std::vector<PointCloud> res(clouds.size()); size_t w = 0;
   for (size_t k = 0; k < clouds.size(); k++) { res[k] = to_cloud(std::vector<ll_point>(out.begin() + w, out.begin() + w + cnt[k])); w += cnt[k]; }
   return res;
+}
+
+// ---- Maps_keyframe (cell_map_keyframe.hpp:1002-1494) over the cells of a full-resolution Points_cloud_map --------------------------
+enum Feature_type { e_feature_sphere = LL_CELL_SPHERE, e_feature_line = LL_CELL_LINE, e_feature_plane = LL_CELL_PLANE };
+class Maps_keyframe {
+ public:
+  explicit Maps_keyframe(Context& ctx) : ctx_(ctx) { ctx_.check(ll_keyframe_create(ctx_.get(), &kf_)); }
+  ~Maps_keyframe() { ll_keyframe_release(kf_); }
+  Maps_keyframe(const Maps_keyframe&) = delete; Maps_keyframe& operator=(const Maps_keyframe&) = delete;
+  // m_pt_cell_map_full.append_cloud(pts, &cell_vec), then add_cells(cell_vec) on every open keyframe (laser_mapping.hpp:1527-1533)
+  static void append_cloud(Context& ctx, Points_cloud_map& full, const PointCloud& pts, const std::vector<Maps_keyframe*>& open) {
+    std::vector<ll_keyframe*> h; for (Maps_keyframe* k : open) h.push_back(k->kf_);
+    ctx.check(ll_keyframe_append(ctx.get(), full.get(), pts.data(), pts.size(), LL_FMT_PCL32, LL_HOST, h.data(), (int)h.size()));
+  }
+  // analyze (:1487-1494) over the cells as `full` holds them now; if_update_mean_and_cov_incrementally is the map's setting
+  int analyze(Points_cloud_map& full, int if_update_mean_and_cov_incrementally = 0) {
+    ctx_.check(ll_keyframe_analyze(ctx_.get(), full.get(), kf_, if_update_mean_and_cov_incrementally, &info_)); return 0;
+  }
+  PointCloud extract_specify_points(Feature_type select_type) const { return cloud(select_type); }   // :1263-1280
+  PointCloud get_all_pointcloud() const { return cloud(LL_CELL_ALL); }                                // :1282-1290
+  std::array<float, 3> get_center() const { return {{info_.center[0], info_.center[1], info_.center[2]}}; }   // :1292-1302
+  const ll_keyframe_info& info() const { return info_; }   // m_roi_range, m_ratio_nonzero_*, cell and point counts
+  // max_similiarity_of_two_image(img_a, img_b) (:1157-1202) of keyframe a's and keyframe b's line or plane image, as ll_loop_search computes it
+  static float max_similiarity_of_two_image(Context& ctx, const Maps_keyframe& a, const Maps_keyframe& b, Feature_type which) {
+    const ll_keyframe* kfs[2] = {b.kf_, a.kf_};
+    ll_loop_cfg cfg; ll_loop_cfg_default(&cfg);
+    float sp = 0.f, sl = 0.f; int n = 0;
+    ctx.check(ll_loop_search(ctx.get(), kfs, 2, 1, &cfg, &sp, &sl, nullptr, &n));
+    return which == e_feature_line ? sl : sp;
+  }
+  ll_keyframe* get() const { return kf_; }
+ private:
+  PointCloud cloud(int which) const {
+    size_t n = 0; const ll_point* dev = nullptr;
+    ctx_.check(ll_keyframe_cloud(ctx_.get(), kf_, which, nullptr, 0, &n, &dev));
+    std::vector<ll_point> out(n);
+    if (n) ctx_.check(ll_keyframe_cloud(ctx_.get(), kf_, which, out.data(), n, &n, &dev));
+    return to_cloud(out);
+  }
+  Context& ctx_; ll_keyframe* kf_ = nullptr; ll_keyframe_info info_ = {};
+};
+// service_loop_detection's candidate search (laser_mapping.hpp:988-1033) for keyframes[newest]: the candidates his ascending
+inline std::vector<int> loop_search(Context& ctx, const std::vector<Maps_keyframe*>& keyframes, int newest, const ll_loop_cfg& cfg) {
+  std::vector<const ll_keyframe*> h; for (Maps_keyframe* k : keyframes) h.push_back(k->get());
+  std::vector<int> cand((size_t)(newest > 0 ? newest : 1)); int n = 0;
+  ctx.check(ll_loop_search(ctx.get(), h.data(), (int)h.size(), newest, &cfg, nullptr, nullptr, cand.data(), &n));
+  cand.resize(n); return cand;
 }
 
 }  // namespace ll200

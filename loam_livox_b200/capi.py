@@ -43,7 +43,10 @@ EXPORTS = [
     "ll_mapper_recovery_default", "ll_mapper_set_recovery", "ll_mapper_recovery_read", "ll_mapper_recovery_last_inputs",
     "ll_pose_graph_create", "ll_pose_graph_release", "ll_pose_graph_optimize", "ll_pose_graph_step", "ll_pose_graph_loop_edge",
     "ll_keyframes_repose", "ll_keyframe_affine",
+    "ll_keyframe_create", "ll_keyframe_release", "ll_keyframe_append", "ll_keyframe_analyze", "ll_keyframe_get_info", "ll_keyframe_cells",
+    "ll_keyframe_images", "ll_keyframe_cloud", "ll_loop_cfg_default", "ll_loop_search",
 ]
+LL_CELL_SPHERE, LL_CELL_LINE, LL_CELL_PLANE, LL_CELL_ALL = 0, 1, 2, -1
 
 
 class Config(C.Structure):
@@ -165,6 +168,20 @@ class PgSummary(C.Structure):
                [(n, C.c_longlong) for n in ("cycles_eval", "cycles_elim", "cycles_border", "cycles_total")]
 
 
+class KeyframeInfo(C.Structure):
+    """ll_keyframe_info: what Maps_keyframe::analyze leaves (centre, ROI range, nonzero ratios) and the typed clouds' sizes."""
+    _fields_ = [(n, C.c_int) for n in ("cells", "line_cells", "plane_cells", "accumulate_frames")] + \
+               [("center", C.c_float * 3), ("roi_range", C.c_float), ("ratio_nonzero_line", C.c_float), ("ratio_nonzero_plane", C.c_float)] + \
+               [(n, C.c_size_t) for n in ("line_points", "plane_points", "all_points")]
+
+
+class LoopCfg(C.Structure):
+    """ll_loop_cfg: the gates of service_loop_detection's candidate search."""
+    _fields_ = [("minimum_keyframe_differen", C.c_int)] + \
+               [(n, C.c_float) for n in ("avail_ratio_plane", "avail_ratio_line", "maximum_roi_difference", "minimum_similarity_linear",
+                                         "minimum_similarity_planar")] + [("plane_with_line", C.c_double)]
+
+
 class LoamLivoxError(RuntimeError):
     pass
 
@@ -278,10 +295,28 @@ def lib():
     L.ll_pose_graph_loop_edge.argtypes = [vp, vp, C.POINTER(Pose), ci, C.POINTER(Pose), ci, C.POINTER(PgEdge)]
     L.ll_keyframes_repose.argtypes = [vp, vp, sz, vp, ci, vp, vp, cf, vp, vp]
     L.ll_keyframe_affine.argtypes = [C.POINTER(Pose), C.POINTER(Pose), vp, vp]
+    L.ll_keyframe_create.argtypes = [vp, C.POINTER(vp)]
+    L.ll_keyframe_release.argtypes = [vp]
+    L.ll_keyframe_append.argtypes = [vp, vp, vp, sz, ci, ci, vp, ci]
+    L.ll_keyframe_analyze.argtypes = [vp, vp, vp, ci, C.POINTER(KeyframeInfo)]
+    L.ll_keyframe_get_info.argtypes = [vp, C.POINTER(KeyframeInfo)]
+    L.ll_keyframe_cells.argtypes = [vp, vp, vp, vp, vp, vp, ci, C.POINTER(ci)]
+    L.ll_keyframe_images.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.ll_keyframe_cloud.argtypes = [vp, vp, ci, vp, sz, C.POINTER(sz), C.POINTER(vp)]
+    L.ll_loop_cfg_default.argtypes = [C.POINTER(LoopCfg)]
+    L.ll_loop_search.argtypes = [vp, vp, ci, ci, C.POINTER(LoopCfg), vp, vp, vp, C.POINTER(ci)]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64
     _LIB = L
     return L
+
+
+def default_loop_cfg(**kw) -> LoopCfg:
+    c = LoopCfg()
+    lib().ll_loop_cfg_default(C.byref(c))
+    for k, v in kw.items():
+        setattr(c, k, v)
+    return c
 
 
 def default_config(**kw) -> Config:

@@ -18,33 +18,11 @@
 #include "common.cuh"
 #include "kernels.cuh"
 #include "exact_math.cuh"
+#include "cellmap.cuh"
 
-#define CM_EMPTY 0xffffffffffffffffull
-#define CM_BIAS (1 << 20)             // cell indices -2^20 ... 2^20 - 1 fit the 21-bit fields of a key; an append rejects points beyond them
 #define CM_MAX_VOXELS_PER_CELL 512.0  // finest leaf an assembly accepts: cell size / 512 (see ll_cellmap_assemble)
 #define CM_VOXEL_BIAS 1024            // a cell's points lie within one cell of its lower corner: 512 voxels and this margin fit 13 bits
 
-struct ll_cellmap {
-  int device = 0;
-  float resolution = 0.5f;          // what set_resolution(r) stores: r / 2
-  int revisit_threshold = 2147483647;
-  int current_frame_idx = 0;
-  int n_pts = 0, cap_pts = 0;       // used / allocated entries of the point store (dead points included until the next rebuild)
-  int n_cells = 0;                  // cells after the last append (the first append into an empty map is set_point_cloud)
-  int n_out_of_range = 0;           // points rejected so far for a cell index beyond the key's range
-  int table_cap = 0;                // power of two
-  unsigned long long* keys = nullptr; int* last_update = nullptr; int* create_frame = nullptr; int* epoch = nullptr; int* bump = nullptr;
-  int* d_counters = nullptr;        // [0] number of cells, [1] scratch
-  float4* pts = nullptr; int* pt_slot = nullptr; int* pt_epoch = nullptr;
-  DevBuf table_buf, store_buf, store_alt, out_buf, tmp_buf;
-};
-
-__device__ __forceinline__ unsigned long long cm_pack(int k, int j, int i) {
-  return ((unsigned long long)(unsigned)(k + CM_BIAS) << 42) | ((unsigned long long)(unsigned)(j + CM_BIAS) << 21) | (unsigned long long)(unsigned)(i + CM_BIAS);
-}
-__device__ __forceinline__ void cm_unpack(unsigned long long key, int& k, int& j, int& i) {
-  k = (int)((key >> 42) & 0x1fffffull) - CM_BIAS; j = (int)((key >> 21) & 0x1fffffull) - CM_BIAS; i = (int)(key & 0x1fffffull) - CM_BIAS;
-}
 __device__ __forceinline__ unsigned cm_hash(unsigned long long key, unsigned mask) { return (unsigned)((key * 0x9E3779B97F4A7C15ull) >> 32) & mask; }
 
 // pass 1: cell lookup / creation for every new point (find_cell with if_add = 1)
@@ -386,7 +364,7 @@ int ll_cellmap_assemble(ll_ctx* ctx, ll_cellmap* m, const double q_wxyz[4], cons
     float4* np = st.pts; int* ns = st.slot; int* ne = st.epoch;
     cm_rebuild_kernel<<<ll_div_up(n_new > 0 ? n_new : 1, 256), 256, 0, s>>>(m->pts, m->pt_slot, m->pt_epoch, ikeep, cnt + 2, d_out, cslot, cnt + 3, m->epoch, np, ns, ne, cap_new);
     { DevBuf t = m->store_buf; m->store_buf = m->store_alt; m->store_alt = t; }   // stream-ordered: later work on this stream sees the new store
-    m->pts = np; m->pt_slot = ns; m->pt_epoch = ne; m->cap_pts = cap_new; m->n_pts = n_new;
+    m->pts = np; m->pt_slot = ns; m->pt_epoch = ne; m->cap_pts = cap_new; m->n_pts = n_new; m->generation++;
     ctx->launches++;
   }
   *n_out = (size_t)n_cen;
@@ -563,6 +541,6 @@ int cm_import(ll_ctx* ctx, ll_cellmap* m, int frame_idx, int n_out_of_range, con
   LL_CUDA(ctx, cudaMemcpyAsync(m->d_counters, c, sizeof(c), cudaMemcpyHostToDevice, s));
   LL_CUDA(ctx, cudaGetLastError());
   LL_CUDA(ctx, cudaStreamSynchronize(s));
-  m->n_pts = n_live; m->n_cells = n_cells; m->current_frame_idx = frame_idx; m->n_out_of_range = n_out_of_range;
+  m->n_pts = n_live; m->n_cells = n_cells; m->current_frame_idx = frame_idx; m->n_out_of_range = n_out_of_range; m->generation++;
   return LL_OK;
 }

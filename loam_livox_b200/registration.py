@@ -636,6 +636,21 @@ class Scene_alignment:
         self.scales_run = runs.value
         return res
 
+    def align_keyframes(self, keyframe_a: "Keyframe", keyframe_b: "Keyframe"):
+        """find_tranfrom_of_two_mappings(keyframe_a, keyframe_b) on the keyframes' device-resident typed clouds (scene_alignment.hpp:275-303):
+        source = a's line / plane cells, target = b's, t_init = (a.get_center() - b.get_center()) in float, then double."""
+        sl, nsl = keyframe_a.device_cloud(capi.LL_CELL_LINE)
+        sp, nsp = keyframe_a.device_cloud(capi.LL_CELL_PLANE)
+        tl, ntl = keyframe_b.device_cloud(capi.LL_CELL_LINE)
+        tp, ntp = keyframe_b.device_cloud(capi.LL_CELL_PLANE)
+        self.cfg.t_init[:] = [float(v) for v in (keyframe_a.get_center() - keyframe_b.get_center()).astype(np.float32)]
+        res, runs = capi.RegResult(), C.c_int()
+        self.ctx.check(self.ctx._lib.ll_scene_align(self.ctx.h, sl, nsl, sp, nsp, tl, ntl, tp, ntp, capi.LL_FMT_XYZI16, capi.LL_DEVICE, C.byref(self.cfg),
+                                                    C.byref(res), C.byref(runs)))
+        self.m_q_w_curr, self.m_t_w_curr = np.array(res.q_w_curr), np.array(res.t_w_curr)
+        self.scales_run = runs.value
+        return res
+
 
 def pg_edges(id_begin, id_end, q_wxyz, t, information=None):
     """An array of capi.PgEdge (Ceres_pose_graph_3d::Constraint3d): information defaults to the identity, as the reference always passes."""
@@ -766,6 +781,95 @@ class Points_cloud_map:
         self.ctx.check(self.ctx._lib.ll_cellmap_assemble(self.ctx.h, self.h, q.ctypes.data, t.ctypes.data, float(search_range), float(fov_angle), float(leaf), int(bool(replace)),
                                                          out.ctypes.data, cap, C.byref(n), C.byref(nf), C.byref(dev)))
         return out[:n.value].copy(), nf.value
+
+
+class Keyframe:
+    """Maps_keyframe<float> over the cells of a full-resolution Points_cloud_map (loam_livox/source/cell_map_keyframe.hpp:1002-1494): cells
+    from append (laser_mapping.hpp:1527-1533), analyze() for the types, centre, ROI range and feature images, the typed clouds on the device."""
+
+    def __init__(self, ctx: Context):
+        self.ctx = ctx
+        h = C.c_void_p()
+        ctx.check(ctx._lib.ll_keyframe_create(ctx.h, C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx._lib.ll_keyframe_release(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def append(ctx: Context, cellmap: "Points_cloud_map", pts, open_keyframes):
+        """append_cloud(pts, &cell_vec) on the cell map, then add_cells(cell_vec) on every open keyframe."""
+        pts, fmt = _pts(pts)
+        hs = (C.c_void_p * max(len(open_keyframes), 1))(*[k.h for k in open_keyframes])
+        ctx.check(ctx._lib.ll_keyframe_append(ctx.h, cellmap.h, pts.ctypes.data, pts.shape[0], fmt, capi.LL_HOST, hs, len(open_keyframes)))
+
+    def analyze(self, cellmap: "Points_cloud_map", incremental_cov: bool = False) -> capi.KeyframeInfo:
+        info = capi.KeyframeInfo()
+        self.ctx.check(self.ctx._lib.ll_keyframe_analyze(self.ctx.h, cellmap.h, self.h, int(bool(incremental_cov)), C.byref(info)))
+        return info
+
+    def info(self) -> capi.KeyframeInfo:
+        info = capi.KeyframeInfo()
+        if self.ctx._lib.ll_keyframe_get_info(self.h, C.byref(info)) != capi.LL_OK:
+            raise LoamLivoxError("keyframe not analyzed since its last append")
+        return info
+
+    def get_center(self):
+        return np.array(self.info().center, np.float32)
+
+    def cells(self, analyzed: bool = True):
+        """(keys uint64, incarnations, types, feature vectors [n, 3]) in the keyframe's cell order; types / vectors need an analysis."""
+        n = C.c_int()
+        self.ctx.check(self.ctx._lib.ll_keyframe_cells(self.ctx.h, self.h, None, None, None, None, 0, C.byref(n)))
+        k, e = np.zeros(n.value, np.uint64), np.zeros(n.value, np.int32)
+        t, v = np.zeros(n.value, np.int32), np.zeros((n.value, 3), np.float32)
+        self.ctx.check(self.ctx._lib.ll_keyframe_cells(self.ctx.h, self.h, k.ctypes.data, e.ctypes.data, t.ctypes.data if analyzed else None,
+                                                       v.ctypes.data if analyzed else None, n.value, C.byref(n)))
+        return k, e, t, v
+
+    def images(self):
+        """[4, 60, 60]: line counts, plane counts (before the blur), blurred line image, blurred plane image."""
+        out = np.zeros((4, 60, 60), np.float32)
+        self.ctx.check(self.ctx._lib.ll_keyframe_images(self.ctx.h, self.h, *[out[i].ctypes.data for i in range(4)]))
+        return out
+
+    def extract_specify_points(self, which: int):
+        """which = capi.LL_CELL_LINE / LL_CELL_PLANE / LL_CELL_ALL -> n x 4 float32 (intensity 0)."""
+        n, dev = C.c_size_t(), C.c_void_p()
+        self.ctx.check(self.ctx._lib.ll_keyframe_cloud(self.ctx.h, self.h, which, None, 0, C.byref(n), C.byref(dev)))
+        out = np.zeros((n.value, 4), np.float32)
+        self.ctx.check(self.ctx._lib.ll_keyframe_cloud(self.ctx.h, self.h, which, out.ctypes.data, n.value, C.byref(n), C.byref(dev)))
+        return out
+
+    def get_all_pointcloud(self):
+        return self.extract_specify_points(capi.LL_CELL_ALL)
+
+    def device_cloud(self, which: int):
+        """(device pointer, point count) of a typed cloud, for ll_scene_align with LL_DEVICE."""
+        n, dev = C.c_size_t(), C.c_void_p()
+        self.ctx.check(self.ctx._lib.ll_keyframe_cloud(self.ctx.h, self.h, which, None, 0, C.byref(n), C.byref(dev)))
+        return dev.value, n.value
+
+
+def loop_search(ctx: Context, keyframes, newest: int = -1, cfg: capi.LoopCfg = None):
+    """service_loop_detection's candidate search (laser_mapping.hpp:988-1033) for keyframes[newest] against every earlier keyframe:
+    (sim_plane [newest], sim_line [newest], candidate indices ascending)."""
+    n = len(keyframes)
+    newest = n - 1 if newest < 0 else newest
+    cfg = cfg if cfg is not None else capi.default_loop_cfg()
+    hs = (C.c_void_p * max(n, 1))(*[k.h for k in keyframes])
+    sp, sl, cand = np.zeros(max(newest, 1), np.float32), np.zeros(max(newest, 1), np.float32), np.zeros(max(newest, 1), np.int32)
+    nc = C.c_int()
+    ctx.check(ctx._lib.ll_loop_search(ctx.h, hs, n, newest, C.byref(cfg), sp.ctypes.data, sl.ctypes.data, cand.ctypes.data, C.byref(nc)))
+    return sp[:newest], sl[:newest], cand[:nc.value].tolist()
 
 
 class SequenceError(LoamLivoxError):
