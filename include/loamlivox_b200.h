@@ -329,7 +329,8 @@ void ll_mapper_config_default(ll_mapper_config* cfg);
 int  ll_mapper_create(ll_ctx* ctx, const ll_mapper_config* cfg, ll_mapper** out);
 void ll_mapper_release(ll_mapper* mapper);
 /* One raw scan through process_new_scan (laser_mapping.hpp:1316-1521): features, match-map refresh from the cell maps, registration
- * (out->status 1 accepted/skipped, 0 rejected and discarded), world-frame features appended to the cell maps, pose adopted. */
+ * (out->status 1 accepted/skipped, 0 rejected and discarded), world-frame features appended to the cell maps, pose adopted.
+ * LL_ERR_INVALID for an unknown fmt or where or a null raw of n > 0 points, LL_ERR_CAPACITY for n over max_scan_points: nothing changed. */
 int  ll_mapper_process_scan(ll_mapper* mapper, const void* raw, size_t n, int fmt, int where, double stamp, ll_reg_result* out, ll_mapper_stats* stats);
 /* One sensor frame through Laser_feature::laserCloudHandler and, for every piece it publishes, Laser_mapping::process_new_scan
  * (laser_feature_extractor.hpp:305-389, laser_mapping.hpp:1316-1521): what the shipped configs run (common/odom_mode 1, if_motion_deblur 0).
@@ -339,7 +340,8 @@ int  ll_mapper_process_scan(ll_mapper* mapper, const void* raw, size_t n, int fm
  * read); piece i's features are the piece-i clouds of the contributing heads in head order, down-sampled by the extractor's and the mapping
  * node's VoxelGrids.  odom_mode 1 registers every piece as a scan of its own (frame index, time-stamp range, map refresh, append and pose
  * adoption per piece), 0 only piece 0.  out / stats (stats may be NULL) receive one entry per published piece; cap is their length.
- * LL_ERR_INVALID (nothing changed) for odom_mode outside {0, 1}, pieces outside 1 ... 16 or cap below the pieces to publish;
+ * LL_ERR_INVALID (nothing changed) for odom_mode outside {0, 1}, pieces outside 1 ... 16, cap below the pieces to publish, an unknown
+ * fmt or where or a null cloud of points;
  * LL_ERR_CAPACITY up front when the heads exceed max_scan_points, and before piece i's registration when its features exceed max_features
  * (*n_pieces then counts the pieces completed, whose entries are valid). */
 #define LL_MAX_PIECES_PER_FRAME 16

@@ -162,8 +162,8 @@ struct SyncEvents {
   cudaEvent_t fork = nullptr, join = nullptr;     // stream <-> stream2
   cudaEvent_t fork3 = nullptr, join3 = nullptr;   // stream <-> stream3
   cudaEvent_t it[2] = {nullptr, nullptr};         // ICP iteration `it` has been snapshot into PinnedStage::snap[it & 1]
-  // the sequence calls' front end (ll_ctx::fe_stream): fork / join of its own three streams, `ready` behind a whole front end, and `free[a]`
-  // behind the last copy of an input's features out of the front end's buffers (scans: [0], tmp_a / tmp_b; frames: [arena])
+  // fork / join of the sequence calls' front-end streams (ll_ctx::fe_stream); and the streaming mapper's input loop: `ready` behind a whole
+  // front end, and `free[a]` behind the last copy of an input's features out of the front end's buffers (scans: [0], tmp_a / tmp_b; frames: [arena])
   cudaEvent_t fe_fork = nullptr, fe_join = nullptr, fe_fork3 = nullptr, fe_join3 = nullptr, fe_ready = nullptr, fe_free[2] = {nullptr, nullptr};
   template <typename F> void each(F&& f) {
     for (cudaEvent_t* e : {&fork, &join, &fork3, &join3, &it[0], &it[1], &fe_fork, &fe_join, &fe_fork3, &fe_join3, &fe_ready, &fe_free[0], &fe_free[1]}) f(*e);

@@ -317,32 +317,8 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
   return LL_OK;
 }
 
-// One scan: features -> mapper_step.
-int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int where, double stamp, ll_reg_result* out, ll_mapper_stats* stats) {
-  if (!m || !out) return LL_ERR_INVALID;
-  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
-  if (stats) memset(stats, 0, sizeof(*stats));
-  const double tp = now_ms();
-  int nc = 0, ns = 0, dropped = 0;
-  LL_TRY(scan_front_end(ctx, raw, n, fmt, where, stamp, &m->cfg.pipeline, &nc, &ns, &dropped));
-  out_init(m, out);
-  if (stats) { stats->n_corner = nc; stats->n_surf = ns; stats->ms_front_end = (float)(now_ms() - tp); }
-  if (dropped) return LL_OK;                                                     // laser_feature_extractor.hpp:287
-  return mapper_step(m, nc, ns, (double)ctx->last_full_max_t, out, stats);
-}
-
 }  // extern "C"
 
-// The pieces a frame is cut into and the entries it publishes; LL_ERR_INVALID for a bad odom_mode, pieces or cap.
-static int frame_publish(ll_mapper* m, int odom_mode, int cap, int* pieces, int* publish) {
-  ll_ctx* ctx = m->ctx;
-  *pieces = m->cfg.reg.if_motion_deblur ? 1 : m->cfg.pipeline.pieces;   // laser_feature_extractor.hpp:305-309
-  if (*pieces < 1 || *pieces > m->frame_pieces) { ctx->set_error("pieces must be 1 ... 16"); return LL_ERR_INVALID; }
-  if (odom_mode != 0 && odom_mode != 1) { ctx->set_error("odom_mode must be 0 or 1"); return LL_ERR_INVALID; }
-  *publish = odom_mode ? *pieces : 1;                                            // :385-388
-  if (cap < *publish) { ctx->set_error("cap smaller than the pieces to publish"); return LL_ERR_INVALID; }
-  return LL_OK;
-}
 static int frame_arena(ll_mapper* m, int a, FrameArena* fa) {
   ll_ctx* ctx = m->ctx;
   const int cap = m->frame_pieces * ctx->cfg.max_scan_points;
@@ -359,70 +335,19 @@ static int first_piece_over(const ll_mapper* m, const FrameOut& fo, int publish)
   return publish;
 }
 
-// The published pieces of a frame whose front end has completed (fo: its read-back; fa: its arena): per piece its features into A.feat and
-// mapper_step.  A rejected piece leaves the pose as it was, and the next piece continues from there.  `copied` runs once piece 0's features
-// are enqueued for copying; free_ev (may be null) is recorded behind the last copy out of `fa`.
-template <typename F>
-static int frame_pieces(ll_mapper* m, const FrameArena& fa, const FrameOut& fo, int publish, float ms_front_end, ll_reg_result* out, ll_mapper_stats* stats,
-                        int* n_pieces, cudaEvent_t free_ev, F&& copied) {
-  ll_ctx* ctx = m->ctx;
-  for (int i = 0; i < publish; i++) {
-    const int c0 = i ? fo.out_end[0][i - 1] : 0, s0 = i ? fo.out_end[1][i - 1] : 0;
-    const int nc = fo.out_end[0][i] - c0, nsf = fo.out_end[1][i] - s0;
-    ll_mapper_stats* st = stats ? stats + i : nullptr;
-    if (st) { memset(st, 0, sizeof(*st)); st->n_corner = nc; st->n_surf = nsf; st->ms_front_end = i == 0 ? ms_front_end : 0.f; }
-    out_init(m, out + i);
-    if (nc + nsf > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
-    LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat, fa.cls[0] + c0, (size_t)nc * 16, cudaMemcpyDeviceToDevice, ctx->stream));
-    LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat + nc, fa.cls[1] + s0, (size_t)nsf * 16, cudaMemcpyDeviceToDevice, ctx->stream));
-    if (free_ev && i == publish - 1) LL_CUDA(ctx, cudaEventRecord(free_ev, ctx->stream));
-    if (i == 0) LL_TRY(copied());
-    LL_TRY(mapper_step(m, nc, nsf, (double)ll_ord2f(fo.tmax[i]), out + i, st));
-    *n_pieces = i + 1;
-  }
-  return LL_OK;
-}
-
-// One frame: the piecewise front end (every head, every piece, one host read), then per published piece its features into A.feat and
-// mapper_step.
-extern "C" int ll_mapper_process_frame(ll_mapper* m, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
-                                       int odom_mode, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces) {
-  if (!m || !out || !raws || !ns || !stamps || !n_pieces || n_heads < 1 || n_heads > LL_MAX_HEADS) return LL_ERR_INVALID;
-  *n_pieces = 0;
-  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
-  int pieces = 0, publish = 0;
-  LL_TRY(frame_publish(m, odom_mode, cap, &pieces, &publish));
-  size_t total = 0;
-  for (int h = 0; h < n_heads; h++) { if (!raws[h] && ns[h]) return LL_ERR_INVALID; total += ns[h]; }
-  if (total > (size_t)ctx->cfg.max_scan_points) { ctx->set_error("frame (all heads) larger than max_scan_points"); return LL_ERR_CAPACITY; }
-  const double tp = now_ms();
-  FrameArena fa; LL_TRY(frame_arena(m, 0, &fa));
-  LL_TRY(frame_front_end(ctx, ctx->own_front(), fa, n_heads, raws, ns, fmt, where, stamps, pieces, &m->cfg.pipeline));
-  LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  const FrameOut fo = ctx->pin->frame;
-  const float ms_front_end = (float)(now_ms() - tp);
-  if (fo.heads_live == 0) return LL_OK;                                          // laser_feature_extractor.hpp:287, every head
-  return frame_pieces(m, fa, fo, publish, ms_front_end, out, stats, n_pieces, nullptr, [] { return LL_OK; });
-}
-
-// ---------------------------------------------------------------------------------------------- sequences
-// The front end of input k + 1 is enqueued on the context's front-end streams (ll_ctx::fe_stream) before the mapper step(s) of input k, so it
-// runs under them.  Nothing the mapper step reads or writes is touched by the front end, whose results only reach the mapper through the copy
-// into A.feat; the extractor's host bookkeeping advances in input order.  So every result is the one-by-one calls'.
+// ---------------------------------------------------------------------------------------------- the input loop
+// ll_mapper_process_scans / _frames: the front end of input k + 1 is enqueued on the streams `fs` (ll_ctx::fe_stream) before the mapper
+// step(s) of input k, so it runs under them.  Nothing the mapper step reads or writes is touched by the front end, whose results only reach the
+// mapper through the copy into A.feat; the extractor's host bookkeeping advances in input order.  So a sequence gives the results of its inputs
+// called one at a time.  ll_mapper_process_scan / _frame are the loops of one input on the context's own streams (ll_ctx::own_front): their
+// front end keeps the greatest priority, as every other call of the context, and nothing is enqueued ahead.
 //
 // A front end enqueued ahead of an input that then fails: it is drained (it reads the caller's inputs) and its host bookkeeping undone, so that
 // the extractor stands where the one-by-one calls leave it.
 struct Ahead { ExtractState saved; bool on = false; };
-static void sequence_unwind(ll_ctx* ctx, const Ahead& a) {
-  const FrontStreams fs = ctx->pipe_front();
+static void sequence_unwind(ll_ctx* ctx, const FrontStreams& fs, const Ahead& a) {
   for (cudaStream_t s : {fs.main, fs.corner, fs.petals}) cudaStreamSynchronize(s);
   if (a.on) ctx->ex = a.saved;
-}
-static int check_format(ll_ctx* ctx, int fmt, int where) {
-  if ((fmt != LL_FMT_XYZI16 && fmt != LL_FMT_PCL32 && fmt != LL_FMT_STRIDED) || (where != LL_HOST && where != LL_DEVICE)) {
-    ctx->set_error("unknown point format or memory kind"); return LL_ERR_INVALID;
-  }
-  return LL_OK;
 }
 // Host records are staged in stage_in: reserved for max_scan_points records before the first front end, because a reallocation (cudaFree)
 // would synchronise the device in the middle of the sequence.
@@ -433,10 +358,44 @@ static int reserve_stage(ll_ctx* ctx, int fmt, int where) {
   return LL_OK;
 }
 
-static int frames_run(ll_mapper* m, int n_frames, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
-                      int pieces, int publish, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces, int* done, Ahead& ahead) {
+// Argument checks, before anything is enqueued or the extractor's bookkeeping moves: LL_ERR_INVALID for an unknown format or memory kind or a
+// null cloud of points (n clouds), LL_ERR_CAPACITY for an input over max_scan_points.
+static int check_clouds(ll_ctx* ctx, int fmt, int where, size_t n, const void* const* raws, const size_t* ns) {
+  if ((fmt != LL_FMT_XYZI16 && fmt != LL_FMT_PCL32 && fmt != LL_FMT_STRIDED) || (where != LL_HOST && where != LL_DEVICE)) {
+    ctx->set_error("unknown point format or memory kind"); return LL_ERR_INVALID;
+  }
+  for (size_t k = 0; k < n; k++) if (!raws[k] && ns[k]) { ctx->set_error("null cloud of " + std::to_string(ns[k]) + " points"); return LL_ERR_INVALID; }
+  return LL_OK;
+}
+static int scans_check(ll_ctx* ctx, int n_scans, const void* const* raws, const size_t* ns, int fmt, int where) {
+  LL_TRY(check_clouds(ctx, fmt, where, (size_t)n_scans, raws, ns));
+  for (int k = 0; k < n_scans; k++) if (ns[k] > (size_t)ctx->cfg.max_scan_points) { ctx->set_error("scan " + std::to_string(k) + " larger than max_scan_points"); return LL_ERR_CAPACITY; }
+  return LL_OK;
+}
+// Frames also give the pieces a frame is cut into and the entries it publishes; LL_ERR_INVALID for a bad odom_mode, pieces or cap.
+static int frames_check(ll_mapper* m, int n_frames, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, int odom_mode, int cap,
+                        int* pieces, int* publish) {
   ll_ctx* ctx = m->ctx;
-  const FrontStreams fs = ctx->pipe_front();
+  *pieces = m->cfg.reg.if_motion_deblur ? 1 : m->cfg.pipeline.pieces;   // laser_feature_extractor.hpp:305-309
+  if (*pieces < 1 || *pieces > m->frame_pieces) { ctx->set_error("pieces must be 1 ... 16"); return LL_ERR_INVALID; }
+  if (odom_mode != 0 && odom_mode != 1) { ctx->set_error("odom_mode must be 0 or 1"); return LL_ERR_INVALID; }
+  *publish = odom_mode ? *pieces : 1;                                            // :385-388
+  if (cap < *publish) { ctx->set_error("cap smaller than the pieces to publish"); return LL_ERR_INVALID; }
+  LL_TRY(check_clouds(ctx, fmt, where, (size_t)n_frames * n_heads, raws, ns));
+  for (int f = 0; f < n_frames; f++) {
+    size_t total = 0; for (int h = 0; h < n_heads; h++) total += ns[(size_t)f * n_heads + h];
+    if (total > (size_t)ctx->cfg.max_scan_points) { ctx->set_error("frame " + std::to_string(f) + " (all heads) larger than max_scan_points"); return LL_ERR_CAPACITY; }
+  }
+  return LL_OK;
+}
+
+// Frame f: the piecewise front end (every head, every piece, one host read) into arena f & 1, then per published piece its features into
+// A.feat and mapper_step.  A rejected piece leaves the pose as it was, and the next piece continues from there.
+static int frames_run(ll_mapper* m, const FrontStreams& fs, int n_frames, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where,
+                      const double* stamps, int pieces, int publish, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces, int* done) {
+  ll_ctx* ctx = m->ctx;
+  LL_TRY(reserve_stage(ctx, fmt, where));
+  for (int f = 0; f < n_frames; f++) n_pieces[f] = 0;
   FrameArena fa[2]; LL_TRY(frame_arena(m, 0, &fa[0])); LL_TRY(frame_arena(m, 1, &fa[1]));
   auto enqueue = [&](int f) -> int {   // frame f's front end into arena f & 1, behind the last copy out of it (frame f - 2's)
     const size_t o = (size_t)f * n_heads;
@@ -445,31 +404,59 @@ static int frames_run(ll_mapper* m, int n_frames, int n_heads, const void* const
     LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_ready, fs.main));
     return LL_OK;
   };
-  double t = now_ms();
-  LL_TRY(enqueue(0));
-  float ms_enqueue = (float)(now_ms() - t);
-  for (int f = 0; f < n_frames; f++) {
-    ahead.on = false;
-    t = now_ms();
-    LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.fe_ready));
-    const FrameOut fo = ctx->pin->frame;   // read before the next front end is enqueued (PinnedStage)
-    const float ms_front_end = ms_enqueue + (float)(now_ms() - t);
-    // the next front end goes under this frame's steps unless one of its pieces will stop the sequence
-    const bool next = f + 1 < n_frames && (fo.heads_live == 0 || first_piece_over(m, fo, publish) == publish);
-    auto enqueue_next = [&]() -> int {
-      if (!next) return LL_OK;
-      ahead.saved = ctx->ex; ahead.on = true;
-      const double t1 = now_ms();
-      LL_TRY(enqueue(f + 1));
-      ms_enqueue = (float)(now_ms() - t1);
-      return LL_OK;
-    };
-    if (fo.heads_live == 0) LL_TRY(enqueue_next());                             // laser_feature_extractor.hpp:287, every head
-    else LL_TRY(frame_pieces(m, fa[f & 1], fo, publish, ms_front_end, out + (size_t)f * cap, stats ? stats + (size_t)f * cap : nullptr, &n_pieces[f],
-                             ctx->sev.fe_free[f & 1], enqueue_next));
-    *done = f + 1;
-  }
-  return LL_OK;
+  Ahead ahead;
+  const int st = [&]() -> int {
+    double t = now_ms();
+    LL_TRY(enqueue(0));
+    float ms_enqueue = (float)(now_ms() - t);
+    for (int f = 0; f < n_frames; f++) {
+      ahead.on = false;
+      t = now_ms();
+      LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.fe_ready));
+      const FrameOut fo = ctx->pin->frame;   // read before the next front end is enqueued (PinnedStage)
+      const float ms_front_end = ms_enqueue + (float)(now_ms() - t);
+      // the next front end goes under this frame's steps unless one of its pieces will stop the sequence
+      const bool next = f + 1 < n_frames && (fo.heads_live == 0 || first_piece_over(m, fo, publish) == publish);
+      auto enqueue_next = [&]() -> int {
+        if (!next) return LL_OK;
+        ahead.saved = ctx->ex; ahead.on = true;
+        const double t1 = now_ms();
+        LL_TRY(enqueue(f + 1));
+        ms_enqueue = (float)(now_ms() - t1);
+        return LL_OK;
+      };
+      if (fo.heads_live == 0) LL_TRY(enqueue_next());                           // laser_feature_extractor.hpp:287, every head
+      for (int i = 0; fo.heads_live != 0 && i < publish; i++) {
+        const int c0 = i ? fo.out_end[0][i - 1] : 0, s0 = i ? fo.out_end[1][i - 1] : 0;
+        const int nc = fo.out_end[0][i] - c0, nsf = fo.out_end[1][i] - s0;
+        ll_reg_result* o = out + (size_t)f * cap + i;
+        ll_mapper_stats* ps = stats ? stats + (size_t)f * cap + i : nullptr;
+        if (ps) { memset(ps, 0, sizeof(*ps)); ps->n_corner = nc; ps->n_surf = nsf; ps->ms_front_end = i == 0 ? ms_front_end : 0.f; }
+        out_init(m, o);
+        if (nc + nsf > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
+        LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat, fa[f & 1].cls[0] + c0, (size_t)nc * 16, cudaMemcpyDeviceToDevice, ctx->stream));
+        LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat + nc, fa[f & 1].cls[1] + s0, (size_t)nsf * 16, cudaMemcpyDeviceToDevice, ctx->stream));
+        if (i == publish - 1) LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[f & 1], ctx->stream));
+        if (i == 0) LL_TRY(enqueue_next());
+        LL_TRY(mapper_step(m, nc, nsf, (double)ll_ord2f(fo.tmax[i]), o, ps));
+        n_pieces[f] = i + 1;
+      }
+      *done = f + 1;
+    }
+    return LL_OK;
+  }();
+  if (st != LL_OK) sequence_unwind(ctx, fs, ahead);
+  return st;
+}
+
+extern "C" int ll_mapper_process_frame(ll_mapper* m, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+                                       int odom_mode, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces) {
+  if (!m || !out || !raws || !ns || !stamps || !n_pieces || n_heads < 1 || n_heads > LL_MAX_HEADS) return LL_ERR_INVALID;
+  *n_pieces = 0;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  int pieces = 0, publish = 0, done = 0;
+  LL_TRY(frames_check(m, 1, n_heads, raws, ns, fmt, where, odom_mode, cap, &pieces, &publish));
+  return frames_run(m, ctx->own_front(), 1, n_heads, raws, ns, fmt, where, stamps, pieces, publish, out, stats, cap, n_pieces, &done);
 }
 
 extern "C" int ll_mapper_process_frames(ll_mapper* m, int n_frames, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where,
@@ -478,59 +465,60 @@ extern "C" int ll_mapper_process_frames(ll_mapper* m, int n_frames, int n_heads,
   if (!m || !out || !raws || !ns || !stamps || !n_pieces || !n_frames_done || n_frames < 1 || n_heads < 1 || n_heads > LL_MAX_HEADS) return LL_ERR_INVALID;
   ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
   int pieces = 0, publish = 0;
-  LL_TRY(frame_publish(m, odom_mode, cap, &pieces, &publish));
-  LL_TRY(check_format(ctx, fmt, where));
-  const size_t n_in = (size_t)n_frames * n_heads;
-  for (size_t k = 0; k < n_in; k++) if (!raws[k] && ns[k]) { ctx->set_error("null cloud of " + std::to_string(ns[k]) + " points"); return LL_ERR_INVALID; }
-  for (int f = 0; f < n_frames; f++) {
-    size_t total = 0; for (int h = 0; h < n_heads; h++) total += ns[(size_t)f * n_heads + h];
-    if (total > (size_t)ctx->cfg.max_scan_points) { ctx->set_error("frame " + std::to_string(f) + " (all heads) larger than max_scan_points"); return LL_ERR_CAPACITY; }
-  }
-  LL_TRY(reserve_stage(ctx, fmt, where));
-  for (int f = 0; f < n_frames; f++) n_pieces[f] = 0;
-  Ahead ahead; int done = 0;
-  const int st = frames_run(m, n_frames, n_heads, raws, ns, fmt, where, stamps, pieces, publish, out, stats, cap, n_pieces, &done, ahead);
-  if (st != LL_OK) sequence_unwind(ctx, ahead);
-  *n_frames_done = done;
-  return st;
+  LL_TRY(frames_check(m, n_frames, n_heads, raws, ns, fmt, where, odom_mode, cap, &pieces, &publish));
+  return frames_run(m, ctx->pipe_front(), n_frames, n_heads, raws, ns, fmt, where, stamps, pieces, publish, out, stats, cap, n_pieces, n_frames_done);
 }
 
-static int scans_run(ll_mapper* m, int n_scans, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps, ll_reg_result* out,
-                     ll_mapper_stats* stats, int* done, Ahead& ahead) {
+// Scan k: the front end, its features into A.feat (scan_front_end_finish) and mapper_step.
+static int scans_run(ll_mapper* m, const FrontStreams& fs, int n_scans, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+                     ll_reg_result* out, ll_mapper_stats* stats, int* done) {
   ll_ctx* ctx = m->ctx;
-  const FrontStreams fs = ctx->pipe_front();
   const ll_pipeline_cfg* pc = &m->cfg.pipeline;
+  LL_TRY(reserve_stage(ctx, fmt, where));
   auto enqueue = [&](int k) -> int {   // behind the copy of scan k - 1's features out of tmp_a / tmp_b
     LL_CUDA(ctx, cudaStreamWaitEvent(fs.main, ctx->sev.fe_free[0], 0));
     LL_TRY(scan_front_end_enqueue(ctx, fs, raws[k], ns[k], fmt, where, stamps[k], pc));
     LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_ready, fs.main));
     return LL_OK;
   };
-  double t = now_ms();
-  LL_TRY(enqueue(0));
-  float ms_enqueue = (float)(now_ms() - t);
-  for (int k = 0; k < n_scans; k++) {
-    ahead.on = false;
-    ll_mapper_stats* st = stats ? stats + k : nullptr;
-    if (st) memset(st, 0, sizeof(*st));
-    t = now_ms();
-    LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.fe_ready));
-    int nc = 0, nsf = 0, dropped = 0;
-    LL_TRY(scan_front_end_finish(ctx, ctx->stream, pc, &nc, &nsf, &dropped));   // reads the pinned counts before the next front end is enqueued
-    LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[0], ctx->stream));
-    const float ms_front_end = ms_enqueue + (float)(now_ms() - t);
-    if (k + 1 < n_scans) {
-      ahead.saved = ctx->ex; ahead.on = true;
-      const double t1 = now_ms();
-      LL_TRY(enqueue(k + 1));
-      ms_enqueue = (float)(now_ms() - t1);
+  Ahead ahead;
+  const int st = [&]() -> int {
+    double t = now_ms();
+    LL_TRY(enqueue(0));
+    float ms_enqueue = (float)(now_ms() - t);
+    for (int k = 0; k < n_scans; k++) {
+      ahead.on = false;
+      ll_mapper_stats* ps = stats ? stats + k : nullptr;
+      if (ps) memset(ps, 0, sizeof(*ps));
+      t = now_ms();
+      LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.fe_ready));
+      int nc = 0, nsf = 0, dropped = 0;
+      LL_TRY(scan_front_end_finish(ctx, ctx->stream, pc, &nc, &nsf, &dropped));   // reads the pinned counts before the next front end is enqueued
+      LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[0], ctx->stream));
+      const float ms_front_end = ms_enqueue + (float)(now_ms() - t);
+      if (k + 1 < n_scans) {
+        ahead.saved = ctx->ex; ahead.on = true;
+        const double t1 = now_ms();
+        LL_TRY(enqueue(k + 1));
+        ms_enqueue = (float)(now_ms() - t1);
+      }
+      out_init(m, out + k);
+      if (ps) { ps->n_corner = nc; ps->n_surf = nsf; ps->ms_front_end = ms_front_end; }
+      if (!dropped) LL_TRY(mapper_step(m, nc, nsf, (double)ctx->last_full_max_t, out + k, ps));   // laser_feature_extractor.hpp:287
+      *done = k + 1;
     }
-    out_init(m, out + k);
-    if (st) { st->n_corner = nc; st->n_surf = nsf; st->ms_front_end = ms_front_end; }
-    if (!dropped) LL_TRY(mapper_step(m, nc, nsf, (double)ctx->last_full_max_t, out + k, st));   // laser_feature_extractor.hpp:287
-    *done = k + 1;
-  }
-  return LL_OK;
+    return LL_OK;
+  }();
+  if (st != LL_OK) sequence_unwind(ctx, fs, ahead);
+  return st;
+}
+
+extern "C" int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int where, double stamp, ll_reg_result* out, ll_mapper_stats* stats) {
+  if (!m || !out) return LL_ERR_INVALID;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  int done = 0;
+  LL_TRY(scans_check(ctx, 1, &raw, &n, fmt, where));
+  return scans_run(m, ctx->own_front(), 1, &raw, &n, fmt, where, &stamp, out, stats, &done);
 }
 
 extern "C" int ll_mapper_process_scans(ll_mapper* m, int n_scans, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
@@ -538,15 +526,8 @@ extern "C" int ll_mapper_process_scans(ll_mapper* m, int n_scans, const void* co
   if (n_scans_done) *n_scans_done = 0;
   if (!m || !out || !raws || !ns || !stamps || !n_scans_done || n_scans < 1) return LL_ERR_INVALID;
   ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
-  LL_TRY(check_format(ctx, fmt, where));
-  for (int k = 0; k < n_scans; k++) if (!raws[k] && ns[k]) { ctx->set_error("null cloud of " + std::to_string(ns[k]) + " points"); return LL_ERR_INVALID; }
-  for (int k = 0; k < n_scans; k++) if (ns[k] > (size_t)ctx->cfg.max_scan_points) { ctx->set_error("scan " + std::to_string(k) + " larger than max_scan_points"); return LL_ERR_CAPACITY; }
-  LL_TRY(reserve_stage(ctx, fmt, where));
-  Ahead ahead; int done = 0;
-  const int st = scans_run(m, n_scans, raws, ns, fmt, where, stamps, out, stats, &done, ahead);
-  if (st != LL_OK) sequence_unwind(ctx, ahead);
-  *n_scans_done = done;
-  return st;
+  LL_TRY(scans_check(ctx, n_scans, raws, ns, fmt, where));
+  return scans_run(m, ctx->pipe_front(), n_scans, raws, ns, fmt, where, stamps, out, stats, n_scans_done);
 }
 
 // ---------------------------------------------------------------------------------------------- checkpoint

@@ -917,27 +917,16 @@ class Laser_mapping:
             pass
 
     def process_new_scan(self, raw, stamp, where=capi.LL_HOST, n=None, fmt=None):
-        if where == capi.LL_HOST:
-            pts, fmt = _pts(raw)
-            ptr, n = pts.ctypes.data, pts.shape[0]
-        else:
-            ptr = int(raw)
+        ptrs, sizes, fmt, _keep = self._clouds([raw], where, None if n is None else [n], fmt)
         res, stats = capi.RegResult(), capi.MapperStats()
-        self.ctx.check(self.ctx._lib.ll_mapper_process_scan(self.h, ptr, n, fmt, where, float(stamp), C.byref(res), C.byref(stats)))
+        self.ctx.check(self.ctx._lib.ll_mapper_process_scan(self.h, ptrs[0], sizes[0], fmt, where, float(stamp), C.byref(res), C.byref(stats)))
         return res, stats
 
     def process_new_frame(self, heads, stamps, odom_mode=1, where=capi.LL_HOST, ns=None, fmt=None):
         """One sensor frame (a list of raw clouds, one per head; Mid-100: 3) cut into pieces, every piece registered as a scan of its own
         (odom_mode 1, the shipped configs; 0: piece 0 only).  Returns a list of (RegResult, MapperStats), one per published piece."""
         k = len(heads)
-        if where == capi.LL_HOST:
-            arrs = [_pts(h) for h in heads]
-            fmt = arrs[0][1] if arrs else capi.LL_FMT_XYZI16
-            ptrs = (C.c_void_p * k)(*[a.ctypes.data for a, _ in arrs])
-            sizes = (C.c_size_t * k)(*[a.shape[0] for a, _ in arrs])
-        else:
-            ptrs = (C.c_void_p * k)(*[int(h) for h in heads])
-            sizes = (C.c_size_t * k)(*[int(n) for n in ns])
+        ptrs, sizes, fmt, _keep = self._clouds(heads, where, ns, fmt)
         st = (C.c_double * k)(*[float(t) for t in stamps])
         cap = capi.LL_MAX_PIECES_PER_FRAME
         res, stats, n = (capi.RegResult * cap)(), (capi.MapperStats * cap)(), C.c_int()

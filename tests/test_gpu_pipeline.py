@@ -1,7 +1,8 @@
 """The sequence calls of the streaming mapper (ll_mapper_process_frames / _scans: the front end of input k + 1 runs on the device while input k
-is registered) against the same inputs run one by one (ll_mapper_process_frame / _scan) on a mapper and context of their own: every
-ll_reg_result field but the gpu_ms_* timings bit for bit, every integer field of ll_mapper_stats, the pose, the frame index and the kernel
-launch count.  Also the error paths: validation before anything is enqueued, and a piece or scan over max_features in mid-sequence."""
+is registered) against the same inputs run one by one (ll_mapper_process_frame / _scan, the same loop over one input with nothing enqueued
+ahead) on a mapper and context of their own: every ll_reg_result field but the gpu_ms_* timings bit for bit, every integer field of
+ll_mapper_stats, the pose, the frame index and the kernel launch count.  Also the error paths: validation before anything is enqueued, and a
+piece or scan over max_features in mid-sequence."""
 import ctypes as C
 import os
 import sys
@@ -333,8 +334,9 @@ def _scans_call(gm, raws, stamps, n_scans=None, fmt=None, where=None, ns=None, n
 
 @pytest.mark.gpu
 def test_validation_errors_change_nothing(ctxs):
-    """Every validation error of both calls returns before anything is enqueued: nothing done, pose and frame index unchanged, and the next
-    call continues exactly as the one-by-one arm."""
+    """Every validation error of the sequence and the single calls returns before anything is enqueued: nothing done, pose and frame index
+    unchanged, and the next call continues exactly as the one-by-one arm.  After a rejected single call the mapper's image (which holds the
+    extractor's time bookkeeping) is that of a mapper that never saw the call, also when the call was the first input of a fresh mapper."""
     capi = _capi()
     frames, stamps = stream_frames(5, S.SEED + 3000)
     raws, ts = [f[0] for f in frames], [t[0] for t in stamps]
@@ -354,6 +356,28 @@ def test_validation_errors_change_nothing(ctxs):
         status, done, _ = _scans_call(gb, raws[2:4], ts[2:4], **kw)
         assert status == code and done == 0 and state(gb) == before, kw
     assert frames_seq(gb, frames[2:], stamps[2:]) == frames_single(ga, frames[2:], stamps[2:]) and state(ga) == state(gb)
+    ga.close(); gb.close()
+    # the single calls: gb sees each rejected call, then both take the next input; the first case is the first input of a fresh mapper,
+    # stamped apart from the first real input
+    frames, stamps = stream_frames(6, S.SEED + 3050)
+    raws, ts = [f[0] for f in frames], [t[0] for t in stamps]
+    cases = ((dict(fmt=7, stamps=[50.0]), capi.LL_ERR_INVALID), (dict(where=5), capi.LL_ERR_INVALID), (dict(null=0), capi.LL_ERR_INVALID),
+             (dict(ns=[big]), capi.LL_ERR_CAPACITY), (dict(odom_mode=2), capi.LL_ERR_INVALID), (dict(cap=2), capi.LL_ERR_INVALID))
+    ga, gb = mapper(ctxs[0]), mapper(ctxs[1])
+    for k, (kw, code) in enumerate(cases):
+        assert _raw_frame(gb, frames[k], **{"stamps": stamps[k], **kw}) == (code, 0, []), kw
+        assert state(gb) == state(ga) and gb.save() == ga.save(), kw
+        assert frames_single(gb, frames[k:k + 1], stamps[k:k + 1]) == frames_single(ga, frames[k:k + 1], stamps[k:k + 1]), kw
+    assert state(gb) == state(ga) and gb.save() == ga.save()
+    ga.close(); gb.close()
+    cases = ((dict(fmt=7, stamp=50.0), capi.LL_ERR_INVALID), (dict(where=5), capi.LL_ERR_INVALID), (dict(null=True), capi.LL_ERR_INVALID),
+             (dict(n=big), capi.LL_ERR_CAPACITY))
+    ga, gb = mapper(ctxs[0]), mapper(ctxs[1])
+    for k, (kw, code) in enumerate(cases):
+        assert _single_raw_scan_status(gb, raws[k], **{"stamp": ts[k], **kw})[0] == code, kw
+        assert state(gb) == state(ga) and gb.save() == ga.save(), kw
+        assert scans_single(gb, raws[k:k + 1], ts[k:k + 1]) == scans_single(ga, raws[k:k + 1], ts[k:k + 1]), kw
+    assert state(gb) == state(ga) and gb.save() == ga.save()
     ga.close(); gb.close()
 
 
@@ -412,15 +436,18 @@ def test_max_features_in_mid_sequence(ctxs):
             c.close()
 
 
-def _raw_frame(gm, heads, stamps):
+def _raw_frame(gm, heads, stamps, odom_mode=1, cap=16, fmt=None, where=None, ns=None, null=None):
     """ll_mapper_process_frame directly: (status, *n_pieces, entries of the completed pieces)."""
     capi = _capi()
     arrs = [np.ascontiguousarray(h, np.float32) for h in heads]
     ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
-    sizes = (C.c_size_t * len(arrs))(*[a.shape[0] for a in arrs])
+    if null is not None:
+        ptrs[null] = None
+    sizes = (C.c_size_t * len(arrs))(*(ns or [a.shape[0] for a in arrs]))
     st = (C.c_double * len(arrs))(*stamps)
     res, stats, n = (capi.RegResult * 16)(), (capi.MapperStats * 16)(), C.c_int(-1)
-    status = gm.ctx._lib.ll_mapper_process_frame(gm.h, len(arrs), ptrs, sizes, capi.LL_FMT_XYZI16, capi.LL_HOST, st, 1, res, stats, 16, C.byref(n))
+    status = gm.ctx._lib.ll_mapper_process_frame(gm.h, len(arrs), ptrs, sizes, capi.LL_FMT_XYZI16 if fmt is None else fmt, capi.LL_HOST if where is None else where,
+                                                 st, odom_mode, res, stats, cap, C.byref(n))
     return status, n.value, [entry(res[i], stats[i]) for i in range(n.value)]
 
 
@@ -483,11 +510,12 @@ def test_mapper_error_after_the_next_front_end_is_enqueued(ctxs):
     ga.close(); gb.close()
 
 
-def _single_raw_scan_status(gm, raw, stamp):
+def _single_raw_scan_status(gm, raw, stamp, fmt=None, where=None, n=None, null=False):
     capi = _capi()
     a = np.ascontiguousarray(raw, np.float32)
     res, st = capi.RegResult(), capi.MapperStats()
-    status = gm.ctx._lib.ll_mapper_process_scan(gm.h, C.c_void_p(a.ctypes.data), a.shape[0], capi.LL_FMT_XYZI16, capi.LL_HOST, stamp, C.byref(res), C.byref(st))
+    status = gm.ctx._lib.ll_mapper_process_scan(gm.h, None if null else C.c_void_p(a.ctypes.data), a.shape[0] if n is None else n,
+                                                capi.LL_FMT_XYZI16 if fmt is None else fmt, capi.LL_HOST if where is None else where, stamp, C.byref(res), C.byref(st))
     return status, entry(res, st)
 
 
