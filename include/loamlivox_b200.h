@@ -747,6 +747,83 @@ void ll_loop_cfg_default(ll_loop_cfg* cfg);
 int  ll_loop_search(ll_ctx* ctx, const ll_keyframe* const* kfs, int n, int newest, const ll_loop_cfg* cfg, float* sim_plane, float* sim_line, int* candidates,
                     int* n_candidates);
 
+/* ---- loop closure inside the streaming mapper (loop_closure/if_enable_loop_closure; DESIGN.md §4.6) -------------------------------------
+ * Off by default.  When on, every step whose features are appended (a rejected step, or one held back by recovery, does nothing here and does
+ * not count as a frame) also runs Laser_mapping::process_new_scan's keyframe block (laser_mapping.hpp:1442, 1446-1459, 1480-1487, 1523-1564)
+ * and, for a keyframe it closes, service_loop_detection (:874-1127), with every full cloud kept on the device:
+ *   cloud   the step's full cloud (a scan: the front end's full cloud; a piece: the piece's full slices of every head, in head order), moved
+ *           into the world by the registration pose (fp64, g_if_undistore = 0), pushed to the full history under the feature history's push
+ *           condition and popped past maximum_history_size, appended to the mapper's full-resolution cell map (resolution and revisit
+ *           threshold of the mapper's cell_resolution / threshold_cell_revisit, :617-618) and to every open keyframe (ll_keyframe_append).
+ *   close   the front keyframe at scans_of_each_keyframe frames, with the mapper's pose after this step and its frame index (:1534-1543).
+ *   open    when the back keyframe reaches scans_between_two_keyframe frames: the full history, VoxelGridded at surround_pointcloud_resolution,
+ *           becomes that keyframe's accumulated cloud (:943-944 filters the same cloud later), the history is cleared and a keyframe opened.
+ *   process a closed keyframe in the step that closes it: ll_keyframe_analyze, its pose and odometry edge, ll_loop_search over every earlier
+ *           keyframe, the candidates in ascending order through ll_scene_align on the typed clouds (`his += 10` above twice the threshold, `his
+ *           += 5` between the threshold and twice it, a loop below it), then ll_pose_graph_loop_edge, ll_pose_graph_optimize and the refined
+ *           clouds of the published keyframes (pc_idx = n - 1, n - 3, ...; VoxelGrid 0.2, :903, and the affine of ll_keyframes_repose).
+ * maximum_keyframe_in_waiting_list is not a setting: a closed keyframe is processed in the step that closes it, so the waiting list never holds
+ * more than one and its pop (:1554-1557) cannot fire.  After the first loop the reference searches no more (if_end, :990-993): the mapper then
+ * stops all loop-closure work.  Loop closure never changes the odometry: an error of its work other than LL_ERR_CUDA does not fail the step.
+ * A failed alignment ends that keyframe's search (LL_LOOP_FAILED); any other error is logged (LL_LOOP_ERROR) and stops loop closure for good.
+ * LL_ERR_CUDA is returned.  It is a runtime setting: it is not part of a mapper image, and a
+ * loaded mapper has it off. */
+typedef struct {
+  int    scans_of_each_keyframe;              /* loop_closure/scans_of_each_keyframe (300)                                                  */
+  int    scans_between_two_keyframe;          /* loop_closure/scans_between_two_keyframe (100); must be < scans_of_each_keyframe           */
+  ll_loop_cfg loop;                           /* the search's gates (minimum_keyframe_differen 200 in rosbag_loop.launch)                   */
+  float  map_alignment_resolution;            /* loop_closure/map_alignment_resolution (0.1)                                                */
+  int    map_alignment_maximum_icp_iteration; /* loop_closure/map_alignment_maximum_icp_iteration (5)                                      */
+  float  map_alignment_inlier_threshold;      /* loop_closure/map_alignment_inlier_threshold (0.20)                                        */
+  int    scene_alignment_maximum_residual_block;   /* loop_closure/scene_alignment_maximum_residual_block (3000)                           */
+  double surround_pointcloud_resolution;      /* mapping/surround_pointcloud_resolution (0.30): the accumulated clouds' VoxelGrid leaf     */
+  int    incremental_cov;                     /* common/if_update_mean_and_cov_incrementally (1)                                            */
+  int    rng_seed;                            /* ll_align_cfg::rng_seed of every alignment                                                  */
+  int    max_cells;                           /* the full map's cell table (as ll_cellmap_create; 0: its default)                          */
+  long long reserve_map_points;               /* the full map's point store allocated by ll_mapper_set_loop_closure                        */
+  long long reserve_history_points;           /* the full history allocated by ll_mapper_set_loop_closure                                  */
+  int    reserve_keyframes;                   /* keyframes whose poses, edges and graph are allocated by ll_mapper_set_loop_closure        */
+} ll_loop_closure_cfg;
+/* The values rosbag_loop.launch runs: performance_precision.yaml with if_enable_loop_closure 1 and minimum_keyframe_differen 200. */
+void ll_mapper_loop_closure_default(ll_loop_closure_cfg* cfg);
+/* cfg NULL: loop closure off, its buffers and results released.  Otherwise every value is checked (LL_ERR_INVALID, the mapper unchanged;
+ * scans_between_two_keyframe >= scans_of_each_keyframe is refused: the reference then calls back() on an empty keyframe list after a close),
+ * everything the reservations cover is allocated, and loop closure starts again from an empty full map and one open keyframe (:626). */
+int  ll_mapper_set_loop_closure(ll_mapper* mapper, const ll_loop_closure_cfg* cfg);
+enum { LL_LOOP_KEYFRAME = 0, LL_LOOP_ALIGNMENT = 1, LL_LOOP_CLOSED = 2, LL_LOOP_ERROR = 3 };   /* ll_loop_event::kind                  */
+enum { LL_LOOP_SKIP10 = 0, LL_LOOP_SKIP5 = 1, LL_LOOP_ACCEPT = 2, LL_LOOP_FAILED = 3 };   /* ll_loop_event::decision                          */
+typedef struct {
+  int32_t kind;                      /* LL_LOOP_KEYFRAME: a keyframe closed and processed; LL_LOOP_ALIGNMENT: one candidate aligned;
+                                        LL_LOOP_CLOSED: the loop closed; LL_LOOP_ERROR: the loop work of the step ending at
+                                        ending_frame_idx returned `status` (e.g. LL_ERR_CAPACITY of the full map's cell table) and loop
+                                        closure stopped                                                                                  */
+  int32_t keyframe;                  /* the newest keyframe's index (0, 1, ... in closing order)                                        */
+  int32_t ending_frame_idx;          /* KEYFRAME: m_ending_frame_idx (the mapper's frame index after the closing step); ERROR: the step */
+  int32_t n_candidates;              /* KEYFRAME: ll_loop_search's candidates (0 once the loop is closed)                               */
+  ll_keyframe_info info;             /* KEYFRAME: ll_keyframe_analyze's result                                                          */
+  double  q_wxyz[4], t[3];           /* KEYFRAME: the keyframe's pose                                                                   */
+  int32_t his;                       /* ALIGNMENT, CLOSED: the earlier keyframe                                                         */
+  int32_t scales_run;                /* ALIGNMENT: ll_scene_align's *scales_run                                                          */
+  int32_t decision;                  /* ALIGNMENT: LL_LOOP_SKIP10, LL_LOOP_SKIP5, LL_LOOP_ACCEPT, or LL_LOOP_FAILED: ll_scene_align
+                                        returned `status` (e.g. LL_ERR_CAPACITY: the typed clouds exceed max_features) and this keyframe's
+                                        search ends there                                                                                */
+  int32_t status;
+  double  inlier_threshold;          /* ALIGNMENT: the alignment's inlier_threshold                                                     */
+  double  icp_q_wxyz[4], icp_t[3];   /* ALIGNMENT: the alignment's pose                                                                 */
+  ll_pg_edge edge;                   /* CLOSED: the loop edge                                                                           */
+  ll_pg_summary summary;             /* CLOSED: ll_pose_graph_optimize's summary                                                        */
+} ll_loop_event;
+#define LL_LOOP_LOG 1024
+/* Drains up to cap events, oldest first, from a ring of LL_LOOP_LOG (entries past cap stay); *n_dropped = events overwritten unread. */
+int  ll_mapper_loop_read(ll_mapper* mapper, ll_loop_event* out, int cap, int* n, int* n_dropped);
+/* The processed keyframes (*n, may be 0) and whether the loop is closed.  poses_ori: their poses (pose3d_map_ori); poses_opt: after the
+ * optimization (temp_pose_3d_map; the poses_ori values before the loop closes); edge: the loop edge (zeros before).  Arrays hold cap
+ * keyframes (LL_ERR_CAPACITY, nothing written, when short); any may be NULL. */
+int  ll_mapper_loop_result(ll_mapper* mapper, int* n, int* closed, ll_pose* poses_ori, ll_pose* poses_opt, int cap, ll_pg_edge* edge);
+/* The refined cloud of published keyframe k (after the loop closed; k = n - 1, n - 3, ..., else LL_ERR_INVALID), as ll_keyframe_cloud offers
+ * its clouds: on the device (*out_dev, valid until loop closure is set again) and copied to out_host (cap points) when that is not NULL. */
+int  ll_mapper_loop_cloud(ll_mapper* mapper, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev);
+
 /* ---- multi-GPU ------------------------------------------------------------------------------------- */
 /* One process per GPU.  The 28-double normal equations (+4 counters) are all-reduced inside the solver kernel
  * through peer-mapped staging buffers (CUDA IPC over NVLink); the host only exchanges the IPC handles once. */

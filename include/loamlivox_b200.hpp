@@ -310,6 +310,28 @@ class Laser_mapping {
     if (dropped) *dropped = total;
     return out;
   }
+  // loop closure (ll_mapper_set_loop_closure, loop_closure/if_enable_loop_closure): cfg NULL turns it off; a bad value throws and leaves the
+  // mapper unchanged.  Not part of an image: a mapper from load_from_image has it off.
+  void set_loop_closure(const ll_loop_closure_cfg* cfg) { ctx_.check(ll_mapper_set_loop_closure(mapper_, cfg)); }
+  // the loop-closure events since the last read, oldest first (ll_mapper_loop_read); *dropped = events overwritten unread
+  std::vector<ll_loop_event> loop_log(int* dropped = nullptr) {
+    std::vector<ll_loop_event> out, buf(LL_LOOP_LOG);
+    int n = 0, d = 0, total = 0;
+    do {
+      ctx_.check(ll_mapper_loop_read(mapper_, buf.data(), (int)buf.size(), &n, &d));
+      out.insert(out.end(), buf.begin(), buf.begin() + n); total += d;
+    } while (n == (int)buf.size());
+    if (dropped) *dropped = total;
+    return out;
+  }
+  // the keyframe poses before (pose3d_map_ori) and after the optimization (temp_pose_3d_map), the loop edge; returns whether the loop is closed
+  bool loop_result(std::vector<ll_pose>* poses_ori, std::vector<ll_pose>* poses_opt, ll_pg_edge* edge = nullptr) {
+    int n = 0, closed = 0;
+    ctx_.check(ll_mapper_loop_result(mapper_, &n, &closed, nullptr, nullptr, 0, nullptr));
+    poses_ori->resize(n); poses_opt->resize(n);
+    ctx_.check(ll_mapper_loop_result(mapper_, &n, &closed, poses_ori->data(), poses_opt->data(), n, edge));
+    return closed != 0;
+  }
   std::array<double, 4> m_q_w_curr{{1, 0, 0, 0}};   // (w, x, y, z)
   std::array<double, 3> m_t_w_curr{{0, 0, 0}};
   int m_current_frame_index = 0;

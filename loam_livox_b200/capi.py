@@ -25,6 +25,9 @@ LL_RECOVERY_LOG = 1024
 LL_TRACKING, LL_SUSPECT, LL_LOST = 0, 1, 2
 LL_BAD_NONE, LL_BAD_REJECTED, LL_BAD_INLIER = 0, 1, 2
 LL_PG_MAX_BORDER = 64
+LL_LOOP_LOG = 1024
+LL_LOOP_KEYFRAME, LL_LOOP_ALIGNMENT, LL_LOOP_CLOSED, LL_LOOP_ERROR = 0, 1, 2, 3
+LL_LOOP_SKIP10, LL_LOOP_SKIP5, LL_LOOP_ACCEPT, LL_LOOP_FAILED = 0, 1, 2, 3
 LL_MAPPER_IMAGE_MAGIC, LL_MAPPER_IMAGE_VERSION = b"LLMAPIMG", 1
 (LL_IMAGE_CONFIG, LL_IMAGE_SCALARS, LL_IMAGE_HISTORY_CORNER, LL_IMAGE_HISTORY_SURF, LL_IMAGE_SNAPSHOT_CORNER, LL_IMAGE_SNAPSHOT_SURF, LL_IMAGE_CELLS_CORNER,
  LL_IMAGE_CELLS_SURF, LL_IMAGE_SECTIONS) = range(9)
@@ -45,6 +48,7 @@ EXPORTS = [
     "ll_keyframes_repose", "ll_keyframe_affine",
     "ll_keyframe_create", "ll_keyframe_release", "ll_keyframe_append", "ll_keyframe_analyze", "ll_keyframe_get_info", "ll_keyframe_cells",
     "ll_keyframe_images", "ll_keyframe_cloud", "ll_loop_cfg_default", "ll_loop_search",
+    "ll_mapper_loop_closure_default", "ll_mapper_set_loop_closure", "ll_mapper_loop_read", "ll_mapper_loop_result", "ll_mapper_loop_cloud",
 ]
 LL_CELL_SPHERE, LL_CELL_LINE, LL_CELL_PLANE, LL_CELL_ALL = 0, 1, 2, -1
 
@@ -182,6 +186,22 @@ class LoopCfg(C.Structure):
                                          "minimum_similarity_planar")] + [("plane_with_line", C.c_double)]
 
 
+class LoopClosureCfg(C.Structure):
+    """ll_loop_closure_cfg: the streaming mapper's keyframe schedule, search gates, alignment, accumulated-cloud leaf and reservations."""
+    _fields_ = [("scans_of_each_keyframe", C.c_int), ("scans_between_two_keyframe", C.c_int), ("loop", LoopCfg),
+                ("map_alignment_resolution", C.c_float), ("map_alignment_maximum_icp_iteration", C.c_int), ("map_alignment_inlier_threshold", C.c_float),
+                ("scene_alignment_maximum_residual_block", C.c_int), ("surround_pointcloud_resolution", C.c_double), ("incremental_cov", C.c_int),
+                ("rng_seed", C.c_int), ("max_cells", C.c_int), ("reserve_map_points", C.c_longlong), ("reserve_history_points", C.c_longlong),
+                ("reserve_keyframes", C.c_int)]
+
+
+class LoopEvent(C.Structure):
+    """ll_loop_event: a processed keyframe, one alignment of a candidate, or the closed loop."""
+    _fields_ = [(n, C.c_int32) for n in ("kind", "keyframe", "ending_frame_idx", "n_candidates")] + [("info", KeyframeInfo),
+                ("q_wxyz", C.c_double * 4), ("t", C.c_double * 3)] + [(n, C.c_int32) for n in ("his", "scales_run", "decision", "status")] + \
+               [("inlier_threshold", C.c_double), ("icp_q_wxyz", C.c_double * 4), ("icp_t", C.c_double * 3), ("edge", PgEdge), ("summary", PgSummary)]
+
+
 class LoamLivoxError(RuntimeError):
     pass
 
@@ -305,6 +325,11 @@ def lib():
     L.ll_keyframe_cloud.argtypes = [vp, vp, ci, vp, sz, C.POINTER(sz), C.POINTER(vp)]
     L.ll_loop_cfg_default.argtypes = [C.POINTER(LoopCfg)]
     L.ll_loop_search.argtypes = [vp, vp, ci, ci, C.POINTER(LoopCfg), vp, vp, vp, C.POINTER(ci)]
+    L.ll_mapper_loop_closure_default.argtypes = [C.POINTER(LoopClosureCfg)]
+    L.ll_mapper_set_loop_closure.argtypes = [vp, C.POINTER(LoopClosureCfg)]
+    L.ll_mapper_loop_read.argtypes = [vp, C.POINTER(LoopEvent), ci, C.POINTER(ci), C.POINTER(ci)]
+    L.ll_mapper_loop_result.argtypes = [vp, C.POINTER(ci), C.POINTER(ci), vp, vp, ci, C.POINTER(PgEdge)]
+    L.ll_mapper_loop_cloud.argtypes = [vp, ci, vp, sz, C.POINTER(sz), C.POINTER(vp)]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64
     _LIB = L

@@ -272,3 +272,58 @@ struct FrameArena { FrameDev* dev; float4* cls[2]; float4* mid[2]; int cap; DevB
 // are then cls[0] / cls[1] [out_end[.][i - 1], out_end[.][i]).
 int frame_front_end(ll_ctx* ctx, const FrontStreams& fs, const FrameArena& fa, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
                     int pieces, const ll_pipeline_cfg* pc);
+
+// ---------------------------------------------------------------------------------------------- streaming mapper (mapper.cu, loop.cu)
+// m_laser_cloud_{corner,surface}_history (std::list<PointCloud>, :1446-1478) as ONE flat device array: the clouds of the window lie one after the
+// other in push order, so the concatenation of mode 0 (:518-531) is the live range itself.  Two arenas, ping-pong: when the tail reaches the end of
+// one, the live range is copied to the start of the other (no allocation per scan in steady state).
+struct HistoryWindow {
+  DevBuf buf[2]; int cur = 0;
+  std::vector<std::pair<size_t, size_t>> segs;   // (offset, count) in points, oldest first
+  size_t tail = 0;                               // first free point of buf[cur]
+  size_t head() const { return segs.empty() ? tail : segs.front().first; }
+  size_t live() const { return tail - head(); }
+  const float4* data() const { return (const float4*)buf[cur].p + head(); }
+  int push(ll_ctx* ctx, const float4* d_pts, size_t n) {
+    cudaStream_t s = ctx->stream;
+    const size_t cap = buf[cur].cap / 16;
+    if (tail + n > cap) {   // slide: live range + the new cloud into the other arena
+      const size_t need = live() + n;
+      DevBuf& o = buf[cur ^ 1];
+      LL_CUDA(ctx, cudaStreamSynchronize(s));   // (the other arena may be reallocated; nothing may still read it)
+      LL_CUDA(ctx, o.reserve((need + need / 2 + 1024) * 16));
+      const size_t h = head(), lv = live();
+      if (lv) LL_CUDA(ctx, cudaMemcpyAsync(o.p, (const float4*)buf[cur].p + h, lv * 16, cudaMemcpyDeviceToDevice, s));
+      for (auto& sg : segs) sg.first -= h;
+      cur ^= 1; tail = lv;
+    }
+    if (n) LL_CUDA(ctx, cudaMemcpyAsync((float4*)buf[cur].p + tail, d_pts, n * 16, cudaMemcpyDeviceToDevice, s));
+    segs.emplace_back(tail, n); tail += n;
+    return LL_OK;
+  }
+  int reserve(ll_ctx* ctx, size_t points) { for (auto& b : buf) LL_CUDA(ctx, b.reserve_floor((points + points / 2 + 1024) * 16)); return LL_OK; }
+  void pop_front() { if (!segs.empty()) segs.erase(segs.begin()); }
+  void clear() { segs.clear(); tail = 0; }
+  void release() { buf[0].release(); buf[1].release(); segs.clear(); tail = 0; }
+};
+
+// ll_keyframes_repose on device inputs (posegraph.cu).
+int keyframes_repose_dev(ll_ctx* ctx, const float4* d_in, int n, const int* seg_end, int n_kf, const ll_pose* poses_ori, const ll_pose* poses_opt, float leaf,
+                         float4* d_mid, float4* d_out, int* d_end, int* d_oend, float* d_aff, int* out_end);
+extern "C" void pg_odometry_edge(const ll_pose* prev, int id_prev, const ll_pose* cur, int id_cur, ll_pg_edge* out);
+
+// The streaming mapper's loop closure (loop.cu; ll_mapper_set_loop_closure).  The step's full cloud is captured into the loop closure's own
+// buffer before the next input's front end may overwrite the context's arrays: loop_scan_cloud after scan_front_end_finish (the front end's
+// full cloud, compacted again from the extractor's state), loop_frame_clouds after a frame's front end (every published piece's full slices of
+// every head); loop_select_piece picks piece i's.  loop_step runs at the end of a mapper step that appended its features (d_pose: the
+// registration pose on the device; pushed: the feature history took the step).
+struct LoopClosure;
+int  loop_set(ll_ctx* ctx, LoopClosure** lc, const ll_loop_closure_cfg* cfg, const ll_mapper_config& mcfg, int pieces);
+void loop_release(LoopClosure* lc);
+int  loop_scan_cloud(ll_ctx* ctx, LoopClosure* lc, const ll_pipeline_cfg* pc);
+int  loop_frame_clouds(ll_ctx* ctx, LoopClosure* lc, const FrameDev* dev, const size_t* ns, int n_heads, int publish);
+void loop_select_piece(LoopClosure* lc, int i);
+int  loop_step(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool pushed, int frame_index, const double q_w_curr[4], const double t_w_curr[3]);
+int  loop_read(LoopClosure* lc, ll_loop_event* out, int cap, int* n, int* n_dropped);
+int  loop_result(const LoopClosure* lc, int* n, int* closed, ll_pose* poses_ori, ll_pose* poses_opt, int cap, ll_pg_edge* edge);
+int  loop_cloud(ll_ctx* ctx, const LoopClosure* lc, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev);

@@ -21,38 +21,6 @@
 
 static inline double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
-// m_laser_cloud_{corner,surface}_history (std::list<PointCloud>, :1446-1478) as ONE flat device array: the clouds of the window lie one after the
-// other in push order, so the concatenation of mode 0 (:518-531) is the live range itself.  Two arenas, ping-pong: when the tail reaches the end of
-// one, the live range is copied to the start of the other (no allocation per scan in steady state).
-struct HistoryWindow {
-  DevBuf buf[2]; int cur = 0;
-  std::vector<std::pair<size_t, size_t>> segs;   // (offset, count) in points, oldest first
-  size_t tail = 0;                               // first free point of buf[cur]
-  size_t head() const { return segs.empty() ? tail : segs.front().first; }
-  size_t live() const { return tail - head(); }
-  const float4* data() const { return (const float4*)buf[cur].p + head(); }
-  int push(ll_ctx* ctx, const float4* d_pts, size_t n) {
-    cudaStream_t s = ctx->stream;
-    const size_t cap = buf[cur].cap / 16;
-    if (tail + n > cap) {   // slide: live range + the new cloud into the other arena
-      const size_t need = live() + n;
-      DevBuf& o = buf[cur ^ 1];
-      LL_CUDA(ctx, cudaStreamSynchronize(s));   // (the other arena may be reallocated; nothing may still read it)
-      LL_CUDA(ctx, o.reserve((need + need / 2 + 1024) * 16));
-      const size_t h = head(), lv = live();
-      if (lv) LL_CUDA(ctx, cudaMemcpyAsync(o.p, (const float4*)buf[cur].p + h, lv * 16, cudaMemcpyDeviceToDevice, s));
-      for (auto& sg : segs) sg.first -= h;
-      cur ^= 1; tail = lv;
-    }
-    if (n) LL_CUDA(ctx, cudaMemcpyAsync((float4*)buf[cur].p + tail, d_pts, n * 16, cudaMemcpyDeviceToDevice, s));
-    segs.emplace_back(tail, n); tail += n;
-    return LL_OK;
-  }
-  int reserve(ll_ctx* ctx, size_t points) { for (auto& b : buf) LL_CUDA(ctx, b.reserve_floor((points + points / 2 + 1024) * 16)); return LL_OK; }
-  void pop_front() { if (!segs.empty()) segs.erase(segs.begin()); }
-  void release() { buf[0].release(); buf[1].release(); segs.clear(); tail = 0; }
-};
-
 // Tracking-loss recovery (ll_mapper_set_recovery; DESIGN.md §4.3.2): the detection state, the attempt's own buffers (allocated when it is
 // turned on), the step log and what the last attempt passed to the search.
 struct Recovery {
@@ -99,6 +67,7 @@ struct ll_mapper {
   FrontGraph frame_graph[2];   // the device part of the front end, replayed per arena
   int frame_pieces = 0;        // the pieces `frame` was laid out for
   Recovery rec;                // tracking-loss recovery (off unless ll_mapper_set_recovery turned it on)
+  LoopClosure* lc = nullptr;   // loop closure (off unless ll_mapper_set_loop_closure turned it on)
 };
 
 // frame: the front end's device record and, per class, the gathered piece segments and the first VoxelGrid's outputs
@@ -190,6 +159,7 @@ void ll_mapper_release(ll_mapper* m) {
   for (FrontGraph& g : m->frame_graph) if (g.exec) cudaGraphExecDestroy(g.exec);
   m->frame[0].release(); m->frame[1].release(); m->frame_vg[0].release(); m->frame_vg[1].release();
   ll_reloc_field_release(m->rec.field); if (m->rec.whole) ll_map_release(m->rec.whole); m->rec.buf.release();
+  loop_release(m->lc);
   delete m;
 }
 int ll_mapper_pose(const ll_mapper* m, double q_wxyz[4], double t[3], int* frame_index) {
@@ -290,6 +260,7 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
   const double tr0 = now_ms();
   // history window (:1439-1478): r_diff / t_diff compare the pose adopted from the PREVIOUS scan (m_q_w_curr is only overwritten at :1498) with the
   // pose of the last addition; history_add_t_step = history_add_angle_step = 0 (:83-84)
+  bool pushed = false;
   {
     const double* q = m->q_w_curr; const double* lq = m->last_his_add_q;
     double dot = fabs(q[0] * lq[0] + q[1] * lq[1] + q[2] * lq[2] + q[3] * lq[3]); if (dot > 1.0) dot = 1.0;
@@ -298,6 +269,7 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
     const double t_diff = sqrt(t2);
     if ((int)m->his_corner.segs.size() < m->cfg.maximum_history_size || t_diff > 0.0 || r_diff > 0.0 * 57.3) {
       for (int k = 0; k < 4; k++) m->last_his_add_q[k] = m->q_w_curr[k]; for (int k = 0; k < 3; k++) m->last_his_add_t[k] = m->t_w_curr[k];
+      pushed = true;
       LL_TRY(m->his_corner.push(ctx, w0, (size_t)hc[0]));
       LL_TRY(m->his_surf.push(ctx, w1, (size_t)hc[1]));
     }
@@ -314,6 +286,7 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
   if (stats) { stats->appended_corner = hc[0]; stats->appended_surf = hc[1]; stats->ms_append = (float)(now_ms() - tp); }
   if (m->rec.on) m->rec.ring[m->rec.cur].appended = 1;
   for (int k = 0; k < 4; k++) m->q_w_curr[k] = out->q_w_curr[k]; for (int k = 0; k < 3; k++) m->t_w_curr[k] = out->t_w_curr[k];   // :1496-1505
+  if (m->lc) LL_TRY(loop_step(ctx, m->lc, d_pose, pushed, m->frame_index, m->q_w_curr, m->t_w_curr));   // :1523-1564
   return LL_OK;
 }
 
@@ -425,6 +398,10 @@ static int frames_run(ll_mapper* m, const FrontStreams& fs, int n_frames, int n_
         ms_enqueue = (float)(now_ms() - t1);
         return LL_OK;
       };
+      if (m->lc && fo.heads_live != 0) {   // the published pieces' full clouds, before the next front end (behind fe_free) overwrites tmp_c
+        LL_TRY(loop_frame_clouds(ctx, m->lc, fa[f & 1].dev, ns + (size_t)f * n_heads, n_heads, publish));
+        LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[(f + 1) & 1], ctx->stream));
+      }
       if (fo.heads_live == 0) LL_TRY(enqueue_next());                           // laser_feature_extractor.hpp:287, every head
       for (int i = 0; fo.heads_live != 0 && i < publish; i++) {
         const int c0 = i ? fo.out_end[0][i - 1] : 0, s0 = i ? fo.out_end[1][i - 1] : 0;
@@ -438,6 +415,7 @@ static int frames_run(ll_mapper* m, const FrontStreams& fs, int n_frames, int n_
         LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat + nc, fa[f & 1].cls[1] + s0, (size_t)nsf * 16, cudaMemcpyDeviceToDevice, ctx->stream));
         if (i == publish - 1) LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[f & 1], ctx->stream));
         if (i == 0) LL_TRY(enqueue_next());
+        if (m->lc) loop_select_piece(m->lc, i);
         LL_TRY(mapper_step(m, nc, nsf, (double)ll_ord2f(fo.tmax[i]), o, ps));
         n_pieces[f] = i + 1;
       }
@@ -494,6 +472,7 @@ static int scans_run(ll_mapper* m, const FrontStreams& fs, int n_scans, const vo
       LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.fe_ready));
       int nc = 0, nsf = 0, dropped = 0;
       LL_TRY(scan_front_end_finish(ctx, ctx->stream, pc, &nc, &nsf, &dropped));   // reads the pinned counts before the next front end is enqueued
+      if (m->lc && !dropped) LL_TRY(loop_scan_cloud(ctx, m->lc, pc));            // the full cloud, before the next front end overwrites the extractor
       LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[0], ctx->stream));
       const float ms_front_end = ms_enqueue + (float)(now_ms() - t);
       if (k + 1 < n_scans) {
@@ -1143,6 +1122,40 @@ int ll_mapper_recovery_last_inputs(ll_mapper* m, ll_reloc_cfg* coarse, ll_reloc_
     if (dst[k] && R.n_last[k]) LL_CUDA(ctx, cudaMemcpyAsync(dst[k], src[k], R.n_last[k] * 16, cudaMemcpyDeviceToHost, ctx->stream));
   LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return LL_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- loop closure (loop.cu; DESIGN.md §4.6)
+void ll_mapper_loop_closure_default(ll_loop_closure_cfg* c) {
+  if (!c) return;
+  memset(c, 0, sizeof(*c));
+  c->scans_of_each_keyframe = 300; c->scans_between_two_keyframe = 100;            // performance_precision.yaml loop_closure/
+  ll_loop_cfg_default(&c->loop); c->loop.minimum_keyframe_differen = 200;          // rosbag_loop.launch
+  c->map_alignment_resolution = 0.1f; c->map_alignment_maximum_icp_iteration = 5; c->map_alignment_inlier_threshold = 0.20f;
+  c->scene_alignment_maximum_residual_block = 3000;
+  c->surround_pointcloud_resolution = 0.30;                                        // mapping/surround_pointcloud_resolution
+  c->incremental_cov = 1;                                                          // common/if_update_mean_and_cov_incrementally
+  c->rng_seed = 0; c->max_cells = 0;
+  c->reserve_map_points = 1 << 22; c->reserve_history_points = 1 << 22; c->reserve_keyframes = 1024;
+}
+
+int ll_mapper_set_loop_closure(ll_mapper* m, const ll_loop_closure_cfg* cfg) {
+  if (!m) return LL_ERR_INVALID;
+  return loop_set(m->ctx, &m->lc, cfg, m->cfg, m->frame_pieces);
+}
+
+int ll_mapper_loop_read(ll_mapper* m, ll_loop_event* out, int cap, int* n, int* n_dropped) {
+  if (!m || !n || cap < 0 || (cap > 0 && !out)) return LL_ERR_INVALID;
+  return loop_read(m->lc, out, cap, n, n_dropped);
+}
+
+int ll_mapper_loop_result(ll_mapper* m, int* n, int* closed, ll_pose* poses_ori, ll_pose* poses_opt, int cap, ll_pg_edge* edge) {
+  if (!m || cap < 0) return LL_ERR_INVALID;
+  return loop_result(m->lc, n, closed, poses_ori, poses_opt, cap, edge);
+}
+
+int ll_mapper_loop_cloud(ll_mapper* m, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev) {
+  if (!m || !n_out) return LL_ERR_INVALID;
+  return loop_cloud(m->ctx, m->lc, k, out_host, cap, n_out, out_dev);
 }
 
 }  // extern "C"

@@ -514,6 +514,24 @@ static void pg_rotation(const double* q, double* R) {   // Eigen's QuaternionBas
   R[6] = txz - twy; R[7] = tyz + twx; R[8] = 1 - (txx + tyy);
 }
 
+// ll_keyframes_repose on device input: keyframe k is d_in[seg_end[k - 1] .. seg_end[k]) of n points (host ends, n_kf 1 ... 256), down-sampled into d_mid
+// and moved into d_out (each as large as the input); d_end, d_oend (n_kf ints) and d_aff (12 n_kf floats) are the caller's device scratch.
+// out_end[k] = the end of keyframe k's output, read back after the work on the context's stream has completed.
+int keyframes_repose_dev(ll_ctx* ctx, const float4* d_in, int n, const int* seg_end, int n_kf, const ll_pose* poses_ori, const ll_pose* poses_opt, float leaf,
+                         float4* d_mid, float4* d_out, int* d_end, int* d_oend, float* d_aff, int* out_end) {
+  cudaStream_t s = ctx->stream;
+  std::vector<int> h(seg_end, seg_end + n_kf); std::vector<float> aff(12 * (size_t)n_kf);
+  for (int k = 0; k < n_kf; k++) ll_keyframe_affine(&poses_ori[k], &poses_opt[k], &aff[12 * k], &aff[12 * k + 9]);
+  LL_CUDA(ctx, cudaMemcpyAsync(d_end, h.data(), n_kf * sizeof(int), cudaMemcpyHostToDevice, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(d_aff, aff.data(), aff.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+  LL_TRY(launch_voxel_grid_segments(ctx, s, ctx->scratch, d_in, n, d_end, n_kf, leaf, d_mid, d_oend));
+  if (n) { repose_kernel<<<ll_div_up(n, 256), 256, 0, s>>>(d_mid, d_oend, n_kf, d_aff, d_out); ctx->launches++; LL_CUDA(ctx, cudaGetLastError()); }
+  LL_CUDA(ctx, cudaMemcpyAsync(h.data(), d_oend, n_kf * sizeof(int), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  std::copy(h.begin(), h.end(), out_end);
+  return LL_OK;
+}
+
 extern "C" {
 
 void ll_keyframe_affine(const ll_pose* ori, const ll_pose* opt, float R_aff[9], float T_aff[3]) {
@@ -540,15 +558,10 @@ int ll_keyframes_repose(ll_ctx* ctx, const ll_point* clouds, size_t n, const siz
   LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) {
     d_in = c.take<float4>(n); d_mid = c.take<float4>(n); d_out = c.take<float4>(n); d_end = c.take<int>(n_kf); d_oend = c.take<int>(n_kf); d_aff = c.take<float>(12 * (size_t)n_kf);
   }));
-  std::vector<int> h(n_kf); std::vector<float> aff(12 * (size_t)n_kf);
-  for (int k = 0; k < n_kf; k++) { h[k] = (int)seg_end[k]; ll_keyframe_affine(&poses_ori[k], &poses_opt[k], &aff[12 * k], &aff[12 * k + 9]); }
-  LL_CUDA(ctx, cudaMemcpyAsync(d_end, h.data(), n_kf * sizeof(int), cudaMemcpyHostToDevice, s));
-  LL_CUDA(ctx, cudaMemcpyAsync(d_aff, aff.data(), aff.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+  std::vector<int> h(n_kf);
+  for (int k = 0; k < n_kf; k++) h[k] = (int)seg_end[k];
   LL_TRY(upload_cloud(ctx, s, clouds, n, LL_FMT_XYZI16, LL_HOST, d_in));
-  LL_TRY(launch_voxel_grid_segments(ctx, s, ctx->scratch, d_in, (int)n, d_end, n_kf, leaf, d_mid, d_oend));
-  if (n) { repose_kernel<<<ll_div_up((int)n, 256), 256, 0, s>>>(d_mid, d_oend, n_kf, d_aff, d_out); ctx->launches++; LL_CUDA(ctx, cudaGetLastError()); }
-  LL_CUDA(ctx, cudaMemcpyAsync(h.data(), d_oend, n_kf * sizeof(int), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  LL_TRY(keyframes_repose_dev(ctx, d_in, (int)n, h.data(), n_kf, poses_ori, poses_opt, leaf, d_mid, d_out, d_end, d_oend, d_aff, h.data()));
   for (int k = 0; k < n_kf; k++) n_out_per_seg[k] = (size_t)(h[k] - (k ? h[k - 1] : 0));
   if (out && h[n_kf - 1] > 0) { LL_CUDA(ctx, cudaMemcpyAsync(out, d_out, (size_t)h[n_kf - 1] * 16, cudaMemcpyDeviceToHost, s)); LL_CUDA(ctx, cudaStreamSynchronize(s)); }
   return LL_OK;
@@ -641,6 +654,18 @@ static void pg_hrot(const double* q, const double* v, double* o) {   // Eigen's 
   double c[3] = {q[2] * v[2] - q[3] * v[1], q[3] * v[0] - q[1] * v[2], q[1] * v[1] - q[2] * v[0]};
   c[0] += c[0]; c[1] += c[1]; c[2] += c[2];
   o[0] = v[0] + q[0] * c[0] + (q[2] * c[2] - q[3] * c[1]); o[1] = v[1] + q[0] * c[1] + (q[3] * c[0] - q[1] * c[2]); o[2] = v[2] + q[0] * c[2] + (q[1] * c[1] - q[2] * c[0]);
+}
+
+// The odometry edge of service_loop_detection (laser_mapping.hpp:952-958): q = q_prev^-1 q_cur, t = q_prev^-1 (t_cur - t_prev), information = I.
+void pg_odometry_edge(const ll_pose* prev, int id_prev, const ll_pose* cur, int id_cur, ll_pg_edge* out) {
+  double qi[4], d[3];
+  memset(out, 0, sizeof(*out));
+  pg_qinv(prev->q_wxyz, qi);
+  for (int k = 0; k < 3; k++) d[k] = cur->t[k] - prev->t[k];
+  pg_hrot(qi, d, out->t);
+  pg_hmul(qi, cur->q_wxyz, out->q_wxyz);
+  out->id_begin = id_prev; out->id_end = id_cur;
+  for (int k = 0; k < 6; k++) out->information[7 * k] = 1.0;
 }
 
 void ll_pose_graph_loop_edge(const double icp_q_wxyz[4], const double icp_t[3], const ll_pose* pose_a, int id_a, const ll_pose* pose_b, int id_b, ll_pg_edge* out) {

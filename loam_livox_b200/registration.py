@@ -1028,6 +1028,58 @@ class Laser_mapping:
             if n.value < capi.LL_RECOVERY_LOG:
                 return out, total
 
+    def set_loop_closure(self, enable: bool = True, **kw):
+        """Loop closure (ll_mapper_set_loop_closure; DESIGN.md §4.6): from now on every appended step feeds the keyframes of the full-resolution map,
+        and each closed keyframe is searched against the earlier ones until the first loop closes.  kw overrides fields of
+        ll_mapper_loop_closure_default (loop=dict(...) the search's gates); enable=False turns it off.  Returns the capi.LoopClosureCfg in force."""
+        if not enable:
+            self.ctx.check(self.ctx._lib.ll_mapper_set_loop_closure(self.h, None))
+            return None
+        cfg = capi.LoopClosureCfg()
+        self.ctx._lib.ll_mapper_loop_closure_default(C.byref(cfg))
+        for k, v in kw.items():
+            if not hasattr(cfg, k):
+                raise AttributeError(k)
+            if k == "loop" and isinstance(v, dict):
+                for kk, vv in v.items():
+                    if not hasattr(cfg.loop, kk):
+                        raise AttributeError(kk)
+                    setattr(cfg.loop, kk, vv)
+            else:
+                setattr(cfg, k, v)
+        self.ctx.check(self.ctx._lib.ll_mapper_set_loop_closure(self.h, C.byref(cfg)))
+        return cfg
+
+    def loop_log(self):
+        """The loop-closure events since the last read (capi.LoopEvent, oldest first) and how many were overwritten unread."""
+        out, total = [], 0
+        buf, n, dropped = (capi.LoopEvent * capi.LL_LOOP_LOG)(), C.c_int(), C.c_int()
+        while True:
+            self.ctx.check(self.ctx._lib.ll_mapper_loop_read(self.h, buf, capi.LL_LOOP_LOG, C.byref(n), C.byref(dropped)))
+            total += dropped.value
+            out += [capi.LoopEvent.from_buffer_copy(buf[i]) for i in range(n.value)]
+            if n.value < capi.LL_LOOP_LOG:
+                return out, total
+
+    def loop_result(self):
+        """{"closed": bool, "poses_ori", "poses_opt": float64 [n, 7] (q w, x, y, z, t), "edge": capi.PgEdge} (ll_mapper_loop_result)."""
+        L = self.ctx._lib
+        n, closed = C.c_int(), C.c_int()
+        self.ctx.check(L.ll_mapper_loop_result(self.h, C.byref(n), C.byref(closed), None, None, 0, None))
+        ori, opt, edge = (capi.Pose * max(n.value, 1))(), (capi.Pose * max(n.value, 1))(), capi.PgEdge()
+        self.ctx.check(L.ll_mapper_loop_result(self.h, C.byref(n), C.byref(closed), ori, opt, n.value, C.byref(edge)))
+        as_np = lambda P: np.array([list(P[i].q_wxyz) + list(P[i].t) for i in range(n.value)], np.float64).reshape(n.value, 7)
+        return {"closed": bool(closed.value), "poses_ori": as_np(ori), "poses_opt": as_np(opt), "edge": edge}
+
+    def loop_cloud(self, k: int):
+        """The refined cloud of published keyframe k (ll_mapper_loop_cloud), float32 [n, 4]."""
+        n = C.c_size_t()
+        self.ctx.check(self.ctx._lib.ll_mapper_loop_cloud(self.h, int(k), None, 0, C.byref(n), None))
+        out = np.zeros((n.value, 4), np.float32)
+        if n.value:
+            self.ctx.check(self.ctx._lib.ll_mapper_loop_cloud(self.h, int(k), out.ctypes.data, n.value, C.byref(n), None))
+        return out
+
     def recovery_last_inputs(self):
         """What the last relocalization attempt passed to the search (ll_mapper_recovery_last_inputs): {"corner", "surf", "score_corner",
         "score_surf": float32 [n, 4]; "rot_coarse", "rot_fine": [n, 4]; "coarse": RelocCfg; "fine": RelocFineCfg; "tmpl": RegState}; the cfgs point
