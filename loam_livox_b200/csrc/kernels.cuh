@@ -252,6 +252,9 @@ ll_reloc_field* reloc_field_create(int device);
 size_t reloc_field_storage_cap(const ll_reloc_field* f);   // bytes its storage holds
 int reloc_field_reserve(ll_ctx* ctx, ll_reloc_field* f, long long n_vox, int max_hyp);
 int reloc_field_build_into(ll_ctx* ctx, const ll_map* map, float res, int trunc, int max_hypotheses, ll_reloc_field* f);
+// a (x) b, the Hamilton product of (w, x, y, z) quaternions in fp64, each component summed left to right as written (the fine rotations, the
+// recovery's yaw circle).
+void quat_mul(const double* a, const double* b, double* o);
 
 // ---------------------------------------------------------------------------------------------- host driver pieces (api.cu)
 // Registration of the features already resident in A.feat (corners then surfaces): the batch of one.  Core of ll_register / ll_scan_to_pose.

@@ -853,12 +853,6 @@ extern "C" int ll_mapper_set_pose(ll_mapper* m, const double q_wxyz[4], const do
 // build shared with ll_reloc_field_build, the VoxelGrid launcher for the score points and ll_relocalize_field on device inputs.
 namespace {
 
-void qmul(const double* a, const double* b, double* o) {   // Hamilton product, as reloc.cu forms the fine rotations
-  o[0] = a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3];
-  o[1] = a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2];
-  o[2] = a[0] * b[2] - a[1] * b[3] + a[2] * b[0] + a[3] * b[1];
-  o[3] = a[0] * b[3] + a[1] * b[2] - a[2] * b[1] + a[3] * b[0];
-}
 void yaw_quat(double deg, double* q) { const double a = deg * (M_PI / 180.0) * 0.5; q[0] = cos(a); q[1] = 0; q[2] = 0; q[3] = sin(a); }
 int coarse_yaws(const ll_recovery_cfg& c) { return (int)std::lround(360.0 / c.yaw_step_deg); }
 int fine_yaws(const ll_recovery_cfg& c) { return 2 * (int)std::floor(0.5 * c.yaw_step_deg / c.fine_yaw_step_deg + 1e-9) + 1; }
@@ -948,11 +942,11 @@ static int recovery_attempt(ll_mapper* m, int nc, int ns, const ll_reg_state& st
   double qy[4], qyc[4], tilt[4];
   yaw_quat(yaw * (180.0 / M_PI), qy);
   qyc[0] = qy[0]; qyc[1] = -qy[1]; qyc[2] = -qy[2]; qyc[3] = -qy[3];
-  qmul(qyc, q, tilt);
+  quat_mul(qyc, q, tilt);
   { const double nn = sqrt(tilt[0] * tilt[0] + tilt[1] * tilt[1] + tilt[2] * tilt[2] + tilt[3] * tilt[3]); for (int k = 0; k < 4; k++) tilt[k] /= nn; }
   const int n_yaw = coarse_yaws(c);
   R.rot_c.resize((size_t)n_yaw * 4);
-  for (int k = 0; k < n_yaw; k++) { double a[4]; yaw_quat(k * (360.0 / n_yaw), a); qmul(a, tilt, &R.rot_c[(size_t)k * 4]); }
+  for (int k = 0; k < n_yaw; k++) { double a[4]; yaw_quat(k * (360.0 / n_yaw), a); quat_mul(a, tilt, &R.rot_c[(size_t)k * 4]); }
   int dims[3]; float lo[3];
   LL_TRY(ll_reloc_field_read(R.field, 0, dims, lo, nullptr, 0));
   const double W = c.window_base + c.window_growth * R.bad;

@@ -18,36 +18,35 @@
 #define RELOC_TILE 1024    // score points rotated into shared memory per pass (3 x 8 KB)
 #define RELOC_GROUP 64     // lattice translations per CTA (8 warps x 8)
 
-struct ll_reloc_index {
+namespace {
+struct RelocGrid { const uint32_t* bits; int dims[3]; double lo[3]; double res; int dilate; };
+
+// What both searches keep: the map a search was built on, its grid and the buffers of its coarse stage.
+struct RelocBase {
   int device = 0;
   const ll_map* map = nullptr; const float4* src[2] = {nullptr, nullptr}; int n_src[2] = {0, 0};   // the map it was built on
-  float res = 0.f; int dilate = 0; int max_hyp = 0;
-  int dims[3] = {0, 0, 0}; float lo[3] = {0, 0, 0};
-  long long n_vox = 0, n_words = 0;
-  DevBuf storage;   // everything below, allocated once by ll_reloc_index_build
-  uint32_t* bits = nullptr;             // [n_words] the dilated occupancy, x fastest, bit v & 31 of word v >> 5
-  int32_t* scores = nullptr;            // [max_hyp]
+  RelocGrid grid = {};   // dilate: the index's dilate, the field's trunc; bits: the index's bitmask, null for the field
+  int max_hyp = 0;
+  long long n_vox = 0;
+  DevBuf storage;   // everything below and the derived object's arrays, allocated once by its build
+  int32_t* scores = nullptr;            // [max_hyp] coarse scores
   unsigned long long* peaks = nullptr;  // [max_hyp] peak keys (score << 32 | ~h), unordered
   int* counts = nullptr;                // [0] peaks, [1] candidates
   unsigned long long* cand = nullptr;   // [LL_MAX_BATCH] the first K peaks
+};
+}  // namespace
+
+struct ll_reloc_index : RelocBase {
+  long long n_words = 0;
+  uint32_t* bits = nullptr;             // [n_words] the dilated occupancy, x fastest, bit v & 31 of word v >> 5
   float4* pts = nullptr;                // [LL_RELOC_MAX_SCORE_POINTS] score points (scan frame)
   double* rot = nullptr;                // [max_hyp x 4] hypothesis rotations (w, x, y, z)
 };
 
 #define RELOC_MAX_TRUNC 15   // T^2 <= 225 fits a byte
 
-struct ll_reloc_field {
-  int device = 0;
-  const ll_map* map = nullptr; const float4* src[2] = {nullptr, nullptr}; int n_src[2] = {0, 0};   // the map it was built on
-  float res = 0.f; int trunc = 0; int max_hyp = 0;
-  int dims[3] = {0, 0, 0}; float lo[3] = {0, 0, 0};
-  long long n_vox = 0;
-  DevBuf storage;   // everything below, allocated once by ll_reloc_field_build
+struct ll_reloc_field : RelocBase {
   uint8_t* d2[2] = {nullptr, nullptr};  // [n_vox] per class ([0] corner, [1] surface): min(T^2, squared voxel distance to the class's nearest point)
-  int32_t* scores = nullptr;            // [max_hyp] coarse scores
-  unsigned long long* peaks = nullptr;  // [max_hyp] peak keys (score << 32 | ~h), unordered
-  int* counts = nullptr;                // [0] peaks, [1] candidates
-  unsigned long long* cand = nullptr;   // [LL_MAX_BATCH] the first K peaks
   int32_t* fine = nullptr;              // [max_hyp] the fine groups' scores, group-major
   unsigned long long* picks = nullptr;  // [LL_MAX_BATCH] each fine group's pick key (score << 32 | ~index)
   int32_t* verify = nullptr;            // [LL_MAX_BATCH] the score of each refined pose
@@ -57,8 +56,6 @@ struct ll_reloc_field {
 };
 
 namespace {
-
-struct RelocGrid { const uint32_t* bits; int dims[3]; double lo[3]; double res; int dilate; };
 
 // Cell of p on axis a = floor((p_a - lo_a) / res) + dilate in fp64, compared as a double before it becomes an integer.
 __device__ __forceinline__ bool grid_cell(const RelocGrid& g, float x, float y, float z, long long* v) {
@@ -200,12 +197,6 @@ __global__ void reloc_gather_kernel(const float4* __restrict__ src, const int* _
   if (i < n) dst[i] = src[idx[i]];
 }
 
-RelocGrid grid_of(const ll_reloc_index* x) {
-  RelocGrid g; g.bits = x->bits; g.res = (double)x->res; g.dilate = x->dilate;
-  for (int a = 0; a < 3; a++) { g.dims[a] = x->dims[a]; g.lo[a] = (double)x->lo[a]; }
-  return g;
-}
-
 void index_layout(ll_reloc_index* x, Carve& c) {
   x->bits = c.take<uint32_t>((size_t)x->n_words); x->scores = c.take<int32_t>(x->max_hyp); x->peaks = c.take<unsigned long long>(x->max_hyp);
   x->counts = c.take<int>(2); x->cand = c.take<unsigned long long>(LL_MAX_BATCH); x->pts = c.take<float4>(LL_RELOC_MAX_SCORE_POINTS);
@@ -217,16 +208,20 @@ int check_map(ll_ctx* ctx, const ll_map* map) {
   return LL_OK;
 }
 
-// The grid of a map: lo = the minimum of the finite bounding box both trees keep (d_bbox, read before anything is enqueued) and
-// dims_a = floor((hi_a - lo_a) / res) + 1 + 2 pad.  A map without a finite point: LL_ERR_INVALID; more than 2^30 voxels: LL_ERR_CAPACITY.
-int map_grid(ll_ctx* ctx, const ll_map* map, float res, int pad, int dims[3], float lo[3]) {
+// A build's checks, then the map's grid into b (only on success): lo = the minimum of the finite bounding box both trees keep (d_bbox), dims_a =
+// floor((hi_a - lo_a) / res) + 1 + 2 pad.  A map without a finite point: LL_ERR_INVALID; more than 2^30 voxels: LL_ERR_CAPACITY.
+int build_grid(ll_ctx* ctx, const ll_map* map, float res, int pad, bool pad_ok, const char* pad_error, int max_hypotheses, RelocBase* b) {
+  LL_TRY(check_map(ctx, map));
+  if (!(res > 0.f) || !std::isfinite(res)) { ctx->set_error("res must be a finite value > 0"); return LL_ERR_INVALID; }
+  if (!pad_ok) { ctx->set_error(pad_error); return LL_ERR_INVALID; }
+  if (max_hypotheses < 1 || max_hypotheses > RELOC_MAX_HYP) { ctx->set_error("max_hypotheses must be 1 ... 2^24"); return LL_ERR_INVALID; }
+  cudaSetDevice(ctx->device);
   cudaStream_t s = ctx->stream;
   const BucketTree* tr[2] = {&map->corner, &map->surf};
   float bb[2][6];
   for (int c = 0; c < 2; c++) if (tr[c]->n_src > 0) LL_CUDA(ctx, cudaMemcpyAsync(bb[c], tr[c]->d_bbox, sizeof(bb[c]), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
-  float hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-  for (int a = 0; a < 3; a++) lo[a] = INFINITY;
+  float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
   bool any = false;
   for (int c = 0; c < 2; c++) {
     if (tr[c]->n_src <= 0) continue;
@@ -237,6 +232,7 @@ int map_grid(ll_ctx* ctx, const ll_map* map, float res, int pad, int dims[3], fl
     for (int a = 0; a < 3; a++) { lo[a] = std::min(lo[a], bb[c][a]); hi[a] = std::max(hi[a], bb[c][3 + a]); }
   }
   if (!any) { ctx->set_error("the map has no finite point"); return LL_ERR_INVALID; }
+  int dims[3];
   double nv = 1.0;
   for (int a = 0; a < 3; a++) {
     const double d = std::floor(((double)hi[a] - (double)lo[a]) / (double)res) + 1.0 + 2.0 * pad;
@@ -244,7 +240,23 @@ int map_grid(ll_ctx* ctx, const ll_map* map, float res, int pad, int dims[3], fl
     dims[a] = (int)d; nv *= d;
   }
   if (nv > (double)RELOC_MAX_VOXELS) { ctx->set_error("more than 2^30 voxels"); return LL_ERR_CAPACITY; }
+  b->device = ctx->device; b->max_hyp = max_hypotheses; b->n_vox = (long long)dims[0] * dims[1] * dims[2];
+  b->grid = {nullptr, {dims[0], dims[1], dims[2]}, {(double)lo[0], (double)lo[1], (double)lo[2]}, (double)res, pad};
   return LL_OK;
+}
+
+int check_device(ll_ctx* ctx, const RelocBase* b, const char* noun) {
+  if (b->device != ctx->device) { ctx->set_error(std::string(noun) + " and context are on different devices"); return LL_ERR_INVALID; }
+  return LL_OK;
+}
+
+// A relocalization's first checks: the map is whole, b (the "index" / "field") was built on it as it is now, and b is on the context's device.
+int check_built_on(ll_ctx* ctx, const RelocBase* b, const ll_map* map, const char* noun) {
+  LL_TRY(check_map(ctx, map));
+  if (b->map != map || b->src[0] != map->corner.src || b->src[1] != map->surf.src || b->n_src[0] != map->corner.n_src || b->n_src[1] != map->surf.n_src) {
+    ctx->set_error(std::string("the ") + noun + " was built on another map (or the map was rebuilt since)"); return LL_ERR_INVALID;
+  }
+  return check_device(ctx, b, noun);
 }
 
 bool unit_quaternions(ll_ctx* ctx, const double* rot, int n, const char* what) {
@@ -278,13 +290,67 @@ int check_points(ll_ctx* ctx, const void* pts, size_t n, int fmt, int where, con
   return LL_OK;
 }
 
+// The last checks of both relocalizations: the template's gate, the score points' count and the batch's capacity for K items of M features.
+int check_refinement(ll_ctx* ctx, const ll_reg_state* tmpl, size_t n_score, const char* score_what, int K, size_t M) {
+  if (tmpl->current_frame_index <= tmpl->mapping_init_accumulate_frames) {
+    ctx->set_error("the template's frame index is at or below mapping_init_accumulate_frames: every refinement would skip the ICP (:199)"); return LL_ERR_INVALID;
+  }
+  if (n_score > LL_RELOC_MAX_SCORE_POINTS) { ctx->set_error(std::string("more than LL_RELOC_MAX_SCORE_POINTS ") + score_what); return LL_ERR_CAPACITY; }
+  if ((size_t)K * M > (size_t)ctx->cfg.max_features) { ctx->set_error("K x the features (" + std::to_string((size_t)K * M) + ") exceed max_features"); return LL_ERR_CAPACITY; }
+  int Ms[LL_MAX_BATCH]; for (int j = 0; j < K; j++) Ms[j] = (int)M;
+  return solve_capacity(ctx, K, Ms, tmpl->if_motion_deblur ? 1 : 0);
+}
+
+// Hypothesis h = i + nt0 (j + nt1 k) + n_lat r of a lattice: q = rotation r of rot, t = t0 + (i, j, k) step.
+void lattice_pose(const double* rot, const double* t0, const double* step, const int* nt, int h, double* q, double* t) {
+  const int n_lat = nt[0] * nt[1] * nt[2];
+  const int r = h / n_lat, l = h - r * n_lat, li[3] = {l % nt[0], (l / nt[0]) % nt[1], l / (nt[0] * nt[1])};
+  for (int k = 0; k < 4; k++) q[k] = rot[4 * r + k];
+  for (int k = 0; k < 3; k++) t[k] = t0[k] + (double)li[k] * step[k];
+}
+
+// The peaks of the H scores in b->scores, then the first K of them (*n) into cand: score, hypothesis and its pose (lattice_pose of cfg).
+template <typename Cand> int coarse_candidates(ll_ctx* ctx, RelocBase* b, const ll_reloc_cfg* cfg, long long H, int K, Cand* cand, int* n) {
+  cudaStream_t s = ctx->stream;
+  LL_CUDA(ctx, cudaMemsetAsync(b->counts, 0, 2 * sizeof(int), s));
+  reloc_peak_kernel<<<(unsigned)((H + 255) / 256), 256, 0, s>>>(b->scores, cfg->nt[0], cfg->nt[1], cfg->nt[2], cfg->n_rot, cfg->rot_cyclic ? 1 : 0, (int)H, b->peaks, b->counts);
+  reloc_select_kernel<<<1, 1024, 0, s>>>(b->peaks, b->counts, K, b->cand);
+  ctx->launches += 2;
+  LL_CUDA(ctx, cudaGetLastError());
+  unsigned long long keys[LL_MAX_BATCH]; int cnt[2] = {0, 0};
+  LL_CUDA(ctx, cudaMemcpyAsync(cnt, b->counts, sizeof(cnt), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(keys, b->cand, sizeof(keys), cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  *n = cnt[1];
+  for (int j = 0; j < *n; j++) {
+    cand[j].score = (int32_t)(keys[j] >> 32); cand[j].hypothesis = (int)(0xffffffffu - (unsigned)(keys[j] & 0xffffffffu));
+    lattice_pose(cfg->rot_wxyz, cfg->t0, cfg->step, cfg->nt, cand[j].hypothesis, cand[j].q_wxyz, cand[j].t);
+  }
+  return LL_OK;
+}
+
+// One registration batch of the same features, item j the template at seed pose (q[j], t[j]) with the identity increment.
+int refine(ll_ctx* ctx, const ll_map* map, int n, const double* const* q, const double* const* t, const ll_reg_state* tmpl, const void* corner,
+           size_t n_corner, const void* surf, size_t n_surf, int fmt, int where, ll_reg_result* refined, int* item_status) {
+  ll_reg_state in[LL_MAX_BATCH];
+  const void* cs[LL_MAX_BATCH]; const void* ss[LL_MAX_BATCH]; size_t ncs[LL_MAX_BATCH], nss[LL_MAX_BATCH];
+  for (int j = 0; j < n; j++) {
+    in[j] = *tmpl;
+    for (int k = 0; k < 4; k++) { in[j].q_w_last[k] = q[j][k]; in[j].q_w_curr[k] = q[j][k]; }
+    for (int k = 0; k < 3; k++) { in[j].t_w_last[k] = t[j][k]; in[j].t_w_curr[k] = t[j][k]; }
+    for (int k = 0; k < 7; k++) in[j].para_buffer_incremental[k] = k == 3 ? 1.0 : 0.0;
+    cs[j] = corner; ss[j] = surf; ncs[j] = n_corner; nss[j] = n_surf;
+  }
+  return ll_register_batch(ctx, map, n, cs, ncs, ss, nss, fmt, where, in, refined, item_status);
+}
+
 // Upload of the score points and the rotations, then the score kernel: scores[0 .. H) of the index, on the context's stream.
 int enqueue_scores(ll_ctx* ctx, ll_reloc_index* idx, const void* pts, size_t n, int fmt, int where, const ll_reloc_cfg* cfg) {
   cudaStream_t s = ctx->stream;
   LL_TRY(upload_cloud(ctx, s, pts, n, fmt, where, idx->pts));
   LL_CUDA(ctx, cudaMemcpyAsync(idx->rot, cfg->rot_wxyz, (size_t)cfg->n_rot * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
   ScoreArgs a;
-  a.g = grid_of(idx); a.pts = idx->pts; a.n_pts = (int)n; a.rot = idx->rot; a.scores = idx->scores;
+  a.g = idx->grid; a.pts = idx->pts; a.n_pts = (int)n; a.rot = idx->rot; a.scores = idx->scores;
   for (int k = 0; k < 3; k++) { a.t0[k] = cfg->t0[k]; a.step[k] = cfg->step[k]; a.nt[k] = cfg->nt[k]; }
   a.n_lat = cfg->nt[0] * cfg->nt[1] * cfg->nt[2];
   a.blocks_per_rot = ll_div_up(a.n_lat, RELOC_GROUP);
@@ -393,12 +459,6 @@ __global__ void __launch_bounds__(1024) reloc_pick_kernel(const int32_t* __restr
   }
 }
 
-RelocGrid field_grid(const ll_reloc_field* f) {
-  RelocGrid g; g.bits = nullptr; g.res = (double)f->res; g.dilate = f->trunc;
-  for (int a = 0; a < 3; a++) { g.dims[a] = f->dims[a]; g.lo[a] = (double)f->lo[a]; }
-  return g;
-}
-
 void field_layout(ll_reloc_field* f, Carve& c) {
   for (int k = 0; k < 2; k++) f->d2[k] = c.take<uint8_t>((size_t)f->n_vox);
   f->scores = c.take<int32_t>(f->max_hyp); f->peaks = c.take<unsigned long long>(f->max_hyp); f->counts = c.take<int>(2);
@@ -406,21 +466,6 @@ void field_layout(ll_reloc_field* f, Carve& c) {
   f->verify = c.take<int32_t>(LL_MAX_BATCH);
   for (int k = 0; k < 2; k++) f->pts[k] = c.take<float4>(LL_RELOC_MAX_SCORE_POINTS);
   f->rot = c.take<double>((size_t)f->max_hyp * 4); f->t0 = c.take<double>(LL_MAX_BATCH * 3);
-}
-
-// Everything ll_reloc_field_scores and ll_relocalize_field check about the field and the score points.
-int check_field_use(ll_ctx* ctx, const ll_reloc_field* f, const void* sc, size_t n_sc, const void* ss, size_t n_ss, int fmt, int where) {
-  if (f->device != ctx->device) { ctx->set_error("field and context are on different devices"); return LL_ERR_INVALID; }
-  LL_TRY(check_points(ctx, sc, n_sc, fmt, where, "corner score points"));
-  LL_TRY(check_points(ctx, ss, n_ss, fmt, where, "surface score points"));
-  return LL_OK;
-}
-
-int check_score_counts(ll_ctx* ctx, size_t n_sc, size_t n_ss) {
-  if (n_sc > LL_RELOC_MAX_SCORE_POINTS || n_ss > LL_RELOC_MAX_SCORE_POINTS) {
-    ctx->set_error("more than LL_RELOC_MAX_SCORE_POINTS score points in a class"); return LL_ERR_CAPACITY;
-  }
-  return LL_OK;
 }
 
 // The rotations (n_groups x n_rot, host) and origins (n_groups, host) of the groups uploaded, then the score kernel: out[0 .. n_groups x n_rot x
@@ -431,7 +476,7 @@ int enqueue_field_scores(ll_ctx* ctx, ll_reloc_field* f, int n_sc, int n_ss, int
   LL_CUDA(ctx, cudaMemcpyAsync(f->rot, rot, (size_t)n_groups * n_rot * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
   LL_CUDA(ctx, cudaMemcpyAsync(f->t0, t0, (size_t)n_groups * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
   FieldScoreArgs a;
-  a.g = field_grid(f);
+  a.g = f->grid;
   for (int c = 0; c < 2; c++) { a.d2[c] = f->d2[c]; a.pts[c] = f->pts[c]; }
   a.n_pts[0] = n_sc; a.n_pts[1] = n_ss; a.rot = f->rot; a.t0 = f->t0; a.scores = out;
   for (int k = 0; k < 3; k++) { a.step[k] = step[k]; a.nt[k] = nt[k]; }
@@ -443,21 +488,16 @@ int enqueue_field_scores(ll_ctx* ctx, ll_reloc_field* f, int n_sc, int n_ss, int
   return LL_OK;
 }
 
-int upload_score_points(ll_ctx* ctx, ll_reloc_field* f, const void* sc, size_t n_sc, const void* ss, size_t n_ss, int fmt, int where) {
-  LL_TRY(upload_cloud(ctx, ctx->stream, sc, n_sc, fmt, where, f->pts[0]));
-  LL_TRY(upload_cloud(ctx, ctx->stream, ss, n_ss, fmt, where, f->pts[1]));
-  return LL_OK;
-}
+template <typename T> void release(T* x) { if (!x) return; cudaSetDevice(x->device); x->storage.release(); delete x; }
 
-// q1 (x) q2, the Hamilton product in fp64, each component summed left to right as written.
+}  // namespace
+
 void quat_mul(const double* a, const double* b, double* o) {
   o[0] = a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3];
   o[1] = a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2];
   o[2] = a[0] * b[2] - a[1] * b[3] + a[2] * b[0] + a[3] * b[1];
   o[3] = a[0] * b[3] + a[1] * b[2] - a[2] * b[1] + a[3] * b[0];
 }
-
-}  // namespace
 
 // The live points of a cell map in store order (cm_live_points, cellmap.cu) are gathered here.
 int launch_gather_points(ll_ctx* ctx, cudaStream_t s, const float4* src, const int* idx, int n, float4* dst) {
@@ -483,18 +523,9 @@ int reloc_field_reserve(ll_ctx* ctx, ll_reloc_field* f, long long n_vox, int max
 // mapper's recovery: its own, once per loss episode).  On an error f holds no field (its map is cleared).
 int reloc_field_build_into(ll_ctx* ctx, const ll_map* map, float res, int trunc, int max_hypotheses, ll_reloc_field* f) {
   f->map = nullptr; f->src[0] = f->src[1] = nullptr; f->n_src[0] = f->n_src[1] = 0;
-  LL_TRY(check_map(ctx, map));
-  if (!(res > 0.f) || !std::isfinite(res)) { ctx->set_error("res must be a finite value > 0"); return LL_ERR_INVALID; }
-  if (trunc < 1 || trunc > RELOC_MAX_TRUNC) { ctx->set_error("trunc must be 1 ... 15"); return LL_ERR_INVALID; }
-  if (max_hypotheses < 1 || max_hypotheses > RELOC_MAX_HYP) { ctx->set_error("max_hypotheses must be 1 ... 2^24"); return LL_ERR_INVALID; }
-  cudaSetDevice(ctx->device);
+  LL_TRY(build_grid(ctx, map, res, trunc, trunc >= 1 && trunc <= RELOC_MAX_TRUNC, "trunc must be 1 ... 15", max_hypotheses, f));
   cudaStream_t s = ctx->stream;
-  int dims[3]; float lo[3];
-  LL_TRY(map_grid(ctx, map, res, trunc, dims, lo));
   const BucketTree* tr[2] = {&map->corner, &map->surf};
-  f->device = ctx->device; f->res = res; f->trunc = trunc; f->max_hyp = max_hypotheses;
-  for (int a = 0; a < 3; a++) { f->dims[a] = dims[a]; f->lo[a] = lo[a]; }
-  f->n_vox = (long long)dims[0] * dims[1] * dims[2];
   { const cudaError_t e = f->storage.carve([&](Carve& c) { field_layout(f, c); });
     if (e != cudaSuccess) { ctx->set_error(std::string("field allocation: ") + cudaGetErrorString(e)); return LL_ERR_CUDA; } }
   uint8_t* tmp = nullptr;   // occupancy, then the pass between y and z
@@ -502,13 +533,12 @@ int reloc_field_build_into(ll_ctx* ctx, const ll_map* map, float res, int trunc,
     if (e != cudaSuccess) { ctx->set_error(std::string("field scratch: ") + cudaGetErrorString(e)); return LL_ERR_CUDA; } }
   int st = LL_OK;
   auto cu = [&](cudaError_t e) { if (e != cudaSuccess && st == LL_OK) { ctx->set_error(std::string("field build: ") + cudaGetErrorString(e)); st = LL_ERR_CUDA; } };
-  const RelocGrid g = field_grid(f);
   const unsigned blocks = (unsigned)((f->n_vox + 255) / 256);
   for (int c = 0; c < 2; c++) {
     cu(cudaMemsetAsync(tmp, 0, (size_t)f->n_vox, s));
-    if (tr[c]->n_src > 0) { reloc_field_mark_kernel<<<ll_div_up(tr[c]->n_src, 256), 256, 0, s>>>(tr[c]->src, tr[c]->n_src, g, tmp); ctx->launches++; }
+    if (tr[c]->n_src > 0) { reloc_field_mark_kernel<<<ll_div_up(tr[c]->n_src, 256), 256, 0, s>>>(tr[c]->src, tr[c]->n_src, f->grid, tmp); ctx->launches++; }
     uint8_t* io[3][2] = {{tmp, f->d2[c]}, {f->d2[c], tmp}, {tmp, f->d2[c]}};
-    for (int a = 0; a < 3; a++) { reloc_edt_kernel<<<blocks, 256, 0, s>>>(io[a][0], io[a][1], dims[0], dims[1], dims[2], a, trunc, a == 0 ? 1 : 0, f->n_vox); ctx->launches++; }
+    for (int a = 0; a < 3; a++) { reloc_edt_kernel<<<blocks, 256, 0, s>>>(io[a][0], io[a][1], f->grid.dims[0], f->grid.dims[1], f->grid.dims[2], a, trunc, a == 0 ? 1 : 0, f->n_vox); ctx->launches++; }
   }
   cu(cudaGetLastError());
   cu(cudaStreamSynchronize(s));
@@ -523,20 +553,14 @@ extern "C" {
 int ll_reloc_index_build(ll_ctx* ctx, const ll_map* map, float res, int dilate, int max_hypotheses, ll_reloc_index** out) {
   if (!ctx || !map || !out) return LL_ERR_INVALID;
   *out = nullptr;
-  LL_TRY(check_map(ctx, map));
-  if (!(res > 0.f) || !std::isfinite(res)) { ctx->set_error("res must be a finite value > 0"); return LL_ERR_INVALID; }
-  if (dilate < 0 || dilate > RELOC_MAX_DILATE) { ctx->set_error("dilate must be 0 ... 4"); return LL_ERR_INVALID; }
-  if (max_hypotheses < 1 || max_hypotheses > RELOC_MAX_HYP) { ctx->set_error("max_hypotheses must be 1 ... 2^24"); return LL_ERR_INVALID; }
-  cudaSetDevice(ctx->device);
+  RelocBase base;
+  LL_TRY(build_grid(ctx, map, res, dilate, dilate >= 0 && dilate <= RELOC_MAX_DILATE, "dilate must be 0 ... 4", max_hypotheses, &base));
   cudaStream_t s = ctx->stream;
-  int dims[3]; float lo[3];
-  LL_TRY(map_grid(ctx, map, res, dilate, dims, lo));
   const BucketTree* tr[2] = {&map->corner, &map->surf};
-  ll_reloc_index* x = new ll_reloc_index();
-  x->device = ctx->device; x->map = map; x->res = res; x->dilate = dilate; x->max_hyp = max_hypotheses;
+  ll_reloc_index* x = new ll_reloc_index{base};
+  x->map = map;
   for (int c = 0; c < 2; c++) { x->src[c] = tr[c]->src; x->n_src[c] = tr[c]->n_src; }
-  for (int a = 0; a < 3; a++) { x->dims[a] = dims[a]; x->lo[a] = lo[a]; }
-  x->n_vox = (long long)dims[0] * dims[1] * dims[2]; x->n_words = (x->n_vox + 31) / 32;
+  x->n_words = (x->n_vox + 31) / 32;
   auto fail = [&](int st) { x->storage.release(); delete x; return st; };
   { const cudaError_t e = x->storage.carve([&](Carve& c) { index_layout(x, c); });
     if (e != cudaSuccess) { ctx->set_error(std::string("index allocation: ") + cudaGetErrorString(e)); return fail(LL_ERR_CUDA); } }
@@ -547,16 +571,16 @@ int ll_reloc_index_build(ll_ctx* ctx, const ll_map* map, float res, int dilate, 
     if (e != cudaSuccess) { ctx->set_error(std::string("index scratch: ") + cudaGetErrorString(e)); return fail(LL_ERR_CUDA); }
   }
   uint32_t* occ = dilate > 0 ? tmp : x->bits;
+  x->grid.bits = x->bits;
   int st = LL_OK;
   auto cu = [&](cudaError_t e) { if (e != cudaSuccess && st == LL_OK) { ctx->set_error(std::string("index build: ") + cudaGetErrorString(e)); st = LL_ERR_CUDA; } };
   cu(cudaMemsetAsync(occ, 0, (size_t)x->n_words * 4, s));
-  RelocGrid g = grid_of(x); g.bits = nullptr;
-  for (int c = 0; c < 2; c++) if (x->n_src[c] > 0) { reloc_mark_kernel<<<ll_div_up(x->n_src[c], 256), 256, 0, s>>>(x->src[c], x->n_src[c], g, occ); ctx->launches++; }
+  for (int c = 0; c < 2; c++) if (tr[c]->n_src > 0) { reloc_mark_kernel<<<ll_div_up(tr[c]->n_src, 256), 256, 0, s>>>(tr[c]->src, tr[c]->n_src, base.grid, occ); ctx->launches++; }
   if (dilate > 0) {
     const long long threads = x->n_words * 32;
     const unsigned blocks = (unsigned)((threads + 255) / 256);
     uint32_t* io[3][2] = {{tmp, x->bits}, {x->bits, tmp}, {tmp, x->bits}};
-    for (int a = 0; a < 3; a++) { reloc_dilate_kernel<<<blocks, 256, 0, s>>>(io[a][0], io[a][1], dims[0], dims[1], dims[2], a, dilate, x->n_vox, x->n_words); ctx->launches++; }
+    for (int a = 0; a < 3; a++) { reloc_dilate_kernel<<<blocks, 256, 0, s>>>(io[a][0], io[a][1], x->grid.dims[0], x->grid.dims[1], x->grid.dims[2], a, dilate, x->n_vox, x->n_words); ctx->launches++; }
   }
   cu(cudaGetLastError());
   cu(cudaStreamSynchronize(s));
@@ -565,17 +589,12 @@ int ll_reloc_index_build(ll_ctx* ctx, const ll_map* map, float res, int dilate, 
   return LL_OK;
 }
 
-void ll_reloc_index_release(ll_reloc_index* idx) {
-  if (!idx) return;
-  cudaSetDevice(idx->device);
-  idx->storage.release();
-  delete idx;
-}
+void ll_reloc_index_release(ll_reloc_index* idx) { release(idx); }
 
 int ll_reloc_index_read(const ll_reloc_index* idx, int dims[3], float lo[3], uint32_t* words, size_t cap_words) {
   if (!idx) return LL_ERR_INVALID;
-  if (dims) for (int a = 0; a < 3; a++) dims[a] = idx->dims[a];
-  if (lo) for (int a = 0; a < 3; a++) lo[a] = idx->lo[a];
+  if (dims) for (int a = 0; a < 3; a++) dims[a] = idx->grid.dims[a];
+  if (lo) for (int a = 0; a < 3; a++) lo[a] = (float)idx->grid.lo[a];
   if (!words) return LL_OK;
   if (cap_words < (size_t)idx->n_words) return LL_ERR_CAPACITY;
   cudaSetDevice(idx->device);
@@ -590,7 +609,7 @@ int ll_reloc_scores(ll_ctx* ctx, const ll_reloc_index* cidx, const void* score_p
   long long H = 0;
   LL_TRY(check_cfg(ctx, idx->max_hyp, cfg, &H));
   if (n_score > LL_RELOC_MAX_SCORE_POINTS) { ctx->set_error("more than LL_RELOC_MAX_SCORE_POINTS score points"); return LL_ERR_CAPACITY; }
-  if (idx->device != ctx->device) { ctx->set_error("index and context are on different devices"); return LL_ERR_INVALID; }
+  LL_TRY(check_device(ctx, idx, "index"));
   cudaSetDevice(ctx->device);
   LL_TRY(enqueue_scores(ctx, idx, score_pts, n_score, fmt, where, cfg));
   LL_CUDA(ctx, cudaMemcpyAsync(scores, idx->scores, (size_t)H * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -604,11 +623,7 @@ int ll_relocalize(ll_ctx* ctx, const ll_map* map, const ll_reloc_index* cidx, co
   if (!ctx || !map || !cidx || !cfg || !tmpl || !cand || !refined || !item_status || !n_cand || !best) return LL_ERR_INVALID;
   ll_reloc_index* idx = const_cast<ll_reloc_index*>(cidx);
   *n_cand = 0; *best = -1;
-  LL_TRY(check_map(ctx, map));
-  if (idx->map != map || idx->src[0] != map->corner.src || idx->src[1] != map->surf.src || idx->n_src[0] != map->corner.n_src || idx->n_src[1] != map->surf.n_src) {
-    ctx->set_error("the index was built on another map (or the map was rebuilt since)"); return LL_ERR_INVALID;
-  }
-  if (idx->device != ctx->device) { ctx->set_error("index and context are on different devices"); return LL_ERR_INVALID; }
+  LL_TRY(check_built_on(ctx, idx, map, "index"));
   LL_TRY(check_points(ctx, score_pts, n_score, fmt, where, "score points"));
   LL_TRY(check_points(ctx, corner, n_corner, fmt, where, "corner features"));
   LL_TRY(check_points(ctx, surf, n_surf, fmt, where, "surface features"));
@@ -616,49 +631,18 @@ int ll_relocalize(ll_ctx* ctx, const ll_map* map, const ll_reloc_index* cidx, co
   LL_TRY(check_cfg(ctx, idx->max_hyp, cfg, &H));
   const int K = cfg->max_candidates;
   if (K < 1 || K > LL_MAX_BATCH) { ctx->set_error("max_candidates must be 1 ... LL_MAX_BATCH"); return LL_ERR_INVALID; }
-  if (tmpl->current_frame_index <= tmpl->mapping_init_accumulate_frames) {
-    ctx->set_error("the template's frame index is at or below mapping_init_accumulate_frames: every refinement would skip the ICP (:199)"); return LL_ERR_INVALID;
-  }
-  if (n_score > LL_RELOC_MAX_SCORE_POINTS) { ctx->set_error("more than LL_RELOC_MAX_SCORE_POINTS score points"); return LL_ERR_CAPACITY; }
-  // the batch's own capacity check, for the largest batch this call can run (K items of the same features)
-  const size_t M = n_corner + n_surf;
-  if ((size_t)K * M > (size_t)ctx->cfg.max_features) { ctx->set_error("K x the features (" + std::to_string((size_t)K * M) + ") exceed max_features"); return LL_ERR_CAPACITY; }
-  { int Ms[LL_MAX_BATCH]; for (int j = 0; j < K; j++) Ms[j] = (int)M;
-    LL_TRY(solve_capacity(ctx, K, Ms, tmpl->if_motion_deblur ? 1 : 0)); }
+  LL_TRY(check_refinement(ctx, tmpl, n_score, "score points", K, n_corner + n_surf));
   cudaSetDevice(ctx->device);
-  cudaStream_t s = ctx->stream;
   // scores -> peaks -> the first K peaks
   LL_TRY(enqueue_scores(ctx, idx, score_pts, n_score, fmt, where, cfg));
-  LL_CUDA(ctx, cudaMemsetAsync(idx->counts, 0, 2 * sizeof(int), s));
-  reloc_peak_kernel<<<(unsigned)((H + 255) / 256), 256, 0, s>>>(idx->scores, cfg->nt[0], cfg->nt[1], cfg->nt[2], cfg->n_rot, cfg->rot_cyclic ? 1 : 0, (int)H, idx->peaks, idx->counts);
-  reloc_select_kernel<<<1, 1024, 0, s>>>(idx->peaks, idx->counts, K, idx->cand);
-  ctx->launches += 2;
-  LL_CUDA(ctx, cudaGetLastError());
-  unsigned long long keys[LL_MAX_BATCH]; int cnt[2] = {0, 0};
-  LL_CUDA(ctx, cudaMemcpyAsync(cnt, idx->counts, sizeof(cnt), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaMemcpyAsync(keys, idx->cand, sizeof(keys), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaStreamSynchronize(s));
-  const int n = cnt[1];
+  int n = 0;
+  LL_TRY(coarse_candidates(ctx, idx, cfg, H, K, cand, &n));
   if (n == 0) return LL_OK;
   // refinement: the candidates as the items of one registration batch, each seeded at its hypothesis
-  const int n_lat = cfg->nt[0] * cfg->nt[1] * cfg->nt[2];
-  ll_reg_state in[LL_MAX_BATCH];
-  const void* cs[LL_MAX_BATCH]; const void* ss[LL_MAX_BATCH]; size_t ncs[LL_MAX_BATCH], nss[LL_MAX_BATCH];
-  for (int j = 0; j < n; j++) {
-    const int h = (int)(0xffffffffu - (unsigned)(keys[j] & 0xffffffffu));
-    const int r = h / n_lat, l = h - r * n_lat, li[3] = {l % cfg->nt[0], (l / cfg->nt[0]) % cfg->nt[1], l / (cfg->nt[0] * cfg->nt[1])};
-    ll_reloc_candidate& c = cand[j];
-    c.score = (int32_t)(keys[j] >> 32); c.hypothesis = h;
-    for (int k = 0; k < 4; k++) c.q_wxyz[k] = cfg->rot_wxyz[4 * r + k];
-    for (int k = 0; k < 3; k++) c.t[k] = cfg->t0[k] + (double)li[k] * cfg->step[k];
-    in[j] = *tmpl;
-    for (int k = 0; k < 4; k++) { in[j].q_w_last[k] = c.q_wxyz[k]; in[j].q_w_curr[k] = c.q_wxyz[k]; }
-    for (int k = 0; k < 3; k++) { in[j].t_w_last[k] = c.t[k]; in[j].t_w_curr[k] = c.t[k]; }
-    for (int k = 0; k < 7; k++) in[j].para_buffer_incremental[k] = k == 3 ? 1.0 : 0.0;
-    cs[j] = corner; ss[j] = surf; ncs[j] = n_corner; nss[j] = n_surf;
-  }
+  const double* q[LL_MAX_BATCH]; const double* t[LL_MAX_BATCH];
+  for (int j = 0; j < n; j++) { q[j] = cand[j].q_wxyz; t[j] = cand[j].t; }
   *n_cand = n;
-  LL_TRY(ll_register_batch(ctx, map, n, cs, ncs, ss, nss, fmt, where, in, refined, item_status));
+  LL_TRY(refine(ctx, map, n, q, t, tmpl, corner, n_corner, surf, n_surf, fmt, where, refined, item_status));
   // the choice: the smallest inlier_threshold (:559) among the accepted registrations, ties to the lower rank
   for (int j = 0; j < n; j++) {
     const ll_reg_result& r = refined[j];
@@ -678,17 +662,12 @@ int ll_reloc_field_build(ll_ctx* ctx, const ll_map* map, float res, int trunc, i
   return LL_OK;
 }
 
-void ll_reloc_field_release(ll_reloc_field* field) {
-  if (!field) return;
-  cudaSetDevice(field->device);
-  field->storage.release();
-  delete field;
-}
+void ll_reloc_field_release(ll_reloc_field* field) { release(field); }
 
 int ll_reloc_field_read(const ll_reloc_field* field, int which, int dims[3], float lo[3], uint8_t* d2, size_t cap) {
   if (!field || (which != 0 && which != 1)) return LL_ERR_INVALID;
-  if (dims) for (int a = 0; a < 3; a++) dims[a] = field->dims[a];
-  if (lo) for (int a = 0; a < 3; a++) lo[a] = field->lo[a];
+  if (dims) for (int a = 0; a < 3; a++) dims[a] = field->grid.dims[a];
+  if (lo) for (int a = 0; a < 3; a++) lo[a] = (float)field->grid.lo[a];
   if (!d2) return LL_OK;
   if (cap < (size_t)field->n_vox) return LL_ERR_CAPACITY;
   cudaSetDevice(field->device);
@@ -700,12 +679,15 @@ int ll_reloc_field_scores(ll_ctx* ctx, const ll_reloc_field* cfield, const void*
                           int where, const ll_reloc_cfg* cfg, int32_t* scores) {
   if (!ctx || !cfield || !cfg || !scores) return LL_ERR_INVALID;
   ll_reloc_field* f = const_cast<ll_reloc_field*>(cfield);   // (its work buffers; the fields themselves are not changed)
-  LL_TRY(check_field_use(ctx, f, score_corner, n_sc, score_surf, n_ss, fmt, where));
+  LL_TRY(check_device(ctx, f, "field"));
+  LL_TRY(check_points(ctx, score_corner, n_sc, fmt, where, "corner score points"));
+  LL_TRY(check_points(ctx, score_surf, n_ss, fmt, where, "surface score points"));
   long long H = 0;
   LL_TRY(check_cfg(ctx, f->max_hyp, cfg, &H));
-  LL_TRY(check_score_counts(ctx, n_sc, n_ss));
+  if (std::max(n_sc, n_ss) > LL_RELOC_MAX_SCORE_POINTS) { ctx->set_error("more than LL_RELOC_MAX_SCORE_POINTS score points in a class"); return LL_ERR_CAPACITY; }
   cudaSetDevice(ctx->device);
-  LL_TRY(upload_score_points(ctx, f, score_corner, n_sc, score_surf, n_ss, fmt, where));
+  LL_TRY(upload_cloud(ctx, ctx->stream, score_corner, n_sc, fmt, where, f->pts[0]));
+  LL_TRY(upload_cloud(ctx, ctx->stream, score_surf, n_ss, fmt, where, f->pts[1]));
   LL_TRY(enqueue_field_scores(ctx, f, (int)n_sc, (int)n_ss, 1, cfg->rot_wxyz, cfg->n_rot, cfg->t0, cfg->step, cfg->nt, f->scores));
   LL_CUDA(ctx, cudaMemcpyAsync(scores, f->scores, (size_t)H * 4, cudaMemcpyDeviceToHost, ctx->stream));
   LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -719,11 +701,9 @@ int ll_relocalize_field(ll_ctx* ctx, const ll_map* map, const ll_reloc_field* cf
   if (!ctx || !map || !cfield || !coarse || !fine || !tmpl || !cand || !refined || !item_status || !n_cand || !best) return LL_ERR_INVALID;
   ll_reloc_field* f = const_cast<ll_reloc_field*>(cfield);
   *n_cand = 0; *best = -1;
-  LL_TRY(check_map(ctx, map));
-  if (f->map != map || f->src[0] != map->corner.src || f->src[1] != map->surf.src || f->n_src[0] != map->corner.n_src || f->n_src[1] != map->surf.n_src) {
-    ctx->set_error("the field was built on another map (or the map was rebuilt since)"); return LL_ERR_INVALID;
-  }
-  LL_TRY(check_field_use(ctx, f, score_corner, n_sc, score_surf, n_ss, fmt, where));
+  LL_TRY(check_built_on(ctx, f, map, "field"));
+  LL_TRY(check_points(ctx, score_corner, n_sc, fmt, where, "corner score points"));
+  LL_TRY(check_points(ctx, score_surf, n_ss, fmt, where, "surface score points"));
   LL_TRY(check_points(ctx, corner, n_corner, fmt, where, "corner features"));
   LL_TRY(check_points(ctx, surf, n_surf, fmt, where, "surface features"));
   long long H = 0;
@@ -742,43 +722,21 @@ int ll_relocalize_field(ll_ctx* ctx, const ll_map* map, const ll_reloc_field* cf
     ctx->set_error("max_candidates x the fine hypotheses exceed the field's max_hypotheses (" + std::to_string(f->max_hyp) + ")"); return LL_ERR_INVALID;
   }
   if (!unit_quaternions(ctx, fine->rot_wxyz, fine->n_rot, "fine rotation")) return LL_ERR_INVALID;
-  if (tmpl->current_frame_index <= tmpl->mapping_init_accumulate_frames) {
-    ctx->set_error("the template's frame index is at or below mapping_init_accumulate_frames: every refinement would skip the ICP (:199)"); return LL_ERR_INVALID;
-  }
-  LL_TRY(check_score_counts(ctx, n_sc, n_ss));
-  // the batch's own capacity check, for the largest batch this call can run (K items of the same features)
-  const size_t M = n_corner + n_surf;
-  if ((size_t)K * M > (size_t)ctx->cfg.max_features) { ctx->set_error("K x the features (" + std::to_string((size_t)K * M) + ") exceed max_features"); return LL_ERR_CAPACITY; }
-  { int Ms[LL_MAX_BATCH]; for (int j = 0; j < K; j++) Ms[j] = (int)M;
-    LL_TRY(solve_capacity(ctx, K, Ms, tmpl->if_motion_deblur ? 1 : 0)); }
+  LL_TRY(check_refinement(ctx, tmpl, std::max(n_sc, n_ss), "score points in a class", K, n_corner + n_surf));
   cudaSetDevice(ctx->device);
   cudaStream_t s = ctx->stream;
   // 1. coarse: scores -> peaks -> the first K peaks
-  LL_TRY(upload_score_points(ctx, f, score_corner, n_sc, score_surf, n_ss, fmt, where));
+  LL_TRY(upload_cloud(ctx, ctx->stream, score_corner, n_sc, fmt, where, f->pts[0]));
+  LL_TRY(upload_cloud(ctx, ctx->stream, score_surf, n_ss, fmt, where, f->pts[1]));
   LL_TRY(enqueue_field_scores(ctx, f, (int)n_sc, (int)n_ss, 1, coarse->rot_wxyz, coarse->n_rot, coarse->t0, coarse->step, coarse->nt, f->scores));
-  LL_CUDA(ctx, cudaMemsetAsync(f->counts, 0, 2 * sizeof(int), s));
-  reloc_peak_kernel<<<(unsigned)((H + 255) / 256), 256, 0, s>>>(f->scores, coarse->nt[0], coarse->nt[1], coarse->nt[2], coarse->n_rot, coarse->rot_cyclic ? 1 : 0, (int)H,
-                                                                f->peaks, f->counts);
-  reloc_select_kernel<<<1, 1024, 0, s>>>(f->peaks, f->counts, K, f->cand);
-  ctx->launches += 2;
-  LL_CUDA(ctx, cudaGetLastError());
-  unsigned long long keys[LL_MAX_BATCH]; int cnt[2] = {0, 0};
-  LL_CUDA(ctx, cudaMemcpyAsync(cnt, f->counts, sizeof(cnt), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaMemcpyAsync(keys, f->cand, sizeof(keys), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaStreamSynchronize(s));
-  const int n = cnt[1];
+  int n = 0;
+  LL_TRY(coarse_candidates(ctx, f, coarse, H, K, cand, &n));
   if (n == 0) return LL_OK;
   // 2. fine: group j = the rotations q_j (x) dq_r and the lattice origin t_j - ((nt - 1) / 2) step; its pick is its best hypothesis
-  const int n_lat = coarse->nt[0] * coarse->nt[1] * coarse->nt[2];
   std::vector<double> rot_f((size_t)n * fine->n_rot * 4);
   double t0_f[LL_MAX_BATCH * 3];
   for (int j = 0; j < n; j++) {
-    const int h = (int)(0xffffffffu - (unsigned)(keys[j] & 0xffffffffu));
-    const int r = h / n_lat, l = h - r * n_lat, li[3] = {l % coarse->nt[0], (l / coarse->nt[0]) % coarse->nt[1], l / (coarse->nt[0] * coarse->nt[1])};
-    ll_reloc_field_candidate& c = cand[j];
-    c.score = (int32_t)(keys[j] >> 32); c.hypothesis = h;
-    for (int k = 0; k < 4; k++) c.q_wxyz[k] = coarse->rot_wxyz[4 * r + k];
-    for (int k = 0; k < 3; k++) c.t[k] = coarse->t0[k] + (double)li[k] * coarse->step[k];
+    const ll_reloc_field_candidate& c = cand[j];
     for (int rr = 0; rr < fine->n_rot; rr++) quat_mul(c.q_wxyz, fine->rot_wxyz + 4 * rr, &rot_f[((size_t)j * fine->n_rot + rr) * 4]);
     for (int k = 0; k < 3; k++) t0_f[3 * j + k] = c.t[k] - (double)((fine->nt[k] - 1) / 2) * fine->step[k];
   }
@@ -789,24 +747,16 @@ int ll_relocalize_field(ll_ctx* ctx, const ll_map* map, const ll_reloc_field* cf
   LL_CUDA(ctx, cudaMemcpyAsync(picks, f->picks, (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   // 3. refinement: the picks as the items of one registration batch, seeded as ll_relocalize seeds its candidates
-  ll_reg_state in[LL_MAX_BATCH];
-  const void* cs[LL_MAX_BATCH]; const void* ss[LL_MAX_BATCH]; size_t ncs[LL_MAX_BATCH], nss[LL_MAX_BATCH];
+  const double* q[LL_MAX_BATCH]; const double* t[LL_MAX_BATCH];
   for (int j = 0; j < n; j++) {
     ll_reloc_field_candidate& c = cand[j];
-    const int i = (int)(0xffffffffu - (unsigned)(picks[j] & 0xffffffffu));
-    const int r = i / (int)n_lat_f, l = i - r * (int)n_lat_f, li[3] = {l % fine->nt[0], (l / fine->nt[0]) % fine->nt[1], l / (fine->nt[0] * fine->nt[1])};
-    c.fine_score = (int32_t)(picks[j] >> 32); c.fine_index = i;
-    for (int k = 0; k < 4; k++) c.fine_q_wxyz[k] = rot_f[((size_t)j * fine->n_rot + r) * 4 + k];
-    for (int k = 0; k < 3; k++) c.fine_t[k] = t0_f[3 * j + k] + (double)li[k] * fine->step[k];
+    c.fine_score = (int32_t)(picks[j] >> 32); c.fine_index = (int)(0xffffffffu - (unsigned)(picks[j] & 0xffffffffu));
+    lattice_pose(&rot_f[(size_t)j * fine->n_rot * 4], &t0_f[3 * j], fine->step, fine->nt, c.fine_index, c.fine_q_wxyz, c.fine_t);
     c.verify_score = 0; c.reserved = 0;
-    in[j] = *tmpl;
-    for (int k = 0; k < 4; k++) { in[j].q_w_last[k] = c.fine_q_wxyz[k]; in[j].q_w_curr[k] = c.fine_q_wxyz[k]; }
-    for (int k = 0; k < 3; k++) { in[j].t_w_last[k] = c.fine_t[k]; in[j].t_w_curr[k] = c.fine_t[k]; }
-    for (int k = 0; k < 7; k++) in[j].para_buffer_incremental[k] = k == 3 ? 1.0 : 0.0;
-    cs[j] = corner; ss[j] = surf; ncs[j] = n_corner; nss[j] = n_surf;
+    q[j] = c.fine_q_wxyz; t[j] = c.fine_t;
   }
   *n_cand = n;
-  LL_TRY(ll_register_batch(ctx, map, n, cs, ncs, ss, nss, fmt, where, in, refined, item_status));
+  LL_TRY(refine(ctx, map, n, q, t, tmpl, corner, n_corner, surf, n_surf, fmt, where, refined, item_status));
   // 4. verify: the same score at every refined pose (one group of one rotation and one translation each)
   double rot_v[LL_MAX_BATCH * 4], t0_v[LL_MAX_BATCH * 3];
   for (int j = 0; j < n; j++) {

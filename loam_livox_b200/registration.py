@@ -458,6 +458,27 @@ def reloc_scores(ctx: Context, index: RelocIndex, score_pts, rot_wxyz, t0, step,
     return out
 
 
+def _features(corners, surfs):
+    """(corners, surfaces, their one point format) of relocalize and relocalize_field."""
+    c, fmt = _pts(corners)
+    s, fmt2 = _pts(surfs)
+    if fmt != fmt2:
+        raise ValueError("corners and surfaces in one point format")
+    return c, s, fmt
+
+
+def _coarse_args(state, yaw_step_deg, tilt_q, window, k):
+    """(`state` or capi.default_reg_state past the initialisation gate, the coarse capi.RelocCfg of the yaw circle and the window's lattice,
+    its keepalive) of relocalize and relocalize_field."""
+    if state is None:
+        state = capi.default_reg_state()
+        state.current_frame_index = state.mapping_init_accumulate_frames + 1
+    rot = yaw_circle(yaw_step_deg, tilt_q)
+    t0, step, nt = window_lattice(window)
+    cfg, keep = reloc_cfg(rot, t0, step, nt, k, cyclic=True)
+    return state, cfg, keep
+
+
 def relocalize(ctx: Context, match_map: Map, index: RelocIndex, corners, surfs, score_leaf: float = 0.5, window=((-1.0, 1.0, 1.0), (-1.0, 1.0, 1.0), (0.0, 0.0, 0.0)),
                yaw_step_deg: float = 10.0, tilt_q=None, k: int = 8, state: capi.RegState | None = None, score_pts=None):
     """Find the pose of a scan (its scan-frame corner / surface features) in `match_map` without an initial guess (ll_relocalize).
@@ -467,22 +488,14 @@ def relocalize(ctx: Context, match_map: Map, index: RelocIndex, corners, surfs, 
     (((x0, x1, dx), (y0, y1, dy), (z0, z1, dz))).  The first k peaks of the score are refined by the batched registration with `state` (default:
     capi.default_reg_state past the initialisation gate).  Returns {"candidates": [{hypothesis, score, q, t}], "refined": [RegResult],
     "item_status": [int], "best": rank or -1, "n_score": int}."""
-    c, fmt = _pts(corners)
-    s, fmt2 = _pts(surfs)
-    if fmt != fmt2:
-        raise ValueError("corners and surfaces in one point format")
+    c, s, fmt = _features(corners, surfs)
     if score_pts is None:
         both = np.concatenate([c[:, :4], s[:, :4]] if fmt == capi.LL_FMT_XYZI16 else [c[:, [0, 1, 2, 4]], s[:, [0, 1, 2, 4]]], axis=0)
         score_pts = voxel_grid_filter(ctx, both, float(score_leaf))
     sp, sfmt = _pts(score_pts)
     if sfmt != fmt:
         sp = np.ascontiguousarray(sp[:, [0, 1, 2, 4]] if sfmt == capi.LL_FMT_PCL32 else np.concatenate([sp, np.zeros((sp.shape[0], 4), np.float32)], axis=1))
-    if state is None:
-        state = capi.default_reg_state()
-        state.current_frame_index = state.mapping_init_accumulate_frames + 1
-    rot = yaw_circle(yaw_step_deg, tilt_q)
-    t0, step, nt = window_lattice(window)
-    cfg, _keep = reloc_cfg(rot, t0, step, nt, k, cyclic=True)
+    state, cfg, _keep = _coarse_args(state, yaw_step_deg, tilt_q, window, k)
     K = int(k)
     cand, res, status = (capi.RelocCandidate * K)(), (capi.RegResult * K)(), (C.c_int * K)()
     n, best = C.c_int(), C.c_int()
@@ -581,21 +594,13 @@ def relocalize_field(ctx: Context, match_map: Map, field: RelocField, corners, s
     of each is refined by the batched registration with `state`, and the accepted item of the largest field score at its refined pose wins.
     Returns {"candidates": [{hypothesis, score, q, t, fine_index, fine_score, fine_q, fine_t, verify_score}], "refined": [RegResult],
     "item_status": [int], "best": rank or -1, "n_score": (corner, surface)}."""
-    c, fmt = _pts(corners)
-    s, fmt2 = _pts(surfs)
-    if fmt != fmt2:
-        raise ValueError("corners and surfaces in one point format")
+    c, s, fmt = _features(corners, surfs)
     if score_pts is None:
         score_pts = (voxel_grid_filter(ctx, c, float(score_leaf)), voxel_grid_filter(ctx, s, float(score_leaf)))
         if fmt == capi.LL_FMT_PCL32:
             score_pts = tuple(np.concatenate([p, np.zeros((p.shape[0], 4), np.float32)], axis=1) for p in score_pts)
     sc, ss = _score_pair(fmt, *score_pts)
-    if state is None:
-        state = capi.default_reg_state()
-        state.current_frame_index = state.mapping_init_accumulate_frames + 1
-    rot = yaw_circle(yaw_step_deg, tilt_q)
-    t0, step, nt = window_lattice(window)
-    cfg, _keep = reloc_cfg(rot, t0, step, nt, k, cyclic=True)
+    state, cfg, _keep = _coarse_args(state, yaw_step_deg, tilt_q, window, k)
     dq, fstep, fnt = fine_search(yaw_step_deg, window, fine_yaw_step_deg, fine_t_step, fine_t_half)
     fcfg, _keep2 = fine_cfg(dq, fstep, fnt)
     K = int(k)
