@@ -824,6 +824,39 @@ int  ll_mapper_loop_result(ll_mapper* mapper, int* n, int* closed, ll_pose* pose
  * its clouds: on the device (*out_dev, valid until loop closure is set again) and copied to out_host (cap points) when that is not NULL. */
 int  ll_mapper_loop_cloud(ll_mapper* mapper, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev);
 
+/* ---- spinning-lidar front end: the Velodyne branch of Laser_feature::laserCloudHandler (DESIGN.md §4.7) ---------------------------------
+ * laser_feature_extractor.hpp:393-825 with lidar_type other than "livox": NaN and near points removed (:399-400), ring and relative time per
+ * point (:403-504), the rings concatenated (:510-521), curvature and neighbour flags (:524-598), per ring 6 sub-scans sorted by curvature with
+ * the sharp and flat picks (:631-768), and the less-flat points VoxelGridded per ring at plane_resolution / 2 (:771-776).  Five clouds, in the
+ * reference's push order: the full ring-ordered cloud (/laser_points_2, intensity = ring + 0.1 relTime), sharp (/laser_cloud_sharp), less
+ * sharp, flat and less flat.  Stated deviations: the result is defined on the kept points (the reference reads past the filtered cloud when a
+ * point was removed); the neighbour walks stop at the ends of the cloud; fewer than 5 kept points give empty feature clouds; a point with a
+ * coordinate of magnitude above 1e36 is removed with the non-finite ones.  The 20-frame start-up delay (m_para_system_delay) is the caller's. */
+typedef struct ll_spin ll_spin;
+typedef struct {
+  int   scan_line;          /* feature_extraction/scan_line: 16 or 64, anything else LL_ERR_INVALID (:160-164)                          */
+  float minimum_range;      /* feature_extraction/minimum_range (0.1), the removeClosedPointCloud threshold                              */
+  float plane_resolution;   /* feature_extraction/mapping_plane_resolution (0.4 in the shipped YAMLs): the less-flat VoxelGrid leaf is half */
+  int   max_points;         /* input points per call the handle's arenas hold (the reference's per-point arrays: 400000)                 */
+} ll_spin_cfg;
+enum { LL_SPIN_FULL = 0, LL_SPIN_SHARP = 1, LL_SPIN_LESS_SHARP = 2, LL_SPIN_FLAT = 3, LL_SPIN_LESS_FLAT = 4 };
+void ll_spin_cfg_default(ll_spin_cfg* cfg);
+/* A spinning-lidar front end on ctx's device and stream, with its own arenas (ctx's footprint does not change); ctx must outlive it. */
+int  ll_spin_create(ll_ctx* ctx, const ll_spin_cfg* cfg, ll_spin** out);
+void ll_spin_release(ll_spin* spin);
+/* One cloud through the front end: any input format (LL_FMT_STRIDED takes ctx's ll_set_point_layout), host or device.  counts[5] (may be
+ * NULL): the sizes of the five clouds, indexed by LL_SPIN_*.  More than max_points: LL_ERR_CAPACITY, nothing changed.  One host
+ * synchronisation, at the end. */
+int  ll_spin_extract(ll_spin* spin, const void* raw, size_t n, int fmt, int where, size_t counts[5]);
+/* Cloud `which` (LL_SPIN_*) of the last extract: on the device (*out_dev, valid until the next extract on this handle; the less-sharp and
+ * less-flat clouds can go to ll_register / ll_map_build as LL_DEVICE inputs), copied to out_host (cap points) when that is not NULL. */
+int  ll_spin_cloud(ll_spin* spin, int which, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev);
+/* Parity view of the full cloud's points (index order, cap entries; any array may be NULL): ring, curvature (0 outside [5, N - 5)), picked
+ * before the selection (the occlusion and parallel-beam flags as they stand after :524-598) and the label (2 sharp, 1 less sharp, -1 flat, 0). */
+int  ll_spin_point_info(ll_spin* spin, int32_t* ring, float* curvature, int32_t* picked, int32_t* label, size_t cap, size_t* n_out);
+/* Diagnostics of the last extract: chains of the selection and the longest one in points. */
+int  ll_spin_chains(const ll_spin* spin, int* n_chains, int* longest);
+
 /* ---- multi-GPU ------------------------------------------------------------------------------------- */
 /* One process per GPU.  The 28-double normal equations (+4 counters) are all-reduced inside the solver kernel
  * through peer-mapped staging buffers (CUDA IPC over NVLink); the host only exchanges the IPC handles once. */

@@ -455,4 +455,39 @@ inline std::vector<int> loop_search(Context& ctx, const std::vector<Maps_keyfram
   cand.resize(n); return cand;
 }
 
+// Laser_feature's Velodyne branch (laser_feature_extractor.hpp:393-825, scan_line 16 or 64) on the device: laserCloudHandler(cloud) fills
+// the five clouds the reference publishes (/laser_points_2, /laser_cloud_sharp, /laser_cloud_less_sharp, /laser_cloud_flat,
+// /laser_cloud_less_flat).  The 20-frame start-up delay stays the caller's.
+class Laser_feature {
+ public:
+  Laser_feature(Context& ctx, int scan_line = 16, float minimum_range = 0.1f, float plane_resolution = 0.4f) : ctx_(ctx) {
+    ll_spin_cfg cfg; ll_spin_cfg_default(&cfg);
+    cfg.scan_line = scan_line; cfg.minimum_range = minimum_range; cfg.plane_resolution = plane_resolution;
+    ctx_.check(ll_spin_create(ctx_.get(), &cfg, &h_));
+  }
+  ~Laser_feature() { ll_spin_release(h_); }
+  Laser_feature(const Laser_feature&) = delete; Laser_feature& operator=(const Laser_feature&) = delete;
+  void laserCloudHandler(const PointCloud& in) {
+    ctx_.check(ll_spin_extract(h_, in.data(), in.size(), LL_FMT_PCL32, LL_HOST, nullptr));
+    laserCloud = cloud(LL_SPIN_FULL); cornerPointsSharp = cloud(LL_SPIN_SHARP); cornerPointsLessSharp = cloud(LL_SPIN_LESS_SHARP);
+    surfPointsFlat = cloud(LL_SPIN_FLAT); surfPointsLessFlat = cloud(LL_SPIN_LESS_FLAT);
+  }
+  // device form of cloud `which` (LL_SPIN_*), valid until the next laserCloudHandler: an LL_DEVICE input of ll_register / ll_map_build
+  const ll_point* device_cloud(int which, size_t* n) const { const ll_point* d = nullptr; ctx_.check(ll_spin_cloud(h_, which, nullptr, 0, n, &d)); return d; }
+  PointCloud laserCloud, cornerPointsSharp, cornerPointsLessSharp, surfPointsFlat, surfPointsLessFlat;
+  ll_spin* get() const { return h_; }
+ private:
+  PointCloud cloud(int which) const {
+    size_t n = 0;
+    ctx_.check(ll_spin_cloud(h_, which, nullptr, 0, &n, nullptr));
+    std::vector<ll_point> tmp(n);
+    if (n) ctx_.check(ll_spin_cloud(h_, which, tmp.data(), n, &n, nullptr));
+    PointCloud out(n);
+    for (size_t i = 0; i < n; i++) { out[i] = PointXYZI{}; out[i].x = tmp[i].x; out[i].y = tmp[i].y; out[i].z = tmp[i].z; out[i].intensity = tmp[i].intensity; }
+    return out;
+  }
+  Context& ctx_;
+  ll_spin* h_ = nullptr;
+};
+
 }  // namespace ll200

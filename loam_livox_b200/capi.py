@@ -49,8 +49,15 @@ EXPORTS = [
     "ll_keyframe_create", "ll_keyframe_release", "ll_keyframe_append", "ll_keyframe_analyze", "ll_keyframe_get_info", "ll_keyframe_cells",
     "ll_keyframe_images", "ll_keyframe_cloud", "ll_loop_cfg_default", "ll_loop_search",
     "ll_mapper_loop_closure_default", "ll_mapper_set_loop_closure", "ll_mapper_loop_read", "ll_mapper_loop_result", "ll_mapper_loop_cloud",
+    "ll_spin_cfg_default", "ll_spin_create", "ll_spin_release", "ll_spin_extract", "ll_spin_cloud", "ll_spin_point_info", "ll_spin_chains",
 ]
+LL_SPIN_FULL, LL_SPIN_SHARP, LL_SPIN_LESS_SHARP, LL_SPIN_FLAT, LL_SPIN_LESS_FLAT = 0, 1, 2, 3, 4
 LL_CELL_SPHERE, LL_CELL_LINE, LL_CELL_PLANE, LL_CELL_ALL = 0, 1, 2, -1
+
+
+class SpinCfg(C.Structure):
+    """ll_spin_cfg: the Velodyne branch's feature_extraction parameters and the handle's input capacity."""
+    _fields_ = [("scan_line", C.c_int), ("minimum_range", C.c_float), ("plane_resolution", C.c_float), ("max_points", C.c_int)]
 
 
 class Config(C.Structure):
@@ -330,10 +337,25 @@ def lib():
     L.ll_mapper_loop_read.argtypes = [vp, C.POINTER(LoopEvent), ci, C.POINTER(ci), C.POINTER(ci)]
     L.ll_mapper_loop_result.argtypes = [vp, C.POINTER(ci), C.POINTER(ci), vp, vp, ci, C.POINTER(PgEdge)]
     L.ll_mapper_loop_cloud.argtypes = [vp, ci, vp, sz, C.POINTER(sz), C.POINTER(vp)]
+    L.ll_spin_cfg_default.argtypes = [C.POINTER(SpinCfg)]
+    L.ll_spin_create.argtypes = [vp, C.POINTER(SpinCfg), C.POINTER(vp)]
+    L.ll_spin_release.argtypes = [vp]
+    L.ll_spin_extract.argtypes = [vp, vp, sz, ci, ci, vp]
+    L.ll_spin_cloud.argtypes = [vp, ci, vp, sz, C.POINTER(sz), C.POINTER(vp)]
+    L.ll_spin_point_info.argtypes = [vp, vp, vp, vp, vp, sz, C.POINTER(sz)]
+    L.ll_spin_chains.argtypes = [vp, C.POINTER(ci), C.POINTER(ci)]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64
     _LIB = L
     return L
+
+
+def default_spin_cfg(**kw) -> SpinCfg:
+    c = SpinCfg()
+    lib().ll_spin_cfg_default(C.byref(c))
+    for k, v in kw.items():
+        setattr(c, k, v)
+    return c
 
 
 def default_loop_cfg(**kw) -> LoopCfg:

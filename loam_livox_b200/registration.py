@@ -1152,3 +1152,81 @@ def image_info(image) -> dict:
     if st != capi.LL_OK:
         raise LoamLivoxError(f"status {st}: mapper image refused")
     return {n: (list(getattr(info, n)) if isinstance(getattr(info, n), C.Array) else getattr(info, n)) for n, _ in capi.ImageInfo._fields_ if n != "reserved"}
+
+
+class Laser_feature:
+    """The Velodyne branch of Laser_feature::laserCloudHandler (loam_livox/source/laser_feature_extractor.hpp:393-825; scan_line 16 or 64)
+    on the device.  laserCloudHandler(cloud) returns the five clouds the reference publishes: /laser_points_2, /laser_cloud_sharp,
+    /laser_cloud_less_sharp, /laser_cloud_flat, /laser_cloud_less_flat.  The 20-frame start-up delay stays the caller's."""
+
+    CLOUDS = ("full", "sharp", "less_sharp", "flat", "less_flat")
+
+    def __init__(self, ctx: Context, scan_line: int = 16, minimum_range: float = 0.1, plane_resolution: float = 0.4, max_points: int = 400000):
+        self.ctx = ctx
+        cfg = capi.default_spin_cfg(scan_line=scan_line, minimum_range=minimum_range, plane_resolution=plane_resolution, max_points=max_points)
+        h = C.c_void_p()
+        ctx.check(ctx._lib.ll_spin_create(ctx.h, C.byref(cfg), C.byref(h)))
+        self.h = h
+        self.counts = np.zeros(5, np.uint64)
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx._lib.ll_spin_release(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def extract(self, raw, where=capi.LL_HOST, n=None, fmt=None):
+        """One cloud: a float32 array [n, 4] / [n, 8] (where = LL_HOST), or a device pointer with n and fmt (LL_DEVICE); returns the counts."""
+        counts = (C.c_size_t * 5)()
+        if where == capi.LL_HOST and fmt is None:
+            raw, fmt = _pts(raw)
+            ptr, n = raw.ctypes.data, raw.shape[0]
+        elif where == capi.LL_HOST:
+            ptr = raw.ctypes.data if isinstance(raw, np.ndarray) else C.cast(C.c_char_p(raw), C.c_void_p).value
+        else:
+            ptr = raw
+        self.ctx.check(self.ctx._lib.ll_spin_extract(self.h, ptr, n, fmt, where, counts))
+        self.counts = np.array(list(counts), np.uint64)
+        return self.counts
+
+    def extract_from_pointcloud2(self, data: bytes, n_points: int):
+        """A sensor_msgs/PointCloud2 payload in the context's point layout (Context.set_point_layout)."""
+        buf = np.frombuffer(data, np.uint8)
+        return self.extract(np.ascontiguousarray(buf), capi.LL_HOST, n_points, capi.LL_FMT_STRIDED)
+
+    def cloud(self, which: int):
+        n, dev = C.c_size_t(), C.c_void_p()
+        self.ctx.check(self.ctx._lib.ll_spin_cloud(self.h, which, None, 0, C.byref(n), C.byref(dev)))
+        out = np.zeros((n.value, 4), np.float32)
+        self.ctx.check(self.ctx._lib.ll_spin_cloud(self.h, which, out.ctypes.data, n.value, C.byref(n), None))
+        return out
+
+    def device_cloud(self, which: int):
+        """(device pointer, point count) of a cloud, valid until the next extract: an LL_DEVICE input of ll_register / ll_map_build."""
+        n, dev = C.c_size_t(), C.c_void_p()
+        self.ctx.check(self.ctx._lib.ll_spin_cloud(self.h, which, None, 0, C.byref(n), C.byref(dev)))
+        return dev.value, n.value
+
+    def laserCloudHandler(self, raw):
+        self.extract(raw)
+        return {name: self.cloud(k) for k, name in enumerate(self.CLOUDS)}
+
+    def point_info(self):
+        """(ring, curvature, picked before the selection, label) per point of the full cloud."""
+        n = C.c_size_t()
+        self.ctx.check(self.ctx._lib.ll_spin_point_info(self.h, None, None, None, None, 0, C.byref(n)))
+        k = n.value
+        ring, curv, picked, label = np.zeros(k, np.int32), np.zeros(k, np.float32), np.zeros(k, np.int32), np.zeros(k, np.int32)
+        self.ctx.check(self.ctx._lib.ll_spin_point_info(self.h, ring.ctypes.data, curv.ctypes.data, picked.ctypes.data, label.ctypes.data, k, C.byref(n)))
+        return ring, curv, picked, label
+
+    def chains(self):
+        """(number of independent chains of the last selection, longest chain in points)."""
+        a, b = C.c_int(), C.c_int()
+        self.ctx.check(self.ctx._lib.ll_spin_chains(self.h, C.byref(a), C.byref(b)))
+        return a.value, b.value

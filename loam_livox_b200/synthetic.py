@@ -285,3 +285,58 @@ def trajectory(n_scans=1000, n_static=50, dt=0.1, speed=1.0, yaw_rate_deg=5.0, z
             y += speed * dt * math.sin(yaw) * 0.3
         poses.append(Pose(quat_from_euler(0.0, 0.0, yaw), np.array([x, y, 0.1])))
     return poses
+
+
+# ------------------------------------------------------------------ spinning lidar (Velodyne VLP-16 / HDL-64 geometry)
+def spin_elevations(scan_line):
+    """Nominal beam elevations (degrees) of a 16- or 64-beam sensor, laid out so that each beam lands in its own ring by the reference's
+    formulas (laser_feature_extractor.hpp:433-460): 16 beams -15 ... 15 in 2-degree steps; 64 beams +2 ... -8.33 in 1/3-degree steps, then
+    -8.83 ... -24.33 in half-degree steps (beams below ring 50 are dropped by the reference)."""
+    if scan_line == 16:
+        return np.array([-15.0 + 2.0 * k for k in range(16)])
+    if scan_line == 64:
+        return np.array([2.0 - k / 3.0 for k in range(32)] + [-8.83 - 0.5 * k for k in range(32)])
+    raise ValueError("scan_line must be 16 or 64")
+
+
+def _open_raycast(origin, dirs, max_range=100.0):
+    """First hit of rays with the floor plane of the room and its pillars, without walls or ceiling; no hit within max_range: inf."""
+    with np.errstate(divide="ignore", invalid="ignore"):
+        t_floor = np.where(dirs[:, 2] < -1e-9, (ROOM_LO[2] - origin[2]) / dirs[:, 2], np.inf)
+        best = t_floor
+        inv = 1.0 / dirs
+        for (px, py) in PILLARS:
+            lo = np.array([px - PILLAR_HALF, py - PILLAR_HALF, ROOM_LO[2]])
+            hi = np.array([px + PILLAR_HALF, py + PILLAR_HALF, ROOM_HI[2]])
+            a, b = (lo - origin) * inv, (hi - origin) * inv
+            tn, tf = np.nanmax(np.minimum(a, b), axis=1), np.nanmin(np.maximum(a, b), axis=1)
+            hit = (tn <= tf) & (tn > 1e-6)
+            best = np.where(hit & (tn < best), tn, best)
+    return np.where(best <= max_range, best, np.inf)
+
+
+def make_spinning_scan(scan_line=16, pose=None, seed=SEED, n_azimuth=1800, start_azimuth_deg=0.0, sweep_deg=360.0, range_sigma=0.004,
+                       nan_frac=0.0, near_frac=0.0, scene="room"):
+    """One sweep of a spinning lidar in the sensor frame, float32 [n_azimuth * scan_line, 4] = x, y, z, intensity, in a driver's firing
+    order: all beams of one azimuth (in beam order), then the next azimuth clockwise (the azimuth decreases, so the reference's orientation
+    -atan2(y, x) grows), from start_azimuth_deg over sweep_deg.  scene "room" ray-casts the closed room, "open" only its floor and pillars (a
+    ray that hits nothing is a NaN point, as drivers publish them).  nan_frac / near_frac of the points are replaced by NaNs / points at 5 cm."""
+    pose = pose or Pose(quat_from_euler(0.0, 0.0, 0.05), np.array([0.3, 0.2, 0.1]))
+    rng = np.random.default_rng(seed)
+    el = np.radians(spin_elevations(scan_line))
+    az = np.radians(start_azimuth_deg - sweep_deg * np.arange(n_azimuth) / n_azimuth)
+    A, E = np.meshgrid(az, el, indexing="ij")   # [azimuth, beam]: firing order
+    d = np.stack([np.cos(E) * np.cos(A), np.cos(E) * np.sin(A), np.sin(E)], axis=-1).reshape(-1, 3)
+    dw = d @ pose.R().T
+    r = raycast(pose.t, dw) if scene == "room" else _open_raycast(pose.t, dw)
+    r = r + rng.normal(0.0, range_sigma, r.shape[0])
+    with np.errstate(invalid="ignore"):
+        pts = d * r[:, None]
+    inten = rng.uniform(1.0, 100.0, r.shape[0])
+    out = np.concatenate([pts, inten[:, None]], axis=1).astype(np.float32)
+    out[~np.isfinite(r), :3] = np.nan
+    near = rng.random(out.shape[0]) < near_frac
+    out[near, :3] = (d[near] * 0.05).astype(np.float32)
+    nan = rng.random(out.shape[0]) < nan_frac
+    out[nan, :3] = np.nan
+    return out
