@@ -857,6 +857,28 @@ int  ll_spin_point_info(ll_spin* spin, int32_t* ring, float* curvature, int32_t*
 /* Diagnostics of the last extract: chains of the selection and the longest one in points. */
 int  ll_spin_chains(const ll_spin* spin, int* n_chains, int* longest);
 
+/* ---- streaming mapper on spinning-lidar sweeps (DESIGN.md §4.7.1) --------------------------------------------------------------------
+ * The reference maps a Velodyne by remapping the feature node's /laser_cloud_less_sharp, /laser_cloud_less_flat and /laser_points_2 onto the
+ * mapping node's /pc2_corners, /pc2_surface and /pc2_full.  ll_mapper_process_sweep is that pipeline in one call: the whole spin front end
+ * (as ll_spin_extract), the mapping node's input VoxelGrids on the less-sharp cloud (pipeline.mapping_leaf_corner) and the less-flat cloud
+ * (pipeline.mapping_leaf_surf), max_t = the largest intensity of the full cloud (-10000 when it is empty; there are no time stamps), then the
+ * mapper step of ll_mapper_process_scan (refresh, registration, append, pose, recovery and loop closure).  Every sweep registers as one
+ * scan: the frame index counts sweeps, and a sweep with fewer than 5 kept points goes through the step with 0 features (past the registration
+ * gate that is LL_ERR_NO_BLOCKS, as for any empty scan: the frame index counted, nothing appended, the pose kept).  After a successful
+ * call ll_spin_cloud gives the last sweep's five clouds, equal to ll_spin_extract's.  spin and mapper must share one context.
+ * Refusals, with nothing changed: LL_ERR_INVALID for null pointers, n_sweeps < 1, an unknown fmt / where or a spin handle of another context;
+ * LL_ERR_CAPACITY for a sweep over the handle's max_points or, with loop closure on, over the context's max_scan_points
+ * (the full cloud loop closure takes from one step).
+ * Features over max_features after the VoxelGrids: LL_ERR_CAPACITY before that sweep's registration (the mapper unchanged by it).
+ * The 20-frame start-up delay (m_para_system_delay) stays the caller's. */
+int  ll_mapper_process_sweep(ll_mapper* mapper, ll_spin* spin, const void* raw, size_t n, int fmt, int where, ll_reg_result* out, ll_mapper_stats* stats);
+/* n_sweeps sweeps: the results of n_sweeps calls of ll_mapper_process_sweep (out[k], stats[k]; every field but gpu_ms_* and the float
+ * timings), the front end of sweep k + 1 running under the step of sweep k.  Validated before anything is enqueued; an error at sweep f stops
+ * there with *n_sweeps_done = f and the mapper as after the single calls up to f (ll_spin_cloud then has nothing extracted when sweep f + 1
+ * had been enqueued ahead). */
+int  ll_mapper_process_sweeps(ll_mapper* mapper, ll_spin* spin, int n_sweeps, const void* const* raws, const size_t* ns, int fmt, int where,
+                              ll_reg_result* out, ll_mapper_stats* stats, int* n_sweeps_done);
+
 /* ---- multi-GPU ------------------------------------------------------------------------------------- */
 /* One process per GPU.  The 28-double normal equations (+4 counters) are all-reduced inside the solver kernel
  * through peer-mapped staging buffers (CUDA IPC over NVLink); the host only exchanges the IPC handles once. */

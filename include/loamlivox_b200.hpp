@@ -208,6 +208,8 @@ class Points_cloud_map {
   Context& ctx_; ll_cellmap* map_ = nullptr;
 };
 
+class Laser_feature;
+
 // ---- Laser_mapping::process_new_scan with everything on the device (laser_mapping.hpp:1316-1521 + :460-566, matching_mode 0 and 1) ----
 class Laser_mapping {
  public:
@@ -279,6 +281,13 @@ class Laser_mapping {
     std::vector<int> status; for (const ll_reg_result& x : r) status.push_back(x.status);
     return status;
   }
+  // one spinning-lidar sweep through `front`'s Velodyne front end into this mapper (ll_mapper_process_sweep: less sharp -> corners, less flat
+  // -> surfaces, the full cloud's largest intensity -> max_t); front's device clouds are then this sweep's.  Returns the registration status.
+  int process_new_sweep(Laser_feature& front, const PointCloud& raw, ll_reg_result* result = nullptr, ll_mapper_stats* stats = nullptr);
+  // several sweeps of recorded data in one call: what process_new_sweep returns for each in turn, the front end of sweep k + 1 under the mapper
+  // step of sweep k.  On an error results / stats hold the sweeps completed before Error is thrown; *done = their number.
+  std::vector<int> process_new_sweeps(Laser_feature& front, const std::vector<PointCloud>& raws, std::vector<ll_reg_result>* results = nullptr,
+                                      std::vector<ll_mapper_stats>* stats = nullptr, int* done_out = nullptr);
   // the whole mapper as one byte image (ll_mapper_save; format in loamlivox_b200.h): load_from_image of it, on any context, continues bit for
   // bit as this mapper does.  The mapper is not modified.
   void save_to_image(std::vector<uint8_t>& image) const {
@@ -489,5 +498,28 @@ class Laser_feature {
   Context& ctx_;
   ll_spin* h_ = nullptr;
 };
+
+inline int Laser_mapping::process_new_sweep(Laser_feature& front, const PointCloud& raw, ll_reg_result* result, ll_mapper_stats* stats) {
+  ll_reg_result r; ll_mapper_stats st;
+  ctx_.check(ll_mapper_process_sweep(mapper_, front.get(), raw.data(), raw.size(), LL_FMT_PCL32, LL_HOST, &r, &st));
+  ctx_.check(ll_mapper_pose(mapper_, m_q_w_curr.data(), m_t_w_curr.data(), &m_current_frame_index));
+  if (result) *result = r; if (stats) *stats = st;
+  return r.status;
+}
+inline std::vector<int> Laser_mapping::process_new_sweeps(Laser_feature& front, const std::vector<PointCloud>& raws, std::vector<ll_reg_result>* results,
+                                                          std::vector<ll_mapper_stats>* stats, int* done_out) {
+  if (raws.empty()) throw Error(LL_ERR_INVALID, "no sweeps");
+  std::vector<const void*> ptrs; std::vector<size_t> ns;
+  for (const PointCloud& c : raws) { ptrs.push_back(c.data()); ns.push_back(c.size()); }
+  std::vector<ll_reg_result> r(raws.size()); std::vector<ll_mapper_stats> st(raws.size()); int done = 0;
+  const int rc = ll_mapper_process_sweeps(mapper_, front.get(), (int)raws.size(), ptrs.data(), ns.data(), LL_FMT_PCL32, LL_HOST, r.data(), st.data(), &done);
+  r.resize(rc == LL_OK ? raws.size() : (size_t)done); st.resize(r.size());
+  if (results) *results = r; if (stats) *stats = st;
+  if (done_out) *done_out = done;
+  ctx_.check(ll_mapper_pose(mapper_, m_q_w_curr.data(), m_t_w_curr.data(), &m_current_frame_index));
+  ctx_.check(rc);
+  std::vector<int> status; for (const ll_reg_result& x : r) status.push_back(x.status);
+  return status;
+}
 
 }  // namespace ll200

@@ -50,6 +50,7 @@ EXPORTS = [
     "ll_keyframe_images", "ll_keyframe_cloud", "ll_loop_cfg_default", "ll_loop_search",
     "ll_mapper_loop_closure_default", "ll_mapper_set_loop_closure", "ll_mapper_loop_read", "ll_mapper_loop_result", "ll_mapper_loop_cloud",
     "ll_spin_cfg_default", "ll_spin_create", "ll_spin_release", "ll_spin_extract", "ll_spin_cloud", "ll_spin_point_info", "ll_spin_chains",
+    "ll_mapper_process_sweep", "ll_mapper_process_sweeps",
 ]
 LL_SPIN_FULL, LL_SPIN_SHARP, LL_SPIN_LESS_SHARP, LL_SPIN_FLAT, LL_SPIN_LESS_FLAT = 0, 1, 2, 3, 4
 LL_CELL_SPHERE, LL_CELL_LINE, LL_CELL_PLANE, LL_CELL_ALL = 0, 1, 2, -1
@@ -344,6 +345,8 @@ def lib():
     L.ll_spin_cloud.argtypes = [vp, ci, vp, sz, C.POINTER(sz), C.POINTER(vp)]
     L.ll_spin_point_info.argtypes = [vp, vp, vp, vp, vp, sz, C.POINTER(sz)]
     L.ll_spin_chains.argtypes = [vp, C.POINTER(ci), C.POINTER(ci)]
+    L.ll_mapper_process_sweep.argtypes = [vp, vp, vp, sz, ci, ci, C.POINTER(RegResult), C.POINTER(MapperStats)]
+    L.ll_mapper_process_sweeps.argtypes = [vp, vp, ci, vp, vp, ci, ci, C.POINTER(RegResult), C.POINTER(MapperStats), C.POINTER(ci)]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64
     _LIB = L

@@ -276,6 +276,17 @@ struct FrameArena { FrameDev* dev; float4* cls[2]; float4* mid[2]; int cap; DevB
 int frame_front_end(ll_ctx* ctx, const FrontStreams& fs, const FrameArena& fa, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
                     int pieces, const ll_pipeline_cfg* pc);
 
+// ---------------------------------------------------------------------------------------------- spinning-lidar sweeps (spin.cu)
+// The streaming mapper's front end of a sweep (ll_mapper_process_sweep(s)): enqueue runs ll_spin_extract's front end on `fs` plus the mapping
+// node's input VoxelGrids (pc->mapping_leaf_corner / _surf) and max_t, without a host synchronisation; once that work has completed, finish
+// reads the counts (the handle's clouds are then this sweep's), applies max_features and copies the features into A.feat on `s`.
+ll_ctx* spin_ctx(const ll_spin* h);
+size_t spin_max_points(const ll_spin* h);
+int spin_sweep_enqueue(ll_spin* h, const FrontStreams& fs, const void* raw, size_t n, int fmt, int where, const ll_pipeline_cfg* pc);
+int spin_sweep_finish(ll_spin* h, cudaStream_t s, size_t n, int* nc_out, int* ns_out, float* max_t);
+const float4* spin_full_cloud(const ll_spin* h, int* n, const int** d_n);   // the last finished sweep's full cloud and its device count
+void spin_forget(ll_spin* h);   // the device clouds no longer match the counts (a sweep enqueued ahead of a failed step): nothing extracted
+
 // ---------------------------------------------------------------------------------------------- streaming mapper (mapper.cu, loop.cu)
 // m_laser_cloud_{corner,surface}_history (std::list<PointCloud>, :1446-1478) as ONE flat device array: the clouds of the window lie one after the
 // other in push order, so the concatenation of mode 0 (:518-531) is the live range itself.  Two arenas, ping-pong: when the tail reaches the end of
@@ -325,6 +336,10 @@ int  loop_set(ll_ctx* ctx, LoopClosure** lc, const ll_loop_closure_cfg* cfg, con
 void loop_release(LoopClosure* lc);
 int  loop_scan_cloud(ll_ctx* ctx, LoopClosure* lc, const ll_pipeline_cfg* pc);
 int  loop_frame_clouds(ll_ctx* ctx, LoopClosure* lc, const FrameDev* dev, const size_t* ns, int n_heads, int publish);
+// A sweep's full ring-ordered cloud (m_laser_cloud_full_res of the remapped Velodyne pipeline): the n points at `full`, a spin handle's buffer,
+// with the device count d_n as its one segment.  Runs before the next sweep's front end may overwrite `full`.
+int  loop_sweep_cloud(ll_ctx* ctx, LoopClosure* lc, const float4* full, int n, const int* d_n);
+size_t loop_step_capacity(const LoopClosure* lc);   // points of the full cloud one step can hand over (max_scan_points: the world-frame buffer, one append)
 void loop_select_piece(LoopClosure* lc, int i);
 int  loop_step(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool pushed, int frame_index, const double q_w_curr[4], const double t_w_curr[3]);
 int  loop_read(LoopClosure* lc, ll_loop_event* out, int cap, int* n, int* n_dropped);

@@ -235,6 +235,18 @@ int loop_frame_clouds(ll_ctx* ctx, LoopClosure* lc, const FrameDev* dev, const s
   return LL_OK;
 }
 
+int loop_sweep_cloud(ll_ctx* ctx, LoopClosure* lc, const float4* full, int n, const int* d_n) {
+  if (lc->closed || lc->stopped) return LL_OK;
+  cudaStream_t s = ctx->stream;
+  LoopInLayout il; LL_CUDA(ctx, lc->in.carve([&](Carve& k) { il.layout(k, lc->in_full, lc->in_scan); }));
+  if (n > 0) LL_CUDA(ctx, cudaMemcpyAsync(il.full, full, (size_t)n * 16, cudaMemcpyDeviceToDevice, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(il.seg_end, d_n, sizeof(int), cudaMemcpyDeviceToDevice, s));   // one segment: the full cloud
+  lc->seg.assign(1, 0); lc->seg_read = false; lc->piece = 0;
+  return LL_OK;
+}
+
+size_t loop_step_capacity(const LoopClosure* lc) { return lc->in_scan; }   // loop_step_work transforms one step's cloud into `world` (in_scan points)
+
 void loop_select_piece(LoopClosure* lc, int i) { lc->piece = i; }
 
 namespace {

@@ -318,16 +318,17 @@ static int first_piece_over(const ll_mapper* m, const FrameOut& fo, int publish)
 // A front end enqueued ahead of an input that then fails: it is drained (it reads the caller's inputs) and its host bookkeeping undone, so that
 // the extractor stands where the one-by-one calls leave it.
 struct Ahead { ExtractState saved; bool on = false; };
+static void sequence_drain(const FrontStreams& fs) { for (cudaStream_t s : {fs.main, fs.corner, fs.petals}) cudaStreamSynchronize(s); }
 static void sequence_unwind(ll_ctx* ctx, const FrontStreams& fs, const Ahead& a) {
-  for (cudaStream_t s : {fs.main, fs.corner, fs.petals}) cudaStreamSynchronize(s);
+  sequence_drain(fs);
   if (a.on) ctx->ex = a.saved;
 }
-// Host records are staged in stage_in: reserved for max_scan_points records before the first front end, because a reallocation (cudaFree)
-// would synchronise the device in the middle of the sequence.
-static int reserve_stage(ll_ctx* ctx, int fmt, int where) {
+// Host records are staged in stage_in: reserved for `points` records (max_scan_points, or a spin handle's max_points) before the first front
+// end, because a reallocation (cudaFree) would synchronise the device in the middle of the sequence.
+static int reserve_stage(ll_ctx* ctx, int fmt, int where, size_t points) {
   if (where != LL_HOST || fmt == LL_FMT_XYZI16) return LL_OK;
   const size_t rec = fmt == LL_FMT_PCL32 ? 32 : (size_t)ctx->layout.point_step;
-  LL_CUDA(ctx, ctx->stage_in.reserve((size_t)ctx->cfg.max_scan_points * rec));
+  LL_CUDA(ctx, ctx->stage_in.reserve(points * rec));
   return LL_OK;
 }
 
@@ -367,7 +368,7 @@ static int frames_check(ll_mapper* m, int n_frames, int n_heads, const void* con
 static int frames_run(ll_mapper* m, const FrontStreams& fs, int n_frames, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where,
                       const double* stamps, int pieces, int publish, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces, int* done) {
   ll_ctx* ctx = m->ctx;
-  LL_TRY(reserve_stage(ctx, fmt, where));
+  LL_TRY(reserve_stage(ctx, fmt, where, (size_t)ctx->cfg.max_scan_points));
   for (int f = 0; f < n_frames; f++) n_pieces[f] = 0;
   FrameArena fa[2]; LL_TRY(frame_arena(m, 0, &fa[0])); LL_TRY(frame_arena(m, 1, &fa[1]));
   auto enqueue = [&](int f) -> int {   // frame f's front end into arena f & 1, behind the last copy out of it (frame f - 2's)
@@ -447,49 +448,93 @@ extern "C" int ll_mapper_process_frames(ll_mapper* m, int n_frames, int n_heads,
   return frames_run(m, ctx->pipe_front(), n_frames, n_heads, raws, ns, fmt, where, stamps, pieces, publish, out, stats, cap, n_pieces, n_frames_done);
 }
 
-// Scan k: the front end, its features into A.feat (scan_front_end_finish) and mapper_step.
-static int scans_run(ll_mapper* m, const FrontStreams& fs, int n_scans, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
-                     ll_reg_result* out, ll_mapper_stats* stats, int* done) {
+// The front end of one kind of single-scan input (a Livox scan, a spinning-lidar sweep) as inputs_run drives it:
+//   enqueue(k)     input k's front end on fs.main (inputs_run orders it behind fe_free[0], the copy of input k - 1's features);
+//   finish(k, ..)  once it has completed: its feature counts, max_t and whether it is dropped, its features copied into A.feat on the context's
+//                  stream (LL_ERR_CAPACITY past max_features, before anything of the step is enqueued);
+//   loop_cloud(k)  its full cloud into the loop closure's input, before the next front end may overwrite it;
+//   save / restore the host bookkeeping around a front end enqueued ahead of an input that then fails.
+struct ScanFront {
+  ll_ctx* ctx; const FrontStreams& fs; const void* const* raws; const size_t* ns; int fmt, where; const double* stamps; const ll_pipeline_cfg* pc;
+  ExtractState saved;
+  int enqueue(int k) { return scan_front_end_enqueue(ctx, fs, raws[k], ns[k], fmt, where, stamps[k], pc); }
+  int finish(int, int* nc, int* nsf, double* max_t, bool* dropped) {
+    int d = 0;
+    LL_TRY(scan_front_end_finish(ctx, ctx->stream, pc, nc, nsf, &d));   // reads the pinned counts before the next front end is enqueued
+    *dropped = d != 0; *max_t = (double)ctx->last_full_max_t;
+    return LL_OK;
+  }
+  int loop_cloud(LoopClosure* lc, int) { return loop_scan_cloud(ctx, lc, pc); }   // the full cloud, compacted again from the extractor's state
+  void save() { saved = ctx->ex; }
+  void restore() { ctx->ex = saved; }
+};
+// A sweep: the spin handle's front end and the mapping node's VoxelGrids (spin_sweep_enqueue).  It is never dropped: every sweep registers.
+struct SweepFront {
+  ll_ctx* ctx; ll_spin* spin; const FrontStreams& fs; const void* const* raws; const size_t* ns; int fmt, where; const ll_pipeline_cfg* pc;
+  int enqueue(int k) { return spin_sweep_enqueue(spin, fs, raws[k], ns[k], fmt, where, pc); }
+  int finish(int k, int* nc, int* nsf, double* max_t, bool* dropped) {
+    float mt = 0.f;
+    const int st = spin_sweep_finish(spin, ctx->stream, ns[k], nc, nsf, &mt);
+    *dropped = false; *max_t = (double)mt;
+    return st;
+  }
+  int loop_cloud(LoopClosure* lc, int) { int n = 0; const int* d_n = nullptr; const float4* full = spin_full_cloud(spin, &n, &d_n); return loop_sweep_cloud(ctx, lc, full, n, d_n); }
+  void save() {}
+  void restore() { spin_forget(spin); }
+};
+
+// Input k: the front end, its features into A.feat and mapper_step.
+template <typename Front>
+static int inputs_run(ll_mapper* m, Front& fe, const FrontStreams& fs, int n_inputs, ll_reg_result* out, ll_mapper_stats* stats, int* done) {
   ll_ctx* ctx = m->ctx;
-  const ll_pipeline_cfg* pc = &m->cfg.pipeline;
-  LL_TRY(reserve_stage(ctx, fmt, where));
-  auto enqueue = [&](int k) -> int {   // behind the copy of scan k - 1's features out of tmp_a / tmp_b
+  auto enqueue = [&](int k) -> int {   // behind the copy of input k - 1's features out of the front end's buffers
     LL_CUDA(ctx, cudaStreamWaitEvent(fs.main, ctx->sev.fe_free[0], 0));
-    LL_TRY(scan_front_end_enqueue(ctx, fs, raws[k], ns[k], fmt, where, stamps[k], pc));
+    LL_TRY(fe.enqueue(k));
     LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_ready, fs.main));
     return LL_OK;
   };
-  Ahead ahead;
+  bool ahead = false;
   const int st = [&]() -> int {
     double t = now_ms();
     LL_TRY(enqueue(0));
     float ms_enqueue = (float)(now_ms() - t);
-    for (int k = 0; k < n_scans; k++) {
-      ahead.on = false;
+    for (int k = 0; k < n_inputs; k++) {
+      ahead = false;
       ll_mapper_stats* ps = stats ? stats + k : nullptr;
       if (ps) memset(ps, 0, sizeof(*ps));
       t = now_ms();
       LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.fe_ready));
-      int nc = 0, nsf = 0, dropped = 0;
-      LL_TRY(scan_front_end_finish(ctx, ctx->stream, pc, &nc, &nsf, &dropped));   // reads the pinned counts before the next front end is enqueued
-      if (m->lc && !dropped) LL_TRY(loop_scan_cloud(ctx, m->lc, pc));            // the full cloud, before the next front end overwrites the extractor
+      int nc = 0, nsf = 0; double max_t = 0; bool dropped = false;
+      LL_TRY(fe.finish(k, &nc, &nsf, &max_t, &dropped));
+      if (m->lc && !dropped) LL_TRY(fe.loop_cloud(m->lc, k));
       LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[0], ctx->stream));
       const float ms_front_end = ms_enqueue + (float)(now_ms() - t);
-      if (k + 1 < n_scans) {
-        ahead.saved = ctx->ex; ahead.on = true;
+      if (k + 1 < n_inputs) {
+        fe.save(); ahead = true;
         const double t1 = now_ms();
         LL_TRY(enqueue(k + 1));
         ms_enqueue = (float)(now_ms() - t1);
       }
       out_init(m, out + k);
       if (ps) { ps->n_corner = nc; ps->n_surf = nsf; ps->ms_front_end = ms_front_end; }
-      if (!dropped) LL_TRY(mapper_step(m, nc, nsf, (double)ctx->last_full_max_t, out + k, ps));   // laser_feature_extractor.hpp:287
+      if (!dropped) LL_TRY(mapper_step(m, nc, nsf, max_t, out + k, ps));   // laser_feature_extractor.hpp:287
       *done = k + 1;
     }
     return LL_OK;
   }();
-  if (st != LL_OK) sequence_unwind(ctx, fs, ahead);
+  if (st != LL_OK) {   // sequence_unwind for any front end
+    sequence_drain(fs);
+    if (ahead) fe.restore();
+  }
   return st;
+}
+
+static int scans_run(ll_mapper* m, const FrontStreams& fs, int n_scans, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+                     ll_reg_result* out, ll_mapper_stats* stats, int* done) {
+  ll_ctx* ctx = m->ctx;
+  LL_TRY(reserve_stage(ctx, fmt, where, (size_t)ctx->cfg.max_scan_points));
+  ScanFront fe{ctx, fs, raws, ns, fmt, where, stamps, &m->cfg.pipeline, ExtractState()};
+  return inputs_run(m, fe, fs, n_scans, out, stats, done);
 }
 
 extern "C" int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int where, double stamp, ll_reg_result* out, ll_mapper_stats* stats) {
@@ -507,6 +552,44 @@ extern "C" int ll_mapper_process_scans(ll_mapper* m, int n_scans, const void* co
   ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
   LL_TRY(scans_check(ctx, n_scans, raws, ns, fmt, where));
   return scans_run(m, ctx->pipe_front(), n_scans, raws, ns, fmt, where, stamps, out, stats, n_scans_done);
+}
+
+// Sweeps: the spin handle must share the mapper's context; a sweep over the handle's max_points, or, with loop closure on, over the loop
+// closure's per-step full cloud (max_scan_points: a sweep's whole kept cloud is one step's, and the kept points can only be fewer), is
+// LL_ERR_CAPACITY before anything is enqueued.
+static int sweeps_check(ll_mapper* m, ll_spin* spin, int n_sweeps, const void* const* raws, const size_t* ns, int fmt, int where) {
+  ll_ctx* ctx = m->ctx;
+  if (spin_ctx(spin) != ctx) { ctx->set_error("spin handle created on another context than the mapper"); return LL_ERR_INVALID; }
+  LL_TRY(check_clouds(ctx, fmt, where, (size_t)n_sweeps, raws, ns));
+  for (int k = 0; k < n_sweeps; k++) {
+    if (ns[k] > spin_max_points(spin)) { ctx->set_error("sweep " + std::to_string(k) + " larger than the spin handle's max_points"); return LL_ERR_CAPACITY; }
+    if (m->lc && ns[k] > loop_step_capacity(m->lc)) { ctx->set_error("sweep " + std::to_string(k) + " larger than max_scan_points with loop closure on"); return LL_ERR_CAPACITY; }
+  }
+  return LL_OK;
+}
+static int sweeps_run(ll_mapper* m, ll_spin* spin, const FrontStreams& fs, int n_sweeps, const void* const* raws, const size_t* ns, int fmt, int where,
+                      ll_reg_result* out, ll_mapper_stats* stats, int* done) {
+  ll_ctx* ctx = m->ctx;
+  LL_TRY(reserve_stage(ctx, fmt, where, spin_max_points(spin)));
+  SweepFront fe{ctx, spin, fs, raws, ns, fmt, where, &m->cfg.pipeline};
+  return inputs_run(m, fe, fs, n_sweeps, out, stats, done);
+}
+
+extern "C" int ll_mapper_process_sweep(ll_mapper* m, ll_spin* spin, const void* raw, size_t n, int fmt, int where, ll_reg_result* out, ll_mapper_stats* stats) {
+  if (!m || !spin || !out) return LL_ERR_INVALID;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  int done = 0;
+  LL_TRY(sweeps_check(m, spin, 1, &raw, &n, fmt, where));
+  return sweeps_run(m, spin, ctx->own_front(), 1, &raw, &n, fmt, where, out, stats, &done);
+}
+
+extern "C" int ll_mapper_process_sweeps(ll_mapper* m, ll_spin* spin, int n_sweeps, const void* const* raws, const size_t* ns, int fmt, int where,
+                                        ll_reg_result* out, ll_mapper_stats* stats, int* n_sweeps_done) {
+  if (n_sweeps_done) *n_sweeps_done = 0;
+  if (!m || !spin || !out || !raws || !ns || !n_sweeps_done || n_sweeps < 1) return LL_ERR_INVALID;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  LL_TRY(sweeps_check(m, spin, n_sweeps, raws, ns, fmt, where));
+  return sweeps_run(m, spin, ctx->pipe_front(), n_sweeps, raws, ns, fmt, where, out, stats, n_sweeps_done);
 }
 
 // ---------------------------------------------------------------------------------------------- checkpoint

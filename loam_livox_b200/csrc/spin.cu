@@ -47,6 +47,7 @@ struct SpinMeta {
   int lf_cnt[SPIN_MAX_RINGS], lf_end[SPIN_MAX_RINGS], vg_end[SPIN_MAX_RINGS];
   int nlf;                       // less-flat points before the VoxelGrid (DeviceSelect count)
   int counts[8];                 // N, sharp, less sharp, flat, less flat, chains, longest chain (points), less flat before the VoxelGrid
+  int feat[4];                   // streaming mapper input: corners and surfaces after the mapping node's VoxelGrids, ll_f2ord of max_t, unused
 };
 
 struct ll_spin {
@@ -56,13 +57,17 @@ struct ll_spin {
   int last_counts[8] = {0};
   int extracted = 0, last_n = 0;
   DevBuf arena, vg_scratch;
-  int* pin = nullptr;            // pinned: SpinMeta::counts
+  int* pin = nullptr;            // pinned: SpinMeta::counts, then SpinMeta::feat (the streaming mapper's sweeps)
   // arena
   float4* in4; float4* filt; float4* cloud; int* rkey[2]; int* rval[2]; unsigned long long* ckey[2]; int* cval[2];
   float* curv; unsigned char* occl; unsigned char* beam; unsigned* picked; unsigned* picked0; unsigned* cut; signed char* label; short* sid;
   unsigned char* lfflag; int* sharp_idx; int* flat_idx;
   float4* out_sharp; float4* out_less_sharp; float4* out_flat; float4* lf_raw; float4* out_less_flat;
   SpinMeta* meta; char* tmp; size_t tmp_bytes = 0;
+  // the streaming mapper's input (spin_sweep_enqueue): the mapping node's VoxelGrid of the less-sharp cloud lands in mvg_corner (with its own
+  // scratch, the chain may run on a second stream), that of the less-flat cloud in lf_raw (free once the per-ring VoxelGrid has read it)
+  DevBuf mvg, vg_scratch2;
+  float4* mvg_corner = nullptr;
 };
 
 static int spin_key_bits(int m) { int b = 0; while ((1 << b) < m) b++; return 32 + b; }
@@ -392,6 +397,23 @@ __global__ void spin_out_kernel(const float4* __restrict__ cloud, SpinMeta* __re
 }
 __global__ void spin_final_kernel(SpinMeta* __restrict__ m, int rings) { m->counts[4] = m->vg_end[rings - 1]; }
 
+// The streaming mapper's max_t: the largest intensity (ring + 0.1 relTime) of the full cloud, from find_min_max_intensity's start value -10000
+// (laser_mapping.hpp:1243-1253, :1336-1347).  One block; the intensities are finite, so the order-preserving int max is the float max.
+#define SPIN_MAXT_THREADS 1024
+__global__ void __launch_bounds__(SPIN_MAXT_THREADS) spin_max_t_kernel(const float4* __restrict__ cloud, SpinMeta* __restrict__ m) {
+  __shared__ int wmax[SPIN_MAXT_THREADS / 32];
+  const int N = m->counts[0];
+  int mx = ll_f2ord(-10000.0f);
+  for (int i = threadIdx.x; i < N; i += SPIN_MAXT_THREADS) mx = max(mx, ll_f2ord(cloud[i].w));
+  mx = __reduce_max_sync(FULL, mx);
+  if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = mx;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    mx = __reduce_max_sync(FULL, wmax[threadIdx.x]);
+    if (threadIdx.x == 0) m->feat[2] = mx;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------------------------------------------------ host
 static void spin_layout(ll_spin* h, Carve& c) {
   const int M = h->cfg.max_points, G = h->rings * SPIN_SUB;
@@ -408,6 +430,7 @@ static void spin_layout(ll_spin* h, Carve& c) {
   h->meta = c.take<SpinMeta>(1);
   h->tmp = c.take<char>(h->tmp_bytes);
 }
+static int spin_corner_cap(const ll_spin* h) { return std::min(h->cfg.max_points, h->rings * SPIN_SUB * SPIN_SHARP_MAX); }   // out_less_sharp's size
 static size_t spin_tmp_bytes(int M) {
   size_t a = 0, b = 0, d = 0, e = 0;
   cub::DeviceSelect::If(nullptr, a, (float4*)nullptr, (float4*)nullptr, (int*)nullptr, M, SpinFilter{0.f});
@@ -417,9 +440,13 @@ static size_t spin_tmp_bytes(int M) {
   return std::max(std::max(a, b), std::max(d, e));
 }
 
-static int spin_run(ll_spin* h, const void* raw, size_t n_, int fmt, int where) {
+// The front end on the streams fs (the extraction on fs.main).  mapping == null (ll_spin_extract): the counts read back with one synchronisation.
+// Otherwise (the streaming mapper's sweep) also the mapping node's input VoxelGrids (laser_mapping.hpp:1367-1373) on the device counts of the
+// less-sharp and less-flat clouds, one stage per chain, and max_t; SpinMeta::counts and ::feat land in the pinned block, without a
+// synchronisation (spin_sweep_finish reads them once the work has completed).
+static int spin_run(ll_spin* h, const FrontStreams& fs, const void* raw, size_t n_, int fmt, int where, const ll_pipeline_cfg* mapping) {
   ll_ctx* ctx = h->ctx;
-  cudaStream_t s = ctx->stream;
+  cudaStream_t s = fs.main;
   const int n = (int)n_, R = h->rings, G = R * SPIN_SUB, B = 256, nb = ll_div_up(n, B);
   SpinMeta* m = h->meta;
   LL_CUDA(ctx, cudaMemsetAsync(m, 0, sizeof(SpinMeta), s));
@@ -448,10 +475,53 @@ static int spin_run(ll_spin* h, const void* raw, size_t n_, int fmt, int where) 
   // select (2), ring sort (histogram, scan, 1 pass), curvature sort (histogram, scan, one pass per 8 key bits), flagged select (2), 10 kernels
   ctx->launches += 2 + 3 + 2 + (uint64_t)(spin_key_bits(h->cfg.max_points) + 7) / 8 + 2 + 10;
   LL_CUDA(ctx, cudaGetLastError());
-  LL_CUDA(ctx, cudaMemcpyAsync(h->pin, m->counts, sizeof(m->counts), cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  if (!mapping) {
+    LL_CUDA(ctx, cudaMemcpyAsync(h->pin, m->counts, sizeof(m->counts), cudaMemcpyDeviceToHost, s));
+    LL_CUDA(ctx, cudaStreamSynchronize(s));
+    return LL_OK;
+  }
+  // less sharp -> corners at mapping_leaf_corner, less flat -> surfaces at mapping_leaf_surf (the remapped /pc2_corners and /pc2_surface)
+  const VgChain c[2] = {
+      {{h->out_less_sharp, std::min(n, spin_corner_cap(h)), &m->counts[2], 1, {mapping->mapping_leaf_corner, 0.f}, {h->mvg_corner, nullptr}, {&m->feat[0], nullptr}},
+       &h->vg_scratch2, fs.corner},
+      {{h->out_less_flat, n, &m->counts[4], 1, {mapping->mapping_leaf_surf, 0.f}, {h->lf_raw, nullptr}, {&m->feat[1], nullptr}}, &h->vg_scratch, fs.main}};
+  LL_TRY(launch_voxel_chains(ctx, s, c, 2, fs.fork, fs.join));
+  spin_max_t_kernel<<<1, SPIN_MAXT_THREADS, 0, s>>>(h->cloud, m); ctx->launches++;
+  LL_CUDA(ctx, cudaGetLastError());
+  static_assert(offsetof(SpinMeta, feat) == offsetof(SpinMeta, counts) + sizeof(SpinMeta::counts), "counts and feat are read back together");
+  LL_CUDA(ctx, cudaMemcpyAsync(h->pin, m->counts, sizeof(m->counts) + sizeof(m->feat), cudaMemcpyDeviceToHost, s));
   return LL_OK;
 }
+
+// ------------------------------------------------------------------------------------------------------ the streaming mapper's sweeps
+ll_ctx* spin_ctx(const ll_spin* h) { return h->ctx; }
+size_t spin_max_points(const ll_spin* h) { return (size_t)h->cfg.max_points; }
+
+int spin_sweep_enqueue(ll_spin* h, const FrontStreams& fs, const void* raw, size_t n, int fmt, int where, const ll_pipeline_cfg* pc) {
+  if (n == 0) {   // no front end: the counts of an empty sweep (the pinned block is free, the previous sweep's finish has read it), and the
+                  // device count of the full cloud that loop_sweep_cloud hands on, in stream order behind the previous sweep's copy (fe_free)
+    for (int k = 0; k < 12; k++) h->pin[k] = 0;
+    h->pin[10] = ll_f2ord(-10000.0f);
+    LL_CUDA(h->ctx, cudaMemsetAsync(&h->meta->counts[0], 0, sizeof(int), fs.main));
+    return LL_OK;
+  }
+  return spin_run(h, fs, raw, n, fmt, where, pc);
+}
+
+int spin_sweep_finish(ll_spin* h, cudaStream_t s, size_t n, int* nc_out, int* ns_out, float* max_t) {
+  ll_ctx* ctx = h->ctx;
+  for (int k = 0; k < 8; k++) h->last_counts[k] = h->pin[k];
+  h->extracted = 1; h->last_n = (int)n;
+  const int nc = h->pin[8], ns = h->pin[9];
+  *nc_out = nc; *ns_out = ns; *max_t = ll_ord2f(h->pin[10]);
+  if (nc + ns > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat, h->mvg_corner, (size_t)nc * 16, cudaMemcpyDeviceToDevice, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat + nc, h->lf_raw, (size_t)ns * 16, cudaMemcpyDeviceToDevice, s));
+  return LL_OK;
+}
+
+const float4* spin_full_cloud(const ll_spin* h, int* n, const int** d_n) { *n = h->last_counts[0]; *d_n = &h->meta->counts[0]; return h->cloud; }
+void spin_forget(ll_spin* h) { h->extracted = 0; }
 
 extern "C" {
 
@@ -473,8 +543,10 @@ int ll_spin_create(ll_ctx* ctx, const ll_spin_cfg* cfg, ll_spin** out) {
   h->ctx = ctx; h->cfg = *cfg; h->rings = cfg->scan_line;
   h->tmp_bytes = spin_tmp_bytes(cfg->max_points);
   cudaError_t e = h->arena.carve([&](Carve& c) { spin_layout(h, c); });
-  if (e == cudaSuccess) e = h->vg_scratch.reserve(voxel_grid_bytes(cfg->max_points, h->rings));
-  if (e == cudaSuccess) e = cudaMallocHost((void**)&h->pin, sizeof(SpinMeta::counts));
+  if (e == cudaSuccess) e = h->vg_scratch.reserve(std::max(voxel_grid_bytes(cfg->max_points, h->rings), voxel_grid_bytes(cfg->max_points)));
+  if (e == cudaSuccess) e = h->mvg.carve([&](Carve& c) { h->mvg_corner = c.take<float4>(spin_corner_cap(h)); });
+  if (e == cudaSuccess) e = h->vg_scratch2.reserve(voxel_grid_bytes(spin_corner_cap(h)));
+  if (e == cudaSuccess) e = cudaMallocHost((void**)&h->pin, sizeof(SpinMeta::counts) + sizeof(SpinMeta::feat));
   if (e != cudaSuccess) { ctx->set_error(std::string("ll_spin_create: ") + cudaGetErrorString(e)); ll_spin_release(h); return LL_ERR_CUDA; }
   *out = h; return LL_OK;
 }
@@ -482,7 +554,7 @@ int ll_spin_create(ll_ctx* ctx, const ll_spin_cfg* cfg, ll_spin** out) {
 void ll_spin_release(ll_spin* h) {
   if (!h) return;
   cudaSetDevice(h->ctx->device);
-  h->arena.release(); h->vg_scratch.release();
+  h->arena.release(); h->vg_scratch.release(); h->mvg.release(); h->vg_scratch2.release();
   if (h->pin) cudaFreeHost(h->pin);
   delete h;
 }
@@ -497,7 +569,7 @@ int ll_spin_extract(ll_spin* h, const void* raw, size_t n, int fmt, int where, s
   cudaSetDevice(ctx->device);
   h->extracted = 0;
   if (n == 0) { for (int k = 0; k < 8; k++) h->last_counts[k] = 0; }
-  else { LL_TRY(spin_run(h, raw, n, fmt, where)); for (int k = 0; k < 8; k++) h->last_counts[k] = h->pin[k]; }
+  else { LL_TRY(spin_run(h, ctx->own_front(), raw, n, fmt, where, nullptr)); for (int k = 0; k < 8; k++) h->last_counts[k] = h->pin[k]; }
   h->extracted = 1; h->last_n = (int)n;
   if (counts) for (int k = 0; k < 5; k++) counts[k] = (size_t)h->last_counts[k];
   return LL_OK;

@@ -986,6 +986,26 @@ class Laser_mapping:
             raise SequenceError(status, self.ctx._lib.ll_last_error(self.ctx.h).decode(), done.value, [(res[i], stats[i]) for i in range(done.value)])
         return [(res[i], stats[i]) for i in range(k)]
 
+    def process_new_sweep(self, front: "Laser_feature", raw, where=capi.LL_HOST, n=None, fmt=None):
+        """One spinning-lidar sweep (ll_mapper_process_sweep): the Velodyne front end of `front` (a Laser_feature on this mapper's context),
+        less sharp -> corners, less flat -> surfaces, the full cloud's largest intensity -> max_t, then the mapper step, as the reference's
+        remapped pipeline runs.  Afterwards front.cloud(k) gives the sweep's five clouds.  Returns (RegResult, MapperStats)."""
+        ptrs, sizes, fmt, _keep = self._clouds([raw], where, None if n is None else [n], fmt)
+        res, stats = capi.RegResult(), capi.MapperStats()
+        self.ctx.check(self.ctx._lib.ll_mapper_process_sweep(self.h, front.h, ptrs[0], sizes[0], fmt, where, C.byref(res), C.byref(stats)))
+        return res, stats
+
+    def process_new_sweeps(self, front: "Laser_feature", raws, where=capi.LL_HOST, ns=None, fmt=None):
+        """Several sweeps in one call: the results of process_new_sweep on each in turn, the front end of sweep k + 1 running on the device
+        under the mapper step of sweep k.  Returns one (RegResult, MapperStats) per sweep; an error raises SequenceError."""
+        k = len(raws)
+        ptrs, sizes, fmt, _keep = self._clouds(raws, where, ns, fmt)
+        res, stats, done = (capi.RegResult * k)(), (capi.MapperStats * k)(), C.c_int()
+        status = self.ctx._lib.ll_mapper_process_sweeps(self.h, front.h, k, ptrs, sizes, fmt, where, res, stats, C.byref(done))
+        if status != capi.LL_OK:
+            raise SequenceError(status, self.ctx._lib.ll_last_error(self.ctx.h).decode(), done.value, [(res[i], stats[i]) for i in range(done.value)])
+        return [(res[i], stats[i]) for i in range(k)]
+
     def pose(self):
         q, t, f = np.empty(4), np.empty(3), C.c_int()
         self.ctx.check(self.ctx._lib.ll_mapper_pose(self.h, q.ctypes.data, t.ctypes.data, C.byref(f)))
