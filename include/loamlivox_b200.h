@@ -67,7 +67,7 @@ void ll_ctx_destroy(ll_ctx* ctx);
 int  ll_ctx_warmup(ll_ctx* ctx);
 const char* ll_last_error(const ll_ctx* ctx);
 /* CUDA stream of the context as a cudaStream_t cast to void* (all work of a context is enqueued on it, except the front end of the sequence
- * calls ll_mapper_process_frames / _scans, which runs on streams of its own and has completed when they return). */
+ * calls ll_mapper_process_frames / _scans / _sweeps, which runs on streams of its own and has completed when they return). */
 void* ll_ctx_stream(ll_ctx* ctx);
 int  ll_ctx_sync(ll_ctx* ctx);
 

@@ -443,10 +443,9 @@ static int item_prologue(ll_ctx* ctx, const ll_map* map, int M, const ll_reg_sta
 
 // ll_scan_to_pose's registration of the front end's features on the device counts (A.dev_counts), with no host read in between: the one item's
 // slot count in the RegBatch is the capacity, and the host learns the counts at its first wait in the ICP loop.  Then, from the front end's
-// counts in pinned memory: st = scan_front_end_finish's outcome for them (LL_OK or LL_ERR_CAPACITY), nc / ns, dropped; `stopped` when the
+// counts in pinned memory: st = front_end_counts' outcome for them (LL_OK or LL_ERR_CAPACITY), nc / ns, dropped; `stopped` when the
 // device counts were zero (dropped, over capacity, or no feature), so that nothing ran and the caller reports the outcome.
 struct DevHandoff { const ll_pipeline_cfg* pc; int st, nc, ns, dropped, stopped; };
-static int front_end_counts(ll_ctx* ctx, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);
 
 // The ICP loops of the batch's items on the device (every item has passed item_prologue and the capacity check): one kNN launch and one solver
 // launch per ICP iteration for all of them.  outs[j] / status[j] belong to item j.  With `hand` (one item), the caller has uploaded the state.
@@ -599,12 +598,23 @@ int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg
   return st;
 }
 
+int features_fit(ll_ctx* ctx, size_t nc, size_t ns) {
+  if (nc + ns <= (size_t)ctx->cfg.max_features) return LL_OK;
+  ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY;
+}
+
+int features_hand_over(ll_ctx* ctx, cudaStream_t s, const float4* corner, int nc, const float4* surf, int ns) {
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat, corner, (size_t)nc * 16, cudaMemcpyDeviceToDevice, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat + nc, surf, (size_t)ns * 16, cudaMemcpyDeviceToDevice, s));
+  return LL_OK;
+}
+
 extern "C" {
 
 int ll_register(ll_ctx* ctx, const ll_map* map, const void* scan_corner, size_t nc, const void* scan_surf, size_t ns, int fmt, int where, const ll_reg_state* in, ll_reg_result* out) {
   if (!ctx || !map || !in || !out) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
-  if ((int)(nc + ns) > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
+  LL_TRY(features_fit(ctx, nc, ns));
   LL_TRY(upload_cloud(ctx, ctx->stream, scan_corner, nc, fmt, where, ctx->A.feat));
   LL_TRY(upload_cloud(ctx, ctx->stream, scan_surf, ns, fmt, where, ctx->A.feat + nc));
   return register_device(ctx, map, (int)nc, (int)ns, in, out);
@@ -934,38 +944,27 @@ int scan_front_end_enqueue(ll_ctx* ctx, const FrontStreams& fs, const void* raw,
   return front_graph(ctx, ctx->fg, fs.main, key, n >= 5, [&] { return front_end_enqueue(ctx, fs, pc, (int)n); });
 }
 
-// The front end's outcome from its counts in pinned memory, once it has completed: the time-stamp range, the feature counts, the drop rule
-// (<= 5 petals, :287) and max_features.
-static int front_end_counts(ll_ctx* ctx, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped) {
+int front_end_counts(ll_ctx* ctx, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped) {
   const int* h = ctx->pin->fe_counts;
   const int nc = h[5], ns = h[7], meta_scans = ctx->pin->fe_meta[1];
   ctx->last_full_min_t = ll_ord2f(h[10]); ctx->last_full_max_t = ll_ord2f(h[11]);
   *nc_out = nc; *ns_out = ns;
   *dropped = (meta_scans <= 5 && !pc->whole_frame) ? 1 : 0;
   if (*dropped) return LL_OK;
-  if (nc + ns > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
-  return LL_OK;
-}
-
-int scan_front_end_finish(ll_ctx* ctx, cudaStream_t s, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped) {
-  const RegArrays& A = ctx->A;
-  LL_TRY(front_end_counts(ctx, pc, nc_out, ns_out, dropped));
-  if (*dropped) return LL_OK;
-  const int nc = *nc_out, ns = *ns_out;
-  LL_CUDA(ctx, cudaMemcpyAsync(A.feat, A.tmp_a, (size_t)nc * 16, cudaMemcpyDeviceToDevice, s));
-  LL_CUDA(ctx, cudaMemcpyAsync(A.feat + nc, A.tmp_b, (size_t)ns * 16, cudaMemcpyDeviceToDevice, s));
-  return LL_OK;
+  return features_fit(ctx, nc, ns);
 }
 
 int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped) {
   LL_TRY(scan_front_end_enqueue(ctx, ctx->own_front(), raw, n, fmt, where, stamp, pc));
   LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return scan_front_end_finish(ctx, ctx->stream, pc, nc_out, ns_out, dropped);
+  LL_TRY(front_end_counts(ctx, pc, nc_out, ns_out, dropped));
+  if (*dropped) return LL_OK;
+  return features_hand_over(ctx, ctx->stream, ctx->A.tmp_a, *nc_out, ctx->A.tmp_b, *ns_out);
 }
 
 // The front end's features into A.feat on the device: corners (counts[5], from tmp_a) then surfaces (counts[7], from tmp_b), and the counts
 // the registration reads, dc = {corners, surfaces}.  dc = {0, 0} and nothing is copied when the frame is dropped (meta[1] <= 5 petals and not
-// whole_frame, :287) or has more features than max_features: scan_front_end_finish's rules.
+// whole_frame, :287) or has more features than max_features: front_end_counts' rules.
 __global__ void feature_handoff_kernel(const int* __restrict__ counts, const int* __restrict__ meta, int whole_frame, int max_features, const float4* __restrict__ corner,
                                        const float4* __restrict__ surf, float4* __restrict__ feat, int* __restrict__ dc) {
   const int nc = counts[5], ns = counts[7];
@@ -1084,9 +1083,8 @@ extern "C" int ll_frame_to_pose(ll_ctx* ctx, const ll_map* map, int n_heads, con
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   const int nc = hc[5], nsf = hc[7];
   if (n_corner_used) *n_corner_used = nc; if (n_surf_used) *n_surf_used = nsf;
-  if (nc + nsf > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
-  LL_CUDA(ctx, cudaMemcpyAsync(A.feat, A.tmp_a, (size_t)nc * 16, cudaMemcpyDeviceToDevice, s));
-  LL_CUDA(ctx, cudaMemcpyAsync(A.feat + nc, A.tmp_b, (size_t)nsf * 16, cudaMemcpyDeviceToDevice, s));
+  LL_TRY(features_fit(ctx, nc, nsf));
+  LL_TRY(features_hand_over(ctx, s, A.tmp_a, nc, A.tmp_b, nsf));
   return register_device(ctx, map, nc, nsf, in, out);
 }
 

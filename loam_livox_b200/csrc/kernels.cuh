@@ -259,11 +259,17 @@ void quat_mul(const double* a, const double* b, double* o);
 // ---------------------------------------------------------------------------------------------- host driver pieces (api.cu)
 // Registration of the features already resident in A.feat (corners then surfaces): the batch of one.  Core of ll_register / ll_scan_to_pose.
 int register_device(ll_ctx* ctx, const ll_map* map, int nc, int ns, const ll_reg_state* in, ll_reg_result* out);
-// The per-scan front end in three parts: enqueue on `fs` (bookkeeping, upload, the front end replayed as a graph; its counts land in
-// ctx->pin->fe_counts / fe_meta), and, once that work has completed, finish (the counts, the drop rule, max_features, the features copied
-// from tmp_a / tmp_b into A.feat on `s`).  scan_front_end = both on the context's own streams with a synchronisation between them.
+// The one limit on the features a registration takes: nc corners plus ns surfaces within max_features, else LL_ERR_CAPACITY ("more features
+// than max_features").
+int features_fit(ll_ctx* ctx, size_t nc, size_t ns);
+// A step's features into A.feat on `s`, where the registration reads them: nc corners from `corner`, then ns surfaces from `surf`.
+int features_hand_over(ll_ctx* ctx, cudaStream_t s, const float4* corner, int nc, const float4* surf, int ns);
+// The per-scan front end in parts: enqueue on `fs` (bookkeeping, upload, the front end replayed as a graph; its counts land in
+// ctx->pin->fe_counts / fe_meta), and, once that work has completed, front_end_counts (the time-stamp range, the counts of the features it
+// left in tmp_a / tmp_b, the drop rule (<= 5 petals, :287) and, unless dropped, features_fit).  scan_front_end = both on the context's own
+// streams with a synchronisation between them, then the features handed over on the context's stream unless the scan is dropped.
 int scan_front_end_enqueue(ll_ctx* ctx, const FrontStreams& fs, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc);
-int scan_front_end_finish(ll_ctx* ctx, cudaStream_t s, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);
+int front_end_counts(ll_ctx* ctx, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);
 int scan_front_end(ll_ctx* ctx, const void* raw, size_t n, int fmt, int where, double stamp, const ll_pipeline_cfg* pc, int* nc_out, int* ns_out, int* dropped);
 // The device arrays of a piecewise frame front end (owned by the streaming mapper): gathered segments of cap points per class, the first
 // VoxelGrids' outputs, the segmented VoxelGrids' scratch arenas (vg[0] on the context's stream, vg[1] on stream2), and the graph of the
@@ -279,11 +285,11 @@ int frame_front_end(ll_ctx* ctx, const FrontStreams& fs, const FrameArena& fa, i
 // ---------------------------------------------------------------------------------------------- spinning-lidar sweeps (spin.cu)
 // The streaming mapper's front end of a sweep (ll_mapper_process_sweep(s)): enqueue runs ll_spin_extract's front end on `fs` plus the mapping
 // node's input VoxelGrids (pc->mapping_leaf_corner / _surf) and max_t, without a host synchronisation; once that work has completed, finish
-// reads the counts (the handle's clouds are then this sweep's), applies max_features and copies the features into A.feat on `s`.
+// reads the counts (the handle's clouds are then this sweep's of n points): the sweep's features, where they lie, and max_t.
 ll_ctx* spin_ctx(const ll_spin* h);
 size_t spin_max_points(const ll_spin* h);
 int spin_sweep_enqueue(ll_spin* h, const FrontStreams& fs, const void* raw, size_t n, int fmt, int where, const ll_pipeline_cfg* pc);
-int spin_sweep_finish(ll_spin* h, cudaStream_t s, size_t n, int* nc_out, int* ns_out, float* max_t);
+void spin_sweep_finish(ll_spin* h, size_t n, const float4** corner, int* nc, const float4** surf, int* ns, float* max_t);
 const float4* spin_full_cloud(const ll_spin* h, int* n, const int** d_n);   // the last finished sweep's full cloud and its device count
 void spin_forget(ll_spin* h);   // the device clouds no longer match the counts (a sweep enqueued ahead of a failed step): nothing extracted
 
@@ -327,7 +333,7 @@ int keyframes_repose_dev(ll_ctx* ctx, const float4* d_in, int n, const int* seg_
 extern "C" void pg_odometry_edge(const ll_pose* prev, int id_prev, const ll_pose* cur, int id_cur, ll_pg_edge* out);
 
 // The streaming mapper's loop closure (loop.cu; ll_mapper_set_loop_closure).  The step's full cloud is captured into the loop closure's own
-// buffer before the next input's front end may overwrite the context's arrays: loop_scan_cloud after scan_front_end_finish (the front end's
+// buffer before the next input's front end may overwrite the context's arrays: loop_scan_cloud after the scan's hand-over (the front end's
 // full cloud, compacted again from the extractor's state), loop_frame_clouds after a frame's front end (every published piece's full slices of
 // every head); loop_select_piece picks piece i's.  loop_step runs at the end of a mapper step that appended its features (d_pose: the
 // registration pose on the device; pushed: the feature history took the step).

@@ -299,30 +299,17 @@ static int frame_arena(ll_mapper* m, int a, FrameArena* fa) {
   *fa = FrameArena{fl.dev, {fl.cls[0], fl.cls[1]}, {fl.mid[0], fl.mid[1]}, cap, {&m->frame_vg[0], &m->frame_vg[1]}, &m->frame_graph[a]};
   return LL_OK;
 }
-// First published piece of a completed front end whose features exceed max_features (publish: none).
-static int first_piece_over(const ll_mapper* m, const FrameOut& fo, int publish) {
-  for (int i = 0; i < publish; i++) {
-    const int nc = fo.out_end[0][i] - (i ? fo.out_end[0][i - 1] : 0), nsf = fo.out_end[1][i] - (i ? fo.out_end[1][i - 1] : 0);
-    if (nc + nsf > m->ctx->cfg.max_features) return i;
-  }
-  return publish;
-}
 
 // ---------------------------------------------------------------------------------------------- the input loop
-// ll_mapper_process_scans / _frames: the front end of input k + 1 is enqueued on the streams `fs` (ll_ctx::fe_stream) before the mapper
-// step(s) of input k, so it runs under them.  Nothing the mapper step reads or writes is touched by the front end, whose results only reach the
-// mapper through the copy into A.feat; the extractor's host bookkeeping advances in input order.  So a sequence gives the results of its inputs
-// called one at a time.  ll_mapper_process_scan / _frame are the loops of one input on the context's own streams (ll_ctx::own_front): their
-// front end keeps the greatest priority, as every other call of the context, and nothing is enqueued ahead.
+// ll_mapper_process_scans / _frames / _sweeps: the front end of input k + 1 is enqueued on the streams `fs` (ll_ctx::fe_stream) before the
+// mapper step(s) of input k, so it runs under them.  Nothing the mapper step reads or writes is touched by the front end, whose results only
+// reach the mapper through the copy into A.feat; the extractor's host bookkeeping advances in input order.  So a sequence gives the results of
+// its inputs called one at a time.  ll_mapper_process_scan / _frame / _sweep are the loops of one input on the context's own streams
+// (ll_ctx::own_front): their front end keeps the greatest priority, as every other call of the context, and nothing is enqueued ahead.
 //
 // A front end enqueued ahead of an input that then fails: it is drained (it reads the caller's inputs) and its host bookkeeping undone, so that
 // the extractor stands where the one-by-one calls leave it.
-struct Ahead { ExtractState saved; bool on = false; };
-static void sequence_drain(const FrontStreams& fs) { for (cudaStream_t s : {fs.main, fs.corner, fs.petals}) cudaStreamSynchronize(s); }
-static void sequence_unwind(ll_ctx* ctx, const FrontStreams& fs, const Ahead& a) {
-  sequence_drain(fs);
-  if (a.on) ctx->ex = a.saved;
-}
+//
 // Host records are staged in stage_in: reserved for `points` records (max_scan_points, or a spin handle's max_points) before the first front
 // end, because a reallocation (cudaFree) would synchronise the device in the middle of the sequence.
 static int reserve_stage(ll_ctx* ctx, int fmt, int where, size_t points) {
@@ -362,198 +349,6 @@ static int frames_check(ll_mapper* m, int n_frames, int n_heads, const void* con
   }
   return LL_OK;
 }
-
-// Frame f: the piecewise front end (every head, every piece, one host read) into arena f & 1, then per published piece its features into
-// A.feat and mapper_step.  A rejected piece leaves the pose as it was, and the next piece continues from there.
-static int frames_run(ll_mapper* m, const FrontStreams& fs, int n_frames, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where,
-                      const double* stamps, int pieces, int publish, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces, int* done) {
-  ll_ctx* ctx = m->ctx;
-  LL_TRY(reserve_stage(ctx, fmt, where, (size_t)ctx->cfg.max_scan_points));
-  for (int f = 0; f < n_frames; f++) n_pieces[f] = 0;
-  FrameArena fa[2]; LL_TRY(frame_arena(m, 0, &fa[0])); LL_TRY(frame_arena(m, 1, &fa[1]));
-  auto enqueue = [&](int f) -> int {   // frame f's front end into arena f & 1, behind the last copy out of it (frame f - 2's)
-    const size_t o = (size_t)f * n_heads;
-    LL_CUDA(ctx, cudaStreamWaitEvent(fs.main, ctx->sev.fe_free[f & 1], 0));
-    LL_TRY(frame_front_end(ctx, fs, fa[f & 1], n_heads, raws + o, ns + o, fmt, where, stamps + o, pieces, &m->cfg.pipeline));
-    LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_ready, fs.main));
-    return LL_OK;
-  };
-  Ahead ahead;
-  const int st = [&]() -> int {
-    double t = now_ms();
-    LL_TRY(enqueue(0));
-    float ms_enqueue = (float)(now_ms() - t);
-    for (int f = 0; f < n_frames; f++) {
-      ahead.on = false;
-      t = now_ms();
-      LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.fe_ready));
-      const FrameOut fo = ctx->pin->frame;   // read before the next front end is enqueued (PinnedStage)
-      const float ms_front_end = ms_enqueue + (float)(now_ms() - t);
-      // the next front end goes under this frame's steps unless one of its pieces will stop the sequence
-      const bool next = f + 1 < n_frames && (fo.heads_live == 0 || first_piece_over(m, fo, publish) == publish);
-      auto enqueue_next = [&]() -> int {
-        if (!next) return LL_OK;
-        ahead.saved = ctx->ex; ahead.on = true;
-        const double t1 = now_ms();
-        LL_TRY(enqueue(f + 1));
-        ms_enqueue = (float)(now_ms() - t1);
-        return LL_OK;
-      };
-      if (m->lc && fo.heads_live != 0) {   // the published pieces' full clouds, before the next front end (behind fe_free) overwrites tmp_c
-        LL_TRY(loop_frame_clouds(ctx, m->lc, fa[f & 1].dev, ns + (size_t)f * n_heads, n_heads, publish));
-        LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[(f + 1) & 1], ctx->stream));
-      }
-      if (fo.heads_live == 0) LL_TRY(enqueue_next());                           // laser_feature_extractor.hpp:287, every head
-      for (int i = 0; fo.heads_live != 0 && i < publish; i++) {
-        const int c0 = i ? fo.out_end[0][i - 1] : 0, s0 = i ? fo.out_end[1][i - 1] : 0;
-        const int nc = fo.out_end[0][i] - c0, nsf = fo.out_end[1][i] - s0;
-        ll_reg_result* o = out + (size_t)f * cap + i;
-        ll_mapper_stats* ps = stats ? stats + (size_t)f * cap + i : nullptr;
-        if (ps) { memset(ps, 0, sizeof(*ps)); ps->n_corner = nc; ps->n_surf = nsf; ps->ms_front_end = i == 0 ? ms_front_end : 0.f; }
-        out_init(m, o);
-        if (nc + nsf > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
-        LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat, fa[f & 1].cls[0] + c0, (size_t)nc * 16, cudaMemcpyDeviceToDevice, ctx->stream));
-        LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat + nc, fa[f & 1].cls[1] + s0, (size_t)nsf * 16, cudaMemcpyDeviceToDevice, ctx->stream));
-        if (i == publish - 1) LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[f & 1], ctx->stream));
-        if (i == 0) LL_TRY(enqueue_next());
-        if (m->lc) loop_select_piece(m->lc, i);
-        LL_TRY(mapper_step(m, nc, nsf, (double)ll_ord2f(fo.tmax[i]), o, ps));
-        n_pieces[f] = i + 1;
-      }
-      *done = f + 1;
-    }
-    return LL_OK;
-  }();
-  if (st != LL_OK) sequence_unwind(ctx, fs, ahead);
-  return st;
-}
-
-extern "C" int ll_mapper_process_frame(ll_mapper* m, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
-                                       int odom_mode, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces) {
-  if (!m || !out || !raws || !ns || !stamps || !n_pieces || n_heads < 1 || n_heads > LL_MAX_HEADS) return LL_ERR_INVALID;
-  *n_pieces = 0;
-  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
-  int pieces = 0, publish = 0, done = 0;
-  LL_TRY(frames_check(m, 1, n_heads, raws, ns, fmt, where, odom_mode, cap, &pieces, &publish));
-  return frames_run(m, ctx->own_front(), 1, n_heads, raws, ns, fmt, where, stamps, pieces, publish, out, stats, cap, n_pieces, &done);
-}
-
-extern "C" int ll_mapper_process_frames(ll_mapper* m, int n_frames, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where,
-                                        const double* stamps, int odom_mode, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces, int* n_frames_done) {
-  if (n_frames_done) *n_frames_done = 0;
-  if (!m || !out || !raws || !ns || !stamps || !n_pieces || !n_frames_done || n_frames < 1 || n_heads < 1 || n_heads > LL_MAX_HEADS) return LL_ERR_INVALID;
-  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
-  int pieces = 0, publish = 0;
-  LL_TRY(frames_check(m, n_frames, n_heads, raws, ns, fmt, where, odom_mode, cap, &pieces, &publish));
-  return frames_run(m, ctx->pipe_front(), n_frames, n_heads, raws, ns, fmt, where, stamps, pieces, publish, out, stats, cap, n_pieces, n_frames_done);
-}
-
-// The front end of one kind of single-scan input (a Livox scan, a spinning-lidar sweep) as inputs_run drives it:
-//   enqueue(k)     input k's front end on fs.main (inputs_run orders it behind fe_free[0], the copy of input k - 1's features);
-//   finish(k, ..)  once it has completed: its feature counts, max_t and whether it is dropped, its features copied into A.feat on the context's
-//                  stream (LL_ERR_CAPACITY past max_features, before anything of the step is enqueued);
-//   loop_cloud(k)  its full cloud into the loop closure's input, before the next front end may overwrite it;
-//   save / restore the host bookkeeping around a front end enqueued ahead of an input that then fails.
-struct ScanFront {
-  ll_ctx* ctx; const FrontStreams& fs; const void* const* raws; const size_t* ns; int fmt, where; const double* stamps; const ll_pipeline_cfg* pc;
-  ExtractState saved;
-  int enqueue(int k) { return scan_front_end_enqueue(ctx, fs, raws[k], ns[k], fmt, where, stamps[k], pc); }
-  int finish(int, int* nc, int* nsf, double* max_t, bool* dropped) {
-    int d = 0;
-    LL_TRY(scan_front_end_finish(ctx, ctx->stream, pc, nc, nsf, &d));   // reads the pinned counts before the next front end is enqueued
-    *dropped = d != 0; *max_t = (double)ctx->last_full_max_t;
-    return LL_OK;
-  }
-  int loop_cloud(LoopClosure* lc, int) { return loop_scan_cloud(ctx, lc, pc); }   // the full cloud, compacted again from the extractor's state
-  void save() { saved = ctx->ex; }
-  void restore() { ctx->ex = saved; }
-};
-// A sweep: the spin handle's front end and the mapping node's VoxelGrids (spin_sweep_enqueue).  It is never dropped: every sweep registers.
-struct SweepFront {
-  ll_ctx* ctx; ll_spin* spin; const FrontStreams& fs; const void* const* raws; const size_t* ns; int fmt, where; const ll_pipeline_cfg* pc;
-  int enqueue(int k) { return spin_sweep_enqueue(spin, fs, raws[k], ns[k], fmt, where, pc); }
-  int finish(int k, int* nc, int* nsf, double* max_t, bool* dropped) {
-    float mt = 0.f;
-    const int st = spin_sweep_finish(spin, ctx->stream, ns[k], nc, nsf, &mt);
-    *dropped = false; *max_t = (double)mt;
-    return st;
-  }
-  int loop_cloud(LoopClosure* lc, int) { int n = 0; const int* d_n = nullptr; const float4* full = spin_full_cloud(spin, &n, &d_n); return loop_sweep_cloud(ctx, lc, full, n, d_n); }
-  void save() {}
-  void restore() { spin_forget(spin); }
-};
-
-// Input k: the front end, its features into A.feat and mapper_step.
-template <typename Front>
-static int inputs_run(ll_mapper* m, Front& fe, const FrontStreams& fs, int n_inputs, ll_reg_result* out, ll_mapper_stats* stats, int* done) {
-  ll_ctx* ctx = m->ctx;
-  auto enqueue = [&](int k) -> int {   // behind the copy of input k - 1's features out of the front end's buffers
-    LL_CUDA(ctx, cudaStreamWaitEvent(fs.main, ctx->sev.fe_free[0], 0));
-    LL_TRY(fe.enqueue(k));
-    LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_ready, fs.main));
-    return LL_OK;
-  };
-  bool ahead = false;
-  const int st = [&]() -> int {
-    double t = now_ms();
-    LL_TRY(enqueue(0));
-    float ms_enqueue = (float)(now_ms() - t);
-    for (int k = 0; k < n_inputs; k++) {
-      ahead = false;
-      ll_mapper_stats* ps = stats ? stats + k : nullptr;
-      if (ps) memset(ps, 0, sizeof(*ps));
-      t = now_ms();
-      LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.fe_ready));
-      int nc = 0, nsf = 0; double max_t = 0; bool dropped = false;
-      LL_TRY(fe.finish(k, &nc, &nsf, &max_t, &dropped));
-      if (m->lc && !dropped) LL_TRY(fe.loop_cloud(m->lc, k));
-      LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[0], ctx->stream));
-      const float ms_front_end = ms_enqueue + (float)(now_ms() - t);
-      if (k + 1 < n_inputs) {
-        fe.save(); ahead = true;
-        const double t1 = now_ms();
-        LL_TRY(enqueue(k + 1));
-        ms_enqueue = (float)(now_ms() - t1);
-      }
-      out_init(m, out + k);
-      if (ps) { ps->n_corner = nc; ps->n_surf = nsf; ps->ms_front_end = ms_front_end; }
-      if (!dropped) LL_TRY(mapper_step(m, nc, nsf, max_t, out + k, ps));   // laser_feature_extractor.hpp:287
-      *done = k + 1;
-    }
-    return LL_OK;
-  }();
-  if (st != LL_OK) {   // sequence_unwind for any front end
-    sequence_drain(fs);
-    if (ahead) fe.restore();
-  }
-  return st;
-}
-
-static int scans_run(ll_mapper* m, const FrontStreams& fs, int n_scans, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
-                     ll_reg_result* out, ll_mapper_stats* stats, int* done) {
-  ll_ctx* ctx = m->ctx;
-  LL_TRY(reserve_stage(ctx, fmt, where, (size_t)ctx->cfg.max_scan_points));
-  ScanFront fe{ctx, fs, raws, ns, fmt, where, stamps, &m->cfg.pipeline, ExtractState()};
-  return inputs_run(m, fe, fs, n_scans, out, stats, done);
-}
-
-extern "C" int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int where, double stamp, ll_reg_result* out, ll_mapper_stats* stats) {
-  if (!m || !out) return LL_ERR_INVALID;
-  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
-  int done = 0;
-  LL_TRY(scans_check(ctx, 1, &raw, &n, fmt, where));
-  return scans_run(m, ctx->own_front(), 1, &raw, &n, fmt, where, &stamp, out, stats, &done);
-}
-
-extern "C" int ll_mapper_process_scans(ll_mapper* m, int n_scans, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
-                                       ll_reg_result* out, ll_mapper_stats* stats, int* n_scans_done) {
-  if (n_scans_done) *n_scans_done = 0;
-  if (!m || !out || !raws || !ns || !stamps || !n_scans_done || n_scans < 1) return LL_ERR_INVALID;
-  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
-  LL_TRY(scans_check(ctx, n_scans, raws, ns, fmt, where));
-  return scans_run(m, ctx->pipe_front(), n_scans, raws, ns, fmt, where, stamps, out, stats, n_scans_done);
-}
-
 // Sweeps: the spin handle must share the mapper's context; a sweep over the handle's max_points, or, with loop closure on, over the loop
 // closure's per-step full cloud (max_scan_points: a sweep's whole kept cloud is one step's, and the kept points can only be fewer), is
 // LL_ERR_CAPACITY before anything is enqueued.
@@ -567,20 +362,205 @@ static int sweeps_check(ll_mapper* m, ll_spin* spin, int n_sweeps, const void* c
   }
   return LL_OK;
 }
-static int sweeps_run(ll_mapper* m, ll_spin* spin, const FrontStreams& fs, int n_sweeps, const void* const* raws, const size_t* ns, int fmt, int where,
-                      ll_reg_result* out, ll_mapper_stats* stats, int* done) {
+
+// One mapper step of an input: its features as the front end left them (nc corners at `corner`, nsf surfaces at `surf`), the largest time
+// stamp of its full cloud, and whether the step runs.
+struct FrontStep { const float4* corner; const float4* surf; int nc, nsf; double max_t; bool runs; };
+
+// The front end of one kind of input as inputs_run drives it:
+//   arenas          the copies of the buffers its results lie in: input k's front end fills copy k % arenas behind fe_free[k % arenas], the
+//                   event of the last hand-over out of it (input k - arenas's);
+//   max_points()    the records stage_in must hold for one input;
+//   enqueue(k)      input k's front end on fs.main;
+//   finish(k, &n)   once it has completed, its results read before the next front end is enqueued: the n steps it gives, step(k, 0 ... n - 1);
+//   loop_cloud(k)   its full cloud(s) into the loop closure's input, before the next front end may overwrite them;
+//   save / restore  the host bookkeeping around a front end enqueued ahead of an input that then fails.
+// A scan: one step, which does not run when the scan is dropped (<= 5 petals and not whole_frame, laser_feature_extractor.hpp:287); its
+// features in tmp_a / tmp_b, max_features refused by front_end_counts.
+struct ScanFront {
+  static constexpr int arenas = 1;
+  ll_ctx* ctx; const FrontStreams& fs; const void* const* raws; const size_t* ns; int fmt, where; const double* stamps; const ll_pipeline_cfg* pc;
+  FrontStep s; ExtractState saved;
+  size_t max_points() const { return (size_t)ctx->cfg.max_scan_points; }
+  int enqueue(int k) { return scan_front_end_enqueue(ctx, fs, raws[k], ns[k], fmt, where, stamps[k], pc); }
+  int finish(int, int* n_steps) {
+    int dropped = 0; *n_steps = 1;
+    LL_TRY(front_end_counts(ctx, pc, &s.nc, &s.nsf, &dropped));
+    s.corner = ctx->A.tmp_a; s.surf = ctx->A.tmp_b; s.max_t = (double)ctx->last_full_max_t; s.runs = !dropped;
+    return LL_OK;
+  }
+  FrontStep step(int, int) const { return s; }
+  int loop_cloud(LoopClosure* lc, int) { return loop_scan_cloud(ctx, lc, pc); }   // the full cloud, compacted again from the extractor's state
+  void save() { saved = ctx->ex; }
+  void restore() { ctx->ex = saved; }
+};
+// A sweep: the spin handle's front end and the mapping node's VoxelGrids (spin_sweep_enqueue).  One step, which always runs: every sweep registers.
+struct SweepFront {
+  static constexpr int arenas = 1;
+  ll_ctx* ctx; ll_spin* spin; const FrontStreams& fs; const void* const* raws; const size_t* ns; int fmt, where; const ll_pipeline_cfg* pc;
+  FrontStep s;
+  size_t max_points() const { return spin_max_points(spin); }
+  int enqueue(int k) { return spin_sweep_enqueue(spin, fs, raws[k], ns[k], fmt, where, pc); }
+  int finish(int k, int* n_steps) {
+    float max_t = 0.f; *n_steps = 1;
+    spin_sweep_finish(spin, ns[k], &s.corner, &s.nc, &s.surf, &s.nsf, &max_t);
+    s.max_t = (double)max_t; s.runs = true;
+    return LL_OK;
+  }
+  FrontStep step(int, int) const { return s; }
+  int loop_cloud(LoopClosure* lc, int) { int n = 0; const int* d_n = nullptr; const float4* full = spin_full_cloud(spin, &n, &d_n); return loop_sweep_cloud(ctx, lc, full, n, d_n); }
+  void save() {}
+  void restore() { spin_forget(spin); }
+};
+// A frame: the piecewise front end (every head, every piece, one host read) into arena k & 1, so that frame k + 1's fills the other while frame
+// k's pieces are still read out.  One step per published piece, none when no head is live (laser_feature_extractor.hpp:287, every head).
+struct FrameFront {
+  static constexpr int arenas = 2;
+  ll_ctx* ctx; const FrontStreams& fs; int n_heads; const void* const* raws; const size_t* ns; int fmt, where; const double* stamps; const ll_pipeline_cfg* pc;
+  int pieces = 0, publish = 0;
+  FrameArena fa[2]; FrameOut fo; ExtractState saved;
+  size_t max_points() const { return (size_t)ctx->cfg.max_scan_points; }
+  int enqueue(int k) { const size_t o = (size_t)k * n_heads; return frame_front_end(ctx, fs, fa[k & 1], n_heads, raws + o, ns + o, fmt, where, stamps + o, pieces, pc); }
+  int finish(int, int* n_steps) { fo = ctx->pin->frame; *n_steps = fo.heads_live != 0 ? publish : 0; return LL_OK; }
+  FrontStep step(int k, int i) const {
+    const int c0 = i ? fo.out_end[0][i - 1] : 0, s0 = i ? fo.out_end[1][i - 1] : 0;
+    return {fa[k & 1].cls[0] + c0, fa[k & 1].cls[1] + s0, fo.out_end[0][i] - c0, fo.out_end[1][i] - s0, (double)ll_ord2f(fo.tmax[i]), true};
+  }
+  int loop_cloud(LoopClosure* lc, int k) { return loop_frame_clouds(ctx, lc, fa[k & 1].dev, ns + (size_t)k * n_heads, n_heads, publish); }
+  void save() { saved = ctx->ex; }
+  void restore() { ctx->ex = saved; }
+};
+
+// Input k: the front end, then per step i its features into A.feat and mapper_step, the entry at out / stats [k * cap + i].  A step that is
+// refused or fails ends the sequence; a rejected step leaves the pose as it was, and the next step continues from there.
+template <typename Front>
+static int inputs_run(ll_mapper* m, Front& fe, int n_inputs, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces, int* done) {
   ll_ctx* ctx = m->ctx;
-  LL_TRY(reserve_stage(ctx, fmt, where, spin_max_points(spin)));
-  SweepFront fe{ctx, spin, fs, raws, ns, fmt, where, &m->cfg.pipeline};
-  return inputs_run(m, fe, fs, n_sweeps, out, stats, done);
+  const FrontStreams& fs = fe.fs;
+  LL_TRY(reserve_stage(ctx, fe.fmt, fe.where, fe.max_points()));
+  auto enqueue = [&](int k) -> int {
+    LL_CUDA(ctx, cudaStreamWaitEvent(fs.main, ctx->sev.fe_free[k % Front::arenas], 0));
+    LL_TRY(fe.enqueue(k));
+    LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_ready, fs.main));
+    return LL_OK;
+  };
+  bool ahead = false;
+  const int st = [&]() -> int {
+    double t = now_ms();
+    LL_TRY(enqueue(0));
+    float ms_enqueue = (float)(now_ms() - t);
+    for (int k = 0; k < n_inputs; k++) {
+      ahead = false;
+      t = now_ms();
+      LL_CUDA(ctx, cudaEventSynchronize(ctx->sev.fe_ready));
+      int n_steps = 0;
+      LL_TRY(fe.finish(k, &n_steps));
+      const float ms_front_end = ms_enqueue + (float)(now_ms() - t);
+      // the next front end goes under this input's steps unless one of them will stop the sequence at features_fit
+      bool next = k + 1 < n_inputs;
+      for (int i = 0; i < n_steps; i++) { const FrontStep s = fe.step(k, i); next = next && (!s.runs || s.nc + s.nsf <= ctx->cfg.max_features); }
+      auto enqueue_next = [&]() -> int {
+        if (!next) return LL_OK;
+        fe.save(); ahead = true;
+        const double t1 = now_ms();
+        LL_TRY(enqueue(k + 1));
+        ms_enqueue = (float)(now_ms() - t1);
+        return LL_OK;
+      };
+      // Two arenas: the full clouds lie outside them (tmp_c), where the next front end overwrites them whichever arena it fills, so they are
+      // captured ahead of the steps, behind an event of their own that the next front end waits on.  One arena: after the step's hand-over,
+      // whose fe_free guards both.
+      if (Front::arenas == 2 && m->lc && n_steps > 0) {
+        LL_TRY(fe.loop_cloud(m->lc, k));
+        LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[(k + 1) % Front::arenas], ctx->stream));
+      }
+      if (n_steps == 0) LL_TRY(enqueue_next());
+      for (int i = 0; i < n_steps; i++) {
+        const FrontStep s = fe.step(k, i);
+        ll_reg_result* o = out + (size_t)k * cap + i;
+        ll_mapper_stats* ps = stats ? stats + (size_t)k * cap + i : nullptr;
+        if (ps) { memset(ps, 0, sizeof(*ps)); ps->n_corner = s.nc; ps->n_surf = s.nsf; ps->ms_front_end = i == 0 ? ms_front_end : 0.f; }
+        out_init(m, o);
+        if (s.runs) {
+          LL_TRY(features_fit(ctx, s.nc, s.nsf));
+          LL_TRY(features_hand_over(ctx, ctx->stream, s.corner, s.nc, s.surf, s.nsf));
+          if (Front::arenas == 1 && m->lc) LL_TRY(fe.loop_cloud(m->lc, k));
+        }
+        if (i == n_steps - 1) LL_CUDA(ctx, cudaEventRecord(ctx->sev.fe_free[k % Front::arenas], ctx->stream));
+        if (i == 0) LL_TRY(enqueue_next());
+        if (m->lc) loop_select_piece(m->lc, i);
+        if (s.runs) LL_TRY(mapper_step(m, s.nc, s.nsf, s.max_t, o, ps));
+        if (n_pieces) n_pieces[k] = i + 1;
+      }
+      *done = k + 1;
+    }
+    return LL_OK;
+  }();
+  if (st != LL_OK) {
+    for (cudaStream_t s : {fs.main, fs.corner, fs.petals}) cudaStreamSynchronize(s);
+    if (ahead) fe.restore();
+  }
+  return st;
+}
+
+static int run_scans(ll_mapper* m, const FrontStreams& fs, int n_scans, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+                     ll_reg_result* out, ll_mapper_stats* stats, int* done) {
+  LL_TRY(scans_check(m->ctx, n_scans, raws, ns, fmt, where));
+  ScanFront fe{m->ctx, fs, raws, ns, fmt, where, stamps, &m->cfg.pipeline};
+  return inputs_run(m, fe, n_scans, out, stats, 1, nullptr, done);
+}
+static int run_frames(ll_mapper* m, const FrontStreams& fs, int n_frames, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where,
+                      const double* stamps, int odom_mode, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces, int* done) {
+  FrameFront fe{m->ctx, fs, n_heads, raws, ns, fmt, where, stamps, &m->cfg.pipeline};
+  LL_TRY(frames_check(m, n_frames, n_heads, raws, ns, fmt, where, odom_mode, cap, &fe.pieces, &fe.publish));
+  for (int f = 0; f < n_frames; f++) n_pieces[f] = 0;
+  LL_TRY(frame_arena(m, 0, &fe.fa[0])); LL_TRY(frame_arena(m, 1, &fe.fa[1]));
+  return inputs_run(m, fe, n_frames, out, stats, cap, n_pieces, done);
+}
+static int run_sweeps(ll_mapper* m, ll_spin* spin, const FrontStreams& fs, int n_sweeps, const void* const* raws, const size_t* ns, int fmt, int where,
+                      ll_reg_result* out, ll_mapper_stats* stats, int* done) {
+  LL_TRY(sweeps_check(m, spin, n_sweeps, raws, ns, fmt, where));
+  SweepFront fe{m->ctx, spin, fs, raws, ns, fmt, where, &m->cfg.pipeline};
+  return inputs_run(m, fe, n_sweeps, out, stats, 1, nullptr, done);
+}
+
+extern "C" int ll_mapper_process_scan(ll_mapper* m, const void* raw, size_t n, int fmt, int where, double stamp, ll_reg_result* out, ll_mapper_stats* stats) {
+  if (!m || !out) return LL_ERR_INVALID;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  int done = 0;
+  return run_scans(m, ctx->own_front(), 1, &raw, &n, fmt, where, &stamp, out, stats, &done);
+}
+
+extern "C" int ll_mapper_process_scans(ll_mapper* m, int n_scans, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+                                       ll_reg_result* out, ll_mapper_stats* stats, int* n_scans_done) {
+  if (n_scans_done) *n_scans_done = 0;
+  if (!m || !out || !raws || !ns || !stamps || !n_scans_done || n_scans < 1) return LL_ERR_INVALID;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  return run_scans(m, ctx->pipe_front(), n_scans, raws, ns, fmt, where, stamps, out, stats, n_scans_done);
+}
+
+extern "C" int ll_mapper_process_frame(ll_mapper* m, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where, const double* stamps,
+                                       int odom_mode, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces) {
+  if (!m || !out || !raws || !ns || !stamps || !n_pieces || n_heads < 1 || n_heads > LL_MAX_HEADS) return LL_ERR_INVALID;
+  *n_pieces = 0;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  int done = 0;
+  return run_frames(m, ctx->own_front(), 1, n_heads, raws, ns, fmt, where, stamps, odom_mode, out, stats, cap, n_pieces, &done);
+}
+
+extern "C" int ll_mapper_process_frames(ll_mapper* m, int n_frames, int n_heads, const void* const* raws, const size_t* ns, int fmt, int where,
+                                        const double* stamps, int odom_mode, ll_reg_result* out, ll_mapper_stats* stats, int cap, int* n_pieces, int* n_frames_done) {
+  if (n_frames_done) *n_frames_done = 0;
+  if (!m || !out || !raws || !ns || !stamps || !n_pieces || !n_frames_done || n_frames < 1 || n_heads < 1 || n_heads > LL_MAX_HEADS) return LL_ERR_INVALID;
+  ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
+  return run_frames(m, ctx->pipe_front(), n_frames, n_heads, raws, ns, fmt, where, stamps, odom_mode, out, stats, cap, n_pieces, n_frames_done);
 }
 
 extern "C" int ll_mapper_process_sweep(ll_mapper* m, ll_spin* spin, const void* raw, size_t n, int fmt, int where, ll_reg_result* out, ll_mapper_stats* stats) {
   if (!m || !spin || !out) return LL_ERR_INVALID;
   ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
   int done = 0;
-  LL_TRY(sweeps_check(m, spin, 1, &raw, &n, fmt, where));
-  return sweeps_run(m, spin, ctx->own_front(), 1, &raw, &n, fmt, where, out, stats, &done);
+  return run_sweeps(m, spin, ctx->own_front(), 1, &raw, &n, fmt, where, out, stats, &done);
 }
 
 extern "C" int ll_mapper_process_sweeps(ll_mapper* m, ll_spin* spin, int n_sweeps, const void* const* raws, const size_t* ns, int fmt, int where,
@@ -588,8 +568,7 @@ extern "C" int ll_mapper_process_sweeps(ll_mapper* m, ll_spin* spin, int n_sweep
   if (n_sweeps_done) *n_sweeps_done = 0;
   if (!m || !spin || !out || !raws || !ns || !n_sweeps_done || n_sweeps < 1) return LL_ERR_INVALID;
   ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
-  LL_TRY(sweeps_check(m, spin, n_sweeps, raws, ns, fmt, where));
-  return sweeps_run(m, spin, ctx->pipe_front(), n_sweeps, raws, ns, fmt, where, out, stats, n_sweeps_done);
+  return run_sweeps(m, spin, ctx->pipe_front(), n_sweeps, raws, ns, fmt, where, out, stats, n_sweeps_done);
 }
 
 // ---------------------------------------------------------------------------------------------- checkpoint

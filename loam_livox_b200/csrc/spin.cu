@@ -508,16 +508,10 @@ int spin_sweep_enqueue(ll_spin* h, const FrontStreams& fs, const void* raw, size
   return spin_run(h, fs, raw, n, fmt, where, pc);
 }
 
-int spin_sweep_finish(ll_spin* h, cudaStream_t s, size_t n, int* nc_out, int* ns_out, float* max_t) {
-  ll_ctx* ctx = h->ctx;
+void spin_sweep_finish(ll_spin* h, size_t n, const float4** corner, int* nc, const float4** surf, int* ns, float* max_t) {
   for (int k = 0; k < 8; k++) h->last_counts[k] = h->pin[k];
   h->extracted = 1; h->last_n = (int)n;
-  const int nc = h->pin[8], ns = h->pin[9];
-  *nc_out = nc; *ns_out = ns; *max_t = ll_ord2f(h->pin[10]);
-  if (nc + ns > ctx->cfg.max_features) { ctx->set_error("more features than max_features"); return LL_ERR_CAPACITY; }
-  LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat, h->mvg_corner, (size_t)nc * 16, cudaMemcpyDeviceToDevice, s));
-  LL_CUDA(ctx, cudaMemcpyAsync(ctx->A.feat + nc, h->lf_raw, (size_t)ns * 16, cudaMemcpyDeviceToDevice, s));
-  return LL_OK;
+  *corner = h->mvg_corner; *nc = h->pin[8]; *surf = h->lf_raw; *ns = h->pin[9]; *max_t = ll_ord2f(h->pin[10]);
 }
 
 const float4* spin_full_cloud(const ll_spin* h, int* n, const int** d_n) { *n = h->last_counts[0]; *d_n = &h->meta->counts[0]; return h->cloud; }

@@ -127,20 +127,37 @@ def test_loop_closure_changes_no_odometry_frames(ctxs, mode):
 
 
 # ---------------------------------------------------------------------------------------------- sequence calls = single calls
-def test_sequence_calls_give_the_single_calls_log(ctxs):
-    poses = _returning(20)
-    raws, stamps = _scans(poses, S.SEED + 5300)
-    a, b = _mapper(ctxs[0], 0, poses[0]), _mapper(ctxs[1], 0, poses[0])
+def _sequence_and_single_calls(ctxs, kind):
+    """a: the single calls, b: the sequence call, both with loop closure on; their entries, one per step.  frames: two pieces each, so the
+    front ends of the sequence alternate between both arenas while the loop closure reads the full clouds that every front end overwrites."""
+    if kind == "scans":
+        poses = _returning(20)
+        raws, stamps = _scans(poses, S.SEED + 5300)
+        a, b = _mapper(ctxs[0], 0, poses[0]), _mapper(ctxs[1], 0, poses[0])
+    else:
+        poses = _returning(12)
+        raws = [S.make_triple_scan(N, p, seed=S.SEED + 5350 + 3 * k) for k, p in enumerate(poses)]
+        stamps = [[100.0 + 0.1 * k] * 3 for k in range(len(poses))]
+        a, b = _mapper(ctxs[0], 0, poses[0], pieces=2), _mapper(ctxs[1], 0, poses[0], pieces=2)
     for m in (a, b):
         m.set_loop_closure(**SMALL)
-    ra = [a.process_new_scan(r, t) for r, t in zip(raws, stamps)]
-    rb = b.process_new_scans(raws, stamps)
-    assert [_entry(x) for x, _ in ra] == [_entry(x) for x, _ in rb]
-    la, lb = a.loop_log()[0], b.loop_log()[0]
-    assert len(la) > 0 and [_ev(e) for e in la] == [_ev(e) for e in lb]
-    xa, xb = a.loop_result(), b.loop_result()
-    assert xa["closed"] == xb["closed"] and xa["poses_ori"].tobytes() == xb["poses_ori"].tobytes() and xa["poses_opt"].tobytes() == xb["poses_opt"].tobytes()
-    a.close(); b.close()
+    if kind == "scans":
+        return a, b, [a.process_new_scan(r, t) for r, t in zip(raws, stamps)], b.process_new_scans(raws, stamps)
+    ra = [e for f, s in zip(raws, stamps) for e in a.process_new_frame(f, s)]
+    rb = [e for f in b.process_new_frames(raws, stamps) for e in f]
+    assert len(ra) == 2 * len(raws)
+    return a, b, ra, rb
+
+
+def test_sequence_calls_give_the_single_calls_log(ctxs):
+    for kind in ("scans", "frames"):
+        a, b, ra, rb = _sequence_and_single_calls(ctxs, kind)
+        assert [_entry(x) for x, _ in ra] == [_entry(x) for x, _ in rb], kind
+        la, lb = a.loop_log()[0], b.loop_log()[0]
+        assert len(la) > 0 and [_ev(e) for e in la] == [_ev(e) for e in lb], kind
+        xa, xb = a.loop_result(), b.loop_result()
+        assert xa["closed"] == xb["closed"] and xa["poses_ori"].tobytes() == xb["poses_ori"].tobytes() and xa["poses_opt"].tobytes() == xb["poses_opt"].tobytes(), kind
+        a.close(); b.close()
 
 
 @pytest.mark.parametrize("each,between", [(6, 5), (6, 1), (3, 2)])
