@@ -766,8 +766,8 @@ int  ll_loop_search(ll_ctx* ctx, const ll_keyframe* const* kfs, int n, int newes
  * more than one and its pop (:1554-1557) cannot fire.  After the first loop the reference searches no more (if_end, :990-993): the mapper then
  * stops all loop-closure work.  Loop closure never changes the odometry: an error of its work other than LL_ERR_CUDA does not fail the step.
  * A failed alignment ends that keyframe's search (LL_LOOP_FAILED); any other error is logged (LL_LOOP_ERROR) and stops loop closure for good.
- * LL_ERR_CUDA is returned.  It is a runtime setting: it is not part of a mapper image, and a
- * loaded mapper has it off. */
+ * LL_ERR_CUDA is returned.  It is not part of a mapper image (a loaded mapper has it off): its state has an image of its own, the loop image
+ * (ll_mapper_loop_save / ll_mapper_loop_load below). */
 typedef struct {
   int    scans_of_each_keyframe;              /* loop_closure/scans_of_each_keyframe (300)                                                  */
   int    scans_between_two_keyframe;          /* loop_closure/scans_between_two_keyframe (100); must be < scans_of_each_keyframe           */
@@ -823,6 +823,82 @@ int  ll_mapper_loop_result(ll_mapper* mapper, int* n, int* closed, ll_pose* pose
 /* The refined cloud of published keyframe k (after the loop closed; k = n - 1, n - 3, ..., else LL_ERR_INVALID), as ll_keyframe_cloud offers
  * its clouds: on the device (*out_dev, valid until loop closure is set again) and copied to out_host (cap points) when that is not NULL. */
 int  ll_mapper_loop_cloud(ll_mapper* mapper, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev);
+
+/* ---- loop image: the mapper's loop closure as a byte image of its own (DESIGN.md §4.6.1) ------------------------------------------------
+ * Checkpoint a run with loop closure on: save the mapper image and the loop image at the same step, then ll_mapper_load the one and
+ * ll_mapper_loop_load the other onto the loaded mapper.  The restored mapper continues bit for bit as the saved one: every ll_reg_result field
+ * except gpu_ms_*, every integer stat, every loop event (but ll_pg_summary::cycles_*, which time the solve and are saved as 0),
+ * ll_mapper_loop_result and every ll_mapper_loop_cloud.  The mapper image is unchanged by loop closure (same bytes with it on or off).
+ *
+ * Format (version 1), one little-endian byte string, with the mapper image's conventions (header of (offset, length) sections, placed back to
+ * back in index order by a writer, canonical contents):
+ *   ll_loop_image_header          magic "LLLOOPIM", version, config_bytes = sizeof(ll_loop_closure_cfg), total_bytes, the sections
+ *   LL_LOOP_IMAGE_CONFIG          the ll_loop_closure_cfg in force, verbatim with its padding bytes zero
+ *   LL_LOOP_IMAGE_SCALARS         ll_loop_image_scalars: the binding stamp, closed / stopped and the counts below
+ *   LL_LOOP_IMAGE_CELLS           the full-resolution cell map: int32 current_frame_idx, int32 n_out_of_range, int64 n_cells, int64 n_points,
+ *                                 ll_image_cell cells[n_cells] (ascending key), ll_image_cell_point points[n_points] (store order: the live
+ *                                 points and those of every incarnation an open keyframe holds), int32 current[n_cells] (the ordinal of each
+ *                                 cell's current incarnation), int32 incarnation[n_points] (each point's).  Ordinals number a cell's kept
+ *                                 incarnations in epoch order: 0 is the cell's first incarnation (kept only while it exists), the later
+ *                                 ones 1, 2, ...; so a cell has current + 1 kept incarnations when its first is kept, current otherwise
+ *                                 (current <= current_frame_idx: a cell is replaced at most once per append).
+ *   LL_LOOP_IMAGE_HISTORY         the full history: int64 n_segments, int64 n_points, int32 size[n_segments] (oldest first), ll_point points[]
+ *   LL_LOOP_IMAGE_OPEN            the open keyframes in list order: ll_loop_image_open open[n_open], then each one's cells as
+ *                                 ll_loop_image_ref (cell rank, incarnation ordinal), ascending
+ *   LL_LOOP_IMAGE_KEYFRAMES       the closed keyframes in closing order: ll_keyframe_info info[n_keyframes]
+ *   LL_LOOP_IMAGE_POSES           ll_pose poses_ori[n_keyframes]
+ *   LL_LOOP_IMAGE_EDGES           ll_pg_edge odometry[n_keyframes - 1] (none without keyframes)
+ *   LL_LOOP_IMAGE_IMAGES          float images[n_keyframes][4][60 * 60] (ll_keyframe_images' order; zeros for a keyframe without cells)
+ *   LL_LOOP_IMAGE_CLOUDS          each closed keyframe's line then plane cloud (info.line_points + info.plane_points ll_point), in order
+ *   LL_LOOP_IMAGE_ACCUMULATED     int64 n_acc (= n_keyframes + n_open - 1), int64 end[n_acc] (non-decreasing), ll_point points[end[n_acc - 1]]
+ *   LL_LOOP_IMAGE_LOOP            closed = 1: ll_pg_edge loop_edge, ll_pose poses_opt[n_keyframes]; closed = 0: empty
+ *   LL_LOOP_IMAGE_EVENTS          the unread events, oldest first: ll_loop_event events[n_events] (n_events <= LL_LOOP_LOG), their
+ *                                 summary.cycles_* (SM clock counters that time the solve, not state) 0
+ * The refined clouds are not saved: ll_mapper_loop_load recomputes them from the accumulated clouds and both pose sets by the code the loop
+ * ran.  Not saved either, as no result depends on them: the capture buffers (empty between calls), the pose-graph arena, hash slots, dead
+ * incarnations no open keyframe holds, a closed keyframe's cell list, per-cell types and all-points cloud (only its info, images and line and
+ * plane clouds are read again), capacities, reservations and arena offsets.  So the same stream gives byte-identical loop images, and
+ * load-then-save reproduces one byte for byte.
+ * The binding stamp (the mapper's frame index, pose, last time stamp, matching mode, and the mapper settings loop closure copied) guards
+ * against pairing a loop image with the wrong mapper: ll_mapper_loop_load refuses an image whose stamp differs from the mapper's.  It is a
+ * guard, not a proof that both images come from the same run and step. */
+#define LL_LOOP_IMAGE_MAGIC "LLLOOPIM"
+#define LL_LOOP_IMAGE_VERSION 1
+enum { LL_LOOP_IMAGE_CONFIG = 0, LL_LOOP_IMAGE_SCALARS = 1, LL_LOOP_IMAGE_CELLS = 2, LL_LOOP_IMAGE_HISTORY = 3, LL_LOOP_IMAGE_OPEN = 4,
+       LL_LOOP_IMAGE_KEYFRAMES = 5, LL_LOOP_IMAGE_POSES = 6, LL_LOOP_IMAGE_EDGES = 7, LL_LOOP_IMAGE_IMAGES = 8, LL_LOOP_IMAGE_CLOUDS = 9,
+       LL_LOOP_IMAGE_ACCUMULATED = 10, LL_LOOP_IMAGE_LOOP = 11, LL_LOOP_IMAGE_EVENTS = 12, LL_LOOP_IMAGE_SECTIONS = 13 };
+typedef struct { char magic[8]; uint32_t version, config_bytes; uint64_t total_bytes; ll_image_section section[LL_LOOP_IMAGE_SECTIONS]; } ll_loop_image_header;   /* 232 B */
+typedef struct {
+  int32_t frame_index, matching_mode;           /* binding stamp: the mapper's m_current_frame_index and matching_mode,                  */
+  int32_t threshold_cell_revisit, maximum_history_size, pieces;   /* its config values loop closure copied (pieces: pipeline.pieces)    */
+  float   cell_resolution;
+  double  last_time_stamp, q_w_curr[4], t_w_curr[3];   /* ... and its last time stamp and pose                                            */
+  int32_t closed, stopped;                      /* 0 / 1: the loop closed (if_end) / an error stopped loop closure                        */
+  int32_t n_keyframes, n_open, n_events, n_dropped;   /* closed keyframes, open keyframes (>= 1), unread events, events overwritten unread */
+} ll_loop_image_scalars;                        /* 112 B */
+typedef struct { int32_t frames, accumulate_frames; int64_t n_cells; } ll_loop_image_open;   /* frames since it opened, m_accumulate_frames */
+typedef struct { int32_t cell, incarnation; } ll_loop_image_ref;                             /* cell rank in LL_LOOP_IMAGE_CELLS, ordinal   */
+typedef struct {
+  uint64_t bytes;
+  int64_t  cells, cell_points;                  /* the full map's cells and kept points                                                   */
+  int64_t  replaced_points;                     /* kept points of replaced incarnations (held by an open keyframe after a revisit)        */
+  int64_t  history_points, cloud_points, accumulated_points;
+  uint32_t version;
+  int32_t  frame_index, matching_mode, closed, stopped, keyframes, open_keyframes, events, dropped;
+  int32_t  max_incarnation;                     /* the largest current ordinal of a cell                                                  */
+} ll_loop_image_summary;                         /* 96 B */
+/* image NULL: *bytes = the size needed.  cap < needed: LL_ERR_CAPACITY, nothing written.  Loop closure off: LL_ERR_INVALID.  The mapper is not
+ * modified (the event ring is not drained). */
+int  ll_mapper_loop_save(ll_mapper* mapper, void* image, size_t cap, size_t* bytes);
+/* Restores loop closure onto `mapper` (typically just made by ll_mapper_load from the mapper image saved at the same step), replacing any loop
+ * closure it has, as ll_mapper_set_loop_closure does.  cfg NULL: the image's config; otherwise equal to it except max_cells and the reserve_*
+ * fields, which size the allocations only (the mapper's later loop images keep the image's config).  The image is validated completely before
+ * anything touches the device: a refused image (LL_ERR_INVALID; a stamp that differs from the mapper's: LL_ERR_INVALID; more cells than half
+ * the table of the effective max_cells: LL_ERR_CAPACITY) changes nothing. */
+int  ll_mapper_loop_load(ll_mapper* mapper, const void* image, size_t bytes, const ll_loop_closure_cfg* cfg);
+/* Host only, no context or GPU: validates a loop image completely (as ll_mapper_loop_load with cfg NULL, but for the stamp and the cell table's
+ * capacity: a mapper loaded with a larger max_cells can save an image that needs that max_cells again) and reports what is in it. */
+int  ll_loop_image_info(const void* image, size_t bytes, ll_loop_image_summary* info);
 
 /* ---- spinning-lidar front end: the Velodyne branch of Laser_feature::laserCloudHandler (DESIGN.md §4.7) ---------------------------------
  * laser_feature_extractor.hpp:393-825 with lidar_type other than "livox": NaN and near points removed (:399-400), ring and relative time per

@@ -320,8 +320,18 @@ class Laser_mapping {
     return out;
   }
   // loop closure (ll_mapper_set_loop_closure, loop_closure/if_enable_loop_closure): cfg NULL turns it off; a bad value throws and leaves the
-  // mapper unchanged.  Not part of an image: a mapper from load_from_image has it off.
+  // mapper unchanged.  Not part of a mapper image (a mapper from load_from_image has it off): loop_save / loop_load carry it.
   void set_loop_closure(const ll_loop_closure_cfg* cfg) { ctx_.check(ll_mapper_set_loop_closure(mapper_, cfg)); }
+  // the loop closure as a loop image of its own (ll_mapper_loop_save; format in loamlivox_b200.h); throws when loop closure is off
+  void loop_save(std::vector<uint8_t>& image) const {
+    size_t n = 0;
+    ctx_.check(ll_mapper_loop_save(mapper_, nullptr, 0, &n));
+    image.resize(n);
+    ctx_.check(ll_mapper_loop_save(mapper_, image.data(), image.size(), &n));
+  }
+  // restores a loop image onto this mapper (ll_mapper_loop_load; typically one from load_from_image of the mapper image saved at the same
+  // step).  cfg NULL: the image's config; otherwise it may differ from it only in max_cells and reserve_*.  A refused image throws and changes nothing.
+  void loop_load(const std::vector<uint8_t>& image, const ll_loop_closure_cfg* cfg = nullptr) { ctx_.check(ll_mapper_loop_load(mapper_, image.data(), image.size(), cfg)); }
   // the loop-closure events since the last read, oldest first (ll_mapper_loop_read); *dropped = events overwritten unread
   std::vector<ll_loop_event> loop_log(int* dropped = nullptr) {
     std::vector<ll_loop_event> out, buf(LL_LOOP_LOG);

@@ -29,6 +29,9 @@ LL_LOOP_LOG = 1024
 LL_LOOP_KEYFRAME, LL_LOOP_ALIGNMENT, LL_LOOP_CLOSED, LL_LOOP_ERROR = 0, 1, 2, 3
 LL_LOOP_SKIP10, LL_LOOP_SKIP5, LL_LOOP_ACCEPT, LL_LOOP_FAILED = 0, 1, 2, 3
 LL_MAPPER_IMAGE_MAGIC, LL_MAPPER_IMAGE_VERSION = b"LLMAPIMG", 1
+LL_LOOP_IMAGE_MAGIC, LL_LOOP_IMAGE_VERSION = b"LLLOOPIM", 1
+(LL_LOOP_IMAGE_CONFIG, LL_LOOP_IMAGE_SCALARS, LL_LOOP_IMAGE_CELLS, LL_LOOP_IMAGE_HISTORY, LL_LOOP_IMAGE_OPEN, LL_LOOP_IMAGE_KEYFRAMES, LL_LOOP_IMAGE_POSES,
+ LL_LOOP_IMAGE_EDGES, LL_LOOP_IMAGE_IMAGES, LL_LOOP_IMAGE_CLOUDS, LL_LOOP_IMAGE_ACCUMULATED, LL_LOOP_IMAGE_LOOP, LL_LOOP_IMAGE_EVENTS, LL_LOOP_IMAGE_SECTIONS) = range(14)
 (LL_IMAGE_CONFIG, LL_IMAGE_SCALARS, LL_IMAGE_HISTORY_CORNER, LL_IMAGE_HISTORY_SURF, LL_IMAGE_SNAPSHOT_CORNER, LL_IMAGE_SNAPSHOT_SURF, LL_IMAGE_CELLS_CORNER,
  LL_IMAGE_CELLS_SURF, LL_IMAGE_SECTIONS) = range(9)
 
@@ -51,6 +54,7 @@ EXPORTS = [
     "ll_mapper_loop_closure_default", "ll_mapper_set_loop_closure", "ll_mapper_loop_read", "ll_mapper_loop_result", "ll_mapper_loop_cloud",
     "ll_spin_cfg_default", "ll_spin_create", "ll_spin_release", "ll_spin_extract", "ll_spin_cloud", "ll_spin_point_info", "ll_spin_chains",
     "ll_mapper_process_sweep", "ll_mapper_process_sweeps",
+    "ll_mapper_loop_save", "ll_mapper_loop_load", "ll_loop_image_info",
 ]
 LL_SPIN_FULL, LL_SPIN_SHARP, LL_SPIN_LESS_SHARP, LL_SPIN_FLAT, LL_SPIN_LESS_FLAT = 0, 1, 2, 3, 4
 LL_CELL_SPHERE, LL_CELL_LINE, LL_CELL_PLANE, LL_CELL_ALL = 0, 1, 2, -1
@@ -210,6 +214,21 @@ class LoopEvent(C.Structure):
                [("inlier_threshold", C.c_double), ("icp_q_wxyz", C.c_double * 4), ("icp_t", C.c_double * 3), ("edge", PgEdge), ("summary", PgSummary)]
 
 
+class LoopImageScalars(C.Structure):
+    """ll_loop_image_scalars: the loop image's binding stamp (the mapper's state it refers to), closed / stopped and the counts."""
+    _fields_ = [(n, C.c_int32) for n in ("frame_index", "matching_mode", "threshold_cell_revisit", "maximum_history_size", "pieces")] + \
+               [("cell_resolution", C.c_float), ("last_time_stamp", C.c_double), ("q_w_curr", C.c_double * 4), ("t_w_curr", C.c_double * 3)] + \
+               [(n, C.c_int32) for n in ("closed", "stopped", "n_keyframes", "n_open", "n_events", "n_dropped")]
+
+
+class LoopImageSummary(C.Structure):
+    """ll_loop_image_summary: what ll_loop_image_info reports about a loop image."""
+    _fields_ = [("bytes", C.c_uint64)] + [(n, C.c_int64) for n in ("cells", "cell_points", "replaced_points", "history_points", "cloud_points",
+                                                                    "accumulated_points")] + \
+               [("version", C.c_uint32)] + [(n, C.c_int32) for n in ("frame_index", "matching_mode", "closed", "stopped", "keyframes", "open_keyframes",
+                                                                     "events", "dropped", "max_incarnation")]
+
+
 class LoamLivoxError(RuntimeError):
     pass
 
@@ -347,6 +366,9 @@ def lib():
     L.ll_spin_chains.argtypes = [vp, C.POINTER(ci), C.POINTER(ci)]
     L.ll_mapper_process_sweep.argtypes = [vp, vp, vp, sz, ci, ci, C.POINTER(RegResult), C.POINTER(MapperStats)]
     L.ll_mapper_process_sweeps.argtypes = [vp, vp, ci, vp, vp, ci, ci, C.POINTER(RegResult), C.POINTER(MapperStats), C.POINTER(ci)]
+    L.ll_mapper_loop_save.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.ll_mapper_loop_load.argtypes = [vp, vp, sz, C.POINTER(LoopClosureCfg)]
+    L.ll_loop_image_info.argtypes = [vp, sz, C.POINTER(LoopImageSummary)]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64
     _LIB = L

@@ -380,56 +380,74 @@ int ll_cellmap_assemble(ll_ctx* ctx, ll_cellmap* m, const double q_wxyz[4], cons
 
 }  // extern "C"
 
-// ---- checkpoint (ll_mapper_save / ll_mapper_load) ---------------------------------------------------------------------------------
+// ---- checkpoint (ll_mapper_save / ll_mapper_load, ll_mapper_loop_save / ll_mapper_loop_load) -------------------------------------------
 // A map leaves as its cells in ascending key (key, create_frame, last_update) and its live points in store order (xyz, rank of the cell in
 // that list), and comes back into an empty table with every cell at epoch 0, bump -1 and every point at epoch 0.  Nothing a result depends on
 // changes: the assembly ranks cells by key and keeps store order inside a voxel, and liveness is only "point epoch == cell epoch".
+// With a held list (the loop image: the (slot << 32 | epoch) ids the open keyframes hold, sorted and distinct) the points of those
+// incarnations leave too, and every kept point and every cell carry an incarnation ordinal (cm_ordinal); the import sets them as the epochs.
+__device__ __forceinline__ bool cm_is_held(const unsigned long long* held, int n_held, int s, int e) {
+  const unsigned long long id = ((unsigned long long)(unsigned)s << 32) | (unsigned)e;
+  const int at = cm_lower_bound(held, n_held, id);
+  return at < n_held && held[at] == id;
+}
 __global__ void cm_occupied_kernel(const unsigned long long* __restrict__ keys, int cap, unsigned char* __restrict__ flag) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s < cap) flag[s] = keys[s] != CM_EMPTY ? 1 : 0;
 }
-__global__ void cm_live_kernel(const int* __restrict__ pt_slot, const int* __restrict__ pt_epoch, int n, const int* __restrict__ epoch, unsigned char* __restrict__ flag) {
+// kept: live, or of an incarnation in the held list (n_held 0: live only)
+__global__ void cm_live_kernel(const int* __restrict__ pt_slot, const int* __restrict__ pt_epoch, int n, const int* __restrict__ epoch, const unsigned long long* __restrict__ held,
+                               int n_held, unsigned char* __restrict__ flag) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= n) return;
   const int s = pt_slot[t];
-  flag[t] = (s >= 0 && pt_epoch[t] == epoch[s]) ? 1 : 0;
+  flag[t] = (s >= 0 && (pt_epoch[t] == epoch[s] || (n_held > 0 && cm_is_held(held, n_held, s, pt_epoch[t])))) ? 1 : 0;
 }
+// cur (NULL: none): the ordinal of every cell's current incarnation
 __global__ void cm_export_cells_kernel(const unsigned long long* __restrict__ sorted_keys, const int* __restrict__ sorted_slots, int n, const int* __restrict__ create_frame,
-                                       const int* __restrict__ last_update, ll_image_cell* __restrict__ out) {
+                                       const int* __restrict__ last_update, ll_image_cell* __restrict__ out, const int* __restrict__ epoch,
+                                       const unsigned long long* __restrict__ held, int n_held, int* __restrict__ cur) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
   const int s = sorted_slots[r];
   ll_image_cell c; c.key = sorted_keys[r]; c.create_frame = create_frame[s]; c.last_update = last_update[s];
   out[r] = c;
+  if (cur) cur[r] = cm_ordinal(held, n_held, s, epoch[s]);
 }
+// ord (NULL: none): the ordinal of every point's incarnation
 __global__ void cm_export_points_kernel(const float4* __restrict__ pts, const int* __restrict__ pt_slot, const int* __restrict__ idx, int n, const int* __restrict__ rank_of_slot,
-                                        ll_image_cell_point* __restrict__ out) {
+                                        ll_image_cell_point* __restrict__ out, const int* __restrict__ pt_epoch, const unsigned long long* __restrict__ held, int n_held,
+                                        int* __restrict__ ord) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
   const int t = idx[r]; const float4 p = pts[t];
   ll_image_cell_point o; o.x = p.x; o.y = p.y; o.z = p.z; o.cell = rank_of_slot[pt_slot[t]];
   out[r] = o;
+  if (ord) ord[r] = cm_ordinal(held, n_held, pt_slot[t], pt_epoch[t]);
 }
-// one thread per cell: the probe sequence of cm_locate_kernel into an empty table (keys are distinct, so every CAS claims a fresh slot)
+// one thread per cell: the probe sequence of cm_locate_kernel into an empty table (keys are distinct, so every CAS claims a fresh slot); cur (NULL:
+// every epoch 0) the cells' epochs
 __global__ void cm_import_cells_kernel(const ll_image_cell* __restrict__ in, int n, unsigned long long* keys, unsigned mask, int* create_frame, int* last_update, int* epoch, int* bump,
-                                       int* __restrict__ slot_of_rank) {
+                                       int* __restrict__ slot_of_rank, const int* __restrict__ cur) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
   const ll_image_cell c = in[r];
   unsigned h = cm_hash(c.key, mask);
   while (atomicCAS(&keys[h], CM_EMPTY, c.key) != CM_EMPTY) h = (h + 1) & mask;
-  create_frame[h] = c.create_frame; last_update[h] = c.last_update; epoch[h] = 0; bump[h] = -1;
+  create_frame[h] = c.create_frame; last_update[h] = c.last_update; epoch[h] = cur ? cur[r] : 0; bump[h] = -1;
   slot_of_rank[r] = (int)h;
 }
+// ord (NULL: every epoch 0) the points' epochs
 __global__ void cm_import_points_kernel(const ll_image_cell_point* __restrict__ in, int n, const int* __restrict__ slot_of_rank, float4* __restrict__ pts, int* __restrict__ pt_slot,
-                                        int* __restrict__ pt_epoch) {
+                                        int* __restrict__ pt_epoch, const int* __restrict__ ord) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= n) return;
   const ll_image_cell_point p = in[t];
-  pts[t] = make_float4(p.x, p.y, p.z, 0.f); pt_slot[t] = slot_of_rank[p.cell]; pt_epoch[t] = 0;
+  pts[t] = make_float4(p.x, p.y, p.z, 0.f); pt_slot[t] = slot_of_rank[p.cell]; pt_epoch[t] = ord ? ord[t] : 0;
 }
 
-// The export's scratch over a table of T slots and a store of N points; rec = the cells then the live points, as the image holds them
+// The export's scratch over a table of T slots and a store of N points; rec = the cells then the kept points, as the image holds them (with a
+// held list: then the cells' current ordinals and the points' ordinals)
 struct CmExport {
   size_t cub_bytes = 0;
   unsigned char* flag; int* slots; unsigned long long* keys; unsigned long long* keys2; int* slots2; int* rank; int* idx; int* cnt; char* cub_tmp; int4* rec;
@@ -444,6 +462,7 @@ struct CmExport {
     slots2 = c.take<int>(T); rank = c.take<int>(T); idx = c.take<int>(N); cnt = c.take<int>(16); cub_tmp = c.take<char>(cub_bytes); rec = c.take<int4>(n_rec);
   }
 };
+static size_t cm_export_rec(size_t n_cells, size_t n_pts, const CmHeld* held) { return n_cells + n_pts + (held ? (n_cells + n_pts + 3) / 4 : 0); }   // int4 records
 
 // Cells in the table and live points in the store, the frame index and the out-of-range count (the map is only read)
 int cm_count(ll_ctx* ctx, ll_cellmap* m, int* n_cells, int* n_live, int* frame_idx, int* n_out_of_range) {
@@ -461,25 +480,42 @@ int cm_count(ll_ctx* ctx, ll_cellmap* m, int* n_cells, int* n_live, int* frame_i
   return LL_OK;
 }
 
-// The store indices of the live points in store order into a.idx (their count into a.cnt[1]), on the context's stream.
-static int cm_select_live(ll_ctx* ctx, ll_cellmap* m, CmExport& a) {
+// The store indices of the kept points (live, and those of the held incarnations) in store order into a.idx (their count into a.cnt[1]), on the
+// context's stream.
+static int cm_select_live(ll_ctx* ctx, ll_cellmap* m, CmExport& a, const CmHeld* held = nullptr) {
   size_t cub_c = a.cub_bytes;
   const int N = m->n_pts;
-  cm_live_kernel<<<ll_div_up(N, 256), 256, 0, ctx->stream>>>(m->pt_slot, m->pt_epoch, N, m->epoch, a.flag);
+  cm_live_kernel<<<ll_div_up(N, 256), 256, 0, ctx->stream>>>(m->pt_slot, m->pt_epoch, N, m->epoch, held ? held->ids : nullptr, held ? held->n : 0, a.flag);
   LL_CUDA(ctx, cub::DeviceSelect::Flagged(a.cub_tmp, cub_c, cub::CountingInputIterator<int>(0), a.flag, a.idx, a.cnt + 1, N, ctx->stream));
   ctx->launches += 2;
   return LL_OK;
 }
 
+// The kept points of a map with a held list (the count cm_export takes); the map is only read.
+int cm_count_kept(ll_ctx* ctx, ll_cellmap* m, const CmHeld& held, int* n_kept) {
+  *n_kept = 0;
+  const int T = m->table_cap, N = m->n_pts;
+  if (N == 0) return LL_OK;
+  CmExport a(T, N);
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { a.layout(c, T, N, 0); }));
+  LL_TRY(cm_select_live(ctx, m, a, &held));
+  LL_CUDA(ctx, cudaMemcpyAsync(n_kept, a.cnt + 1, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return LL_OK;
+}
+
 // The map's cells (ascending key) and live points (store order) into out: n_cells ll_image_cell then n_live ll_image_cell_point, the counts
-// cm_count gave.  One copy to the host; the map's buffers are only read.
-int cm_export(ll_ctx* ctx, ll_cellmap* m, int n_cells, int n_live, void* out) {
+// cm_count gave; with a held list also the points of the held incarnations, then int32 current ordinal[n_cells] and ordinal[n_live] (n_live:
+// cm_count_kept's count).  One copy to the host; the map's buffers are only read.
+int cm_export(ll_ctx* ctx, ll_cellmap* m, int n_cells, int n_live, void* out, const CmHeld* held) {
   cudaStream_t s = ctx->stream;
   const int T = m->table_cap, N = m->n_pts;
   if (n_cells + n_live == 0) return LL_OK;
   CmExport a(T, N);
-  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { a.layout(c, T, N, (size_t)n_cells + n_live); }));
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { a.layout(c, T, N, cm_export_rec((size_t)n_cells, (size_t)n_live, held)); }));
   ll_image_cell* cells = (ll_image_cell*)a.rec; ll_image_cell_point* pts = (ll_image_cell_point*)(a.rec + n_cells);
+  int* cur = held ? (int*)(a.rec + n_cells + n_live) : nullptr; int* ord = held ? cur + n_cells : nullptr;
+  const unsigned long long* h_ids = held ? held->ids : nullptr; const int n_held = held ? held->n : 0;
   size_t cub_c = a.cub_bytes;
   LL_CUDA(ctx, cudaMemsetAsync(a.cnt, 0, 8, s));
   // cells: occupied slots, sorted by key, and the rank of every slot
@@ -490,18 +526,21 @@ int cm_export(ll_ctx* ctx, ll_cellmap* m, int n_cells, int n_live, void* out) {
     cm_gather_keys_kernel<<<ll_div_up(n_cells, 256), 256, 0, s>>>(m->keys, a.slots, a.cnt + 0, a.keys);
     LL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(a.cub_tmp, cub_c, a.keys, a.keys2, a.slots, a.slots2, n_cells, 0, 64, s));
     cm_rank_kernel<<<ll_div_up(n_cells, 256), 256, 0, s>>>(a.slots2, n_cells, a.rank);
-    cm_export_cells_kernel<<<ll_div_up(n_cells, 256), 256, 0, s>>>(a.keys2, a.slots2, n_cells, m->create_frame, m->last_update, cells);
+    cm_export_cells_kernel<<<ll_div_up(n_cells, 256), 256, 0, s>>>(a.keys2, a.slots2, n_cells, m->create_frame, m->last_update, cells, m->epoch, h_ids, n_held, cur);
     ctx->launches += 4;
   }
-  // live points in store order
+  // kept points in store order
   if (N > 0) {
-    LL_TRY(cm_select_live(ctx, m, a));
-    if (n_live > 0) { cm_export_points_kernel<<<ll_div_up(n_live, 256), 256, 0, s>>>(m->pts, m->pt_slot, a.idx, n_live, a.rank, pts); ctx->launches++; }
+    LL_TRY(cm_select_live(ctx, m, a, held));
+    if (n_live > 0) {
+      cm_export_points_kernel<<<ll_div_up(n_live, 256), 256, 0, s>>>(m->pts, m->pt_slot, a.idx, n_live, a.rank, pts, m->pt_epoch, h_ids, n_held, ord);
+      ctx->launches++;
+    }
   }
   LL_CUDA(ctx, cudaGetLastError());
   int h[2] = {0, 0};
   LL_CUDA(ctx, cudaMemcpyAsync(h, a.cnt, 8, cudaMemcpyDeviceToHost, s));
-  LL_CUDA(ctx, cudaMemcpyAsync(out, a.rec, ((size_t)n_cells + n_live) * 16, cudaMemcpyDeviceToHost, s));
+  LL_CUDA(ctx, cudaMemcpyAsync(out, a.rec, ((size_t)n_cells + n_live) * (held ? 20 : 16), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   if (h[0] != n_cells || h[1] != n_live) { ctx->set_error("cell map changed while it was saved"); return LL_ERR_INVALID; }
   return LL_OK;
@@ -519,24 +558,29 @@ int cm_live_points(ll_ctx* ctx, ll_cellmap* m, int n_live, float4* dst) {
 }
 
 // An empty map (just created) in the state of an exported one: in = n_cells ll_image_cell (ascending key) then n_live ll_image_cell_point,
-// host memory, validated by the caller (distinct keys, ranks < n_cells).
-int cm_import(ll_ctx* ctx, ll_cellmap* m, int frame_idx, int n_out_of_range, const void* in, int n_cells, int n_live) {
+// with incarnations then int32 current ordinal[n_cells] and ordinal[n_live] (set as the epochs), host memory, validated by the caller
+// (distinct keys, ranks < n_cells, ordinals <= their cell's current one).  slot_of_rank (NULL: not wanted): each cell's slot, to the host.
+int cm_import(ll_ctx* ctx, ll_cellmap* m, int frame_idx, int n_out_of_range, const void* in, int n_cells, int n_live, bool incarnations, int* slot_of_rank_out) {
   cudaStream_t s = ctx->stream;
   if (m->n_pts != 0 || m->n_cells != 0) { ctx->set_error("import into a cell map that is not empty"); return LL_ERR_INVALID; }
   if (n_cells > m->table_cap / 2) { ctx->set_error("cell table more than half full: create the map with a larger max_cells"); return LL_ERR_CAPACITY; }
   if (n_live > 0) LL_TRY(cm_reserve_store(ctx, m, n_live));
   int4* rec = nullptr; int* slot_of_rank = nullptr;
-  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { rec = c.take<int4>((size_t)n_cells + n_live); slot_of_rank = c.take<int>(n_cells); }));
-  if (n_cells + n_live > 0) LL_CUDA(ctx, cudaMemcpyAsync(rec, in, ((size_t)n_cells + n_live) * 16, cudaMemcpyHostToDevice, s));
+  const CmHeld none{nullptr, 0};
+  const size_t n_rec = cm_export_rec((size_t)n_cells, (size_t)n_live, incarnations ? &none : nullptr);
+  LL_CUDA(ctx, ctx->scratch.carve([&](Carve& c) { rec = c.take<int4>(n_rec); slot_of_rank = c.take<int>(n_cells); }));
+  if (n_cells + n_live > 0) LL_CUDA(ctx, cudaMemcpyAsync(rec, in, ((size_t)n_cells + n_live) * (incarnations ? 20 : 16), cudaMemcpyHostToDevice, s));
+  const int* cur = incarnations ? (const int*)(rec + n_cells + n_live) : nullptr; const int* ord = incarnations ? cur + n_cells : nullptr;
   if (n_cells > 0) {
     cm_import_cells_kernel<<<ll_div_up(n_cells, 256), 256, 0, s>>>((const ll_image_cell*)rec, n_cells, m->keys, (unsigned)(m->table_cap - 1), m->create_frame, m->last_update,
-                                                                   m->epoch, m->bump, slot_of_rank);
+                                                                   m->epoch, m->bump, slot_of_rank, cur);
     ctx->launches++;
   }
   if (n_live > 0) {
-    cm_import_points_kernel<<<ll_div_up(n_live, 256), 256, 0, s>>>((const ll_image_cell_point*)(rec + n_cells), n_live, slot_of_rank, m->pts, m->pt_slot, m->pt_epoch);
+    cm_import_points_kernel<<<ll_div_up(n_live, 256), 256, 0, s>>>((const ll_image_cell_point*)(rec + n_cells), n_live, slot_of_rank, m->pts, m->pt_slot, m->pt_epoch, ord);
     ctx->launches++;
   }
+  if (slot_of_rank_out && n_cells > 0) LL_CUDA(ctx, cudaMemcpyAsync(slot_of_rank_out, slot_of_rank, (size_t)n_cells * 4, cudaMemcpyDeviceToHost, s));
   const int c[3] = {n_cells, 0, n_out_of_range};   // d_counters: cells, scratch, points out of the key's range so far
   LL_CUDA(ctx, cudaMemcpyAsync(m->d_counters, c, sizeof(c), cudaMemcpyHostToDevice, s));
   LL_CUDA(ctx, cudaGetLastError());

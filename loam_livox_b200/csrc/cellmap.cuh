@@ -27,3 +27,18 @@ __device__ __forceinline__ unsigned long long cm_pack(int k, int j, int i) {
 __device__ __forceinline__ void cm_unpack(unsigned long long key, int& k, int& j, int& i) {
   k = (int)((key >> 42) & 0x1fffffull) - CM_BIAS; j = (int)((key >> 21) & 0x1fffffull) - CM_BIAS; i = (int)(key & 0x1fffffull) - CM_BIAS;
 }
+
+// The loop image (ll_mapper_loop_save) keeps, beside a cell's current incarnation, those the open keyframes hold: `held`, their sorted, distinct
+// (slot << 32 | epoch) ids.  A kept incarnation leaves as its ordinal: 0 for the cell's first incarnation (epoch 0, the one ll_keyframe_analyze
+// builds incrementally), otherwise 1 + the held incarnations of the slot with 0 < epoch < e.  Ordinals keep the epoch order of every cell.
+__host__ __device__ inline int cm_lower_bound(const unsigned long long* a, int n, unsigned long long x) {
+  int lo = 0, hi = n;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] < x) lo = mid + 1; else hi = mid; }
+  return lo;
+}
+__host__ __device__ inline int cm_ordinal(const unsigned long long* held, int n_held, int s, int e) {
+  if (e == 0) return 0;
+  const unsigned long long base = (unsigned long long)(unsigned)s << 32;
+  const int lo = cm_lower_bound(held, n_held, base), at = cm_lower_bound(held, n_held, base | (unsigned)e);
+  return 1 + (at - lo) - ((lo < n_held && held[lo] == base) ? 1 : 0);
+}

@@ -235,14 +235,45 @@ int launch_gather_pieces(ll_ctx* ctx, cudaStream_t s, FrameDev* dev, const Frame
 // ---------------------------------------------------------------------------------------------- cell-map checkpoint (cellmap.cu)
 // Cells in the table and live points in the store, current_frame_idx and n_out_of_range; the map is only read.
 int cm_count(ll_ctx* ctx, ll_cellmap* m, int* n_cells, int* n_live, int* frame_idx, int* n_out_of_range);
+// Incarnations kept beside the live points (the loop image): the sorted, distinct (slot << 32 | epoch) ids the open keyframes hold, on the device.
+struct CmHeld { const unsigned long long* ids; int n; };
+// The points of a map that an export with `held` keeps: the live ones and those of the held incarnations.
+int cm_count_kept(ll_ctx* ctx, ll_cellmap* m, const CmHeld& held, int* n_kept);
 // The cells in ascending key then the live points in store order, as the image's cell section holds them (n_cells ll_image_cell, n_live
-// ll_image_cell_point, the counts cm_count gave), copied once to host memory `out`; the map is only read.
-int cm_export(ll_ctx* ctx, ll_cellmap* m, int n_cells, int n_live, void* out);
-// An empty map in the state cm_export recorded (records validated by the caller: keys distinct, cell ranks < n_cells).
-int cm_import(ll_ctx* ctx, ll_cellmap* m, int frame_idx, int n_out_of_range, const void* in, int n_cells, int n_live);
+// ll_image_cell_point, the counts cm_count gave), copied once to host memory `out`; the map is only read.  With `held` (n_live: cm_count_kept's
+// count) the held incarnations' points too, then int32 ordinals (cellmap.cuh, cm_ordinal): each cell's current incarnation, each point's.
+int cm_export(ll_ctx* ctx, ll_cellmap* m, int n_cells, int n_live, void* out, const CmHeld* held = nullptr);
+// An empty map in the state cm_export recorded (records validated by the caller: keys distinct, cell ranks < n_cells; incarnations: the
+// ordinals follow the records and become the epochs).  slot_of_rank (may be NULL): each cell's slot in the new table, host memory.
+int cm_import(ll_ctx* ctx, ll_cellmap* m, int frame_idx, int n_out_of_range, const void* in, int n_cells, int n_live, bool incarnations = false,
+              int* slot_of_rank = nullptr);
 // The n_live live points (the count cm_count gave) in store order, as the map stores them, into the device array dst on the context's stream,
 // by the export's live-point selection; the map is only read.
 int cm_live_points(ll_ctx* ctx, ll_cellmap* m, int n_live, float4* dst);
+
+// ---------------------------------------------------------------------------------------------- byte images (mapper.cu)
+// What the mapper image and the loop image share: a header of magic[8], uint32 version, uint32 config_bytes, uint64 total_bytes and `sections`
+// (offset, length) pairs.  image_structure checks that header (magic, version, the config's size, total_bytes = the image's size) and that every
+// section lies inside the image after the header with no two overlapping; the sections go to sec.  LL_OK or LL_ERR_INVALID and what is wrong.
+struct ImageKind { const char* magic; const char* name; uint32_t version; uint32_t config_bytes; const char* config_name; int sections; };
+int image_structure(const void* image, size_t bytes, const ImageKind& kind, ll_image_section* sec, std::string* err);
+// A history section (int64 n_segments, int64 n_points, int32 size[], ll_point points[]) of L bytes at p: NULL when its counts match the length,
+// the sizes sum to the points and, if `finite`, every point is finite (its parts then in the outputs), else what is wrong.  (The feature
+// histories hold finite points only; the loop closure's full history holds the steps' full clouds as they came, non-finite points included.)
+const char* history_section(const uint8_t* p, uint64_t L, bool finite, int64_t* n_seg, int64_t* n_pts, const uint8_t** sizes, const uint8_t** pts);
+bool finite_xyz(const uint8_t* p);   // the first three floats at p are finite
+int64_t table_capacity(int max_cells);   // the hash-table capacity ll_cellmap_create gives a map of max_cells
+
+// ---------------------------------------------------------------------------------------------- keyframes in the loop image (keyframe.cu)
+int kf_cell_count(const ll_keyframe* kf);
+unsigned kf_accumulate_frames(const ll_keyframe* kf);
+// An open keyframe's cells as the device holds them (ascending key; ids: slot << 32 | epoch), kf_cell_count entries each, to host memory.
+int kf_cell_ids(ll_ctx* ctx, const ll_keyframe* kf, unsigned long long* keys, unsigned long long* ids);
+// A new keyframe as an open one over map m: n cells (keys ascending, ids at m's slots and epochs) and its append count.
+int kf_restore_open(ll_ctx* ctx, ll_cellmap* m, ll_keyframe* kf, const unsigned long long* keys, const unsigned long long* ids, int n, unsigned accumulate_frames);
+// A new keyframe as a closed (analyzed) one with what the search and the alignment read again: its info, its four images (4 x 60 x 60 floats)
+// and its line then plane clouds (host memory).  Its cell list, per-cell types and all-points cloud are not kept: nothing reads them again.
+int kf_restore_closed(ll_ctx* ctx, ll_cellmap* m, ll_keyframe* kf, const ll_keyframe_info& info, const float* img, const void* cloud);
 
 // ---------------------------------------------------------------------------------------------- relocalization (reloc.cu)
 int launch_gather_points(ll_ctx* ctx, cudaStream_t s, const float4* src, const int* idx, int n, float4* dst);   // dst[i] = src[idx[i]]
@@ -349,5 +380,12 @@ size_t loop_step_capacity(const LoopClosure* lc);   // points of the full cloud 
 void loop_select_piece(LoopClosure* lc, int i);
 int  loop_step(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool pushed, int frame_index, const double q_w_curr[4], const double t_w_curr[3]);
 int  loop_read(LoopClosure* lc, ll_loop_event* out, int cap, int* n, int* n_dropped);
+// The loop image (ll_mapper_loop_save / _load / ll_loop_image_info; format: include/loamlivox_b200.h).  stamp: the mapper's binding stamp (the
+// fields of ll_loop_image_scalars before `closed`).  loop_load validates everything on the host first, builds a new loop closure and replaces
+// *lc only when the whole restore succeeded.
+int  loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& stamp, void* image, size_t cap, size_t* bytes);
+int  loop_load(ll_ctx* ctx, LoopClosure** lc, const void* image, size_t bytes, const ll_loop_closure_cfg* cfg, const ll_loop_image_scalars& stamp,
+               const ll_mapper_config& mcfg, int pieces);
+int  loop_image_info(const void* image, size_t bytes, ll_loop_image_summary* info);
 int  loop_result(const LoopClosure* lc, int* n, int* closed, ll_pose* poses_ori, ll_pose* poses_opt, int cap, ll_pg_edge* edge);
 int  loop_cloud(ll_ctx* ctx, const LoopClosure* lc, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev);

@@ -653,3 +653,42 @@ int ll_loop_search(ll_ctx* ctx, const ll_keyframe* const* kfs, int n, int newest
 }
 
 }  // extern "C"
+
+// ---- loop image (ll_mapper_loop_save / ll_mapper_loop_load, loop.cu) ---------------------------------------------------------------------
+int kf_cell_count(const ll_keyframe* kf) { return kf->n_cells; }
+unsigned kf_accumulate_frames(const ll_keyframe* kf) { return kf->accumulate_frames; }
+
+int kf_cell_ids(ll_ctx* ctx, const ll_keyframe* kf, unsigned long long* keys, unsigned long long* ids) {
+  if (kf->n_cells == 0) return LL_OK;
+  LL_CUDA(ctx, cudaMemcpyAsync(keys, kf->keys, (size_t)kf->n_cells * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  LL_CUDA(ctx, cudaMemcpyAsync(ids, kf->ids, (size_t)kf->n_cells * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return LL_OK;
+}
+
+int kf_restore_open(ll_ctx* ctx, ll_cellmap* m, ll_keyframe* kf, const unsigned long long* keys, const unsigned long long* ids, int n, unsigned accumulate_frames) {
+  LL_TRY(kf_reserve_cells(ctx, kf, n));
+  if (n > 0) {
+    LL_CUDA(ctx, cudaMemcpyAsync(kf->keys, keys, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+    LL_CUDA(ctx, cudaMemcpyAsync(kf->ids, ids, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+    LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  }
+  kf->n_cells = n; kf->accumulate_frames = accumulate_frames; kf->analyzed = 0;
+  kf->map = accumulate_frames > 0 ? m : nullptr;   // an append, also of no cell, binds a keyframe to its map
+  kf->generation = m->generation;
+  return LL_OK;
+}
+
+int kf_restore_closed(ll_ctx* ctx, ll_cellmap* m, ll_keyframe* kf, const ll_keyframe_info& info, const float* img, const void* cloud) {
+  kf->map = m; kf->generation = m->generation; kf->n_cells = info.cells; kf->accumulate_frames = (unsigned)info.accumulate_frames;
+  kf->info = info; kf->analyzed = 1; kf->type = nullptr; kf->vec = nullptr; kf->img = nullptr; kf->cloud = nullptr;
+  if (info.cells == 0) return LL_OK;
+  const size_t np = info.line_points + info.plane_points;
+  float* im = nullptr; float4* cl = nullptr;
+  LL_CUDA(ctx, kf->res_buf.carve([&](Carve& c) { im = c.take<float>(4 * KF_PIX); cl = c.take<float4>(np); }));
+  LL_CUDA(ctx, cudaMemcpyAsync(im, img, 4 * KF_PIX * 4, cudaMemcpyHostToDevice, ctx->stream));
+  if (np) LL_CUDA(ctx, cudaMemcpyAsync(cl, cloud, np * 16, cudaMemcpyHostToDevice, ctx->stream));
+  LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  kf->img = im; kf->cloud = cl;
+  return LL_OK;
+}

@@ -4,9 +4,11 @@
 // (transform, VoxelGrid, ll_keyframe_*, ll_loop_search, ll_scene_align, the pose graph, the re-pose) plus one gather kernel.
 #include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <cstring>
 #include "common.cuh"
 #include "kernels.cuh"
+#include "cellmap.cuh"
 
 // grid (chunks, publish x heads): the full slice of head h for piece i goes to segment i after the slices of heads 0 .. h-1
 // (laser_feature_extractor.hpp:353-358 sums the heads' full clouds of a piece in head order).  Block (0, 0) also writes the segment ends.
@@ -84,6 +86,23 @@ const char* loop_cfg_error(const ll_loop_closure_cfg& c) {
   return nullptr;
 }
 
+// The config field by field into zeroed storage: its padding bytes are zero whatever the caller's struct held, so the loop image (which
+// holds the config verbatim) and the comparison of a load's cfg depend on the values only.
+ll_loop_closure_cfg loop_cfg_canonical(const ll_loop_closure_cfg& c) {
+  ll_loop_closure_cfg o; memset(&o, 0, sizeof(o));
+  o.scans_of_each_keyframe = c.scans_of_each_keyframe; o.scans_between_two_keyframe = c.scans_between_two_keyframe;
+  o.loop.minimum_keyframe_differen = c.loop.minimum_keyframe_differen; o.loop.avail_ratio_plane = c.loop.avail_ratio_plane;
+  o.loop.avail_ratio_line = c.loop.avail_ratio_line; o.loop.maximum_roi_difference = c.loop.maximum_roi_difference;
+  o.loop.minimum_similarity_linear = c.loop.minimum_similarity_linear; o.loop.minimum_similarity_planar = c.loop.minimum_similarity_planar;
+  o.loop.plane_with_line = c.loop.plane_with_line;
+  o.map_alignment_resolution = c.map_alignment_resolution; o.map_alignment_maximum_icp_iteration = c.map_alignment_maximum_icp_iteration;
+  o.map_alignment_inlier_threshold = c.map_alignment_inlier_threshold; o.scene_alignment_maximum_residual_block = c.scene_alignment_maximum_residual_block;
+  o.surround_pointcloud_resolution = c.surround_pointcloud_resolution; o.incremental_cov = c.incremental_cov; o.rng_seed = c.rng_seed;
+  o.max_cells = c.max_cells; o.reserve_map_points = c.reserve_map_points; o.reserve_history_points = c.reserve_history_points;
+  o.reserve_keyframes = c.reserve_keyframes;
+  return o;
+}
+
 // A growing device array whose contents survive the growth (DevBuf::reserve does not keep them).
 int grow_keep(ll_ctx* ctx, DevBuf& b, size_t used, size_t need) {
   if (need <= b.cap) return LL_OK;
@@ -107,6 +126,25 @@ void free_keyframes(LoopClosure* lc) {
   for (auto& o : lc->open) ll_keyframe_release(o.kf);
   for (ll_keyframe* k : lc->kfs) ll_keyframe_release(k);
   lc->open.clear(); lc->kfs.clear();
+}
+
+// Mapping_refine::refine_pointcloud (if_save 0) of every keyframe from the accumulated clouds and both pose sets, 256 per launch chain; the
+// readers give the published ones.  The loop's last step, and what ll_mapper_loop_load recomputes (the same code: the same bits).
+int loop_refine(ll_ctx* ctx, LoopClosure* lc) {
+  const int n = (int)lc->kfs.size();
+  const size_t total = lc->acc_end.empty() ? 0 : lc->acc_end[n - 1];
+  RefineLayout rl; LL_CUDA(ctx, lc->refine.carve([&](Carve& k) { rl.layout(k, total); }));
+  lc->ref_end.assign(n, 0);
+  for (int k0 = 0; k0 < n; k0 += 256) {
+    const int nk = std::min(256, n - k0);
+    const size_t b0 = k0 ? lc->acc_end[k0 - 1] : 0;
+    std::vector<int> ends(nk), oend(nk);
+    for (int k = 0; k < nk; k++) ends[k] = (int)(lc->acc_end[k0 + k] - b0);
+    LL_TRY(keyframes_repose_dev(ctx, (const float4*)lc->acc.p + b0, ends[nk - 1], ends.data(), nk, &lc->poses[k0], &lc->opt[k0], 0.2f, rl.mid + b0, rl.out + b0,
+                                rl.end, rl.oend, rl.aff, oend.data()));
+    for (int k = 0; k < nk; k++) lc->ref_end[k0 + k] = (int)b0 + oend[k];   // keyframe k's output: [b0 + oend[k - 1], b0 + oend[k])
+  }
+  return LL_OK;
 }
 
 // The candidates of the newest keyframe (ll_loop_search's, his ascending) through the alignment with the skips of :1048-1052 and
@@ -146,19 +184,7 @@ int loop_align(ll_ctx* ctx, LoopClosure* lc, const std::vector<int>& cand) {
     lc->opt = lc->poses;
     ll_pg_summary sum;
     LL_TRY(ll_pose_graph_optimize(lc->pg, lc->opt.data(), n, edges.data(), (int)edges.size(), 200, &sum));
-    // Mapping_refine::refine_pointcloud (if_save 0) of every keyframe, 256 per launch chain; the readers give the published ones
-    const size_t total = lc->acc_end.empty() ? 0 : lc->acc_end[n - 1];
-    RefineLayout rl; LL_CUDA(ctx, lc->refine.carve([&](Carve& k) { rl.layout(k, total); }));
-    lc->ref_end.assign(n, 0);
-    for (int k0 = 0; k0 < n; k0 += 256) {
-      const int nk = std::min(256, n - k0);
-      const size_t b0 = k0 ? lc->acc_end[k0 - 1] : 0;
-      std::vector<int> ends(nk), oend(nk);
-      for (int k = 0; k < nk; k++) ends[k] = (int)(lc->acc_end[k0 + k] - b0);
-      LL_TRY(keyframes_repose_dev(ctx, (const float4*)lc->acc.p + b0, ends[nk - 1], ends.data(), nk, &lc->poses[k0], &lc->opt[k0], 0.2f, rl.mid + b0, rl.out + b0,
-                                  rl.end, rl.oend, rl.aff, oend.data()));
-      for (int k = 0; k < nk; k++) lc->ref_end[k0 + k] = (int)b0 + oend[k];   // keyframe k's output: [b0 + oend[k - 1], b0 + oend[k])
-    }
+    LL_TRY(loop_refine(ctx, lc));
     ll_loop_event* ce = log_push(lc, LL_LOOP_CLOSED);
     ce->his = his; ce->edge = lc->loop_edge; ce->summary = sum;
     lc->closed = true;
@@ -174,7 +200,7 @@ int loop_set(ll_ctx* ctx, LoopClosure** plc, const ll_loop_closure_cfg* cfg, con
   if (const char* err = loop_cfg_error(*cfg)) { ctx->set_error(std::string("loop closure config: ") + err); return LL_ERR_INVALID; }
   cudaSetDevice(ctx->device);
   LoopClosure* lc = new LoopClosure();
-  lc->cfg = *cfg; lc->cell_res = mcfg.cell_resolution; lc->revisit = mcfg.threshold_cell_revisit; lc->max_history = mcfg.maximum_history_size;
+  lc->cfg = loop_cfg_canonical(*cfg); lc->cell_res = mcfg.cell_resolution; lc->revisit = mcfg.threshold_cell_revisit; lc->max_history = mcfg.maximum_history_size;
   const int st = [&]() -> int {
     const size_t S = (size_t)ctx->cfg.max_scan_points;
     LL_TRY(ll_cellmap_create(ctx, lc->cell_res, lc->revisit, cfg->max_cells, &lc->full));
@@ -364,5 +390,440 @@ int loop_cloud(ll_ctx* ctx, const LoopClosure* lc, int k, ll_point* out_host, si
     LL_CUDA(ctx, cudaMemcpyAsync(out_host, d, std::min(*n_out, cap) * 16, cudaMemcpyDeviceToHost, ctx->stream));
     LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   }
+  return LL_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- loop image
+// Format: include/loamlivox_b200.h ("loop image").  One host validator serves ll_loop_image_info and ll_mapper_loop_load, before anything
+// touches the device; the save writes the sections back to back in index order.
+namespace {
+
+template <typename T> T get(const uint8_t* p) { T v; memcpy(&v, p, sizeof(T)); return v; }
+template <typename T> void put(uint8_t* p, const T& v) { memcpy(p, &v, sizeof(T)); }
+
+const size_t LI_CELLS_HEAD = 24, LI_HIS_HEAD = 16, LI_ACC_HEAD = 8, LI_IMG = 4 * 3600 * 4;   // fixed parts; one keyframe's four images
+const size_t LI_STAMP = offsetof(ll_loop_image_scalars, closed);                                // the binding stamp: the scalars before `closed`
+
+struct LoopCounts { int64_t cells = 0, cell_pts = 0, his_seg = 0, his_pts = 0, open = 0, open_cells = 0, kfs = 0, cloud_pts = 0, acc = 0, acc_pts = 0, events = 0; bool closed = false; };
+
+size_t loop_layout(const LoopCounts& n, ll_loop_image_header* h) {
+  memset(h, 0, sizeof(*h));
+  memcpy(h->magic, LL_LOOP_IMAGE_MAGIC, 8); h->version = LL_LOOP_IMAGE_VERSION; h->config_bytes = sizeof(ll_loop_closure_cfg);
+  const uint64_t K = (uint64_t)n.kfs;
+  const uint64_t len[LL_LOOP_IMAGE_SECTIONS] = {
+      sizeof(ll_loop_closure_cfg), sizeof(ll_loop_image_scalars), LI_CELLS_HEAD + 20 * (uint64_t)(n.cells + n.cell_pts),
+      LI_HIS_HEAD + 4 * (uint64_t)n.his_seg + 16 * (uint64_t)n.his_pts, sizeof(ll_loop_image_open) * (uint64_t)n.open + sizeof(ll_loop_image_ref) * (uint64_t)n.open_cells,
+      sizeof(ll_keyframe_info) * K, sizeof(ll_pose) * K, sizeof(ll_pg_edge) * (K ? K - 1 : 0), LI_IMG * K, 16 * (uint64_t)n.cloud_pts,
+      LI_ACC_HEAD + 8 * (uint64_t)n.acc + 16 * (uint64_t)n.acc_pts, n.closed ? sizeof(ll_pg_edge) + sizeof(ll_pose) * K : 0,
+      sizeof(ll_loop_event) * (uint64_t)n.events};
+  uint64_t off = sizeof(*h);
+  for (int k = 0; k < LL_LOOP_IMAGE_SECTIONS; k++) { h->section[k].offset = off; h->section[k].length = len[k]; off += len[k]; }
+  h->total_bytes = off;
+  return (size_t)off;
+}
+
+struct LoopView {   // a validated loop image
+  ll_loop_image_header h; ll_loop_closure_cfg cfg; ll_loop_image_scalars sc;
+  int32_t frame_idx = 0, n_oor = 0; int64_t n_cells = 0, n_pts = 0; const uint8_t* cells = nullptr; const uint8_t* cur = nullptr;
+  int64_t his_seg = 0, his_pts = 0; const uint8_t* his_sizes = nullptr; const uint8_t* his_pts_p = nullptr;
+  const uint8_t* open = nullptr; const uint8_t* refs = nullptr; int64_t open_cells = 0;
+  const uint8_t *infos = nullptr, *poses = nullptr, *edges = nullptr, *images = nullptr, *clouds = nullptr; int64_t cloud_pts = 0;
+  int64_t n_acc = 0, acc_pts = 0; const uint8_t* acc_end = nullptr; const uint8_t* acc = nullptr;
+  const uint8_t* loop = nullptr; const uint8_t* events = nullptr;
+  int64_t replaced = 0; int32_t max_cur = 0;
+};
+
+bool finite_d(const double* d, int n) { for (int k = 0; k < n; k++) if (!std::isfinite(d[k])) return false; return true; }
+bool finite_pose(const ll_pose& p) { return finite_d(p.q_wxyz, 4) && finite_d(p.t, 3); }
+bool finite_edge(const ll_pg_edge& e) { return finite_d(e.q_wxyz, 4) && finite_d(e.t, 3) && finite_d(e.information, 36); }
+
+// LL_OK, or the code and what is wrong.  load: the image is to be loaded with cfg (NULL: the image's config), so the cell table that cfg's
+// max_cells gives must hold its cells; ll_loop_image_info reports the cell count instead (an image saved by a mapper loaded with a larger
+// max_cells can need one).
+int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_closure_cfg* cfg, LoopView* v, std::string* err) {
+  auto fail = [&](const std::string& msg, int code = LL_ERR_INVALID) { if (err) *err = msg; return code; };
+  static const ImageKind kind{LL_LOOP_IMAGE_MAGIC, "loop", LL_LOOP_IMAGE_VERSION, sizeof(ll_loop_closure_cfg), "ll_loop_closure_cfg", LL_LOOP_IMAGE_SECTIONS};
+  LL_TRY(image_structure(image, bytes, kind, v->h.section, err));
+  const uint8_t* b = (const uint8_t*)image;
+  memcpy(&v->h, b, sizeof(v->h));
+  auto sec = [&](int k) { return b + v->h.section[k].offset; };
+  auto len = [&](int k) { return (uint64_t)v->h.section[k].length; };
+  // config: ll_mapper_set_loop_closure's checks
+  if (len(LL_LOOP_IMAGE_CONFIG) != sizeof(ll_loop_closure_cfg)) return fail("config section length");
+  memcpy(&v->cfg, sec(LL_LOOP_IMAGE_CONFIG), sizeof(v->cfg));
+  if (const char* e = loop_cfg_error(v->cfg)) return fail(std::string("config: ") + e);
+  { const ll_loop_closure_cfg z = loop_cfg_canonical(v->cfg); if (memcmp(&z, &v->cfg, sizeof(z)) != 0) return fail("config padding not zero"); }
+  // scalars
+  if (len(LL_LOOP_IMAGE_SCALARS) != sizeof(ll_loop_image_scalars)) return fail("scalars section length");
+  memcpy(&v->sc, sec(LL_LOOP_IMAGE_SCALARS), sizeof(v->sc));
+  const ll_loop_image_scalars& sc = v->sc;
+  if (!std::isfinite(sc.last_time_stamp) || !finite_d(sc.q_w_curr, 4) || !finite_d(sc.t_w_curr, 3)) return fail("non-finite pose or time stamp");
+  if (sc.frame_index < 0 || (sc.matching_mode != 0 && sc.matching_mode != 1) || sc.threshold_cell_revisit < 1 || !(sc.cell_resolution > 0.f) ||
+      !std::isfinite(sc.cell_resolution) || sc.pieces < 1 || sc.pieces > LL_MAX_PIECES)
+    return fail("binding stamp out of range");
+  if ((sc.closed != 0 && sc.closed != 1) || (sc.stopped != 0 && sc.stopped != 1) || sc.n_keyframes < 0 || sc.n_open < 1 || sc.n_events < 0 ||
+      sc.n_events > LL_LOOP_LOG || sc.n_dropped < 0)
+    return fail("scalars out of range");
+  const int64_t K = sc.n_keyframes;
+  // the full map: keys strictly ascending with bit 63 clear, stamps <= current_frame_idx, ranks < the cell count, ordinals <= their cell's
+  // current one, finite points
+  {
+    const uint8_t* p = sec(LL_LOOP_IMAGE_CELLS); const uint64_t L = len(LL_LOOP_IMAGE_CELLS);
+    if (L < LI_CELLS_HEAD) return fail("cell-map section shorter than its counts");
+    const int32_t fi = get<int32_t>(p), oor = get<int32_t>(p + 4);
+    const int64_t nc = get<int64_t>(p + 8), np = get<int64_t>(p + 16);
+    if (nc < 0 || np < 0 || (uint64_t)nc > (L - LI_CELLS_HEAD) / 20 || (uint64_t)np > (L - LI_CELLS_HEAD) / 20 || LI_CELLS_HEAD + 20 * (uint64_t)(nc + np) != L)
+      return fail("cell-map counts disagree with the section length");
+    if (fi < 0 || oor < 0) return fail("cell-map frame index or out-of-range count negative");
+    const uint8_t* cells = p + LI_CELLS_HEAD; const uint8_t* pts = cells + 16 * nc; const uint8_t* cur = pts + 16 * np; const uint8_t* ord = cur + 4 * nc;
+    uint64_t prev = 0;
+    for (int64_t k = 0; k < nc; k++) {
+      const ll_image_cell e = get<ll_image_cell>(cells + 16 * k);
+      if (e.key >> 63) return fail("cell key with bit 63 set");
+      if (k > 0 && e.key <= prev) return fail("cell keys not strictly ascending");
+      if (e.create_frame < 0 || e.create_frame > fi || e.last_update < 0 || e.last_update > fi) return fail("cell stamp outside 0 ... current_frame_idx");
+      const int32_t c = get<int32_t>(cur + 4 * k);
+      if (c < 0 || c > fi) return fail("incarnation ordinal outside 0 ... current_frame_idx");   // one revisit per cell and append at most
+      v->max_cur = std::max(v->max_cur, c);
+      prev = e.key;
+    }
+    for (int64_t k = 0; k < np; k++) {
+      const ll_image_cell_point q = get<ll_image_cell_point>(pts + 16 * k);
+      if (!(std::isfinite(q.x) && std::isfinite(q.y) && std::isfinite(q.z))) return fail("non-finite cell-map point");
+      if (q.cell < 0 || q.cell >= nc) return fail("cell-map point's cell rank >= the cell count");
+      const int32_t o = get<int32_t>(ord + 4 * k), c = get<int32_t>(cur + 4 * q.cell);
+      if (o < 0 || o > c) return fail("cell-map point's incarnation outside 0 ... its cell's current one");
+      v->replaced += o != c;
+    }
+    v->frame_idx = fi; v->n_oor = oor; v->n_cells = nc; v->n_pts = np; v->cells = cells; v->cur = cur;
+  }
+  // the full history
+  if (const char* e = history_section(sec(LL_LOOP_IMAGE_HISTORY), len(LL_LOOP_IMAGE_HISTORY), false, &v->his_seg, &v->his_pts, &v->his_sizes, &v->his_pts_p)) return fail(e);
+  if (sc.maximum_history_size >= 0 && v->his_seg > sc.maximum_history_size) return fail("more history segments than maximum_history_size");
+  // open keyframes: their cells (cell rank, ordinal) strictly ascending and existing in the map
+  {
+    const uint8_t* p = sec(LL_LOOP_IMAGE_OPEN); const uint64_t L = len(LL_LOOP_IMAGE_OPEN);
+    const uint64_t head = sizeof(ll_loop_image_open) * (uint64_t)sc.n_open;
+    if (head > L) return fail("open-keyframe section shorter than its records");
+    uint64_t refs = 0;
+    for (int k = 0; k < sc.n_open; k++) {
+      const ll_loop_image_open o = get<ll_loop_image_open>(p + sizeof(ll_loop_image_open) * k);
+      if (o.frames < 0 || o.accumulate_frames < 0 || o.n_cells < 0 || (uint64_t)o.n_cells > L / 8) return fail("open keyframe out of range");
+      if (o.accumulate_frames == 0 && o.n_cells > 0) return fail("open keyframe with cells but no append");
+      refs += (uint64_t)o.n_cells;
+    }
+    if (head + sizeof(ll_loop_image_ref) * refs != L) return fail("open-keyframe cells disagree with the section length");
+    const uint8_t* r = p + head;
+    for (int k = 0; k < sc.n_open; k++) {
+      const int64_t n = get<ll_loop_image_open>(p + sizeof(ll_loop_image_open) * k).n_cells;
+      for (int64_t i = 0; i < n; i++, r += 8) {
+        const ll_loop_image_ref x = get<ll_loop_image_ref>(r);
+        if (x.cell < 0 || x.cell >= v->n_cells || x.incarnation < 0 || x.incarnation > get<int32_t>(v->cur + 4 * (int64_t)x.cell))
+          return fail("open keyframe refers to a cell or incarnation the map does not hold");
+        if (i > 0) {
+          const ll_loop_image_ref y = get<ll_loop_image_ref>(r - 8);
+          if (!(y.cell < x.cell || (y.cell == x.cell && y.incarnation < x.incarnation))) return fail("open keyframe's cells not strictly ascending");
+        }
+      }
+    }
+    v->open = p; v->refs = p + head; v->open_cells = (int64_t)refs;
+  }
+  // closed keyframes: infos, poses, the odometry edges between neighbours, images, typed clouds
+  {
+    if (len(LL_LOOP_IMAGE_KEYFRAMES) != sizeof(ll_keyframe_info) * (uint64_t)K || len(LL_LOOP_IMAGE_POSES) != sizeof(ll_pose) * (uint64_t)K ||
+        len(LL_LOOP_IMAGE_EDGES) != sizeof(ll_pg_edge) * (uint64_t)(K ? K - 1 : 0) || len(LL_LOOP_IMAGE_IMAGES) != LI_IMG * (uint64_t)K)
+      return fail("keyframe sections disagree with n_keyframes");
+    v->infos = sec(LL_LOOP_IMAGE_KEYFRAMES); v->poses = sec(LL_LOOP_IMAGE_POSES); v->edges = sec(LL_LOOP_IMAGE_EDGES); v->images = sec(LL_LOOP_IMAGE_IMAGES);
+    uint64_t cloud = 0;
+    for (int64_t k = 0; k < K; k++) {
+      const ll_keyframe_info in = get<ll_keyframe_info>(v->infos + sizeof(ll_keyframe_info) * k);
+      if (in.cells < 0 || in.line_cells < 0 || in.plane_cells < 0 || (int64_t)in.line_cells + in.plane_cells > in.cells || in.accumulate_frames < 0 ||
+          in.all_points > ((size_t)1 << 31) || in.line_points > in.all_points || in.plane_points > in.all_points - in.line_points)
+        return fail("keyframe info out of range");
+      if (in.cells == 0 && in.all_points != 0) return fail("keyframe info out of range");
+      const float f[] = {in.center[0], in.center[1], in.center[2], in.roi_range, in.ratio_nonzero_line, in.ratio_nonzero_plane};
+      for (float x : f) if (!std::isfinite(x)) return fail("non-finite keyframe info");
+      if (!finite_pose(get<ll_pose>(v->poses + sizeof(ll_pose) * k))) return fail("non-finite keyframe pose");
+      if (k > 0) {
+        const ll_pg_edge e = get<ll_pg_edge>(v->edges + sizeof(ll_pg_edge) * (k - 1));
+        if (e.id_begin != k - 1 || e.id_end != k || !finite_edge(e)) return fail("odometry edge out of range");
+      }
+      const uint8_t* im = v->images + LI_IMG * k;
+      for (size_t q = 0; q < LI_IMG / 4; q++) if (!std::isfinite(get<float>(im + 4 * q))) return fail("non-finite keyframe image");
+      cloud += in.line_points + in.plane_points;
+    }
+    if (len(LL_LOOP_IMAGE_CLOUDS) != 16 * cloud) return fail("keyframe clouds disagree with the infos");
+    v->clouds = sec(LL_LOOP_IMAGE_CLOUDS); v->cloud_pts = (int64_t)cloud;
+    for (uint64_t q = 0; q < cloud; q++) if (!finite_xyz(v->clouds + 16 * q)) return fail("non-finite keyframe cloud point");
+  }
+  // accumulated clouds: one per closed keyframe and per open one but the newest
+  {
+    const uint8_t* p = sec(LL_LOOP_IMAGE_ACCUMULATED); const uint64_t L = len(LL_LOOP_IMAGE_ACCUMULATED);
+    if (L < LI_ACC_HEAD) return fail("accumulated section shorter than its count");
+    const int64_t n = get<int64_t>(p);
+    if (n != K + sc.n_open - 1) return fail("accumulated clouds != closed + open keyframes - 1");
+    if ((uint64_t)n > (L - LI_ACC_HEAD) / 8) return fail("accumulated counts disagree with the section length");
+    int64_t prev = 0;
+    for (int64_t k = 0; k < n; k++) {
+      const int64_t e = get<int64_t>(p + LI_ACC_HEAD + 8 * k);
+      if (e < prev) return fail("accumulated cloud ends decreasing");
+      prev = e;
+    }
+    if (prev > INT32_MAX || LI_ACC_HEAD + 8 * (uint64_t)n + 16 * (uint64_t)prev != L) return fail("accumulated counts disagree with the section length");
+    v->n_acc = n; v->acc_pts = prev; v->acc_end = p + LI_ACC_HEAD; v->acc = p + LI_ACC_HEAD + 8 * n;
+    for (int64_t k = 0; k < prev; k++) if (!finite_xyz(v->acc + 16 * k)) return fail("non-finite accumulated point");
+  }
+  // the loop: the edge between two keyframes and the optimized poses, only when closed
+  {
+    const uint64_t L = len(LL_LOOP_IMAGE_LOOP);
+    if (!sc.closed) { if (L != 0) return fail("loop section of an unclosed image not empty"); }
+    else {
+      if (K < 2) return fail("a closed loop needs two keyframes");
+      if (L != sizeof(ll_pg_edge) + sizeof(ll_pose) * (uint64_t)K) return fail("loop section disagrees with n_keyframes");
+      v->loop = sec(LL_LOOP_IMAGE_LOOP);
+      const ll_pg_edge e = get<ll_pg_edge>(v->loop);
+      if (e.id_begin < 0 || e.id_begin >= K || e.id_end < 0 || e.id_end >= K || !finite_edge(e)) return fail("loop edge out of range");
+      for (int64_t k = 0; k < K; k++) if (!finite_pose(get<ll_pose>(v->loop + sizeof(ll_pg_edge) + sizeof(ll_pose) * k))) return fail("non-finite optimized pose");
+    }
+  }
+  // the unread events
+  {
+    if (len(LL_LOOP_IMAGE_EVENTS) != sizeof(ll_loop_event) * (uint64_t)sc.n_events) return fail("events disagree with n_events");
+    v->events = sec(LL_LOOP_IMAGE_EVENTS);
+    for (int k = 0; k < sc.n_events; k++) {
+      const ll_loop_event e = get<ll_loop_event>(v->events + sizeof(ll_loop_event) * k);
+      if (e.kind < LL_LOOP_KEYFRAME || e.kind > LL_LOOP_ERROR) return fail("unknown event kind");
+      if (e.summary.cycles_eval || e.summary.cycles_elim || e.summary.cycles_border || e.summary.cycles_total) return fail("event with timing counters not zero");
+    }
+  }
+  // the caller's config: the image's but for the allocation sizes
+  if (cfg) {
+    ll_loop_closure_cfg x = loop_cfg_canonical(*cfg);
+    x.max_cells = v->cfg.max_cells; x.reserve_map_points = v->cfg.reserve_map_points; x.reserve_history_points = v->cfg.reserve_history_points;
+    x.reserve_keyframes = v->cfg.reserve_keyframes;
+    if (memcmp(&x, &v->cfg, sizeof(x)) != 0) return fail("cfg differs from the image's config in a field other than max_cells and reserve_*");
+    if (const char* e = loop_cfg_error(*cfg)) return fail(std::string("cfg: ") + e);
+  }
+  // ll_cellmap_append does not return from a full table: the import must never make one
+  if (load && v->n_cells > table_capacity(cfg ? cfg->max_cells : v->cfg.max_cells) / 2)
+    return fail("cell table more than half full: load with a larger max_cells", LL_ERR_CAPACITY);
+  if (v->n_pts > ((int64_t)1 << 30) || v->his_pts > INT32_MAX) return fail("more points than a map holds", LL_ERR_CAPACITY);
+  return LL_OK;
+}
+
+// The loop-closure state of a validated image into lc, just made by loop_set (its first open keyframe released) over the mapper it binds to.
+int loop_restore(ll_ctx* ctx, LoopClosure* lc, const LoopView& v) {
+  cudaStream_t s = ctx->stream;
+  const ll_loop_image_scalars& sc = v.sc;
+  const int K = sc.n_keyframes;
+  // the full map, its epochs the image's ordinals
+  std::vector<int> slot(v.n_cells);
+  LL_TRY(cm_import(ctx, lc->full, v.frame_idx, v.n_oor, v.cells, (int)v.n_cells, (int)v.n_pts, true, slot.data()));
+  // the full history, pushed segment by segment from one upload
+  {
+    float4* d = nullptr;
+    if (v.his_pts) {
+      LL_CUDA(ctx, ctx->scratch.carve([&](Carve& k) { d = k.take<float4>((size_t)v.his_pts); }));
+      LL_CUDA(ctx, cudaMemcpyAsync(d, v.his_pts_p, (size_t)v.his_pts * 16, cudaMemcpyHostToDevice, s));
+    }
+    size_t off = 0;
+    for (int64_t k = 0; k < v.his_seg; k++) {
+      const size_t n = (size_t)get<int32_t>(v.his_sizes + 4 * k);
+      LL_TRY(lc->his.push(ctx, d ? d + off : nullptr, n));
+      off += n;
+    }
+    LL_CUDA(ctx, cudaStreamSynchronize(s));   // (the scratch upload may be reallocated by the next carve)
+  }
+  // open keyframes: (cell rank, ordinal) back to (slot, epoch) of the new table
+  const uint8_t* r = v.refs;
+  for (int k = 0; k < sc.n_open; k++) {
+    const ll_loop_image_open o = get<ll_loop_image_open>(v.open + sizeof(ll_loop_image_open) * k);
+    std::vector<unsigned long long> keys(o.n_cells), ids(o.n_cells);
+    for (int64_t i = 0; i < o.n_cells; i++, r += 8) {
+      const ll_loop_image_ref x = get<ll_loop_image_ref>(r);
+      keys[i] = get<ll_image_cell>(v.cells + 16 * (int64_t)x.cell).key;
+      ids[i] = ((unsigned long long)(unsigned)slot[x.cell] << 32) | (unsigned)x.incarnation;
+    }
+    ll_keyframe* kf = nullptr;
+    LL_TRY(ll_keyframe_create(ctx, &kf));
+    lc->open.push_back({kf, o.frames});
+    LL_TRY(kf_restore_open(ctx, lc->full, kf, keys.data(), ids.data(), (int)o.n_cells, (unsigned)o.accumulate_frames));
+  }
+  // closed keyframes, their poses and odometry edges
+  size_t cloud = 0;
+  for (int k = 0; k < K; k++) {
+    const ll_keyframe_info in = get<ll_keyframe_info>(v.infos + sizeof(ll_keyframe_info) * k);
+    ll_keyframe* kf = nullptr;
+    LL_TRY(ll_keyframe_create(ctx, &kf));
+    lc->kfs.push_back(kf);
+    LL_TRY(kf_restore_closed(ctx, lc->full, kf, in, (const float*)(v.images + LI_IMG * k), v.clouds + 16 * cloud));
+    cloud += in.line_points + in.plane_points;
+    lc->poses.push_back(get<ll_pose>(v.poses + sizeof(ll_pose) * k));
+    if (k > 0) lc->edges.push_back(get<ll_pg_edge>(v.edges + sizeof(ll_pg_edge) * (k - 1)));
+  }
+  // accumulated clouds
+  for (int64_t k = 0; k < v.n_acc; k++) lc->acc_end.push_back((size_t)get<int64_t>(v.acc_end + 8 * k));
+  LL_TRY(grow_keep(ctx, lc->acc, 0, (size_t)v.acc_pts * 16 + 64));
+  if (v.acc_pts) LL_CUDA(ctx, cudaMemcpyAsync(lc->acc.p, v.acc, (size_t)v.acc_pts * 16, cudaMemcpyHostToDevice, s));
+  // the loop and its refined clouds, recomputed
+  lc->closed = sc.closed != 0; lc->stopped = sc.stopped != 0;
+  if (lc->closed) {
+    lc->loop_edge = get<ll_pg_edge>(v.loop);
+    lc->opt.resize(K);
+    for (int k = 0; k < K; k++) lc->opt[k] = get<ll_pose>(v.loop + sizeof(ll_pg_edge) + sizeof(ll_pose) * k);
+    LL_TRY(loop_refine(ctx, lc));
+  }
+  // the unread events
+  for (int k = 0; k < sc.n_events; k++) lc->ring[k] = get<ll_loop_event>(v.events + sizeof(ll_loop_event) * k);
+  lc->first = 0; lc->count = (size_t)sc.n_events; lc->dropped = sc.n_dropped;
+  LL_CUDA(ctx, cudaGetLastError());
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  return LL_OK;
+}
+
+}  // namespace
+
+int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& stamp, void* image, size_t cap, size_t* bytes) {
+  cudaStream_t s = ctx->stream;
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  // the incarnations the open keyframes hold (sorted, distinct), on the device for the export
+  std::vector<std::vector<unsigned long long>> okeys(lc->open.size()), oids(lc->open.size());
+  std::vector<unsigned long long> held;
+  LoopCounts n;
+  for (size_t k = 0; k < lc->open.size(); k++) {
+    const int c = kf_cell_count(lc->open[k].kf);
+    okeys[k].resize(c); oids[k].resize(c);
+    LL_TRY(kf_cell_ids(ctx, lc->open[k].kf, okeys[k].data(), oids[k].data()));
+    held.insert(held.end(), oids[k].begin(), oids[k].end());
+    n.open_cells += c;
+  }
+  std::sort(held.begin(), held.end()); held.erase(std::unique(held.begin(), held.end()), held.end());
+  struct Owned { DevBuf b; ~Owned() { b.release(); } } d_held;
+  if (!held.empty()) {
+    LL_CUDA(ctx, d_held.b.reserve(held.size() * 8));
+    LL_CUDA(ctx, cudaMemcpyAsync(d_held.b.p, held.data(), held.size() * 8, cudaMemcpyHostToDevice, s));
+  }
+  const CmHeld H{(const unsigned long long*)d_held.b.p, (int)held.size()};
+  int cells = 0, live = 0, frame_idx = 0, oor = 0, kept = 0;
+  LL_TRY(cm_count(ctx, lc->full, &cells, &live, &frame_idx, &oor));
+  LL_TRY(cm_count_kept(ctx, lc->full, H, &kept));
+  n.cells = cells; n.cell_pts = kept;
+  n.his_seg = (int64_t)lc->his.segs.size(); n.his_pts = (int64_t)lc->his.live();
+  n.open = (int64_t)lc->open.size(); n.kfs = (int64_t)lc->kfs.size();
+  std::vector<ll_keyframe_info> infos(lc->kfs.size());
+  for (size_t k = 0; k < lc->kfs.size(); k++) {
+    if (ll_keyframe_get_info(lc->kfs[k], &infos[k]) != LL_OK) {   // only a keyframe whose analysis failed (LL_LOOP_ERROR) has none
+      ctx->set_error("keyframe " + std::to_string(k) + " was closed by a loop closure that an error stopped and has no analysis: it cannot be saved");
+      return LL_ERR_INVALID;
+    }
+    n.cloud_pts += (int64_t)(infos[k].line_points + infos[k].plane_points);
+  }
+  n.acc = (int64_t)lc->acc_end.size(); n.acc_pts = lc->acc_end.empty() ? 0 : (int64_t)lc->acc_end.back();
+  n.events = (int64_t)lc->count; n.closed = lc->closed;
+  ll_loop_image_header h;
+  const size_t total = loop_layout(n, &h);
+  *bytes = total;
+  if (!image) return LL_OK;
+  if (cap < total) { ctx->set_error("image buffer smaller than the loop image (query the size with image = NULL)"); return LL_ERR_CAPACITY; }
+  uint8_t* b = (uint8_t*)image;
+  auto at = [&](int k) { return b + h.section[k].offset; };
+  memcpy(b, &h, sizeof(h));
+  memcpy(at(LL_LOOP_IMAGE_CONFIG), &lc->cfg, sizeof(lc->cfg));
+  ll_loop_image_scalars sc = stamp;
+  sc.closed = lc->closed ? 1 : 0; sc.stopped = lc->stopped ? 1 : 0;
+  sc.n_keyframes = (int32_t)n.kfs; sc.n_open = (int32_t)n.open; sc.n_events = (int32_t)n.events; sc.n_dropped = lc->dropped;
+  memcpy(at(LL_LOOP_IMAGE_SCALARS), &sc, sizeof(sc));
+  // the full map with the held incarnations
+  uint8_t* p = at(LL_LOOP_IMAGE_CELLS);
+  put<int32_t>(p, frame_idx); put<int32_t>(p + 4, oor); put<int64_t>(p + 8, n.cells); put<int64_t>(p + 16, n.cell_pts);
+  LL_TRY(cm_export(ctx, lc->full, cells, kept, p + LI_CELLS_HEAD, &H));
+  const uint8_t* ecells = p + LI_CELLS_HEAD;
+  // the full history
+  p = at(LL_LOOP_IMAGE_HISTORY);
+  put<int64_t>(p, n.his_seg); put<int64_t>(p + 8, n.his_pts); p += LI_HIS_HEAD;
+  for (const auto& sg : lc->his.segs) { put<int32_t>(p, (int32_t)sg.second); p += 4; }
+  if (n.his_pts) LL_CUDA(ctx, cudaMemcpyAsync(p, lc->his.data(), (size_t)n.his_pts * 16, cudaMemcpyDeviceToHost, s));
+  // open keyframes: (slot, epoch) as (cell rank by key, ordinal)
+  p = at(LL_LOOP_IMAGE_OPEN);
+  uint8_t* refs = p + sizeof(ll_loop_image_open) * lc->open.size();
+  for (size_t k = 0; k < lc->open.size(); k++) {
+    ll_loop_image_open o; memset(&o, 0, sizeof(o));
+    o.frames = lc->open[k].frames; o.accumulate_frames = (int32_t)kf_accumulate_frames(lc->open[k].kf); o.n_cells = (int64_t)okeys[k].size();
+    put(p + sizeof(o) * k, o);
+    for (size_t i = 0; i < okeys[k].size(); i++, refs += 8) {
+      int lo = 0, hi = cells;   // the cell's rank: its key in the exported list
+      while (lo < hi) { const int mid = (lo + hi) >> 1; if (get<ll_image_cell>(ecells + 16 * (size_t)mid).key < okeys[k][i]) lo = mid + 1; else hi = mid; }
+      ll_loop_image_ref x; x.cell = lo;
+      x.incarnation = cm_ordinal(held.data(), (int)held.size(), (int)(oids[k][i] >> 32), (int)(unsigned)(oids[k][i] & 0xffffffffull));
+      put(refs, x);
+    }
+  }
+  // closed keyframes
+  size_t cloud = 0;
+  uint8_t* clouds = at(LL_LOOP_IMAGE_CLOUDS);
+  for (size_t k = 0; k < lc->kfs.size(); k++) {
+    put(at(LL_LOOP_IMAGE_KEYFRAMES) + sizeof(ll_keyframe_info) * k, infos[k]);
+    put(at(LL_LOOP_IMAGE_POSES) + sizeof(ll_pose) * k, lc->poses[k]);
+    if (k > 0) put(at(LL_LOOP_IMAGE_EDGES) + sizeof(ll_pg_edge) * (k - 1), lc->edges[k - 1]);
+    float* im = (float*)(at(LL_LOOP_IMAGE_IMAGES) + LI_IMG * k);
+    LL_TRY(ll_keyframe_images(ctx, lc->kfs[k], im, im + 3600, im + 2 * 3600, im + 3 * 3600));
+    size_t nl = 0, np = 0;
+    LL_TRY(ll_keyframe_cloud(ctx, lc->kfs[k], LL_CELL_LINE, (ll_point*)(clouds + 16 * cloud), infos[k].line_points, &nl, nullptr));
+    LL_TRY(ll_keyframe_cloud(ctx, lc->kfs[k], LL_CELL_PLANE, (ll_point*)(clouds + 16 * (cloud + nl)), infos[k].plane_points, &np, nullptr));
+    cloud += nl + np;
+  }
+  // accumulated clouds
+  p = at(LL_LOOP_IMAGE_ACCUMULATED);
+  put<int64_t>(p, n.acc);
+  for (size_t k = 0; k < lc->acc_end.size(); k++) put<int64_t>(p + LI_ACC_HEAD + 8 * k, (int64_t)lc->acc_end[k]);
+  if (n.acc_pts) LL_CUDA(ctx, cudaMemcpyAsync(p + LI_ACC_HEAD + 8 * n.acc, lc->acc.p, (size_t)n.acc_pts * 16, cudaMemcpyDeviceToHost, s));
+  // the loop
+  if (lc->closed) {
+    p = at(LL_LOOP_IMAGE_LOOP);
+    put(p, lc->loop_edge);
+    memcpy(p + sizeof(ll_pg_edge), lc->opt.data(), sizeof(ll_pose) * lc->opt.size());
+  }
+  // the unread events, oldest first
+  for (size_t k = 0; k < lc->count; k++) {   // the pose graph's SM clock counters time the solve: not state, saved as 0
+    ll_loop_event e = lc->ring[(lc->first + k) % lc->ring.size()];
+    e.summary.cycles_eval = e.summary.cycles_elim = e.summary.cycles_border = e.summary.cycles_total = 0;
+    put(at(LL_LOOP_IMAGE_EVENTS) + sizeof(ll_loop_event) * k, e);
+  }
+  LL_CUDA(ctx, cudaStreamSynchronize(s));
+  return LL_OK;
+}
+
+int loop_load(ll_ctx* ctx, LoopClosure** plc, const void* image, size_t bytes, const ll_loop_closure_cfg* cfg, const ll_loop_image_scalars& stamp,
+              const ll_mapper_config& mcfg, int pieces) {
+  LoopView v; std::string err;
+  const int st = loop_validate(image, bytes, true, cfg, &v, &err);
+  if (st != LL_OK) { ctx->set_error("loop image refused: " + err); return st; }
+  if (memcmp(&v.sc, &stamp, LI_STAMP) != 0) {
+    ctx->set_error("loop image refused: its binding stamp (frame index, pose, time stamp, matching mode, cell_resolution, threshold_cell_revisit, "
+                   "maximum_history_size, pieces) differs from the mapper's");
+    return LL_ERR_INVALID;
+  }
+  cudaSetDevice(ctx->device);
+  LoopClosure* lc = nullptr;
+  LL_TRY(loop_set(ctx, &lc, cfg ? cfg : &v.cfg, mcfg, pieces));
+  free_keyframes(lc);
+  const int rs = loop_restore(ctx, lc, v);
+  if (rs != LL_OK) { loop_release(lc); return rs; }
+  lc->cfg = v.cfg;   // cfg's allocation sizes were read by loop_set only; later images keep the image's config
+  loop_release(*plc);
+  *plc = lc;
+  return LL_OK;
+}
+
+int loop_image_info(const void* image, size_t bytes, ll_loop_image_summary* info) {
+  LoopView v;
+  LL_TRY(loop_validate(image, bytes, false, nullptr, &v, nullptr));
+  memset(info, 0, sizeof(*info));
+  info->bytes = bytes; info->version = v.h.version;
+  info->cells = v.n_cells; info->cell_points = v.n_pts; info->replaced_points = v.replaced;
+  info->history_points = v.his_pts; info->cloud_points = v.cloud_pts; info->accumulated_points = v.acc_pts;
+  info->frame_index = v.sc.frame_index; info->matching_mode = v.sc.matching_mode; info->closed = v.sc.closed; info->stopped = v.sc.stopped;
+  info->keyframes = v.sc.n_keyframes; info->open_keyframes = v.sc.n_open; info->events = v.sc.n_events; info->dropped = v.sc.n_dropped;
+  info->max_incarnation = v.max_cur;
   return LL_OK;
 }

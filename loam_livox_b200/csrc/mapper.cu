@@ -604,35 +604,64 @@ size_t image_layout(const ImageCounts& n, ll_mapper_image_header* h) {
   return (size_t)off;
 }
 
+}  // namespace
+
 bool finite_xyz(const uint8_t* p) { float v[3]; memcpy(v, p, 12); return std::isfinite(v[0]) && std::isfinite(v[1]) && std::isfinite(v[2]); }
-// the hash-table capacity ll_cellmap_create gives a map of max_cells
 int64_t table_capacity(int max_cells) { int64_t cap = 1 << 12; const int64_t want = 2 * (int64_t)(max_cells > 0 ? max_cells : (1 << 20)); while (cap < want) cap <<= 1; return cap; }
+
+int image_structure(const void* image, size_t bytes, const ImageKind& kind, ll_image_section* sec, std::string* err) {
+  auto fail = [&](const std::string& msg) { if (err) *err = msg; return LL_ERR_INVALID; };
+  const uint8_t* b = (const uint8_t*)image;
+  const size_t head = 24 + 16 * (size_t)kind.sections;
+  if (!b || bytes < head) return fail("shorter than the image header");
+  char magic[8]; uint32_t version, config_bytes; uint64_t total;
+  memcpy(magic, b, 8); memcpy(&version, b + 8, 4); memcpy(&config_bytes, b + 12, 4); memcpy(&total, b + 16, 8);
+  memcpy(sec, b + 24, 16 * (size_t)kind.sections);
+  if (memcmp(magic, kind.magic, 8) != 0) return fail(std::string("not a ") + kind.name + " image (magic)");
+  if (version != kind.version) return fail("unknown image version");
+  if (config_bytes != kind.config_bytes) return fail(std::string("config size differs from this library's ") + kind.config_name);
+  if (total != bytes) return fail("image size differs from the header's total_bytes");
+  // every section inside the image after the header, no two overlapping
+  std::vector<int> order(kind.sections);
+  for (int k = 0; k < kind.sections; k++) {
+    const ll_image_section& s = sec[k];
+    if (s.offset < head || s.offset > bytes || s.length > bytes - s.offset) return fail("section outside the image");
+    order[k] = k;
+  }
+  std::sort(order.begin(), order.end(), [&](int a, int c) {
+    const ll_image_section &x = sec[a], &y = sec[c];
+    return x.offset != y.offset ? x.offset < y.offset : x.length < y.length;
+  });
+  for (int k = 1; k < kind.sections; k++) {
+    const ll_image_section &p = sec[order[k - 1]], &q = sec[order[k]];
+    if (p.offset + p.length > q.offset) return fail("overlapping sections");
+  }
+  return LL_OK;
+}
+
+const char* history_section(const uint8_t* p, uint64_t L, bool finite, int64_t* n_seg, int64_t* n_pts, const uint8_t** sizes, const uint8_t** pts) {
+  if (L < HIS_HEAD) return "history section shorter than its counts";
+  const int64_t ns = rd<int64_t>(p), np = rd<int64_t>(p + 8);
+  if (ns < 0 || np < 0 || (uint64_t)ns > (L - HIS_HEAD) / 4 || (uint64_t)np > (L - HIS_HEAD) / 16 || HIS_HEAD + 4 * (uint64_t)ns + 16 * (uint64_t)np != L)
+    return "history counts disagree with the section length";
+  int64_t sum = 0;
+  for (int64_t k = 0; k < ns; k++) { const int32_t z = rd<int32_t>(p + HIS_HEAD + 4 * k); if (z < 0) return "negative history segment size"; sum += z; }
+  if (sum != np) return "history segment sizes do not sum to its points";
+  const uint8_t* q = p + HIS_HEAD + 4 * ns;
+  if (finite) for (int64_t k = 0; k < np; k++) if (!finite_xyz(q + 16 * k)) return "non-finite history point";
+  *n_seg = ns; *n_pts = np; *sizes = p + HIS_HEAD; *pts = q;
+  return nullptr;
+}
+
+namespace {
 
 // LL_OK, or the code and what is wrong.  cfg: the caller's config for a load (NULL: the image's).
 int image_validate(const void* image, size_t bytes, const ll_mapper_config* cfg, ImageView* v, std::string* err) {
   auto fail = [&](const char* msg, int code = LL_ERR_INVALID) { if (err) *err = msg; return code; };
   const uint8_t* b = (const uint8_t*)image;
-  if (!b || bytes < sizeof(ll_mapper_image_header)) return fail("shorter than the image header");
+  static const ImageKind kind{LL_MAPPER_IMAGE_MAGIC, "mapper", LL_MAPPER_IMAGE_VERSION, sizeof(ll_mapper_config), "ll_mapper_config", LL_IMAGE_SECTIONS};
+  LL_TRY(image_structure(image, bytes, kind, v->h.section, err));
   memcpy(&v->h, b, sizeof(v->h));
-  if (memcmp(v->h.magic, LL_MAPPER_IMAGE_MAGIC, 8) != 0) return fail("not a mapper image (magic)");
-  if (v->h.version != LL_MAPPER_IMAGE_VERSION) return fail("unknown image version");
-  if (v->h.config_bytes != sizeof(ll_mapper_config)) return fail("config size differs from this library's ll_mapper_config");
-  if (v->h.total_bytes != bytes) return fail("image size differs from the header's total_bytes");
-  // structure: every section inside the image after the header, no two overlapping
-  int order[LL_IMAGE_SECTIONS];
-  for (int k = 0; k < LL_IMAGE_SECTIONS; k++) {
-    const ll_image_section& s = v->h.section[k];
-    if (s.offset < sizeof(ll_mapper_image_header) || s.offset > bytes || s.length > bytes - s.offset) return fail("section outside the image");
-    order[k] = k;
-  }
-  std::sort(order, order + LL_IMAGE_SECTIONS, [&](int a, int c) {
-    const ll_image_section &x = v->h.section[a], &y = v->h.section[c];
-    return x.offset != y.offset ? x.offset < y.offset : x.length < y.length;
-  });
-  for (int k = 1; k < LL_IMAGE_SECTIONS; k++) {
-    const ll_image_section &p = v->h.section[order[k - 1]], &q = v->h.section[order[k]];
-    if (p.offset + p.length > q.offset) return fail("overlapping sections");
-  }
   auto sec = [&](int k) { return b + v->h.section[k].offset; };
   auto len = [&](int k) { return (uint64_t)v->h.section[k].length; };
   // config: ll_mapper_create's checks and a matching mode the mapper knows
@@ -656,19 +685,8 @@ int image_validate(const void* image, size_t bytes, const ll_mapper_config* cfg,
   if (sc.have_map && (sc.snap_n[0] == 0 || sc.snap_n[1] == 0)) return fail("have_map with an empty snapshot");
   for (int c = 0; c < 2; c++) {
     // history window: counts x element sizes = the length, segment sizes summing to the points, finite points
-    {
-      const uint8_t* p = sec(LL_IMAGE_HISTORY_CORNER + c); const uint64_t L = len(LL_IMAGE_HISTORY_CORNER + c);
-      if (L < HIS_HEAD) return fail("history section shorter than its counts");
-      const int64_t ns = rd<int64_t>(p), np = rd<int64_t>(p + 8);
-      if (ns < 0 || np < 0 || (uint64_t)ns > (L - HIS_HEAD) / 4 || (uint64_t)np > (L - HIS_HEAD) / 16 || HIS_HEAD + 4 * (uint64_t)ns + 16 * (uint64_t)np != L)
-        return fail("history counts disagree with the section length");
-      int64_t sum = 0;
-      for (int64_t k = 0; k < ns; k++) { const int32_t z = rd<int32_t>(p + HIS_HEAD + 4 * k); if (z < 0) return fail("negative history segment size"); sum += z; }
-      if (sum != np) return fail("history segment sizes do not sum to its points");
-      const uint8_t* pts = p + HIS_HEAD + 4 * ns;
-      for (int64_t k = 0; k < np; k++) if (!finite_xyz(pts + 16 * k)) return fail("non-finite history point");
-      v->his[c].n_seg = ns; v->his[c].n_pts = np; v->his[c].sizes = p + HIS_HEAD; v->his[c].pts = pts;
-    }
+    if (const char* e = history_section(sec(LL_IMAGE_HISTORY_CORNER + c), len(LL_IMAGE_HISTORY_CORNER + c), true, &v->his[c].n_seg, &v->his[c].n_pts, &v->his[c].sizes, &v->his[c].pts))
+      return fail(e);
     // snapshot: as many points as snap_n when the index exists, none otherwise
     {
       const uint8_t* p = sec(LL_IMAGE_SNAPSHOT_CORNER + c); const uint64_t L = len(LL_IMAGE_SNAPSHOT_CORNER + c);
@@ -1212,6 +1230,34 @@ int ll_mapper_loop_result(ll_mapper* m, int* n, int* closed, ll_pose* poses_ori,
 int ll_mapper_loop_cloud(ll_mapper* m, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev) {
   if (!m || !n_out) return LL_ERR_INVALID;
   return loop_cloud(m->ctx, m->lc, k, out_host, cap, n_out, out_dev);
+}
+
+// The loop image's binding stamp: what the loop closure's state refers to in the mapper (loop.cu checks it on load).
+static ll_loop_image_scalars loop_stamp(const ll_mapper* m) {
+  ll_loop_image_scalars s; memset(&s, 0, sizeof(s));
+  s.frame_index = m->frame_index; s.matching_mode = m->cfg.matching_mode; s.threshold_cell_revisit = m->cfg.threshold_cell_revisit;
+  s.maximum_history_size = m->cfg.maximum_history_size; s.pieces = m->frame_pieces; s.cell_resolution = m->cfg.cell_resolution;
+  s.last_time_stamp = m->last_time_stamp;
+  for (int k = 0; k < 4; k++) s.q_w_curr[k] = m->q_w_curr[k];
+  for (int k = 0; k < 3; k++) s.t_w_curr[k] = m->t_w_curr[k];
+  return s;
+}
+
+int ll_mapper_loop_save(ll_mapper* m, void* image, size_t cap, size_t* bytes) {
+  if (!m || !bytes) return LL_ERR_INVALID;
+  if (!m->lc) { m->ctx->set_error("loop closure is off: there is no loop image"); return LL_ERR_INVALID; }
+  cudaSetDevice(m->ctx->device);
+  return loop_save(m->ctx, m->lc, loop_stamp(m), image, cap, bytes);
+}
+
+int ll_mapper_loop_load(ll_mapper* m, const void* image, size_t bytes, const ll_loop_closure_cfg* cfg) {
+  if (!m) return LL_ERR_INVALID;
+  return loop_load(m->ctx, &m->lc, image, bytes, cfg, loop_stamp(m), m->cfg, m->frame_pieces);
+}
+
+int ll_loop_image_info(const void* image, size_t bytes, ll_loop_image_summary* info) {
+  if (!info) return LL_ERR_INVALID;
+  return loop_image_info(image, bytes, info);
 }
 
 }  // extern "C"

@@ -1105,6 +1105,32 @@ class Laser_mapping:
             self.ctx.check(self.ctx._lib.ll_mapper_loop_cloud(self.h, int(k), out.ctypes.data, n.value, C.byref(n), None))
         return out
 
+    def save_loop(self) -> bytes:
+        """The loop closure as a loop image of its own (ll_mapper_loop_save; format in include/loamlivox_b200.h).  Save it with save() at the
+        same step; load() of the mapper image then load_loop() of this one continue bit for bit as this mapper does.  Raises when loop closure
+        is off.  The mapper is not modified (its event log is not drained)."""
+        n = C.c_size_t()
+        self.ctx.check(self.ctx._lib.ll_mapper_loop_save(self.h, None, 0, C.byref(n)))
+        buf = bytearray(n.value)
+        self.ctx.check(self.ctx._lib.ll_mapper_loop_save(self.h, (C.c_char * len(buf)).from_buffer(buf), len(buf), C.byref(n)))
+        return bytes(buf)
+
+    def load_loop(self, image, **alloc):
+        """Restore loop closure from a loop image onto this mapper (ll_mapper_loop_load), replacing any it has.  alloc may set max_cells,
+        reserve_map_points, reserve_history_points and reserve_keyframes, which size the allocations; everything else is the image's config.
+        A refused image raises and changes nothing."""
+        img = np.frombuffer(image, np.uint8)
+        cfg = None
+        if alloc:
+            loop_image_info(image)   # validated before its config is read
+            off = int(np.frombuffer(image, np.uint64, count=1, offset=24 + 16 * capi.LL_LOOP_IMAGE_CONFIG)[0])
+            cfg = capi.LoopClosureCfg.from_buffer_copy(bytes(image[off:off + C.sizeof(capi.LoopClosureCfg)]))
+            for k, v in alloc.items():
+                if k not in ("max_cells", "reserve_map_points", "reserve_history_points", "reserve_keyframes"):
+                    raise AttributeError(f"{k}: only the allocation sizes can differ from the image's config")
+                setattr(cfg, k, v)
+        self.ctx.check(self.ctx._lib.ll_mapper_loop_load(self.h, img.ctypes.data, img.shape[0], C.byref(cfg) if cfg is not None else None))
+
     def recovery_last_inputs(self):
         """What the last relocalization attempt passed to the search (ll_mapper_recovery_last_inputs): {"corner", "surf", "score_corner",
         "score_surf": float32 [n, 4]; "rot_coarse", "rot_fine": [n, 4]; "coarse": RelocCfg; "fine": RelocFineCfg; "tmpl": RegState}; the cfgs point
@@ -1172,6 +1198,16 @@ def image_info(image) -> dict:
     if st != capi.LL_OK:
         raise LoamLivoxError(f"status {st}: mapper image refused")
     return {n: (list(getattr(info, n)) if isinstance(getattr(info, n), C.Array) else getattr(info, n)) for n, _ in capi.ImageInfo._fields_ if n != "reserved"}
+
+
+def loop_image_info(image) -> dict:
+    """Validate a loop image completely on the host (no context, no GPU) and report what is in it (ll_loop_image_info)."""
+    img = np.frombuffer(image, np.uint8) if len(image) else np.zeros(1, np.uint8)
+    info = capi.LoopImageSummary()
+    st = capi.lib().ll_loop_image_info(img.ctypes.data, len(image), C.byref(info))
+    if st != capi.LL_OK:
+        raise LoamLivoxError(f"status {st}: loop image refused")
+    return {n: getattr(info, n) for n, _ in capi.LoopImageSummary._fields_}
 
 
 class Laser_feature:
