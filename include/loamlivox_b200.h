@@ -763,8 +763,9 @@ int  ll_loop_search(ll_ctx* ctx, const ll_keyframe* const* kfs, int n, int newes
  *           += 5` between the threshold and twice it, a loop below it), then ll_pose_graph_loop_edge, ll_pose_graph_optimize and the refined
  *           clouds of the published keyframes (pc_idx = n - 1, n - 3, ...; VoxelGrid 0.2, :903, and the affine of ll_keyframes_repose).
  * maximum_keyframe_in_waiting_list is not a setting: a closed keyframe is processed in the step that closes it, so the waiting list never holds
- * more than one and its pop (:1554-1557) cannot fire.  After the first loop the reference searches no more (if_end, :990-993): the mapper then
- * stops all loop-closure work.  Loop closure never changes the odometry: an error of its work other than LL_ERR_CUDA does not fail the step.
+ * more than one and its pop (:1554-1557) cannot fire.  After the first loop the reference searches no more (if_end, :990-993): by default the
+ * mapper then stops all loop-closure work; ll_mapper_set_loop_policy below lets it close further loops.  Loop closure never changes the
+ * odometry: an error of its work other than LL_ERR_CUDA does not fail the step.
  * A failed alignment ends that keyframe's search (LL_LOOP_FAILED); any other error is logged (LL_LOOP_ERROR) and stops loop closure for good.
  * LL_ERR_CUDA is returned.  It is not part of a mapper image (a loaded mapper has it off): its state has an image of its own, the loop image
  * (ll_mapper_loop_save / ll_mapper_loop_load below). */
@@ -816,13 +817,31 @@ typedef struct {
 #define LL_LOOP_LOG 1024
 /* Drains up to cap events, oldest first, from a ring of LL_LOOP_LOG (entries past cap stay); *n_dropped = events overwritten unread. */
 int  ll_mapper_loop_read(ll_mapper* mapper, ll_loop_event* out, int cap, int* n, int* n_dropped);
-/* The processed keyframes (*n, may be 0) and whether the loop is closed.  poses_ori: their poses (pose3d_map_ori); poses_opt: after the
- * optimization (temp_pose_3d_map; the poses_ori values before the loop closes); edge: the loop edge (zeros before).  Arrays hold cap
- * keyframes (LL_ERR_CAPACITY, nothing written, when short); any may be NULL. */
+/* The processed keyframes (*n, may be 0) and whether a loop is closed.  poses_ori: their poses (pose3d_map_ori); poses_opt: after the latest
+ * optimization (temp_pose_3d_map) for the keyframes it covered (n_opt = the newest id of the latest loop edge + 1), the poses_ori values for
+ * the others (all of them before a loop closes); edge: the latest loop edge (zeros before).  Arrays hold cap keyframes (LL_ERR_CAPACITY,
+ * nothing written, when short); any may be NULL. */
 int  ll_mapper_loop_result(ll_mapper* mapper, int* n, int* closed, ll_pose* poses_ori, ll_pose* poses_opt, int cap, ll_pg_edge* edge);
-/* The refined cloud of published keyframe k (after the loop closed; k = n - 1, n - 3, ..., else LL_ERR_INVALID), as ll_keyframe_cloud offers
- * its clouds: on the device (*out_dev, valid until loop closure is set again) and copied to out_host (cap points) when that is not NULL. */
+/* The refined cloud of published keyframe k of the latest optimization (after a loop closed; k = n_opt - 1, n_opt - 3, ..., else
+ * LL_ERR_INVALID), as ll_keyframe_cloud offers its clouds: on the device (*out_dev, valid until the next loop closes or loop closure is set
+ * again) and copied to out_host (cap points) when that is not NULL. */
 int  ll_mapper_loop_cloud(ll_mapper* mapper, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev);
+/* Loops after the first.  The reference stops after its first loop (if_end, :990-993), and so does the default policy {1, 0}.  With
+ * max_loops = M > 1, loop closure goes on after a loop as before it (capture, history, full map, keyframes), with the same candidate walk, and
+ * stops all work after the M-th loop.  A keyframe closed while newest - L < min_keyframes_between_loops (L: the newest keyframe of the last
+ * loop) is analyzed and recorded but not searched (its LL_LOOP_KEYFRAME event has n_candidates 0).  Each loop adds its edge
+ * (ll_pose_graph_loop_edge) to the loop edges so far; the graph of every odometry edge and every loop edge is solved from poses_ori, and every
+ * keyframe up to the closing one is re-posed.  Accumulating loop edges goes beyond the reference, which solves one loop with only its edge.
+ * M <= LL_MAX_LOOPS keeps every solve within LL_PG_MAX_BORDER; the graph of reserve_keyframes poses and reserve_keyframes - 1 + M edges is
+ * allocated when the policy is set. */
+#define LL_MAX_LOOPS (LL_PG_MAX_BORDER / 2)   /* 32: each loop edge adds at most two border poses */
+typedef struct { int32_t max_loops, min_keyframes_between_loops; } ll_loop_policy;   /* 8 B */
+void ll_mapper_loop_policy_default(ll_loop_policy* p);            /* {1, 0}: the reference (first loop, then stop) */
+/* p NULL: the default.  LL_ERR_INVALID, nothing changed: loop closure off, a loop already closed, max_loops outside 1 ... LL_MAX_LOOPS, or
+ * min_keyframes_between_loops < 0.  ll_mapper_set_loop_closure and ll_mapper_loop_load of a version-1 image reset the policy to the default. */
+int  ll_mapper_set_loop_policy(ll_mapper* mapper, const ll_loop_policy* p);
+/* Every loop edge so far, in closing order (*n_loops of them; edges may be NULL to query).  cap < *n_loops: LL_ERR_CAPACITY, nothing written. */
+int  ll_mapper_loop_edges(ll_mapper* mapper, ll_pg_edge* edges, int cap, int* n_loops);
 
 /* ---- loop image: the mapper's loop closure as a byte image of its own (DESIGN.md §4.6.1) ------------------------------------------------
  * Checkpoint a run with loop closure on: save the mapper image and the loop image at the same step, then ll_mapper_load the one and
@@ -830,7 +849,7 @@ int  ll_mapper_loop_cloud(ll_mapper* mapper, int k, ll_point* out_host, size_t c
  * except gpu_ms_*, every integer stat, every loop event (but ll_pg_summary::cycles_*, which time the solve and are saved as 0),
  * ll_mapper_loop_result and every ll_mapper_loop_cloud.  The mapper image is unchanged by loop closure (same bytes with it on or off).
  *
- * Format (version 1), one little-endian byte string, with the mapper image's conventions (header of (offset, length) sections, placed back to
+ * Format (version 1; version 2 differs in LL_LOOP_IMAGE_LOOP only), one little-endian byte string, with the mapper image's conventions (header of (offset, length) sections, placed back to
  * back in index order by a writer, canonical contents):
  *   ll_loop_image_header          magic "LLLOOPIM", version, config_bytes = sizeof(ll_loop_closure_cfg), total_bytes, the sections
  *   LL_LOOP_IMAGE_CONFIG          the ll_loop_closure_cfg in force, verbatim with its padding bytes zero
@@ -852,6 +871,10 @@ int  ll_mapper_loop_cloud(ll_mapper* mapper, int k, ll_point* out_host, size_t c
  *   LL_LOOP_IMAGE_CLOUDS          each closed keyframe's line then plane cloud (info.line_points + info.plane_points ll_point), in order
  *   LL_LOOP_IMAGE_ACCUMULATED     int64 n_acc (= n_keyframes + n_open - 1), int64 end[n_acc] (non-decreasing), ll_point points[end[n_acc - 1]]
  *   LL_LOOP_IMAGE_LOOP            closed = 1: ll_pg_edge loop_edge, ll_pose poses_opt[n_keyframes]; closed = 0: empty
+ *                                 Version 2 (written under a policy other than the default, which writes version 1): always present,
+ *                                 ll_loop_policy policy (max_loops >= 2), int32 n_loops (<= max_loops), int32 0, ll_pg_edge edges[n_loops]
+ *                                 (closing order; their newest ids increase by at least min_keyframes_between_loops), ll_pose poses_opt[n_opt]
+ *                                 (n_opt = the newest id of the last edge + 1, 0 without loops); closed = (n_loops > 0)
  *   LL_LOOP_IMAGE_EVENTS          the unread events, oldest first: ll_loop_event events[n_events] (n_events <= LL_LOOP_LOG), their
  *                                 summary.cycles_* (SM clock counters that time the solve, not state) 0
  * The refined clouds are not saved: ll_mapper_loop_load recomputes them from the accumulated clouds and both pose sets by the code the loop
@@ -864,6 +887,7 @@ int  ll_mapper_loop_cloud(ll_mapper* mapper, int k, ll_point* out_host, size_t c
  * guard, not a proof that both images come from the same run and step. */
 #define LL_LOOP_IMAGE_MAGIC "LLLOOPIM"
 #define LL_LOOP_IMAGE_VERSION 1
+#define LL_LOOP_IMAGE_VERSION_POLICY 2   /* the version a loop closure under a policy other than the default writes (LL_LOOP_IMAGE_LOOP above) */
 enum { LL_LOOP_IMAGE_CONFIG = 0, LL_LOOP_IMAGE_SCALARS = 1, LL_LOOP_IMAGE_CELLS = 2, LL_LOOP_IMAGE_HISTORY = 3, LL_LOOP_IMAGE_OPEN = 4,
        LL_LOOP_IMAGE_KEYFRAMES = 5, LL_LOOP_IMAGE_POSES = 6, LL_LOOP_IMAGE_EDGES = 7, LL_LOOP_IMAGE_IMAGES = 8, LL_LOOP_IMAGE_CLOUDS = 9,
        LL_LOOP_IMAGE_ACCUMULATED = 10, LL_LOOP_IMAGE_LOOP = 11, LL_LOOP_IMAGE_EVENTS = 12, LL_LOOP_IMAGE_SECTIONS = 13 };

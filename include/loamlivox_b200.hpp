@@ -343,7 +343,19 @@ class Laser_mapping {
     if (dropped) *dropped = total;
     return out;
   }
-  // the keyframe poses before (pose3d_map_ori) and after the optimization (temp_pose_3d_map), the loop edge; returns whether the loop is closed
+  // loops after the first (ll_mapper_set_loop_policy): p NULL the default (the reference's first loop, then stop); set after set_loop_closure
+  // and before the first loop, else it throws and changes nothing
+  void set_loop_policy(const ll_loop_policy* p) { ctx_.check(ll_mapper_set_loop_policy(mapper_, p)); }
+  // every loop edge so far, in closing order (ll_mapper_loop_edges)
+  std::vector<ll_pg_edge> loop_edges() {
+    int n = 0;
+    ctx_.check(ll_mapper_loop_edges(mapper_, nullptr, 0, &n));
+    std::vector<ll_pg_edge> out(n);
+    ctx_.check(ll_mapper_loop_edges(mapper_, out.data(), n, &n));
+    return out;
+  }
+  // the keyframe poses before (pose3d_map_ori) and after the latest optimization (temp_pose_3d_map; pose3d_map_ori past the keyframes it
+  // covered), the latest loop edge; returns whether a loop is closed
   bool loop_result(std::vector<ll_pose>* poses_ori, std::vector<ll_pose>* poses_opt, ll_pg_edge* edge = nullptr) {
     int n = 0, closed = 0;
     ctx_.check(ll_mapper_loop_result(mapper_, &n, &closed, nullptr, nullptr, 0, nullptr));

@@ -25,11 +25,12 @@ LL_RECOVERY_LOG = 1024
 LL_TRACKING, LL_SUSPECT, LL_LOST = 0, 1, 2
 LL_BAD_NONE, LL_BAD_REJECTED, LL_BAD_INLIER = 0, 1, 2
 LL_PG_MAX_BORDER = 64
+LL_MAX_LOOPS = LL_PG_MAX_BORDER // 2
 LL_LOOP_LOG = 1024
 LL_LOOP_KEYFRAME, LL_LOOP_ALIGNMENT, LL_LOOP_CLOSED, LL_LOOP_ERROR = 0, 1, 2, 3
 LL_LOOP_SKIP10, LL_LOOP_SKIP5, LL_LOOP_ACCEPT, LL_LOOP_FAILED = 0, 1, 2, 3
 LL_MAPPER_IMAGE_MAGIC, LL_MAPPER_IMAGE_VERSION = b"LLMAPIMG", 1
-LL_LOOP_IMAGE_MAGIC, LL_LOOP_IMAGE_VERSION = b"LLLOOPIM", 1
+LL_LOOP_IMAGE_MAGIC, LL_LOOP_IMAGE_VERSION, LL_LOOP_IMAGE_VERSION_POLICY = b"LLLOOPIM", 1, 2
 (LL_LOOP_IMAGE_CONFIG, LL_LOOP_IMAGE_SCALARS, LL_LOOP_IMAGE_CELLS, LL_LOOP_IMAGE_HISTORY, LL_LOOP_IMAGE_OPEN, LL_LOOP_IMAGE_KEYFRAMES, LL_LOOP_IMAGE_POSES,
  LL_LOOP_IMAGE_EDGES, LL_LOOP_IMAGE_IMAGES, LL_LOOP_IMAGE_CLOUDS, LL_LOOP_IMAGE_ACCUMULATED, LL_LOOP_IMAGE_LOOP, LL_LOOP_IMAGE_EVENTS, LL_LOOP_IMAGE_SECTIONS) = range(14)
 (LL_IMAGE_CONFIG, LL_IMAGE_SCALARS, LL_IMAGE_HISTORY_CORNER, LL_IMAGE_HISTORY_SURF, LL_IMAGE_SNAPSHOT_CORNER, LL_IMAGE_SNAPSHOT_SURF, LL_IMAGE_CELLS_CORNER,
@@ -55,6 +56,7 @@ EXPORTS = [
     "ll_spin_cfg_default", "ll_spin_create", "ll_spin_release", "ll_spin_extract", "ll_spin_cloud", "ll_spin_point_info", "ll_spin_chains",
     "ll_mapper_process_sweep", "ll_mapper_process_sweeps",
     "ll_mapper_loop_save", "ll_mapper_loop_load", "ll_loop_image_info",
+    "ll_mapper_loop_policy_default", "ll_mapper_set_loop_policy", "ll_mapper_loop_edges",
 ]
 LL_SPIN_FULL, LL_SPIN_SHARP, LL_SPIN_LESS_SHARP, LL_SPIN_FLAT, LL_SPIN_LESS_FLAT = 0, 1, 2, 3, 4
 LL_CELL_SPHERE, LL_CELL_LINE, LL_CELL_PLANE, LL_CELL_ALL = 0, 1, 2, -1
@@ -205,6 +207,11 @@ class LoopClosureCfg(C.Structure):
                 ("scene_alignment_maximum_residual_block", C.c_int), ("surround_pointcloud_resolution", C.c_double), ("incremental_cov", C.c_int),
                 ("rng_seed", C.c_int), ("max_cells", C.c_int), ("reserve_map_points", C.c_longlong), ("reserve_history_points", C.c_longlong),
                 ("reserve_keyframes", C.c_int)]
+
+
+class LoopPolicy(C.Structure):
+    """ll_loop_policy: how many loops the streaming mapper closes, and the keyframes between the newest keyframes of two loops."""
+    _fields_ = [("max_loops", C.c_int32), ("min_keyframes_between_loops", C.c_int32)]
 
 
 class LoopEvent(C.Structure):
@@ -369,6 +376,9 @@ def lib():
     L.ll_mapper_loop_save.argtypes = [vp, vp, sz, C.POINTER(sz)]
     L.ll_mapper_loop_load.argtypes = [vp, vp, sz, C.POINTER(LoopClosureCfg)]
     L.ll_loop_image_info.argtypes = [vp, sz, C.POINTER(LoopImageSummary)]
+    L.ll_mapper_loop_policy_default.argtypes = [C.POINTER(LoopPolicy)]
+    L.ll_mapper_set_loop_policy.argtypes = [vp, C.POINTER(LoopPolicy)]
+    L.ll_mapper_loop_edges.argtypes = [vp, vp, ci, C.POINTER(ci)]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64
     _LIB = L

@@ -253,9 +253,10 @@ int cm_live_points(ll_ctx* ctx, ll_cellmap* m, int n_live, float4* dst);
 
 // ---------------------------------------------------------------------------------------------- byte images (mapper.cu)
 // What the mapper image and the loop image share: a header of magic[8], uint32 version, uint32 config_bytes, uint64 total_bytes and `sections`
-// (offset, length) pairs.  image_structure checks that header (magic, version, the config's size, total_bytes = the image's size) and that every
-// section lies inside the image after the header with no two overlapping; the sections go to sec.  LL_OK or LL_ERR_INVALID and what is wrong.
-struct ImageKind { const char* magic; const char* name; uint32_t version; uint32_t config_bytes; const char* config_name; int sections; };
+// (offset, length) pairs.  image_structure checks that header (magic, a version in version ... max_version, the config's size, total_bytes = the
+// image's size) and that every section lies inside the image after the header with no two overlapping; the sections go to sec.  LL_OK or
+// LL_ERR_INVALID and what is wrong.
+struct ImageKind { const char* magic; const char* name; uint32_t version, max_version; uint32_t config_bytes; const char* config_name; int sections; };
 int image_structure(const void* image, size_t bytes, const ImageKind& kind, ll_image_section* sec, std::string* err);
 // A history section (int64 n_segments, int64 n_points, int32 size[], ll_point points[]) of L bytes at p: NULL when its counts match the length,
 // the sizes sum to the points and, if `finite`, every point is finite (its parts then in the outputs), else what is wrong.  (The feature
@@ -389,3 +390,6 @@ int  loop_load(ll_ctx* ctx, LoopClosure** lc, const void* image, size_t bytes, c
 int  loop_image_info(const void* image, size_t bytes, ll_loop_image_summary* info);
 int  loop_result(const LoopClosure* lc, int* n, int* closed, ll_pose* poses_ori, ll_pose* poses_opt, int cap, ll_pg_edge* edge);
 int  loop_cloud(ll_ctx* ctx, const LoopClosure* lc, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev);
+// ll_mapper_set_loop_policy (lc NULL: loop closure off, refused) and ll_mapper_loop_edges
+int  loop_set_policy(ll_ctx* ctx, LoopClosure* lc, const ll_loop_policy* p);
+int  loop_edges(const LoopClosure* lc, ll_pg_edge* edges, int cap, int* n_loops);

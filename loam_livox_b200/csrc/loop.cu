@@ -54,11 +54,13 @@ struct LoopClosure {
   std::vector<ll_pg_edge> edges;                     // constrain_vec
   DevBuf acc; std::vector<size_t> acc_end;           // accumulated clouds, down-sampled, in keyframe order (map_id_pc)
   ll_pose_graph* pg = nullptr;
-  bool closed = false;                               // if_end
+  ll_loop_policy policy{1, 0};                       // ll_mapper_set_loop_policy; the default is the reference's if_end
   bool stopped = false;                              // an error of the loop work stopped it (LL_LOOP_ERROR)
   bool seg_read = false;                             // seg holds the captured cloud's ends (read by the first step after a capture)
   int piece = 0;                                     // the step's piece of the captured frame
-  ll_pg_edge loop_edge{}; std::vector<ll_pose> opt;  // constrain_vec_temp.back(), temp_pose_3d_map
+  std::vector<ll_pg_edge> loops;                     // every loop edge, in closing order (constrain_vec_temp.back() of each loop)
+  std::vector<ll_pose> opt;                          // temp_pose_3d_map of the latest loop: its n_opt keyframes
+  bool done() const { return (int)loops.size() >= policy.max_loops; }   // all loop-closure work stops (if_end after the first loop by default)
   DevBuf refine; std::vector<int> ref_end;           // RefineLayout: the re-posed clouds of every keyframe
   std::vector<ll_loop_event> ring; size_t first = 0, count = 0; int dropped = 0;
 };
@@ -131,7 +133,7 @@ void free_keyframes(LoopClosure* lc) {
 // Mapping_refine::refine_pointcloud (if_save 0) of every keyframe from the accumulated clouds and both pose sets, 256 per launch chain; the
 // readers give the published ones.  The loop's last step, and what ll_mapper_loop_load recomputes (the same code: the same bits).
 int loop_refine(ll_ctx* ctx, LoopClosure* lc) {
-  const int n = (int)lc->kfs.size();
+  const int n = (int)lc->opt.size();   // n_opt: the keyframes of the latest optimization (later ones keep its refined clouds)
   const size_t total = lc->acc_end.empty() ? 0 : lc->acc_end[n - 1];
   RefineLayout rl; LL_CUDA(ctx, lc->refine.carve([&](Carve& k) { rl.layout(k, total); }));
   lc->ref_end.assign(n, 0);
@@ -178,16 +180,19 @@ int loop_align(ll_ctx* ctx, LoopClosure* lc, const std::vector<int>& cand) {
     if (r.inlier_threshold > thr2) { e->decision = LL_LOOP_SKIP10; skip_to = his + 10; continue; }
     if (!(r.inlier_threshold < thr)) { e->decision = LL_LOOP_SKIP5; skip_to = his + 5; continue; }
     e->decision = LL_LOOP_ACCEPT;
-    // the loop (:1056-1100): the edge, the graph on the odometry edges plus this one, the refined clouds
-    ll_pose_graph_loop_edge(r.q_w_curr, r.t_w_curr, &lc->poses[his], his, &lc->poses[newest], newest, &lc->loop_edge);
-    std::vector<ll_pg_edge> edges = lc->edges; edges.push_back(lc->loop_edge);
-    lc->opt = lc->poses;
+    // the loop (:1056-1100): the edge, the graph on the odometry edges plus every loop edge so far (the reference's one loop: this one only),
+    // solved from poses_ori, the refined clouds
+    ll_pg_edge le;
+    ll_pose_graph_loop_edge(r.q_w_curr, r.t_w_curr, &lc->poses[his], his, &lc->poses[newest], newest, &le);
+    std::vector<ll_pg_edge> edges = lc->edges; edges.insert(edges.end(), lc->loops.begin(), lc->loops.end()); edges.push_back(le);
+    std::vector<ll_pose> opt = lc->poses;
     ll_pg_summary sum;
-    LL_TRY(ll_pose_graph_optimize(lc->pg, lc->opt.data(), n, edges.data(), (int)edges.size(), 200, &sum));
+    LL_TRY(ll_pose_graph_optimize(lc->pg, opt.data(), n, edges.data(), (int)edges.size(), 200, &sum));
+    lc->opt.swap(opt);
     LL_TRY(loop_refine(ctx, lc));
+    lc->loops.push_back(le);
     ll_loop_event* ce = log_push(lc, LL_LOOP_CLOSED);
-    ce->his = his; ce->edge = lc->loop_edge; ce->summary = sum;
-    lc->closed = true;
+    ce->his = his; ce->edge = le; ce->summary = sum;
     return LL_OK;
   }
   return LL_OK;
@@ -237,7 +242,7 @@ void loop_release(LoopClosure* lc) {
 }
 
 int loop_scan_cloud(ll_ctx* ctx, LoopClosure* lc, const ll_pipeline_cfg* pc) {
-  if (lc->closed || lc->stopped) return LL_OK;
+  if (lc->done() || lc->stopped) return LL_OK;
   cudaStream_t s = ctx->stream;
   LoopInLayout il; LL_CUDA(ctx, lc->in.carve([&](Carve& k) { il.layout(k, lc->in_full, lc->in_scan); }));
   // the front end's compaction again, on the extractor's state of this scan, keeping the full cloud (the front end keeps only the features)
@@ -249,7 +254,7 @@ int loop_scan_cloud(ll_ctx* ctx, LoopClosure* lc, const ll_pipeline_cfg* pc) {
 }
 
 int loop_frame_clouds(ll_ctx* ctx, LoopClosure* lc, const FrameDev* dev, const size_t* ns, int n_heads, int publish) {
-  if (lc->closed || lc->stopped) return LL_OK;
+  if (lc->done() || lc->stopped) return LL_OK;
   cudaStream_t s = ctx->stream;
   LoopInLayout il; LL_CUDA(ctx, lc->in.carve([&](Carve& k) { il.layout(k, lc->in_full, lc->in_scan); }));
   FrameBases B; int base = 0, max_n = 0;
@@ -262,7 +267,7 @@ int loop_frame_clouds(ll_ctx* ctx, LoopClosure* lc, const FrameDev* dev, const s
 }
 
 int loop_sweep_cloud(ll_ctx* ctx, LoopClosure* lc, const float4* full, int n, const int* d_n) {
-  if (lc->closed || lc->stopped) return LL_OK;
+  if (lc->done() || lc->stopped) return LL_OK;
   cudaStream_t s = ctx->stream;
   LoopInLayout il; LL_CUDA(ctx, lc->in.carve([&](Carve& k) { il.layout(k, lc->in_full, lc->in_scan); }));
   if (n > 0) LL_CUDA(ctx, cudaMemcpyAsync(il.full, full, (size_t)n * 16, cudaMemcpyDeviceToDevice, s));
@@ -329,7 +334,9 @@ int loop_step_work(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool push
   LL_TRY(ll_keyframe_analyze(ctx, lc->full, closing, c.incremental_cov, &info));
   std::vector<int> cand(id + 1);
   int nc = 0;
-  LL_TRY(ll_loop_search(ctx, lc->kfs.data(), id + 1, id, &c.loop, nullptr, nullptr, cand.data(), &nc));
+  // the gap after the last loop (L its newest keyframe): a keyframe with id - L < min_keyframes_between_loops is recorded, not searched
+  const bool search = lc->loops.empty() || id - std::max(lc->loops.back().id_begin, lc->loops.back().id_end) >= lc->policy.min_keyframes_between_loops;
+  if (search) LL_TRY(ll_loop_search(ctx, lc->kfs.data(), id + 1, id, &c.loop, nullptr, nullptr, cand.data(), &nc));
   cand.resize(nc);
   ll_loop_event* ke = log_push(lc, LL_LOOP_KEYFRAME);
   ke->ending_frame_idx = frame_index; ke->n_candidates = nc; ke->info = info;
@@ -341,7 +348,7 @@ int loop_step_work(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool push
 
 // Loop closure never fails the step: an error of its work other than LL_ERR_CUDA is logged (LL_LOOP_ERROR) and stops it for good.
 int loop_step(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool pushed, int frame_index, const double q_w_curr[4], const double t_w_curr[3]) {
-  if (lc->closed || lc->stopped) return LL_OK;
+  if (lc->done() || lc->stopped) return LL_OK;
   const int st = loop_step_work(ctx, lc, d_pose, pushed, frame_index, q_w_curr, t_w_curr);
   if (st == LL_OK || st == LL_ERR_CUDA) return st;
   ll_loop_event* e = log_push(lc, LL_LOOP_ERROR);
@@ -365,19 +372,56 @@ int loop_read(LoopClosure* lc, ll_loop_event* out, int cap, int* n, int* n_dropp
 
 int loop_result(const LoopClosure* lc, int* n, int* closed, ll_pose* poses_ori, ll_pose* poses_opt, int cap, ll_pg_edge* edge) {
   const int N = lc ? (int)lc->poses.size() : 0;
+  const bool any = lc && !lc->loops.empty();
   if ((poses_ori || poses_opt) && cap < N) return LL_ERR_CAPACITY;
   if (n) *n = N;
-  if (closed) *closed = lc && lc->closed ? 1 : 0;
+  if (closed) *closed = any ? 1 : 0;
   if (poses_ori && N) memcpy(poses_ori, lc->poses.data(), N * sizeof(ll_pose));
-  if (poses_opt && N) memcpy(poses_opt, lc->closed ? lc->opt.data() : lc->poses.data(), N * sizeof(ll_pose));
-  if (edge) { if (lc && lc->closed) *edge = lc->loop_edge; else memset(edge, 0, sizeof(*edge)); }
+  if (poses_opt && N) {   // the latest optimum for its n_opt keyframes, poses_ori after them
+    const int n_opt = any ? (int)lc->opt.size() : 0;
+    if (n_opt) memcpy(poses_opt, lc->opt.data(), n_opt * sizeof(ll_pose));
+    if (N > n_opt) memcpy(poses_opt + n_opt, lc->poses.data() + n_opt, (N - n_opt) * sizeof(ll_pose));
+  }
+  if (edge) { if (any) *edge = lc->loops.back(); else memset(edge, 0, sizeof(*edge)); }
+  return LL_OK;
+}
+
+int loop_edges(const LoopClosure* lc, ll_pg_edge* edges, int cap, int* n_loops) {
+  const int n = lc ? (int)lc->loops.size() : 0;
+  if (edges && cap < n) return LL_ERR_CAPACITY;
+  *n_loops = n;
+  if (edges && n) memcpy(edges, lc->loops.data(), n * sizeof(ll_pg_edge));
+  return LL_OK;
+}
+
+// The pose graph of reserve_keyframes poses and reserve_keyframes - 1 + max_loops edges (every odometry edge and every loop edge), so that no
+// solve up to reserve_keyframes allocates device memory.  Built aside: a failure changes nothing.
+static int loop_reserve_graph(ll_ctx* ctx, LoopClosure* lc, int max_loops) {
+  const int K = std::max(lc->cfg.reserve_keyframes, 2);
+  ll_pose_graph* pg = nullptr;
+  LL_TRY(ll_pose_graph_create(ctx, K, K - 1 + max_loops, &pg));
+  ll_pose_graph_release(lc->pg);
+  lc->pg = pg;
+  return LL_OK;
+}
+
+int loop_set_policy(ll_ctx* ctx, LoopClosure* lc, const ll_loop_policy* p) {
+  ll_loop_policy q{1, 0};
+  if (p) q = *p;
+  if (!lc) { ctx->set_error("loop closure is off: set it before its policy"); return LL_ERR_INVALID; }
+  if (!lc->loops.empty()) { ctx->set_error("a loop has closed already: the policy is set before the first loop"); return LL_ERR_INVALID; }
+  if (q.max_loops < 1 || q.max_loops > LL_MAX_LOOPS) { ctx->set_error("max_loops must be 1 ... LL_MAX_LOOPS"); return LL_ERR_INVALID; }
+  if (q.min_keyframes_between_loops < 0) { ctx->set_error("min_keyframes_between_loops must be >= 0"); return LL_ERR_INVALID; }
+  cudaSetDevice(ctx->device);
+  if (q.max_loops != lc->policy.max_loops) LL_TRY(loop_reserve_graph(ctx, lc, q.max_loops));
+  lc->policy = q;
   return LL_OK;
 }
 
 int loop_cloud(ll_ctx* ctx, const LoopClosure* lc, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev) {
-  if (!lc || !lc->closed) { ctx->set_error("no loop closed"); return LL_ERR_INVALID; }
-  const int N = (int)lc->kfs.size();
-  if (k < 0 || k >= N || (N - 1 - k) % 2 != 0) { ctx->set_error("keyframe k is not one the loop publishes (n - 1, n - 3, ...)"); return LL_ERR_INVALID; }
+  if (!lc || lc->loops.empty()) { ctx->set_error("no loop closed"); return LL_ERR_INVALID; }
+  const int N = (int)lc->opt.size();   // n_opt: loop_refine's layout of the latest loop
+  if (k < 0 || k >= N || (N - 1 - k) % 2 != 0) { ctx->set_error("keyframe k is not one the latest loop publishes (n_opt - 1, n_opt - 3, ...)"); return LL_ERR_INVALID; }
   RefineLayout rl; Carve c(lc->refine.p); rl.layout(c, lc->acc_end[N - 1]);
   // a chunk's outputs start where its inputs do (keyframes 256 c ...): keyframe k's output ends at ref_end[k] and starts at its predecessor's
   // end, or at the chunk's start
@@ -404,17 +448,27 @@ template <typename T> void put(uint8_t* p, const T& v) { memcpy(p, &v, sizeof(T)
 const size_t LI_CELLS_HEAD = 24, LI_HIS_HEAD = 16, LI_ACC_HEAD = 8, LI_IMG = 4 * 3600 * 4;   // fixed parts; one keyframe's four images
 const size_t LI_STAMP = offsetof(ll_loop_image_scalars, closed);                                // the binding stamp: the scalars before `closed`
 
-struct LoopCounts { int64_t cells = 0, cell_pts = 0, his_seg = 0, his_pts = 0, open = 0, open_cells = 0, kfs = 0, cloud_pts = 0, acc = 0, acc_pts = 0, events = 0; bool closed = false; };
+const size_t LI_LOOP2_HEAD = sizeof(ll_loop_policy) + 8;   // version 2's LOOP section: the policy, n_loops, 0
+
+bool policy_default(const ll_loop_policy& p) { return p.max_loops == 1 && p.min_keyframes_between_loops == 0; }
+int edge_newest(const ll_pg_edge& e) { return std::max(e.id_begin, e.id_end); }
+
+// v2: a policy other than the default (version 2); loops, n_opt: its loop edges and the latest optimization's keyframes
+struct LoopCounts { int64_t cells = 0, cell_pts = 0, his_seg = 0, his_pts = 0, open = 0, open_cells = 0, kfs = 0, cloud_pts = 0, acc = 0, acc_pts = 0, events = 0;
+                    bool v2 = false; int64_t loops = 0, n_opt = 0; };
 
 size_t loop_layout(const LoopCounts& n, ll_loop_image_header* h) {
   memset(h, 0, sizeof(*h));
-  memcpy(h->magic, LL_LOOP_IMAGE_MAGIC, 8); h->version = LL_LOOP_IMAGE_VERSION; h->config_bytes = sizeof(ll_loop_closure_cfg);
+  memcpy(h->magic, LL_LOOP_IMAGE_MAGIC, 8); h->version = n.v2 ? LL_LOOP_IMAGE_VERSION_POLICY : LL_LOOP_IMAGE_VERSION;
+  h->config_bytes = sizeof(ll_loop_closure_cfg);
+  const uint64_t loop_len = n.v2 ? LI_LOOP2_HEAD + sizeof(ll_pg_edge) * (uint64_t)n.loops + sizeof(ll_pose) * (uint64_t)n.n_opt
+                                 : n.loops ? sizeof(ll_pg_edge) + sizeof(ll_pose) * (uint64_t)n.n_opt : 0;
   const uint64_t K = (uint64_t)n.kfs;
   const uint64_t len[LL_LOOP_IMAGE_SECTIONS] = {
       sizeof(ll_loop_closure_cfg), sizeof(ll_loop_image_scalars), LI_CELLS_HEAD + 20 * (uint64_t)(n.cells + n.cell_pts),
       LI_HIS_HEAD + 4 * (uint64_t)n.his_seg + 16 * (uint64_t)n.his_pts, sizeof(ll_loop_image_open) * (uint64_t)n.open + sizeof(ll_loop_image_ref) * (uint64_t)n.open_cells,
       sizeof(ll_keyframe_info) * K, sizeof(ll_pose) * K, sizeof(ll_pg_edge) * (K ? K - 1 : 0), LI_IMG * K, 16 * (uint64_t)n.cloud_pts,
-      LI_ACC_HEAD + 8 * (uint64_t)n.acc + 16 * (uint64_t)n.acc_pts, n.closed ? sizeof(ll_pg_edge) + sizeof(ll_pose) * K : 0,
+      LI_ACC_HEAD + 8 * (uint64_t)n.acc + 16 * (uint64_t)n.acc_pts, loop_len,
       sizeof(ll_loop_event) * (uint64_t)n.events};
   uint64_t off = sizeof(*h);
   for (int k = 0; k < LL_LOOP_IMAGE_SECTIONS; k++) { h->section[k].offset = off; h->section[k].length = len[k]; off += len[k]; }
@@ -429,7 +483,8 @@ struct LoopView {   // a validated loop image
   const uint8_t* open = nullptr; const uint8_t* refs = nullptr; int64_t open_cells = 0;
   const uint8_t *infos = nullptr, *poses = nullptr, *edges = nullptr, *images = nullptr, *clouds = nullptr; int64_t cloud_pts = 0;
   int64_t n_acc = 0, acc_pts = 0; const uint8_t* acc_end = nullptr; const uint8_t* acc = nullptr;
-  const uint8_t* loop = nullptr; const uint8_t* events = nullptr;
+  ll_loop_policy policy{1, 0}; int64_t n_loops = 0, n_opt = 0;   // the LOOP section: the policy (version 2), loop edges and optimized poses
+  const uint8_t* loop_edges = nullptr; const uint8_t* loop_opt = nullptr; const uint8_t* events = nullptr;
   int64_t replaced = 0; int32_t max_cur = 0;
 };
 
@@ -442,7 +497,7 @@ bool finite_edge(const ll_pg_edge& e) { return finite_d(e.q_wxyz, 4) && finite_d
 // max_cells can need one).
 int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_closure_cfg* cfg, LoopView* v, std::string* err) {
   auto fail = [&](const std::string& msg, int code = LL_ERR_INVALID) { if (err) *err = msg; return code; };
-  static const ImageKind kind{LL_LOOP_IMAGE_MAGIC, "loop", LL_LOOP_IMAGE_VERSION, sizeof(ll_loop_closure_cfg), "ll_loop_closure_cfg", LL_LOOP_IMAGE_SECTIONS};
+  static const ImageKind kind{LL_LOOP_IMAGE_MAGIC, "loop", LL_LOOP_IMAGE_VERSION, LL_LOOP_IMAGE_VERSION_POLICY, sizeof(ll_loop_closure_cfg), "ll_loop_closure_cfg", LL_LOOP_IMAGE_SECTIONS};
   LL_TRY(image_structure(image, bytes, kind, v->h.section, err));
   const uint8_t* b = (const uint8_t*)image;
   memcpy(&v->h, b, sizeof(v->h));
@@ -573,18 +628,45 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
     v->n_acc = n; v->acc_pts = prev; v->acc_end = p + LI_ACC_HEAD; v->acc = p + LI_ACC_HEAD + 8 * n;
     for (int64_t k = 0; k < prev; k++) if (!finite_xyz(v->acc + 16 * k)) return fail("non-finite accumulated point");
   }
-  // the loop: the edge between two keyframes and the optimized poses, only when closed
+  // the loop.  Version 1: the edge between two keyframes and the optimized poses, only when closed.  Version 2: the policy, the loop edges in
+  // closing order and the latest optimized poses
   {
     const uint64_t L = len(LL_LOOP_IMAGE_LOOP);
-    if (!sc.closed) { if (L != 0) return fail("loop section of an unclosed image not empty"); }
-    else {
-      if (K < 2) return fail("a closed loop needs two keyframes");
-      if (L != sizeof(ll_pg_edge) + sizeof(ll_pose) * (uint64_t)K) return fail("loop section disagrees with n_keyframes");
-      v->loop = sec(LL_LOOP_IMAGE_LOOP);
-      const ll_pg_edge e = get<ll_pg_edge>(v->loop);
-      if (e.id_begin < 0 || e.id_begin >= K || e.id_end < 0 || e.id_end >= K || !finite_edge(e)) return fail("loop edge out of range");
-      for (int64_t k = 0; k < K; k++) if (!finite_pose(get<ll_pose>(v->loop + sizeof(ll_pg_edge) + sizeof(ll_pose) * k))) return fail("non-finite optimized pose");
+    const uint8_t* p = sec(LL_LOOP_IMAGE_LOOP);
+    if (v->h.version == LL_LOOP_IMAGE_VERSION) {
+      if (!sc.closed) { if (L != 0) return fail("loop section of an unclosed image not empty"); }
+      else {
+        if (K < 2) return fail("a closed loop needs two keyframes");
+        if (L != sizeof(ll_pg_edge) + sizeof(ll_pose) * (uint64_t)K) return fail("loop section disagrees with n_keyframes");
+        const ll_pg_edge e = get<ll_pg_edge>(p);
+        if (e.id_begin < 0 || e.id_begin >= K || e.id_end < 0 || e.id_end >= K || !finite_edge(e)) return fail("loop edge out of range");
+        v->n_loops = 1; v->n_opt = K;
+      }
+    } else {
+      if (L < LI_LOOP2_HEAD) return fail("version-2 loop section shorter than its policy and count");
+      v->policy = get<ll_loop_policy>(p);
+      const int32_t nl = get<int32_t>(p + sizeof(ll_loop_policy)), pad = get<int32_t>(p + sizeof(ll_loop_policy) + 4);
+      if (v->policy.max_loops < 2 || v->policy.max_loops > LL_MAX_LOOPS) return fail("version-2 max_loops outside 2 ... LL_MAX_LOOPS (the default policy writes version 1)");
+      if (v->policy.min_keyframes_between_loops < 0) return fail("negative min_keyframes_between_loops");
+      if (pad != 0) return fail("loop section padding not zero");
+      if (nl < 0 || nl > v->policy.max_loops) return fail("n_loops outside 0 ... max_loops");
+      if (L < LI_LOOP2_HEAD + sizeof(ll_pg_edge) * (uint64_t)nl) return fail("loop section shorter than its edges");
+      int prev = -1;
+      for (int k = 0; k < nl; k++) {
+        const ll_pg_edge e = get<ll_pg_edge>(p + LI_LOOP2_HEAD + sizeof(ll_pg_edge) * k);
+        if (e.id_begin < 0 || e.id_begin >= K || e.id_end < 0 || e.id_end >= K || e.id_begin == e.id_end || !finite_edge(e)) return fail("loop edge out of range");
+        const int nw = edge_newest(e);
+        if (k > 0 && (nw <= prev || nw - prev < v->policy.min_keyframes_between_loops)) return fail("loop edges' newest keyframes not increasing by the gap");
+        prev = nw;
+      }
+      v->n_loops = nl; v->n_opt = nl ? prev + 1 : 0;
+      if ((sc.closed != 0) != (nl > 0)) return fail("closed disagrees with n_loops");
+      if (L != LI_LOOP2_HEAD + sizeof(ll_pg_edge) * (uint64_t)nl + sizeof(ll_pose) * (uint64_t)v->n_opt) return fail("loop section disagrees with its edges");
     }
+    const size_t head = v->h.version == LL_LOOP_IMAGE_VERSION ? 0 : LI_LOOP2_HEAD;
+    v->loop_edges = p + head;
+    v->loop_opt = p + head + sizeof(ll_pg_edge) * (size_t)v->n_loops;
+    for (int64_t k = 0; k < v->n_opt; k++) if (!finite_pose(get<ll_pose>(v->loop_opt + sizeof(ll_pose) * k))) return fail("non-finite optimized pose");
   }
   // the unread events
   {
@@ -665,14 +747,13 @@ int loop_restore(ll_ctx* ctx, LoopClosure* lc, const LoopView& v) {
   for (int64_t k = 0; k < v.n_acc; k++) lc->acc_end.push_back((size_t)get<int64_t>(v.acc_end + 8 * k));
   LL_TRY(grow_keep(ctx, lc->acc, 0, (size_t)v.acc_pts * 16 + 64));
   if (v.acc_pts) LL_CUDA(ctx, cudaMemcpyAsync(lc->acc.p, v.acc, (size_t)v.acc_pts * 16, cudaMemcpyHostToDevice, s));
-  // the loop and its refined clouds, recomputed
-  lc->closed = sc.closed != 0; lc->stopped = sc.stopped != 0;
-  if (lc->closed) {
-    lc->loop_edge = get<ll_pg_edge>(v.loop);
-    lc->opt.resize(K);
-    for (int k = 0; k < K; k++) lc->opt[k] = get<ll_pose>(v.loop + sizeof(ll_pg_edge) + sizeof(ll_pose) * k);
-    LL_TRY(loop_refine(ctx, lc));
-  }
+  // the policy, the loops and the latest loop's refined clouds, recomputed
+  if (!policy_default(v.policy)) LL_TRY(loop_set_policy(ctx, lc, &v.policy));
+  lc->stopped = sc.stopped != 0;
+  for (int64_t k = 0; k < v.n_loops; k++) lc->loops.push_back(get<ll_pg_edge>(v.loop_edges + sizeof(ll_pg_edge) * k));
+  lc->opt.resize((size_t)v.n_opt);
+  for (int64_t k = 0; k < v.n_opt; k++) lc->opt[k] = get<ll_pose>(v.loop_opt + sizeof(ll_pose) * k);
+  if (v.n_loops) LL_TRY(loop_refine(ctx, lc));
   // the unread events
   for (int k = 0; k < sc.n_events; k++) lc->ring[k] = get<ll_loop_event>(v.events + sizeof(ll_loop_event) * k);
   lc->first = 0; lc->count = (size_t)sc.n_events; lc->dropped = sc.n_dropped;
@@ -719,7 +800,8 @@ int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& s
     n.cloud_pts += (int64_t)(infos[k].line_points + infos[k].plane_points);
   }
   n.acc = (int64_t)lc->acc_end.size(); n.acc_pts = lc->acc_end.empty() ? 0 : (int64_t)lc->acc_end.back();
-  n.events = (int64_t)lc->count; n.closed = lc->closed;
+  n.events = (int64_t)lc->count; n.v2 = !policy_default(lc->policy);
+  n.loops = (int64_t)lc->loops.size(); n.n_opt = n.loops ? (int64_t)lc->opt.size() : 0;
   ll_loop_image_header h;
   const size_t total = loop_layout(n, &h);
   *bytes = total;
@@ -730,7 +812,7 @@ int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& s
   memcpy(b, &h, sizeof(h));
   memcpy(at(LL_LOOP_IMAGE_CONFIG), &lc->cfg, sizeof(lc->cfg));
   ll_loop_image_scalars sc = stamp;
-  sc.closed = lc->closed ? 1 : 0; sc.stopped = lc->stopped ? 1 : 0;
+  sc.closed = lc->loops.empty() ? 0 : 1; sc.stopped = lc->stopped ? 1 : 0;
   sc.n_keyframes = (int32_t)n.kfs; sc.n_open = (int32_t)n.open; sc.n_events = (int32_t)n.events; sc.n_dropped = lc->dropped;
   memcpy(at(LL_LOOP_IMAGE_SCALARS), &sc, sizeof(sc));
   // the full map with the held incarnations
@@ -777,11 +859,15 @@ int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& s
   put<int64_t>(p, n.acc);
   for (size_t k = 0; k < lc->acc_end.size(); k++) put<int64_t>(p + LI_ACC_HEAD + 8 * k, (int64_t)lc->acc_end[k]);
   if (n.acc_pts) LL_CUDA(ctx, cudaMemcpyAsync(p + LI_ACC_HEAD + 8 * n.acc, lc->acc.p, (size_t)n.acc_pts * 16, cudaMemcpyDeviceToHost, s));
-  // the loop
-  if (lc->closed) {
-    p = at(LL_LOOP_IMAGE_LOOP);
-    put(p, lc->loop_edge);
-    memcpy(p + sizeof(ll_pg_edge), lc->opt.data(), sizeof(ll_pose) * lc->opt.size());
+  // the loop: version 1 the edge of the one loop, version 2 the policy and every loop edge; then the optimized poses
+  p = at(LL_LOOP_IMAGE_LOOP);
+  if (n.v2) {
+    put(p, lc->policy); put<int32_t>(p + sizeof(ll_loop_policy), (int32_t)n.loops); put<int32_t>(p + sizeof(ll_loop_policy) + 4, 0);
+    p += LI_LOOP2_HEAD;
+  }
+  if (n.loops) {
+    memcpy(p, lc->loops.data(), sizeof(ll_pg_edge) * lc->loops.size());
+    memcpy(p + sizeof(ll_pg_edge) * lc->loops.size(), lc->opt.data(), sizeof(ll_pose) * (size_t)n.n_opt);
   }
   // the unread events, oldest first
   for (size_t k = 0; k < lc->count; k++) {   // the pose graph's SM clock counters time the solve: not state, saved as 0

@@ -618,7 +618,7 @@ int image_structure(const void* image, size_t bytes, const ImageKind& kind, ll_i
   memcpy(magic, b, 8); memcpy(&version, b + 8, 4); memcpy(&config_bytes, b + 12, 4); memcpy(&total, b + 16, 8);
   memcpy(sec, b + 24, 16 * (size_t)kind.sections);
   if (memcmp(magic, kind.magic, 8) != 0) return fail(std::string("not a ") + kind.name + " image (magic)");
-  if (version != kind.version) return fail("unknown image version");
+  if (version < kind.version || version > kind.max_version) return fail("unknown image version");
   if (config_bytes != kind.config_bytes) return fail(std::string("config size differs from this library's ") + kind.config_name);
   if (total != bytes) return fail("image size differs from the header's total_bytes");
   // every section inside the image after the header, no two overlapping
@@ -659,7 +659,7 @@ namespace {
 int image_validate(const void* image, size_t bytes, const ll_mapper_config* cfg, ImageView* v, std::string* err) {
   auto fail = [&](const char* msg, int code = LL_ERR_INVALID) { if (err) *err = msg; return code; };
   const uint8_t* b = (const uint8_t*)image;
-  static const ImageKind kind{LL_MAPPER_IMAGE_MAGIC, "mapper", LL_MAPPER_IMAGE_VERSION, sizeof(ll_mapper_config), "ll_mapper_config", LL_IMAGE_SECTIONS};
+  static const ImageKind kind{LL_MAPPER_IMAGE_MAGIC, "mapper", LL_MAPPER_IMAGE_VERSION, LL_MAPPER_IMAGE_VERSION, sizeof(ll_mapper_config), "ll_mapper_config", LL_IMAGE_SECTIONS};
   LL_TRY(image_structure(image, bytes, kind, v->h.section, err));
   memcpy(&v->h, b, sizeof(v->h));
   auto sec = [&](int k) { return b + v->h.section[k].offset; };
@@ -1230,6 +1230,20 @@ int ll_mapper_loop_result(ll_mapper* m, int* n, int* closed, ll_pose* poses_ori,
 int ll_mapper_loop_cloud(ll_mapper* m, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev) {
   if (!m || !n_out) return LL_ERR_INVALID;
   return loop_cloud(m->ctx, m->lc, k, out_host, cap, n_out, out_dev);
+}
+
+void ll_mapper_loop_policy_default(ll_loop_policy* p) {
+  if (p) { p->max_loops = 1; p->min_keyframes_between_loops = 0; }
+}
+
+int ll_mapper_set_loop_policy(ll_mapper* m, const ll_loop_policy* p) {
+  if (!m) return LL_ERR_INVALID;
+  return loop_set_policy(m->ctx, m->lc, p);
+}
+
+int ll_mapper_loop_edges(ll_mapper* m, ll_pg_edge* edges, int cap, int* n_loops) {
+  if (!m || !n_loops || cap < 0) return LL_ERR_INVALID;
+  return loop_edges(m->lc, edges, cap, n_loops);
 }
 
 // The loop image's binding stamp: what the loop closure's state refers to in the mapper (loop.cu checks it on load).

@@ -1055,7 +1055,7 @@ class Laser_mapping:
 
     def set_loop_closure(self, enable: bool = True, **kw):
         """Loop closure (ll_mapper_set_loop_closure; DESIGN.md §4.6): from now on every appended step feeds the keyframes of the full-resolution map,
-        and each closed keyframe is searched against the earlier ones until the first loop closes.  kw overrides fields of
+        and each closed keyframe is searched against the earlier ones until the first loop closes (set_loop_policy: further loops).  kw overrides fields of
         ll_mapper_loop_closure_default (loop=dict(...) the search's gates); enable=False turns it off.  Returns the capi.LoopClosureCfg in force."""
         if not enable:
             self.ctx.check(self.ctx._lib.ll_mapper_set_loop_closure(self.h, None))
@@ -1075,6 +1075,23 @@ class Laser_mapping:
         self.ctx.check(self.ctx._lib.ll_mapper_set_loop_closure(self.h, C.byref(cfg)))
         return cfg
 
+    def set_loop_policy(self, max_loops: int = 1, min_keyframes_between_loops: int = 0):
+        """Loops after the first (ll_mapper_set_loop_policy): close up to max_loops loops, the newest keyframes of two loops at least
+        min_keyframes_between_loops apart; every loop edge joins one pose graph.  The defaults are the reference's (first loop, then stop).  Set
+        after set_loop_closure (which resets it) and before the first loop; a refused policy raises and changes nothing.  Returns the
+        capi.LoopPolicy in force."""
+        p = capi.LoopPolicy(max_loops=max_loops, min_keyframes_between_loops=min_keyframes_between_loops)
+        self.ctx.check(self.ctx._lib.ll_mapper_set_loop_policy(self.h, C.byref(p)))
+        return p
+
+    def loop_edges(self):
+        """Every loop edge so far, in closing order (ll_mapper_loop_edges): a list of capi.PgEdge."""
+        n = C.c_int()
+        self.ctx.check(self.ctx._lib.ll_mapper_loop_edges(self.h, None, 0, C.byref(n)))
+        buf = (capi.PgEdge * max(n.value, 1))()
+        self.ctx.check(self.ctx._lib.ll_mapper_loop_edges(self.h, buf, n.value, C.byref(n)))
+        return [capi.PgEdge.from_buffer_copy(buf[i]) for i in range(n.value)]
+
     def loop_log(self):
         """The loop-closure events since the last read (capi.LoopEvent, oldest first) and how many were overwritten unread."""
         out, total = [], 0
@@ -1087,7 +1104,8 @@ class Laser_mapping:
                 return out, total
 
     def loop_result(self):
-        """{"closed": bool, "poses_ori", "poses_opt": float64 [n, 7] (q w, x, y, z, t), "edge": capi.PgEdge} (ll_mapper_loop_result)."""
+        """{"closed": bool, "poses_ori", "poses_opt": float64 [n, 7] (q w, x, y, z, t), "edge": capi.PgEdge} (ll_mapper_loop_result): poses_opt is the
+        latest optimization's for the keyframes it covered and poses_ori after them; edge the latest loop edge."""
         L = self.ctx._lib
         n, closed = C.c_int(), C.c_int()
         self.ctx.check(L.ll_mapper_loop_result(self.h, C.byref(n), C.byref(closed), None, None, 0, None))
@@ -1097,7 +1115,7 @@ class Laser_mapping:
         return {"closed": bool(closed.value), "poses_ori": as_np(ori), "poses_opt": as_np(opt), "edge": edge}
 
     def loop_cloud(self, k: int):
-        """The refined cloud of published keyframe k (ll_mapper_loop_cloud), float32 [n, 4]."""
+        """The refined cloud of published keyframe k of the latest loop (ll_mapper_loop_cloud), float32 [n, 4]."""
         n = C.c_size_t()
         self.ctx.check(self.ctx._lib.ll_mapper_loop_cloud(self.h, int(k), None, 0, C.byref(n), None))
         out = np.zeros((n.value, 4), np.float32)
