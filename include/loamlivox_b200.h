@@ -284,7 +284,7 @@ int ll_frame_to_pose(ll_ctx* ctx, const ll_map* map, int n_heads, const void* co
 /* ---- a14: device-resident voxel-cell map (matching_mode 1) ---------------------------------------------- */
 /* Replaces Points_cloud_map<float> as the matching path uses it (cell_map_keyframe.hpp:476-1000): `resolution` is what
  * Laser_mapping passes to set_resolution (1.0 => 0.5 m cells, :674-679), `revisit_threshold` = m_minimum_revisit_threshold
- * (common/threshold_cell_revisit, >= 1).  max_cells sizes the hash table (0 = 1 Mi cells). */
+ * (common/threshold_cell_revisit, >= 1).  max_cells sizes the hash table (0 = 1 Mi cells; at most 2^29, LL_ERR_INVALID above). */
 typedef struct ll_cellmap ll_cellmap;
 int  ll_cellmap_create(ll_ctx* ctx, float resolution, int revisit_threshold, int max_cells, ll_cellmap** out);
 void ll_cellmap_release(ll_cellmap* map);
@@ -310,7 +310,7 @@ typedef struct {
   int   threshold_cell_revisit;                 /* common/threshold_cell_revisit                                                           */
   float maximum_search_range_corner, maximum_search_range_surface, maximum_in_fov_angle;   /* mapping/... (:691-695)                      */
   int   down_sample_replace;                    /* m_down_sample_replace (:277)                                                            */
-  int   max_cells;                              /* hash-table sizing of each cell map (0 = 1 Mi cells)                                     */
+  int   max_cells;                              /* hash-table sizing of each cell map (0 = 1 Mi cells; at most 2^29)                       */
   int   matching_mode;                          /* mapping/matching_mode (:689): 0 = sliding window of the last maximum_history_size feature clouds
                                                    (:518-531,1439-1478; what both shipped YAMLs select), 1 = cells in range and in the FOV (:471-516)   */
   int   maximum_history_size;                   /* mapping/maximum_histroy_buffer (:687; YAML 400 / 200)                                   */
@@ -780,7 +780,7 @@ typedef struct {
   double surround_pointcloud_resolution;      /* mapping/surround_pointcloud_resolution (0.30): the accumulated clouds' VoxelGrid leaf     */
   int    incremental_cov;                     /* common/if_update_mean_and_cov_incrementally (1)                                            */
   int    rng_seed;                            /* ll_align_cfg::rng_seed of every alignment                                                  */
-  int    max_cells;                           /* the full map's cell table (as ll_cellmap_create; 0: its default)                          */
+  int    max_cells;                           /* the full map's cell table (as ll_cellmap_create; 0: its default; at most 2^29)            */
   long long reserve_map_points;               /* the full map's point store allocated by ll_mapper_set_loop_closure                        */
   long long reserve_history_points;           /* the full history allocated by ll_mapper_set_loop_closure                                  */
   int    reserve_keyframes;                   /* keyframes whose poses, edges and graph are allocated by ll_mapper_set_loop_closure        */

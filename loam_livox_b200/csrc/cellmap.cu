@@ -212,6 +212,8 @@ struct CmAssemble {
 };
 static size_t cm_assemble_bytes(int T, int N) { CmAssemble a(T, N); return layout_bytes([&](Carve& c) { a.layout(c, T, N); }); }
 
+int64_t table_capacity(int max_cells) { int64_t cap = 1 << 12; const int64_t want = 2 * (int64_t)(max_cells > 0 ? max_cells : (1 << 20)); while (cap < want) cap <<= 1; return cap; }
+
 extern "C" {
 
 // Size every buffer of the map for `store_points` stored points and appends of up to `scan_points` points, now: after this, appends and assemblies
@@ -233,10 +235,10 @@ int ll_cellmap_reserve(ll_ctx* ctx, ll_cellmap* m, size_t store_points, size_t s
 
 int ll_cellmap_create(ll_ctx* ctx, float resolution, int revisit_threshold, int max_cells, ll_cellmap** out) {
   // revisit_threshold < 1 would replace a cell at every point that touches it (only the last point of a call would stay); it is refused
-  if (!ctx || !out || !(resolution > 0.f) || revisit_threshold < 1) return LL_ERR_INVALID;
+  if (!ctx || !out || !(resolution > 0.f) || revisit_threshold < 1 || max_cells > MAX_CELLS) return LL_ERR_INVALID;
   cudaSetDevice(ctx->device);
   ll_cellmap* m = new ll_cellmap(); m->device = ctx->device; m->resolution = resolution * 0.5f; m->revisit_threshold = revisit_threshold;
-  int cap = 1 << 12; while (cap < 2 * (max_cells > 0 ? max_cells : (1 << 20))) cap <<= 1;
+  const int cap = (int)table_capacity(max_cells);
   m->table_cap = cap;
   const cudaError_t e = m->table_buf.carve([&](Carve& c) {
     m->keys = c.take<unsigned long long>(cap);

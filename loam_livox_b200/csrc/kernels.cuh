@@ -250,20 +250,9 @@ int cm_import(ll_ctx* ctx, ll_cellmap* m, int frame_idx, int n_out_of_range, con
 // The n_live live points (the count cm_count gave) in store order, as the map stores them, into the device array dst on the context's stream,
 // by the export's live-point selection; the map is only read.
 int cm_live_points(ll_ctx* ctx, ll_cellmap* m, int n_live, float4* dst);
-
-// ---------------------------------------------------------------------------------------------- byte images (mapper.cu)
-// What the mapper image and the loop image share: a header of magic[8], uint32 version, uint32 config_bytes, uint64 total_bytes and `sections`
-// (offset, length) pairs.  image_structure checks that header (magic, a version in version ... max_version, the config's size, total_bytes = the
-// image's size) and that every section lies inside the image after the header with no two overlapping; the sections go to sec.  LL_OK or
-// LL_ERR_INVALID and what is wrong.
-struct ImageKind { const char* magic; const char* name; uint32_t version, max_version; uint32_t config_bytes; const char* config_name; int sections; };
-int image_structure(const void* image, size_t bytes, const ImageKind& kind, ll_image_section* sec, std::string* err);
-// A history section (int64 n_segments, int64 n_points, int32 size[], ll_point points[]) of L bytes at p: NULL when its counts match the length,
-// the sizes sum to the points and, if `finite`, every point is finite (its parts then in the outputs), else what is wrong.  (The feature
-// histories hold finite points only; the loop closure's full history holds the steps' full clouds as they came, non-finite points included.)
-const char* history_section(const uint8_t* p, uint64_t L, bool finite, int64_t* n_seg, int64_t* n_pts, const uint8_t** sizes, const uint8_t** pts);
-bool finite_xyz(const uint8_t* p);   // the first three floats at p are finite
-int64_t table_capacity(int max_cells);   // the hash-table capacity ll_cellmap_create gives a map of max_cells
+// The largest max_cells a cell map takes (LL_ERR_INVALID above): its table of 2^30 slots is the largest whose sizes stay within int.
+const int MAX_CELLS = 1 << 29;
+int64_t table_capacity(int max_cells);   // the hash-table capacity ll_cellmap_create gives a map of max_cells (any int: computed in int64)
 
 // ---------------------------------------------------------------------------------------------- keyframes in the loop image (keyframe.cu)
 int kf_cell_count(const ll_keyframe* kf);
@@ -393,3 +382,61 @@ int  loop_cloud(ll_ctx* ctx, const LoopClosure* lc, int k, ll_point* out_host, s
 // ll_mapper_set_loop_policy (lc NULL: loop closure off, refused) and ll_mapper_loop_edges
 int  loop_set_policy(ll_ctx* ctx, LoopClosure* lc, const ll_loop_policy* p);
 int  loop_edges(const LoopClosure* lc, ll_pg_edge* edges, int cap, int* n_loops);
+
+// A log of the last entries (recovery's steps, loop closure's events), oldest first: a push into a full log overwrites the oldest unread entry
+// and counts it as dropped; a read takes the oldest entries and clears the dropped count.
+template <typename T> struct EventLog {
+  std::vector<T> ring; size_t first = 0, count = 0; int dropped = 0;   // count entries from ring[first]
+  void open(size_t cap) { if (ring.empty()) ring.resize(cap); }
+  T* push() {   // the new entry, zeroed
+    if (count == ring.size()) { first = (first + 1) % ring.size(); count--; dropped++; }
+    T* e = &ring[(first + count) % ring.size()]; count++;
+    memset(e, 0, sizeof(*e));
+    return e;
+  }
+  const T& at(size_t k) const { return ring[(first + k) % ring.size()]; }   // the k-th oldest
+  void read(T* out, int cap, int* n, int* n_dropped) {
+    const size_t k = count < (size_t)cap ? count : (size_t)cap;
+    for (size_t i = 0; i < k; i++) out[i] = at(i);
+    if (k > 0) { first = (first + k) % ring.size(); count -= k; }
+    *n = (int)k;
+    if (n_dropped) *n_dropped = dropped;
+    dropped = 0;
+  }
+  void restore(const void* entries, size_t n, int n_dropped) { memcpy(ring.data(), entries, n * sizeof(T)); first = 0; count = n; dropped = n_dropped; }
+};
+
+// ---------------------------------------------------------------------------------------------- byte images (checkpoint.cu)
+// What the mapper image and the loop image share (format: include/loamlivox_b200.h).  The checks run on the host before anything touches the
+// device and give NULL or what is wrong (LL_ERR_INVALID); the writes copy device data on the context's stream, for the caller to synchronise.
+template <typename T> T img_get(const uint8_t* p) { T v; memcpy(&v, p, sizeof(T)); return v; }   // unaligned typed read / write
+template <typename T> void img_put(uint8_t* p, const T& v) { memcpy(p, &v, sizeof(T)); }
+const size_t HIS_HEAD = 16, CELLS_HEAD = 24;   // the fixed part of a history and a cell-map section
+// A header of magic[8], uint32 version, uint32 config_bytes, uint64 total_bytes and `sections` (offset, length) pairs.  image_header writes
+// it for sections of lengths len[] back to back in index order and returns the image's size; image_structure checks it (magic, a version in
+// version ... max_version, the config's size, total_bytes = the image's size, every section inside the image after the header, no two
+// overlapping) and gives the sections.
+struct ImageKind { const char* magic; const char* name; uint32_t version, max_version; uint32_t config_bytes; const char* config_name; int sections; };
+size_t image_header(const ImageKind& kind, uint32_t version, const uint64_t* len, void* header);
+int image_structure(const void* image, size_t bytes, const ImageKind& kind, ll_image_section* sec, std::string* err);
+bool finite_xyz(const uint8_t* p);       // the first three floats at p are finite
+bool finite_d(const double* d, int n);
+// The history section.  The restore pushes segment by segment from one upload and synchronises.  `finite`: every point must be finite (the
+// feature histories; the loop closure's full history holds the steps' full clouds as they came).
+struct HistoryView { int64_t n_seg = 0, n_pts = 0; const uint8_t* sizes = nullptr; const uint8_t* pts = nullptr; };
+uint64_t history_bytes(const HistoryWindow& w);
+int history_write(ll_ctx* ctx, const HistoryWindow& w, uint8_t* p);
+const char* history_section(const uint8_t* p, uint64_t L, bool finite, HistoryView* v);
+int history_restore(ll_ctx* ctx, HistoryWindow& w, const HistoryView& v);
+// The cell-map section: cm_count's head and cm_export's records, with incarnations (the loop image) their ordinals too.
+struct CellsView {
+  int32_t frame_idx = 0, n_oor = 0; int64_t n_cells = 0, n_pts = 0; const uint8_t* rec = nullptr;
+  const uint8_t* cur = nullptr; int32_t max_cur = 0; int64_t replaced = 0;   // incarnations: the cells' current ordinals, their largest, points not current
+};
+uint64_t cells_bytes(const CellsView& n, bool incarnations);
+int cells_write(ll_ctx* ctx, ll_cellmap* m, const CellsView& n, uint8_t* p, const CmHeld* held = nullptr);
+const char* cells_section(const uint8_t* p, uint64_t L, bool incarnations, CellsView* v);
+int cells_restore(ll_ctx* ctx, ll_cellmap* m, const CellsView& v, bool incarnations, int* slot_of_rank = nullptr);
+// The load's capacity rule (LL_ERR_CAPACITY): the cells at most half the table of *max_cells (NULL: not checked), at most 2^30 cell-map points
+// and 2^31 - 1 history points.
+const char* load_capacity(const CellsView& c, const HistoryView& h, const int* max_cells);

@@ -62,7 +62,7 @@ struct LoopClosure {
   std::vector<ll_pose> opt;                          // temp_pose_3d_map of the latest loop: its n_opt keyframes
   bool done() const { return (int)loops.size() >= policy.max_loops; }   // all loop-closure work stops (if_end after the first loop by default)
   DevBuf refine; std::vector<int> ref_end;           // RefineLayout: the re-posed clouds of every keyframe
-  std::vector<ll_loop_event> ring; size_t first = 0, count = 0; int dropped = 0;
+  EventLog<ll_loop_event> log;
 };
 
 namespace {
@@ -81,7 +81,7 @@ const char* loop_cfg_error(const ll_loop_closure_cfg& c) {
   if (c.scene_alignment_maximum_residual_block < 1) return "scene_alignment_maximum_residual_block must be >= 1";
   if (!pos(c.surround_pointcloud_resolution) || !pos((float)c.surround_pointcloud_resolution)) return "surround_pointcloud_resolution must be finite and > 0";
   if (c.incremental_cov != 0 && c.incremental_cov != 1) return "incremental_cov must be 0 or 1";
-  if (c.max_cells < 0) return "max_cells must be >= 0";
+  if (c.max_cells < 0 || c.max_cells > MAX_CELLS) return "max_cells must be 0 ... 2^29";
   if (c.reserve_map_points < 0 || c.reserve_map_points > INT32_MAX || c.reserve_history_points < 0 || c.reserve_history_points > INT32_MAX)
     return "reservations must be 0 ... 2^31 - 1 points";
   if (c.reserve_keyframes < 0 || c.reserve_keyframes > (1 << 20)) return "reserve_keyframes must be 0 ... 2^20";
@@ -118,9 +118,8 @@ int grow_keep(ll_ctx* ctx, DevBuf& b, size_t used, size_t need) {
 }
 
 ll_loop_event* log_push(LoopClosure* lc, int kind) {
-  if (lc->count == lc->ring.size()) { lc->first = (lc->first + 1) % lc->ring.size(); lc->count--; lc->dropped++; }
-  ll_loop_event* e = &lc->ring[(lc->first + lc->count) % lc->ring.size()]; lc->count++;
-  memset(e, 0, sizeof(*e)); e->kind = kind; e->keyframe = (int)lc->kfs.size() - 1;
+  ll_loop_event* e = lc->log.push();
+  e->kind = kind; e->keyframe = (int)lc->kfs.size() - 1;
   return e;
 }
 
@@ -223,7 +222,7 @@ int loop_set(ll_ctx* ctx, LoopClosure** plc, const ll_loop_closure_cfg* cfg, con
     ll_keyframe* kf = nullptr;
     LL_TRY(ll_keyframe_create(ctx, &kf));
     lc->open.push_back({kf, 0});   // :626
-    lc->ring.resize(LL_LOOP_LOG);
+    lc->log.open(LL_LOOP_LOG);
     return LL_OK;
   }();
   if (st != LL_OK) { loop_release(lc); return st; }
@@ -358,15 +357,9 @@ int loop_step(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool pushed, i
 }
 
 int loop_read(LoopClosure* lc, ll_loop_event* out, int cap, int* n, int* n_dropped) {
+  if (lc) { lc->log.read(out, cap, n, n_dropped); return LL_OK; }
   *n = 0;
   if (n_dropped) *n_dropped = 0;
-  if (!lc) return LL_OK;
-  const int k = (int)std::min((size_t)cap, lc->count);
-  for (int i = 0; i < k; i++) out[i] = lc->ring[(lc->first + i) % lc->ring.size()];
-  if (k > 0) { lc->first = (lc->first + k) % lc->ring.size(); lc->count -= k; }
-  *n = k;
-  if (n_dropped) *n_dropped = lc->dropped;
-  lc->dropped = 0;
   return LL_OK;
 }
 
@@ -442,53 +435,26 @@ int loop_cloud(ll_ctx* ctx, const LoopClosure* lc, int k, ll_point* out_host, si
 // touches the device; the save writes the sections back to back in index order.
 namespace {
 
-template <typename T> T get(const uint8_t* p) { T v; memcpy(&v, p, sizeof(T)); return v; }
-template <typename T> void put(uint8_t* p, const T& v) { memcpy(p, &v, sizeof(T)); }
-
-const size_t LI_CELLS_HEAD = 24, LI_HIS_HEAD = 16, LI_ACC_HEAD = 8, LI_IMG = 4 * 3600 * 4;   // fixed parts; one keyframe's four images
-const size_t LI_STAMP = offsetof(ll_loop_image_scalars, closed);                                // the binding stamp: the scalars before `closed`
-
-const size_t LI_LOOP2_HEAD = sizeof(ll_loop_policy) + 8;   // version 2's LOOP section: the policy, n_loops, 0
+const ImageKind LOOP_IMAGE{LL_LOOP_IMAGE_MAGIC, "loop", LL_LOOP_IMAGE_VERSION, LL_LOOP_IMAGE_VERSION_POLICY, sizeof(ll_loop_closure_cfg), "ll_loop_closure_cfg",
+                           LL_LOOP_IMAGE_SECTIONS};
+const size_t LI_ACC_HEAD = 8, LI_IMG = 4 * 3600 * 4;                   // the accumulated section's fixed part; one keyframe's four images
+const size_t LI_STAMP = offsetof(ll_loop_image_scalars, closed);       // the binding stamp: the scalars before `closed`
+const size_t LI_LOOP2_HEAD = sizeof(ll_loop_policy) + 8;               // version 2's LOOP section: the policy, n_loops, 0
 
 bool policy_default(const ll_loop_policy& p) { return p.max_loops == 1 && p.min_keyframes_between_loops == 0; }
 int edge_newest(const ll_pg_edge& e) { return std::max(e.id_begin, e.id_end); }
 
-// v2: a policy other than the default (version 2); loops, n_opt: its loop edges and the latest optimization's keyframes
-struct LoopCounts { int64_t cells = 0, cell_pts = 0, his_seg = 0, his_pts = 0, open = 0, open_cells = 0, kfs = 0, cloud_pts = 0, acc = 0, acc_pts = 0, events = 0;
-                    bool v2 = false; int64_t loops = 0, n_opt = 0; };
-
-size_t loop_layout(const LoopCounts& n, ll_loop_image_header* h) {
-  memset(h, 0, sizeof(*h));
-  memcpy(h->magic, LL_LOOP_IMAGE_MAGIC, 8); h->version = n.v2 ? LL_LOOP_IMAGE_VERSION_POLICY : LL_LOOP_IMAGE_VERSION;
-  h->config_bytes = sizeof(ll_loop_closure_cfg);
-  const uint64_t loop_len = n.v2 ? LI_LOOP2_HEAD + sizeof(ll_pg_edge) * (uint64_t)n.loops + sizeof(ll_pose) * (uint64_t)n.n_opt
-                                 : n.loops ? sizeof(ll_pg_edge) + sizeof(ll_pose) * (uint64_t)n.n_opt : 0;
-  const uint64_t K = (uint64_t)n.kfs;
-  const uint64_t len[LL_LOOP_IMAGE_SECTIONS] = {
-      sizeof(ll_loop_closure_cfg), sizeof(ll_loop_image_scalars), LI_CELLS_HEAD + 20 * (uint64_t)(n.cells + n.cell_pts),
-      LI_HIS_HEAD + 4 * (uint64_t)n.his_seg + 16 * (uint64_t)n.his_pts, sizeof(ll_loop_image_open) * (uint64_t)n.open + sizeof(ll_loop_image_ref) * (uint64_t)n.open_cells,
-      sizeof(ll_keyframe_info) * K, sizeof(ll_pose) * K, sizeof(ll_pg_edge) * (K ? K - 1 : 0), LI_IMG * K, 16 * (uint64_t)n.cloud_pts,
-      LI_ACC_HEAD + 8 * (uint64_t)n.acc + 16 * (uint64_t)n.acc_pts, loop_len,
-      sizeof(ll_loop_event) * (uint64_t)n.events};
-  uint64_t off = sizeof(*h);
-  for (int k = 0; k < LL_LOOP_IMAGE_SECTIONS; k++) { h->section[k].offset = off; h->section[k].length = len[k]; off += len[k]; }
-  h->total_bytes = off;
-  return (size_t)off;
-}
-
 struct LoopView {   // a validated loop image
   ll_loop_image_header h; ll_loop_closure_cfg cfg; ll_loop_image_scalars sc;
-  int32_t frame_idx = 0, n_oor = 0; int64_t n_cells = 0, n_pts = 0; const uint8_t* cells = nullptr; const uint8_t* cur = nullptr;
-  int64_t his_seg = 0, his_pts = 0; const uint8_t* his_sizes = nullptr; const uint8_t* his_pts_p = nullptr;
+  CellsView cells;
+  HistoryView his;
   const uint8_t* open = nullptr; const uint8_t* refs = nullptr; int64_t open_cells = 0;
   const uint8_t *infos = nullptr, *poses = nullptr, *edges = nullptr, *images = nullptr, *clouds = nullptr; int64_t cloud_pts = 0;
   int64_t n_acc = 0, acc_pts = 0; const uint8_t* acc_end = nullptr; const uint8_t* acc = nullptr;
   ll_loop_policy policy{1, 0}; int64_t n_loops = 0, n_opt = 0;   // the LOOP section: the policy (version 2), loop edges and optimized poses
   const uint8_t* loop_edges = nullptr; const uint8_t* loop_opt = nullptr; const uint8_t* events = nullptr;
-  int64_t replaced = 0; int32_t max_cur = 0;
 };
 
-bool finite_d(const double* d, int n) { for (int k = 0; k < n; k++) if (!std::isfinite(d[k])) return false; return true; }
 bool finite_pose(const ll_pose& p) { return finite_d(p.q_wxyz, 4) && finite_d(p.t, 3); }
 bool finite_edge(const ll_pg_edge& e) { return finite_d(e.q_wxyz, 4) && finite_d(e.t, 3) && finite_d(e.information, 36); }
 
@@ -497,8 +463,7 @@ bool finite_edge(const ll_pg_edge& e) { return finite_d(e.q_wxyz, 4) && finite_d
 // max_cells can need one).
 int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_closure_cfg* cfg, LoopView* v, std::string* err) {
   auto fail = [&](const std::string& msg, int code = LL_ERR_INVALID) { if (err) *err = msg; return code; };
-  static const ImageKind kind{LL_LOOP_IMAGE_MAGIC, "loop", LL_LOOP_IMAGE_VERSION, LL_LOOP_IMAGE_VERSION_POLICY, sizeof(ll_loop_closure_cfg), "ll_loop_closure_cfg", LL_LOOP_IMAGE_SECTIONS};
-  LL_TRY(image_structure(image, bytes, kind, v->h.section, err));
+  LL_TRY(image_structure(image, bytes, LOOP_IMAGE, v->h.section, err));
   const uint8_t* b = (const uint8_t*)image;
   memcpy(&v->h, b, sizeof(v->h));
   auto sec = [&](int k) { return b + v->h.section[k].offset; };
@@ -520,41 +485,10 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
       sc.n_events > LL_LOOP_LOG || sc.n_dropped < 0)
     return fail("scalars out of range");
   const int64_t K = sc.n_keyframes;
-  // the full map: keys strictly ascending with bit 63 clear, stamps <= current_frame_idx, ranks < the cell count, ordinals <= their cell's
-  // current one, finite points
-  {
-    const uint8_t* p = sec(LL_LOOP_IMAGE_CELLS); const uint64_t L = len(LL_LOOP_IMAGE_CELLS);
-    if (L < LI_CELLS_HEAD) return fail("cell-map section shorter than its counts");
-    const int32_t fi = get<int32_t>(p), oor = get<int32_t>(p + 4);
-    const int64_t nc = get<int64_t>(p + 8), np = get<int64_t>(p + 16);
-    if (nc < 0 || np < 0 || (uint64_t)nc > (L - LI_CELLS_HEAD) / 20 || (uint64_t)np > (L - LI_CELLS_HEAD) / 20 || LI_CELLS_HEAD + 20 * (uint64_t)(nc + np) != L)
-      return fail("cell-map counts disagree with the section length");
-    if (fi < 0 || oor < 0) return fail("cell-map frame index or out-of-range count negative");
-    const uint8_t* cells = p + LI_CELLS_HEAD; const uint8_t* pts = cells + 16 * nc; const uint8_t* cur = pts + 16 * np; const uint8_t* ord = cur + 4 * nc;
-    uint64_t prev = 0;
-    for (int64_t k = 0; k < nc; k++) {
-      const ll_image_cell e = get<ll_image_cell>(cells + 16 * k);
-      if (e.key >> 63) return fail("cell key with bit 63 set");
-      if (k > 0 && e.key <= prev) return fail("cell keys not strictly ascending");
-      if (e.create_frame < 0 || e.create_frame > fi || e.last_update < 0 || e.last_update > fi) return fail("cell stamp outside 0 ... current_frame_idx");
-      const int32_t c = get<int32_t>(cur + 4 * k);
-      if (c < 0 || c > fi) return fail("incarnation ordinal outside 0 ... current_frame_idx");   // one revisit per cell and append at most
-      v->max_cur = std::max(v->max_cur, c);
-      prev = e.key;
-    }
-    for (int64_t k = 0; k < np; k++) {
-      const ll_image_cell_point q = get<ll_image_cell_point>(pts + 16 * k);
-      if (!(std::isfinite(q.x) && std::isfinite(q.y) && std::isfinite(q.z))) return fail("non-finite cell-map point");
-      if (q.cell < 0 || q.cell >= nc) return fail("cell-map point's cell rank >= the cell count");
-      const int32_t o = get<int32_t>(ord + 4 * k), c = get<int32_t>(cur + 4 * q.cell);
-      if (o < 0 || o > c) return fail("cell-map point's incarnation outside 0 ... its cell's current one");
-      v->replaced += o != c;
-    }
-    v->frame_idx = fi; v->n_oor = oor; v->n_cells = nc; v->n_pts = np; v->cells = cells; v->cur = cur;
-  }
-  // the full history
-  if (const char* e = history_section(sec(LL_LOOP_IMAGE_HISTORY), len(LL_LOOP_IMAGE_HISTORY), false, &v->his_seg, &v->his_pts, &v->his_sizes, &v->his_pts_p)) return fail(e);
-  if (sc.maximum_history_size >= 0 && v->his_seg > sc.maximum_history_size) return fail("more history segments than maximum_history_size");
+  // the full map with its incarnation ordinals, and the full history
+  if (const char* e = cells_section(sec(LL_LOOP_IMAGE_CELLS), len(LL_LOOP_IMAGE_CELLS), true, &v->cells)) return fail(e);
+  if (const char* e = history_section(sec(LL_LOOP_IMAGE_HISTORY), len(LL_LOOP_IMAGE_HISTORY), false, &v->his)) return fail(e);
+  if (sc.maximum_history_size >= 0 && v->his.n_seg > sc.maximum_history_size) return fail("more history segments than maximum_history_size");
   // open keyframes: their cells (cell rank, ordinal) strictly ascending and existing in the map
   {
     const uint8_t* p = sec(LL_LOOP_IMAGE_OPEN); const uint64_t L = len(LL_LOOP_IMAGE_OPEN);
@@ -562,7 +496,7 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
     if (head > L) return fail("open-keyframe section shorter than its records");
     uint64_t refs = 0;
     for (int k = 0; k < sc.n_open; k++) {
-      const ll_loop_image_open o = get<ll_loop_image_open>(p + sizeof(ll_loop_image_open) * k);
+      const ll_loop_image_open o = img_get<ll_loop_image_open>(p + sizeof(ll_loop_image_open) * k);
       if (o.frames < 0 || o.accumulate_frames < 0 || o.n_cells < 0 || (uint64_t)o.n_cells > L / 8) return fail("open keyframe out of range");
       if (o.accumulate_frames == 0 && o.n_cells > 0) return fail("open keyframe with cells but no append");
       refs += (uint64_t)o.n_cells;
@@ -570,13 +504,13 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
     if (head + sizeof(ll_loop_image_ref) * refs != L) return fail("open-keyframe cells disagree with the section length");
     const uint8_t* r = p + head;
     for (int k = 0; k < sc.n_open; k++) {
-      const int64_t n = get<ll_loop_image_open>(p + sizeof(ll_loop_image_open) * k).n_cells;
+      const int64_t n = img_get<ll_loop_image_open>(p + sizeof(ll_loop_image_open) * k).n_cells;
       for (int64_t i = 0; i < n; i++, r += 8) {
-        const ll_loop_image_ref x = get<ll_loop_image_ref>(r);
-        if (x.cell < 0 || x.cell >= v->n_cells || x.incarnation < 0 || x.incarnation > get<int32_t>(v->cur + 4 * (int64_t)x.cell))
+        const ll_loop_image_ref x = img_get<ll_loop_image_ref>(r);
+        if (x.cell < 0 || x.cell >= v->cells.n_cells || x.incarnation < 0 || x.incarnation > img_get<int32_t>(v->cells.cur + 4 * (int64_t)x.cell))
           return fail("open keyframe refers to a cell or incarnation the map does not hold");
         if (i > 0) {
-          const ll_loop_image_ref y = get<ll_loop_image_ref>(r - 8);
+          const ll_loop_image_ref y = img_get<ll_loop_image_ref>(r - 8);
           if (!(y.cell < x.cell || (y.cell == x.cell && y.incarnation < x.incarnation))) return fail("open keyframe's cells not strictly ascending");
         }
       }
@@ -591,20 +525,20 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
     v->infos = sec(LL_LOOP_IMAGE_KEYFRAMES); v->poses = sec(LL_LOOP_IMAGE_POSES); v->edges = sec(LL_LOOP_IMAGE_EDGES); v->images = sec(LL_LOOP_IMAGE_IMAGES);
     uint64_t cloud = 0;
     for (int64_t k = 0; k < K; k++) {
-      const ll_keyframe_info in = get<ll_keyframe_info>(v->infos + sizeof(ll_keyframe_info) * k);
+      const ll_keyframe_info in = img_get<ll_keyframe_info>(v->infos + sizeof(ll_keyframe_info) * k);
       if (in.cells < 0 || in.line_cells < 0 || in.plane_cells < 0 || (int64_t)in.line_cells + in.plane_cells > in.cells || in.accumulate_frames < 0 ||
           in.all_points > ((size_t)1 << 31) || in.line_points > in.all_points || in.plane_points > in.all_points - in.line_points)
         return fail("keyframe info out of range");
       if (in.cells == 0 && in.all_points != 0) return fail("keyframe info out of range");
       const float f[] = {in.center[0], in.center[1], in.center[2], in.roi_range, in.ratio_nonzero_line, in.ratio_nonzero_plane};
       for (float x : f) if (!std::isfinite(x)) return fail("non-finite keyframe info");
-      if (!finite_pose(get<ll_pose>(v->poses + sizeof(ll_pose) * k))) return fail("non-finite keyframe pose");
+      if (!finite_pose(img_get<ll_pose>(v->poses + sizeof(ll_pose) * k))) return fail("non-finite keyframe pose");
       if (k > 0) {
-        const ll_pg_edge e = get<ll_pg_edge>(v->edges + sizeof(ll_pg_edge) * (k - 1));
+        const ll_pg_edge e = img_get<ll_pg_edge>(v->edges + sizeof(ll_pg_edge) * (k - 1));
         if (e.id_begin != k - 1 || e.id_end != k || !finite_edge(e)) return fail("odometry edge out of range");
       }
       const uint8_t* im = v->images + LI_IMG * k;
-      for (size_t q = 0; q < LI_IMG / 4; q++) if (!std::isfinite(get<float>(im + 4 * q))) return fail("non-finite keyframe image");
+      for (size_t q = 0; q < LI_IMG / 4; q++) if (!std::isfinite(img_get<float>(im + 4 * q))) return fail("non-finite keyframe image");
       cloud += in.line_points + in.plane_points;
     }
     if (len(LL_LOOP_IMAGE_CLOUDS) != 16 * cloud) return fail("keyframe clouds disagree with the infos");
@@ -615,12 +549,12 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
   {
     const uint8_t* p = sec(LL_LOOP_IMAGE_ACCUMULATED); const uint64_t L = len(LL_LOOP_IMAGE_ACCUMULATED);
     if (L < LI_ACC_HEAD) return fail("accumulated section shorter than its count");
-    const int64_t n = get<int64_t>(p);
+    const int64_t n = img_get<int64_t>(p);
     if (n != K + sc.n_open - 1) return fail("accumulated clouds != closed + open keyframes - 1");
     if ((uint64_t)n > (L - LI_ACC_HEAD) / 8) return fail("accumulated counts disagree with the section length");
     int64_t prev = 0;
     for (int64_t k = 0; k < n; k++) {
-      const int64_t e = get<int64_t>(p + LI_ACC_HEAD + 8 * k);
+      const int64_t e = img_get<int64_t>(p + LI_ACC_HEAD + 8 * k);
       if (e < prev) return fail("accumulated cloud ends decreasing");
       prev = e;
     }
@@ -638,14 +572,14 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
       else {
         if (K < 2) return fail("a closed loop needs two keyframes");
         if (L != sizeof(ll_pg_edge) + sizeof(ll_pose) * (uint64_t)K) return fail("loop section disagrees with n_keyframes");
-        const ll_pg_edge e = get<ll_pg_edge>(p);
+        const ll_pg_edge e = img_get<ll_pg_edge>(p);
         if (e.id_begin < 0 || e.id_begin >= K || e.id_end < 0 || e.id_end >= K || !finite_edge(e)) return fail("loop edge out of range");
         v->n_loops = 1; v->n_opt = K;
       }
     } else {
       if (L < LI_LOOP2_HEAD) return fail("version-2 loop section shorter than its policy and count");
-      v->policy = get<ll_loop_policy>(p);
-      const int32_t nl = get<int32_t>(p + sizeof(ll_loop_policy)), pad = get<int32_t>(p + sizeof(ll_loop_policy) + 4);
+      v->policy = img_get<ll_loop_policy>(p);
+      const int32_t nl = img_get<int32_t>(p + sizeof(ll_loop_policy)), pad = img_get<int32_t>(p + sizeof(ll_loop_policy) + 4);
       if (v->policy.max_loops < 2 || v->policy.max_loops > LL_MAX_LOOPS) return fail("version-2 max_loops outside 2 ... LL_MAX_LOOPS (the default policy writes version 1)");
       if (v->policy.min_keyframes_between_loops < 0) return fail("negative min_keyframes_between_loops");
       if (pad != 0) return fail("loop section padding not zero");
@@ -653,7 +587,7 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
       if (L < LI_LOOP2_HEAD + sizeof(ll_pg_edge) * (uint64_t)nl) return fail("loop section shorter than its edges");
       int prev = -1;
       for (int k = 0; k < nl; k++) {
-        const ll_pg_edge e = get<ll_pg_edge>(p + LI_LOOP2_HEAD + sizeof(ll_pg_edge) * k);
+        const ll_pg_edge e = img_get<ll_pg_edge>(p + LI_LOOP2_HEAD + sizeof(ll_pg_edge) * k);
         if (e.id_begin < 0 || e.id_begin >= K || e.id_end < 0 || e.id_end >= K || e.id_begin == e.id_end || !finite_edge(e)) return fail("loop edge out of range");
         const int nw = edge_newest(e);
         if (k > 0 && (nw <= prev || nw - prev < v->policy.min_keyframes_between_loops)) return fail("loop edges' newest keyframes not increasing by the gap");
@@ -666,14 +600,14 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
     const size_t head = v->h.version == LL_LOOP_IMAGE_VERSION ? 0 : LI_LOOP2_HEAD;
     v->loop_edges = p + head;
     v->loop_opt = p + head + sizeof(ll_pg_edge) * (size_t)v->n_loops;
-    for (int64_t k = 0; k < v->n_opt; k++) if (!finite_pose(get<ll_pose>(v->loop_opt + sizeof(ll_pose) * k))) return fail("non-finite optimized pose");
+    for (int64_t k = 0; k < v->n_opt; k++) if (!finite_pose(img_get<ll_pose>(v->loop_opt + sizeof(ll_pose) * k))) return fail("non-finite optimized pose");
   }
   // the unread events
   {
     if (len(LL_LOOP_IMAGE_EVENTS) != sizeof(ll_loop_event) * (uint64_t)sc.n_events) return fail("events disagree with n_events");
     v->events = sec(LL_LOOP_IMAGE_EVENTS);
     for (int k = 0; k < sc.n_events; k++) {
-      const ll_loop_event e = get<ll_loop_event>(v->events + sizeof(ll_loop_event) * k);
+      const ll_loop_event e = img_get<ll_loop_event>(v->events + sizeof(ll_loop_event) * k);
       if (e.kind < LL_LOOP_KEYFRAME || e.kind > LL_LOOP_ERROR) return fail("unknown event kind");
       if (e.summary.cycles_eval || e.summary.cycles_elim || e.summary.cycles_border || e.summary.cycles_total) return fail("event with timing counters not zero");
     }
@@ -686,10 +620,8 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
     if (memcmp(&x, &v->cfg, sizeof(x)) != 0) return fail("cfg differs from the image's config in a field other than max_cells and reserve_*");
     if (const char* e = loop_cfg_error(*cfg)) return fail(std::string("cfg: ") + e);
   }
-  // ll_cellmap_append does not return from a full table: the import must never make one
-  if (load && v->n_cells > table_capacity(cfg ? cfg->max_cells : v->cfg.max_cells) / 2)
-    return fail("cell table more than half full: load with a larger max_cells", LL_ERR_CAPACITY);
-  if (v->n_pts > ((int64_t)1 << 30) || v->his_pts > INT32_MAX) return fail("more points than a map holds", LL_ERR_CAPACITY);
+  const int max_cells = cfg ? cfg->max_cells : v->cfg.max_cells;
+  if (const char* e = load_capacity(v->cells, v->his, load ? &max_cells : nullptr)) return fail(e, LL_ERR_CAPACITY);
   return LL_OK;
 }
 
@@ -698,32 +630,18 @@ int loop_restore(ll_ctx* ctx, LoopClosure* lc, const LoopView& v) {
   cudaStream_t s = ctx->stream;
   const ll_loop_image_scalars& sc = v.sc;
   const int K = sc.n_keyframes;
-  // the full map, its epochs the image's ordinals
-  std::vector<int> slot(v.n_cells);
-  LL_TRY(cm_import(ctx, lc->full, v.frame_idx, v.n_oor, v.cells, (int)v.n_cells, (int)v.n_pts, true, slot.data()));
-  // the full history, pushed segment by segment from one upload
-  {
-    float4* d = nullptr;
-    if (v.his_pts) {
-      LL_CUDA(ctx, ctx->scratch.carve([&](Carve& k) { d = k.take<float4>((size_t)v.his_pts); }));
-      LL_CUDA(ctx, cudaMemcpyAsync(d, v.his_pts_p, (size_t)v.his_pts * 16, cudaMemcpyHostToDevice, s));
-    }
-    size_t off = 0;
-    for (int64_t k = 0; k < v.his_seg; k++) {
-      const size_t n = (size_t)get<int32_t>(v.his_sizes + 4 * k);
-      LL_TRY(lc->his.push(ctx, d ? d + off : nullptr, n));
-      off += n;
-    }
-    LL_CUDA(ctx, cudaStreamSynchronize(s));   // (the scratch upload may be reallocated by the next carve)
-  }
+  // the full map, its epochs the image's ordinals, and the full history
+  std::vector<int> slot(v.cells.n_cells);
+  LL_TRY(cells_restore(ctx, lc->full, v.cells, true, slot.data()));
+  LL_TRY(history_restore(ctx, lc->his, v.his));
   // open keyframes: (cell rank, ordinal) back to (slot, epoch) of the new table
   const uint8_t* r = v.refs;
   for (int k = 0; k < sc.n_open; k++) {
-    const ll_loop_image_open o = get<ll_loop_image_open>(v.open + sizeof(ll_loop_image_open) * k);
+    const ll_loop_image_open o = img_get<ll_loop_image_open>(v.open + sizeof(ll_loop_image_open) * k);
     std::vector<unsigned long long> keys(o.n_cells), ids(o.n_cells);
     for (int64_t i = 0; i < o.n_cells; i++, r += 8) {
-      const ll_loop_image_ref x = get<ll_loop_image_ref>(r);
-      keys[i] = get<ll_image_cell>(v.cells + 16 * (int64_t)x.cell).key;
+      const ll_loop_image_ref x = img_get<ll_loop_image_ref>(r);
+      keys[i] = img_get<ll_image_cell>(v.cells.rec + 16 * (int64_t)x.cell).key;
       ids[i] = ((unsigned long long)(unsigned)slot[x.cell] << 32) | (unsigned)x.incarnation;
     }
     ll_keyframe* kf = nullptr;
@@ -734,29 +652,27 @@ int loop_restore(ll_ctx* ctx, LoopClosure* lc, const LoopView& v) {
   // closed keyframes, their poses and odometry edges
   size_t cloud = 0;
   for (int k = 0; k < K; k++) {
-    const ll_keyframe_info in = get<ll_keyframe_info>(v.infos + sizeof(ll_keyframe_info) * k);
+    const ll_keyframe_info in = img_get<ll_keyframe_info>(v.infos + sizeof(ll_keyframe_info) * k);
     ll_keyframe* kf = nullptr;
     LL_TRY(ll_keyframe_create(ctx, &kf));
     lc->kfs.push_back(kf);
     LL_TRY(kf_restore_closed(ctx, lc->full, kf, in, (const float*)(v.images + LI_IMG * k), v.clouds + 16 * cloud));
     cloud += in.line_points + in.plane_points;
-    lc->poses.push_back(get<ll_pose>(v.poses + sizeof(ll_pose) * k));
-    if (k > 0) lc->edges.push_back(get<ll_pg_edge>(v.edges + sizeof(ll_pg_edge) * (k - 1)));
+    lc->poses.push_back(img_get<ll_pose>(v.poses + sizeof(ll_pose) * k));
+    if (k > 0) lc->edges.push_back(img_get<ll_pg_edge>(v.edges + sizeof(ll_pg_edge) * (k - 1)));
   }
   // accumulated clouds
-  for (int64_t k = 0; k < v.n_acc; k++) lc->acc_end.push_back((size_t)get<int64_t>(v.acc_end + 8 * k));
+  for (int64_t k = 0; k < v.n_acc; k++) lc->acc_end.push_back((size_t)img_get<int64_t>(v.acc_end + 8 * k));
   LL_TRY(grow_keep(ctx, lc->acc, 0, (size_t)v.acc_pts * 16 + 64));
   if (v.acc_pts) LL_CUDA(ctx, cudaMemcpyAsync(lc->acc.p, v.acc, (size_t)v.acc_pts * 16, cudaMemcpyHostToDevice, s));
   // the policy, the loops and the latest loop's refined clouds, recomputed
   if (!policy_default(v.policy)) LL_TRY(loop_set_policy(ctx, lc, &v.policy));
   lc->stopped = sc.stopped != 0;
-  for (int64_t k = 0; k < v.n_loops; k++) lc->loops.push_back(get<ll_pg_edge>(v.loop_edges + sizeof(ll_pg_edge) * k));
+  for (int64_t k = 0; k < v.n_loops; k++) lc->loops.push_back(img_get<ll_pg_edge>(v.loop_edges + sizeof(ll_pg_edge) * k));
   lc->opt.resize((size_t)v.n_opt);
-  for (int64_t k = 0; k < v.n_opt; k++) lc->opt[k] = get<ll_pose>(v.loop_opt + sizeof(ll_pose) * k);
+  for (int64_t k = 0; k < v.n_opt; k++) lc->opt[k] = img_get<ll_pose>(v.loop_opt + sizeof(ll_pose) * k);
   if (v.n_loops) LL_TRY(loop_refine(ctx, lc));
-  // the unread events
-  for (int k = 0; k < sc.n_events; k++) lc->ring[k] = get<ll_loop_event>(v.events + sizeof(ll_loop_event) * k);
-  lc->first = 0; lc->count = (size_t)sc.n_events; lc->dropped = sc.n_dropped;
+  lc->log.restore(v.events, (size_t)sc.n_events, sc.n_dropped);   // the unread events
   LL_CUDA(ctx, cudaGetLastError());
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   return LL_OK;
@@ -770,13 +686,13 @@ int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& s
   // the incarnations the open keyframes hold (sorted, distinct), on the device for the export
   std::vector<std::vector<unsigned long long>> okeys(lc->open.size()), oids(lc->open.size());
   std::vector<unsigned long long> held;
-  LoopCounts n;
+  uint64_t open_cells = 0;
   for (size_t k = 0; k < lc->open.size(); k++) {
     const int c = kf_cell_count(lc->open[k].kf);
     okeys[k].resize(c); oids[k].resize(c);
     LL_TRY(kf_cell_ids(ctx, lc->open[k].kf, okeys[k].data(), oids[k].data()));
     held.insert(held.end(), oids[k].begin(), oids[k].end());
-    n.open_cells += c;
+    open_cells += c;
   }
   std::sort(held.begin(), held.end()); held.erase(std::unique(held.begin(), held.end()), held.end());
   struct Owned { DevBuf b; ~Owned() { b.release(); } } d_held;
@@ -785,25 +701,32 @@ int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& s
     LL_CUDA(ctx, cudaMemcpyAsync(d_held.b.p, held.data(), held.size() * 8, cudaMemcpyHostToDevice, s));
   }
   const CmHeld H{(const unsigned long long*)d_held.b.p, (int)held.size()};
-  int cells = 0, live = 0, frame_idx = 0, oor = 0, kept = 0;
-  LL_TRY(cm_count(ctx, lc->full, &cells, &live, &frame_idx, &oor));
+  CellsView cells; int nc = 0, live = 0, kept = 0;
+  LL_TRY(cm_count(ctx, lc->full, &nc, &live, &cells.frame_idx, &cells.n_oor));
   LL_TRY(cm_count_kept(ctx, lc->full, H, &kept));
-  n.cells = cells; n.cell_pts = kept;
-  n.his_seg = (int64_t)lc->his.segs.size(); n.his_pts = (int64_t)lc->his.live();
-  n.open = (int64_t)lc->open.size(); n.kfs = (int64_t)lc->kfs.size();
-  std::vector<ll_keyframe_info> infos(lc->kfs.size());
-  for (size_t k = 0; k < lc->kfs.size(); k++) {
+  cells.n_cells = nc; cells.n_pts = kept;
+  const size_t K = lc->kfs.size();
+  std::vector<ll_keyframe_info> infos(K);
+  uint64_t cloud_pts = 0;
+  for (size_t k = 0; k < K; k++) {
     if (ll_keyframe_get_info(lc->kfs[k], &infos[k]) != LL_OK) {   // only a keyframe whose analysis failed (LL_LOOP_ERROR) has none
       ctx->set_error("keyframe " + std::to_string(k) + " was closed by a loop closure that an error stopped and has no analysis: it cannot be saved");
       return LL_ERR_INVALID;
     }
-    n.cloud_pts += (int64_t)(infos[k].line_points + infos[k].plane_points);
+    cloud_pts += infos[k].line_points + infos[k].plane_points;
   }
-  n.acc = (int64_t)lc->acc_end.size(); n.acc_pts = lc->acc_end.empty() ? 0 : (int64_t)lc->acc_end.back();
-  n.events = (int64_t)lc->count; n.v2 = !policy_default(lc->policy);
-  n.loops = (int64_t)lc->loops.size(); n.n_opt = n.loops ? (int64_t)lc->opt.size() : 0;
+  const uint64_t acc_pts = lc->acc_end.empty() ? 0 : lc->acc_end.back();
+  // v2: a policy other than the default (version 2); n_opt: the latest optimization's keyframes
+  const bool v2 = !policy_default(lc->policy);
+  const uint64_t n_loops = lc->loops.size(), n_opt = n_loops ? lc->opt.size() : 0;
+  const uint64_t loop_len = v2 ? LI_LOOP2_HEAD + sizeof(ll_pg_edge) * n_loops + sizeof(ll_pose) * n_opt : n_loops ? sizeof(ll_pg_edge) + sizeof(ll_pose) * n_opt : 0;
+  const uint64_t len[LL_LOOP_IMAGE_SECTIONS] = {
+      sizeof(ll_loop_closure_cfg), sizeof(ll_loop_image_scalars), cells_bytes(cells, true), history_bytes(lc->his),
+      sizeof(ll_loop_image_open) * lc->open.size() + sizeof(ll_loop_image_ref) * open_cells, sizeof(ll_keyframe_info) * K, sizeof(ll_pose) * K,
+      sizeof(ll_pg_edge) * (K ? K - 1 : 0), LI_IMG * K, 16 * cloud_pts, LI_ACC_HEAD + 8 * lc->acc_end.size() + 16 * acc_pts, loop_len,
+      sizeof(ll_loop_event) * lc->log.count};
   ll_loop_image_header h;
-  const size_t total = loop_layout(n, &h);
+  const size_t total = image_header(LOOP_IMAGE, v2 ? LL_LOOP_IMAGE_VERSION_POLICY : LL_LOOP_IMAGE_VERSION, len, &h);
   *bytes = total;
   if (!image) return LL_OK;
   if (cap < total) { ctx->set_error("image buffer smaller than the loop image (query the size with image = NULL)"); return LL_ERR_CAPACITY; }
@@ -813,40 +736,34 @@ int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& s
   memcpy(at(LL_LOOP_IMAGE_CONFIG), &lc->cfg, sizeof(lc->cfg));
   ll_loop_image_scalars sc = stamp;
   sc.closed = lc->loops.empty() ? 0 : 1; sc.stopped = lc->stopped ? 1 : 0;
-  sc.n_keyframes = (int32_t)n.kfs; sc.n_open = (int32_t)n.open; sc.n_events = (int32_t)n.events; sc.n_dropped = lc->dropped;
+  sc.n_keyframes = (int32_t)K; sc.n_open = (int32_t)lc->open.size(); sc.n_events = (int32_t)lc->log.count; sc.n_dropped = lc->log.dropped;
   memcpy(at(LL_LOOP_IMAGE_SCALARS), &sc, sizeof(sc));
-  // the full map with the held incarnations
-  uint8_t* p = at(LL_LOOP_IMAGE_CELLS);
-  put<int32_t>(p, frame_idx); put<int32_t>(p + 4, oor); put<int64_t>(p + 8, n.cells); put<int64_t>(p + 16, n.cell_pts);
-  LL_TRY(cm_export(ctx, lc->full, cells, kept, p + LI_CELLS_HEAD, &H));
-  const uint8_t* ecells = p + LI_CELLS_HEAD;
-  // the full history
-  p = at(LL_LOOP_IMAGE_HISTORY);
-  put<int64_t>(p, n.his_seg); put<int64_t>(p + 8, n.his_pts); p += LI_HIS_HEAD;
-  for (const auto& sg : lc->his.segs) { put<int32_t>(p, (int32_t)sg.second); p += 4; }
-  if (n.his_pts) LL_CUDA(ctx, cudaMemcpyAsync(p, lc->his.data(), (size_t)n.his_pts * 16, cudaMemcpyDeviceToHost, s));
+  // the full map with the held incarnations, the full history
+  LL_TRY(cells_write(ctx, lc->full, cells, at(LL_LOOP_IMAGE_CELLS), &H));
+  const uint8_t* ecells = at(LL_LOOP_IMAGE_CELLS) + CELLS_HEAD;
+  LL_TRY(history_write(ctx, lc->his, at(LL_LOOP_IMAGE_HISTORY)));
   // open keyframes: (slot, epoch) as (cell rank by key, ordinal)
-  p = at(LL_LOOP_IMAGE_OPEN);
+  uint8_t* p = at(LL_LOOP_IMAGE_OPEN);
   uint8_t* refs = p + sizeof(ll_loop_image_open) * lc->open.size();
   for (size_t k = 0; k < lc->open.size(); k++) {
     ll_loop_image_open o; memset(&o, 0, sizeof(o));
     o.frames = lc->open[k].frames; o.accumulate_frames = (int32_t)kf_accumulate_frames(lc->open[k].kf); o.n_cells = (int64_t)okeys[k].size();
-    put(p + sizeof(o) * k, o);
+    img_put(p + sizeof(o) * k, o);
     for (size_t i = 0; i < okeys[k].size(); i++, refs += 8) {
-      int lo = 0, hi = cells;   // the cell's rank: its key in the exported list
-      while (lo < hi) { const int mid = (lo + hi) >> 1; if (get<ll_image_cell>(ecells + 16 * (size_t)mid).key < okeys[k][i]) lo = mid + 1; else hi = mid; }
+      int lo = 0, hi = (int)cells.n_cells;   // the cell's rank: its key in the exported list
+      while (lo < hi) { const int mid = (lo + hi) >> 1; if (img_get<ll_image_cell>(ecells + 16 * (size_t)mid).key < okeys[k][i]) lo = mid + 1; else hi = mid; }
       ll_loop_image_ref x; x.cell = lo;
       x.incarnation = cm_ordinal(held.data(), (int)held.size(), (int)(oids[k][i] >> 32), (int)(unsigned)(oids[k][i] & 0xffffffffull));
-      put(refs, x);
+      img_put(refs, x);
     }
   }
   // closed keyframes
   size_t cloud = 0;
   uint8_t* clouds = at(LL_LOOP_IMAGE_CLOUDS);
-  for (size_t k = 0; k < lc->kfs.size(); k++) {
-    put(at(LL_LOOP_IMAGE_KEYFRAMES) + sizeof(ll_keyframe_info) * k, infos[k]);
-    put(at(LL_LOOP_IMAGE_POSES) + sizeof(ll_pose) * k, lc->poses[k]);
-    if (k > 0) put(at(LL_LOOP_IMAGE_EDGES) + sizeof(ll_pg_edge) * (k - 1), lc->edges[k - 1]);
+  for (size_t k = 0; k < K; k++) {
+    img_put(at(LL_LOOP_IMAGE_KEYFRAMES) + sizeof(ll_keyframe_info) * k, infos[k]);
+    img_put(at(LL_LOOP_IMAGE_POSES) + sizeof(ll_pose) * k, lc->poses[k]);
+    if (k > 0) img_put(at(LL_LOOP_IMAGE_EDGES) + sizeof(ll_pg_edge) * (k - 1), lc->edges[k - 1]);
     float* im = (float*)(at(LL_LOOP_IMAGE_IMAGES) + LI_IMG * k);
     LL_TRY(ll_keyframe_images(ctx, lc->kfs[k], im, im + 3600, im + 2 * 3600, im + 3 * 3600));
     size_t nl = 0, np = 0;
@@ -856,24 +773,24 @@ int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& s
   }
   // accumulated clouds
   p = at(LL_LOOP_IMAGE_ACCUMULATED);
-  put<int64_t>(p, n.acc);
-  for (size_t k = 0; k < lc->acc_end.size(); k++) put<int64_t>(p + LI_ACC_HEAD + 8 * k, (int64_t)lc->acc_end[k]);
-  if (n.acc_pts) LL_CUDA(ctx, cudaMemcpyAsync(p + LI_ACC_HEAD + 8 * n.acc, lc->acc.p, (size_t)n.acc_pts * 16, cudaMemcpyDeviceToHost, s));
+  img_put<int64_t>(p, (int64_t)lc->acc_end.size());
+  for (size_t k = 0; k < lc->acc_end.size(); k++) img_put<int64_t>(p + LI_ACC_HEAD + 8 * k, (int64_t)lc->acc_end[k]);
+  if (acc_pts) LL_CUDA(ctx, cudaMemcpyAsync(p + LI_ACC_HEAD + 8 * lc->acc_end.size(), lc->acc.p, (size_t)acc_pts * 16, cudaMemcpyDeviceToHost, s));
   // the loop: version 1 the edge of the one loop, version 2 the policy and every loop edge; then the optimized poses
   p = at(LL_LOOP_IMAGE_LOOP);
-  if (n.v2) {
-    put(p, lc->policy); put<int32_t>(p + sizeof(ll_loop_policy), (int32_t)n.loops); put<int32_t>(p + sizeof(ll_loop_policy) + 4, 0);
+  if (v2) {
+    img_put(p, lc->policy); img_put<int32_t>(p + sizeof(ll_loop_policy), (int32_t)n_loops); img_put<int32_t>(p + sizeof(ll_loop_policy) + 4, 0);
     p += LI_LOOP2_HEAD;
   }
-  if (n.loops) {
+  if (n_loops) {
     memcpy(p, lc->loops.data(), sizeof(ll_pg_edge) * lc->loops.size());
-    memcpy(p + sizeof(ll_pg_edge) * lc->loops.size(), lc->opt.data(), sizeof(ll_pose) * (size_t)n.n_opt);
+    memcpy(p + sizeof(ll_pg_edge) * lc->loops.size(), lc->opt.data(), sizeof(ll_pose) * (size_t)n_opt);
   }
   // the unread events, oldest first
-  for (size_t k = 0; k < lc->count; k++) {   // the pose graph's SM clock counters time the solve: not state, saved as 0
-    ll_loop_event e = lc->ring[(lc->first + k) % lc->ring.size()];
+  for (size_t k = 0; k < lc->log.count; k++) {   // the pose graph's SM clock counters time the solve: not state, saved as 0
+    ll_loop_event e = lc->log.at(k);
     e.summary.cycles_eval = e.summary.cycles_elim = e.summary.cycles_border = e.summary.cycles_total = 0;
-    put(at(LL_LOOP_IMAGE_EVENTS) + sizeof(ll_loop_event) * k, e);
+    img_put(at(LL_LOOP_IMAGE_EVENTS) + sizeof(ll_loop_event) * k, e);
   }
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   return LL_OK;
@@ -906,10 +823,10 @@ int loop_image_info(const void* image, size_t bytes, ll_loop_image_summary* info
   LL_TRY(loop_validate(image, bytes, false, nullptr, &v, nullptr));
   memset(info, 0, sizeof(*info));
   info->bytes = bytes; info->version = v.h.version;
-  info->cells = v.n_cells; info->cell_points = v.n_pts; info->replaced_points = v.replaced;
-  info->history_points = v.his_pts; info->cloud_points = v.cloud_pts; info->accumulated_points = v.acc_pts;
+  info->cells = v.cells.n_cells; info->cell_points = v.cells.n_pts; info->replaced_points = v.cells.replaced;
+  info->history_points = v.his.n_pts; info->cloud_points = v.cloud_pts; info->accumulated_points = v.acc_pts;
   info->frame_index = v.sc.frame_index; info->matching_mode = v.sc.matching_mode; info->closed = v.sc.closed; info->stopped = v.sc.stopped;
   info->keyframes = v.sc.n_keyframes; info->open_keyframes = v.sc.n_open; info->events = v.sc.n_events; info->dropped = v.sc.n_dropped;
-  info->max_incarnation = v.max_cur;
+  info->max_incarnation = v.cells.max_cur;
   return LL_OK;
 }

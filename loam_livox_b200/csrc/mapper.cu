@@ -31,8 +31,8 @@ struct Recovery {
   ll_reloc_field* field = nullptr;
   ll_map* whole = nullptr;            // mode 1: the whole map, rebuilt in place once per episode
   DevBuf buf;                         // the step's features and the score points of each class (RecoveryLayout)
-  std::vector<ll_recovery_step> ring; size_t first = 0, count = 0; int dropped = 0;   // the log: count entries from ring[first]
-  size_t cur = 0;                     // the ring slot of the current step's entry
+  EventLog<ll_recovery_step> log;
+  ll_recovery_step* cur = nullptr;    // the current step's entry
   // the last attempt's inputs (the parity hook): host copies of the rotations and cfgs, the device features and score points in buf
   bool have_last = false;
   std::vector<double> rot_c, rot_f;
@@ -284,7 +284,7 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
     fprintf(stderr, "ll_mapper trace: frame %d append %.2f ms = features %.2f + history %.2f + cells %.2f + %.2f\n", m->frame_index, now_ms() - tp, tr0 - tp, tr1 - tr0, tr2 - tr1, now_ms() - tr2);
   m->map_dirty = true;                                                           // m_if_mapping_updated_* (:1490-1491)
   if (stats) { stats->appended_corner = hc[0]; stats->appended_surf = hc[1]; stats->ms_append = (float)(now_ms() - tp); }
-  if (m->rec.on) m->rec.ring[m->rec.cur].appended = 1;
+  if (m->rec.on) m->rec.cur->appended = 1;
   for (int k = 0; k < 4; k++) m->q_w_curr[k] = out->q_w_curr[k]; for (int k = 0; k < 3; k++) m->t_w_curr[k] = out->t_w_curr[k];   // :1496-1505
   if (m->lc) LL_TRY(loop_step(ctx, m->lc, d_pose, pushed, m->frame_index, m->q_w_curr, m->t_w_curr));   // :1523-1564
   return LL_OK;
@@ -577,90 +577,22 @@ extern "C" int ll_mapper_process_sweeps(ll_mapper* m, ll_spin* spin, int n_sweep
 // One host validator serves ll_mapper_image_info and ll_mapper_load, before anything touches the device.
 namespace {
 
-template <typename T> T rd(const uint8_t* p) { T v; memcpy(&v, p, sizeof(T)); return v; }
-template <typename T> void wr(uint8_t* p, const T& v) { memcpy(p, &v, sizeof(T)); }
-
-const size_t HIS_HEAD = 16, SNAP_HEAD = 8, CELLS_HEAD = 24;   // the fixed part of a history, snapshot and cell-map section
+const ImageKind MAPPER_IMAGE{LL_MAPPER_IMAGE_MAGIC, "mapper", LL_MAPPER_IMAGE_VERSION, LL_MAPPER_IMAGE_VERSION, sizeof(ll_mapper_config), "ll_mapper_config",
+                             LL_IMAGE_SECTIONS};
+const size_t SNAP_HEAD = 8;   // the fixed part of a snapshot section
 
 struct ImageView {   // a validated image
   ll_mapper_image_header h; ll_mapper_config cfg; ll_mapper_image_scalars sc;
-  struct { int64_t n_seg = 0, n_pts = 0; const uint8_t* sizes = nullptr; const uint8_t* pts = nullptr; } his[2];
+  HistoryView his[2];
   struct { int64_t n = 0; const uint8_t* pts = nullptr; } snap[2];
-  struct { int32_t frame_idx = 0, n_oor = 0; int64_t n_cells = 0, n_pts = 0; const uint8_t* rec = nullptr; } cells[2];
+  CellsView cells[2];
 };
-struct ImageCounts { int64_t his_seg[2], his_pts[2], snap[2], cells[2], cell_pts[2]; };
-
-// The canonical placement: the sections back to back after the header, in index order.  Returns the image's size.
-size_t image_layout(const ImageCounts& n, ll_mapper_image_header* h) {
-  memset(h, 0, sizeof(*h));
-  memcpy(h->magic, LL_MAPPER_IMAGE_MAGIC, 8); h->version = LL_MAPPER_IMAGE_VERSION; h->config_bytes = sizeof(ll_mapper_config);
-  const uint64_t len[LL_IMAGE_SECTIONS] = {sizeof(ll_mapper_config), sizeof(ll_mapper_image_scalars),
-                                           HIS_HEAD + 4 * (uint64_t)n.his_seg[0] + 16 * (uint64_t)n.his_pts[0], HIS_HEAD + 4 * (uint64_t)n.his_seg[1] + 16 * (uint64_t)n.his_pts[1],
-                                           SNAP_HEAD + 16 * (uint64_t)n.snap[0], SNAP_HEAD + 16 * (uint64_t)n.snap[1],
-                                           CELLS_HEAD + 16 * (uint64_t)(n.cells[0] + n.cell_pts[0]), CELLS_HEAD + 16 * (uint64_t)(n.cells[1] + n.cell_pts[1])};
-  uint64_t off = sizeof(*h);
-  for (int k = 0; k < LL_IMAGE_SECTIONS; k++) { h->section[k].offset = off; h->section[k].length = len[k]; off += len[k]; }
-  h->total_bytes = off;
-  return (size_t)off;
-}
-
-}  // namespace
-
-bool finite_xyz(const uint8_t* p) { float v[3]; memcpy(v, p, 12); return std::isfinite(v[0]) && std::isfinite(v[1]) && std::isfinite(v[2]); }
-int64_t table_capacity(int max_cells) { int64_t cap = 1 << 12; const int64_t want = 2 * (int64_t)(max_cells > 0 ? max_cells : (1 << 20)); while (cap < want) cap <<= 1; return cap; }
-
-int image_structure(const void* image, size_t bytes, const ImageKind& kind, ll_image_section* sec, std::string* err) {
-  auto fail = [&](const std::string& msg) { if (err) *err = msg; return LL_ERR_INVALID; };
-  const uint8_t* b = (const uint8_t*)image;
-  const size_t head = 24 + 16 * (size_t)kind.sections;
-  if (!b || bytes < head) return fail("shorter than the image header");
-  char magic[8]; uint32_t version, config_bytes; uint64_t total;
-  memcpy(magic, b, 8); memcpy(&version, b + 8, 4); memcpy(&config_bytes, b + 12, 4); memcpy(&total, b + 16, 8);
-  memcpy(sec, b + 24, 16 * (size_t)kind.sections);
-  if (memcmp(magic, kind.magic, 8) != 0) return fail(std::string("not a ") + kind.name + " image (magic)");
-  if (version < kind.version || version > kind.max_version) return fail("unknown image version");
-  if (config_bytes != kind.config_bytes) return fail(std::string("config size differs from this library's ") + kind.config_name);
-  if (total != bytes) return fail("image size differs from the header's total_bytes");
-  // every section inside the image after the header, no two overlapping
-  std::vector<int> order(kind.sections);
-  for (int k = 0; k < kind.sections; k++) {
-    const ll_image_section& s = sec[k];
-    if (s.offset < head || s.offset > bytes || s.length > bytes - s.offset) return fail("section outside the image");
-    order[k] = k;
-  }
-  std::sort(order.begin(), order.end(), [&](int a, int c) {
-    const ll_image_section &x = sec[a], &y = sec[c];
-    return x.offset != y.offset ? x.offset < y.offset : x.length < y.length;
-  });
-  for (int k = 1; k < kind.sections; k++) {
-    const ll_image_section &p = sec[order[k - 1]], &q = sec[order[k]];
-    if (p.offset + p.length > q.offset) return fail("overlapping sections");
-  }
-  return LL_OK;
-}
-
-const char* history_section(const uint8_t* p, uint64_t L, bool finite, int64_t* n_seg, int64_t* n_pts, const uint8_t** sizes, const uint8_t** pts) {
-  if (L < HIS_HEAD) return "history section shorter than its counts";
-  const int64_t ns = rd<int64_t>(p), np = rd<int64_t>(p + 8);
-  if (ns < 0 || np < 0 || (uint64_t)ns > (L - HIS_HEAD) / 4 || (uint64_t)np > (L - HIS_HEAD) / 16 || HIS_HEAD + 4 * (uint64_t)ns + 16 * (uint64_t)np != L)
-    return "history counts disagree with the section length";
-  int64_t sum = 0;
-  for (int64_t k = 0; k < ns; k++) { const int32_t z = rd<int32_t>(p + HIS_HEAD + 4 * k); if (z < 0) return "negative history segment size"; sum += z; }
-  if (sum != np) return "history segment sizes do not sum to its points";
-  const uint8_t* q = p + HIS_HEAD + 4 * ns;
-  if (finite) for (int64_t k = 0; k < np; k++) if (!finite_xyz(q + 16 * k)) return "non-finite history point";
-  *n_seg = ns; *n_pts = np; *sizes = p + HIS_HEAD; *pts = q;
-  return nullptr;
-}
-
-namespace {
 
 // LL_OK, or the code and what is wrong.  cfg: the caller's config for a load (NULL: the image's).
 int image_validate(const void* image, size_t bytes, const ll_mapper_config* cfg, ImageView* v, std::string* err) {
   auto fail = [&](const char* msg, int code = LL_ERR_INVALID) { if (err) *err = msg; return code; };
   const uint8_t* b = (const uint8_t*)image;
-  static const ImageKind kind{LL_MAPPER_IMAGE_MAGIC, "mapper", LL_MAPPER_IMAGE_VERSION, LL_MAPPER_IMAGE_VERSION, sizeof(ll_mapper_config), "ll_mapper_config", LL_IMAGE_SECTIONS};
-  LL_TRY(image_structure(image, bytes, kind, v->h.section, err));
+  LL_TRY(image_structure(image, bytes, MAPPER_IMAGE, v->h.section, err));
   memcpy(&v->h, b, sizeof(v->h));
   auto sec = [&](int k) { return b + v->h.section[k].offset; };
   auto len = [&](int k) { return (uint64_t)v->h.section[k].length; };
@@ -668,61 +600,32 @@ int image_validate(const void* image, size_t bytes, const ll_mapper_config* cfg,
   if (len(LL_IMAGE_CONFIG) != sizeof(ll_mapper_config)) return fail("config section length");
   memcpy(&v->cfg, sec(LL_IMAGE_CONFIG), sizeof(v->cfg));
   if (!(v->cfg.cell_resolution > 0.f) || v->cfg.threshold_cell_revisit < 1) return fail("config: cell_resolution must be > 0 and threshold_cell_revisit >= 1");
+  if (v->cfg.max_cells > MAX_CELLS) return fail("config: max_cells must be <= 2^29");
   if (v->cfg.matching_mode != 0 && v->cfg.matching_mode != 1) return fail("config: matching_mode must be 0 or 1");
   // scalars
   if (len(LL_IMAGE_SCALARS) != sizeof(ll_mapper_image_scalars)) return fail("scalars section length");
   memcpy(&v->sc, sec(LL_IMAGE_SCALARS), sizeof(v->sc));
   const ll_mapper_image_scalars& sc = v->sc;
-  {
-    const double d[] = {sc.last_time_stamp, sc.q_w_curr[0], sc.q_w_curr[1], sc.q_w_curr[2], sc.q_w_curr[3], sc.t_w_curr[0], sc.t_w_curr[1], sc.t_w_curr[2],
-                        sc.last_his_add_q[0], sc.last_his_add_q[1], sc.last_his_add_q[2], sc.last_his_add_q[3], sc.last_his_add_t[0], sc.last_his_add_t[1], sc.last_his_add_t[2],
-                        sc.first_receive_time, sc.current_time, sc.last_maximum_time_stamp};
-    for (double x : d) if (!std::isfinite(x)) return fail("non-finite pose or time stamp");
-  }
+  const double times[] = {sc.last_time_stamp, sc.first_receive_time, sc.current_time, sc.last_maximum_time_stamp};
+  if (!finite_d(times, 4) || !finite_d(sc.q_w_curr, 4) || !finite_d(sc.t_w_curr, 3) || !finite_d(sc.last_his_add_q, 4) || !finite_d(sc.last_his_add_t, 3))
+    return fail("non-finite pose or time stamp");
   if (sc.frame_index < 0 || (sc.map_dirty != 0 && sc.map_dirty != 1) || (sc.have_map != 0 && sc.have_map != 1) || sc.reserved != 0 ||
       sc.snap_n[0] < 0 || sc.snap_n[1] < 0 || sc.fov[0] < 0 || sc.fov[1] < 0)
     return fail("scalars out of range");
   if (sc.have_map && (sc.snap_n[0] == 0 || sc.snap_n[1] == 0)) return fail("have_map with an empty snapshot");
   for (int c = 0; c < 2; c++) {
-    // history window: counts x element sizes = the length, segment sizes summing to the points, finite points
-    if (const char* e = history_section(sec(LL_IMAGE_HISTORY_CORNER + c), len(LL_IMAGE_HISTORY_CORNER + c), true, &v->his[c].n_seg, &v->his[c].n_pts, &v->his[c].sizes, &v->his[c].pts))
-      return fail(e);
+    if (const char* e = history_section(sec(LL_IMAGE_HISTORY_CORNER + c), len(LL_IMAGE_HISTORY_CORNER + c), true, &v->his[c])) return fail(e);
     // snapshot: as many points as snap_n when the index exists, none otherwise
     {
       const uint8_t* p = sec(LL_IMAGE_SNAPSHOT_CORNER + c); const uint64_t L = len(LL_IMAGE_SNAPSHOT_CORNER + c);
       if (L < SNAP_HEAD) return fail("snapshot section shorter than its count");
-      const int64_t n = rd<int64_t>(p);
+      const int64_t n = img_get<int64_t>(p);
       if (n < 0 || (uint64_t)n > (L - SNAP_HEAD) / 16 || SNAP_HEAD + 16 * (uint64_t)n != L) return fail("snapshot count disagrees with the section length");
       if (n != (sc.have_map ? sc.snap_n[c] : 0)) return fail("snapshot disagrees with have_map / snap_n");
       for (int64_t k = 0; k < n; k++) if (!finite_xyz(p + SNAP_HEAD + 16 * k)) return fail("non-finite snapshot point");
       v->snap[c].n = n; v->snap[c].pts = p + SNAP_HEAD;
     }
-    // cell map: keys strictly ascending with bit 63 clear, stamps <= current_frame_idx, ranks < the cell count, finite points
-    {
-      const uint8_t* p = sec(LL_IMAGE_CELLS_CORNER + c); const uint64_t L = len(LL_IMAGE_CELLS_CORNER + c);
-      if (L < CELLS_HEAD) return fail("cell-map section shorter than its counts");
-      const int32_t fi = rd<int32_t>(p), oor = rd<int32_t>(p + 4);
-      const int64_t nc = rd<int64_t>(p + 8), np = rd<int64_t>(p + 16);
-      if (nc < 0 || np < 0 || (uint64_t)nc > (L - CELLS_HEAD) / 16 || (uint64_t)np > (L - CELLS_HEAD) / 16 || CELLS_HEAD + 16 * (uint64_t)(nc + np) != L)
-        return fail("cell-map counts disagree with the section length");
-      if (fi < 0 || oor < 0) return fail("cell-map frame index or out-of-range count negative");
-      const uint8_t* cells = p + CELLS_HEAD;
-      uint64_t prev = 0;
-      for (int64_t k = 0; k < nc; k++) {
-        const ll_image_cell e = rd<ll_image_cell>(cells + 16 * k);
-        if (e.key >> 63) return fail("cell key with bit 63 set");
-        if (k > 0 && e.key <= prev) return fail("cell keys not strictly ascending");
-        if (e.create_frame < 0 || e.create_frame > fi || e.last_update < 0 || e.last_update > fi) return fail("cell stamp outside 0 ... current_frame_idx");
-        prev = e.key;
-      }
-      const uint8_t* pts = cells + 16 * nc;
-      for (int64_t k = 0; k < np; k++) {
-        const ll_image_cell_point q = rd<ll_image_cell_point>(pts + 16 * k);
-        if (!(std::isfinite(q.x) && std::isfinite(q.y) && std::isfinite(q.z))) return fail("non-finite cell-map point");
-        if (q.cell < 0 || q.cell >= nc) return fail("cell-map point's cell rank >= the cell count");
-      }
-      v->cells[c].frame_idx = fi; v->cells[c].n_oor = oor; v->cells[c].n_cells = nc; v->cells[c].n_pts = np; v->cells[c].rec = cells;
-    }
+    if (const char* e = cells_section(sec(LL_IMAGE_CELLS_CORNER + c), len(LL_IMAGE_CELLS_CORNER + c), false, &v->cells[c])) return fail(e);
   }
   // the caller's config: the image's but for the buffer sizes
   if (cfg) {
@@ -730,10 +633,10 @@ int image_validate(const void* image, size_t bytes, const ll_mapper_config* cfg,
     x.max_cells = v->cfg.max_cells; x.reserve_map_points = v->cfg.reserve_map_points; x.reserve_store_points = v->cfg.reserve_store_points;
     if (memcmp(&x, &v->cfg, sizeof(x)) != 0) return fail("cfg differs from the image's config in a field other than max_cells, reserve_map_points, reserve_store_points");
   }
-  const int64_t cap = table_capacity(cfg ? cfg->max_cells : v->cfg.max_cells);
+  const int max_cells = cfg ? cfg->max_cells : v->cfg.max_cells;
   for (int c = 0; c < 2; c++) {
-    if (v->cells[c].n_cells > cap / 2) return fail("cell table more than half full: create the map with a larger max_cells", LL_ERR_CAPACITY);
-    if (v->cells[c].n_pts > ((int64_t)1 << 30) || v->his[c].n_pts > INT32_MAX || v->snap[c].n > INT32_MAX) return fail("more points than a map holds", LL_ERR_CAPACITY);
+    if (const char* e = load_capacity(v->cells[c], v->his[c], &max_cells)) return fail(e, LL_ERR_CAPACITY);
+    if (v->snap[c].n > INT32_MAX) return fail("more points than a map holds", LL_ERR_CAPACITY);
   }
   return LL_OK;
 }
@@ -749,26 +652,10 @@ int mapper_restore(ll_mapper* m, const ImageView& v) {
   m->map_dirty = sc.map_dirty != 0;
   for (int c = 0; c < 2; c++) { m->snap_n[c] = sc.snap_n[c]; m->fov[c] = sc.fov[c]; }
   ctx->ex.first_receive_time = sc.first_receive_time; ctx->ex.current_time = sc.current_time; ctx->ex.last_maximum_time_stamp = sc.last_maximum_time_stamp;
-  // the history window, pushed segment by segment from one upload
   HistoryWindow* his[2] = {&m->his_corner, &m->his_surf};
-  for (int c = 0; c < 2; c++) {
-    float4* d = nullptr;
-    const size_t np = (size_t)v.his[c].n_pts;
-    if (np) {
-      LL_CUDA(ctx, ctx->scratch.carve([&](Carve& k) { d = k.take<float4>(np); }));
-      LL_CUDA(ctx, cudaMemcpyAsync(d, v.his[c].pts, np * 16, cudaMemcpyHostToDevice, s));
-    }
-    size_t off = 0;
-    for (int64_t k = 0; k < v.his[c].n_seg; k++) {
-      const size_t n = (size_t)rd<int32_t>(v.his[c].sizes + 4 * k);
-      LL_TRY(his[c]->push(ctx, d ? d + off : nullptr, n));
-      off += n;
-    }
-    LL_CUDA(ctx, cudaStreamSynchronize(s));   // (the scratch upload may be reallocated by the next carve)
-  }
-  // both cell maps
+  for (int c = 0; c < 2; c++) LL_TRY(history_restore(ctx, *his[c], v.his[c]));
   ll_cellmap* cm[2] = {m->cells_corner, m->cells_surf};
-  for (int c = 0; c < 2; c++) LL_TRY(cm_import(ctx, cm[c], v.cells[c].frame_idx, v.cells[c].n_oor, v.cells[c].rec, (int)v.cells[c].n_cells, (int)v.cells[c].n_pts));
+  for (int c = 0; c < 2; c++) LL_TRY(cells_restore(ctx, cm[c], v.cells[c], false));
   // the snapshot and its index (the build is deterministic: the kNN answers are the saved mapper's)
   m->have_map = false;
   if (sc.have_map) {
@@ -793,23 +680,26 @@ extern "C" int ll_mapper_save(ll_mapper* m, void* image, size_t cap, size_t* byt
   HistoryWindow* his[2] = {&m->his_corner, &m->his_surf};
   ll_cellmap* cm[2] = {m->cells_corner, m->cells_surf};
   const BucketTree* snap[2] = {&m->match_map->corner, &m->match_map->surf};
-  ImageCounts n; int frame_idx[2], oor[2];
+  int64_t n_snap[2]; CellsView cells[2];
   for (int c = 0; c < 2; c++) {
-    n.his_seg[c] = (int64_t)his[c]->segs.size(); n.his_pts[c] = (int64_t)his[c]->live();
-    n.snap[c] = m->have_map ? snap[c]->n_src : 0;
-    if (m->have_map && n.snap[c] != m->snap_n[c]) { ctx->set_error("match-map index and snapshot disagree"); return LL_ERR_INVALID; }
-    int cells = 0, live = 0;
-    LL_TRY(cm_count(ctx, cm[c], &cells, &live, &frame_idx[c], &oor[c]));
-    n.cells[c] = cells; n.cell_pts[c] = live;
+    n_snap[c] = m->have_map ? snap[c]->n_src : 0;
+    if (m->have_map && n_snap[c] != m->snap_n[c]) { ctx->set_error("match-map index and snapshot disagree"); return LL_ERR_INVALID; }
+    int nc = 0, live = 0;
+    LL_TRY(cm_count(ctx, cm[c], &nc, &live, &cells[c].frame_idx, &cells[c].n_oor));
+    cells[c].n_cells = nc; cells[c].n_pts = live;
   }
+  const uint64_t len[LL_IMAGE_SECTIONS] = {sizeof(ll_mapper_config), sizeof(ll_mapper_image_scalars), history_bytes(*his[0]), history_bytes(*his[1]),
+                                           SNAP_HEAD + 16 * (uint64_t)n_snap[0], SNAP_HEAD + 16 * (uint64_t)n_snap[1], cells_bytes(cells[0], false),
+                                           cells_bytes(cells[1], false)};
   ll_mapper_image_header h;
-  const size_t total = image_layout(n, &h);
+  const size_t total = image_header(MAPPER_IMAGE, LL_MAPPER_IMAGE_VERSION, len, &h);
   *bytes = total;
   if (!image) return LL_OK;
   if (cap < total) { ctx->set_error("image buffer smaller than the image (query the size with image = NULL)"); return LL_ERR_CAPACITY; }
   uint8_t* b = (uint8_t*)image;
+  auto at = [&](int k) { return b + h.section[k].offset; };
   memcpy(b, &h, sizeof(h));
-  memcpy(b + h.section[LL_IMAGE_CONFIG].offset, &m->cfg, sizeof(m->cfg));
+  memcpy(at(LL_IMAGE_CONFIG), &m->cfg, sizeof(m->cfg));
   ll_mapper_image_scalars sc; memset(&sc, 0, sizeof(sc));
   sc.frame_index = m->frame_index; sc.map_dirty = m->map_dirty ? 1 : 0; sc.have_map = m->have_map ? 1 : 0;
   for (int c = 0; c < 2; c++) { sc.snap_n[c] = m->snap_n[c]; sc.fov[c] = m->fov[c]; }
@@ -817,18 +707,13 @@ extern "C" int ll_mapper_save(ll_mapper* m, void* image, size_t cap, size_t* byt
   for (int k = 0; k < 4; k++) { sc.q_w_curr[k] = m->q_w_curr[k]; sc.last_his_add_q[k] = m->last_his_add_q[k]; }
   for (int k = 0; k < 3; k++) { sc.t_w_curr[k] = m->t_w_curr[k]; sc.last_his_add_t[k] = m->last_his_add_t[k]; }
   sc.first_receive_time = ctx->ex.first_receive_time; sc.current_time = ctx->ex.current_time; sc.last_maximum_time_stamp = ctx->ex.last_maximum_time_stamp;
-  memcpy(b + h.section[LL_IMAGE_SCALARS].offset, &sc, sizeof(sc));
+  memcpy(at(LL_IMAGE_SCALARS), &sc, sizeof(sc));
   for (int c = 0; c < 2; c++) {
-    uint8_t* p = b + h.section[LL_IMAGE_HISTORY_CORNER + c].offset;
-    wr<int64_t>(p, n.his_seg[c]); wr<int64_t>(p + 8, n.his_pts[c]); p += HIS_HEAD;
-    for (const auto& sg : his[c]->segs) { wr<int32_t>(p, (int32_t)sg.second); p += 4; }
-    if (n.his_pts[c]) LL_CUDA(ctx, cudaMemcpyAsync(p, his[c]->data(), (size_t)n.his_pts[c] * 16, cudaMemcpyDeviceToHost, s));
-    p = b + h.section[LL_IMAGE_SNAPSHOT_CORNER + c].offset;
-    wr<int64_t>(p, n.snap[c]);
-    if (n.snap[c]) LL_CUDA(ctx, cudaMemcpyAsync(p + SNAP_HEAD, snap[c]->src, (size_t)n.snap[c] * 16, cudaMemcpyDeviceToHost, s));
-    p = b + h.section[LL_IMAGE_CELLS_CORNER + c].offset;
-    wr<int32_t>(p, frame_idx[c]); wr<int32_t>(p + 4, oor[c]); wr<int64_t>(p + 8, n.cells[c]); wr<int64_t>(p + 16, n.cell_pts[c]);
-    LL_TRY(cm_export(ctx, cm[c], (int)n.cells[c], (int)n.cell_pts[c], p + CELLS_HEAD));
+    LL_TRY(history_write(ctx, *his[c], at(LL_IMAGE_HISTORY_CORNER + c)));
+    uint8_t* p = at(LL_IMAGE_SNAPSHOT_CORNER + c);
+    img_put<int64_t>(p, n_snap[c]);
+    if (n_snap[c]) LL_CUDA(ctx, cudaMemcpyAsync(p + SNAP_HEAD, snap[c]->src, (size_t)n_snap[c] * 16, cudaMemcpyDeviceToHost, s));
+    LL_TRY(cells_write(ctx, cm[c], cells[c], at(LL_IMAGE_CELLS_CORNER + c)));
   }
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   return LL_OK;
@@ -1089,10 +974,7 @@ static int recovery_attempt(ll_mapper* m, int nc, int ns, const ll_reg_state& st
 static int recovery_step(ll_mapper* m, int nc, int ns, const ll_reg_state& st, const ll_reg_result* out, bool* hold) {
   Recovery& R = m->rec;
   const ll_recovery_cfg& c = R.cfg;
-  if (R.count == R.ring.size()) { R.first = (R.first + 1) % R.ring.size(); R.count--; R.dropped++; }   // the oldest unread entry is overwritten
-  R.cur = (R.first + R.count) % R.ring.size(); R.count++;
-  ll_recovery_step* e = &R.ring[R.cur];
-  memset(e, 0, sizeof(*e));
+  ll_recovery_step* e = R.cur = R.log.push();
   e->frame_index = st.current_frame_index; e->state_before = R.state; e->best = -1;
   for (int k = 0; k < 4; k++) e->q_wxyz[k] = m->q_w_curr[k];
   for (int k = 0; k < 3; k++) e->t[k] = m->t_w_curr[k];
@@ -1156,20 +1038,14 @@ int ll_mapper_set_recovery(ll_mapper* m, const ll_recovery_cfg* cfg) {
     LL_CUDA(ctx, ctx->scratch.reserve_floor(side)); LL_CUDA(ctx, ctx->scratch2.reserve_floor(side));
     for (BucketTree* t : {&R.whole->corner, &R.whole->surf}) LL_CUDA(ctx, t->storage.reserve_floor(tree_storage_bytes(W)));
   }
-  if (R.ring.empty()) R.ring.resize(LL_RECOVERY_LOG);
+  R.log.open(LL_RECOVERY_LOG);
   R.cfg = *cfg; R.on = true; R.state = LL_TRACKING; R.bad = 0; R.field_valid = false;
   return LL_OK;
 }
 
 int ll_mapper_recovery_read(ll_mapper* m, ll_recovery_step* out, int cap, int* n, int* n_dropped) {
   if (!m || !n || cap < 0 || (cap > 0 && !out)) return LL_ERR_INVALID;
-  Recovery& R = m->rec;
-  const int k = (int)std::min((size_t)cap, R.count);
-  for (int i = 0; i < k; i++) out[i] = R.ring[(R.first + i) % R.ring.size()];
-  if (k > 0) { R.first = (R.first + k) % R.ring.size(); R.count -= k; }
-  *n = k;
-  if (n_dropped) *n_dropped = R.dropped;
-  R.dropped = 0;
+  m->rec.log.read(out, cap, n, n_dropped);
   return LL_OK;
 }
 

@@ -2,6 +2,7 @@
 images that ll_mapper_image_info accepts and reports; the validator refuses every kind of corruption before any device is involved; the
 ctypes struct has the header's size; and the C++ mirror's save / load compiles, links and runs (without a GPU it stops at the context)."""
 import ctypes as C
+import functools
 import os
 import struct
 import subprocess
@@ -9,13 +10,12 @@ import subprocess
 import numpy as np
 import pytest
 
+import image_writer
+from image_writer import CELL, CELL_POINT, key
 from loam_livox_b200 import capi
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = 8 + 4 + 4 + 8 + 16 * capi.LL_IMAGE_SECTIONS   # ll_mapper_image_header
-CELL = np.dtype([("key", "<u8"), ("create_frame", "<i4"), ("last_update", "<i4")])   # ll_image_cell
-CELL_POINT = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("cell", "<i4")])    # ll_image_cell_point
-BIAS = 1 << 20
 
 
 # ---------------------------------------------------------------------------------------------- writer of the documented layout
@@ -37,16 +37,11 @@ def points(n, seed):
 
 
 def history(sizes, seed) -> bytes:
-    n = int(sum(sizes))
-    return struct.pack("<qq", len(sizes), n) + np.asarray(sizes, "<i4").tobytes() + points(n, seed).tobytes()
+    return image_writer.history(sizes, points(int(sum(sizes)), seed))
 
 
 def snapshot(n, seed) -> bytes:
     return struct.pack("<q", n) + points(n, seed).tobytes()
-
-
-def key(k, j, i):
-    return ((k + BIAS) << 42) | ((j + BIAS) << 21) | (i + BIAS)
 
 
 def cellmap(frame_idx=6, n_out_of_range=0, n_cells=5, n_points=9, seed=0, cells=None, pts=None) -> bytes:
@@ -69,18 +64,7 @@ def parts(**cfg):
             cellmap(seed=5), cellmap(n_cells=7, n_points=4, seed=6)]
 
 
-def image(sections, magic=b"LLMAPIMG", version=1, config_bytes=None, total=None, offsets=None) -> bytes:
-    """Header + the sections back to back in index order (offsets: per-section overrides)."""
-    offs, off = [], HEADER
-    for s in sections:
-        offs.append(off)
-        off += len(s)
-    if offsets:
-        for k, o in offsets.items():
-            offs[k] = o
-    head = struct.pack("<8sIIQ", magic, version, C.sizeof(capi.MapperConfig) if config_bytes is None else config_bytes, off if total is None else total)
-    head += b"".join(struct.pack("<QQ", o, len(s)) for o, s in zip(offs, sections))
-    return head + b"".join(sections)
+image = functools.partial(image_writer.image, magic=b"LLMAPIMG", config_bytes=C.sizeof(capi.MapperConfig))
 
 
 def info(img):
@@ -244,6 +228,11 @@ def test_bad_configs_are_refused():
     p = parts()
     p[0] = p[0][:-8]
     assert status(image(p)) == capi.LL_ERR_INVALID
+
+
+def test_max_cells_above_2_29_is_refused():
+    assert status(image(parts(max_cells=2**29))) == capi.LL_OK
+    assert status(image(parts(max_cells=2**29 + 1))) == capi.LL_ERR_INVALID   # ll_cellmap_create refuses it
 
 
 def test_null_arguments_are_refused():

@@ -146,6 +146,15 @@ def test_table_exactly_half_full_then_one_over(ctx, oracle):
         g.append_cloud(_pts([(100.25, 0.25, 0.25)]))
 
 
+def test_max_cells_above_2_29_is_refused(ctx):
+    # the largest table has 2^30 slots (max_cells 2^29): beyond it, 2 x max_cells and the capacity would leave int
+    import ctypes as C
+    from loam_livox_b200 import capi
+    for max_cells in (1 << 30, 2**31 - 1):
+        h = C.c_void_p()
+        assert ctx._lib.ll_cellmap_create(ctx.h, 1.0, 2000, max_cells, C.byref(h)) == capi.LL_ERR_INVALID and not h.value, max_cells
+
+
 def test_many_points_in_one_voxel(ctx, oracle):
     rng = np.random.default_rng(11)
     g, o = _maps(ctx, oracle)

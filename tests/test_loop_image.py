@@ -3,24 +3,20 @@ images that ll_loop_image_info accepts and reports; the validator refuses every 
 it just inside, before any device is involved; the ctypes mirrors have the C layout; the entry points are exported with the header's
 parameter counts; and the C++ mirror's loop_save / loop_load compiles, links and runs (without a GPU it stops at the context)."""
 import ctypes as C
+import functools
 import struct
 import subprocess
 
 import numpy as np
 import pytest
 
+import image_writer
+from image_writer import CELL, CELL_POINT, key
 from loam_livox_b200 import capi
 from test_recovery_cabi import _compile, _header_params
 
 HEADER = 24 + 16 * capi.LL_LOOP_IMAGE_SECTIONS   # ll_loop_image_header
-CELL = np.dtype([("key", "<u8"), ("create_frame", "<i4"), ("last_update", "<i4")])   # ll_image_cell
-CELL_POINT = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("cell", "<i4")])    # ll_image_cell_point
-BIAS = 1 << 20
 IMG = 4 * 3600   # floats of one keyframe's four images
-
-
-def key(k, j, i):
-    return ((k + BIAS) << 42) | ((j + BIAS) << 21) | (i + BIAS)
 
 
 # ---------------------------------------------------------------------------------------------- writer of the documented layout
@@ -51,8 +47,7 @@ def cells(frame_idx=12, n_out_of_range=0, keys=None, stamps=None, cur=(0, 1, 0, 
 
 
 def history(sizes=(3, 2), seed=2) -> bytes:
-    n = int(sum(sizes))
-    return struct.pack("<qq", len(sizes), n) + np.asarray(sizes, "<i4").tobytes() + np.random.default_rng(seed).uniform(-9, 9, (n, 4)).astype("<f4").tobytes()
+    return image_writer.history(sizes, np.random.default_rng(seed).uniform(-9, 9, (int(sum(sizes)), 4)).astype("<f4"))
 
 
 def open_kfs(kfs=((4, 4, [(0, 0), (1, 0), (1, 1)]), (2, 2, [(3, 2)]), (0, 0, []))) -> bytes:
@@ -102,16 +97,7 @@ def parts(closed=False):
             np.zeros(2 * IMG, "<f4").tobytes(), points(2 + 3 + 1, 5), accumulated(), loop, events()]
 
 
-def image(sections, magic=b"LLLOOPIM", version=1, config_bytes=None, total=None, offsets=None) -> bytes:
-    offs, off = [], HEADER
-    for s in sections:
-        offs.append(off)
-        off += len(s)
-    for k, o in (offsets or {}).items():
-        offs[k] = o
-    head = struct.pack("<8sIIQ", magic, version, C.sizeof(capi.LoopClosureCfg) if config_bytes is None else config_bytes, off if total is None else total)
-    head += b"".join(struct.pack("<QQ", o, len(s)) for o, s in zip(offs, sections))
-    return head + b"".join(sections)
+image = functools.partial(image_writer.image, magic=b"LLLOOPIM", config_bytes=C.sizeof(capi.LoopClosureCfg))
 
 
 def summary(img):
@@ -287,6 +273,11 @@ def test_a_full_table_is_reported_not_refused():
     assert st == capi.LL_OK and got.cells == n
     from loam_livox_b200.registration import loop_image_info
     assert loop_image_info(image(p))["cells"] == n
+
+
+def test_max_cells_above_2_29_is_refused():
+    assert status(with_part(0, config(max_cells=2**29))) == capi.LL_OK
+    assert status(with_part(0, config(max_cells=2**29 + 1))) == capi.LL_ERR_INVALID   # ll_cellmap_create refuses it
 
 
 def test_config_padding_must_be_zero():
