@@ -1,5 +1,5 @@
-"""The keyframe oracle (oracle/orc_keyframe.hpp through tests/cpp/keyframe_oracle.cpp) for the tests, and NumPy restatements of the loop
-search's gates and of the keyframe's ROI range."""
+"""The keyframe oracle (oracle/orc_keyframe.hpp through tests/cpp/keyframe_oracle.cpp) for the tests, NumPy restatements of the loop search's
+gates, the keyframe's ROI range and its direction count images, and fp64 references of the blur and the normalised correlation."""
 import atexit
 import ctypes as C
 import os
@@ -206,3 +206,60 @@ def numpy_roi_range(centers):
     n = np.sqrt((d[:, 0] * d[:, 0] + (d[:, 1] * d[:, 1] + d[:, 2] * d[:, 2])).astype(np.float32)).astype(np.float32)
     u = np.unique(n)
     return c, u[int(np.ceil(np.float32(len(u) - 1) * np.float32(0.9)))]
+
+
+def numpy_images(types, vecs):
+    """The direction count images of analyze (:1487-1494) from the cell types and vectors: basis = eigenvectors of I + sum v v^T over plane cells
+    (fp64), reversed, column 2 = column 0 x column 1 (float); each vector's bin from the float of the double atan2 / asin.  Returns (line counts,
+    plane counts, the image frame coordinates [n, 3] of every vector)."""
+    types, vecs = np.asarray(types), np.asarray(vecs, np.float32)
+    M = np.eye(3)
+    for v in vecs[types == 2]:
+        M += np.outer(v, v).astype(np.float32).astype(np.float64)
+    _, V = eig3(M)
+    R = np.c_[V[:, 2], V[:, 1]].astype(np.float32)
+    r0, r1 = R[:, 0], R[:, 1]
+    R = np.c_[R, np.array([r0[1] * r1[2] - r0[2] * r1[1], r0[2] * r1[0] - r0[0] * r1[2], r0[0] * r1[1] - r0[1] * r1[0]], np.float32)]
+    imgs = np.zeros((2, 60, 60), np.float32)
+    frame = np.zeros((len(vecs), 3), np.float32)
+    for r, (t, v) in enumerate(zip(types, vecs)):
+        if t not in (1, 2):
+            continue
+        a = np.array([R[0, c] * v[0] + (R[1, c] * v[1] + R[2, c] * v[2]) for c in range(3)], np.float32)   # Eigen's dot order, in float
+        frame[r] = a
+        if a[0] < 0:
+            a = -a
+        phi = np.float64(np.float32(np.arctan2(np.float64(a[1]), np.float64(a[0])))) + np.pi / 2
+        th = np.float64(np.float32(np.arcsin(np.float64(a[2])))) + np.pi / 2
+        pi, ti = (min(max(int(np.floor(x / (np.pi / 60))), 0), 59) for x in (phi, th))
+        imgs[0 if t == 1 else 1, pi, ti] += 1
+    return imgs[0], imgs[1], frame
+
+
+def fp64_gaussian_kernel():
+    t = np.exp(-((np.arange(9) - 4.0) ** 2) / (2.0 * 16.0))
+    return t / t.sum()
+
+
+def fp64_blur(img):
+    """apply_guassian_blur(img, 4, 4) in fp64: the circular 9 x 9 Gaussian (sigma 4) of the 60 x 60 image."""
+    g = fp64_gaussian_kernel()
+    a = np.asarray(img, np.float64)
+    out = np.zeros((60, 60))
+    for s in range(9):
+        for t in range(9):
+            out += g[s] * g[t] * np.roll(a, (4 - s, 4 - t), axis=(0, 1))
+    return out
+
+
+def fp64_similarity(a, b):
+    """CCORR_NORMED of the template a over b wrap-padded by 30, in fp64, max over the 61 x 61 positions (0 at a zero norm)."""
+    T = np.asarray(a, np.float64)
+    P = np.pad(np.asarray(b, np.float64), 30, mode="wrap")
+    W = np.lib.stride_tricks.sliding_window_view(P, (60, 60))
+    num = np.einsum("yxrc,rc->yx", W, T)
+    den = np.einsum("yxrc,yxrc->yx", W, W)
+    t = np.sqrt(den * (T * T).sum())
+    with np.errstate(invalid="ignore", divide="ignore"):
+        r = np.where(t > 0, num / np.where(t > 0, t, 1.0), 0.0)
+    return float(r.max())

@@ -202,26 +202,11 @@ def test_oracle_roi_range_and_images_match_numpy():
     centers = (ijk.astype(np.float32) * np.float32(0.5) + np.float32(0.25)).astype(np.float32)
     c, roi = K.numpy_roi_range(centers)
     assert np.array_equal(c, info["center"]) and roi == info["roi_range"]
-    # the direction images from the cell vectors: basis = eigenvectors of I + sum v v^T over plane cells (fp64), reversed, col 2 = col 0 x col 1
-    M = np.eye(3)
-    for v in vec[typ == K_PLANE]:
-        M += np.outer(v, v).astype(np.float32).astype(np.float64)
-    w, V = K.eig3(M)
-    R = np.c_[V[:, 2], V[:, 1]].astype(np.float32)
-    R = np.c_[R, np.cross(R[:, 0], R[:, 1]).astype(np.float32)]
     imgs = m.images(k)
-    for t, idx in ((K_LINE, 0), (K_PLANE, 1)):
-        cnt = np.zeros((60, 60), np.float32)
-        for v in vec[typ == t]:
-            a = (R.T.astype(np.float64) @ v.astype(np.float64)).astype(np.float32)
-            if a[0] < 0:
-                a = -a
-            phi = np.float64(np.float32(np.arctan2(np.float64(a[1]), np.float64(a[0])))) + np.pi / 2
-            th = np.float64(np.float32(np.arcsin(np.float64(a[2])))) + np.pi / 2
-            pi, ti = (min(max(int(np.floor(x / (np.pi / 60))), 0), 59) for x in (phi, th))
-            cnt[pi, ti] += 1
+    cnt_line, cnt_plane, _ = K.numpy_images(typ, vec)
+    for cnt, idx, ratio in ((cnt_line, 0, info["ratio_line"]), (cnt_plane, 1, info["ratio_plane"])):
         assert np.array_equal(cnt, imgs[idx])
-        assert np.float32((cnt >= 1).sum()) / np.float32(3600) == (info["ratio_line"] if t == K_LINE else info["ratio_plane"])
+        assert np.float32((cnt >= 1).sum()) / np.float32(3600) == ratio
         assert np.array_equal(K.blur(cnt), imgs[2 + idx])
 
 
@@ -301,3 +286,202 @@ def test_fp32_against_fp64_typing_on_a_scene():
         differ += t32 != t
     print(f"fp32 vs fp64 typing: {differ} of {typed} cells differ")
     assert typed > 500 and differ <= 0.01 * typed
+
+
+# ---- the constructed edge cases (keyframe_cases.py): each reaches its edge, and the oracle equals the NumPy and fp64 references on it --------
+import keyframe_cases as KC   # noqa: E402
+
+
+def _oracle_keyframe(cloud, incremental=False):
+    m = K.OracleMap(1.0, incremental=incremental)
+    k = m.new_keyframe()
+    m.append(cloud, [k])
+    m.analyze(k)
+    return m, k
+
+
+def _key(ijk):
+    B = 1 << 20
+    i, j, k = ijk
+    return np.uint64(((k + B) << 42) | ((j + B) << 21) | (i + B))
+
+
+def _fp64_type(p, c):
+    """determine_feature on the exact (fp64) mean and covariance."""
+    p = np.asarray(p, np.float64)
+    if len(p) < 5 or np.linalg.norm(c - p.mean(0)) > 0.375:
+        return K_SPHERE
+    w = np.linalg.eigvalsh(np.cov(p.T, ddof=1))
+    return K_PLANE if w[1] / 3 > w[0] else (K_LINE if w[2] / 3 > w[1] else K_SPHERE)
+
+
+@pytest.mark.parametrize("name", list(KC.cell_cases()))
+def test_cell_cases_oracle_equals_the_references(name):
+    """Every cell lies in its designed map cell; the keyframe's types and vectors are those of the one-cell oracle (Points_cloud_cell) on its
+    points, batch and incremental; the images, centre and ROI equal the NumPy restatements, the blur the fp64 one."""
+    cells = KC.cell_cases()[name]
+    for ijk, p, what in cells:
+        assert (KC.cell_of(p) == np.array(ijk)).all(), what
+    for inc in (False, True):
+        m, k = _oracle_keyframe(KC.cells_cloud(cells), inc)
+        keys, _, typ, vec = m.cells(k)
+        order = {int(x): r for r, x in enumerate(keys)}
+        assert len(order) == len(cells)
+        for ijk, p, what in cells:
+            t, v, _, _ = K.cell_type(p, KC.centre(*ijk), incremental=inc)
+            r = order[int(_key(ijk))]
+            assert typ[r] == t and np.array_equal(vec[r], v), (what, inc)
+        info, imgs = m.info(k), m.images(k)
+        cl, cp, _ = K.numpy_images(typ, vec)
+        assert np.array_equal(imgs[0], cl) and np.array_equal(imgs[1], cp)
+        centres = np.array([KC.centre(*ijk) for ijk, _, _ in sorted(cells, key=lambda c: int(_key(c[0])))], np.float32)
+        c, roi = K.numpy_roi_range(centres)
+        assert np.array_equal(c, info["center"]) and roi == info["roi_range"]
+        for a in (0, 1):
+            assert np.abs(imgs[2 + a] - K.fp64_blur(imgs[a])).max() <= 1e-6 * max(1.0, float(imgs[a].max()))
+
+
+def test_cell_cases_reach_their_edges():
+    cc = KC.cell_cases()
+    get = {(name, what): (ijk, p) for name, cells in cc.items() for ijk, p, what in cells}
+
+    def typed(name, what, inc=False):
+        ijk, p = get[(name, what)]
+        return K.cell_type(p, KC.centre(*ijk), incremental=inc)
+    # incremental: 5 and 6 points keep the 4-point covariance, the 7th starts the recurrence
+    for rep in range(3):
+        ijk, p = [(c[0], c[1]) for c in cc["points_1_to_8"] if c[0] == (8, rep, 0)][0]
+        c4 = K.cell_type(p[:4], KC.centre(*ijk), incremental=True)[3]
+        for n, same in ((5, True), (6, True), (7, False)):
+            assert np.array_equal(K.cell_type(p[:n], KC.centre(*ijk), incremental=True)[3], c4) == same
+    # exact ties of the one-third rule: w1 = 3 w0 types LINE (not PLANE), w2 = 3 w1 SPHERE (not LINE)
+    t, _, _, cov = typed("one_third", "plane tie")
+    w = np.sort(np.diag(cov).astype(np.float64))
+    assert np.count_nonzero(cov - np.diag(np.diag(cov))) == 0 and w[1] * (1.0 / 3.0) == w[0] and t == K_LINE
+    t, _, _, cov = typed("one_third", "line tie")
+    w = np.sort(np.diag(cov).astype(np.float64))
+    assert np.count_nonzero(cov - np.diag(np.diag(cov))) == 0 and w[2] * (1.0 / 3.0) == w[1] and w[1] * (1.0 / 3.0) < w[0] and t == K_SPHERE
+    # one float either side of each boundary: the oracle's type flips between the two coordinates
+    for rule, want in (("plane", (K_PLANE, K_LINE)), ("line", (K_LINE, K_SPHERE))):
+        (ia, pa), (ib, pb) = get[("one_third", f"{rule} flip below")], get[("one_third", f"{rule} flip above")]
+        a, b = KC.one_third_flip(KC.centre(*ia), 2 if rule == "plane" else 1), KC.one_third_flip(KC.centre(*ib), 2 if rule == "plane" else 1)
+        assert np.array_equal(pa, KC.six_axes(KC.centre(*ia), *a[0])) and np.array_equal(pb, KC.six_axes(KC.centre(*ib), *b[1]))
+        assert {typed("one_third", f"{rule} flip below")[0], typed("one_third", f"{rule} flip above")[0]} <= set(want) | {K_SPHERE}
+        for e, (lo, hi) in ((ia, a), (ib, b)):
+            tl = K.cell_type(KC.six_axes(KC.centre(*e), *lo), KC.centre(*e))[0]
+            th = K.cell_type(KC.six_axes(KC.centre(*e), *hi), KC.centre(*e))[0]
+            assert tl != th and sum(x != y for x, y in zip(lo, hi)) == 1
+    # identical points: the covariance is rounding noise
+    assert not typed("identical_points", "5 x 0.3: zero covariance")[3].any()
+    cov = typed("identical_points", "7 x 0.7: rank 1, three equal entries")[3]
+    assert len(np.unique(cov)) == 1 and cov[0, 0] != 0
+    cov = typed("identical_points", "5 x 123.456: a negative eigenvalue")[3]
+    assert np.linalg.eigvalsh(cov.astype(np.float64)).min() < 0
+    # axis-aligned: the vector is exactly an axis; the diagonal lines pin the first of equal components positive
+    for a in range(3):
+        for kind, want in (("line", K_LINE), ("plane", K_PLANE)):
+            t, v, _, _ = typed("axis_aligned", f"{kind} axis {a}")
+            assert t == want and np.array_equal(v, np.eye(3, dtype=np.float32)[a])
+    for what, sy in (("line (1, 1, 0)", 1), ("line (1, -1, 0)", -1)):
+        t, v, _, _ = typed("axis_aligned", what)
+        assert t == K_LINE and v[0] > 0 and v[1] == sy * v[0] and v[2] == 0
+    # the centre gate: the mean one float inside 0.375, at it exactly (typed), one float outside (not typed)
+    for s, (want_d, want_t) in enumerate(((-1, K_PLANE), (0, K_PLANE), (1, K_SPHERE))):
+        ijk, p = get[("centre_gate", ["gate below", "gate at", "gate above"][s])]
+        c = KC.centre(*ijk)
+        _, _, m, _ = K.cell_type(p, c)
+        e = (c - m).astype(np.float32)
+        dn = np.sqrt(np.float32(e[0] * e[0] + np.float32(e[1] * e[1] + e[2] * e[2])))
+        assert np.sign(dn - np.float32(0.375)) == want_d and K.cell_type(p, c)[0] == want_t
+    # far cells: how often the float covariance types a cell differently from the exact one (reported, not asserted)
+    differ = sum(K.cell_type(p, KC.centre(*ijk))[0] != _fp64_type(p, KC.centre(*ijk).astype(np.float64)) for ijk, p, _ in cc["far_cells"])
+    print(f"far cells: {differ} of {len(cc['far_cells'])} typed differently from the fp64 typing")
+    assert len(cc["big_cell"][0][1]) >= 100000
+
+
+@pytest.mark.parametrize("name", list(KC.direction_cases()))
+def test_direction_cases_paint_their_designed_images(name):
+    cloud, want_line, want_plane = KC.direction_cases()[name]
+    m, k = _oracle_keyframe(cloud)
+    _, _, typ, vec = m.cells(k)
+    imgs, info = m.images(k), m.info(k)
+    assert np.array_equal(imgs[0], want_line) and np.array_equal(imgs[1], want_plane)
+    cl, cp, frame = K.numpy_images(typ, vec)
+    assert np.array_equal(cl, imgs[0]) and np.array_equal(cp, imgs[1])
+    assert info["ratio_line"] == np.float32((want_line >= 1).sum()) / np.float32(3600)
+    for a in (0, 1):
+        assert np.abs(imgs[2 + a] - K.fp64_blur(imgs[a])).max() <= 1e-6 * max(1.0, float(imgs[a].max()))
+    if name.startswith("clamps"):
+        lines = frame[typ == K_LINE]
+        # x' = +0 on every axis line that is not along the image's x' axis; asin(-1) with the identity basis, asin(+1) with +y normals
+        assert (np.abs(lines[:, 2]) == 1).sum() == 1 and not np.signbit(lines[:, 0]).any()
+        assert lines[np.abs(lines[:, 2]) == 1][0, 2] == (1 if name == "clamps_y_normals" else -1)
+
+
+def test_growth_appends_reach_their_edges():
+    m = K.OracleMap(1.0, revisit_threshold=2)
+    ks = [m.new_keyframe(), m.new_keyframe()]
+    sizes = []
+    for cloud, op in KC.growth_appends():
+        m.append(cloud, [ks[i] for i in op])
+        sizes.append(m.info(ks[0])["cells"])
+    assert sizes[1] <= 4096 < sizes[-1] and m.info(ks[1])["cells"] < sizes[-1]
+    keys, inc, _, _ = m.cells(ks[0])
+    assert inc.max() == 1 and len(np.unique(keys)) == len(keys) - 1   # the revisited cell held in both incarnations
+
+
+@pytest.mark.parametrize("name", list(KC.roi_cases()))
+def test_roi_cases_equal_numpy(name):
+    cloud = KC.roi_cases()[name]
+    m, k = _oracle_keyframe(cloud)
+    c, roi = K.numpy_roi_range(np.array([KC.centre(*x) for x in sorted(set(map(tuple, KC.cell_of(cloud))), key=lambda x: int(_key(x)))], np.float32))
+    info = m.info(k)
+    assert np.array_equal(c, info["center"]) and roi == info["roi_range"]
+
+
+def test_roi_cases_reach_their_edges():
+    us = {}
+    for name, cloud in KC.roi_cases().items():
+        cent = np.array([KC.centre(*x) for x in sorted(set(map(tuple, KC.cell_of(cloud))), key=lambda x: int(_key(x)))], np.float32)
+        c = K.numpy_roi_range(cent)[0]
+        d = cent - c
+        us[name] = len(np.unique(np.sqrt((d[:, 0] * d[:, 0] + (d[:, 1] * d[:, 1] + d[:, 2] * d[:, 2])).astype(np.float32))))
+        assert len(cent) == (len(cloud) - 1 if name == 'duplicate_distances' else len(cloud))   # one cell taken twice there
+    assert us["one_cell"] == 1 and us["cube_corners"] == 1 and us["duplicate_distances"] < 24
+    onto = {n: float(np.float32(us[n] - 1) * np.float32(0.9)).is_integer() for n in us if n.startswith("distinct")}
+    assert any(onto.values()) and not all(onto.values())
+
+
+def test_blur_of_a_cyclic_shift_is_the_shifted_blur():
+    r = np.random.default_rng(9)
+    img = np.zeros((60, 60), np.float32)
+    img[0, :] = 1
+    img[:, 59] += 2
+    img[r.integers(0, 60, 30), r.integers(0, 60, 30)] += 5
+    img[17, 42] = 1000
+    for s in ((1, 0), (0, 1), (30, 30), (59, 7), (-13, 29)):
+        assert np.array_equal(K.blur(np.roll(img, s, (0, 1))), np.roll(K.blur(img), s, (0, 1)))
+    assert np.abs(K.blur(img) - K.fp64_blur(img)).max() <= 1e-6 * float(img.max())
+
+
+@pytest.mark.parametrize("name", ["newest_1", "cyclic_shifts", "zero_and_one_pixel"])
+def test_search_cases_oracle_equals_fp64(name):
+    kfs = KC.search_cases()[name]
+    imgs = []
+    for px, planes in kfs:
+        cl = np.zeros((60, 60), np.float32)
+        for (p, t), n in px.items():
+            cl[p, t] = n
+        cp = np.zeros((60, 60), np.float32)
+        cp[30, 30] = planes
+        imgs.append((K.blur(cp), K.blur(cl)))
+    a = imgs[-1]
+    for b, (px, _) in zip(imgs[:-1], kfs[:-1]):
+        for w in (0, 1):
+            s = K.similarity(a[w], b[w])
+            assert abs(s - K.fp64_similarity(a[w], b[w])) <= 2e-6
+    if name == "cyclic_shifts":
+        # every cyclic shift of the newest's line image scores exactly 1: the wrap pad reaches every offset, and num = den = sum T^2 bit for bit
+        for b, (px, _) in zip(imgs[:-2], kfs[:-2]):
+            assert K.similarity(a[1], b[1]) == 1.0
+        assert K.similarity(a[1], imgs[-2][1]) < 1.0
