@@ -843,6 +843,29 @@ int  ll_mapper_set_loop_policy(ll_mapper* mapper, const ll_loop_policy* p);
 /* Every loop edge so far, in closing order (*n_loops of them; edges may be NULL to query).  cap < *n_loops: LL_ERR_CAPACITY, nothing written. */
 int  ll_mapper_loop_edges(ll_mapper* mapper, ll_pg_edge* edges, int cap, int* n_loops);
 
+/* ---- loop feedback: the optimized trajectory back into the odometry (DESIGN.md §4.6.2) ----------------------------------------------------
+ * Off by default, and then every output is what it is without this API.  With it on (matching mode 0), the step that closes a loop (its
+ * LL_LOOP_CLOSED event) then moves the mapper onto the optimized trajectory:
+ *   every live segment of both history windows (one step's world-frame features, frame index s) by A(s) o A_prev(s)^-1, where A is
+ *           ll_loop_correction over this loop's poses and A_prev the same over the previous loop's (the identity before the first loop);
+ *   the mapper's pose becomes the newest keyframe's optimized pose, the pose of the last window addition moves with the newest correction,
+ *           and the next step rebuilds its match map from the moved window.
+ * Loop closure stays in the odometry frame: with C the correction applied last (A of the latest loop at its newest keyframe, the identity
+ * before a loop), it receives C^-1 o pose instead of the mapper's pose, for the step's full cloud and for the keyframe poses it records.  A
+ * failure of the feedback other than LL_ERR_CUDA is checked before anything moves, logged as LL_LOOP_ERROR and stops loop closure.
+ * Refused (LL_ERR_INVALID, nothing changed): loop closure off, a loop already closed, on = 1 in matching mode 1 (a cell-map point does not
+ * record its step), maximum_history_size above LL_LOOP_FEEDBACK_MAX_SEGMENTS, or keyframes restored from a loop image of version 1 or 2
+ * (their frame indices are not recorded there).  ll_mapper_set_loop_closure and ll_mapper_loop_load of such an image turn it off. */
+#define LL_LOOP_FEEDBACK_MAX_SEGMENTS 4096   /* window segments the correction kernel stages in shared memory (both windows: 32 KiB) */
+int  ll_mapper_set_loop_feedback(ll_mapper* mapper, int on);
+/* C (q_wxyz, t) and how many corrections were applied.  Loop closure off: the identity and 0. */
+int  ll_mapper_loop_correction_read(ll_mapper* mapper, double q_wxyz[4], double t[3], int* n_applied);
+/* Host only, no context: the correction of the step with frame index s for keyframes 0 ... n - 1 closed at frame indices f[] (strictly
+ * ascending), in fp64.  A_k = opt_k o ori_k^-1 (A_0 the identity: the graph holds pose 0 constant); A_0 for s <= f[0], A_(n-1) for
+ * s >= f[n - 1], A_k at s = f[k], and between two keyframes, u = (s - f[k]) / (f[k + 1] - f[k]), the slerp of the rotations (the shorter arc)
+ * and the linear interpolation of the translations.  LL_ERR_INVALID: a NULL array, n < 1 or f not strictly ascending. */
+int  ll_loop_correction(const ll_pose* ori, const ll_pose* opt, const int* f, int n, int s, double q_wxyz[4], double t[3]);
+
 /* ---- loop image: the mapper's loop closure as a byte image of its own (DESIGN.md §4.6.1) ------------------------------------------------
  * Checkpoint a run with loop closure on: save the mapper image and the loop image at the same step, then ll_mapper_load the one and
  * ll_mapper_loop_load the other onto the loaded mapper.  The restored mapper continues bit for bit as the saved one: every ll_reg_result field
@@ -888,9 +911,17 @@ int  ll_mapper_loop_edges(ll_mapper* mapper, ll_pg_edge* edges, int cap, int* n_
 #define LL_LOOP_IMAGE_MAGIC "LLLOOPIM"
 #define LL_LOOP_IMAGE_VERSION 1
 #define LL_LOOP_IMAGE_VERSION_POLICY 2   /* the version a loop closure under a policy other than the default writes (LL_LOOP_IMAGE_LOOP above) */
+/* Version 3, written with loop feedback on (whatever the policy): the header holds one more section, LL_LOOP_IMAGE_FEEDBACK, after the
+ * thirteen; LL_LOOP_IMAGE_LOOP has version 2's layout with max_loops 1 ... LL_MAX_LOOPS.  LL_LOOP_IMAGE_FEEDBACK: int32 on (1), int32
+ * n_applied (<= n_loops; < n_loops only when stopped), double c_q_wxyz[4], c_t[3] (the identity when n_applied is 0), int64 n_keyframes (the
+ * scalars'), int64 n_segments, int32 f[n_keyframes] (each closed keyframe's frame index, strictly ascending), int32 frame[n_segments] (the
+ * frame index of every live segment of the mapper's history windows, oldest first, strictly ascending).  Every frame index is within
+ * 0 ... the stamp's frame_index, and ll_mapper_loop_load refuses the image unless n_segments equals the mapper's window segments. */
+#define LL_LOOP_IMAGE_VERSION_FEEDBACK 3
 enum { LL_LOOP_IMAGE_CONFIG = 0, LL_LOOP_IMAGE_SCALARS = 1, LL_LOOP_IMAGE_CELLS = 2, LL_LOOP_IMAGE_HISTORY = 3, LL_LOOP_IMAGE_OPEN = 4,
        LL_LOOP_IMAGE_KEYFRAMES = 5, LL_LOOP_IMAGE_POSES = 6, LL_LOOP_IMAGE_EDGES = 7, LL_LOOP_IMAGE_IMAGES = 8, LL_LOOP_IMAGE_CLOUDS = 9,
-       LL_LOOP_IMAGE_ACCUMULATED = 10, LL_LOOP_IMAGE_LOOP = 11, LL_LOOP_IMAGE_EVENTS = 12, LL_LOOP_IMAGE_SECTIONS = 13 };
+       LL_LOOP_IMAGE_ACCUMULATED = 10, LL_LOOP_IMAGE_LOOP = 11, LL_LOOP_IMAGE_EVENTS = 12, LL_LOOP_IMAGE_SECTIONS = 13,
+       LL_LOOP_IMAGE_FEEDBACK = 13, LL_LOOP_IMAGE_SECTIONS_FEEDBACK = 14 };
 typedef struct { char magic[8]; uint32_t version, config_bytes; uint64_t total_bytes; ll_image_section section[LL_LOOP_IMAGE_SECTIONS]; } ll_loop_image_header;   /* 232 B */
 typedef struct {
   int32_t frame_index, matching_mode;           /* binding stamp: the mapper's m_current_frame_index and matching_mode,                  */

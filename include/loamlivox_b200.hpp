@@ -346,6 +346,15 @@ class Laser_mapping {
   // loops after the first (ll_mapper_set_loop_policy): p NULL the default (the reference's first loop, then stop); set after set_loop_closure
   // and before the first loop, else it throws and changes nothing
   void set_loop_policy(const ll_loop_policy* p) { ctx_.check(ll_mapper_set_loop_policy(mapper_, p)); }
+  // loop feedback (ll_mapper_set_loop_feedback; matching mode 0): after each loop the history windows and the pose move onto the optimized
+  // trajectory.  Set after set_loop_closure and before the first loop, else it throws and changes nothing
+  void set_loop_feedback(bool on) { ctx_.check(ll_mapper_set_loop_feedback(mapper_, on ? 1 : 0)); }
+  // the correction applied last (q_wxyz, t) and how many were applied (ll_mapper_loop_correction_read)
+  int loop_correction(double q_wxyz[4], double t[3]) {
+    int n = 0;
+    ctx_.check(ll_mapper_loop_correction_read(mapper_, q_wxyz, t, &n));
+    return n;
+  }
   // every loop edge so far, in closing order (ll_mapper_loop_edges)
   std::vector<ll_pg_edge> loop_edges() {
     int n = 0;

@@ -30,7 +30,9 @@ LL_LOOP_LOG = 1024
 LL_LOOP_KEYFRAME, LL_LOOP_ALIGNMENT, LL_LOOP_CLOSED, LL_LOOP_ERROR = 0, 1, 2, 3
 LL_LOOP_SKIP10, LL_LOOP_SKIP5, LL_LOOP_ACCEPT, LL_LOOP_FAILED = 0, 1, 2, 3
 LL_MAPPER_IMAGE_MAGIC, LL_MAPPER_IMAGE_VERSION = b"LLMAPIMG", 1
-LL_LOOP_IMAGE_MAGIC, LL_LOOP_IMAGE_VERSION, LL_LOOP_IMAGE_VERSION_POLICY = b"LLLOOPIM", 1, 2
+LL_LOOP_IMAGE_MAGIC, LL_LOOP_IMAGE_VERSION, LL_LOOP_IMAGE_VERSION_POLICY, LL_LOOP_IMAGE_VERSION_FEEDBACK = b"LLLOOPIM", 1, 2, 3
+LL_LOOP_IMAGE_FEEDBACK, LL_LOOP_IMAGE_SECTIONS_FEEDBACK = 13, 14
+LL_LOOP_FEEDBACK_MAX_SEGMENTS = 4096
 (LL_LOOP_IMAGE_CONFIG, LL_LOOP_IMAGE_SCALARS, LL_LOOP_IMAGE_CELLS, LL_LOOP_IMAGE_HISTORY, LL_LOOP_IMAGE_OPEN, LL_LOOP_IMAGE_KEYFRAMES, LL_LOOP_IMAGE_POSES,
  LL_LOOP_IMAGE_EDGES, LL_LOOP_IMAGE_IMAGES, LL_LOOP_IMAGE_CLOUDS, LL_LOOP_IMAGE_ACCUMULATED, LL_LOOP_IMAGE_LOOP, LL_LOOP_IMAGE_EVENTS, LL_LOOP_IMAGE_SECTIONS) = range(14)
 (LL_IMAGE_CONFIG, LL_IMAGE_SCALARS, LL_IMAGE_HISTORY_CORNER, LL_IMAGE_HISTORY_SURF, LL_IMAGE_SNAPSHOT_CORNER, LL_IMAGE_SNAPSHOT_SURF, LL_IMAGE_CELLS_CORNER,
@@ -57,6 +59,7 @@ EXPORTS = [
     "ll_mapper_process_sweep", "ll_mapper_process_sweeps",
     "ll_mapper_loop_save", "ll_mapper_loop_load", "ll_loop_image_info",
     "ll_mapper_loop_policy_default", "ll_mapper_set_loop_policy", "ll_mapper_loop_edges",
+    "ll_mapper_set_loop_feedback", "ll_mapper_loop_correction_read", "ll_loop_correction",
 ]
 LL_SPIN_FULL, LL_SPIN_SHARP, LL_SPIN_LESS_SHARP, LL_SPIN_FLAT, LL_SPIN_LESS_FLAT = 0, 1, 2, 3, 4
 LL_CELL_SPHERE, LL_CELL_LINE, LL_CELL_PLANE, LL_CELL_ALL = 0, 1, 2, -1
@@ -379,6 +382,9 @@ def lib():
     L.ll_mapper_loop_policy_default.argtypes = [C.POINTER(LoopPolicy)]
     L.ll_mapper_set_loop_policy.argtypes = [vp, C.POINTER(LoopPolicy)]
     L.ll_mapper_loop_edges.argtypes = [vp, vp, ci, C.POINTER(ci)]
+    L.ll_mapper_set_loop_feedback.argtypes = [vp, ci]
+    L.ll_mapper_loop_correction_read.argtypes = [vp, vp, vp, C.POINTER(ci)]
+    L.ll_loop_correction.argtypes = [C.POINTER(Pose), C.POINTER(Pose), vp, ci, ci, vp, vp]
     L.ll_launch_count.argtypes = [vp]
     L.ll_launch_count.restype = C.c_uint64
     _LIB = L

@@ -8,11 +8,12 @@
 
 size_t image_header(const ImageKind& kind, uint32_t version, const uint64_t* len, void* header) {
   uint8_t* h = (uint8_t*)header;
-  const uint64_t head = 24 + 16 * (uint64_t)kind.sections;
+  const int sections = kind.count(version);
+  const uint64_t head = 24 + 16 * (uint64_t)sections;
   memset(h, 0, head);
   memcpy(h, kind.magic, 8); img_put<uint32_t>(h + 8, version); img_put<uint32_t>(h + 12, kind.config_bytes);
   uint64_t off = head;
-  for (int k = 0; k < kind.sections; k++) { img_put<uint64_t>(h + 24 + 16 * k, off); img_put<uint64_t>(h + 32 + 16 * k, len[k]); off += len[k]; }
+  for (int k = 0; k < sections; k++) { img_put<uint64_t>(h + 24 + 16 * k, off); img_put<uint64_t>(h + 32 + 16 * k, len[k]); off += len[k]; }
   img_put<uint64_t>(h + 16, off);
   return (size_t)off;
 }
@@ -20,18 +21,20 @@ size_t image_header(const ImageKind& kind, uint32_t version, const uint64_t* len
 int image_structure(const void* image, size_t bytes, const ImageKind& kind, ll_image_section* sec, std::string* err) {
   auto fail = [&](const std::string& msg) { if (err) *err = msg; return LL_ERR_INVALID; };
   const uint8_t* b = (const uint8_t*)image;
-  const size_t head = 24 + 16 * (size_t)kind.sections;
-  if (!b || bytes < head) return fail("shorter than the image header");
+  if (!b || bytes < 24 + 16 * (size_t)kind.sections) return fail("shorter than the image header");
   char magic[8]; uint32_t version, config_bytes; uint64_t total;
   memcpy(magic, b, 8); memcpy(&version, b + 8, 4); memcpy(&config_bytes, b + 12, 4); memcpy(&total, b + 16, 8);
-  memcpy(sec, b + 24, 16 * (size_t)kind.sections);
   if (memcmp(magic, kind.magic, 8) != 0) return fail(std::string("not a ") + kind.name + " image (magic)");
   if (version < kind.version || version > kind.max_version) return fail("unknown image version");
+  const int sections = kind.count(version);
+  const size_t head = 24 + 16 * (size_t)sections;
+  if (bytes < head) return fail("shorter than the image header");
+  memcpy(sec, b + 24, 16 * (size_t)sections);
   if (config_bytes != kind.config_bytes) return fail(std::string("config size differs from this library's ") + kind.config_name);
   if (total != bytes) return fail("image size differs from the header's total_bytes");
   // every section inside the image after the header, no two overlapping
-  std::vector<int> order(kind.sections);
-  for (int k = 0; k < kind.sections; k++) {
+  std::vector<int> order(sections);
+  for (int k = 0; k < sections; k++) {
     const ll_image_section& s = sec[k];
     if (s.offset < head || s.offset > bytes || s.length > bytes - s.offset) return fail("section outside the image");
     order[k] = k;
@@ -40,7 +43,7 @@ int image_structure(const void* image, size_t bytes, const ImageKind& kind, ll_i
     const ll_image_section &x = sec[a], &y = sec[c];
     return x.offset != y.offset ? x.offset < y.offset : x.length < y.length;
   });
-  for (int k = 1; k < kind.sections; k++) {
+  for (int k = 1; k < sections; k++) {
     const ll_image_section &p = sec[order[k - 1]], &q = sec[order[k]];
     if (p.offset + p.length > q.offset) return fail("overlapping sections");
   }

@@ -103,6 +103,7 @@ struct PinnedStage {
   double x[7];            // x of the solver parity hooks
   double pose[7];         // ll_transform / ll_transform_dev
   double mapper_pose[7];  // the mapper's world-frame transform of the new features
+  double loop_pose[7];    // loop feedback: the step's pose in the odometry frame (loop closure's transform of the step's full cloud)
   double extract_time;    // ExtractState::d_time
   int fe_counts[12];      // front end: RegArrays::counts ([0..2] get_features, [4..7] VoxelGrid outputs, [10..11] time-stamp range)
   int fe_meta[3];         // front end: ExtractState::d_meta
@@ -359,6 +360,10 @@ extern "C" void pg_odometry_edge(const ll_pose* prev, int id_prev, const ll_pose
 // every head); loop_select_piece picks piece i's.  loop_step runs at the end of a mapper step that appended its features (d_pose: the
 // registration pose on the device; pushed: the feature history took the step).
 struct LoopClosure;
+// What loop feedback (ll_mapper_set_loop_feedback; DESIGN.md §4.6.2) reads and moves in the mapper: its two history windows, the frame index
+// of each window segment (the windows are pushed and popped together: one index per segment of both), its pose, the pose of its last window
+// addition and its refresh flag.
+struct MapperWindow { HistoryWindow* his[2]; std::vector<int>* frame; double* q; double* t; double* last_q; double* last_t; bool* map_dirty; };
 int  loop_set(ll_ctx* ctx, LoopClosure** lc, const ll_loop_closure_cfg* cfg, const ll_mapper_config& mcfg, int pieces);
 void loop_release(LoopClosure* lc);
 int  loop_scan_cloud(ll_ctx* ctx, LoopClosure* lc, const ll_pipeline_cfg* pc);
@@ -368,20 +373,24 @@ int  loop_frame_clouds(ll_ctx* ctx, LoopClosure* lc, const FrameDev* dev, const 
 int  loop_sweep_cloud(ll_ctx* ctx, LoopClosure* lc, const float4* full, int n, const int* d_n);
 size_t loop_step_capacity(const LoopClosure* lc);   // points of the full cloud one step can hand over (max_scan_points: the world-frame buffer, one append)
 void loop_select_piece(LoopClosure* lc, int i);
-int  loop_step(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool pushed, int frame_index, const double q_w_curr[4], const double t_w_curr[3]);
+int  loop_step(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool pushed, int frame_index, const MapperWindow& mw);
 int  loop_read(LoopClosure* lc, ll_loop_event* out, int cap, int* n, int* n_dropped);
 // The loop image (ll_mapper_loop_save / _load / ll_loop_image_info; format: include/loamlivox_b200.h).  stamp: the mapper's binding stamp (the
 // fields of ll_loop_image_scalars before `closed`).  loop_load validates everything on the host first, builds a new loop closure and replaces
 // *lc only when the whole restore succeeded.
-int  loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& stamp, void* image, size_t cap, size_t* bytes);
+// With loop feedback on, the image (version 3) holds the window's frame indices, and its load sets them in the mapper.
+int  loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& stamp, const MapperWindow& mw, void* image, size_t cap, size_t* bytes);
 int  loop_load(ll_ctx* ctx, LoopClosure** lc, const void* image, size_t bytes, const ll_loop_closure_cfg* cfg, const ll_loop_image_scalars& stamp,
-               const ll_mapper_config& mcfg, int pieces);
+               const ll_mapper_config& mcfg, int pieces, const MapperWindow& mw);
 int  loop_image_info(const void* image, size_t bytes, ll_loop_image_summary* info);
 int  loop_result(const LoopClosure* lc, int* n, int* closed, ll_pose* poses_ori, ll_pose* poses_opt, int cap, ll_pg_edge* edge);
 int  loop_cloud(ll_ctx* ctx, const LoopClosure* lc, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev);
 // ll_mapper_set_loop_policy (lc NULL: loop closure off, refused) and ll_mapper_loop_edges
 int  loop_set_policy(ll_ctx* ctx, LoopClosure* lc, const ll_loop_policy* p);
 int  loop_edges(const LoopClosure* lc, ll_pg_edge* edges, int cap, int* n_loops);
+// ll_mapper_set_loop_feedback (lc NULL: loop closure off, refused) and ll_mapper_loop_correction_read
+int  loop_set_feedback(ll_ctx* ctx, LoopClosure* lc, const ll_mapper_config& mcfg, int on);
+void loop_correction(const LoopClosure* lc, double q_wxyz[4], double t[3], int* n_applied);
 
 // A log of the last entries (recovery's steps, loop closure's events), oldest first: a push into a full log overwrites the oldest unread entry
 // and counts it as dropped; a read takes the oldest entries and clears the dropped count.
@@ -415,8 +424,11 @@ const size_t HIS_HEAD = 16, CELLS_HEAD = 24;   // the fixed part of a history an
 // A header of magic[8], uint32 version, uint32 config_bytes, uint64 total_bytes and `sections` (offset, length) pairs.  image_header writes
 // it for sections of lengths len[] back to back in index order and returns the image's size; image_structure checks it (magic, a version in
 // version ... max_version, the config's size, total_bytes = the image's size, every section inside the image after the header, no two
-// overlapping) and gives the sections.
-struct ImageKind { const char* magic; const char* name; uint32_t version, max_version; uint32_t config_bytes; const char* config_name; int sections; };
+// overlapping) and gives the sections.  From version more_from on (0: never) the header holds one section more than `sections`.
+struct ImageKind {
+  const char* magic; const char* name; uint32_t version, max_version; uint32_t config_bytes; const char* config_name; int sections; uint32_t more_from = 0;
+  int count(uint32_t v) const { return sections + (more_from && v >= more_from ? 1 : 0); }
+};
 size_t image_header(const ImageKind& kind, uint32_t version, const uint64_t* len, void* header);
 int image_structure(const void* image, size_t bytes, const ImageKind& kind, ll_image_section* sec, std::string* err);
 bool finite_xyz(const uint8_t* p);       // the first three floats at p are finite

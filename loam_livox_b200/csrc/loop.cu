@@ -1,7 +1,8 @@
 // Loop closure inside the streaming mapper (ll_mapper_set_loop_closure; DESIGN.md §4.6): Laser_mapping::process_new_scan's keyframe block
 // (loam_livox/source/laser_mapping.hpp:1442, 1446-1459, 1480-1487, 1523-1564) and service_loop_detection (:874-1127), run by the mapper step
 // that appends its features, with every full cloud on the device.  Everything below is host orchestration of the library's own entry points
-// (transform, VoxelGrid, ll_keyframe_*, ll_loop_search, ll_scene_align, the pose graph, the re-pose) plus one gather kernel.
+// (transform, VoxelGrid, ll_keyframe_*, ll_loop_search, ll_scene_align, the pose graph, the re-pose) plus one gather kernel and, with loop
+// feedback on, one kernel that moves the mapper's history windows onto the optimized trajectory.
 #include <algorithm>
 #include <cmath>
 #include <cstddef>
@@ -9,6 +10,7 @@
 #include "common.cuh"
 #include "kernels.cuh"
 #include "cellmap.cuh"
+#include "exact_math.cuh"
 
 // grid (chunks, publish x heads): the full slice of head h for piece i goes to segment i after the slices of heads 0 .. h-1
 // (laser_feature_extractor.hpp:353-358 sums the heads' full clouds of a piece in head order).  Block (0, 0) also writes the segment ends.
@@ -24,6 +26,35 @@ __global__ void lc_gather_full_kernel(const FrameSlices* __restrict__ sl, FrameB
   const int t = threadIdx.x;
   if (t < publish) { int e = 0; for (int p = 0; p <= t; p++) for (int hh = 0; hh < n_heads; hh++) e += sl[hh].len[2][p]; seg_end[t] = e; }
 }
+
+// Loop feedback (DESIGN.md §4.6.2): both history windows moved in place, window w's point i (c: nc points, then s: ns points) by the delta of
+// its segment, the first whose end (ends[w * n_seg ...], staged in shared memory) is past i.  delta: n_seg poses (q w, x, y, z, t), fp64 from the
+// float point and rounded once, intensity kept: transform_kernel's arithmetic (qrot_d, then + t).
+__global__ void lc_window_correct_kernel(float4* __restrict__ c, int nc, float4* __restrict__ s, int ns, const int* __restrict__ ends, int n_seg,
+                                         const double* __restrict__ delta) {
+  extern __shared__ int sh_end[];
+  for (int k = threadIdx.x; k < 2 * n_seg; k += blockDim.x) sh_end[k] = ends[k];
+  __syncthreads();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nc + ns) return;
+  const bool surf = i >= nc;
+  const int j = surf ? i - nc : i;
+  const int* e = sh_end + (surf ? n_seg : 0);
+  int lo = 0, hi = n_seg - 1;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (e[mid] > j) hi = mid; else lo = mid + 1; }
+  float4* p = surf ? s + j : c + j;
+  const float4 v = *p;
+  const double* d = delta + 7 * lo;
+  const double q[4] = {d[0], d[1], d[2], d[3]};
+  double wx, wy, wz; qrot_d(q, (double)v.x, (double)v.y, (double)v.z, wx, wy, wz);
+  *p = make_float4((float)(wx + d[4]), (float)(wy + d[5]), (float)(wz + d[6]), v.w);
+}
+
+// feedback: the step's odometry-frame pose, then per window segment its delta (7 doubles) and both windows' segment ends
+struct FeedbackLayout {
+  double* pose; double* delta; int* ends;
+  void layout(Carve& k, size_t n_seg) { pose = k.take<double>(7); delta = k.take<double>(7 * n_seg); ends = k.take<int>(2 * n_seg); }
+};
 
 // in: the step's full cloud (a scan: the compaction's three outputs, only `full` kept; a frame: the published pieces one after another), the
 // compaction's counts, the pieces' ends
@@ -63,6 +94,13 @@ struct LoopClosure {
   bool done() const { return (int)loops.size() >= policy.max_loops; }   // all loop-closure work stops (if_end after the first loop by default)
   DevBuf refine; std::vector<int> ref_end;           // RefineLayout: the re-posed clouds of every keyframe
   EventLog<ll_loop_event> log;
+  // loop feedback (ll_mapper_set_loop_feedback): each closed keyframe's frame index (-1: restored from an image that does not record it), the
+  // correction applied last (C) and how many were applied; fb: FeedbackLayout for maximum_history_size segments
+  bool feedback = false;
+  std::vector<int> kf_frame;
+  ll_pose corr{{1, 0, 0, 0}, {0, 0, 0}};
+  int n_applied = 0;
+  DevBuf fb;
 };
 
 namespace {
@@ -117,6 +155,57 @@ int grow_keep(ll_ctx* ctx, DevBuf& b, size_t used, size_t need) {
   return LL_OK;
 }
 
+// ---- poses in fp64 (ll_pose: q w, x, y, z and t), as the feedback and ll_loop_correction compose them
+const ll_pose IDENTITY{{1, 0, 0, 0}, {0, 0, 0}};
+void qrot_h(const double* q, const double* v, double* o) {   // qrot_d's association on the host
+  const double ux = q[1], uy = q[2], uz = q[3], w = q[0];
+  double cx = uy * v[2] - uz * v[1], cy = uz * v[0] - ux * v[2], cz = ux * v[1] - uy * v[0];
+  cx = cx + cx; cy = cy + cy; cz = cz + cz;
+  const double dx = uy * cz - uz * cy, dy = uz * cx - ux * cz, dz = ux * cy - uy * cx;
+  o[0] = (v[0] + cx * w) + dx; o[1] = (v[1] + cy * w) + dy; o[2] = (v[2] + cz * w) + dz;
+}
+ll_pose compose(const ll_pose& a, const ll_pose& b) {   // a o b: (q_a q_b, R_a t_b + t_a)
+  ll_pose o; quat_mul(a.q_wxyz, b.q_wxyz, o.q_wxyz);
+  double r[3]; qrot_h(a.q_wxyz, b.t, r);
+  for (int k = 0; k < 3; k++) o.t[k] = r[k] + a.t[k];
+  return o;
+}
+ll_pose inverse(const ll_pose& a) {   // (q*, -(R* t))
+  ll_pose o; o.q_wxyz[0] = a.q_wxyz[0]; for (int k = 1; k < 4; k++) o.q_wxyz[k] = -a.q_wxyz[k];
+  double r[3]; qrot_h(o.q_wxyz, a.t, r);
+  for (int k = 0; k < 3; k++) o.t[k] = -r[k];
+  return o;
+}
+bool finite_pose(const ll_pose& p) { return finite_d(p.q_wxyz, 4) && finite_d(p.t, 3); }
+
+// A_k = opt_k o ori_k^-1; A_0 the identity (the graph holds pose 0 constant)
+ll_pose keyframe_correction(const ll_pose* ori, const ll_pose* opt, int k) { return k == 0 ? IDENTITY : compose(opt[k], inverse(ori[k])); }
+
+// ll_loop_correction on checked inputs (f strictly ascending, n >= 1)
+ll_pose correction_at(const ll_pose* ori, const ll_pose* opt, const int* f, int n, int s) {
+  if (s <= f[0]) return IDENTITY;
+  if (s >= f[n - 1]) return keyframe_correction(ori, opt, n - 1);
+  const int k = (int)(std::upper_bound(f, f + n, s) - f) - 1;   // f[k] <= s < f[k + 1]
+  const ll_pose a = keyframe_correction(ori, opt, k);
+  if (s == f[k]) return a;
+  const ll_pose b = keyframe_correction(ori, opt, k + 1);
+  const double u = (double)(s - f[k]) / (double)(f[k + 1] - f[k]);
+  // slerp along the shorter arc: theta the angle between the quaternions as 4-vectors, 2 atan2(|a - b|, |a + b|)
+  double qb[4], dot = 0, dn = 0, sn = 0;
+  for (int j = 0; j < 4; j++) dot = dot + a.q_wxyz[j] * b.q_wxyz[j];
+  for (int j = 0; j < 4; j++) qb[j] = dot < 0 ? -b.q_wxyz[j] : b.q_wxyz[j];
+  for (int j = 0; j < 4; j++) { const double x = a.q_wxyz[j] - qb[j], y = a.q_wxyz[j] + qb[j]; dn = dn + x * x; sn = sn + y * y; }
+  const double theta = 2.0 * std::atan2(std::sqrt(dn), std::sqrt(sn));
+  ll_pose o;
+  if (theta == 0.0) { for (int j = 0; j < 4; j++) o.q_wxyz[j] = a.q_wxyz[j]; }
+  else {
+    const double st = std::sin(theta), wa = std::sin((1.0 - u) * theta) / st, wb = std::sin(u * theta) / st;
+    for (int j = 0; j < 4; j++) o.q_wxyz[j] = wa * a.q_wxyz[j] + wb * qb[j];
+  }
+  for (int j = 0; j < 3; j++) o.t[j] = a.t[j] + u * (b.t[j] - a.t[j]);
+  return o;
+}
+
 ll_loop_event* log_push(LoopClosure* lc, int kind) {
   ll_loop_event* e = lc->log.push();
   e->kind = kind; e->keyframe = (int)lc->kfs.size() - 1;
@@ -148,9 +237,58 @@ int loop_refine(ll_ctx* ctx, LoopClosure* lc) {
   return LL_OK;
 }
 
+// Loop feedback after a loop (DESIGN.md §4.6.2): prev holds the previous loop's optimized poses, lc->opt this loop's.  Everything is computed
+// and checked on the host before the one upload and the one launch; the mapper's host state moves after them.
+int feedback_apply(ll_ctx* ctx, LoopClosure* lc, const std::vector<ll_pose>& prev, const MapperWindow& mw) {
+  const int n = (int)lc->opt.size(), np = lc->n_applied ? (int)prev.size() : 0;
+  const std::vector<int>& fr = *mw.frame;
+  const int S = (int)fr.size();
+  const HistoryWindow& hc = *mw.his[0]; const HistoryWindow& hs = *mw.his[1];
+  if ((size_t)S != hc.segs.size() || (size_t)S != hs.segs.size()) { ctx->set_error("loop feedback: window segments and their frame indices disagree"); return LL_ERR_INVALID; }
+  if (S > lc->max_history) { ctx->set_error("loop feedback: more window segments than maximum_history_size"); return LL_ERR_INVALID; }
+  if (hc.live() + hs.live() > (size_t)INT32_MAX) { ctx->set_error("loop feedback: more than 2^31 - 1 window points"); return LL_ERR_INVALID; }
+  for (int k = 0; k < n; k++) if (lc->kf_frame[k] < 0 || (k && lc->kf_frame[k] <= lc->kf_frame[k - 1])) { ctx->set_error("loop feedback: keyframe frame indices"); return LL_ERR_INVALID; }
+  std::vector<double> delta(7 * (size_t)S);
+  std::vector<int> ends(2 * (size_t)S);
+  for (int i = 0; i < S; i++) {
+    const ll_pose a = correction_at(lc->poses.data(), lc->opt.data(), lc->kf_frame.data(), n, fr[i]);
+    const ll_pose b = np ? correction_at(lc->poses.data(), prev.data(), lc->kf_frame.data(), np, fr[i]) : IDENTITY;
+    const ll_pose d = compose(a, inverse(b));
+    if (!finite_pose(d)) { ctx->set_error("loop feedback: non-finite correction"); return LL_ERR_INVALID; }
+    memcpy(&delta[7 * (size_t)i], d.q_wxyz, 4 * sizeof(double)); memcpy(&delta[7 * (size_t)i + 4], d.t, 3 * sizeof(double));
+    ends[i] = (int)(hc.segs[i].first + hc.segs[i].second - hc.head()); ends[S + i] = (int)(hs.segs[i].first + hs.segs[i].second - hs.head());
+  }
+  const ll_pose a_new = keyframe_correction(lc->poses.data(), lc->opt.data(), n - 1);
+  ll_pose last; memcpy(last.q_wxyz, mw.last_q, sizeof(last.q_wxyz)); memcpy(last.t, mw.last_t, sizeof(last.t));
+  last = compose(compose(a_new, inverse(lc->corr)), last);   // the last addition was in the frame of the previous correction
+  if (!finite_pose(a_new) || !finite_pose(last) || !finite_pose(lc->opt[n - 1])) { ctx->set_error("loop feedback: non-finite correction"); return LL_ERR_INVALID; }
+  const int nc = (int)hc.live(), ns = (int)hs.live();
+  if (S > 0 && nc + ns > 0) {
+    cudaStream_t s = ctx->stream;
+    FeedbackLayout fl; LL_CUDA(ctx, lc->fb.carve([&](Carve& k) { fl.layout(k, (size_t)S); }));   // (reserved: no reallocation)
+    LL_CUDA(ctx, cudaMemcpyAsync(fl.delta, delta.data(), delta.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+    LL_CUDA(ctx, cudaMemcpyAsync(fl.ends, ends.data(), ends.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    lc_window_correct_kernel<<<ll_div_up(nc + ns, 256), 256, 2 * S * sizeof(int), s>>>((float4*)hc.data(), nc, (float4*)hs.data(), ns, fl.ends, S, fl.delta);
+    ctx->launches++;
+    LL_CUDA(ctx, cudaGetLastError());
+  }
+  memcpy(mw.q, lc->opt[n - 1].q_wxyz, 4 * sizeof(double)); memcpy(mw.t, lc->opt[n - 1].t, 3 * sizeof(double));
+  memcpy(mw.last_q, last.q_wxyz, 4 * sizeof(double)); memcpy(mw.last_t, last.t, 3 * sizeof(double));
+  *mw.map_dirty = true;
+  lc->corr = a_new; lc->n_applied++;
+  return LL_OK;
+}
+
+// The feedback's device buffer for maximum_history_size segments, so that no step allocates it.
+int feedback_reserve(ll_ctx* ctx, LoopClosure* lc) {
+  cudaSetDevice(ctx->device);
+  FeedbackLayout fl; LL_CUDA(ctx, lc->fb.reserve_floor(layout_bytes([&](Carve& k) { fl.layout(k, (size_t)std::max(lc->max_history, 0)); })));
+  return LL_OK;
+}
+
 // The candidates of the newest keyframe (ll_loop_search's, his ascending) through the alignment with the skips of :1048-1052 and
-// :1113-1116, and on a loop the graph and the refined clouds (:1056-1100).
-int loop_align(ll_ctx* ctx, LoopClosure* lc, const std::vector<int>& cand) {
+// :1113-1116, and on a loop the graph, the refined clouds (:1056-1100) and, with loop feedback on, the correction of the mapper.
+int loop_align(ll_ctx* ctx, LoopClosure* lc, const std::vector<int>& cand, const MapperWindow& mw) {
   const ll_loop_closure_cfg& c = lc->cfg;
   const int n = (int)lc->kfs.size(), newest = n - 1;
   ll_align_cfg acfg; ll_align_cfg_default(&acfg);
@@ -192,6 +330,7 @@ int loop_align(ll_ctx* ctx, LoopClosure* lc, const std::vector<int>& cand) {
     lc->loops.push_back(le);
     ll_loop_event* ce = log_push(lc, LL_LOOP_CLOSED);
     ce->his = his; ce->edge = le; ce->summary = sum;
+    if (lc->feedback) LL_TRY(feedback_apply(ctx, lc, opt, mw));   // (opt: the previous loop's poses after the swap)
     return LL_OK;
   }
   return LL_OK;
@@ -281,10 +420,19 @@ void loop_select_piece(LoopClosure* lc, int i) { lc->piece = i; }
 
 namespace {
 
-int loop_step_work(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool pushed, int frame_index, const double q_w_curr[4], const double t_w_curr[3]) {
+int loop_step_work(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool pushed, int frame_index, const MapperWindow& mw) {
   cudaStream_t s = ctx->stream;
   const ll_loop_closure_cfg& c = lc->cfg;
   LoopInLayout il; LL_CUDA(ctx, lc->in.carve([&](Carve& k) { il.layout(k, lc->in_full, lc->in_scan); }));   // (reserved: no reallocation)
+  // the step's pose: the mapper's, or after a correction C^-1 o the mapper's (loop closure stays in the odometry frame)
+  ll_pose p; memcpy(p.q_wxyz, mw.q, sizeof(p.q_wxyz)); memcpy(p.t, mw.t, sizeof(p.t));
+  if (lc->n_applied) {
+    p = compose(inverse(lc->corr), p);
+    double* h = ctx->pin->loop_pose; memcpy(h, p.q_wxyz, 4 * sizeof(double)); memcpy(h + 4, p.t, 3 * sizeof(double));
+    FeedbackLayout fl; LL_CUDA(ctx, lc->fb.carve([&](Carve& k) { fl.layout(k, (size_t)std::max(lc->max_history, 0)); }));   // (reserved: no reallocation)
+    LL_CUDA(ctx, cudaMemcpyAsync(fl.pose, h, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
+    d_pose = fl.pose;
+  }
   if (!lc->seg_read) {   // the captured cloud's ends (the mapper step has synchronised the stream already: no wait here)
     LL_CUDA(ctx, cudaMemcpyAsync(lc->seg.data(), il.seg_end, lc->seg.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
     LL_CUDA(ctx, cudaStreamSynchronize(s));
@@ -325,8 +473,8 @@ int loop_step_work(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool push
   if (!closing) return LL_OK;
   // process it now (:931-960): analyze, the pose and its odometry edge, then the search
   lc->kfs.push_back(closing);
-  ll_pose p; for (int k = 0; k < 4; k++) p.q_wxyz[k] = q_w_curr[k]; for (int k = 0; k < 3; k++) p.t[k] = t_w_curr[k];
   lc->poses.push_back(p);
+  lc->kf_frame.push_back(frame_index);
   const int id = (int)lc->kfs.size() - 1;
   if (id >= 1) { ll_pg_edge e; pg_odometry_edge(&lc->poses[id - 1], id - 1, &lc->poses[id], id, &e); lc->edges.push_back(e); }
   ll_keyframe_info info;
@@ -340,15 +488,15 @@ int loop_step_work(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool push
   ll_loop_event* ke = log_push(lc, LL_LOOP_KEYFRAME);
   ke->ending_frame_idx = frame_index; ke->n_candidates = nc; ke->info = info;
   memcpy(ke->q_wxyz, p.q_wxyz, sizeof(p.q_wxyz)); memcpy(ke->t, p.t, sizeof(p.t));
-  return loop_align(ctx, lc, cand);
+  return loop_align(ctx, lc, cand, mw);
 }
 
 }  // namespace
 
 // Loop closure never fails the step: an error of its work other than LL_ERR_CUDA is logged (LL_LOOP_ERROR) and stops it for good.
-int loop_step(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool pushed, int frame_index, const double q_w_curr[4], const double t_w_curr[3]) {
+int loop_step(ll_ctx* ctx, LoopClosure* lc, const double* d_pose, bool pushed, int frame_index, const MapperWindow& mw) {
   if (lc->done() || lc->stopped) return LL_OK;
-  const int st = loop_step_work(ctx, lc, d_pose, pushed, frame_index, q_w_curr, t_w_curr);
+  const int st = loop_step_work(ctx, lc, d_pose, pushed, frame_index, mw);
   if (st == LL_OK || st == LL_ERR_CUDA) return st;
   ll_loop_event* e = log_push(lc, LL_LOOP_ERROR);
   e->status = st; e->ending_frame_idx = frame_index;
@@ -411,6 +559,25 @@ int loop_set_policy(ll_ctx* ctx, LoopClosure* lc, const ll_loop_policy* p) {
   return LL_OK;
 }
 
+int loop_set_feedback(ll_ctx* ctx, LoopClosure* lc, const ll_mapper_config& mcfg, int on) {
+  if (!lc) { ctx->set_error("loop closure is off: set it before loop feedback"); return LL_ERR_INVALID; }
+  if (!lc->loops.empty()) { ctx->set_error("a loop has closed already: loop feedback is set before the first loop"); return LL_ERR_INVALID; }
+  if (on && mcfg.matching_mode != 0) { ctx->set_error("loop feedback needs matching mode 0 (a cell-map point of mode 1 does not record its step)"); return LL_ERR_INVALID; }
+  if (on && mcfg.maximum_history_size > LL_LOOP_FEEDBACK_MAX_SEGMENTS) { ctx->set_error("loop feedback: maximum_history_size above LL_LOOP_FEEDBACK_MAX_SEGMENTS"); return LL_ERR_INVALID; }
+  if (on && std::any_of(lc->kf_frame.begin(), lc->kf_frame.end(), [](int f) { return f < 0; })) {
+    ctx->set_error("loop feedback: keyframes restored from a loop image that does not record their frame indices"); return LL_ERR_INVALID;
+  }
+  if (on) LL_TRY(feedback_reserve(ctx, lc));
+  lc->feedback = on != 0;
+  return LL_OK;
+}
+
+void loop_correction(const LoopClosure* lc, double q_wxyz[4], double t[3], int* n_applied) {
+  const ll_pose c = lc ? lc->corr : IDENTITY;
+  memcpy(q_wxyz, c.q_wxyz, sizeof(c.q_wxyz)); memcpy(t, c.t, sizeof(c.t));
+  if (n_applied) *n_applied = lc ? lc->n_applied : 0;
+}
+
 int loop_cloud(ll_ctx* ctx, const LoopClosure* lc, int k, ll_point* out_host, size_t cap, size_t* n_out, const ll_point** out_dev) {
   if (!lc || lc->loops.empty()) { ctx->set_error("no loop closed"); return LL_ERR_INVALID; }
   const int N = (int)lc->opt.size();   // n_opt: loop_refine's layout of the latest loop
@@ -435,17 +602,18 @@ int loop_cloud(ll_ctx* ctx, const LoopClosure* lc, int k, ll_point* out_host, si
 // touches the device; the save writes the sections back to back in index order.
 namespace {
 
-const ImageKind LOOP_IMAGE{LL_LOOP_IMAGE_MAGIC, "loop", LL_LOOP_IMAGE_VERSION, LL_LOOP_IMAGE_VERSION_POLICY, sizeof(ll_loop_closure_cfg), "ll_loop_closure_cfg",
-                           LL_LOOP_IMAGE_SECTIONS};
+const ImageKind LOOP_IMAGE{LL_LOOP_IMAGE_MAGIC, "loop", LL_LOOP_IMAGE_VERSION, LL_LOOP_IMAGE_VERSION_FEEDBACK, sizeof(ll_loop_closure_cfg), "ll_loop_closure_cfg",
+                           LL_LOOP_IMAGE_SECTIONS, LL_LOOP_IMAGE_VERSION_FEEDBACK};
 const size_t LI_ACC_HEAD = 8, LI_IMG = 4 * 3600 * 4;                   // the accumulated section's fixed part; one keyframe's four images
 const size_t LI_STAMP = offsetof(ll_loop_image_scalars, closed);       // the binding stamp: the scalars before `closed`
 const size_t LI_LOOP2_HEAD = sizeof(ll_loop_policy) + 8;               // version 2's LOOP section: the policy, n_loops, 0
+const size_t LI_FB_HEAD = 8 + sizeof(ll_pose) + 16;                    // version 3's FEEDBACK section: on, n_applied, C, n_keyframes, n_segments
 
 bool policy_default(const ll_loop_policy& p) { return p.max_loops == 1 && p.min_keyframes_between_loops == 0; }
 int edge_newest(const ll_pg_edge& e) { return std::max(e.id_begin, e.id_end); }
 
 struct LoopView {   // a validated loop image
-  ll_loop_image_header h; ll_loop_closure_cfg cfg; ll_loop_image_scalars sc;
+  ll_loop_image_header h; ll_image_section sec[LL_LOOP_IMAGE_SECTIONS_FEEDBACK]; ll_loop_closure_cfg cfg; ll_loop_image_scalars sc;
   CellsView cells;
   HistoryView his;
   const uint8_t* open = nullptr; const uint8_t* refs = nullptr; int64_t open_cells = 0;
@@ -453,9 +621,10 @@ struct LoopView {   // a validated loop image
   int64_t n_acc = 0, acc_pts = 0; const uint8_t* acc_end = nullptr; const uint8_t* acc = nullptr;
   ll_loop_policy policy{1, 0}; int64_t n_loops = 0, n_opt = 0;   // the LOOP section: the policy (version 2), loop edges and optimized poses
   const uint8_t* loop_edges = nullptr; const uint8_t* loop_opt = nullptr; const uint8_t* events = nullptr;
+  // the FEEDBACK section (version 3): n_applied, C, the keyframes' and the window segments' frame indices
+  bool feedback = false; int n_applied = 0; ll_pose corr; int64_t n_fb_seg = 0; const uint8_t* kf_frame = nullptr; const uint8_t* seg_frame = nullptr;
 };
 
-bool finite_pose(const ll_pose& p) { return finite_d(p.q_wxyz, 4) && finite_d(p.t, 3); }
 bool finite_edge(const ll_pg_edge& e) { return finite_d(e.q_wxyz, 4) && finite_d(e.t, 3) && finite_d(e.information, 36); }
 
 // LL_OK, or the code and what is wrong.  load: the image is to be loaded with cfg (NULL: the image's config), so the cell table that cfg's
@@ -463,11 +632,11 @@ bool finite_edge(const ll_pg_edge& e) { return finite_d(e.q_wxyz, 4) && finite_d
 // max_cells can need one).
 int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_closure_cfg* cfg, LoopView* v, std::string* err) {
   auto fail = [&](const std::string& msg, int code = LL_ERR_INVALID) { if (err) *err = msg; return code; };
-  LL_TRY(image_structure(image, bytes, LOOP_IMAGE, v->h.section, err));
+  LL_TRY(image_structure(image, bytes, LOOP_IMAGE, v->sec, err));
   const uint8_t* b = (const uint8_t*)image;
   memcpy(&v->h, b, sizeof(v->h));
-  auto sec = [&](int k) { return b + v->h.section[k].offset; };
-  auto len = [&](int k) { return (uint64_t)v->h.section[k].length; };
+  auto sec = [&](int k) { return b + v->sec[k].offset; };
+  auto len = [&](int k) { return (uint64_t)v->sec[k].length; };
   // config: ll_mapper_set_loop_closure's checks
   if (len(LL_LOOP_IMAGE_CONFIG) != sizeof(ll_loop_closure_cfg)) return fail("config section length");
   memcpy(&v->cfg, sec(LL_LOOP_IMAGE_CONFIG), sizeof(v->cfg));
@@ -562,8 +731,8 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
     v->n_acc = n; v->acc_pts = prev; v->acc_end = p + LI_ACC_HEAD; v->acc = p + LI_ACC_HEAD + 8 * n;
     for (int64_t k = 0; k < prev; k++) if (!finite_xyz(v->acc + 16 * k)) return fail("non-finite accumulated point");
   }
-  // the loop.  Version 1: the edge between two keyframes and the optimized poses, only when closed.  Version 2: the policy, the loop edges in
-  // closing order and the latest optimized poses
+  // the loop.  Version 1: the edge between two keyframes and the optimized poses, only when closed.  Versions 2 and 3: the policy, the loop
+  // edges in closing order and the latest optimized poses
   {
     const uint64_t L = len(LL_LOOP_IMAGE_LOOP);
     const uint8_t* p = sec(LL_LOOP_IMAGE_LOOP);
@@ -580,7 +749,8 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
       if (L < LI_LOOP2_HEAD) return fail("version-2 loop section shorter than its policy and count");
       v->policy = img_get<ll_loop_policy>(p);
       const int32_t nl = img_get<int32_t>(p + sizeof(ll_loop_policy)), pad = img_get<int32_t>(p + sizeof(ll_loop_policy) + 4);
-      if (v->policy.max_loops < 2 || v->policy.max_loops > LL_MAX_LOOPS) return fail("version-2 max_loops outside 2 ... LL_MAX_LOOPS (the default policy writes version 1)");
+      const int lo = v->h.version == LL_LOOP_IMAGE_VERSION_POLICY ? 2 : 1;   // (without feedback the default policy writes version 1)
+      if (v->policy.max_loops < lo || v->policy.max_loops > LL_MAX_LOOPS) return fail("max_loops outside " + std::to_string(lo) + " ... LL_MAX_LOOPS");
       if (v->policy.min_keyframes_between_loops < 0) return fail("negative min_keyframes_between_loops");
       if (pad != 0) return fail("loop section padding not zero");
       if (nl < 0 || nl > v->policy.max_loops) return fail("n_loops outside 0 ... max_loops");
@@ -601,6 +771,31 @@ int loop_validate(const void* image, size_t bytes, bool load, const ll_loop_clos
     v->loop_edges = p + head;
     v->loop_opt = p + head + sizeof(ll_pg_edge) * (size_t)v->n_loops;
     for (int64_t k = 0; k < v->n_opt; k++) if (!finite_pose(img_get<ll_pose>(v->loop_opt + sizeof(ll_pose) * k))) return fail("non-finite optimized pose");
+  }
+  // loop feedback (version 3): the correction, the keyframes' frame indices and the window segments' (their count is checked by the load)
+  if (v->h.version == LL_LOOP_IMAGE_VERSION_FEEDBACK) {
+    const uint8_t* p = sec(LL_LOOP_IMAGE_FEEDBACK); const uint64_t L = len(LL_LOOP_IMAGE_FEEDBACK);
+    if (L < LI_FB_HEAD) return fail("feedback section shorter than its head");
+    const int32_t on = img_get<int32_t>(p), na = img_get<int32_t>(p + 4);
+    v->corr = img_get<ll_pose>(p + 8);
+    const int64_t nk = img_get<int64_t>(p + 8 + sizeof(ll_pose)), ns = img_get<int64_t>(p + 16 + sizeof(ll_pose));
+    if (on != 1) return fail("feedback flag not 1");
+    if (na < 0 || na > v->n_loops || (na < v->n_loops && !sc.stopped)) return fail("corrections applied outside 0 ... n_loops (fewer only when stopped)");
+    if (!finite_pose(v->corr)) return fail("non-finite correction");
+    if (na == 0 && memcmp(&v->corr, &IDENTITY, sizeof(ll_pose)) != 0) return fail("a correction other than the identity before one was applied");
+    if (nk != K) return fail("feedback keyframes disagree with n_keyframes");
+    if (ns < 0 || (uint64_t)ns > (L - LI_FB_HEAD) / 4 || LI_FB_HEAD + 4 * ((uint64_t)nk + (uint64_t)ns) != L) return fail("feedback counts disagree with the section length");
+    if (sc.maximum_history_size >= 0 && ns > sc.maximum_history_size) return fail("more window segments than maximum_history_size");
+    const uint8_t* kf = p + LI_FB_HEAD; const uint8_t* sg = kf + 4 * nk;
+    for (int64_t k = 0; k < nk; k++) {
+      const int32_t f = img_get<int32_t>(kf + 4 * k);
+      if (f < 0 || f > sc.frame_index || (k && f <= img_get<int32_t>(kf + 4 * (k - 1)))) return fail("keyframe frame indices not strictly ascending within 0 ... frame_index");
+    }
+    for (int64_t k = 0; k < ns; k++) {
+      const int32_t f = img_get<int32_t>(sg + 4 * k);
+      if (f < 0 || f > sc.frame_index || (k && f <= img_get<int32_t>(sg + 4 * (k - 1)))) return fail("window frame indices not strictly ascending within 0 ... frame_index");
+    }
+    v->feedback = true; v->n_applied = na; v->n_fb_seg = ns; v->kf_frame = kf; v->seg_frame = sg;
   }
   // the unread events
   {
@@ -672,6 +867,14 @@ int loop_restore(ll_ctx* ctx, LoopClosure* lc, const LoopView& v) {
   lc->opt.resize((size_t)v.n_opt);
   for (int64_t k = 0; k < v.n_opt; k++) lc->opt[k] = img_get<ll_pose>(v.loop_opt + sizeof(ll_pose) * k);
   if (v.n_loops) LL_TRY(loop_refine(ctx, lc));
+  // loop feedback: on with its frame indices (version 3), else off with the keyframes' frame indices unknown
+  lc->kf_frame.assign((size_t)K, -1);
+  if (v.feedback) {
+    LL_TRY(feedback_reserve(ctx, lc));
+    lc->feedback = true;
+    for (int k = 0; k < K; k++) lc->kf_frame[k] = img_get<int32_t>(v.kf_frame + 4 * k);
+    lc->corr = v.corr; lc->n_applied = v.n_applied;
+  }
   lc->log.restore(v.events, (size_t)sc.n_events, sc.n_dropped);   // the unread events
   LL_CUDA(ctx, cudaGetLastError());
   LL_CUDA(ctx, cudaStreamSynchronize(s));
@@ -680,7 +883,7 @@ int loop_restore(ll_ctx* ctx, LoopClosure* lc, const LoopView& v) {
 
 }  // namespace
 
-int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& stamp, void* image, size_t cap, size_t* bytes) {
+int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& stamp, const MapperWindow& mw, void* image, size_t cap, size_t* bytes) {
   cudaStream_t s = ctx->stream;
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   // the incarnations the open keyframes hold (sorted, distinct), on the device for the export
@@ -716,23 +919,29 @@ int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& s
     cloud_pts += infos[k].line_points + infos[k].plane_points;
   }
   const uint64_t acc_pts = lc->acc_end.empty() ? 0 : lc->acc_end.back();
-  // v2: a policy other than the default (version 2); n_opt: the latest optimization's keyframes
-  const bool v2 = !policy_default(lc->policy);
+  // v2: a policy other than the default (version 2) or loop feedback (version 3, which adds the FEEDBACK section); n_opt: the latest
+  // optimization's keyframes
+  const bool v3 = lc->feedback, v2 = v3 || !policy_default(lc->policy);
+  const uint64_t n_seg = v3 ? mw.frame->size() : 0;
   const uint64_t n_loops = lc->loops.size(), n_opt = n_loops ? lc->opt.size() : 0;
   const uint64_t loop_len = v2 ? LI_LOOP2_HEAD + sizeof(ll_pg_edge) * n_loops + sizeof(ll_pose) * n_opt : n_loops ? sizeof(ll_pg_edge) + sizeof(ll_pose) * n_opt : 0;
-  const uint64_t len[LL_LOOP_IMAGE_SECTIONS] = {
+  const uint64_t len[LL_LOOP_IMAGE_SECTIONS_FEEDBACK] = {
       sizeof(ll_loop_closure_cfg), sizeof(ll_loop_image_scalars), cells_bytes(cells, true), history_bytes(lc->his),
       sizeof(ll_loop_image_open) * lc->open.size() + sizeof(ll_loop_image_ref) * open_cells, sizeof(ll_keyframe_info) * K, sizeof(ll_pose) * K,
       sizeof(ll_pg_edge) * (K ? K - 1 : 0), LI_IMG * K, 16 * cloud_pts, LI_ACC_HEAD + 8 * lc->acc_end.size() + 16 * acc_pts, loop_len,
-      sizeof(ll_loop_event) * lc->log.count};
-  ll_loop_image_header h;
-  const size_t total = image_header(LOOP_IMAGE, v2 ? LL_LOOP_IMAGE_VERSION_POLICY : LL_LOOP_IMAGE_VERSION, len, &h);
+      sizeof(ll_loop_event) * lc->log.count, LI_FB_HEAD + 4 * (K + n_seg)};
+  uint8_t hbuf[24 + 16 * LL_LOOP_IMAGE_SECTIONS_FEEDBACK];
+  const uint32_t version = v3 ? LL_LOOP_IMAGE_VERSION_FEEDBACK : v2 ? LL_LOOP_IMAGE_VERSION_POLICY : LL_LOOP_IMAGE_VERSION;
+  const size_t total = image_header(LOOP_IMAGE, version, len, hbuf);
+  const size_t head = 24 + 16 * (size_t)LOOP_IMAGE.count(version);
+  ll_image_section sec[LL_LOOP_IMAGE_SECTIONS_FEEDBACK];
+  memcpy(sec, hbuf + 24, head - 24);
   *bytes = total;
   if (!image) return LL_OK;
   if (cap < total) { ctx->set_error("image buffer smaller than the loop image (query the size with image = NULL)"); return LL_ERR_CAPACITY; }
   uint8_t* b = (uint8_t*)image;
-  auto at = [&](int k) { return b + h.section[k].offset; };
-  memcpy(b, &h, sizeof(h));
+  auto at = [&](int k) { return b + sec[k].offset; };
+  memcpy(b, hbuf, head);
   memcpy(at(LL_LOOP_IMAGE_CONFIG), &lc->cfg, sizeof(lc->cfg));
   ll_loop_image_scalars sc = stamp;
   sc.closed = lc->loops.empty() ? 0 : 1; sc.stopped = lc->stopped ? 1 : 0;
@@ -792,12 +1001,21 @@ int loop_save(ll_ctx* ctx, const LoopClosure* lc, const ll_loop_image_scalars& s
     e.summary.cycles_eval = e.summary.cycles_elim = e.summary.cycles_border = e.summary.cycles_total = 0;
     img_put(at(LL_LOOP_IMAGE_EVENTS) + sizeof(ll_loop_event) * k, e);
   }
+  // loop feedback: the correction, then the keyframes' and the window segments' frame indices
+  if (v3) {
+    p = at(LL_LOOP_IMAGE_FEEDBACK);
+    img_put<int32_t>(p, 1); img_put<int32_t>(p + 4, lc->n_applied); img_put(p + 8, lc->corr);
+    img_put<int64_t>(p + 8 + sizeof(ll_pose), (int64_t)K); img_put<int64_t>(p + 16 + sizeof(ll_pose), (int64_t)n_seg);
+    p += LI_FB_HEAD;
+    for (size_t k = 0; k < K; k++, p += 4) img_put<int32_t>(p, lc->kf_frame[k]);
+    for (uint64_t k = 0; k < n_seg; k++, p += 4) img_put<int32_t>(p, (*mw.frame)[k]);
+  }
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   return LL_OK;
 }
 
 int loop_load(ll_ctx* ctx, LoopClosure** plc, const void* image, size_t bytes, const ll_loop_closure_cfg* cfg, const ll_loop_image_scalars& stamp,
-              const ll_mapper_config& mcfg, int pieces) {
+              const ll_mapper_config& mcfg, int pieces, const MapperWindow& mw) {
   LoopView v; std::string err;
   const int st = loop_validate(image, bytes, true, cfg, &v, &err);
   if (st != LL_OK) { ctx->set_error("loop image refused: " + err); return st; }
@@ -806,6 +1024,11 @@ int loop_load(ll_ctx* ctx, LoopClosure** plc, const void* image, size_t bytes, c
                    "maximum_history_size, pieces) differs from the mapper's");
     return LL_ERR_INVALID;
   }
+  if (v.feedback && ((size_t)v.n_fb_seg != mw.his[0]->segs.size() || (size_t)v.n_fb_seg != mw.his[1]->segs.size())) {
+    ctx->set_error("loop image refused: its window segments differ from the mapper's history windows");
+    return LL_ERR_INVALID;
+  }
+  if (v.feedback && mcfg.matching_mode != 0) { ctx->set_error("loop image refused: loop feedback needs matching mode 0"); return LL_ERR_INVALID; }
   cudaSetDevice(ctx->device);
   LoopClosure* lc = nullptr;
   LL_TRY(loop_set(ctx, &lc, cfg ? cfg : &v.cfg, mcfg, pieces));
@@ -813,6 +1036,8 @@ int loop_load(ll_ctx* ctx, LoopClosure** plc, const void* image, size_t bytes, c
   const int rs = loop_restore(ctx, lc, v);
   if (rs != LL_OK) { loop_release(lc); return rs; }
   lc->cfg = v.cfg;   // cfg's allocation sizes were read by loop_set only; later images keep the image's config
+  if (v.feedback) mw.frame->clear();
+  for (int64_t k = 0; v.feedback && k < v.n_fb_seg; k++) mw.frame->push_back(img_get<int32_t>(v.seg_frame + 4 * k));
   loop_release(*plc);
   *plc = lc;
   return LL_OK;
@@ -828,5 +1053,13 @@ int loop_image_info(const void* image, size_t bytes, ll_loop_image_summary* info
   info->frame_index = v.sc.frame_index; info->matching_mode = v.sc.matching_mode; info->closed = v.sc.closed; info->stopped = v.sc.stopped;
   info->keyframes = v.sc.n_keyframes; info->open_keyframes = v.sc.n_open; info->events = v.sc.n_events; info->dropped = v.sc.n_dropped;
   info->max_incarnation = v.cells.max_cur;
+  return LL_OK;
+}
+
+extern "C" int ll_loop_correction(const ll_pose* ori, const ll_pose* opt, const int* f, int n, int s, double q_wxyz[4], double t[3]) {
+  if (!ori || !opt || !f || n < 1 || !q_wxyz || !t) return LL_ERR_INVALID;
+  for (int k = 1; k < n; k++) if (f[k] <= f[k - 1]) return LL_ERR_INVALID;
+  const ll_pose c = correction_at(ori, opt, f, n, s);
+  memcpy(q_wxyz, c.q_wxyz, sizeof(c.q_wxyz)); memcpy(t, c.t, sizeof(c.t));
   return LL_OK;
 }

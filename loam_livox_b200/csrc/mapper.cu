@@ -48,6 +48,7 @@ struct RecoveryLayout {
 struct ll_mapper {
   ll_ctx* ctx = nullptr;
   HistoryWindow his_corner, his_surf;
+  std::vector<int> his_frame;   // the frame index of each window segment (both windows push and pop together); loop feedback reads it
   double last_his_add_q[4] = {1, 0, 0, 0}, last_his_add_t[3] = {0, 0, 0};   // m_last_his_add_q / _t (uninitialised members in the reference: defined as identity / 0)
   ll_mapper_config cfg;
   ll_cellmap* cells_corner = nullptr; ll_cellmap* cells_surf = nullptr;
@@ -176,6 +177,10 @@ static void out_init(const ll_mapper* m, ll_reg_result* out) {
 
 static int recovery_step(ll_mapper* m, int nc, int ns, const ll_reg_state& st, const ll_reg_result* out, bool* hold);
 
+static MapperWindow mapper_window(ll_mapper* m) {
+  return MapperWindow{{&m->his_corner, &m->his_surf}, &m->his_frame, m->q_w_curr, m->t_w_curr, m->last_his_add_q, m->last_his_add_t, &m->map_dirty};
+}
+
 // One mapper step on features already in A.feat (nc corners, then ns surfaces) whose full cloud's largest time stamp is max_t: (refresh the
 // match map) -> registration -> world-frame features -> VoxelGrid -> history window and cell maps -> pose.  Every registered scan of
 // ll_mapper_process_scan and every published piece of ll_mapper_process_frame goes through it.
@@ -272,8 +277,9 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
       pushed = true;
       LL_TRY(m->his_corner.push(ctx, w0, (size_t)hc[0]));
       LL_TRY(m->his_surf.push(ctx, w1, (size_t)hc[1]));
+      m->his_frame.push_back(m->frame_index);
     }
-    if ((int)m->his_corner.segs.size() > m->cfg.maximum_history_size) m->his_corner.pop_front();
+    if ((int)m->his_corner.segs.size() > m->cfg.maximum_history_size) { m->his_corner.pop_front(); m->his_frame.erase(m->his_frame.begin()); }
     if ((int)m->his_surf.segs.size() > m->cfg.maximum_history_size) m->his_surf.pop_front();
   }
   const double tr1 = now_ms();
@@ -286,7 +292,7 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
   if (stats) { stats->appended_corner = hc[0]; stats->appended_surf = hc[1]; stats->ms_append = (float)(now_ms() - tp); }
   if (m->rec.on) m->rec.cur->appended = 1;
   for (int k = 0; k < 4; k++) m->q_w_curr[k] = out->q_w_curr[k]; for (int k = 0; k < 3; k++) m->t_w_curr[k] = out->t_w_curr[k];   // :1496-1505
-  if (m->lc) LL_TRY(loop_step(ctx, m->lc, d_pose, pushed, m->frame_index, m->q_w_curr, m->t_w_curr));   // :1523-1564
+  if (m->lc) LL_TRY(loop_step(ctx, m->lc, d_pose, pushed, m->frame_index, mapper_window(m)));   // :1523-1564
   return LL_OK;
 }
 
@@ -654,6 +660,11 @@ int mapper_restore(ll_mapper* m, const ImageView& v) {
   ctx->ex.first_receive_time = sc.first_receive_time; ctx->ex.current_time = sc.current_time; ctx->ex.last_maximum_time_stamp = sc.last_maximum_time_stamp;
   HistoryWindow* his[2] = {&m->his_corner, &m->his_surf};
   for (int c = 0; c < 2; c++) LL_TRY(history_restore(ctx, *his[c], v.his[c]));
+  // The image does not hold the segments' frame indices (a version-3 loop image does, and its load sets them).  Here they are numbered up to
+  // the frame index: ascending and no later than it, so before any keyframe a loop closure set on this mapper can close, whose correction at
+  // such a step is the identity.
+  m->his_frame.resize((size_t)v.his[0].n_seg);
+  for (size_t k = 0; k < m->his_frame.size(); k++) m->his_frame[k] = sc.frame_index - (int)(m->his_frame.size() - 1 - k);
   ll_cellmap* cm[2] = {m->cells_corner, m->cells_surf};
   for (int c = 0; c < 2; c++) LL_TRY(cells_restore(ctx, cm[c], v.cells[c], false));
   // the snapshot and its index (the build is deterministic: the kNN answers are the saved mapper's)
@@ -1137,12 +1148,23 @@ int ll_mapper_loop_save(ll_mapper* m, void* image, size_t cap, size_t* bytes) {
   if (!m || !bytes) return LL_ERR_INVALID;
   if (!m->lc) { m->ctx->set_error("loop closure is off: there is no loop image"); return LL_ERR_INVALID; }
   cudaSetDevice(m->ctx->device);
-  return loop_save(m->ctx, m->lc, loop_stamp(m), image, cap, bytes);
+  return loop_save(m->ctx, m->lc, loop_stamp(m), mapper_window(m), image, cap, bytes);
 }
 
 int ll_mapper_loop_load(ll_mapper* m, const void* image, size_t bytes, const ll_loop_closure_cfg* cfg) {
   if (!m) return LL_ERR_INVALID;
-  return loop_load(m->ctx, &m->lc, image, bytes, cfg, loop_stamp(m), m->cfg, m->frame_pieces);
+  return loop_load(m->ctx, &m->lc, image, bytes, cfg, loop_stamp(m), m->cfg, m->frame_pieces, mapper_window(m));
+}
+
+int ll_mapper_set_loop_feedback(ll_mapper* m, int on) {
+  if (!m) return LL_ERR_INVALID;
+  return loop_set_feedback(m->ctx, m->lc, m->cfg, on);
+}
+
+int ll_mapper_loop_correction_read(ll_mapper* m, double q_wxyz[4], double t[3], int* n_applied) {
+  if (!m || !q_wxyz || !t) return LL_ERR_INVALID;
+  loop_correction(m->lc, q_wxyz, t, n_applied);
+  return LL_OK;
 }
 
 int ll_loop_image_info(const void* image, size_t bytes, ll_loop_image_summary* info) {

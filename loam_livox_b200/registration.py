@@ -1084,6 +1084,18 @@ class Laser_mapping:
         self.ctx.check(self.ctx._lib.ll_mapper_set_loop_policy(self.h, C.byref(p)))
         return p
 
+    def set_loop_feedback(self, on: bool = True):
+        """Loop feedback (ll_mapper_set_loop_feedback; matching mode 0): after each loop the history windows and the pose move onto the
+        optimized trajectory, and loop closure goes on in the odometry frame.  Set after set_loop_closure (which turns it off) and before the
+        first loop; a refusal raises and changes nothing."""
+        self.ctx.check(self.ctx._lib.ll_mapper_set_loop_feedback(self.h, int(bool(on))))
+
+    def loop_correction(self):
+        """(q wxyz, t, n_applied) (ll_mapper_loop_correction_read): the correction applied last and how many were applied."""
+        q, t, n = np.zeros(4), np.zeros(3), C.c_int()
+        self.ctx.check(self.ctx._lib.ll_mapper_loop_correction_read(self.h, q.ctypes.data, t.ctypes.data, C.byref(n)))
+        return q, t, n.value
+
     def loop_edges(self):
         """Every loop edge so far, in closing order (ll_mapper_loop_edges): a list of capi.PgEdge."""
         n = C.c_int()
@@ -1216,6 +1228,22 @@ def image_info(image) -> dict:
     if st != capi.LL_OK:
         raise LoamLivoxError(f"status {st}: mapper image refused")
     return {n: (list(getattr(info, n)) if isinstance(getattr(info, n), C.Array) else getattr(info, n)) for n, _ in capi.ImageInfo._fields_ if n != "reserved"}
+
+
+def loop_correction(poses_ori, poses_opt, f, s: int):
+    """ll_loop_correction (host only): the correction (q wxyz, t) of the step with frame index s, for keyframes closed at frame indices f
+    (strictly ascending) with poses_ori / poses_opt [n, 7] (q w, x, y, z, t)."""
+    ori, opt = (np.ascontiguousarray(np.asarray(P, np.float64).reshape(-1, 7)) for P in (poses_ori, poses_opt))
+    fa = np.ascontiguousarray(np.asarray(f, np.int32))
+    n = fa.shape[0]
+    if ori.shape[0] != n or opt.shape[0] != n:
+        raise ValueError("poses_ori, poses_opt and f must have one entry per keyframe")
+    q, t = np.zeros(4), np.zeros(3)
+    st = capi.lib().ll_loop_correction(ori.ctypes.data_as(C.POINTER(capi.Pose)), opt.ctypes.data_as(C.POINTER(capi.Pose)), fa.ctypes.data, n, int(s),
+                                       q.ctypes.data, t.ctypes.data)
+    if st != capi.LL_OK:
+        raise LoamLivoxError(f"status {st}: ll_loop_correction refused its inputs")
+    return q, t
 
 
 def loop_image_info(image) -> dict:
