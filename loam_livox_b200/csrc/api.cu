@@ -322,15 +322,9 @@ static int map_index(ll_ctx* ctx, ll_map* m, const void* corner, size_t nc, cons
     if (st == LL_OK) st = upload_cloud(ctx, ctx->stream, surf, ns, fmt, where, b_s);
     if (st != LL_OK) return st;
   }
-  // the two indices side by side: corner on the side stream with its own scratch, surface on the context's stream
   cudaStream_t s = ctx->stream;
-  LL_CUDA(ctx, cudaEventRecord(ctx->sev.fork, s));
-  LL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->sev.fork, 0));
-  st = build_bucket_tree(ctx, ctx->stream2, ctx->scratch2, d_c, (int)nc, &m->corner);
-  const int st2 = build_bucket_tree(ctx, s, ctx->scratch, d_s, (int)ns, &m->surf);
-  LL_CUDA(ctx, cudaEventRecord(ctx->sev.join, ctx->stream2));
-  LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->sev.join, 0));
-  if (st == LL_OK) st = st2;
+  const float4* src[2] = {d_c, d_s}; const size_t n[2] = {nc, ns};
+  st = map_side_pair(ctx, s, [&](int c, cudaStream_t cs, DevBuf& scr) { return build_bucket_tree(ctx, cs, scr, src[c], (int)n[c], &m->tree[c]); });
   // host inputs may be freed by the caller as soon as this returns; device inputs are consumed in stream order (the per-scan refresh never waits)
   if (st == LL_OK && where == LL_HOST && cudaStreamSynchronize(s) != cudaSuccess) st = LL_ERR_CUDA;
   return st;
@@ -340,7 +334,7 @@ static int map_build_common(ll_ctx* ctx, const void* corner, size_t nc, const vo
   cudaSetDevice(ctx->device);
   ll_map* m = new ll_map(); m->device = ctx->device;
   int st = map_index(ctx, m, corner, nc, surf, ns, fmt, where);
-  if (st != LL_OK) { m->corner.storage.release(); m->surf.storage.release(); delete m; return st; }
+  if (st != LL_OK) { ll_map_release(m); return st; }
   *out = m; return LL_OK;
 }
 // Re-index an existing snapshot in place (device buffers are reused when large enough): the per-scan refresh of
@@ -356,9 +350,9 @@ int ll_map_build(ll_ctx* ctx, const void* corner, size_t nc, const void* surf, s
 void ll_map_release(ll_map* map) {
   if (!map) return;
   cudaSetDevice(map->device);
-  map->corner.storage.release(); map->surf.storage.release(); map->shard_owner.release(); delete map;
+  for (BucketTree& t : map->tree) t.storage.release(); map->shard_owner.release(); delete map;
 }
-size_t ll_map_size(const ll_map* map, int which) { return map ? (size_t)(which == 0 ? map->corner.n : map->surf.n) : 0; }
+size_t ll_map_size(const ll_map* map, int which) { return map ? (size_t)map->tree[which != 0].n : 0; }
 
 int ll_knn(ll_ctx* ctx, const ll_map* map, int which, const ll_point* queries, size_t nq, int32_t* idx5, float* sqdist5) {
   if (!ctx || !map) return LL_ERR_INVALID;
@@ -367,7 +361,7 @@ int ll_knn(ll_ctx* ctx, const ll_map* map, int which, const ll_point* queries, s
   float4* d_q; int* d_idx; float* d_d;
   LL_CUDA(ctx, ctx->feat_buf.carve([&](Carve& c) { d_q = c.take<float4>(nq); d_idx = c.take<int>(nq * LL_KNN); d_d = c.take<float>(nq * LL_KNN); }));
   LL_CUDA(ctx, cudaMemcpyAsync(d_q, queries, nq * 16, cudaMemcpyHostToDevice, ctx->stream));
-  LL_TRY(launch_knn_query(ctx, which == 0 ? map->corner : map->surf, d_q, (int)nq, d_idx, d_d));
+  LL_TRY(launch_knn_query(ctx, map->tree[which != 0], d_q, (int)nq, d_idx, d_d));
   LL_CUDA(ctx, cudaMemcpyAsync(idx5, d_idx, nq * 20, cudaMemcpyDeviceToHost, ctx->stream));
   LL_CUDA(ctx, cudaMemcpyAsync(sqdist5, d_d, nq * 20, cudaMemcpyDeviceToHost, ctx->stream));
   LL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -391,7 +385,7 @@ static void fill_state(RegDevState* h, const ll_reg_state* in) {
 struct RegBatch { int n; int nc[LL_MAX_BATCH], ns[LL_MAX_BATCH], off[LL_MAX_BATCH + 1]; const ll_reg_state* in[LL_MAX_BATCH]; };
 static KnnBlocksArgs knn_args(ll_ctx* ctx, const ll_map* map, const RegBatch& b, bool debug) {
   const RegArrays& A = ctx->A;
-  KnnBlocksArgs a; a.corner = make_view(map->corner); a.surf = make_view(map->surf); a.feat = A.feat; a.M = b.off[b.n]; a.n_items = b.n;
+  KnnBlocksArgs a; a.corner = make_view(map->tree[0]); a.surf = make_view(map->tree[1]); a.feat = A.feat; a.M = b.off[b.n]; a.n_items = b.n;
   for (int j = 0; j < b.n; j++) {
     const ll_reg_state* in = b.in[j]; KnnItem& I = a.item[j];
     I.off = b.off[j]; I.n_corner = b.nc[j]; I.n_surf = b.ns[j]; I.icp_line = in->icp_line; I.icp_plane = in->icp_plane;
@@ -426,7 +420,7 @@ static SolveArgs solve_args(ll_ctx* ctx, int M, SolveMode mode, int max_iter) {
 
 // The gate (:199): CORNER_MIN_MAP_NUM 0, SURFACE_MIN_MAP_NUM 50.
 static bool reg_gate(const ll_map* map, const ll_reg_state* in) {
-  return map->corner.n_src > 0 && map->surf.n_src > 50 && in->current_frame_index > in->mapping_init_accumulate_frames;
+  return map->tree[0].n_src > 0 && map->tree[1].n_src > 50 && in->current_frame_index > in->mapping_init_accumulate_frames;
 }
 // What an item returns before any device work: the result initialised from its state, the gate (:199) and the empty item.  Returns 1 when the
 // item goes on to the device; else *status is its outcome (LL_OK with registered = 0 under the gate, LL_ERR_NO_BLOCKS without features).

@@ -113,7 +113,7 @@ __host__ __device__ inline int shard_cell_index(const ShardGrid& g, float x, flo
 
 struct ll_map {
   int device = 0;
-  BucketTree corner, surf;
+  BucketTree tree[2];   // 0 corner, 1 surface
   // sharding (world == 1: everything owned).  A sharded snapshot indexes only the points of the cells this rank owns plus the halo of the match
   // gates around them; the owner table (rank per cell) lives on the device for the query side and on the host for ll_map_shard_info.
   int rank = 0, world = 1; float cell_size = 0.f;

@@ -13,6 +13,18 @@ TreeView make_view(const BucketTree& t);
 int build_bucket_tree(ll_ctx* ctx, cudaStream_t s, DevBuf& scratch, const float4* d_src, int n_src, BucketTree* t);
 size_t tree_scratch_bytes(int n_src);   // what build_bucket_tree carves from `scratch` and from BucketTree::storage for n_src points
 size_t tree_storage_bytes(int n_src);
+// The map side's two halves side by side (the index builds of ll_map_build / _rebuild, the mapper's whole-map and append VoxelGrids):
+// half(c, stream, scratch) enqueues class c, the corner half (0) on stream2 with scratch2 first, then the surface half (1) on `s` with scratch.
+// Both halves are enqueued and the join is always recorded, so `s` is behind both whatever they return; returns the first non-OK status.
+template <class F> int map_side_pair(ll_ctx* ctx, cudaStream_t s, F&& half) {
+  LL_CUDA(ctx, cudaEventRecord(ctx->sev.fork, s));
+  LL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->sev.fork, 0));
+  const int st0 = half(0, ctx->stream2, ctx->scratch2);
+  const int st1 = half(1, s, ctx->scratch);
+  LL_CUDA(ctx, cudaEventRecord(ctx->sev.join, ctx->stream2));
+  LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->sev.join, 0));
+  return st0 != LL_OK ? st0 : st1;
+}
 // Bounding box of the finite points (knn.cu): bbox[0..2] = min, bbox[3..5] = max (ll_f2ord encoding), bbox[6] = their count.
 // bbox_init_kernel (one warp) resets it; every bbox_kernel launch after that widens it by one more cloud.
 __global__ void bbox_init_kernel(int* bbox);

@@ -47,11 +47,11 @@ struct RecoveryLayout {
 
 struct ll_mapper {
   ll_ctx* ctx = nullptr;
-  HistoryWindow his_corner, his_surf;
+  HistoryWindow his[2];         // per class (0 corner, 1 surface), as cells and the match map's trees
   std::vector<int> his_frame;   // the frame index of each window segment (both windows push and pop together); loop feedback reads it
   double last_his_add_q[4] = {1, 0, 0, 0}, last_his_add_t[3] = {0, 0, 0};   // m_last_his_add_q / _t (uninitialised members in the reference: defined as identity / 0)
   ll_mapper_config cfg;
-  ll_cellmap* cells_corner = nullptr; ll_cellmap* cells_surf = nullptr;
+  ll_cellmap* cells[2] = {nullptr, nullptr};
   ll_map* match_map = nullptr;
   int frame_index = 0;
   double last_time_stamp = 0;   // m_last_time_stamp (laser_mapping.hpp:140)
@@ -79,14 +79,18 @@ struct FrameLayout {
 
 // snap: the match-map snapshot (the two whole-map VoxelGrid outputs) and their counts
 struct SnapLayout {
-  float4* c; float4* s; int* cnt;
-  void layout(Carve& k, size_t mc, size_t ms) { c = k.take<float4>(mc + 1); s = k.take<float4>(ms + 1); cnt = k.take<int>(2); }
+  float4* cls[2]; int* cnt;
+  void layout(Carve& k, size_t mc, size_t ms) { cls[0] = k.take<float4>(mc + 1); cls[1] = k.take<float4>(ms + 1); cnt = k.take<int>(2); }
 };
-// work: a scan's features in the world frame (w2 corner, w3 surface), down-sampled (w0, w1), their counts and the pose
+// work: a scan's features per class down-sampled and in the world frame, their counts and the pose
 struct WorkLayout {
-  float4* w0; float4* w1; float4* w2; float4* w3; int* cnt; double* pose;
-  void layout(Carve& k, size_t n) { w0 = k.take<float4>(n); w1 = k.take<float4>(n); w2 = k.take<float4>(n); w3 = k.take<float4>(n); cnt = k.take<int>(2); pose = k.take<double>(7); }
+  float4* down[2]; float4* world[2]; int* cnt; double* pose;
+  void layout(Carve& k, size_t n) { for (float4*& p : down) p = k.take<float4>(n); for (float4*& p : world) p = k.take<float4>(n); cnt = k.take<int>(2); pose = k.take<double>(7); }
 };
+
+// The mapper's per-class settings (0 corner, 1 surface): the leaf of the map side's VoxelGrids and the range of the mode-1 assembly.
+static float class_leaf(const ll_mapper_config& cfg, int c) { return c ? cfg.plane_resolution : cfg.line_resolution; }
+static float class_range(const ll_mapper_config& cfg, int c) { return c ? cfg.maximum_search_range_surface : cfg.maximum_search_range_corner; }
 
 // Every buffer whose size follows the map is allocated here, once, for the configured reservation (a reallocation inside a scan call
 // synchronises the device and stalls that call for far longer than the scan takes; one such stall per doubling of the map dominates the mean
@@ -101,19 +105,19 @@ static int mapper_reserve(ll_ctx* ctx, ll_mapper* m) {
     FrameLayout fl; for (DevBuf& b : m->frame) LL_CUDA(ctx, b.reserve_floor(layout_bytes([&](Carve& c) { fl.layout(c, cap); })));
     for (DevBuf& b : m->frame_vg) LL_CUDA(ctx, b.reserve_floor(std::max(voxel_grid_bytes((int)cap, P), voxel_grid_bytes(ctx->cfg.max_scan_points, 1))));
     m->frame_pieces = P; }
-  if (S) { LL_TRY(ll_cellmap_reserve(ctx, m->cells_corner, S, F)); LL_TRY(ll_cellmap_reserve(ctx, m->cells_surf, S, F)); }
-  // The two map-side arenas, each at the largest of its consumers.  Both: the append's VoxelGrid of a scan's features (corner half on stream2 /
-  // scratch2, surface half on the context's stream / scratch) and the refresh's whole-map VoxelGrid and index build (the halves side by side
-  // the same way).  scratch alone: the registration's query sort and K10 hash set.
+  if (S) for (ll_cellmap* cm : m->cells) LL_TRY(ll_cellmap_reserve(ctx, cm, S, F));
+  // The two map-side arenas, each at the largest of its consumers.  Both: the append's VoxelGrid of a scan's features and the refresh's
+  // whole-map VoxelGrid and index build, whose halves map_side_pair runs side by side (corner on stream2 / scratch2, surface on the context's
+  // stream / scratch).  scratch alone: the registration's query sort and K10 hash set.
   size_t side = voxel_grid_bytes(F);
   if (R) side = std::max(side, std::max(voxel_grid_bytes((int)R), tree_scratch_bytes((int)R)));
   const size_t reg = std::max(query_sort_bytes(F, 1), layout_bytes([&](Carve& c) { l1_set_layout(c, F); }));
   LL_CUDA(ctx, ctx->scratch.reserve_floor(std::max(side, reg)));
   LL_CUDA(ctx, ctx->scratch2.reserve_floor(side));
   if (!R) return LL_OK;
-  LL_TRY(m->his_corner.reserve(ctx, R)); LL_TRY(m->his_surf.reserve(ctx, R));
+  for (HistoryWindow& h : m->his) LL_TRY(h.reserve(ctx, R));
   SnapLayout sn; LL_CUDA(ctx, m->snap.reserve_floor(layout_bytes([&](Carve& c) { sn.layout(c, R, R); })));
-  for (BucketTree* t : {&m->match_map->corner, &m->match_map->surf}) LL_CUDA(ctx, t->storage.reserve_floor(tree_storage_bytes((int)R)));
+  for (BucketTree& t : m->match_map->tree) LL_CUDA(ctx, t.storage.reserve_floor(tree_storage_bytes((int)R)));
   return LL_OK;
 }
 
@@ -138,9 +142,9 @@ void ll_mapper_config_default(ll_mapper_config* c) {
 int ll_mapper_create(ll_ctx* ctx, const ll_mapper_config* cfg, ll_mapper** out) {
   if (!ctx || !cfg || !out) return LL_ERR_INVALID;
   ll_mapper* m = new ll_mapper(); m->ctx = ctx; m->cfg = *cfg;
-  int st = ll_cellmap_create(ctx, cfg->cell_resolution, cfg->threshold_cell_revisit, cfg->max_cells, &m->cells_corner);
-  if (st == LL_OK) st = ll_cellmap_create(ctx, cfg->cell_resolution, cfg->threshold_cell_revisit, cfg->max_cells, &m->cells_surf);
-  if (st != LL_OK) { ll_cellmap_release(m->cells_corner); delete m; return st; }
+  int st = LL_OK;
+  for (int c = 0; c < 2 && st == LL_OK; c++) st = ll_cellmap_create(ctx, cfg->cell_resolution, cfg->threshold_cell_revisit, cfg->max_cells, &m->cells[c]);
+  if (st != LL_OK) { ll_cellmap_release(m->cells[0]); delete m; return st; }
   for (int k = 0; k < 4; k++) m->q_w_curr[k] = cfg->reg.q_w_curr[k];
   for (int k = 0; k < 3; k++) m->t_w_curr[k] = cfg->reg.t_w_curr[k];
   ll_extract_reset(ctx);
@@ -154,9 +158,10 @@ int ll_mapper_create(ll_ctx* ctx, const ll_mapper_config* cfg, ll_mapper** out) 
 void ll_mapper_release(ll_mapper* m) {
   if (!m) return;
   cudaSetDevice(m->ctx->device);
-  ll_cellmap_release(m->cells_corner); ll_cellmap_release(m->cells_surf);
+  for (ll_cellmap* cm : m->cells) ll_cellmap_release(cm);
   if (m->match_map) ll_map_release(m->match_map);
-  m->work.release(); m->snap.release(); m->his_corner.release(); m->his_surf.release();
+  m->work.release(); m->snap.release();
+  for (HistoryWindow& h : m->his) h.release();
   for (FrontGraph& g : m->frame_graph) if (g.exec) cudaGraphExecDestroy(g.exec);
   m->frame[0].release(); m->frame[1].release(); m->frame_vg[0].release(); m->frame_vg[1].release();
   ll_reloc_field_release(m->rec.field); if (m->rec.whole) ll_map_release(m->rec.whole); m->rec.buf.release();
@@ -178,7 +183,7 @@ static void out_init(const ll_mapper* m, ll_reg_result* out) {
 static int recovery_step(ll_mapper* m, int nc, int ns, const ll_reg_state& st, const ll_reg_result* out, bool* hold);
 
 static MapperWindow mapper_window(ll_mapper* m) {
-  return MapperWindow{{&m->his_corner, &m->his_surf}, &m->his_frame, m->q_w_curr, m->t_w_curr, m->last_his_add_q, m->last_his_add_t, &m->map_dirty};
+  return MapperWindow{{&m->his[0], &m->his[1]}, &m->his_frame, m->q_w_curr, m->t_w_curr, m->last_his_add_q, m->last_his_add_t, &m->map_dirty};
 }
 
 // One mapper step on features already in A.feat (nc corners, then ns surfaces) whose full cloud's largest time stamp is max_t: (refresh the
@@ -198,37 +203,30 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
   m->frame_index++;                                                              // m_current_frame_index++ (:1350)
   // ---- update_buff_for_matching (mode 1): snapshot of the cells in range and in the FOV, whole-map VoxelGrid, index
   if (m->map_dirty) {
-    size_t mc = 0, ms = 0; const ll_point* d_mc = nullptr; const ll_point* d_ms = nullptr; int fov_c = 0, fov_s = 0;
-    if (m->cfg.matching_mode == 0) {   // :518-531: the concatenation of the history window (the live range of the flat array)
-      mc = m->his_corner.live(); ms = m->his_surf.live(); d_mc = (const ll_point*)m->his_corner.data(); d_ms = (const ll_point*)m->his_surf.data();
-    } else {
-    LL_TRY(ll_cellmap_assemble(ctx, m->cells_corner, m->q_w_curr, m->t_w_curr, m->cfg.maximum_search_range_corner, m->cfg.maximum_in_fov_angle, m->cfg.line_resolution,
-                               m->cfg.down_sample_replace, nullptr, 0, &mc, &fov_c, &d_mc));
-    LL_TRY(ll_cellmap_assemble(ctx, m->cells_surf, m->q_w_curr, m->t_w_curr, m->cfg.maximum_search_range_surface, m->cfg.maximum_in_fov_angle, m->cfg.plane_resolution,
-                               m->cfg.down_sample_replace, nullptr, 0, &ms, &fov_s, &d_ms));
+    size_t n[2] = {0, 0}; const ll_point* src[2] = {nullptr, nullptr}; int fov[2] = {0, 0};
+    for (int c = 0; c < 2; c++) {
+      if (m->cfg.matching_mode == 0) { n[c] = m->his[c].live(); src[c] = (const ll_point*)m->his[c].data(); }   // :518-531: the concatenation of the history window (the live range of the flat array)
+      else LL_TRY(ll_cellmap_assemble(ctx, m->cells[c], m->q_w_curr, m->t_w_curr, class_range(m->cfg, c), m->cfg.maximum_in_fov_angle, class_leaf(m->cfg, c),
+                                      m->cfg.down_sample_replace, nullptr, 0, &n[c], &fov[c], &src[c]));
     }
-    SnapLayout sn; LL_CUDA(ctx, m->snap.carve([&](Carve& c) { sn.layout(c, mc, ms); }));
-    float4* s0 = sn.c; float4* s1 = sn.s; int* d_sc = sn.cnt;
+    SnapLayout sn; LL_CUDA(ctx, m->snap.carve([&](Carve& k) { sn.layout(k, n[0], n[1]); }));
+    LL_TRY(map_side_pair(ctx, s, [&](int c, cudaStream_t cs, DevBuf& scr) -> int {   // the whole-map VoxelGrids (:533-537)
+      if (n[c] > 0) return launch_voxel_grid(ctx, cs, scr, (const float4*)src[c], (int)n[c], nullptr, class_leaf(m->cfg, c), sn.cls[c], sn.cnt + c);
+      LL_CUDA(ctx, cudaMemsetAsync(sn.cnt + c, 0, 4, cs)); return LL_OK;
+    }));
     int hc[2] = {0, 0};
-    // the two whole-map VoxelGrids side by side (corner on the side stream with its own scratch)
-    cudaStream_t s2 = ctx->stream2;
-    LL_CUDA(ctx, cudaEventRecord(ctx->sev.fork, s)); LL_CUDA(ctx, cudaStreamWaitEvent(s2, ctx->sev.fork, 0));
-    if (mc > 0) LL_TRY(launch_voxel_grid(ctx, s2, ctx->scratch2, (const float4*)d_mc, (int)mc, nullptr, m->cfg.line_resolution, s0, d_sc)); else LL_CUDA(ctx, cudaMemsetAsync(d_sc, 0, 4, s2));      // :533-534
-    if (ms > 0) LL_TRY(launch_voxel_grid(ctx, s, ctx->scratch, (const float4*)d_ms, (int)ms, nullptr, m->cfg.plane_resolution, s1, d_sc + 1)); else LL_CUDA(ctx, cudaMemsetAsync(d_sc + 1, 0, 4, s));   // :536-537
-    LL_CUDA(ctx, cudaEventRecord(ctx->sev.join, s2)); LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->sev.join, 0));
-    LL_CUDA(ctx, cudaMemcpyAsync(hc, d_sc, 8, cudaMemcpyDeviceToHost, s));
+    LL_CUDA(ctx, cudaMemcpyAsync(hc, sn.cnt, 8, cudaMemcpyDeviceToHost, s));
     LL_CUDA(ctx, cudaStreamSynchronize(s));
     m->have_map = false;
     if (hc[0] > 0 && hc[1] > 0) {
-      LL_TRY(ll_map_rebuild(ctx, m->match_map, s0, (size_t)hc[0], s1, (size_t)hc[1], LL_FMT_XYZI16, LL_DEVICE));   // buffers reused: no allocation per scan
+      LL_TRY(ll_map_rebuild(ctx, m->match_map, sn.cls[0], (size_t)hc[0], sn.cls[1], (size_t)hc[1], LL_FMT_XYZI16, LL_DEVICE));   // buffers reused: no allocation per scan
       m->have_map = true;
     }                      // :544-545
-    m->snap_n[0] = hc[0]; m->snap_n[1] = hc[1]; m->fov[0] = fov_c; m->fov[1] = fov_s;
+    for (int c = 0; c < 2; c++) { m->snap_n[c] = hc[c]; m->fov[c] = fov[c]; }
     m->map_dirty = false;
   }
   if (stats) { stats->ms_refresh = (float)(now_ms() - tp); stats->map_corner = m->snap_n[0]; stats->map_surf = m->snap_n[1]; stats->cells_in_fov_corner = m->fov[0]; stats->cells_in_fov_surf = m->fov[1]; }
   WorkLayout wl; LL_CUDA(ctx, m->work.carve([&](Carve& c) { wl.layout(c, (size_t)(nc > ns ? nc : ns)); }));
-  float4* w0 = wl.w0; float4* w1 = wl.w1; float4* w2 = wl.w2; float4* w3 = wl.w3; int* d_cnt = wl.cnt;
   int hc[2] = {0, 0};
   // ---- init_pointcloud_registration + find_out_incremental_transfrom (:1266-1297, :1405)
   ll_reg_state st = m->cfg.reg;
@@ -253,14 +251,13 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
   double* h = ctx->pin->mapper_pose; for (int k = 0; k < 4; k++) h[k] = out->q_w_curr[k]; for (int k = 0; k < 3; k++) h[4 + k] = out->t_w_curr[k];
   double* d_pose = wl.pose;
   LL_CUDA(ctx, cudaMemcpyAsync(d_pose, h, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
-  {
-    cudaStream_t s2 = ctx->stream2;
-    LL_CUDA(ctx, cudaEventRecord(ctx->sev.fork, s)); LL_CUDA(ctx, cudaStreamWaitEvent(s2, ctx->sev.fork, 0));
-    if (nc > 0) { LL_TRY(launch_transform(ctx, s2, d_pose, A.feat, nc, w2)); LL_TRY(launch_voxel_grid(ctx, s2, ctx->scratch2, w2, nc, nullptr, m->cfg.line_resolution, w0, d_cnt)); } else LL_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, 4, s2));
-    if (ns > 0) { LL_TRY(launch_transform(ctx, s, d_pose, A.feat + nc, ns, w3)); LL_TRY(launch_voxel_grid(ctx, s, ctx->scratch, w3, ns, nullptr, m->cfg.plane_resolution, w1, d_cnt + 1)); } else LL_CUDA(ctx, cudaMemsetAsync(d_cnt + 1, 0, 4, s));
-    LL_CUDA(ctx, cudaEventRecord(ctx->sev.join, s2)); LL_CUDA(ctx, cudaStreamWaitEvent(s, ctx->sev.join, 0));
-  }
-  LL_CUDA(ctx, cudaMemcpyAsync(hc, d_cnt, 8, cudaMemcpyDeviceToHost, s));
+  const int n[2] = {nc, ns}; const float4* feat[2] = {A.feat, A.feat + nc};
+  LL_TRY(map_side_pair(ctx, s, [&](int c, cudaStream_t cs, DevBuf& scr) -> int {
+    if (n[c] <= 0) { LL_CUDA(ctx, cudaMemsetAsync(wl.cnt + c, 0, 4, cs)); return LL_OK; }
+    LL_TRY(launch_transform(ctx, cs, d_pose, feat[c], n[c], wl.world[c]));
+    return launch_voxel_grid(ctx, cs, scr, wl.world[c], n[c], nullptr, class_leaf(m->cfg, c), wl.down[c], wl.cnt + c);
+  }));
+  LL_CUDA(ctx, cudaMemcpyAsync(hc, wl.cnt, 8, cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   const double tr0 = now_ms();
   // history window (:1439-1478): r_diff / t_diff compare the pose adopted from the PREVIOUS scan (m_q_w_curr is only overwritten at :1498) with the
@@ -272,22 +269,19 @@ static int mapper_step(ll_mapper* m, int nc, int ns, double max_t, ll_reg_result
     const double r_diff = 2.0 * acos(dot) * 57.3;
     double t2 = 0; for (int k = 0; k < 3; k++) t2 += (m->t_w_curr[k] - m->last_his_add_t[k]) * (m->t_w_curr[k] - m->last_his_add_t[k]);
     const double t_diff = sqrt(t2);
-    if ((int)m->his_corner.segs.size() < m->cfg.maximum_history_size || t_diff > 0.0 || r_diff > 0.0 * 57.3) {
+    if ((int)m->his[0].segs.size() < m->cfg.maximum_history_size || t_diff > 0.0 || r_diff > 0.0 * 57.3) {
       for (int k = 0; k < 4; k++) m->last_his_add_q[k] = m->q_w_curr[k]; for (int k = 0; k < 3; k++) m->last_his_add_t[k] = m->t_w_curr[k];
       pushed = true;
-      LL_TRY(m->his_corner.push(ctx, w0, (size_t)hc[0]));
-      LL_TRY(m->his_surf.push(ctx, w1, (size_t)hc[1]));
+      for (int c = 0; c < 2; c++) LL_TRY(m->his[c].push(ctx, wl.down[c], (size_t)hc[c]));
       m->his_frame.push_back(m->frame_index);
     }
-    if ((int)m->his_corner.segs.size() > m->cfg.maximum_history_size) { m->his_corner.pop_front(); m->his_frame.erase(m->his_frame.begin()); }
-    if ((int)m->his_surf.segs.size() > m->cfg.maximum_history_size) m->his_surf.pop_front();
+    for (int c = 0; c < 2; c++)   // each window by its own segment count; the frame indices follow the corner window's
+      if ((int)m->his[c].segs.size() > m->cfg.maximum_history_size) { m->his[c].pop_front(); if (c == 0) m->his_frame.erase(m->his_frame.begin()); }
   }
-  const double tr1 = now_ms();
-  LL_TRY(ll_cellmap_append(ctx, m->cells_corner, w0, (size_t)hc[0], LL_FMT_XYZI16, LL_DEVICE));
-  const double tr2 = now_ms();
-  LL_TRY(ll_cellmap_append(ctx, m->cells_surf, w1, (size_t)hc[1], LL_FMT_XYZI16, LL_DEVICE));
+  double tcell[3] = {now_ms(), 0, 0};   // before the cell maps, after the corner's, after the surface's
+  for (int c = 0; c < 2; c++) { LL_TRY(ll_cellmap_append(ctx, m->cells[c], wl.down[c], (size_t)hc[c], LL_FMT_XYZI16, LL_DEVICE)); tcell[c + 1] = now_ms(); }
   if (m->trace && now_ms() - tp > 10.0)   // LL_MAPPER_TRACE=1: where a slow append went (transform + VoxelGrid + sync | history | corner cells | surface cells)
-    fprintf(stderr, "ll_mapper trace: frame %d append %.2f ms = features %.2f + history %.2f + cells %.2f + %.2f\n", m->frame_index, now_ms() - tp, tr0 - tp, tr1 - tr0, tr2 - tr1, now_ms() - tr2);
+    fprintf(stderr, "ll_mapper trace: frame %d append %.2f ms = features %.2f + history %.2f + cells %.2f + %.2f\n", m->frame_index, now_ms() - tp, tr0 - tp, tcell[0] - tr0, tcell[1] - tcell[0], tcell[2] - tcell[1]);
   m->map_dirty = true;                                                           // m_if_mapping_updated_* (:1490-1491)
   if (stats) { stats->appended_corner = hc[0]; stats->appended_surf = hc[1]; stats->ms_append = (float)(now_ms() - tp); }
   if (m->rec.on) m->rec.cur->appended = 1;
@@ -658,23 +652,20 @@ int mapper_restore(ll_mapper* m, const ImageView& v) {
   m->map_dirty = sc.map_dirty != 0;
   for (int c = 0; c < 2; c++) { m->snap_n[c] = sc.snap_n[c]; m->fov[c] = sc.fov[c]; }
   ctx->ex.first_receive_time = sc.first_receive_time; ctx->ex.current_time = sc.current_time; ctx->ex.last_maximum_time_stamp = sc.last_maximum_time_stamp;
-  HistoryWindow* his[2] = {&m->his_corner, &m->his_surf};
-  for (int c = 0; c < 2; c++) LL_TRY(history_restore(ctx, *his[c], v.his[c]));
+  for (int c = 0; c < 2; c++) LL_TRY(history_restore(ctx, m->his[c], v.his[c]));
   // The image does not hold the segments' frame indices (a version-3 loop image does, and its load sets them).  Here they are numbered up to
   // the frame index: ascending and no later than it, so before any keyframe a loop closure set on this mapper can close, whose correction at
   // such a step is the identity.
   m->his_frame.resize((size_t)v.his[0].n_seg);
   for (size_t k = 0; k < m->his_frame.size(); k++) m->his_frame[k] = sc.frame_index - (int)(m->his_frame.size() - 1 - k);
-  ll_cellmap* cm[2] = {m->cells_corner, m->cells_surf};
-  for (int c = 0; c < 2; c++) LL_TRY(cells_restore(ctx, cm[c], v.cells[c], false));
+  for (int c = 0; c < 2; c++) LL_TRY(cells_restore(ctx, m->cells[c], v.cells[c], false));
   // the snapshot and its index (the build is deterministic: the kNN answers are the saved mapper's)
   m->have_map = false;
   if (sc.have_map) {
-    const size_t n0 = (size_t)v.snap[0].n, n1 = (size_t)v.snap[1].n;
-    SnapLayout sn; LL_CUDA(ctx, m->snap.carve([&](Carve& k) { sn.layout(k, n0, n1); }));
-    LL_CUDA(ctx, cudaMemcpyAsync(sn.c, v.snap[0].pts, n0 * 16, cudaMemcpyHostToDevice, s));
-    LL_CUDA(ctx, cudaMemcpyAsync(sn.s, v.snap[1].pts, n1 * 16, cudaMemcpyHostToDevice, s));
-    LL_TRY(ll_map_rebuild(ctx, m->match_map, sn.c, n0, sn.s, n1, LL_FMT_XYZI16, LL_DEVICE));
+    const size_t n[2] = {(size_t)v.snap[0].n, (size_t)v.snap[1].n};
+    SnapLayout sn; LL_CUDA(ctx, m->snap.carve([&](Carve& k) { sn.layout(k, n[0], n[1]); }));
+    for (int c = 0; c < 2; c++) LL_CUDA(ctx, cudaMemcpyAsync(sn.cls[c], v.snap[c].pts, n[c] * 16, cudaMemcpyHostToDevice, s));
+    LL_TRY(ll_map_rebuild(ctx, m->match_map, sn.cls[0], n[0], sn.cls[1], n[1], LL_FMT_XYZI16, LL_DEVICE));
     m->have_map = true;
   }
   LL_CUDA(ctx, cudaStreamSynchronize(s));
@@ -688,18 +679,15 @@ extern "C" int ll_mapper_save(ll_mapper* m, void* image, size_t cap, size_t* byt
   ll_ctx* ctx = m->ctx; cudaSetDevice(ctx->device);
   cudaStream_t s = ctx->stream;
   LL_CUDA(ctx, cudaStreamSynchronize(s));
-  HistoryWindow* his[2] = {&m->his_corner, &m->his_surf};
-  ll_cellmap* cm[2] = {m->cells_corner, m->cells_surf};
-  const BucketTree* snap[2] = {&m->match_map->corner, &m->match_map->surf};
   int64_t n_snap[2]; CellsView cells[2];
   for (int c = 0; c < 2; c++) {
-    n_snap[c] = m->have_map ? snap[c]->n_src : 0;
+    n_snap[c] = m->have_map ? m->match_map->tree[c].n_src : 0;
     if (m->have_map && n_snap[c] != m->snap_n[c]) { ctx->set_error("match-map index and snapshot disagree"); return LL_ERR_INVALID; }
     int nc = 0, live = 0;
-    LL_TRY(cm_count(ctx, cm[c], &nc, &live, &cells[c].frame_idx, &cells[c].n_oor));
+    LL_TRY(cm_count(ctx, m->cells[c], &nc, &live, &cells[c].frame_idx, &cells[c].n_oor));
     cells[c].n_cells = nc; cells[c].n_pts = live;
   }
-  const uint64_t len[LL_IMAGE_SECTIONS] = {sizeof(ll_mapper_config), sizeof(ll_mapper_image_scalars), history_bytes(*his[0]), history_bytes(*his[1]),
+  const uint64_t len[LL_IMAGE_SECTIONS] = {sizeof(ll_mapper_config), sizeof(ll_mapper_image_scalars), history_bytes(m->his[0]), history_bytes(m->his[1]),
                                            SNAP_HEAD + 16 * (uint64_t)n_snap[0], SNAP_HEAD + 16 * (uint64_t)n_snap[1], cells_bytes(cells[0], false),
                                            cells_bytes(cells[1], false)};
   ll_mapper_image_header h;
@@ -720,11 +708,11 @@ extern "C" int ll_mapper_save(ll_mapper* m, void* image, size_t cap, size_t* byt
   sc.first_receive_time = ctx->ex.first_receive_time; sc.current_time = ctx->ex.current_time; sc.last_maximum_time_stamp = ctx->ex.last_maximum_time_stamp;
   memcpy(at(LL_IMAGE_SCALARS), &sc, sizeof(sc));
   for (int c = 0; c < 2; c++) {
-    LL_TRY(history_write(ctx, *his[c], at(LL_IMAGE_HISTORY_CORNER + c)));
+    LL_TRY(history_write(ctx, m->his[c], at(LL_IMAGE_HISTORY_CORNER + c)));
     uint8_t* p = at(LL_IMAGE_SNAPSHOT_CORNER + c);
     img_put<int64_t>(p, n_snap[c]);
-    if (n_snap[c]) LL_CUDA(ctx, cudaMemcpyAsync(p + SNAP_HEAD, snap[c]->src, (size_t)n_snap[c] * 16, cudaMemcpyDeviceToHost, s));
-    LL_TRY(cells_write(ctx, cm[c], cells[c], at(LL_IMAGE_CELLS_CORNER + c)));
+    if (n_snap[c]) LL_CUDA(ctx, cudaMemcpyAsync(p + SNAP_HEAD, m->match_map->tree[c].src, (size_t)n_snap[c] * 16, cudaMemcpyDeviceToHost, s));
+    LL_TRY(cells_write(ctx, m->cells[c], cells[c], at(LL_IMAGE_CELLS_CORNER + c)));
   }
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   return LL_OK;
@@ -770,12 +758,10 @@ static int whole_map_clouds(ll_mapper* m, float4* vg[2], int hc[2]) {
   ll_ctx* ctx = m->ctx;
   cudaStream_t s = ctx->stream;
   size_t n[2] = {0, 0};
-  ll_cellmap* cm[2] = {m->cells_corner, m->cells_surf};
-  const HistoryWindow* his[2] = {&m->his_corner, &m->his_surf};
   if (m->cfg.matching_mode == 0) {
-    for (int c = 0; c < 2; c++) n[c] = his[c]->live();
+    for (int c = 0; c < 2; c++) n[c] = m->his[c].live();
   } else {
-    for (int c = 0; c < 2; c++) { int cells = 0, live = 0, fi = 0, oor = 0; LL_TRY(cm_count(ctx, cm[c], &cells, &live, &fi, &oor)); n[c] = (size_t)live; }
+    for (int c = 0; c < 2; c++) { int cells = 0, live = 0, fi = 0, oor = 0; LL_TRY(cm_count(ctx, m->cells[c], &cells, &live, &fi, &oor)); n[c] = (size_t)live; }
   }
   if (n[0] == 0 || n[1] == 0) { ctx->set_error("the mapper has no map yet (a class is empty)"); return LL_ERR_INVALID; }
   float4* in[2] = {nullptr, nullptr}; int* d_cnt;
@@ -783,11 +769,10 @@ static int whole_map_clouds(ll_mapper* m, float4* vg[2], int hc[2]) {
     if (m->cfg.matching_mode == 1) { in[0] = c.take<float4>(n[0]); in[1] = c.take<float4>(n[1]); }
     vg[0] = c.take<float4>(n[0]); vg[1] = c.take<float4>(n[1]); d_cnt = c.take<int>(2);
   }));
-  const float leaf[2] = {m->cfg.line_resolution, m->cfg.plane_resolution};
   for (int c = 0; c < 2; c++) {
-    const float4* src = his[c]->data();
-    if (m->cfg.matching_mode == 1) { LL_TRY(cm_live_points(ctx, cm[c], (int)n[c], in[c])); src = in[c]; }
-    LL_TRY(launch_voxel_grid(ctx, s, ctx->scratch, src, (int)n[c], nullptr, leaf[c], vg[c], d_cnt + c));
+    const float4* src = m->his[c].data();
+    if (m->cfg.matching_mode == 1) { LL_TRY(cm_live_points(ctx, m->cells[c], (int)n[c], in[c])); src = in[c]; }
+    LL_TRY(launch_voxel_grid(ctx, s, ctx->scratch, src, (int)n[c], nullptr, class_leaf(m->cfg, c), vg[c], d_cnt + c));
   }
   LL_CUDA(ctx, cudaMemcpyAsync(hc, d_cnt, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
@@ -861,7 +846,7 @@ size_t buf_caps(ll_mapper* m) {   // the bytes held by every buffer an attempt m
   ll_ctx* ctx = m->ctx;
   size_t b = ctx->scratch.cap + ctx->scratch2.cap + ctx->feat_buf.cap + ctx->stage_in.cap + m->rec.buf.cap;
   if (m->rec.field) b += reloc_field_storage_cap(m->rec.field);
-  if (m->rec.whole) b += m->rec.whole->corner.storage.cap + m->rec.whole->surf.storage.cap;
+  if (m->rec.whole) for (const BucketTree& t : m->rec.whole->tree) b += t.storage.cap;
   return b;
 }
 
@@ -1047,7 +1032,7 @@ int ll_mapper_set_recovery(ll_mapper* m, const ll_recovery_cfg* cfg) {
     LL_CUDA(ctx, ctx->feat_buf.reserve_floor((size_t)W * 4 * 16 + 64));
     const size_t side = std::max(voxel_grid_bytes(W), tree_scratch_bytes(W));
     LL_CUDA(ctx, ctx->scratch.reserve_floor(side)); LL_CUDA(ctx, ctx->scratch2.reserve_floor(side));
-    for (BucketTree* t : {&R.whole->corner, &R.whole->surf}) LL_CUDA(ctx, t->storage.reserve_floor(tree_storage_bytes(W)));
+    for (BucketTree& t : R.whole->tree) LL_CUDA(ctx, t.storage.reserve_floor(tree_storage_bytes(W)));
   }
   R.log.open(LL_RECOVERY_LOG);
   R.cfg = *cfg; R.on = true; R.state = LL_TRACKING; R.bad = 0; R.field_valid = false;

@@ -217,14 +217,13 @@ int build_grid(ll_ctx* ctx, const ll_map* map, float res, int pad, bool pad_ok, 
   if (max_hypotheses < 1 || max_hypotheses > RELOC_MAX_HYP) { ctx->set_error("max_hypotheses must be 1 ... 2^24"); return LL_ERR_INVALID; }
   cudaSetDevice(ctx->device);
   cudaStream_t s = ctx->stream;
-  const BucketTree* tr[2] = {&map->corner, &map->surf};
   float bb[2][6];
-  for (int c = 0; c < 2; c++) if (tr[c]->n_src > 0) LL_CUDA(ctx, cudaMemcpyAsync(bb[c], tr[c]->d_bbox, sizeof(bb[c]), cudaMemcpyDeviceToHost, s));
+  for (int c = 0; c < 2; c++) if (map->tree[c].n_src > 0) LL_CUDA(ctx, cudaMemcpyAsync(bb[c], map->tree[c].d_bbox, sizeof(bb[c]), cudaMemcpyDeviceToHost, s));
   LL_CUDA(ctx, cudaStreamSynchronize(s));
   float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
   bool any = false;
   for (int c = 0; c < 2; c++) {
-    if (tr[c]->n_src <= 0) continue;
+    if (map->tree[c].n_src <= 0) continue;
     bool ok = true;
     for (int a = 0; a < 3; a++) ok = ok && std::isfinite(bb[c][a]) && std::isfinite(bb[c][3 + a]) && bb[c][a] <= bb[c][3 + a];
     if (!ok) continue;   // no finite point in this cloud
@@ -253,7 +252,7 @@ int check_device(ll_ctx* ctx, const RelocBase* b, const char* noun) {
 // A relocalization's first checks: the map is whole, b (the "index" / "field") was built on it as it is now, and b is on the context's device.
 int check_built_on(ll_ctx* ctx, const RelocBase* b, const ll_map* map, const char* noun) {
   LL_TRY(check_map(ctx, map));
-  if (b->map != map || b->src[0] != map->corner.src || b->src[1] != map->surf.src || b->n_src[0] != map->corner.n_src || b->n_src[1] != map->surf.n_src) {
+  if (b->map != map || b->src[0] != map->tree[0].src || b->src[1] != map->tree[1].src || b->n_src[0] != map->tree[0].n_src || b->n_src[1] != map->tree[1].n_src) {
     ctx->set_error(std::string("the ") + noun + " was built on another map (or the map was rebuilt since)"); return LL_ERR_INVALID;
   }
   return check_device(ctx, b, noun);
@@ -525,7 +524,6 @@ int reloc_field_build_into(ll_ctx* ctx, const ll_map* map, float res, int trunc,
   f->map = nullptr; f->src[0] = f->src[1] = nullptr; f->n_src[0] = f->n_src[1] = 0;
   LL_TRY(build_grid(ctx, map, res, trunc, trunc >= 1 && trunc <= RELOC_MAX_TRUNC, "trunc must be 1 ... 15", max_hypotheses, f));
   cudaStream_t s = ctx->stream;
-  const BucketTree* tr[2] = {&map->corner, &map->surf};
   { const cudaError_t e = f->storage.carve([&](Carve& c) { field_layout(f, c); });
     if (e != cudaSuccess) { ctx->set_error(std::string("field allocation: ") + cudaGetErrorString(e)); return LL_ERR_CUDA; } }
   uint8_t* tmp = nullptr;   // occupancy, then the pass between y and z
@@ -535,8 +533,9 @@ int reloc_field_build_into(ll_ctx* ctx, const ll_map* map, float res, int trunc,
   auto cu = [&](cudaError_t e) { if (e != cudaSuccess && st == LL_OK) { ctx->set_error(std::string("field build: ") + cudaGetErrorString(e)); st = LL_ERR_CUDA; } };
   const unsigned blocks = (unsigned)((f->n_vox + 255) / 256);
   for (int c = 0; c < 2; c++) {
+    const BucketTree& t = map->tree[c];
     cu(cudaMemsetAsync(tmp, 0, (size_t)f->n_vox, s));
-    if (tr[c]->n_src > 0) { reloc_field_mark_kernel<<<ll_div_up(tr[c]->n_src, 256), 256, 0, s>>>(tr[c]->src, tr[c]->n_src, f->grid, tmp); ctx->launches++; }
+    if (t.n_src > 0) { reloc_field_mark_kernel<<<ll_div_up(t.n_src, 256), 256, 0, s>>>(t.src, t.n_src, f->grid, tmp); ctx->launches++; }
     uint8_t* io[3][2] = {{tmp, f->d2[c]}, {f->d2[c], tmp}, {tmp, f->d2[c]}};
     for (int a = 0; a < 3; a++) { reloc_edt_kernel<<<blocks, 256, 0, s>>>(io[a][0], io[a][1], f->grid.dims[0], f->grid.dims[1], f->grid.dims[2], a, trunc, a == 0 ? 1 : 0, f->n_vox); ctx->launches++; }
   }
@@ -544,7 +543,7 @@ int reloc_field_build_into(ll_ctx* ctx, const ll_map* map, float res, int trunc,
   cu(cudaStreamSynchronize(s));
   if (st != LL_OK) return st;
   f->map = map;
-  for (int c = 0; c < 2; c++) { f->src[c] = tr[c]->src; f->n_src[c] = tr[c]->n_src; }
+  for (int c = 0; c < 2; c++) { f->src[c] = map->tree[c].src; f->n_src[c] = map->tree[c].n_src; }
   return LL_OK;
 }
 
@@ -556,10 +555,9 @@ int ll_reloc_index_build(ll_ctx* ctx, const ll_map* map, float res, int dilate, 
   RelocBase base;
   LL_TRY(build_grid(ctx, map, res, dilate, dilate >= 0 && dilate <= RELOC_MAX_DILATE, "dilate must be 0 ... 4", max_hypotheses, &base));
   cudaStream_t s = ctx->stream;
-  const BucketTree* tr[2] = {&map->corner, &map->surf};
   ll_reloc_index* x = new ll_reloc_index{base};
   x->map = map;
-  for (int c = 0; c < 2; c++) { x->src[c] = tr[c]->src; x->n_src[c] = tr[c]->n_src; }
+  for (int c = 0; c < 2; c++) { x->src[c] = map->tree[c].src; x->n_src[c] = map->tree[c].n_src; }
   x->n_words = (x->n_vox + 31) / 32;
   auto fail = [&](int st) { x->storage.release(); delete x; return st; };
   { const cudaError_t e = x->storage.carve([&](Carve& c) { index_layout(x, c); });
@@ -575,7 +573,7 @@ int ll_reloc_index_build(ll_ctx* ctx, const ll_map* map, float res, int dilate, 
   int st = LL_OK;
   auto cu = [&](cudaError_t e) { if (e != cudaSuccess && st == LL_OK) { ctx->set_error(std::string("index build: ") + cudaGetErrorString(e)); st = LL_ERR_CUDA; } };
   cu(cudaMemsetAsync(occ, 0, (size_t)x->n_words * 4, s));
-  for (int c = 0; c < 2; c++) if (tr[c]->n_src > 0) { reloc_mark_kernel<<<ll_div_up(tr[c]->n_src, 256), 256, 0, s>>>(tr[c]->src, tr[c]->n_src, base.grid, occ); ctx->launches++; }
+  for (const BucketTree& t : map->tree) if (t.n_src > 0) { reloc_mark_kernel<<<ll_div_up(t.n_src, 256), 256, 0, s>>>(t.src, t.n_src, base.grid, occ); ctx->launches++; }
   if (dilate > 0) {
     const long long threads = x->n_words * 32;
     const unsigned blocks = (unsigned)((threads + 255) / 256);

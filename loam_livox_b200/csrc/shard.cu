@@ -123,7 +123,7 @@ int ll_map_build_sharded(ll_ctx* ctx, const void* corner, size_t nc, const void*
     g.dims[k] = (int)floorf((hi[k] - lo[k]) * g.inv_cell) + 1;
     ncell *= (size_t)g.dims[k];
   }
-  auto fail = [&](int st, const char* why) { if (why) ctx->set_error(why); m->corner.storage.release(); m->surf.storage.release(); m->shard_owner.release(); delete m; return st; };
+  auto fail = [&](int st, const char* why) { if (why) ctx->set_error(why); ll_map_release(m); return st; };
   if (ncell > ((size_t)1 << 24)) return fail(LL_ERR_CAPACITY, "shard grid has more than 2^24 cells: raise cell_size");
   // ---- points per cell -> owner table (host, deterministic) -> device
   int* d_hist; unsigned char* d_keep; int* d_cnt; char* d_tmp;
@@ -141,7 +141,6 @@ int ll_map_build_sharded(ll_ctx* ctx, const void* corner, size_t nc, const void*
   // ---- this rank's shard of each cloud: owner cells + halo, compacted in input order, then indexed
   // (1 + 1e-4) h + 1 mm: a superset is always safe, and it absorbs the rounding of the fp32 box arithmetic against the fp32 gate test
   const float4* srcs[2] = {d_c, d_s}; const size_t ns2[2] = {nc, ns}; const float halos[2] = {halo_corner * 1.0001f + 1e-3f, halo_surf * 1.0001f + 1e-3f};
-  BucketTree* trees[2] = {&m->corner, &m->surf};
   for (int w = 0; w < 2; w++) {
     int kept = 0;
     if (ns2[w] > 0) {
@@ -151,7 +150,7 @@ int ll_map_build_sharded(ll_ctx* ctx, const void* corner, size_t nc, const void*
       if (cudaMemcpyAsync(&kept, d_cnt, 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) return fail(LL_ERR_CUDA, "shard count read-back failed");
     }
     m->shard_total[w] = (long long)ns2[w];
-    const int st = build_bucket_tree(ctx, s, ctx->scratch, d_k, kept, trees[w]);
+    const int st = build_bucket_tree(ctx, s, ctx->scratch, d_k, kept, &m->tree[w]);
     if (st != LL_OK) return fail(st, nullptr);
   }
   if (cudaStreamSynchronize(s) != cudaSuccess) return fail(LL_ERR_CUDA, "shard build failed");
@@ -164,7 +163,7 @@ int ll_map_shard_info(const ll_map* map, ll_shard_info* info, int* owner_out, si
   memset(info, 0, sizeof(*info));
   info->rank = map->rank; info->world = map->world; info->cell_size = map->grid.cell; info->halo_corner = map->halo[0]; info->halo_surf = map->halo[1];
   for (int k = 0; k < 3; k++) { info->origin[k] = map->grid.origin[k]; info->dims[k] = map->grid.dims[k]; }
-  info->kept_corner = (long long)map->corner.n_src; info->kept_surf = (long long)map->surf.n_src; info->total_corner = map->shard_total[0]; info->total_surf = map->shard_total[1];
+  info->kept_corner = (long long)map->tree[0].n_src; info->kept_surf = (long long)map->tree[1].n_src; info->total_corner = map->shard_total[0]; info->total_surf = map->shard_total[1];
   if (owner_out) {
     if (owner_cap < map->h_owner.size()) return LL_ERR_CAPACITY;
     memcpy(owner_out, map->h_owner.data(), map->h_owner.size() * sizeof(int));
